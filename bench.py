@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- VGICP linearize throughput (M points.factors / s) on B200, next to the CPU path.
+"""bench.py -- VGICP linearize throughput (M points.factors / s) on H100, next to the CPU path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl reference] [--verify K]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl reference] [--verify K] [--dump-outputs DIR]
 
 A "step" is one relinearization pass of the hot path over the workload's whole factor set (every
 NonlinearFactorSetGPU::linearize call the workload contains, back to back).  Default workload:
@@ -16,13 +16,14 @@ value      whole-job points.factors / s, inputs resident in HBM, CUDA events on 
 e2e        the same through the C-ABI with HOST buffers: poses H2D from pinned memory + launch (+ exchange) + the result
            (pair slab for the sharded global-mapping sweep, gb_linearized6 records otherwise) D2H, every step
 roofline   algorithmic bytes per launch (SURVEY 8(d) B_sweep, from gb_sweep_stats) / measured launch duration vs
-           MEASURED_PEAKS.json hbm_gbs; next to it the miss-aware byte count and (from the committed ncu capture) the DRAM
-           traffic and the DRAM fraction
+           MEASURED_PEAKS.json hbm_gbs (else the H100 SXM data sheet's 3.35 TB/s); next to it the miss-aware byte count
 parity_check   --verify K (default 4): after the timed region K random pairs are recomputed with the fp64 CPU oracle and
            compared with the rows of the exchanged pair slab (at N > 1 that includes rows produced by other ranks)
 --impl reference   the CPU path (oracle port of gtsam_points::IntegratedVGICPFactor, fp64, all host threads) on a
            bounded sample of the same workload.  The only place besides cpu_baseline / parity_check where bench.py
            executes oracle/.  Builds its sample on the host (numpy / scipy): libglim_b200.so is not loaded.
+--dump-outputs DIR   what the last timed step computed (pair slab or records; the frame for preprocess) as DIR/<name>.npy;
+           inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -40,6 +41,9 @@ sys.path.insert(0, ROOT)
 METRIC = "VGICP linearize throughput"
 UNIT = "M points*factors/s"
 WORKLOADS = ["single_pair", "odometry_gpu", "sub_mapping_gpu", "global_mapping_gpu", "livox_stress"]
+L2_BYTES = 50e6  # H100: inputs that fit are re-read from L2 across steps, so the L2 is flushed between timed steps
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet (HBM3), used when MEASURED_PEAKS.json gives no measured figure
+DUMP_BYTES = 64_000_000
 
 
 def parse_args():
@@ -55,6 +59,7 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-other-workloads", action="store_true", help="skip roofline_by_workload in the default N = 1 line")
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="CPU work budget for the cpu_baseline sample")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -116,7 +121,7 @@ def workload_config(name, w, extra):
         "factor_sets_per_step": len(w.sets),
         "factors_per_step": int(sum(len(s.factors) for s in w.sets)),
         "point_factors_per_step": int(w.point_factors),
-        "l2": "inputs larger than L2 (no flush)" if sum(len(c[0]) for c in w.host_clouds if c is not None) * 36 > 126e6 else "L2 flushed between steps (256 MB write)",
+        "l2": "inputs larger than L2 (no flush)" if sum(len(c[0]) for c in w.host_clouds if c is not None) * 36 > L2_BYTES else "L2 flushed between steps (256 MB write)",
     }
     cfg.update({k: v for k, v in w.notes.items() if not k.startswith("_")})
     cfg.update(extra)
@@ -367,7 +372,7 @@ class Env:
         self.world = int(os.environ.get("WORLD_SIZE", "1"))
         self.local_rank = int(os.environ.get("LOCAL_RANK", "0"))
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py needs a B200: no CUDA device visible (there is no CPU fallback)")
+            raise SystemExit("bench.py needs an H100: no CUDA device visible (there is no CPU fallback)")
         torch.cuda.set_device(self.local_rank)
         if self.world > 1:
             os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
@@ -442,31 +447,31 @@ def load_peaks():
         return {}
 
 
-def ncu_traffic(name, world, scale):
-    """DRAM bytes per launch from the committed ncu --set full capture of this workload (1 GPU, full scale only)."""
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        if world == 1 and scale == 1.0 and name in tj:
-            return tj[name]["dram_bytes_per_launch"], tj[name]["source"]
-    except Exception:
-        pass
-    return None, None
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: every array as out_dir/<name>.npy, float32 kept, anything else as float64; an array larger than its share of
+    DUMP_BYTES is cut to a fixed, seeded sample of its rows."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BYTES // max(1, len(arrays))
+    for name, a in arrays.items():
+        a = np.atleast_1d(np.asarray(a))
+        a = a.astype(np.float32 if a.dtype == np.float32 else np.float64)
+        if a.nbytes > share:
+            keep = max(1, share // (a.nbytes // len(a)))
+            a = a[np.sort(np.random.default_rng(0).choice(len(a), keep, replace=False))]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def roofline_of(name, my_bytes, miss_bytes, k_launches, kernel_ms_per_launch, world, scale):
     peaks = load_peaks()
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
     achieved = my_bytes / max(1, k_launches) / (kernel_ms_per_launch * 1e-3) / 1e9
-    traffic, traffic_src = ncu_traffic(name, world, scale)
     r = {"bound": "hbm", "kernel": "k_vgicp_sweep3 / k_vgicp_sweep5 <LINEARIZE>", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-         "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)",
+         "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else f"H100 SXM data sheet, {HBM_PEAK_GBS:.0f} GB/s",
          "algorithmic_bytes_per_launch": my_bytes / max(1, k_launches), "launch_ms": kernel_ms_per_launch,
-         "traffic": traffic, "traffic_source": traffic_src,
          # what the kernel must actually fetch: a miss reads 16 B of the point, not 48
          "miss_aware_bytes_per_launch": miss_bytes / max(1, k_launches) if miss_bytes is not None else None,
          "miss_aware_frac": (miss_bytes / max(1, k_launches) / (kernel_ms_per_launch * 1e-3) / 1e9 / peak) if miss_bytes is not None else None,
-         "dram_frac": (traffic / (kernel_ms_per_launch * 1e-3) / 1e9 / peak) if traffic else None,
-         "note": "frac = SURVEY 8(d) B_sweep (48 B per point.factor + 48 B per target voxel + 16 B per bucket + 552 B per factor, no credit for reuse) / CUDA-event launch time / peak: the CONTRACT figure, not a DRAM utilisation -- clouds shared by consecutive factors are served from L2 and misses read 16 B, so B_sweep can exceed what HBM delivers (frac > 1 is possible); dram_frac = ncu DRAM bytes / launch time / peak is the real HBM utilisation"}
+         "note": "frac = SURVEY 8(d) B_sweep (48 B per point.factor + 48 B per target voxel + 16 B per bucket + 552 B per factor, no credit for reuse) / CUDA-event launch time / peak: the CONTRACT figure, not a DRAM utilisation -- clouds shared by consecutive factors are served from L2 and misses read 16 B, so B_sweep can exceed what HBM delivers (frac > 1 is possible)"}
     return r
 
 
@@ -483,7 +488,7 @@ def measure_simple(env, name, w, steps, warmup):
         sweeps.append(sw)
     ctx.synchronize()
     sizes = [len(c[0]) for c in w.host_clouds]
-    small = sum(sizes) * 36 <= 126e6
+    small = sum(sizes) * 36 <= L2_BYTES
     my_pf = sum(sw.point_factors for sw in sweeps)
     my_bytes = sum(sw.algorithmic_bytes for sw in sweeps)
 
@@ -515,7 +520,7 @@ def measure_simple(env, name, w, steps, warmup):
 
     for _ in range(3):
         step_e2e()
-    e_steps = max(3, min(steps, 50))
+    e_steps = steps
     ems, _, _, _ = env.timed(step_e2e, e_steps, False)
     F = sum(sw.F for sw in sweeps)
     out = {
@@ -688,7 +693,7 @@ def main():
     total_pf = all_pf if sharded else all_pf * world  # replicas: every rank processes the whole stream
     ctx.synchronize()
 
-    small_inputs = sum(sizes) * 36 <= 126e6
+    small_inputs = sum(sizes) * 36 <= L2_BYTES
 
     def step_device():
         for sw, slab, ps in zip(sweeps, slabs, peers):
@@ -718,6 +723,15 @@ def main():
     if profiling:
         torch.cuda.profiler.stop()
     gpu_launches = (ctx.kernel_launches - launches0) * world  # every rank launches the same sequence
+    if args.dump_outputs and rank == 0:
+        outs = {}
+        for si, (sw, slab, ps) in enumerate(zip(sweeps, slabs, peers)):
+            if ps is not None or slab is not None:
+                outs[f"pair_slab{si}"] = ps.fetch() if ps is not None else slab.cpu().numpy()
+            elif sw.F:
+                rec = sw.fetch()
+                outs[f"linearized{si}"] = rec.view(np.float64).reshape(len(rec), -1)
+        dump_outputs(args.dump_outputs, outs)
     ms_per_step = ms / args.steps
     value = total_pf / (ms_per_step * 1e-3) / 1e6
 
@@ -774,7 +788,7 @@ def main():
 
     for _ in range(3):
         step_e2e()
-    e_steps = max(3, min(args.steps, 50))
+    e_steps = args.steps
     ems, _, _, _ = env.timed(step_e2e, e_steps, False)
     e2e_val = total_pf / (ems / e_steps * 1e-3) / 1e6
 
@@ -834,13 +848,13 @@ def main():
             del sweeps, slabs, peers
             others = {}
             names = {"single_pair": "M1", "odometry_gpu": "M2", "sub_mapping_gpu": "M3", "livox_stress": "M5"}
-            others["M4 global_mapping_gpu"] = {"value": value, "launch_ms": roofline["launch_ms"], "frac": roofline["frac"], "miss_aware_frac": roofline["miss_aware_frac"], "dram_frac": roofline["dram_frac"], "traffic": roofline["traffic"], "e2e": e2e_val}
+            others["M4 global_mapping_gpu"] = {"value": value, "launch_ms": roofline["launch_ms"], "frac": roofline["frac"], "miss_aware_frac": roofline["miss_aware_frac"], "e2e": e2e_val}
             for nm, tag in names.items():
                 try:
                     wo = build_workload(nm, ctx, 1.0, use_gpu=True)
-                    r = measure_simple(env, nm, wo, max(10, min(args.steps, 30)), 3)
+                    r = measure_simple(env, nm, wo, args.steps, 3)
                     others[f"{tag} {nm}"] = {"value": r["value"], "launch_ms": r["roofline"]["launch_ms"], "frac": r["roofline"]["frac"], "miss_aware_frac": r["roofline"]["miss_aware_frac"],
-                                             "dram_frac": r["roofline"]["dram_frac"], "traffic": r["roofline"]["traffic"], "e2e": r["e2e"]["value"], "inlier_fraction": round(r["inlier_fraction"], 3),
+                                             "e2e": r["e2e"]["value"], "inlier_fraction": round(r["inlier_fraction"], 3),
                                              "factors_per_launch": int(sum(len(s.factors) for s in wo.sets) / len(wo.sets))}
                     del wo
                 except Exception as ex:  # never lose the headline line to a secondary measurement

@@ -46,7 +46,7 @@ def run(env, args, metric_name):
 
     for _ in range(max(3, args.warmup)):
         step_device()
-    steps = max(10, min(args.steps, 200))
+    steps = args.steps
     l0 = env.ctx.kernel_launches
     ms, _, t0, t1 = env.timed(step_device, steps, False)
     launches = env.ctx.kernel_launches - l0
@@ -60,6 +60,8 @@ def run(env, args, metric_name):
         clocks = sampler.summary(t0, t1e)
     fr, normals, covs, cloud = step_e2e()
     m = fr.size()
+    if args.dump_outputs and env.rank == 0:
+        bench.dump_outputs(args.dump_outputs, {"points": fr.points, "times": fr.times, "neighbors": fr.neighbors.reshape(m, -1), "normals": normals, "covs": covs})
     # parity spot check against the CPU pipeline (indices exact, covariances 1e-9)
     threads = bench.host_threads()
     ref = cpu_preprocess(pts, tms, params, threads)
@@ -76,7 +78,7 @@ def run(env, args, metric_name):
     threads = min(t_cpu, key=lambda t: t_cpu[t])
     cpu_ms = 1e3 * t_cpu[threads]
     peaks = bench.load_peaks()
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", bench.HBM_PEAK_GBS))
     # algorithmic bytes: raw point + time in (40 B), frame products out (point 32 + time 8 + k neighbours 4k + cov 128 + normal 32), device cloud planes (52 B)
     alg = n * 40 + m * (32 + 8 + 4 * params.k_correspondences + 128 + 32 + 52)
     per = ms / steps

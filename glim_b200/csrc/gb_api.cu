@@ -130,8 +130,8 @@ static gb_status ctx_create(int device, cudaStream_t stream, bool own, gb_ctx** 
   GB_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   GB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    gb_set_error("device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    gb_set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     return GB_ERR_NO_DEVICE;
   }
   gb_ctx* c = new (std::nothrow) gb_ctx();
@@ -500,8 +500,8 @@ static void build_items(gb_sweep* s, FactorDesc* descs, std::vector<int2>& tiles
   tiles.clear();
   const size_t F = s->F;
   if (!s->strided) {
-    // TAIL TAPERING (guided self-scheduling): with ~38 us per 2048-point item, the last wave of a sweep leaves warps idle for
-    // up to one item time -- 1 % of a 2.7 ms single-GPU sweep but 9 % of the 0.4 ms share of one of 8 ranks.  The factors that
+    // TAIL TAPERING (guided self-scheduling): the last wave of a sweep leaves warps idle for up to one 2048-point item time --
+    // little of a single-GPU sweep but a large share of one of 8 ranks' shard.  The factors that
     // hold the last ~1.5 item-times of work per warp get items of a quarter of the size, the last 0.4 a sixteenth.
     const double warps = (double)s->capacity * 8.0;
     uint64_t total = 0;
@@ -613,10 +613,10 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   s->graph_exec = nullptr; s->graph_state = 0;
 
   // kernel generation and work-item policy
-  // Kernel policy (measured on B200, profiles/r02_ab_kernels.txt): small sweeps -- about one item per warp: an odometry
-  // frame, a single pair -- run k_vgicp_sweep5 with one wave of equally expensive STRIDED items (-25 % on the odometry
+  // Kernel policy (A/B runs of the kernels, scripts/ab_sweep.py): small sweeps -- about one item per warp: an odometry
+  // frame, a single pair -- run k_vgicp_sweep5 with one wave of equally expensive STRIDED items (faster on the odometry
   // workload); large sweeps run k_vgicp_sweep3 with contiguous 2048-point items drawn from the queue (its simpler hot loops
-  // are 5-9 % faster there).  GB_KERNEL = 3 / 4 / 5 forces one kernel (4 = the bulk-async staged experiment).
+  // are faster there).  GB_KERNEL = 3 / 4 / 5 forces one kernel (4 = the bulk-async staged experiment).
   const int kv = env_int("GB_KERNEL", 0);
   s->stage_points = env_int("GB_STAGE", 128) == 64 ? 64 : 128;
   const int ctas_per_sm = (kv == 4 && s->stage_points == 64) ? 3 : 2;
@@ -633,7 +633,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     int tile = env_int("GB_TILE", 0);
     if (tile <= 0) {
       // contiguous items: ~GB_ITEMS_PER_WARP items per warp (first one static, the rest drawn dynamically), between 128 and
-      // 2048 points each (profiles/tune_sweep_r0*.txt)
+      // 2048 points each
       const uint64_t ipw = (uint64_t)std::max(1, env_int("GB_ITEMS_PER_WARP", s->kernel_version == 4 ? 4 : 6));
       const uint64_t want = total_pts / (warps * ipw) + 1;
       tile = (int)std::min<uint64_t>(2048, std::max<uint64_t>(s->kernel_version == 4 ? T : 128, want));
@@ -975,9 +975,8 @@ extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int worl
   ps->buf_floats = align_up(num_pairs * GB_SLAB_STRIDE * sizeof(float), 256) / sizeof(float);
   ps->local = nullptr; ps->step = 0; ps->parity = 0; ps->completed_parity = 0; ps->d_timeout = nullptr; ps->connected = (world == 1);
   // fused: the sweep's epilogue stores every finished row straight into all peers; deferred: rows go to the local buffer and
-  // the exchange kernel pushes them (see gb_launch_peer_signal_wait).  Measured (BASELINE.md 4.1): the peer stores cost the
-  // sweep ~5 us at 4 ranks and ~13 us at 8, the exchange kernel is 5-9 us longer than the flag-only one -> fused up to 4
-  // ranks, deferred above.  GB_PEER_PUSH=fused|deferred forces one.
+  // the exchange kernel pushes them (see gb_launch_peer_signal_wait).  The peer stores' cost to the sweep grows with the
+  // rank count faster than the exchange kernel's extra time -> fused up to 4 ranks, deferred above.  GB_PEER_PUSH=fused|deferred forces one.
   {
     const char* e = getenv("GB_PEER_PUSH");
     ps->deferred = world > 4;

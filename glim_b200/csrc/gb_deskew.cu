@@ -7,8 +7,7 @@
 // (gb_deskew_pose_table, also exported so it can be checked without a GPU).  The O(N) part -- one table lookup and one or two
 // 4x4 * 4-vector products per point, fp64 -- is the kernel.  Oracle: go_deskew_const_vel / go_deskew_imu.
 //
-// NOT YET RUN ON A GPU: written after round 1's GPU budget was spent.  The host table is verified on the CPU against the
-// oracle (tests/test_deskew.py); the kernel's parity test is marked xfail(strict=False) until it has run once.
+// The host table is verified on the CPU against the oracle, the kernel on the GPU (tests/test_deskew.py).
 #include "gb_internal.cuh"
 
 #include <math.h>

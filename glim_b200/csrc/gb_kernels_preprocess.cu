@@ -1,4 +1,4 @@
-// gb_kernels_preprocess.cu -- per-frame preprocess on the GPU (sm_100a): k-NN, covariance / normal
+// gb_kernels_preprocess.cu -- per-frame preprocess on the GPU (sm_90a): k-NN, covariance / normal
 // estimation, voxel-grid downsampling.
 //
 // Replaces, at GLIM's call sites:

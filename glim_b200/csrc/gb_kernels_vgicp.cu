@@ -1,4 +1,4 @@
-// gb_kernels_vgicp.cu -- the fused VGICP linearize / error sweep and the overlap kernel (sm_100a).
+// gb_kernels_vgicp.cu -- the fused VGICP linearize / error sweep and the overlap kernel (sm_90a).
 //
 // Replaces gtsam_points::IntegratedVGICPFactorGPU::linearize / ::error as driven by
 // NonlinearFactorSetGPU (GLIM call sites: src/glim/odometry/odometry_estimation_gpu.cpp:144,161,383-386;
@@ -27,7 +27,7 @@
 //   k_vgicp_sweep5  small sweeps (an odometry frame, a single pair -- about one item per warp): one wave of STRIDED items
 //                   sized by each factor's last inlier fraction, descriptor / pose cache in shared memory.
 //   k_vgicp_sweep4  experiment, never the default: source tiles staged into shared memory by bulk async copies
-//                   (cp.async.bulk / UBLKCP + mbarrier).  1.7-2x slower than sweep3 (profiles/r02_ab_kernels_a.txt): the
+//                   (cp.async.bulk / UBLKCP + mbarrier).  Slower than sweep3 when it was measured: the
 //                   carve-out shrinks L1 and the path is latency-, not issue-bound.  Kept as the measured negative result.
 #include "gb_internal.cuh"
 #include "gb_vgicp_math.cuh"  // PoseF, transform, fused_mahalanobis, accumulate_hit, surface_ok, slab_to_record (also compiled for the host by the CPU test)
@@ -316,7 +316,7 @@ __global__ void __launch_bounds__(kThreads, MINB) k_vgicp_sweep4(
   }
 
   // Descriptor reads keep their address space (LDS from the cache or LDG from the table): a merged generic pointer made the
-  // compiler re-load D.mask / D.inv_res with generic LD.E inside the stage loop (26 % of the stall samples of the first version).
+  // compiler re-load D.mask / D.inv_res with generic LD.E inside the stage loop (a large share of the stall samples of the first version).
   auto desc_of = [&](int f) -> FactorDesc { FactorDesc d; if (cached) d = cache->desc[f]; else d = descs[f]; return d; };
   auto tiles_of = [&](int f) -> int { return cached ? cache->desc[f].num_tiles : descs[f].num_tiles; };
   // lane 0: start the copy of `cnt` points of factor f's source cloud
@@ -521,9 +521,9 @@ __global__ void __launch_bounds__(kThreads, MINB) k_vgicp_sweep4(
 // for the next item is issued at the start of the current one).  An item's completion ticket is published LAZILY: an
 // atom.release issued while the next item's first loads are in flight (no __threadfence, i.e. no MEMBAR.SC + L1
 // invalidation per item), and a factor's epilogue runs after the next item's reduction.  Measured on the global-mapping
-// sweep and its 1/8 shards (profiles/r02_shard_emulate.txt): -1.6 % / -3.4 % against fence + ticket per item.
-// Tried and dropped (same file): reading the queue one item ahead in registers (+2 % time: the kernel sits at the 128-register
-// cap) and copying the next item's descriptor / pose to shared memory with cp.async during the current item (+1.6 %: the
+// sweep and its 1/8 shards: faster than a fence + ticket per item.
+// Tried and dropped: reading the queue one item ahead in registers (slower: the kernel sits at the 128-register
+// cap) and copying the next item's descriptor / pose to shared memory with cp.async during the current item (slower: the
 // three dependent L2 round trips between two items are already covered by the other 15 warps of the SM).
 // =============================================================================================
 constexpr int kSubMax = 512;   // queue capacity per warp (points per round)
@@ -1010,9 +1010,9 @@ gb_status gb_launch_sweep(gb_sweep* s, int mode) {
 // Deferred exchange: the four CTAs of peer p copy this rank's finished rows (written by the sweep into the local buffer of the step
 // parity) into peer p's buffer -- 128-bit stores through the IPC mapping, ~164 KB per peer at 8 ranks -- then publishes this
 // rank's step to that peer and waits for the peer's flag.  The CTAs are independent (one per peer): no ordering between them.
-// Why not from the sweep's epilogue (GB_PEER_PUSH=fused, the round-1 design): stores to peer memory issued from the 148 busy
-// SMs cost the sweep 3.5-6 % at 8 ranks (profiles/r02_bench_n8_fused_push*.json, r02_bench_n8_nccl.json: per-rank kernel 0.398 ms fused against 0.374 ms for the
-// same shard without the peer stores) while the whole exchange is ~1 MB per rank and step.
+// Why not from the sweep's epilogue (GB_PEER_PUSH=fused, the round-1 design): stores to peer memory issued from all the busy
+// SMs slow the sweep down at 8 ranks (against the same shard without the peer stores) while the whole exchange is ~1 MB per rank
+// and step.
 struct PeerExchange {
   float* dst[GB_MAX_PEERS];   // every rank's buffer of the step parity, as mapped here
   unsigned* flags[GB_MAX_PEERS];

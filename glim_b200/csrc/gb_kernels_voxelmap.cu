@@ -1,4 +1,4 @@
-// gb_kernels_voxelmap.cu -- deterministic GPU build of the Gaussian voxel map (sm_100a).
+// gb_kernels_voxelmap.cu -- deterministic GPU build of the Gaussian voxel map (sm_90a).
 //
 // Replaces gtsam_points::GaussianVoxelMapGPU(resolution, 8192*2, 10, 1e-3, stream)::insert(cloud)
 // (GLIM call sites: src/glim/odometry/odometry_estimation_gpu.cpp:103-104; src/glim/mapping/sub_mapping.cpp:398-399;
@@ -195,8 +195,8 @@ gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resol
   int nb = init_buckets;
   static const int load_mult = getenv("GB_TABLE_MULT") ? atoi(getenv("GB_TABLE_MULT")) : 8;  // experiment knob; 8 = the oracle's rule
   while ((long long)nb < (long long)load_mult * V) nb *= 2;  // load factor <= 1/8: the XOR-of-primes hash clusters, and lookups that
-                                                             // MISS (65 % of them in global mapping) walk until the first empty slot
-                                                             // (profiles/tune_tablemult_r01.txt); same rule as the oracle
+                                                             // MISS (most of them in global mapping) walk until the first empty slot;
+                                                             // same rule as the oracle
   for (;;) {
     GB_CUDA(gb_dev_malloc(ctx->device, sizeof(int4) * (size_t)nb, (void**)&m->buckets));
     k_table_clear<<<(nb + 255) / 256, 256, 0, st>>>(nb, m->buckets);

@@ -1,6 +1,6 @@
 """Sharding of a global-mapping relinearization sweep across the GPUs of one box (SURVEY.md 8(e)).
 
-The reference has no multi-GPU notion (SURVEY 0.6); this is the B200-native addition north_star asks for.
+The reference has no multi-GPU notion (SURVEY 0.6); this is the multi-GPU addition north_star asks for.
 Every rank holds all submap clouds and voxel maps (replicated at insert time, ~1.5 GB); the (target, source) PAIRS of the
 factor graph are partitioned over the ranks -- both voxel levels of a pair stay together; by default `world` CONTIGUOUS chunks
 of the reference's source-major factor order, cut at equal cost (measured inliers, then per-rank kernel-time feedback), so that

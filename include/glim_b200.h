@@ -1,5 +1,5 @@
 /*
- * glim_b200.h -- C-ABI of libglim_b200.so: the B200-native (sm_100a) VGICP scan-matching hot path
+ * glim_b200.h -- C-ABI of libglim_b200.so: the H100-native (sm_90a) VGICP scan-matching hot path
  * of koide3/glim, behind the surface GLIM's modules use from gtsam_points.
  *
  * Every entry point cites the reference interface it replaces (paths relative to the GLIM tree,
@@ -164,7 +164,7 @@ GB_API gb_status gb_sweep_stats(const gb_sweep* sweep, uint64_t* point_factors, 
  *      flags, allocated with cudaMalloc and shared with the other ranks of the box through CUDA IPC.  When one is attached
  *      to a sweep (ONE sweep per slab), the epilogue of the LAST factor of every pair sums the pair's factor records in fp64
  *      and stores the finished row -- up to 4 ranks straight into EVERY rank's buffer over NVLink (fused push), above 4 ranks
- *      into this rank's buffer only (deferred push: stores to peer memory from the busy SMs cost the sweep 3.5-6 % at 8
+ *      into this rank's buffer only (deferred push: stores to peer memory from the busy SMs slow the sweep down at 8
  *      ranks, DESIGN.md section 8).  gb_peer_slab_signal_wait() launches the kernel that (deferred push only: four CTAs per
  *      peer) copies the rank's rows into that peer's buffer, publishes this rank's completion flag and waits for the peers'.
  *      Each pair is owned by exactly one rank, so the "all-reduce" is an all-gather done by the producers.  No NCCL call, no

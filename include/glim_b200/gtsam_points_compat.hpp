@@ -447,7 +447,7 @@ inline void cuda_mem_get_info(std::size_t* free_bytes, std::size_t* total_bytes)
 /// gtsam_points::cuda_device_names()  (debug.cpp:84): one entry per visible device (the C-ABI reports the count, not the marketing name)
 inline std::vector<std::string> cuda_device_names() {
   std::vector<std::string> names;
-  for (int d = 0; d < gb_device_count(); d++) names.push_back("CUDA device " + std::to_string(d) + " (sm_100a)");
+  for (int d = 0; d < gb_device_count(); d++) names.push_back("CUDA device " + std::to_string(d) + " (sm_90a)");
   return names;
 }
 

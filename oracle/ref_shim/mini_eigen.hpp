@@ -2,7 +2,7 @@
 // cloud_deskewing.cpp use, WRITTEN HERE (Eigen is not installed in this environment and nothing of it is copied).
 //
 // TEST INFRASTRUCTURE ONLY (see oracle/Makefile, target _ref): it lets those two reference translation units compile
-// UNMODIFIED from /root/reference so that their control flow and formulas -- not a restatement of them -- can be run against
+// UNMODIFIED from a GLIM source tree so that their control flow and formulas -- not a restatement of them -- can be run against
 // oracle/glim_oracle.c.  What this does NOT pin is Eigen's own arithmetic: fixed-size products are evaluated here as plain
 // sequential sums, SelfAdjointEigenSolver<Matrix3d>::computeDirect, Quaterniond(Matrix3d) / slerp / toRotationMatrix follow
 // Eigen's published algorithms as restated by us.  Every object is a plain value (no expression templates, no alignment tricks).

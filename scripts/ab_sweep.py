@@ -50,7 +50,7 @@ def main():
         t0 = time.time()
         w = bench.build_workload(name, env.ctx, 1.0, use_gpu=True)
         sizes = [len(c[0]) for c in w.host_clouds]
-        small = sum(sizes) * 36 <= 126e6
+        small = sum(sizes) * 36 <= bench.L2_BYTES
         ref_inl = None
         for label, e in cfgs:
             for k in KEYS:

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Summarise an .ncu-rep (run here, no GPU needed): key metrics of each profiled launch + the SASS lines with the most
-stall samples.  usage: python scripts/ncu_summary.py gpurun_out/prof.ncu-rep > profiles/<name>.md"""
+stall samples.  usage: python scripts/ncu_summary.py prof.ncu-rep > prof.md"""
 import csv
 import io
 import subprocess

@@ -2,7 +2,7 @@
 """What does ONE rank's share of the global-mapping sweep cost on its own?  Runs, on one GPU, the shard every rank of an
 N-GPU job would run (same partition as bench.py, calibrated by measured inliers; plain slab instead of the peer slab) and
 prints the per-shard kernel times next to T(N=1)/N.  Separates the size-regime loss of the sweep kernel from the cost of the
-NVLink exchange in the multi-GPU numbers (profiles/r02_bench_n8.json).
+NVLink exchange in the multi-GPU numbers.
 usage: python scripts/shard_emulate.py [N ...]   env: AB_CONFIGS="label=K1:V1;K2:V2,label2=..." for kernel knobs"""
 import json
 import os

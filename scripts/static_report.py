@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Static (no-GPU) evidence for every kernel in libglim_b200.so: ptxas resources (registers, spills, shared memory) from the
-build logs and selected SASS mnemonic counts from `cuobjdump -sass`.  Output: markdown on stdout
-(kept as profiles/r02_static_resources.md).  Measurement plumbing; nothing here is imported by the product."""
+build logs and selected SASS mnemonic counts from `cuobjdump -sass`.  Output: markdown on stdout.
+Measurement plumbing; nothing here is imported by the product."""
 import collections
 import os
 import re
@@ -56,7 +56,7 @@ def ptxas_resources():
             continue
         txt = open(os.path.join(BUILD, log)).read()
         for m in re.finditer(
-            r"Compiling entry function '([^']+)' for 'sm_100a'\n.*?\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n"
+            r"Compiling entry function '([^']+)' for 'sm_90a'\n.*?\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n"
             r"ptxas info\s+: Used (\d+) registers(?:, used (\d+) barriers)?(?:, (\d+) bytes cumulative stack size)?(?:, (\d+) bytes smem)?",
             txt,
         ):
@@ -101,7 +101,7 @@ def main():
     sass = sass_counts()
     names = sorted(set(res) | set(sass))
     dm = demangle(names)
-    print("# Static resources and SASS mnemonics of every kernel in `libglim_b200.so` (sm_100a, nvcc 12.9, `-O3 -lineinfo`)")
+    print("# Static resources and SASS mnemonics of every kernel in `libglim_b200.so` (sm_90a, nvcc 12.9, `-O3 -lineinfo`)")
     print()
     print("Produced without a GPU by `python scripts/static_report.py` from `glim_b200/csrc/build/*.ptxas.log` (`-Xptxas -v`) and")
     print("`cuobjdump -sass glim_b200/libglim_b200.so`.  Template arguments of the sweep kernels: `k_vgicp_sweep3<MODE, PEER, SV>`,")

@@ -9,11 +9,11 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
 
 
 def pytest_collection_modifyitems(config, items):
-    """gpu-marked tests are SKIPPED (not errored) on a box without a B200; everything else runs everywhere."""
+    """gpu-marked tests are SKIPPED (not errored) on a machine without an H100; everything else runs everywhere."""
     try:
         from glim_b200 import capi
 
@@ -22,7 +22,7 @@ def pytest_collection_modifyitems(config, items):
         have_gpu = False
     if have_gpu:
         return
-    skip = pytest.mark.skip(reason="needs a B200 (no CUDA device visible)")
+    skip = pytest.mark.skip(reason="needs an H100 (no CUDA device visible)")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

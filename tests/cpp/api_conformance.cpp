@@ -1,10 +1,11 @@
 // api_conformance.cpp -- COMPILE-ONLY: the reference's OWN headers (include/glim/preprocess/cloud_preprocessor.hpp,
 // include/glim/common/cloud_covariance_estimation.hpp, include/glim/common/cloud_deskewing.hpp, found on the include path under
-// /root/reference and compiled against the Eigen stand-in of oracle/ref_shim/) and the shims of
+// a GLIM source tree and compiled against the Eigen stand-in of oracle/ref_shim/) and the shims of
 // include/glim_b200/glim_preprocess_compat.hpp in ONE translation unit.  Every function template below is written once and
 // instantiated twice -- with the reference's classes and with the shim's -- so it only compiles if the shim offers the same
 // member names, overloads and argument order GLIM's call sites use (odometry_estimation_imu.cpp:313-328, sub_mapping.cpp:365,:376,
-// cloud_preprocessor.cpp:77).  Built by tests/test_cpp_shim.py where /root/reference exists.
+// cloud_preprocessor.cpp:77).  A manual check, not run by the test suite (GLIM's headers are not part of this repository):
+//   g++ -std=c++17 -fsyntax-only -Ioracle/ref_shim -I<GLIM source tree>/include -Iinclude tests/cpp/api_conformance.cpp
 #include <glim/common/cloud_covariance_estimation.hpp>
 #include <glim/common/cloud_deskewing.hpp>
 #include <glim/preprocess/cloud_preprocessor.hpp>

@@ -1,12 +1,13 @@
 """Extracts the shipped parameter values the hot path's call sites are constructed with from the reference's own config files
-(/root/reference/config/*.json, JSON with // comments) into tests/golden/reference_config_values.json.  The fixture travels (the
-GPU box has no /root/reference); tests/test_reference_config_values.py checks the product's defaults against it and, where the
-reference tree is present, that the fixture is still what the files say.  Run: python tests/golden/make_reference_config_fixture.py"""
+(<GLIM source tree>/config/*.json, JSON with // comments) into tests/golden/reference_config_values.json;
+tests/test_reference_config_values.py checks the product's defaults against it.
+Run: python tests/golden/make_reference_config_fixture.py <GLIM source tree>"""
 import json
 import os
 import re
+import sys
 
-REF = "/root/reference/config"
+REF = None  # <GLIM source tree>/config, from the command line
 FILES = ["config_preprocess", "config_odometry_gpu", "config_odometry_cpu", "config_sub_mapping_gpu", "config_global_mapping_gpu"]
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_config_values.json")
 
@@ -43,6 +44,7 @@ def extract():
 
 
 if __name__ == "__main__":
+    REF = os.path.join(sys.argv[1], "config")
     with open(OUT, "w") as f:
         json.dump(extract(), f, indent=1, sort_keys=True)
     print("wrote", OUT)

@@ -27,11 +27,11 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(L, name), name
 
 
-def test_library_is_sm100a_only_and_links_no_torch():
+def test_library_is_sm90a_only_and_links_no_torch():
     out = os.popen(f"cuobjdump --list-elf {capi.SO_PATH} 2>/dev/null").read()
     if out.strip():
         archs = set(re.findall(r"sm_(\d+a?)", out))
-        assert archs == {"100a"}, archs
+        assert archs == {"90a"}, archs
     # library NAMES only: the load addresses ldd prints are random hex strings (ASLR) and may well contain "c10"
     libs = [line.split()[0] for line in os.popen(f"ldd {capi.SO_PATH}").read().splitlines() if line.strip()]
     assert libs and not [l for l in libs if "torch" in l or "c10" in l], libs

@@ -2,7 +2,7 @@
 
 CPU: the oracle's two overloads against an independent numpy / scipy implementation; the product's HOST half
 (gb_deskew_pose_table: time table + pose per slot, needs no device) against the oracle.
-GPU: the kernel (gb_deskew) against the oracle (first passed on the driver's B200 at the end of round 1)."""
+GPU: the kernel (gb_deskew) against the oracle."""
 import numpy as np
 import pytest
 

@@ -1,4 +1,4 @@
-"""Multi-GPU tests on a real box (skipped unless >= 2 B200s are visible): bench.py under torchrun with every result-exchange
+"""Multi-GPU tests on a real box (skipped unless >= 2 H100s are visible): bench.py under torchrun with every result-exchange
 path (peer push from the sweep, peer push by the exchange kernel, NCCL all-reduce) must give the same Hessian slab checksum
 as a single GPU."""
 import json

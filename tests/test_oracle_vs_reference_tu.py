@@ -1,18 +1,17 @@
 """The oracle (and the product's host halves) against the reference's OWN translation units.
 
-oracle/_ref/libglim_ref.so = /root/reference/src/glim/common/cloud_covariance_estimation.cpp and cloud_deskewing.cpp compiled
-UNMODIFIED, from where they lie, against the stand-in headers of oracle/ref_shim/ (recipe: `make -C oracle _ref`; Eigen, GTSAM,
+tests/golden/reference_tu_golden.npz = what GLIM's cloud_covariance_estimation.cpp, cloud_deskewing.cpp and cloud_preprocessor.cpp
+compute, compiled UNMODIFIED against the stand-in headers of oracle/ref_shim/ (recipe: `make -C oracle _ref`; Eigen, GTSAM,
 spdlog and gtsam_points are not installed here, the stand-ins are written in this repository).  What that pins: the control flow
 and formulas of those two files -- neighbour indexing, population covariance, the PLANE regularization constants, (3,3) = 0, the
 normal's flip towards the sensor, the 0.1 ms time table, the IMU cursor / clamp / held-last-pose rules, the composition order of the
 transforms.  What it does not: Eigen's and GTSAM's own arithmetic (direct 3x3 eigen-solver, quaternion slerp, Pose3::Expmap), which
 the stand-ins restate from the published algorithms.  The VGICP factor itself lives in gtsam_points and stays unpinned.
 
-The .so is a build product (git-ignored); it is built in the container that has /root/reference and travels to the GPU box.
-Without it (fresh checkout elsewhere) these tests skip."""
+Recorded by tests/golden/make_reference_tu_golden.py: per-point outputs for a fixed, seeded sample of rows, exact ones as digests."""
 import ctypes as C
+import hashlib
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -23,24 +22,35 @@ from tests.test_deskew import IMU_P, IMU_T, T_IL, V, W, scan_like
 from tests.util import scan_pair
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "oracle", "_ref", "libglim_ref.so")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_tu_golden.npz")
+
+CONST_VEL_CASES = {"vw": (V, W), "v": (V, np.zeros(3)), "w": (np.zeros(3), W), "none": (np.zeros(3), np.zeros(3))}
+# (shift of the IMU times, number of IMU poses): all of them; poses that end before the scan does; a scan that starts before them
+IMU_CASES = {"full": (0.0, len(IMU_T)), "short": (0.0, 6), "late": (0.05, len(IMU_T))}
+CROP_LO, CROP_HI = np.array([-3.0, -2.0, -5.0]), np.array([4.0, 2.5, 5.0])
+T_IMU_CROP = synth.pose(0.5, -0.2, 0.1, 0.4, 0.0, 0.0)
+RANDOM_TARGET = 2000
 
 
 @pytest.fixture(scope="module")
 def ref():
-    if os.path.isdir("/root/reference/src/glim/common"):
-        subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-s", "_ref"])
-    if not os.path.exists(SO):
-        pytest.skip("oracle/_ref/libglim_ref.so is not built (needs /root/reference: make -C oracle _ref)")
-    L = C.CDLL(SO)
-    vp, i32 = C.c_void_p, C.c_int
-    L.ref_covariance_estimate.argtypes = [i32, vp, vp, i32, i32, i32, vp, vp]
-    L.ref_covariance_estimate_sample.argtypes = [i32, vp, vp, i32, i32, vp]
-    L.ref_deskew_const_vel.argtypes = [vp, vp, vp, i32, vp, vp, vp]
-    L.ref_deskew_imu.argtypes = [vp, i32, vp, vp, C.c_double, i32, vp, vp, vp]
-    return L
+    with np.load(GOLDEN) as g:
+        return {k: g[k] for k in g.files}
 
 
+def sample_rows(n, k=256):
+    """the rows of an n-point output that the golden file keeps"""
+    return np.sort(np.random.default_rng(20240).choice(n, min(k, n), replace=False))
+
+
+def digest(a):
+    """SHA-256 of an array's shape and values (as fp64 with -0.0 -> 0.0, or int64): equal digests <=> np.array_equal"""
+    a = np.ascontiguousarray(a)
+    a = a.astype(np.float64) + 0.0 if a.dtype.kind == "f" else a.astype(np.int64)
+    return hashlib.sha256(repr(a.shape).encode() + a.tobytes()).hexdigest()
+
+
+# the calls into oracle/_ref/libglim_ref.so whose results tests/golden/make_reference_tu_golden.py records
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
@@ -69,33 +79,43 @@ def test_covariance_oracle_equals_reference_translation_unit(ref, k):
     sp = scan_pair()
     pts = sp["points"][0]
     nb = synth.knn(pts, 10).astype(np.int32)
-    n_ref, c_ref = ref_cov(ref, pts, nb, k)
+    rows = sample_rows(len(pts))
+    n_ref, c_ref = ref[f"cov0_k{k}/normals"], ref[f"cov0_k{k}/covs"]
     n_orc, c_orc = oracle.covariance_estimate(pts, nb, k_neighbors=k, num_threads=2)
-    ok = well_conditioned(pts, nb, k)
-    assert ok.mean() > 0.9
+    n_orc, c_orc = n_orc[rows], c_orc[rows]
+    assert well_conditioned(pts, nb, k).mean() > 0.9
+    ok = well_conditioned(pts, nb, k)[rows]
     assert np.abs(c_ref[ok] - c_orc[ok]).max() < 1e-10
     assert np.abs(n_ref[ok] - n_orc[ok]).max() < 1e-10  # same sign: both flip towards the sensor origin
-    loose = well_conditioned(pts, nb, k, 1e-6)           # nearly isotropic in the plane's normal direction: 1e-13 / gap
+    loose = well_conditioned(pts, nb, k, 1e-6)[rows]     # nearly isotropic in the plane's normal direction: 1e-13 / gap
     assert np.abs(c_ref[loose] - c_orc[loose]).max() < 1e-6
     # invariants the reference file enforces on EVERY point, conditioned or not
-    for c, nr in ((c_ref, n_ref), (c_orc, n_orc)):
+    for c, nr, p in ((c_ref, n_ref, pts[rows]), (c_orc, n_orc, pts[rows])):
         assert np.all(c[:, 3, :] == 0) and np.all(c[:, :, 3] == 0) and np.all(nr[:, 3] == 0)
-        assert np.all(np.einsum("ni,ni->n", pts, nr) <= 1e-12)
+        assert np.all(np.einsum("ni,ni->n", p, nr) <= 1e-12)
         assert np.allclose(np.linalg.eigvalsh(c[:, :3, :3]), [1e-3, 1.0, 1.0], atol=1e-9)
 
 
 def test_plane_regularization_makes_the_divisor_irrelevant(ref):
     """SURVEY C.4: the (points, neighbors, k) overload divides by k - 1 (cloud_covariance_estimation.cpp:153) -- irrelevant under
-    PLANE because only the eigenvectors survive.  Checked on the reference code itself."""
+    PLANE because only the eigenvectors survive.  Checked on the reference code's own results."""
     sp = scan_pair()
     pts = sp["points"][1]
     nb = synth.knn(pts, 10).astype(np.int32)
-    _, c_pop = ref_cov(ref, pts, nb)
-    c_smp = np.zeros((len(pts), 16))
-    ref.ref_covariance_estimate_sample(len(pts), _p(np.ascontiguousarray(pts)), _p(nb), 10, 10, _p(c_smp))
-    c_smp = c_smp.reshape(-1, 4, 4).transpose(0, 2, 1)
-    ok = well_conditioned(pts, nb, 10)
+    c_pop, c_smp = ref["cov1_k10/covs"], ref["cov1_sample/covs"]
+    ok = well_conditioned(pts, nb, 10)[sample_rows(len(pts))]
+    assert ok.mean() > 0.9
     assert np.abs(c_pop[ok] - c_smp[ok]).max() < 1e-9
+
+
+def ref_deskew(ref, seed, times):
+    """the reference's deskewed points of the scan_like(seed) scan: {case: sampled rows}, and the rows"""
+    return {k.split("/", 1)[1]: v for k, v in ref.items() if k.startswith(f"deskew{seed}/")}, sample_rows(len(times))
+
+
+def imu_case(name):
+    dt, m = IMU_CASES[name]
+    return IMU_T[:m] + dt, IMU_P[:m]
 
 
 def ref_deskew_cv(L, T, v, w, times, pts):
@@ -114,13 +134,14 @@ def ref_deskew_imu(L, T, imu_t, imu_p, stamp, times, pts):
 
 def test_deskew_oracle_equals_reference_translation_unit(ref):
     times, pts = scan_like(seed=3)
-    for v, w in ((V, W), (V, np.zeros(3)), (np.zeros(3), W), (np.zeros(3), np.zeros(3))):
-        assert np.abs(ref_deskew_cv(ref, T_IL, v, w, times, pts) - oracle.deskew_const_vel(T_IL, v, w, times, pts)).max() < 1e-11
-    assert np.abs(ref_deskew_imu(ref, T_IL, IMU_T, IMU_P, 100.0, times, pts) - oracle.deskew_imu(T_IL, IMU_T, IMU_P, 100.0, times, pts)).max() < 1e-11
-    # IMU poses that end before the scan does: the last pose is held (cloud_deskewing.cpp:104-105)
-    assert np.abs(ref_deskew_imu(ref, T_IL, IMU_T[:6], IMU_P[:6], 100.0, times, pts) - oracle.deskew_imu(T_IL, IMU_T[:6], IMU_P[:6], 100.0, times, pts)).max() < 1e-11
-    # a scan that starts before the first IMU pose: p is clamped to 0 (:111)
-    assert np.abs(ref_deskew_imu(ref, T_IL, IMU_T + 0.05, IMU_P, 100.0, times, pts) - oracle.deskew_imu(T_IL, IMU_T + 0.05, IMU_P, 100.0, times, pts)).max() < 1e-11
+    got, rows = ref_deskew(ref, 3, times)
+    for name, (v, w) in CONST_VEL_CASES.items():
+        assert np.abs(got[f"cv_{name}"] - oracle.deskew_const_vel(T_IL, v, w, times, pts)[rows]).max() < 1e-11
+    # "short": IMU poses that end before the scan does: the last pose is held (cloud_deskewing.cpp:104-105);
+    # "late": a scan that starts before the first IMU pose: p is clamped to 0 (:111)
+    for name in IMU_CASES:
+        it, ip = imu_case(name)
+        assert np.abs(got[f"imu_{name}"] - oracle.deskew_imu(T_IL, it, ip, 100.0, times, pts)[rows]).max() < 1e-11
 
 
 def test_product_host_pose_table_equals_reference_translation_unit(ref):
@@ -128,10 +149,11 @@ def test_product_host_pose_table_equals_reference_translation_unit(ref):
     from glim_b200 import preprocess
 
     times, pts = scan_like(seed=4)
+    got, rows = ref_deskew(ref, 4, times)
     idx, Ts = preprocess.deskew_pose_table(T_IL, times, linear_vel=V, angular_vel=W)
-    assert np.abs(np.einsum("nij,nj->ni", Ts[idx], pts) - ref_deskew_cv(ref, T_IL, V, W, times, pts)).max() < 1e-11
+    assert np.abs(np.einsum("nij,nj->ni", Ts[idx], pts)[rows] - got["cv_vw"]).max() < 1e-11
     idx, Ts = preprocess.deskew_pose_table(T_IL, times, imu_times=IMU_T, imu_poses=IMU_P, stamp=100.0)
-    assert np.abs(np.einsum("nij,nj->ni", Ts[idx], pts) - ref_deskew_imu(ref, T_IL, IMU_T, IMU_P, 100.0, times, pts)).max() < 1e-11
+    assert np.abs(np.einsum("nij,nj->ni", Ts[idx], pts)[rows] - got["imu_full"]).max() < 1e-11
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -169,13 +191,30 @@ def ref_preprocess(L, P, T, stamp=10.0, intensities=None, **kw):
     return op[:m], ot[:m], oi[:m], nb[:m], end.value, list(seen)
 
 
-@pytest.fixture(scope="module")
-def frame():
+def make_frame():
     sc = synth.make_hall_scene()
     P, T = synth.scan(sc, "hdl32", synth.arc_trajectory(8)[2], synth.rng_for(41), n_rays=32 * 250)
     P = P.copy()
     P[17, 1] = np.nan  # dropped by the finite gate (cloud_preprocessor.cpp:123)
     return P, T
+
+
+def intensities(P):
+    return np.linspace(0.0, 1.0, len(P))
+
+
+def preprocess_cases():
+    """{name: (reference parameters, oracle composition arguments)}"""
+    return {
+        "voxelgrid": (dict(), dict()),
+        "cropbox lidar": (dict(crop_bbox_frame=1, crop_bbox_min=CROP_LO, crop_bbox_max=CROP_HI), dict(crop=(CROP_LO, CROP_HI))),
+        "outliers": (dict(enable_outlier_removal=1, outlier_removal_k=8, outlier_std_mul_factor=1.0), dict(sor=(8, 1.0))),
+    }
+
+
+@pytest.fixture(scope="module")
+def frame():
+    return make_frame()
 
 
 def canonical(pts, tms, nb, extra=None):
@@ -195,55 +234,47 @@ def test_preprocess_composition_equals_reference_translation_unit(ref, frame):
     from tests.test_gpu_parity import _cpu_frame
 
     P, T = frame
-    lo, hi = np.array([-3.0, -2.0, -5.0]), np.array([4.0, 2.5, 5.0])
-    cases = {
-        "voxelgrid": (dict(), dict()),
-        "cropbox lidar": (dict(crop_bbox_frame=1, crop_bbox_min=lo, crop_bbox_max=hi), dict(crop=(lo, hi))),
-        "outliers": (dict(enable_outlier_removal=1, outlier_removal_k=8, outlier_std_mul_factor=1.0), dict(sor=(8, 1.0))),
-    }
-    for name, (rkw, okw) in cases.items():
-        pts, tms, _, nb, end, seen = ref_preprocess(ref, P, T, **rkw)
+    for name, (_, okw) in preprocess_cases().items():
+        g = f"pre_{name}/"
         o_pts, o_tms, o_nb, _, _ = _cpu_frame(P, T, 0.2, 1.0, 60.0, 10, **okw)
-        assert len(pts) == len(o_pts) > 1000, name
-        assert np.array_equal(tms, o_tms), name  # the sequence of times is order-free
-        for a, b in zip(canonical(pts, tms, nb), canonical(o_pts, o_tms, o_nb)):
-            assert np.array_equal(a, b), name
-        assert end == 10.0 + o_tms[-1], name
+        assert ref[g + "n"] == len(o_pts) > 1000, name
+        assert ref[g + "tms"] == digest(o_tms), name  # the sequence of times is order-free
+        assert list(ref[g + "canonical"]) == [digest(a) for a in canonical(o_pts, o_tms, o_nb)], name
+        assert ref[g + "end"] == 10.0 + o_tms[-1], name
     # the code defaults of CloudPreprocessorParams (cloud_preprocessor.cpp:27-36,58) as the product's gb_preprocess_default_params
     # documents them next to the shipped config
-    assert seen == [1.0, 100.0, 0.15, 0.3, 2.0, 8.0]
+    assert list(ref["pre_voxelgrid/seen"]) == [1.0, 100.0, 0.15, 0.3, 2.0, 8.0]
     # random grid: rate = target / N (cloud_preprocessor.cpp:105), survivors keep their order, then the same gates
-    target = 2000
-    pts, tms, _, nb, _, _ = ref_preprocess(ref, P, T, use_random_grid_downsampling=1, downsample_resolution=1.0, downsample_target=target, seed=5)
-    mask = oracle.randomgrid_sampling(P, 1.0, target / len(P), seed=5)
+    mask = oracle.randomgrid_sampling(P, 1.0, RANDOM_TARGET / len(P), seed=5)
     o_pts, o_tms, o_nb, _, _ = _cpu_frame(P, T, None, 1.0, 60.0, 10, mask=mask)
-    assert len(pts) == len(o_pts) > 500
-    for a, b in zip(canonical(pts, tms, nb), canonical(o_pts, o_tms, o_nb)):
-        assert np.array_equal(a, b)
+    assert ref["pre_randomgrid/n"] == len(o_pts) > 500
+    assert list(ref["pre_randomgrid/canonical"]) == [digest(a) for a in canonical(o_pts, o_tms, o_nb)]
+
+
+def global_shutter_oracle(P, T):
+    """the oracle's voxel grid + gates of the global-shutter frame, ordered by the ORIGINAL times: (points, times, intensities)"""
+    o_pts, o_tms, o_it = oracle.voxelgrid_sampling(P, 0.2, times=T, intensities=intensities(P))
+    sq = (o_pts[:, :3] ** 2).sum(1)
+    keep = np.nonzero((sq > 1.0) & (sq < 3600.0) & np.isfinite(o_pts).all(1))[0]
+    keep = keep[np.argsort(o_tms[keep], kind="stable")]
+    return o_pts[keep], o_tms[keep], o_it[keep]
 
 
 def test_preprocess_global_shutter_intensities_and_imu_crop_box(ref, frame):
     P, T = frame
-    inten = np.linspace(0.0, 1.0, len(P))
-    pts, tms, it, nb, end, _ = ref_preprocess(ref, P, T, intensities=inten, global_shutter=1)
     # global shutter: the points are still ordered by their ORIGINAL times, then every time becomes 0 (:135-140) -> scan_end_time = stamp
-    o_pts, o_tms, o_it = oracle.voxelgrid_sampling(P, 0.2, times=T, intensities=inten)
-    sq = (o_pts[:, :3] ** 2).sum(1)
-    keep = np.nonzero((sq > 1.0) & (sq < 3600.0) & np.isfinite(o_pts).all(1))[0]
-    keep = keep[np.argsort(o_tms[keep], kind="stable")]
-    assert np.all(tms == 0.0) and end == 10.0
-    zero_nb = np.zeros((len(pts), 1), np.int64)
-    got, want = canonical(pts, o_tms[keep], zero_nb, it), canonical(o_pts[keep], o_tms[keep], zero_nb, o_it[keep])
-    assert np.array_equal(got[0], want[0]) and np.array_equal(got[3], want[3])  # intensities travel with the points
+    o_pts, o_tms, o_it = global_shutter_oracle(P, T)
+    assert ref["pre_global_shutter/tms_all_zero"] and ref["pre_global_shutter/end"] == 10.0
+    zero_nb = np.zeros((len(o_pts), 1), np.int64)
+    want = canonical(o_pts, o_tms, zero_nb, o_it)
+    got = ref["pre_global_shutter/shutter_canonical"]  # the reference's points / intensities, ordered by the oracle's original times
+    assert got[0] == digest(want[0]) and got[1] == digest(want[3])  # intensities travel with the points
     # crop box given in the IMU frame: p_imu = T_imu_lidar * p_lidar (:152-157); points INSIDE the box are removed
-    T_il = synth.pose(0.5, -0.2, 0.1, 0.4, 0.0, 0.0)
-    lo, hi = np.array([-3.0, -2.0, -5.0]), np.array([4.0, 2.5, 5.0])
-    pts2, _, _, _, _, _ = ref_preprocess(ref, P, T, crop_bbox_frame=2, crop_bbox_min=lo, crop_bbox_max=hi, T_imu_lidar=T_il)
-    base = o_pts[keep]
-    p_imu = base[:, :3] @ T_il[:3, :3].T + T_il[:3, 3]
-    inside = (p_imu >= lo).all(1) & (p_imu <= hi).all(1)
-    assert 0 < inside.sum() < len(base)
-    assert np.array_equal(pts2[np.lexsort(pts2[:, :3].T)], base[~inside][np.lexsort(base[~inside][:, :3].T)])
+    p_imu = o_pts[:, :3] @ T_IMU_CROP[:3, :3].T + T_IMU_CROP[:3, 3]
+    inside = (p_imu >= CROP_LO).all(1) & (p_imu <= CROP_HI).all(1)
+    assert 0 < inside.sum() < len(o_pts)
+    kept = o_pts[~inside]
+    assert ref["pre_imu_crop/points_sorted"] == digest(kept[np.lexsort(kept[:, :3].T)])
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -260,8 +291,7 @@ def test_stand_in_primitives_eigen_solver(ref):
             w[0] = w[1] * 1e-6  # a flat neighbourhood: smallest eigenvalue far below the others
         A = (Q * w) @ Q.T
         A = 0.5 * (A + A.T) * rng.choice([1e-3, 1.0, 1e3])
-        vals, vecs = np.zeros(3), np.zeros(9)
-        ref.ref_shim_eigen_sym3(_p(np.ascontiguousarray(A.T.reshape(9))), _p(vals), _p(vecs))
+        vals, vecs = ref["eigen/vals"][trial], ref["eigen/vecs"][trial]
         V = vecs.reshape(3, 3).T
         ew, eV = np.linalg.eigh(A)
         scale = np.abs(ew).max()
@@ -279,16 +309,13 @@ def test_stand_in_primitives_slerp_and_expmap(ref):
     from scipy.spatial.transform import Rotation as Rot, Slerp
 
     rng = np.random.default_rng(12)
-    for _ in range(200):
+    for trial in range(200):
         r0, r1 = Rot.from_rotvec(rng.normal(size=3) * rng.uniform(0, 2.5)), Rot.from_rotvec(rng.normal(size=3) * rng.uniform(0, 2.5))
         t = float(rng.uniform(0, 1))
-        out = np.zeros(9)
-        ref.ref_shim_slerp.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p]
-        ref.ref_shim_slerp(_p(np.ascontiguousarray(r0.as_matrix().T.reshape(9))), _p(np.ascontiguousarray(r1.as_matrix().T.reshape(9))), t, _p(out))
+        out = ref["slerp/out"][trial]
         want = Slerp([0, 1], Rot.from_matrix([r0.as_matrix(), r1.as_matrix()]))([t])[0].as_matrix()
         assert np.abs(out.reshape(3, 3).T - want).max() < 1e-12
-    for _ in range(200):
+    for trial in range(200):
         xi = np.concatenate([rng.normal(size=3) * rng.choice([0.0, 1e-9, 0.3, 2.0]), rng.normal(size=3) * 3.0])
-        T = np.zeros(16)
-        ref.ref_shim_pose3_expmap(_p(xi), _p(T))
+        T = ref["expmap/out"][trial]
         assert np.abs(T.reshape(4, 4).T - synth.se3_exp(xi)).max() < 1e-12  # synth.se3_exp: the closed form with the V(omega) matrix
