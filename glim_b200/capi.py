@@ -26,6 +26,7 @@ SYMBOLS = [
     "gb_peer_slab_signal_wait", "gb_peer_slab_device_ptr", "gb_peer_slab_fetch", "gb_peer_slab_fetch_async",
     "gb_overlap", "gb_covariances", "gb_find_neighbors", "gb_voxelgrid_sampling", "gb_preprocess_default_params", "gb_preprocess", "gb_merge_frames",
     "gb_deskew_pose_table", "gb_deskew",
+    "gb_align_default_params", "gb_vgicp_align",
 ]
 
 GB_SLAB_STRIDE = 96
@@ -50,6 +51,22 @@ class Preprocessed(C.Structure):
     _fields_ = [("num_points", C.c_size_t), ("last_time", C.c_double), ("times", C.c_void_p), ("xyzw", C.c_void_p), ("intensities", C.c_void_p), ("neighbors", C.c_void_p),
                 ("normals4", C.c_void_p), ("cov4x4", C.c_void_p), ("cloud", C.c_void_p)]
 
+
+class AlignParams(C.Structure):
+    """gb_align_params (include/glim_b200.h)."""
+    _fields_ = [("max_iterations", C.c_int), ("lambda_initial", C.c_double), ("lambda_factor", C.c_double), ("lambda_upper_bound", C.c_double),
+                ("relative_error_tol", C.c_double), ("absolute_error_tol", C.c_double), ("step_translation_tol", C.c_double), ("step_rotation_tol", C.c_double)]
+
+
+class AlignResult(C.Structure):
+    """gb_align_result (include/glim_b200.h)."""
+    _fields_ = [("T_target_source", C.c_double * 16), ("error", C.c_double), ("num_inliers", C.c_double), ("lambda_", C.c_double),
+                ("iterations", C.c_int), ("trials", C.c_int), ("status", C.c_int)]
+
+
+# gb_align_result::status
+ALIGN_CONVERGED, ALIGN_MAX_ITERATIONS, ALIGN_LAMBDA_EXCEEDED, ALIGN_DEGENERATE = 0, 1, 2, 3
+ALIGN_STATUS_NAMES = {0: "CONVERGED", 1: "MAX_ITERATIONS", 2: "LAMBDA_EXCEEDED", 3: "DEGENERATE"}
 
 _lib = None
 
@@ -120,6 +137,8 @@ def lib():
     L.gb_voxelgrid_sampling.argtypes = [vp, sz, vp, vp, vp, f64, vp, vp, vp, vp]
     L.gb_deskew_pose_table.argtypes = [vp, vp, vp, sz, vp, vp, f64, sz, vp, vp, vp, vp]
     L.gb_deskew.argtypes = [vp, vp, vp, vp, sz, vp, vp, f64, sz, vp, vp, vp, vp]
+    L.gb_align_default_params.argtypes = [vp]
+    L.gb_vgicp_align.argtypes = [vp, sz, vp, vp, vp, vp, vp]
     for name in SYMBOLS:
         getattr(L, name)  # AttributeError here means the library and include/glim_b200.h are out of sync
     _lib = L

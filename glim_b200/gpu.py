@@ -8,6 +8,8 @@ include/glim_b200/gtsam_points_compat.hpp.
     IntegratedVGICPFactorGPU(target_key | fixed_target_pose, source_key, voxelmap, source)   :144, :161
     NonlinearFactorSetGPU.add(...) / .linearize(values)     odometry_estimation_gpu.cpp:383-386
     overlap_gpu(voxelmap(s), source, delta(s))              odometry_estimation_gpu.cpp:231, :248
+    align_vgicp(problems, T_init, params)                   the LM loop of odometry_estimation_cpu.cpp:105-150 /
+                                                            global_mapping_pose_graph.cpp:405-417, many problems per call
 """
 from __future__ import annotations
 
@@ -379,6 +381,43 @@ class PeerSlab:
         if getattr(self, "h", None) and self.ctx.h:
             lib().gb_peer_slab_destroy(self.h)
             self.h = None
+
+
+def align_params(**overrides) -> capi.AlignParams:
+    """gb_align_default_params (the odometry_estimation_cpu values) with the given fields replaced."""
+    p = capi.AlignParams()
+    check(lib().gb_align_default_params(C.byref(p)))
+    for k, v in overrides.items():
+        if k not in dict(capi.AlignParams._fields_):
+            raise capi.GlimB200Error(f"gb_align_params has no field {k!r}")
+        setattr(p, k, v)
+    return p
+
+
+def align_vgicp(problems: list[list[IntegratedVGICPFactorGPU]], T_init, params=None, ctx: Context | None = None) -> list[dict]:
+    """gb_vgicp_align: Levenberg-Marquardt registration of every problem in one call (odometry_estimation_cpu.cpp:105-150,
+    global_mapping_pose_graph.cpp:405-417).  problems[p] = the factors (levels) of problem p, used as unary factors on
+    T_target_source with the target fixed at identity (their keys are not read); T_init: (P,4,4) or one (4,4) per problem;
+    params: None (defaults), a dict of field overrides or a capi.AlignParams.
+    -> per problem {T_target_source (4,4), error, num_inliers, lambda, iterations, trials, status, status_name}"""
+    P = len(problems)
+    if P == 0:
+        return []
+    if params is None or isinstance(params, dict):
+        params = align_params(**(params or {}))
+    flat = [f for prob in problems for f in prob]
+    ctx = ctx or (flat[0].ctx if flat else default_context())
+    off = np.zeros(P + 1, np.uint64)
+    off[1:] = np.cumsum([len(prob) for prob in problems])
+    T0 = pose16(np.asarray(T_init, dtype=np.float64).reshape(P, 4, 4))
+    arr = (C.c_void_p * max(1, len(flat)))(*[f._handle() for f in flat])
+    res = (capi.AlignResult * P)()
+    check(lib().gb_vgicp_align(ctx.h, P, ptr(off), C.cast(arr, C.c_void_p), ptr(T0), C.byref(params), C.cast(res, C.c_void_p)))
+    return [{
+        "T_target_source": np.array(r.T_target_source[:]).reshape(4, 4).T.copy(),
+        "error": r.error, "num_inliers": r.num_inliers, "lambda": r.lambda_,
+        "iterations": r.iterations, "trials": r.trials, "status": r.status, "status_name": capi.ALIGN_STATUS_NAMES.get(r.status, "?"),
+    } for r in res]
 
 
 def overlap_gpu(voxelmaps, source: PointCloudGPU, deltas, ctx: Context | None = None) -> float:

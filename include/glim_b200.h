@@ -133,6 +133,56 @@ GB_API gb_status gb_vgicp_error(gb_factor* factor, const double T_lin[16], const
 GB_API gb_status gb_factor_set_linearize(gb_ctx* ctx, size_t num_factors, gb_factor* const* factors, const double* T_target_source /* F x 16 */, gb_linearized6* out /* F */);
 GB_API gb_status gb_factor_set_error(gb_ctx* ctx, size_t num_factors, gb_factor* const* factors, const double* T_lin /* F x 16 */, const double* T_eval /* F x 16 */, double* errors /* F */);
 
+/* ---- Scan registration: Levenberg-Marquardt on VGICP factors, many problems in one call
+ *      (odometry_estimation_cpu.cpp:105-150: one unary IntegratedVGICPFactor(Pose3(), X(current), voxelmap, frame) per level,
+ *      LevenbergMarquardtOptimizerExt; global_mapping_pose_graph.cpp:405-417: loop candidates, 10 iterations each).
+ *      A problem is the set of factors (levels) that share one unknown T_target_source, the target pose fixed to identity;
+ *      the factors of problem p are factors[factor_offsets[p] .. factor_offsets[p+1]).  Factors keep their flags.
+ *
+ *      The rule (gtsam_points' LevenbergMarquardtOptimizerExt is not vendored: GTSAM's documented LM defaults plus GLIM's
+ *      termination callback, DESIGN.md section 7 [EXT]).  Per problem, T = T_init, lambda = lambda_initial, need_lin = 1;
+ *      while the problem is active:
+ *        1. if need_lin: linearize every factor at T; H = sum H_ss, b = sum b_s, e = sum error, n = sum num_inliers
+ *           (record order, fp64); iterations += 1.  n == 0 on the first linearization: stop, DEGENERATE, T = T_init.
+ *        2. solve (H + lambda I) delta = -b by a 6x6 fp64 Cholesky (tangent [rot; trans]); a failed factorization is a
+ *           rejected trial.  T' = T Exp(delta); trials += 1.
+ *        3. e' = sum error(T_lin = T, T_eval = T') (inliers of T, residuals at T').
+ *        4. e' < e: accept: T = T', lambda /= lambda_factor, need_lin = 1, then the first that holds:
+ *             CONVERGED if |t(Exp(delta))| < step_translation_tol and |w| < step_rotation_tol, unless both are < 1e-10;
+ *             CONVERGED if e - e' <= absolute_error_tol or (e - e') / e <= relative_error_tol;
+ *             MAX_ITERATIONS if iterations >= max_iterations;
+ *           and in every case e = e'.
+ *        5. otherwise reject: lambda *= lambda_factor, need_lin = 0; LAMBDA_EXCEEDED if lambda > lambda_upper_bound.
+ *      Each round is at most four launches for the whole batch (linearize sweep if any problem needs it, solve, error
+ *      sweep, accept) and one small device-to-host copy; finished problems are swept until the whole batch has finished. ---- */
+#define GB_ALIGN_CONVERGED 0
+#define GB_ALIGN_MAX_ITERATIONS 1
+#define GB_ALIGN_LAMBDA_EXCEEDED 2
+#define GB_ALIGN_DEGENERATE 3
+typedef struct gb_align_params {
+  int max_iterations;          /* linearizations per problem (8: config_odometry_cpu.json:23; 10: global_mapping_pose_graph.cpp:412) */
+  double lambda_initial;       /* 1e-5 (> 0) */
+  double lambda_factor;        /* 10 (> 1) */
+  double lambda_upper_bound;   /* 1e5 (finite) */
+  double relative_error_tol;   /* 1e-5 */
+  double absolute_error_tol;   /* 0.1 (odometry_estimation_cpu.cpp:118) */
+  double step_translation_tol; /* 1e-3 m (odometry_estimation_cpu.cpp:135); <= 0 turns the step test off */
+  double step_rotation_tol;    /* 1e-3 deg in rad (same line); <= 0 turns the step test off */
+} gb_align_params;
+typedef struct gb_align_result {
+  double T_target_source[16];  /* column-major */
+  double error;                /* error of the returned pose with the inliers of its last linearization (what LM holds) */
+  double num_inliers;          /* of the last linearization (inlier_fraction = num_inliers / source size) */
+  double lambda;
+  int iterations, trials, status; /* GB_ALIGN_* */
+} gb_align_result;
+GB_API gb_status gb_align_default_params(gb_align_params* params); /* the odometry_estimation_cpu values above */
+/* Every input is validated before any launch: offsets must start at 0 and increase strictly (no empty problem), no factor
+ * may be NULL, T_init must be finite, and the parameters must satisfy the bounds above (and lambda_initial must not
+ * underflow to 0 within max_iterations accepted steps). */
+GB_API gb_status gb_vgicp_align(gb_ctx* ctx, size_t num_problems, const size_t* factor_offsets /* P + 1 */, gb_factor* const* factors,
+                                const double* T_init /* P x 16 */, const gb_align_params* params, gb_align_result* results /* P */);
+
 /* ---- Solver hand-off (SURVEY A.3; global_mapping.cpp:492-501 feeds these to isam2->update): the blocks of
  *      gtsam::HessianFactor(k_t, k_s, G11 = H_tt, G12 = H_ts, g1 = -b_t, G22 = H_ss, g2 = -b_s, f = error_scale * error),
  *      6x6 blocks column-major, from one factor record or from one fp32 row of the pair slab (levels pre-summed on the
