@@ -144,9 +144,6 @@ static gb_status ctx_create(int device, cudaStream_t stream, bool own, gb_ctx** 
     if (e != cudaSuccess) { delete c; gb_set_error("cudaStreamCreate: %s", cudaGetErrorString(e)); return GB_ERR_CUDA; }
   }
   c->num_sms = prop.multiProcessorCount;
-  c->scratch = nullptr; c->scratch_cap = 0;
-  c->pinned = nullptr; c->pinned_cap = 0;
-  c->launches = 0;
   c->refs.store(1);
   { DevPool& P = g_pools[device & 15]; std::lock_guard<std::mutex> lock(P.mu); P.ctxs.push_back(c); }
   *out = c;
@@ -225,30 +222,15 @@ gb_status gb_ctx_pinned(gb_ctx* ctx, size_t bytes, void** out) {
 // ---------------------------------------------------------------------------------------------
 // clouds
 // ---------------------------------------------------------------------------------------------
-static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
-extern "C" gb_status gb_cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, const double* cov4x4, const double* normals4, gb_cloud** out) {
-  GB_REQUIRE(ctx && out, "null ctx / output");
-  GB_REQUIRE(n == 0 || xyzw, "null points");
-  GB_REQUIRE(n < (size_t)1 << 30, "too many points");
-  *out = nullptr;
-  GB_CUDA(cudaSetDevice(ctx->device));
-  gb_cloud* c = new (std::nothrow) gb_cloud();
-  if (!c) return GB_ERR_INTERNAL;
-  c->device = ctx->device; c->n = n; c->base = nullptr; c->bytes = 0;
-  c->p0 = nullptr; c->p1 = nullptr; c->p2 = nullptr; c->normals = nullptr; c->perm = nullptr; c->inv_perm = nullptr;
-  if (n == 0) { *out = c; return GB_OK; }
-  // the reference casts Vector4d / Matrix4d to float on the host before the copy (SURVEY K1); so do we,
-  // straight into the device plane layout, staged through pinned memory
-  const size_t b0 = align_up(sizeof(float4) * n, 256), b1 = b0, b2 = align_up(sizeof(float) * n, 256), b3 = normals4 ? b0 : 0;
-  const size_t total = b0 + b1 + b2 + b3;
-  char* h = nullptr;
-  gb_status st = gb_ctx_pinned(ctx, total, (void**)&h);
-  if (st != GB_OK) { delete c; return st; }
-  float4* h0 = (float4*)h;
-  float4* h1 = (float4*)(h + b0);
-  float* h2 = (float*)(h + b0 + b1);
-  float4* h3 = (float4*)(h + b0 + b1 + b2);
+// the reference casts Vector4d / Matrix4d to float on the host before the copy (SURVEY K1); so do we, straight into the
+// plane layout in pinned memory, then stage the planes in scratch and Morton-sort them into the cloud on the device
+static gb_status cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, const double* cov4x4, const double* normals4, gb_cloud* c) {
+  Carver size;
+  gb_cloud_planes(size, n, normals4 != nullptr);
+  const size_t planes_b = size.off;
+  Carver hc;
+  GB_CHECK(gb_ctx_pinned(ctx, planes_b, (void**)&hc.base));
+  const gb_planes h = gb_cloud_planes(hc, n, normals4 != nullptr);
   // fp64 -> fp32 cast straight into the plane layout; split over a few host threads for large clouds (the single-threaded
   // loop was 1.6 ms for 60 k points and 25 ms for 500 k: more than everything the GPU does per frame)
   auto pack = [&](size_t i0, size_t i1) {
@@ -259,10 +241,10 @@ extern "C" gb_status gb_cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, 
         const double* C = cov4x4 + 16 * i;  // column-major 4x4: (r,c) at c*4+r; upper triangle
         c00 = (float)C[0]; c01 = (float)C[4]; c02 = (float)C[8]; c11 = (float)C[5]; c12 = (float)C[9]; c22 = (float)C[10];
       }
-      h0[i] = make_float4((float)p[0], (float)p[1], (float)p[2], c00);
-      h1[i] = make_float4(c01, c02, c11, c12);
-      h2[i] = c22;
-      if (normals4) h3[i] = make_float4((float)normals4[4 * i], (float)normals4[4 * i + 1], (float)normals4[4 * i + 2], 0.f);
+      h.p0[i] = make_float4((float)p[0], (float)p[1], (float)p[2], c00);
+      h.p1[i] = make_float4(c01, c02, c11, c12);
+      h.p2[i] = c22;
+      if (normals4) h.normals[i] = make_float4((float)normals4[4 * i], (float)normals4[4 * i + 1], (float)normals4[4 * i + 2], 0.f);
     }
   };
   {
@@ -278,25 +260,29 @@ extern "C" gb_status gb_cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, 
       for (auto& x : th) x.join();
     }
   }
-  const size_t bperm = align_up(sizeof(int) * n, 256);
-  cudaError_t e = gb_dev_malloc(ctx->device, total + 2 * bperm, &c->base);
-  if (e != cudaSuccess) { delete c; gb_set_error("cudaMalloc(%zu): %s", total + 2 * bperm, cudaGetErrorString(e)); return GB_ERR_OUT_OF_MEMORY; }
-  c->bytes = total + 2 * bperm;
-  char* d = (char*)c->base;
-  c->p0 = (float4*)d; c->p1 = (float4*)(d + b0); c->p2 = (float*)(d + b0 + b1); c->normals = normals4 ? (float4*)(d + b0 + b1 + b2) : nullptr;
-  c->perm = (int*)(d + total); c->inv_perm = (int*)(d + total + bperm);
-  // stage the planes in the caller's order in scratch, then Morton-sort them into place on the device
-  char* scratch = nullptr;
-  st = gb_ctx_scratch(ctx, gb_cloud_reorder_scratch_bytes(n, total), (void**)&scratch);
-  if (st == GB_OK) {
-    e = cudaMemcpyAsync(scratch, h, total, cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) { gb_set_error("upload: %s", cudaGetErrorString(e)); st = GB_ERR_CUDA; }
-  }
-  if (st == GB_OK) st = gb_cloud_reorder_impl(ctx, c, scratch, b0, b1, b2, b3);
-  if (st == GB_OK) {
-    e = cudaStreamSynchronize(ctx->stream);  // the pinned staging buffer is reused by the next call
-    if (e != cudaSuccess) { gb_set_error("upload: %s", cudaGetErrorString(e)); st = GB_ERR_CUDA; }
-  }
+  const size_t cub_b = gb_cub_temp_bytes(n);
+  gb_planes staged;
+  gb_sort_tmp t;
+  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+    staged = gb_cloud_planes(cv, n, normals4 != nullptr);
+    t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
+  }));
+  GB_CUDA(cudaMemcpyAsync(staged.p0, h.p0, planes_b, cudaMemcpyHostToDevice, ctx->stream));
+  GB_CHECK(gb_cloud_build(ctx, c, n, staged, t));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));  // the pinned staging buffer is reused by the next call
+  return GB_OK;
+}
+
+extern "C" gb_status gb_cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, const double* cov4x4, const double* normals4, gb_cloud** out) {
+  GB_REQUIRE(ctx && out, "null ctx / output");
+  GB_REQUIRE(n == 0 || xyzw, "null points");
+  GB_REQUIRE(n < (size_t)1 << 30, "too many points");
+  *out = nullptr;
+  GB_CUDA(cudaSetDevice(ctx->device));
+  gb_cloud* c = new (std::nothrow) gb_cloud();
+  if (!c) return GB_ERR_INTERNAL;
+  c->device = ctx->device;
+  const gb_status st = n > 0 ? cloud_upload(ctx, n, xyzw, cov4x4, normals4, c) : GB_OK;
   if (st != GB_OK) { gb_dev_free(ctx->device, c->base); delete c; return st; }
   *out = c;
   return GB_OK;
@@ -595,14 +581,6 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   if (!s) return GB_ERR_INTERNAL;
   ctx_retain(ctx);
   s->ctx = ctx; s->F = F; s->factors.assign(factors, factors + F);
-  s->d_descs = nullptr; s->d_tiles = nullptr; s->d_poses = nullptr; s->d_poses_eval = nullptr; s->d_accum = nullptr; s->d_done = nullptr; s->d_out = nullptr;
-  s->h_poses_eval = nullptr; s->h_out = nullptr; s->d_slab = nullptr; s->num_pairs = 0;
-  s->d_tile_ctr = nullptr; s->ctr_base = 0;
-  s->peer = nullptr; s->d_pair_ptr = nullptr; s->d_pair_factors = nullptr; s->d_pair_done = nullptr; s->d_peer_tables = nullptr;
-  s->num_tiles = 0; s->point_factors = 0; s->algorithmic_bytes = 0; s->key = 0; s->stale = false;
-  s->h_pose_slot[0] = s->h_pose_slot[1] = nullptr; s->pose_ev[0] = s->pose_ev[1] = nullptr; s->pose_slot = 0;
-  s->pool_d = nullptr; s->pool_d_cap = 0; s->pool_h = nullptr; s->pool_h_cap = 0;
-  s->graph_exec = nullptr; s->graph_state = 0;
 
   // kernel generation and work-item policy
   // Kernel policy (A/B runs of the kernels, scripts/ab_sweep.py): small sweeps -- about one item per warp: an odometry
@@ -615,8 +593,6 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   const bool small = F > 0 && total_pts <= warps * 2048;
   s->kernel_version = (kv == 3 || kv == 5) ? kv : (small ? 5 : 3);
   s->strided = (s->kernel_version == 5 && small && env_int("GB_STRIDED", 1)) ? 1 : 0;
-  s->calibrated = false;
-  s->h_descs = nullptr; s->h_tiles = nullptr; s->tiles_cap = 0;
   {
     // contiguous items: ~6 items per warp (first one static, the rest drawn dynamically), between 128 and 2048 points each,
     // in whole rows of 32 points
@@ -956,7 +932,7 @@ extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int worl
   if (!ps) return GB_ERR_INTERNAL;
   ps->ctx = ctx; ps->num_pairs = num_pairs; ps->world = world; ps->rank = rank;
   ps->buf_floats = align_up(num_pairs * GB_SLAB_STRIDE * sizeof(float), 256) / sizeof(float);
-  ps->local = nullptr; ps->step = 0; ps->parity = 0; ps->completed_parity = 0; ps->d_timeout = nullptr; ps->connected = (world == 1);
+  ps->connected = (world == 1);
   // fused: the sweep's epilogue stores every finished row straight into all peers; deferred: rows go to the local buffer and
   // the exchange kernel pushes them (see gb_launch_peer_signal_wait).  The peer stores' cost to the sweep grows with the
   // rank count faster than the exchange kernel's extra time -> fused up to 4 ranks, deferred above.  GB_PEER_PUSH=fused|deferred forces one.
@@ -966,8 +942,6 @@ extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int worl
     if (e && !strcmp(e, "fused")) ps->deferred = false;
     if (e && !strcmp(e, "deferred")) ps->deferred = true;
   }
-  ps->d_my_pairs = nullptr; ps->num_my_pairs = 0;
-  for (int p = 0; p < GB_MAX_PEERS; p++) { ps->peer[p] = nullptr; ps->opened[p] = false; }
   const size_t bytes = peer_alloc_bytes(num_pairs, world);
   cudaError_t e = cudaMalloc((void**)&ps->local, bytes + 256);
   if (e != cudaSuccess) { delete ps; gb_set_error("cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e)); return GB_ERR_OUT_OF_MEMORY; }
@@ -976,7 +950,6 @@ extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int worl
   if (e != cudaSuccess) { cudaFree(ps->local); delete ps; gb_set_error("peer slab init: %s", cudaGetErrorString(e)); return GB_ERR_CUDA; }
   ps->d_timeout = (int*)(ps->local + bytes);
   ps->peer[rank] = ps->local;
-  ps->h_pinned = nullptr;
   e = cudaMallocHost((void**)&ps->h_pinned, num_pairs * GB_SLAB_STRIDE * sizeof(float) + 64);
   if (e != cudaSuccess) { cudaFree(ps->local); delete ps; gb_set_error("cudaMallocHost: %s", cudaGetErrorString(e)); return GB_ERR_OUT_OF_MEMORY; }
   ctx_retain(ctx);
@@ -1193,8 +1166,7 @@ extern "C" gb_status gb_merge_frames(gb_ctx* ctx, size_t K, const gb_cloud* cons
   if (out_cloud) {
     c = new (std::nothrow) gb_cloud();
     if (!c) return GB_ERR_INTERNAL;
-    c->device = ctx->device; c->n = 0; c->base = nullptr; c->bytes = 0;
-    c->p0 = nullptr; c->p1 = nullptr; c->p2 = nullptr; c->normals = nullptr; c->perm = nullptr; c->inv_perm = nullptr;
+    c->device = ctx->device;
   }
   gb_status st = gb_merge_frames_impl(ctx, (int)K, frames, poses, resolution, target, seed, out_xyzw, out_cov4x4, num_out, c);
   if (st == GB_OK) {
@@ -1239,8 +1211,7 @@ extern "C" gb_status gb_preprocess(gb_ctx* ctx, size_t n, const double* xyzw, co
   if (P->estimate_covariances) {
     c = new (std::nothrow) gb_cloud();
     if (!c) return GB_ERR_INTERNAL;
-    c->device = ctx->device; c->n = 0; c->base = nullptr; c->bytes = 0;
-    c->p0 = nullptr; c->p1 = nullptr; c->p2 = nullptr; c->normals = nullptr; c->perm = nullptr; c->inv_perm = nullptr;
+    c->device = ctx->device;
   }
   gb_status st = gb_preprocess_impl(ctx, n, xyzw, times, intensities, P, out, c);
   if (st == GB_OK) {

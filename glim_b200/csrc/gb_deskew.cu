@@ -114,8 +114,6 @@ __global__ void __launch_bounds__(256) k_deskew(int n, const double4* __restrict
   out[i] = d;
 }
 
-inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
 }  // namespace
 
 // time table (cloud_deskewing.cpp:25-35 / :75-82) + one pose per entry; HOST ONLY (no device needed)
@@ -188,13 +186,15 @@ extern "C" gb_status gb_deskew(gb_ctx* ctx, const double T_imu_lidar[16], const 
   size_t m = 0;
   GB_CHECK(gb_deskew_pose_table(T_imu_lidar, linear_vel, angular_vel, n_imu, imu_times, imu_poses, stamp, n, times, idx.data(), table.data(), &m));
   cudaStream_t st = ctx->stream;
-  const size_t pts_b = align_up(sizeof(double4) * n, 256), idx_b = align_up(sizeof(int) * n, 256), tab_b = align_up(sizeof(double) * 16 * (m + 1), 256);
-  char* base = nullptr;
-  GB_CHECK(gb_ctx_scratch(ctx, 2 * pts_b + idx_b + tab_b, (void**)&base));
-  double4* d_pts = (double4*)base;
-  double4* d_out = (double4*)(base + pts_b);
-  int* d_idx = (int*)(base + 2 * pts_b);
-  double* d_tab = (double*)(base + 2 * pts_b + idx_b);
+  double4 *d_pts, *d_out;
+  int* d_idx;
+  double* d_tab;
+  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+    d_pts = cv.take<double4>(n);
+    d_out = cv.take<double4>(n);
+    d_idx = cv.take<int>(n);
+    d_tab = cv.take<double>(16 * (m + 1));  // the table, then T_post
+  }));
   double* d_post = T_post ? d_tab + 16 * m : nullptr;
   GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * n, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(d_idx, idx.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));

@@ -43,30 +43,30 @@ void gb_set_error(const char* fmt, ...);
 // Voxel map: open-addressing table of 16-byte buckets {cx, cy, cz, voxel index (-1 = empty)} and
 // 48-byte voxel records (3 x float4): {mx, my, mz, c00} {c01, c02, c11, c12} {c22, num_points, 0, 0}.
 struct gb_cloud {
-  int device;       // clouds / voxel maps do NOT keep their creating context: they outlive it when frames migrate between threads
-  size_t n;
-  float4* p0;
-  float4* p1;
-  float* p2;
-  float4* normals;  // {nx, ny, nz, 0} or nullptr
+  int device = 0;   // clouds / voxel maps do NOT keep their creating context: they outlive it when frames migrate between threads
+  size_t n = 0;
+  float4* p0 = nullptr;
+  float4* p1 = nullptr;
+  float* p2 = nullptr;
+  float4* normals = nullptr;  // {nx, ny, nz, 0} or nullptr
   // Points are stored in Morton order of their 1/16 m cell (gather locality of the sweep kernel: lanes of a warp
   // then hit the same few voxels).  perm[j] = original index of stored point j, inv_perm = its inverse; nullptr = identity.
-  int* perm;
-  int* inv_perm;
-  void* base;       // one allocation
-  size_t bytes;
+  int* perm = nullptr;
+  int* inv_perm = nullptr;
+  void* base = nullptr;       // one allocation
+  size_t bytes = 0;
 };
 
 struct gb_voxelmap {
-  int device;
-  float resolution, inv_res;
-  int max_scan;
-  int num_voxels, num_buckets;
-  int num_dropped_points;
-  int4* buckets;
-  float4* voxels;   // 3 float4 per voxel
-  void* base;
-  size_t bytes;
+  int device = 0;
+  float resolution = 0.f, inv_res = 0.f;
+  int max_scan = 0;
+  int num_voxels = 0, num_buckets = 0;
+  int num_dropped_points = 0;
+  int4* buckets = nullptr;
+  float4* voxels = nullptr;   // 3 float4 per voxel
+  void* base = nullptr;
+  size_t bytes = 0;
 };
 
 // device-side factor descriptor (80 B)
@@ -110,87 +110,87 @@ struct PeerPush {
 };
 
 struct gb_peer_slab {
-  gb_ctx* ctx;
-  size_t num_pairs;
-  int world, rank;
-  size_t buf_floats;              // floats per buffer
-  char* local;                    // cudaMalloc: [buffer 0][buffer 1][flags: world x u32, padded]
-  char* peer[GB_MAX_PEERS];       // every rank's allocation as mapped here (peer[rank] == local)
-  bool opened[GB_MAX_PEERS];
-  unsigned step;                  // last launched step
-  int parity;                     // buffer written by the NEXT launch
-  int completed_parity;           // buffer completed by the last signal_wait
-  int* d_timeout;
-  float* h_pinned;                // num_pairs x GB_SLAB_STRIDE, for the fetches
-  bool connected;
+  gb_ctx* ctx = nullptr;
+  size_t num_pairs = 0;
+  int world = 0, rank = 0;
+  size_t buf_floats = 0;          // floats per buffer
+  char* local = nullptr;          // cudaMalloc: [buffer 0][buffer 1][flags: world x u32, padded]
+  char* peer[GB_MAX_PEERS] = {};  // every rank's allocation as mapped here (peer[rank] == local)
+  bool opened[GB_MAX_PEERS] = {};
+  unsigned step = 0;              // last launched step
+  int parity = 0;                 // buffer written by the NEXT launch
+  int completed_parity = 0;       // buffer completed by the last signal_wait
+  int* d_timeout = nullptr;
+  float* h_pinned = nullptr;      // num_pairs x GB_SLAB_STRIDE, for the fetches
+  bool connected = false;
   // deferred exchange (default): the sweep stores finished pair rows into the LOCAL buffer only; the exchange kernel that
   // follows it copies this rank's rows to every peer (one CTA per peer) before it publishes the completion flags
-  bool deferred;
-  int* d_my_pairs;                // pair ids owned by the attached sweep
-  int num_my_pairs;
+  bool deferred = false;
+  int* d_my_pairs = nullptr;      // pair ids owned by the attached sweep
+  int num_my_pairs = 0;
 };
 
 #define GB_ACC_STRIDE 32      // doubles per factor in the accumulation buffer (29 used)
 #define GB_OUT_DOUBLES 122    // gb_linearized6
 
 struct gb_sweep {
-  gb_ctx* ctx;
-  size_t F;
+  gb_ctx* ctx = nullptr;
+  size_t F = 0;
   std::vector<gb_factor*> factors;
-  FactorDesc* d_descs;
-  int2* d_tiles;          // work items {factor, first point}, factor-major
-  double* d_poses;        // F x 16 (T_lin)
-  double* d_poses_eval;   // F x 16 (error mode)
-  double* d_accum;        // F x acc_slots x GB_ACC_STRIDE, zero between sweeps (self-cleaning)
-  int acc_slots;          // power of two: copies of each factor's accumulator (spreads same-address atomics of few-factor sweeps)
-  unsigned* d_done;       // F tickets, zero between sweeps
-  unsigned long long* d_tile_ctr;  // dynamic tile queue head, monotonic across launches
-  unsigned long long ctr_base;     // value of the counter at the start of the next launch
-  double* d_out;          // F x 122
-  double* h_poses_eval;   // pinned
-  double* h_out;          // pinned
-  float* d_slab;
-  size_t num_pairs;
-  gb_peer_slab* peer;             // fused exchange target (or nullptr)
-  int* d_pair_ptr;                // CSR pair -> factors (device), built when a peer slab is attached
-  int* d_pair_factors;
-  unsigned* d_pair_done;
-  PeerPush* d_peer_tables;        // [2]: one per step parity
-  std::vector<int> h_pair;        // pair id per factor
-  int num_tiles, tile_size, grid;   // work items, points per item, CTAs
-  int kernel_version;               // 5 = small sweeps (one wave of strided items); 3 = large sweeps (queue of contiguous items) (GB_KERNEL=3/5 forces one)
-  bool any_sv;                      // some factor of the sweep has surface validation on
-  int strided;                      // v5, about one item per warp: item j of a factor owns the rows j, j + J, ... (see k_vgicp_sweep5)
-  bool calibrated;                  // strided: the item table has been re-sized from measured inlier fractions
-  int capacity;                     // CTAs of a full grid
-  FactorDesc* h_descs;              // pinned copies (re-uploaded when the item table is re-sized)
-  int2* h_tiles;
-  size_t tiles_cap;
-  uint64_t point_factors, algorithmic_bytes;
-  uint64_t key;           // cache key
-  bool stale;             // a factor of this sweep was destroyed: it can no longer be launched
-  double* h_pose_slot[2]; // pinned pose staging, double buffered (no stream sync in gb_sweep_set_poses)
-  cudaEvent_t pose_ev[2]; // recorded after the H2D that read the slot
-  int pose_slot;
-  cudaGraphExec_t graph_exec;       // small sweeps: poses H2D -> kernel -> records D2H as ONE graph launch (gb_factor_set_linearize)
-  int graph_state;                  // 0 = not built, 1 = valid, -1 = capture failed (plain launches from then on)
-  void* pool_d; size_t pool_d_cap;  // the blocks this sweep took from its context's pool
-  void* pool_h; size_t pool_h_cap;
+  FactorDesc* d_descs = nullptr;
+  int2* d_tiles = nullptr;          // work items {factor, first point}, factor-major
+  double* d_poses = nullptr;        // F x 16 (T_lin)
+  double* d_poses_eval = nullptr;   // F x 16 (error mode)
+  double* d_accum = nullptr;        // F x acc_slots x GB_ACC_STRIDE, zero between sweeps (self-cleaning)
+  int acc_slots = 0;                // power of two: copies of each factor's accumulator (spreads same-address atomics of few-factor sweeps)
+  unsigned* d_done = nullptr;       // F tickets, zero between sweeps
+  unsigned long long* d_tile_ctr = nullptr;  // dynamic tile queue head, monotonic across launches
+  unsigned long long ctr_base = 0;           // value of the counter at the start of the next launch
+  double* d_out = nullptr;          // F x 122
+  double* h_poses_eval = nullptr;   // pinned
+  double* h_out = nullptr;          // pinned
+  float* d_slab = nullptr;
+  size_t num_pairs = 0;
+  gb_peer_slab* peer = nullptr;     // fused exchange target (or nullptr)
+  int* d_pair_ptr = nullptr;        // CSR pair -> factors (device), built when a peer slab is attached
+  int* d_pair_factors = nullptr;
+  unsigned* d_pair_done = nullptr;
+  PeerPush* d_peer_tables = nullptr;  // [2]: one per step parity
+  std::vector<int> h_pair;            // pair id per factor
+  int num_tiles = 0, tile_size = 0, grid = 0;  // work items, points per item, CTAs
+  int kernel_version = 0;           // 5 = small sweeps (one wave of strided items); 3 = large sweeps (queue of contiguous items) (GB_KERNEL=3/5 forces one)
+  bool any_sv = false;              // some factor of the sweep has surface validation on
+  int strided = 0;                  // v5, about one item per warp: item j of a factor owns the rows j, j + J, ... (see k_vgicp_sweep5)
+  bool calibrated = false;          // strided: the item table has been re-sized from measured inlier fractions
+  int capacity = 0;                 // CTAs of a full grid
+  FactorDesc* h_descs = nullptr;    // pinned copies (re-uploaded when the item table is re-sized)
+  int2* h_tiles = nullptr;
+  size_t tiles_cap = 0;
+  uint64_t point_factors = 0, algorithmic_bytes = 0;
+  uint64_t key = 0;                 // cache key
+  bool stale = false;               // a factor of this sweep was destroyed: it can no longer be launched
+  double* h_pose_slot[2] = {};      // pinned pose staging, double buffered (no stream sync in gb_sweep_set_poses)
+  cudaEvent_t pose_ev[2] = {};      // recorded after the H2D that read the slot
+  int pose_slot = 0;
+  cudaGraphExec_t graph_exec = nullptr;  // small sweeps: poses H2D -> kernel -> records D2H as ONE graph launch (gb_factor_set_linearize)
+  int graph_state = 0;              // 0 = not built, 1 = valid, -1 = capture failed (plain launches from then on)
+  void* pool_d = nullptr; size_t pool_d_cap = 0;  // the blocks this sweep took from its context's pool
+  void* pool_h = nullptr; size_t pool_h_cap = 0;
 };
 
 struct gb_pool_block { void* d; size_t d_cap; void* h; size_t h_cap; };
 
 struct gb_ctx {
-  int device;
-  cudaStream_t stream;
-  bool own_stream;
-  int num_sms;
-  void* scratch;
-  size_t scratch_cap;
-  void* pinned;
-  size_t pinned_cap;
-  uint64_t launches;
-  std::atomic<int> refs;   // owner + live factors / sweeps / peer slabs; the context is torn down when the last one lets go
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  bool own_stream = false;
+  int num_sms = 0;
+  void* scratch = nullptr;
+  size_t scratch_cap = 0;
+  void* pinned = nullptr;
+  size_t pinned_cap = 0;
+  uint64_t launches = 0;
+  std::atomic<int> refs{0};  // owner + live factors / sweeps / peer slabs; the context is torn down when the last one lets go
   std::vector<gb_sweep*> sweep_cache;
   std::vector<gb_pool_block> pool;  // device + pinned blocks of retired sweeps, reused by the next gb_sweep_create
   // A context may be driven from more than one host thread (a frame cloned by the odometry thread is later used by the
@@ -207,13 +207,85 @@ void gb_dev_free(int device, void* p);
 gb_status gb_ctx_scratch(gb_ctx* ctx, size_t bytes, void** out);  // device scratch, valid until the next call
 gb_status gb_ctx_pinned(gb_ctx* ctx, size_t bytes, void** out);   // pinned host staging, same lifetime rule
 
+inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// Carves 256-byte aligned arrays out of one buffer.  Without a base it only measures: a layout is written once, as a
+// function of a Carver, and run first to size the buffer and then to hand out the pointers (gb_carve_scratch).
+struct Carver {
+  char* base = nullptr;
+  size_t off = 0;
+  template <typename T> T* take(size_t count) {
+    T* p = base ? (T*)(base + off) : nullptr;
+    off += align_up(sizeof(T) * count, 256);
+    return p;
+  }
+};
+template <typename Layout> gb_status gb_carve_scratch(gb_ctx* ctx, Layout&& layout) {
+  Carver size;
+  layout(size);
+  Carver cv;
+  GB_CHECK(gb_ctx_scratch(ctx, size.off, (void**)&cv.base));
+  layout(cv);
+  return GB_OK;
+}
+
+// The largest temporary storage of the cub calls the library makes on n items (radix sorts of 64-bit keys with or
+// without int values, inclusive int scans, double sums): one buffer of this size serves them all.
+size_t gb_cub_temp_bytes(size_t n);
+
+// Temporaries of a (key, index) radix sort: the cub storage (shared with the caller's other cub calls) and the arrays.
+struct gb_sort_tmp {
+  void* cub;
+  size_t cub_bytes;
+  unsigned long long* keys;
+  unsigned long long* keys_s;
+  int* idx;
+  int* idx_s;
+};
+inline gb_sort_tmp gb_take_sort_tmp(Carver& cv, size_t n, void* cub, size_t cub_bytes) {
+  gb_sort_tmp t;
+  t.cub = cub;
+  t.cub_bytes = cub_bytes;
+  t.keys = cv.take<unsigned long long>(n);
+  t.keys_s = cv.take<unsigned long long>(n);
+  t.idx = cv.take<int>(n + 1);
+  t.idx_s = cv.take<int>(n + 1);
+  return t;
+}
+
+// Voxel grouping (gb_kernels_voxelmap.cu), shared by the map build, the voxel-grid downsampling and the frame merge.  The
+// caller writes one packed key per point (~0 = no voxel) and idx[i] = i; gb_group_by_key sorts the pairs into keys_s /
+// idx_s, flags the first slot of every voxel and scans the flags: pos[s] = number of voxels up to sorted slot s, so
+// pos[n - 1] is the voxel count.  gb_group_starts then writes starts[v] = first sorted slot of voxel v and
+// starts[V] = number of valid points.  Each counts its own launches.
+gb_status gb_group_by_key(gb_ctx* ctx, int n, const gb_sort_tmp& t, int* flags, int* pos);
+void gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* flags, const int* pos, int* starts);
+
+// Device cloud construction.  gb_cloud_planes lays out the planes of n points (p0, p1, p2, optional normals) at the
+// carver's position; the planes staged in the caller's point order use the same layout as the cloud's own.
+// gb_cloud_build takes c's block (planes, perm, inv_perm) from the device pool and fills it with the Morton reorder of the
+// staged planes; it uses t.cub, t.keys, t.keys_s and t.idx for n points.
+struct gb_planes {
+  float4* p0;
+  float4* p1;
+  float* p2;
+  float4* normals;
+};
+inline gb_planes gb_cloud_planes(Carver& cv, size_t n, bool normals) {
+  gb_planes p;
+  p.p0 = cv.take<float4>(n);
+  p.p1 = cv.take<float4>(n);
+  p.p2 = cv.take<float>(n);
+  p.normals = normals ? cv.take<float4>(n) : nullptr;
+  return p;
+}
+gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n, const gb_planes& staged, const gb_sort_tmp& t);
+
 // kernel launchers (gb_kernels_*.cu)
 enum { GB_MODE_LINEARIZE = 0, GB_MODE_ERROR = 1 };
 gb_status gb_launch_sweep(gb_sweep* s, int mode);
 gb_status gb_launch_peer_signal_wait(gb_peer_slab* ps);
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count);
-gb_status gb_cloud_reorder_impl(gb_ctx* ctx, gb_cloud* c, const void* staged /* device copy of the planes in original order */, size_t b0, size_t b1, size_t b2, size_t b3);
-size_t gb_cloud_reorder_scratch_bytes(size_t n, size_t staged_bytes);
 gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_buckets, int max_scan, double drop_rate, gb_voxelmap* out);
 gb_status gb_covariances_impl(gb_ctx* ctx, size_t n, const double* xyzw, const int32_t* neighbors, int kc, int k, double* normals4, double* cov4x4);
 gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out, gb_cloud* cloud_out);
@@ -229,6 +301,7 @@ gb_status gb_voxelgrid_sampling_impl(gb_ctx* ctx, size_t n, const double* xyzw, 
 #include "gb_vgicp_math.cuh"  // gb_coord, gb_hash (shared with the host-compiled CPU test of the kernel arithmetic)
 // packed 3 x 21-bit voxel key (ascending key = canonical voxel order); false if out of range
 #define GB_KEY_OFFSET (1 << 20)
+constexpr unsigned long long kInvalidKey = ~0ull;  // the key of a point in no voxel: sorts last
 __device__ __forceinline__ bool gb_pack_key(int x, int y, int z, unsigned long long* key) {
   if (x < -GB_KEY_OFFSET || x >= GB_KEY_OFFSET || y < -GB_KEY_OFFSET || y >= GB_KEY_OFFSET || z < -GB_KEY_OFFSET || z >= GB_KEY_OFFSET) return false;
   *key = ((unsigned long long)(x + GB_KEY_OFFSET) << 42) | ((unsigned long long)(y + GB_KEY_OFFSET) << 21) | (unsigned long long)(z + GB_KEY_OFFSET);
@@ -238,6 +311,16 @@ __device__ __forceinline__ void gb_unpack_key(unsigned long long key, int& x, in
   x = (int)((key >> 42) & 0x1FFFFF) - GB_KEY_OFFSET;
   y = (int)((key >> 21) & 0x1FFFFF) - GB_KEY_OFFSET;
   z = (int)(key & 0x1FFFFF) - GB_KEY_OFFSET;
+}
+// 21 bits -> every third bit (Morton interleaving)
+__device__ __forceinline__ unsigned long long gb_spread21(unsigned long long v) {
+  v &= 0x1FFFFFull;
+  v = (v | (v << 32)) & 0x1F00000000FFFFull;
+  v = (v | (v << 16)) & 0x1F0000FF0000FFull;
+  v = (v | (v << 8)) & 0x100F00F00F00F00Full;
+  v = (v | (v << 4)) & 0x10C30C30C30C30C3ull;
+  v = (v | (v << 2)) & 0x1249249249249249ull;
+  return v;
 }
 // linear-probing lookup (SURVEY B.4)
 __device__ __forceinline__ int gb_lookup(const int4* __restrict__ buckets, uint32_t mask, int max_scan, int cx, int cy, int cz) {

@@ -20,13 +20,15 @@
 //                        deterministic hashing), including which voxels run out of probes (<= max_scan)
 //   6. host loop         num_buckets = init doubled until >= 8 V (load factor <= 1/8), then doubled again while
 //                        dropped points > drop_rate * N
+// Steps 2-3 (+ k_voxel_starts) are gb_group_by_key / gb_group_starts, shared with the voxel-grid downsampling and the frame
+// merge of gb_kernels_preprocess.cu.  This file also builds every device cloud (gb_cloud_build: Morton reorder of staged
+// planes), for gb_cloud_upload, gb_preprocess and gb_merge_frames.
 #include "gb_internal.cuh"
 
 #include <cub/cub.cuh>
 
 namespace {
 
-constexpr unsigned long long kInvalidKey = ~0ull;
 constexpr int kEmpty = 0x7fffffff;
 
 // i runs over ORIGINAL point indices (so that voxel sums are accumulated in the caller's point order, like the oracle);
@@ -126,9 +128,23 @@ __global__ void k_table_finalize(int nb, const int4* __restrict__ vcoord, int4* 
   }
 }
 
-inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
 }  // namespace
+
+gb_status gb_group_by_key(gb_ctx* ctx, int n, const gb_sort_tmp& t, int* flags, int* pos) {
+  cudaStream_t st = ctx->stream;
+  size_t tmp = t.cub_bytes;
+  GB_CUDA(cub::DeviceRadixSort::SortPairs(t.cub, tmp, t.keys, t.keys_s, t.idx, t.idx_s, n, 0, 64, st));
+  k_head_flags<<<(n + 255) / 256, 256, 0, st>>>(n, t.keys_s, flags);
+  tmp = t.cub_bytes;
+  GB_CUDA(cub::DeviceScan::InclusiveSum(t.cub, tmp, flags, pos, n, st));
+  ctx->launches += 3;
+  return GB_OK;
+}
+
+void gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* flags, const int* pos, int* starts) {
+  k_voxel_starts<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, t.keys_s, flags, pos, starts);
+  ctx->launches++;
+}
 
 gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_buckets, int max_scan, double drop_rate, gb_voxelmap* m) {
   const int n = (int)cloud->n;
@@ -137,54 +153,33 @@ gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resol
   m->resolution = resolution;
   m->inv_res = 1.0f / resolution;
   m->max_scan = max_scan;
-  m->num_voxels = 0;
-  m->num_dropped_points = 0;
-  m->voxels = nullptr;
-  m->buckets = nullptr;
-  m->base = nullptr;
 
   int V = 0;
   int4* d_vcoord = nullptr;
   int* d_dropped = nullptr;
   if (n > 0) {
-    // scratch layout
-    size_t cub_sort = 0, cub_scan = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, cub_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, n, 0, 64, st);
-    cub::DeviceScan::InclusiveSum(nullptr, cub_scan, (int*)nullptr, (int*)nullptr, n, st);
-    const size_t cub_bytes = align_up(cub_sort > cub_scan ? cub_sort : cub_scan, 256);
-    const size_t keys_b = align_up(sizeof(unsigned long long) * (size_t)n, 256), idx_b = align_up(sizeof(int) * (size_t)(n + 1), 256);
-    const size_t vcoord_b = align_up(sizeof(int4) * (size_t)n, 256);
-    const size_t total = cub_bytes + 2 * keys_b + 5 * idx_b + vcoord_b + 256;
-    char* base = nullptr;
-    GB_CHECK(gb_ctx_scratch(ctx, total, (void**)&base));
-    char* p = base;
-    void* d_cub = p; p += cub_bytes;
-    unsigned long long* d_keys = (unsigned long long*)p; p += keys_b;
-    unsigned long long* d_keys_s = (unsigned long long*)p; p += keys_b;
-    int* d_idx = (int*)p; p += idx_b;
-    int* d_idx_s = (int*)p; p += idx_b;
-    int* d_flags = (int*)p; p += idx_b;
-    int* d_pos = (int*)p; p += idx_b;
-    int* d_starts = (int*)p; p += idx_b;
-    d_vcoord = (int4*)p; p += vcoord_b;
-    d_dropped = (int*)p;
-
-    const int tb = 256, gb = (n + tb - 1) / tb;
-    k_point_keys<<<gb, tb, 0, st>>>(n, cloud->p0, cloud->inv_perm, m->inv_res, d_keys, d_idx);
-    size_t tmp = cub_bytes;
-    GB_CUDA(cub::DeviceRadixSort::SortPairs(d_cub, tmp, d_keys, d_keys_s, d_idx, d_idx_s, n, 0, 64, st));
-    k_head_flags<<<gb, tb, 0, st>>>(n, d_keys_s, d_flags);
-    tmp = cub_bytes;
-    GB_CUDA(cub::DeviceScan::InclusiveSum(d_cub, tmp, d_flags, d_pos, n, st));
+    const size_t cub_b = gb_cub_temp_bytes(n);
+    gb_sort_tmp t;
+    int *d_flags, *d_pos, *d_starts;
+    GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+      t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
+      d_flags = cv.take<int>(n + 1);
+      d_pos = cv.take<int>(n + 1);
+      d_starts = cv.take<int>(n + 1);
+      d_vcoord = cv.take<int4>(n);
+      d_dropped = cv.take<int>(1);
+    }));
+    k_point_keys<<<(n + 255) / 256, 256, 0, st>>>(n, cloud->p0, cloud->inv_perm, m->inv_res, t.keys, t.idx);
+    ctx->launches++;
+    GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
     GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
-    ctx->launches += 4;
     if (V > 0) {
       GB_CUDA(gb_dev_malloc(ctx->device, sizeof(float4) * 3 * (size_t)V, &m->base));
       m->voxels = (float4*)m->base;
-      k_voxel_starts<<<gb, tb, 0, st>>>(n, d_keys_s, d_flags, d_pos, d_starts);
-      k_voxel_reduce<<<(V + 127) / 128, 128, 0, st>>>(V, d_starts, d_keys_s, d_idx_s, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm, m->voxels, d_vcoord);
-      ctx->launches += 2;
+      gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts);
+      k_voxel_reduce<<<(V + 127) / 128, 128, 0, st>>>(V, d_starts, t.keys_s, t.idx_s, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm, m->voxels, d_vcoord);
+      ctx->launches++;
     }
   }
   m->num_voxels = V;
@@ -225,19 +220,10 @@ gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resol
 
 
 // ---------------------------------------------------------------------------------------------
-// Morton reordering of a freshly uploaded cloud (PointCloudGPU::clone keeps the caller's order on the host side of the
+// Morton reordering of a new cloud (PointCloudGPU::clone keeps the caller's order on the host side of the
 // boundary: gb_cloud_download and the voxel-map sums un-permute; only the device storage order changes).
 // ---------------------------------------------------------------------------------------------
 namespace {
-__device__ __forceinline__ unsigned long long spread21(unsigned long long v) {  // 21 bits -> every third bit
-  v &= 0x1FFFFFull;
-  v = (v | (v << 32)) & 0x1F00000000FFFFull;
-  v = (v | (v << 16)) & 0x1F0000FF0000FFull;
-  v = (v | (v << 8)) & 0x100F00F00F00F00Full;
-  v = (v | (v << 4)) & 0x10C30C30C30C30C3ull;
-  v = (v | (v << 2)) & 0x1249249249249249ull;
-  return v;
-}
 __global__ void k_morton_keys(int n, const float4* __restrict__ p0, unsigned long long* __restrict__ keys, int* __restrict__ idx) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -248,7 +234,7 @@ __global__ void k_morton_keys(int n, const float4* __restrict__ p0, unsigned lon
     const float fx = floorf(a.x * s), fy = floorf(a.y * s), fz = floorf(a.z * s);
     if (fabsf(fx) < 1048576.f && fabsf(fy) < 1048576.f && fabsf(fz) < 1048576.f) {
       const unsigned long long x = (unsigned long long)((int)fx + (1 << 20)), y = (unsigned long long)((int)fy + (1 << 20)), z = (unsigned long long)((int)fz + (1 << 20));
-      key = (spread21(x) << 2) | (spread21(y) << 1) | spread21(z);
+      key = (gb_spread21(x) << 2) | (gb_spread21(y) << 1) | gb_spread21(z);
     }
   }
   keys[i] = key;
@@ -267,35 +253,29 @@ __global__ void k_permute_cloud(int n, const int* __restrict__ perm, const float
 }
 }  // namespace
 
-gb_status gb_cloud_reorder_impl(gb_ctx* ctx, gb_cloud* c, const void* staged, size_t b0, size_t b1, size_t b2, size_t b3) {
-  const int n = (int)c->n;
+gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n_, const gb_planes& s, const gb_sort_tmp& t) {
+  const int n = (int)n_;
   cudaStream_t st = ctx->stream;
-  const char* sp = (const char*)staged;
-  const float4* s0 = (const float4*)sp;
-  const float4* s1 = (const float4*)(sp + b0);
-  const float* s2 = (const float*)(sp + b0 + b1);
-  const float4* s3 = b3 ? (const float4*)(sp + b0 + b1 + b2) : nullptr;
-  size_t cub_sort = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, cub_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, n, 0, 64, st);
-  const size_t cub_b = align_up(cub_sort, 256), key_b = align_up(sizeof(unsigned long long) * (size_t)n, 256), idx_b = align_up(sizeof(int) * (size_t)n, 256);
-  // the staged planes live at the start of the ctx scratch buffer; our temporaries go behind them (the caller sized it)
-  char* p = (char*)staged + align_up(b0 + b1 + b2 + b3, 256);
-  void* d_cub = p; p += cub_b;
-  unsigned long long* d_keys = (unsigned long long*)p; p += key_b;
-  unsigned long long* d_keys_s = (unsigned long long*)p; p += key_b;
-  int* d_idx = (int*)p; p += idx_b;
+  gb_planes d;
+  auto layout = [&](Carver& cv) {
+    d = gb_cloud_planes(cv, n_, s.normals != nullptr);
+    c->perm = cv.take<int>(n_);
+    c->inv_perm = cv.take<int>(n_);
+  };
+  Carver size;
+  layout(size);
+  GB_CUDA(gb_dev_malloc(ctx->device, size.off, &c->base));
+  c->bytes = size.off;
+  c->n = n_;
+  Carver cv{(char*)c->base};
+  layout(cv);
+  c->p0 = d.p0; c->p1 = d.p1; c->p2 = d.p2; c->normals = d.normals;
   const int tb = 256, gb = (n + tb - 1) / tb;
-  k_morton_keys<<<gb, tb, 0, st>>>(n, s0, d_keys, d_idx);
-  size_t tmp = cub_b;
-  GB_CUDA(cub::DeviceRadixSort::SortPairs(d_cub, tmp, d_keys, d_keys_s, d_idx, c->perm, n, 0, 64, st));
-  k_permute_cloud<<<gb, tb, 0, st>>>(n, c->perm, s0, s1, s2, s3, c->p0, c->p1, c->p2, c->normals, c->inv_perm);
+  k_morton_keys<<<gb, tb, 0, st>>>(n, s.p0, t.keys, t.idx);
+  size_t tmp = t.cub_bytes;
+  GB_CUDA(cub::DeviceRadixSort::SortPairs(t.cub, tmp, t.keys, t.keys_s, t.idx, c->perm, n, 0, 64, st));
+  k_permute_cloud<<<gb, tb, 0, st>>>(n, c->perm, s.p0, s.p1, s.p2, s.normals, c->p0, c->p1, c->p2, c->normals, c->inv_perm);
   GB_CUDA(cudaGetLastError());
   ctx->launches += 3;
   return GB_OK;
-}
-
-size_t gb_cloud_reorder_scratch_bytes(size_t n, size_t staged_bytes) {
-  size_t cub_sort = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, cub_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, (int)n, 0, 64, (cudaStream_t)0);
-  return align_up(staged_bytes, 256) + align_up(cub_sort, 256) + 2 * align_up(sizeof(unsigned long long) * n, 256) + align_up(sizeof(int) * n, 256) + 256;
 }
