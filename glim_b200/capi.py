@@ -18,6 +18,7 @@ SYMBOLS = [
     "gb_cloud_upload", "gb_cloud_size", "gb_cloud_download", "gb_cloud_device_ptrs", "gb_cloud_destroy",
     "gb_hessian_blocks", "gb_slab_row_hessian_blocks",
     "gb_voxelmap_build", "gb_voxelmap_info", "gb_voxelmap_download", "gb_voxelmap_destroy",
+    "gb_voxelmap_create_incremental", "gb_voxelmap_insert",
     "gb_vgicp_factor_create", "gb_vgicp_factor_destroy", "gb_vgicp_linearize", "gb_vgicp_error",
     "gb_factor_set_linearize", "gb_factor_set_error",
     "gb_sweep_create", "gb_sweep_destroy", "gb_sweep_attach_slab", "gb_sweep_set_poses", "gb_sweep_launch", "gb_sweep_fetch", "gb_sweep_linearize",
@@ -108,6 +109,8 @@ def lib():
     L.gb_voxelmap_info.argtypes = [vp, vp, vp, vp]
     L.gb_voxelmap_download.argtypes = [vp, vp, vp, vp, vp]
     L.gb_voxelmap_destroy.argtypes = [vp]
+    L.gb_voxelmap_create_incremental.argtypes = [vp, f32, i32, i32, f64, i32, i32, vp]
+    L.gb_voxelmap_insert.argtypes = [vp, vp, vp, vp, f64, u64]
     L.gb_vgicp_factor_create.argtypes = [vp, vp, vp, i32, vp]
     L.gb_vgicp_factor_destroy.argtypes = [vp]
     L.gb_vgicp_linearize.argtypes = [vp, vp, vp]

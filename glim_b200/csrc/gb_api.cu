@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <map>
 #include <mutex>
 #include <new>
@@ -348,6 +349,47 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
   *out = m;
   return GB_OK;
 }
+extern "C" gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolution, int init_num_buckets, int max_bucket_scan_count, double target_points_drop_rate,
+                                                    int lru_horizon, int lru_clear_cycle, gb_voxelmap** out) {
+  GB_REQUIRE(ctx && out, "null argument");
+  GB_REQUIRE(resolution > 0.f && std::isfinite(resolution), "resolution must be positive and finite");
+  GB_REQUIRE(init_num_buckets > 0 && (init_num_buckets & (init_num_buckets - 1)) == 0, "init_num_buckets must be a power of two");
+  GB_REQUIRE(max_bucket_scan_count > 0, "max_bucket_scan_count must be positive");
+  GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
+  *out = nullptr;
+  GB_LOCK(ctx);
+  GB_CUDA(cudaSetDevice(ctx->device));
+  gb_voxelmap* m = new (std::nothrow) gb_voxelmap();
+  if (!m) return GB_ERR_INTERNAL;
+  m->resolution = resolution;
+  m->inv_res = 1.0f / resolution;
+  m->max_scan = max_bucket_scan_count;
+  m->init_buckets = init_num_buckets;
+  m->drop_rate = target_points_drop_rate;
+  m->lru_horizon = lru_horizon;
+  m->lru_clear_cycle = lru_clear_cycle;
+  gb_status st = gb_voxelmap_create_incremental_impl(ctx, m);
+  if (st != GB_OK) {
+    gb_dev_free(ctx->device, m->buckets);
+    delete m;
+    return st;
+  }
+  *out = m;
+  return GB_OK;
+}
+extern "C" gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
+  GB_REQUIRE(ctx && map && cloud, "null argument");
+  GB_REQUIRE(map->incremental, "the map comes from gb_voxelmap_build, which keeps no sums: create it with gb_voxelmap_create_incremental");
+  GB_REQUIRE(map->device == ctx->device && cloud->device == ctx->device, "cloud / voxel map live on another device");
+  GB_REQUIRE(sampling_rate > 0.0 && sampling_rate <= 1.0, "sampling_rate must be in (0, 1]");
+  static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  const double* T = T_map_cloud ? T_map_cloud : kIdentity;
+  for (int k = 0; k < 16; k++) GB_REQUIRE(std::isfinite(T[k]), "T_map_cloud must be finite");
+  GB_REQUIRE((uint64_t)map->num_voxels + (uint64_t)cloud->n < (1ull << 31) - 1, "map voxels + cloud points exceed 2^31");
+  GB_LOCK(ctx);
+  GB_CUDA(cudaSetDevice(ctx->device));
+  return gb_voxelmap_insert_impl(ctx, map, cloud, T, sampling_rate, (unsigned long long)seed);
+}
 extern "C" gb_status gb_voxelmap_info(const gb_voxelmap* m, int* num_voxels, int* num_buckets, float* resolution) {
   GB_REQUIRE(m, "null map");
   if (num_voxels) *num_voxels = m->num_voxels;
@@ -564,6 +606,46 @@ static gb_status sweep_learn_inliers(gb_sweep* s) {
   return GB_OK;
 }
 
+// the target part of a factor descriptor
+static void desc_target(FactorDesc& D, const gb_voxelmap* t) {
+  D.buckets = t->buckets; D.voxels = t->voxels;
+  D.mask = (uint32_t)t->num_buckets - 1u;
+  D.max_scan = t->max_scan;
+  D.inv_res = t->inv_res;
+}
+// B_f of SURVEY 8(d): 48 B per source point, 48 B per target voxel, 16 B per bucket, pose in + record out.
+// The bucket term is charged at the SMALLEST table that could hold the voxels (16384 doubled until >= V), not at
+// our deliberately sparse table (>= 8 V): padding we added for speed must not inflate the achieved-GB/s figure.
+static uint64_t factor_bytes(const gb_factor* fa) {
+  const bool sv = (fa->flags & GB_FACTOR_SURFACE_VALIDATION) != 0;
+  uint64_t nb_ref = 16384;
+  while (nb_ref < (uint64_t)fa->target->num_voxels) nb_ref *= 2;
+  return (uint64_t)fa->source->n * (48 + (sv ? 12 : 0)) + (uint64_t)fa->target->num_voxels * 48 + nb_ref * 16 + 64 + 488;  // +12 B / point: the normals, when they are read
+}
+
+// Before every launch: a factor whose target is an incremental map that gb_voxelmap_insert changed since its descriptor was
+// written gets that descriptor re-written (buckets, records, mask) and re-uploaded.  Sweeps over built maps return at once.
+static gb_status sweep_follow_targets(gb_sweep* s) {
+  if (!s->any_incremental) return GB_OK;
+  bool synced = false;
+  for (size_t f = 0; f < s->F; f++) {
+    const gb_factor* fa = s->factors[f];
+    if (!fa || fa->target->version == s->target_versions[f]) continue;
+    if (!synced) {  // an earlier copy of the pinned descriptors may still be in flight
+      GB_CUDA(cudaStreamSynchronize(s->ctx->stream));
+      synced = true;
+    }
+    desc_target(s->h_descs[f], fa->target);
+    s->target_versions[f] = fa->target->version;
+    GB_CUDA(cudaMemcpyAsync(s->d_descs + f, s->h_descs + f, sizeof(FactorDesc), cudaMemcpyHostToDevice, s->ctx->stream));
+  }
+  if (synced) {
+    s->algorithmic_bytes = 0;
+    for (size_t f = 0; f < s->F; f++) if (s->factors[f]) s->algorithmic_bytes += factor_bytes(s->factors[f]);
+  }
+  return GB_OK;
+}
+
 extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* factors, const int32_t* pair_index, gb_sweep** out) {
   GB_REQUIRE(ctx && out, "null argument");
   GB_REQUIRE(F == 0 || factors, "null factor list");
@@ -612,22 +694,16 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     const bool sv = (fa->flags & GB_FACTOR_SURFACE_VALIDATION) != 0;
     D.normals = sv ? fa->source->normals : nullptr;
     any_sv = any_sv || sv;
-    D.buckets = fa->target->buckets; D.voxels = fa->target->voxels;
-    D.mask = (uint32_t)fa->target->num_buckets - 1u;
-    D.max_scan = fa->target->max_scan;
-    D.inv_res = fa->target->inv_res;
+    desc_target(D, fa->target);
+    s->target_versions.push_back(fa->target->version);
+    s->any_incremental = s->any_incremental || fa->target->incremental;
     D.n = (int)fa->source->n;
     D.pair = pair_index ? pair_index[f] : (int)f;
     s->h_pair.push_back(D.pair);
     D.flags = fa->flags;
     D.num_tiles = 1; D.chunk = s->tile_size;
     s->point_factors += (uint64_t)D.n;
-    // B_f of SURVEY 8(d): 48 B per source point, 48 B per target voxel, 16 B per bucket, pose in + record out.
-    // The bucket term is charged at the SMALLEST table that could hold the voxels (16384 doubled until >= V), not at
-    // our deliberately sparse table (>= 8 V): padding we added for speed must not inflate the achieved-GB/s figure.
-    uint64_t nb_ref = 16384;
-    while (nb_ref < (uint64_t)fa->target->num_voxels) nb_ref *= 2;
-    s->algorithmic_bytes += (uint64_t)D.n * (48 + (sv ? 12 : 0)) + (uint64_t)fa->target->num_voxels * 48 + nb_ref * 16 + 64 + 488;  // +12 B / point: the normals, when they are read
+    s->algorithmic_bytes += factor_bytes(fa);
   }
   s->any_sv = any_sv;
   build_items(s, descs.data(), tiles);
@@ -720,6 +796,7 @@ static gb_status sweep_set_eval_poses(gb_sweep* s, const double* T) {
 static gb_status sweep_launch(gb_sweep* s, int mode) {
   if (s->stale) { gb_set_error("a factor of this sweep has been destroyed"); return GB_ERR_INVALID_ARGUMENT; }
   GB_CUDA(cudaSetDevice(s->ctx->device));
+  GB_CHECK(sweep_follow_targets(s));
   return gb_launch_sweep(s, mode);
 }
 extern "C" gb_status gb_sweep_launch(gb_sweep* s) {
@@ -789,6 +866,7 @@ static gb_status sweep_linearize(gb_sweep* s, const double* T, gb_linearized6* o
   if (s->stale) { gb_set_error("a factor of this sweep has been destroyed"); return GB_ERR_INVALID_ARGUMENT; }
   gb_ctx* ctx = s->ctx;
   GB_CUDA(cudaSetDevice(ctx->device));
+  GB_CHECK(sweep_follow_targets(s));  // the graph's kernel reads the descriptors from HBM
   cudaStream_t st = ctx->stream;
   const size_t pose_bytes = sizeof(double) * 16 * s->F, out_bytes = sizeof(double) * GB_OUT_DOUBLES * s->F;
   if (s->graph_state == 0) {

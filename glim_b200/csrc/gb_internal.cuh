@@ -67,6 +67,18 @@ struct gb_voxelmap {
   float4* voxels = nullptr;   // 3 float4 per voxel
   void* base = nullptr;
   size_t bytes = 0;
+  // Incremental maps (gb_voxelmap_create_incremental / gb_voxelmap_insert) also keep, in `base` behind the records, each
+  // voxel's packed key, point count, fp64 sums (Sigma q: 3, Sigma C: 6 unique entries) and the insert that last touched it.
+  // A built map keeps none of this and its version stays 0.
+  bool incremental = false;
+  uint64_t version = 0;        // bumped by every insert: sweeps re-read the target's buckets / records when it changed
+  int init_buckets = 0;
+  double drop_rate = 0.0;
+  int lru_horizon = 0, lru_clear_cycle = 10, lru_counter = 0;
+  unsigned long long* vkeys = nullptr;  // ascending: the voxel numbering
+  int* vn = nullptr;
+  int* vstamp = nullptr;
+  double* vsums = nullptr;     // 9 per voxel: q.x q.y q.z c00 c01 c02 c11 c12 c22
 };
 
 // device-side factor descriptor (80 B)
@@ -176,6 +188,8 @@ struct gb_sweep {
   int graph_state = 0;              // 0 = not built, 1 = valid, -1 = capture failed (plain launches from then on)
   void* pool_d = nullptr; size_t pool_d_cap = 0;  // the blocks this sweep took from its context's pool
   void* pool_h = nullptr; size_t pool_h_cap = 0;
+  bool any_incremental = false;     // some target is an incremental map: its descriptor may go stale (gb_voxelmap_insert)
+  std::vector<uint64_t> target_versions;  // per factor: the target version its descriptor was written from
 };
 
 struct gb_pool_block { void* d; size_t d_cap; void* h; size_t h_cap; };
@@ -287,6 +301,16 @@ gb_status gb_launch_sweep(gb_sweep* s, int mode);
 gb_status gb_launch_peer_signal_wait(gb_peer_slab* ps);
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count);
 gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_buckets, int max_scan, double drop_rate, gb_voxelmap* out);
+gb_status gb_voxelmap_create_incremental_impl(gb_ctx* ctx, gb_voxelmap* m);
+gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, unsigned long long seed);
+// Shared with gb_merge_frames (gb_kernels_preprocess.cu): one frame's points q = R a + t and covariances R C R^T in
+// un-contracted fp64, in the caller's point order (pts: n x double4, cov6: n x 6 upper triangle).  d_frame: GB_FRAME_DESC_BYTES
+// of device scratch for the frame descriptor.  One launch.
+#define GB_FRAME_DESC_BYTES 256
+gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T_colmajor, void* d_frame, double4* pts, double* cov6);
+// k_grid_keys of the voxel-grid paths: key = packed floor(p * inv_res) in fp64 (~0 for non-finite / out-of-range points),
+// idx[i] = i.  One launch.
+void gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx);
 gb_status gb_covariances_impl(gb_ctx* ctx, size_t n, const double* xyzw, const int32_t* neighbors, int kc, int k, double* normals4, double* cov4x4);
 gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out, gb_cloud* cloud_out);
 gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out);
@@ -311,6 +335,14 @@ __device__ __forceinline__ void gb_unpack_key(unsigned long long key, int& x, in
   x = (int)((key >> 42) & 0x1FFFFF) - GB_KEY_OFFSET;
   y = (int)((key >> 21) & 0x1FFFFF) - GB_KEY_OFFSET;
   z = (int)(key & 0x1FFFFF) - GB_KEY_OFFSET;
+}
+// the project's fixed pseudo-random pick ([EXT]: the reference draws with std::mt19937): the points / voxels with the smallest
+// rg_hash(seed, index) are kept (random-grid downsampling, frame-merge thinning, voxel-map insert sampling; the oracle shares it)
+__device__ __forceinline__ unsigned long long rg_hash(unsigned long long seed, unsigned i) {
+  unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(i + 1u);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
 }
 // 21 bits -> every third bit (Morton interleaving)
 __device__ __forceinline__ unsigned long long gb_spread21(unsigned long long v) {

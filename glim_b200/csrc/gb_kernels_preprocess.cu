@@ -247,6 +247,11 @@ __global__ void k_grid_means_counted(const int* __restrict__ num_voxels, const i
 
 }  // namespace
 
+void gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx) {
+  k_grid_keys<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, pts, inv_res, keys, idx);
+  ctx->launches++;
+}
+
 // Calls launch(std::integral_constant<int, K>()) for the instantiated neighbour counts K of the k-NN kernels.
 template <typename Launch> static gb_status knn_dispatch(int k, Launch&& launch) {
   switch (k) {
@@ -525,13 +530,8 @@ __global__ void k_fill_self(int n, int k, int* __restrict__ neighbors) {
 // ---- downsampling, filtering, time order ----
 // random grid (gtsam_points::randomgrid_sampling, cloud_preprocessor.cpp:104-106): every voxel keeps at most
 // ppv = ceil(rate * N / V) of its points.  Which ones is a draw from std::mt19937 in the reference (not reproducible, SURVEY
-// C.2); here it is the ppv points with the smallest hash(seed, index) -- a fixed pseudo-random choice the oracle shares.
-__device__ __forceinline__ unsigned long long rg_hash(unsigned long long seed, unsigned i) {
-  unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(i + 1u);
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
+// C.2); here it is the ppv points with the smallest rg_hash(seed, index) (gb_internal.cuh) -- a fixed pseudo-random choice the
+// oracle shares.
 __global__ void k_randomgrid_select(int n, const int* __restrict__ num_voxels, const int* __restrict__ starts, const int* __restrict__ idx_s, double rate, unsigned long long seed, int* __restrict__ keep) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   const int V = *num_voxels;
@@ -994,6 +994,21 @@ __global__ void k_merge_emit(int n_upper, const int* __restrict__ keep, const in
 }
 
 }  // namespace
+
+static_assert(sizeof(MergeFrame) <= GB_FRAME_DESC_BYTES, "frame descriptor scratch");
+gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T, void* d_frame, double4* pts, double* cov6) {
+  MergeFrame F;
+  F.p0 = c->p0; F.p1 = c->p1; F.p2 = c->p2; F.inv_perm = c->inv_perm; F.n = (int)c->n; F.offset = 0;
+  for (int r = 0; r < 3; r++) for (int cc = 0; cc < 4; cc++) F.T[r * 4 + cc] = T[cc * 4 + r];
+  void* h = nullptr;
+  GB_CHECK(gb_ctx_pinned(ctx, sizeof(MergeFrame), &h));
+  memcpy(h, &F, sizeof(MergeFrame));
+  GB_CUDA(cudaMemcpyAsync(d_frame, h, sizeof(MergeFrame), cudaMemcpyHostToDevice, ctx->stream));
+  const int n = (int)c->n;
+  k_merge_transform<<<(n + 255) / 256, 256, 0, ctx->stream>>>(1, (const MergeFrame*)d_frame, n, pts, cov6);
+  ctx->launches++;
+  return GB_OK;
+}
 
 gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out) {
   cudaStream_t st = ctx->stream;

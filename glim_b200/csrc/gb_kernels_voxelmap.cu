@@ -21,7 +21,8 @@
 //   6. host loop         num_buckets = init doubled until >= 8 V (load factor <= 1/8), then doubled again while
 //                        dropped points > drop_rate * N
 // Steps 2-3 (+ k_voxel_starts) are gb_group_by_key / gb_group_starts, shared with the voxel-grid downsampling and the frame
-// merge of gb_kernels_preprocess.cu.  This file also builds every device cloud (gb_cloud_build: Morton reorder of staged
+// merge of gb_kernels_preprocess.cu.  Step 6 (table_build) also serves the incremental maps of gb_voxelmap_insert, whose
+// pipeline is described below.  This file also builds every device cloud (gb_cloud_build: Morton reorder of staged
 // planes), for gb_cloud_upload, gb_preprocess and gb_merge_frames.
 #include "gb_internal.cuh"
 
@@ -146,6 +147,43 @@ void gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* flags,
   ctx->launches++;
 }
 
+// The hash table of V voxels (vcoord[v] = {x, y, z, points}; d_dropped: one int of scratch, unused when V = 0): num_buckets =
+// init_buckets doubled until >= 8 V, then doubled again while more than drop_rate * total_points points fall out of it.
+// One host synchronisation per attempt.  On failure *buckets may hold a block the caller frees.
+static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dropped, int init_buckets, int max_scan, double drop_rate, double total_points,
+                             int4** buckets, int* num_buckets, int* num_dropped_points) {
+  cudaStream_t st = ctx->stream;
+  int nb = init_buckets;
+  while ((long long)nb < 8ll * V) nb *= 2;  // load factor <= 1/8: the XOR-of-primes hash clusters, and lookups that
+                                                             // MISS (most of them in global mapping) walk until the first empty slot;
+                                                             // same rule as the oracle
+  for (;;) {
+    GB_CUDA(gb_dev_malloc(ctx->device, sizeof(int4) * (size_t)nb, (void**)buckets));
+    k_table_clear<<<(nb + 255) / 256, 256, 0, st>>>(nb, *buckets);
+    ctx->launches++;
+    int dropped = 0;
+    if (V > 0) {
+      GB_CUDA(cudaMemsetAsync(d_dropped, 0, sizeof(int), st));
+      k_table_insert<<<(V + 255) / 256, 256, 0, st>>>(V, d_vcoord, *buckets, (uint32_t)nb - 1u, max_scan, d_dropped);
+      k_table_finalize<<<(nb + 255) / 256, 256, 0, st>>>(nb, d_vcoord, *buckets);
+      ctx->launches += 2;
+      GB_CUDA(cudaMemcpyAsync(&dropped, d_dropped, sizeof(int), cudaMemcpyDeviceToHost, st));
+    } else {
+      k_table_finalize<<<(nb + 255) / 256, 256, 0, st>>>(nb, d_vcoord, *buckets);
+      ctx->launches++;
+    }
+    GB_CUDA(cudaStreamSynchronize(st));
+    GB_CUDA(cudaGetLastError());
+    *num_buckets = nb;
+    *num_dropped_points = dropped;
+    if ((double)dropped <= drop_rate * total_points || nb >= (1 << 28)) break;
+    gb_dev_free(ctx->device, *buckets);
+    *buckets = nullptr;
+    nb *= 2;
+  }
+  return GB_OK;
+}
+
 gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_buckets, int max_scan, double drop_rate, gb_voxelmap* m) {
   const int n = (int)cloud->n;
   cudaStream_t st = ctx->stream;
@@ -184,37 +222,224 @@ gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resol
   }
   m->num_voxels = V;
   m->bytes = sizeof(float4) * 3 * (size_t)V;
+  GB_CHECK(table_build(ctx, V, d_vcoord, d_dropped, init_buckets, max_scan, drop_rate, (double)n, &m->buckets, &m->num_buckets, &m->num_dropped_points));
+  m->bytes += sizeof(int4) * (size_t)m->num_buckets;
+  return GB_OK;
+}
 
-  // hash table: double until the dropped-point rate is acceptable
-  int nb = init_buckets;
-  while ((long long)nb < 8ll * V) nb *= 2;  // load factor <= 1/8: the XOR-of-primes hash clusters, and lookups that
-                                                             // MISS (most of them in global mapping) walk until the first empty slot;
-                                                             // same rule as the oracle
-  for (;;) {
-    GB_CUDA(gb_dev_malloc(ctx->device, sizeof(int4) * (size_t)nb, (void**)&m->buckets));
-    k_table_clear<<<(nb + 255) / 256, 256, 0, st>>>(nb, m->buckets);
-    ctx->launches++;
-    int dropped = 0;
-    if (V > 0) {
-      GB_CUDA(cudaMemsetAsync(d_dropped, 0, sizeof(int), st));
-      k_table_insert<<<(V + 255) / 256, 256, 0, st>>>(V, d_vcoord, m->buckets, (uint32_t)nb - 1u, max_scan, d_dropped);
-      k_table_finalize<<<(nb + 255) / 256, 256, 0, st>>>(nb, d_vcoord, m->buckets);
-      ctx->launches += 2;
-      GB_CUDA(cudaMemcpyAsync(&dropped, d_dropped, sizeof(int), cudaMemcpyDeviceToHost, st));
-    } else {
-      k_table_finalize<<<(nb + 255) / 256, 256, 0, st>>>(nb, d_vcoord, m->buckets);
+// ---------------------------------------------------------------------------------------------
+// Incremental maps (gb_voxelmap_create_incremental / gb_voxelmap_insert; the rule is written once in include/glim_b200.h).
+// One insert is one pass over (the map's voxels, the frame's points):
+//   1. k_merge_transform   (gb_transform_frame, shared with gb_merge_frames) q = R a + t, R C R^T in un-contracted fp64
+//   2. k_grid_keys         (gb_grid_keys) packed floor(q * (1 / r)) in fp64; with sampling_rate < 1 the points whose
+//                          rg_hash(seed, index) is not among the m smallest lose their key (k_ins_sample_*, one radix sort)
+//   3. k_ins_old_keys      the map's voxel keys, tagged old (idx = -1 - v), ahead of the points: after the stable
+//                          gb_group_by_key a voxel's group is its old entry first, then its new points in index order
+//   4. k_ins_merge         one thread per merged voxel: stored sums + the new points one at a time, n, stamp, eviction
+//   5. scan + k_ins_emit   the survivors, in ascending key order, into a new state block (keys, n, stamps, sums, fp32 records)
+//   6. table_build         the build's table kernels and sizing rule
+// Two host synchronisations (survivor count; dropped points of each table attempt).  The old blocks go back to the pool
+// through gb_dev_free, which waits for every stream of the device: a sweep of another context still reading them is safe.
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+__global__ void k_ins_old_keys(int V, const unsigned long long* __restrict__ vkeys, unsigned long long* __restrict__ keys, int* __restrict__ idx) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  keys[v] = vkeys[v];
+  idx[v] = -1 - v;
+}
+__global__ void k_ins_sample_hash(int n, unsigned long long seed, unsigned long long* __restrict__ h) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) h[i] = rg_hash(seed, (unsigned)i);
+}
+// rg_hash is a bijection of the index for a fixed seed, so exactly the m smallest hashes are <= sorted[m - 1]
+__global__ void k_ins_sample_drop(int n, int m, unsigned long long seed, const unsigned long long* __restrict__ sorted, unsigned long long* __restrict__ keys) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && rg_hash(seed, (unsigned)i) > sorted[m - 1]) keys[i] = kInvalidKey;
+}
+
+__global__ void k_ins_merge(int N, const int* __restrict__ num_merged, const int* __restrict__ starts, const int* __restrict__ idx_s,
+                            const int* __restrict__ on, const int* __restrict__ ostamp, const double* __restrict__ osums,
+                            const double4* __restrict__ pts, const double* __restrict__ cov6, int counter, int horizon, int cycle,
+                            int* __restrict__ mn, int* __restrict__ mstamp, double* __restrict__ msums, int* __restrict__ keep, unsigned long long* __restrict__ total) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= N) return;
+  if (v >= *num_merged) { keep[v] = 0; return; }
+  const int b = starts[v], e = starts[v + 1];
+  double s[9];
+  int cnt = 0, stamp = counter, first = b;
+  const int i0 = idx_s[b];
+  if (i0 < 0) {
+    const int o = -1 - i0;
+    for (int k = 0; k < 9; k++) s[k] = osums[9 * (size_t)o + k];
+    cnt = on[o];
+    stamp = ostamp[o];
+    first = b + 1;
+  } else {
+    for (int k = 0; k < 9; k++) s[k] = 0.0;
+  }
+  for (int j = first; j < e; j++) {
+    const int i = idx_s[j];
+    const double4 p = pts[i];
+    const double* c = cov6 + 6 * (size_t)i;
+    s[0] += p.x; s[1] += p.y; s[2] += p.z;
+    for (int k = 0; k < 6; k++) s[3 + k] += c[k];
+  }
+  if (e > first) { cnt += e - first; stamp = counter; }
+  const int c1 = counter + 1;
+  const bool evict = horizon > 0 && c1 % cycle == 0 && stamp + horizon < c1;
+  keep[v] = evict ? 0 : 1;
+  mn[v] = cnt;
+  mstamp[v] = stamp;
+  for (int k = 0; k < 9; k++) msums[9 * (size_t)v + k] = s[k];
+  if (!evict) atomicAdd(total, (unsigned long long)cnt);
+}
+__global__ void k_ins_count(int N, const int* __restrict__ kpos, unsigned long long* __restrict__ kept) { *kept = (unsigned long long)kpos[N - 1]; }
+
+__global__ void k_ins_emit(int N, const int* __restrict__ num_merged, const int* __restrict__ keep, const int* __restrict__ kpos, const int* __restrict__ starts,
+                           const unsigned long long* __restrict__ keys_s, const int* __restrict__ mn, const int* __restrict__ mstamp, const double* __restrict__ msums,
+                           unsigned long long* __restrict__ vkeys, int* __restrict__ vn, int* __restrict__ vstamp, double* __restrict__ vsums,
+                           float4* __restrict__ voxels, int4* __restrict__ vcoord) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= N || v >= *num_merged || !keep[v]) return;
+  const int o = kpos[v] - 1;
+  const unsigned long long key = keys_s[starts[v]];
+  const int cnt = mn[v];
+  double s[9];
+  for (int k = 0; k < 9; k++) s[k] = msums[9 * (size_t)v + k];
+  vkeys[o] = key;
+  vn[o] = cnt;
+  vstamp[o] = mstamp[v];
+  for (int k = 0; k < 9; k++) vsums[9 * (size_t)o + k] = s[k];
+  const double dn = (double)cnt;
+  voxels[3 * (size_t)o + 0] = make_float4((float)(s[0] / dn), (float)(s[1] / dn), (float)(s[2] / dn), (float)(s[3] / dn));
+  voxels[3 * (size_t)o + 1] = make_float4((float)(s[4] / dn), (float)(s[5] / dn), (float)(s[6] / dn), (float)(s[7] / dn));
+  voxels[3 * (size_t)o + 2] = make_float4((float)(s[8] / dn), (float)cnt, 0.f, 0.f);
+  int x, y, z;
+  gb_unpack_key(key, x, y, z);
+  vcoord[o] = make_int4(x, y, z, cnt);
+}
+
+// the state block of V voxels: fp32 records first (gb_voxelmap::voxels), then keys, counts, stamps and sums
+void state_layout(Carver& cv, size_t V, gb_voxelmap* m) {
+  m->voxels = cv.take<float4>(3 * V);
+  m->vkeys = cv.take<unsigned long long>(V);
+  m->vn = cv.take<int>(V);
+  m->vstamp = cv.take<int>(V);
+  m->vsums = cv.take<double>(9 * V);
+}
+
+}  // namespace
+
+gb_status gb_voxelmap_create_incremental_impl(gb_ctx* ctx, gb_voxelmap* m) {
+  m->device = ctx->device;
+  m->incremental = true;
+  GB_CHECK(table_build(ctx, 0, nullptr, nullptr, m->init_buckets, m->max_scan, m->drop_rate, 0.0, &m->buckets, &m->num_buckets, &m->num_dropped_points));
+  m->bytes = sizeof(int4) * (size_t)m->num_buckets;
+  return GB_OK;
+}
+
+gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T, double sampling_rate, unsigned long long seed) {
+  cudaStream_t st = ctx->stream;
+  const int n = (int)cloud->n;
+  const int Vo = m->num_voxels;
+  const int kept = sampling_rate < 1.0 ? (int)(size_t)((double)n * sampling_rate) : n;  // random_sampling's count
+  const int np = kept > 0 ? n : 0;  // points that take part (the unsampled ones get no key)
+  const int N = Vo + np;
+  gb_voxelmap next = *m;  // the map after this insert; m is replaced only when everything has succeeded
+  next.lru_counter = m->lru_counter + 1;
+  next.version = m->version + 1;
+  if (N > 0) {
+    const size_t cub_b = gb_cub_temp_bytes((size_t)N);
+    gb_sort_tmp t;
+    int *d_flags, *d_pos, *d_starts, *d_keep, *d_kpos, *d_mn, *d_mstamp, *d_dropped;
+    double4* d_pts = nullptr;
+    double *d_cov = nullptr, *d_msums;
+    unsigned long long *d_hash = nullptr, *d_info;
+    void* d_frame;
+    int4* d_vcoord;
+    GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+      t = gb_take_sort_tmp(cv, (size_t)N, cv.take<char>(cub_b), cub_b);
+      d_flags = cv.take<int>(N + 1);
+      d_pos = cv.take<int>(N + 1);
+      d_starts = cv.take<int>(N + 1);
+      d_keep = cv.take<int>(N + 1);
+      d_kpos = cv.take<int>(N + 1);
+      d_mn = cv.take<int>(N);
+      d_mstamp = cv.take<int>(N);
+      d_msums = cv.take<double>(9 * (size_t)N);
+      d_vcoord = cv.take<int4>(N);
+      d_dropped = cv.take<int>(1);
+      d_info = cv.take<unsigned long long>(2);  // {points in the surviving voxels, surviving voxels}
+      d_frame = cv.take<char>(GB_FRAME_DESC_BYTES);
+      if (np > 0) {
+        d_pts = cv.take<double4>(np);
+        d_cov = cv.take<double>(6 * (size_t)np);
+        if (kept < n) d_hash = cv.take<unsigned long long>(np);
+      }
+    }));
+    const int tb = 256;
+    if (Vo > 0) {
+      k_ins_old_keys<<<(Vo + tb - 1) / tb, tb, 0, st>>>(Vo, m->vkeys, t.keys, t.idx);
       ctx->launches++;
     }
+    if (np > 0) {
+      GB_CHECK(gb_transform_frame(ctx, cloud, T, d_frame, d_pts, d_cov));
+      gb_grid_keys(ctx, np, d_pts, 1.0 / (double)m->resolution, t.keys + Vo, t.idx + Vo);
+      if (kept < n) {
+        k_ins_sample_hash<<<(np + tb - 1) / tb, tb, 0, st>>>(np, seed, t.keys_s);
+        size_t tmp = cub_b;
+        GB_CUDA(cub::DeviceRadixSort::SortKeys(t.cub, tmp, t.keys_s, d_hash, np, 0, 64, st));
+        k_ins_sample_drop<<<(np + tb - 1) / tb, tb, 0, st>>>(np, kept, seed, d_hash, t.keys + Vo);
+        ctx->launches += 3;
+      }
+    }
+    GB_CUDA(cudaMemsetAsync(d_info, 0, 2 * sizeof(unsigned long long), st));
+    GB_CHECK(gb_group_by_key(ctx, N, t, d_flags, d_pos));
+    gb_group_starts(ctx, N, t, d_flags, d_pos, d_starts);
+    k_ins_merge<<<(N + 127) / 128, 128, 0, st>>>(N, d_pos + (N - 1), d_starts, t.idx_s, m->vn, m->vstamp, m->vsums, d_pts, d_cov, m->lru_counter,
+                                                  m->lru_horizon, m->lru_clear_cycle, d_mn, d_mstamp, d_msums, d_keep, d_info);
+    size_t tmp = cub_b;
+    GB_CUDA(cub::DeviceScan::InclusiveSum(t.cub, tmp, d_keep, d_kpos, N, st));
+    k_ins_count<<<1, 1, 0, st>>>(N, d_kpos, d_info + 1);
+    ctx->launches += 3;
+    unsigned long long info[2] = {0, 0};
+    GB_CUDA(cudaMemcpyAsync(info, d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
-    GB_CUDA(cudaGetLastError());
-    m->num_buckets = nb;
-    m->num_dropped_points = dropped;
-    if ((double)dropped <= drop_rate * (double)n || nb >= (1 << 28)) break;
-    gb_dev_free(ctx->device, m->buckets);
-    m->buckets = nullptr;
-    nb *= 2;
+    const int V = (int)info[1];
+    next.base = nullptr;
+    next.buckets = nullptr;
+    next.num_voxels = V;
+    Carver size;
+    state_layout(size, (size_t)V, &next);
+    next.bytes = V > 0 ? size.off : 0;
+    if (V > 0) {
+      GB_CUDA(gb_dev_malloc(ctx->device, size.off, &next.base));
+      Carver cv{(char*)next.base};
+      state_layout(cv, (size_t)V, &next);
+      k_ins_emit<<<(N + tb - 1) / tb, tb, 0, st>>>(N, d_pos + (N - 1), d_keep, d_kpos, d_starts, t.keys_s, d_mn, d_mstamp, d_msums,
+                                                   next.vkeys, next.vn, next.vstamp, next.vsums, next.voxels, d_vcoord);
+      ctx->launches++;
+    } else {
+      next.voxels = nullptr; next.vkeys = nullptr; next.vn = nullptr; next.vstamp = nullptr; next.vsums = nullptr;
+    }
+    gb_status s = table_build(ctx, V, d_vcoord, d_dropped, m->init_buckets, m->max_scan, m->drop_rate, (double)info[0], &next.buckets, &next.num_buckets, &next.num_dropped_points);
+    if (s != GB_OK) {
+      gb_dev_free(ctx->device, next.base);
+      gb_dev_free(ctx->device, next.buckets);
+      return s;
+    }
+    next.bytes += sizeof(int4) * (size_t)next.num_buckets;
   }
-  m->bytes += sizeof(int4) * (size_t)m->num_buckets;
+  void* old_base = m->base;
+  int4* old_buckets = m->buckets;
+  const bool replaced = N > 0;
+  *m = next;
+  if (replaced) {
+    gb_dev_free(ctx->device, old_base);
+    gb_dev_free(ctx->device, old_buckets);
+  }
   return GB_OK;
 }
 

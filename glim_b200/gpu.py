@@ -5,6 +5,7 @@ include/glim_b200/gtsam_points_compat.hpp.
 
     PointCloudGPU.clone(points, covs)                       odometry_estimation_gpu.cpp:96
     GaussianVoxelMapGPU(resolution, 8192*2, 10, 1e-3).insert(cloud)   odometry_estimation_gpu.cpp:103-104
+    IncrementalVoxelMapGPU(resolution, lru_horizon).insert(cloud, T, rate)   GaussianVoxelMapCPU::insert, odometry_estimation_cpu.cpp:177-191
     IntegratedVGICPFactorGPU(target_key | fixed_target_pose, source_key, voxelmap, source)   :144, :161
     NonlinearFactorSetGPU.add(...) / .linearize(values)     odometry_estimation_gpu.cpp:383-386
     overlap_gpu(voxelmap(s), source, delta(s))              odometry_estimation_gpu.cpp:231, :248
@@ -141,6 +142,45 @@ class GaussianVoxelMapGPU:
         vcov = np.empty((self.num_voxels, 6), np.float32)
         check(lib().gb_voxelmap_download(self.h, ptr(buckets), ptr(vnum), ptr(vmean), ptr(vcov)))
         return buckets, vnum, vmean, vcov
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx and self.ctx.h:
+            lib().gb_voxelmap_destroy(self.h)
+            self.h = None
+
+
+class IncrementalVoxelMapGPU:
+    """A Gaussian voxel map kept on the device across frames (gb_voxelmap_create_incremental / gb_voxelmap_insert): the
+    GaussianVoxelMapCPU::insert + set_lru_horizon target of GLIM's odometry (odometry_estimation_cpu.cpp:67, :177-191).  Accepted
+    wherever a GaussianVoxelMapGPU is (factors, align_vgicp, overlap_gpu); factors and sweeps follow its inserts."""
+
+    def __init__(self, resolution: float, lru_horizon: int = 0, lru_clear_cycle: int = 10, init_num_buckets: int = 16384, max_bucket_scan_count: int = 10,
+                 target_points_drop_rate: float = 1e-3, ctx: Context | None = None):
+        self.ctx = ctx or default_context()
+        self.resolution = float(resolution)
+        self.h = None
+        h = C.c_void_p()
+        check(lib().gb_voxelmap_create_incremental(self.ctx.h, self.resolution, init_num_buckets, max_bucket_scan_count, target_points_drop_rate,
+                                                   int(lru_horizon), int(lru_clear_cycle), C.byref(h)))
+        self.h = h
+        self._info()
+
+    def _info(self):
+        nv, nb, res = C.c_int(), C.c_int(), C.c_float()
+        check(lib().gb_voxelmap_info(self.h, C.byref(nv), C.byref(nb), C.byref(res)))
+        self.num_voxels, self.num_buckets = nv.value, nb.value
+
+    def insert(self, cloud: PointCloudGPU, T=None, sampling_rate: float = 1.0, seed: int = 0):
+        """Insert `cloud` at T_map_cloud (4x4, None = identity), keeping a sampling_rate share of its points."""
+        Tc = pose16(np.asarray(T, dtype=np.float64).reshape(4, 4)) if T is not None else None
+        check(lib().gb_voxelmap_insert(self.ctx.h, self.h, cloud.h, ptr(Tc), float(sampling_rate), int(seed)))
+        self._info()
+        return self
+
+    def voxel_resolution(self) -> float:
+        return self.resolution
+
+    download = GaussianVoxelMapGPU.download
 
     def __del__(self):
         if getattr(self, "h", None) and self.ctx and self.ctx.h:
@@ -422,7 +462,7 @@ def align_vgicp(problems: list[list[IntegratedVGICPFactorGPU]], T_init, params=N
 
 def overlap_gpu(voxelmaps, source: PointCloudGPU, deltas, ctx: Context | None = None) -> float:
     """gtsam_points::overlap_gpu: single (voxelmap, delta) or lists (odometry_estimation_gpu.cpp:231, :248)."""
-    if isinstance(voxelmaps, GaussianVoxelMapGPU):
+    if isinstance(voxelmaps, (GaussianVoxelMapGPU, IncrementalVoxelMapGPU)):
         voxelmaps, deltas = [voxelmaps], [deltas]
     ctx = ctx or source.ctx
     T = len(voxelmaps)

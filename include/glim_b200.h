@@ -115,6 +115,43 @@ GB_API gb_status gb_voxelmap_info(const gb_voxelmap* map, int* num_voxels, int* 
 GB_API gb_status gb_voxelmap_download(const gb_voxelmap* map, int32_t* buckets, int32_t* num_points, float* means, float* cov6);
 GB_API gb_status gb_voxelmap_destroy(gb_voxelmap* map);
 
+/* ---- Incremental device map: the scan-to-map target of GLIM's odometry (odometry_estimation_cpu.cpp:177-191, update_target:
+ *      random_sampling(10 %) from frame 5 on, transform, GaussianVoxelMapCPU::insert on every level; set_lru_horizon(lru_thresh
+ *      = 100) at :67), kept on the device.  The result is an ordinary gb_voxelmap: info, download, destroy, factors, sweeps,
+ *      gb_vgicp_align and gb_overlap take it unchanged, and sweeps created before an insert follow it (their descriptors
+ *      are re-written before the next launch).
+ *
+ *      The rule.  Per voxel the map keeps its packed key, n, fp64 sums Sigma q (3) and Sigma C (6 unique entries) and
+ *      stamp; per map the insert counter c, h = lru_horizon and k = lru_clear_cycle.  One insert:
+ *        1. sample: sampling_rate = 1 keeps every point; otherwise m = (size_t)(n * rate) points are kept (random_sampling's
+ *           count): those with the smallest rg_hash(seed, original index) ([EXT]: the reference draws with std::mt19937).
+ *        2. transform the kept points with finite x, y, z: q = R a + t, C' = R C R^T, un-contracted fp64 (gb_merge_frames'
+ *           association order).
+ *        3. key: floor(q * (1.0 / (double)resolution)) in fp64, as GaussianVoxelMapCPU; points outside the 21-bit key range
+ *           (+-2^20 voxels) are skipped.
+ *        4. accumulate: each touched voxel starts from its stored sums (new voxels from zero) and adds its new points one at
+ *           a time in original index order; then n += count, stamp = c.
+ *        5. evict: c += 1; if h > 0 and c % k == 0, the voxels with stamp + h < c are dropped.  An insert that keeps no
+ *           points still advances c.
+ *        6. finalize: record = (float)(Sigma / n) component-wise, with n, in ascending packed-key order (the build's voxel
+ *           numbering); the table is rebuilt with the build's sizing rule (init_num_buckets doubled until >= 8 V, then while
+ *           more than target_points_drop_rate * Sigma n points are dropped).
+ *      Voxel coordinates come from fp64 keys, while every lookup (sweeps, overlap) uses the fp32 rule of the build: a point
+ *      exactly on a voxel face may resolve to a neighbouring voxel at lookup time.
+ *
+ *      Threading: do not insert into a map while another thread uses it (linearizes a factor on it, builds a sweep over it,
+ *      ...) -- the same caller bug as destroying a map a live factor borrows.  Device work already in flight on another
+ *      context stays safe: the replaced device blocks are recycled only after every stream of the device has drained.
+ *      Like the build, an insert returns after its stream has drained: two host synchronisations per insert. ---- */
+/* An empty map that accepts any number of inserts.  lru_horizon <= 0: no eviction; lru_clear_cycle >= 1 (gtsam_points: 10). */
+GB_API gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolution, int init_num_buckets, int max_bucket_scan_count,
+                                                double target_points_drop_rate, int lru_horizon, int lru_clear_cycle, gb_voxelmap** out);
+/* Insert `cloud` at T_map_cloud (NULL = identity), keeping a sampling_rate share of its points (1 = all).  Every input is
+ * validated before any launch: GB_ERR_INVALID_ARGUMENT for a map from gb_voxelmap_build (it keeps no sums), a non-finite
+ * T, sampling_rate outside (0, 1], or a cloud / map on another device than ctx. */
+GB_API gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_cloud* cloud, const double* T_map_cloud /* 16, col-major */,
+                                    double sampling_rate, uint64_t seed);
+
 /* ---- IntegratedVGICPFactorGPU(target_key | fixed_target_pose, source_key, voxelmap, source, stream, buffer)
  *      (odometry_estimation_gpu.cpp:144,161; sub_mapping.cpp:307; global_mapping.cpp:335,466,860).
  *      Keys and the binary/unary distinction stay on the host side of the boundary: the device only

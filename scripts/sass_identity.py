@@ -20,7 +20,9 @@ def kernels(path):
     for part in re.split(r"\n\s*Function : ", txt)[1:]:
         name, body = part.split("\n", 1)
         body = body.split("\nFatbin ", 1)[0]  # the last function of a cubin is followed by the next fatbin section's header
-        body = "\n".join(l.rstrip() for l in body.splitlines() if l.strip())
+        # runs of blanks collapse: cuobjdump pads its columns to the widest instruction of the cubin, so a new kernel in the
+        # same translation unit would otherwise change the text of every other kernel there
+        body = "\n".join(" ".join(l.split()) for l in body.splitlines() if l.strip())
         out[name.strip()] = hashlib.sha256(body.encode()).hexdigest()
     return out
 
