@@ -1208,6 +1208,14 @@ extern "C" gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, c
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw && neighbors && normals4 && cov4x4, "null argument");
   GB_REQUIRE(k_neighbors > 0 && k_neighbors <= k_correspondences, "k_neighbors must be in [1, k_correspondences]");
+  GB_REQUIRE(n < (size_t)1 << 30, "too many points");
+  // the kernel gathers the points of the first k_neighbors entries of every row: an index outside [0, n) would be an
+  // out-of-bounds device read
+  for (size_t i = 0; i < n; i++)
+    for (int j = 0; j < k_neighbors; j++) {
+      const int32_t q = neighbors[i * (size_t)k_correspondences + j];
+      GB_REQUIRE(q >= 0 && (size_t)q < n, "neighbour index out of range [0, n)");
+    }
   GB_CUDA(cudaSetDevice(ctx->device));
   return gb_covariances_impl(ctx, n, xyzw, neighbors, k_correspondences, k_neighbors, normals4, cov4x4);
 }
@@ -1215,6 +1223,7 @@ extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n, const double* xyzw
   GB_REQUIRE(ctx, "null ctx");
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw && neighbors && k > 0, "null argument");
+  GB_REQUIRE(gb_knn_instantiated(k), "k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
   GB_LOCK(ctx);
   GB_CUDA(cudaSetDevice(ctx->device));
   // >= 4096 points: exact search on a pyramid of hash grids (one Morton sort, cell size 0.25 m x 4^level); fewer: the tiled
@@ -1277,9 +1286,9 @@ extern "C" gb_status gb_preprocess(gb_ctx* ctx, size_t n, const double* xyzw, co
   GB_REQUIRE(ctx && P && out, "null argument");
   out->num_points = 0; out->last_time = 0.0; out->cloud = nullptr;
   GB_REQUIRE(n < (size_t)1 << 30, "too many points");
-  GB_REQUIRE(P->k_correspondences > 0, "k_correspondences must be positive");
+  GB_REQUIRE(gb_knn_instantiated(P->k_correspondences), "k_correspondences is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
   GB_REQUIRE(P->k_neighbors_cov >= 0 && P->k_neighbors_cov <= P->k_correspondences, "k_neighbors_cov must be in [0, k_correspondences]");
-  GB_REQUIRE(!P->enable_outlier_removal || (P->outlier_removal_k > 0 && P->outlier_removal_k <= 32), "outlier_removal_k must be in [1, 32]");
+  GB_REQUIRE(!P->enable_outlier_removal || gb_knn_instantiated(P->outlier_removal_k), "outlier_removal_k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
   GB_REQUIRE(P->crop_bbox_frame >= 0 && P->crop_bbox_frame <= 2, "crop_bbox_frame must be 0 (off), 1 (lidar) or 2 (imu)");
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw, "null points");

@@ -316,6 +316,9 @@ gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n, const double* xyzw, const do
 gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out);
 gb_status gb_find_neighbors_pyramid_impl(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors);
 gb_status gb_find_neighbors_impl(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors);
+// true iff the k-NN kernels are instantiated for k neighbours (1-10, 12, 15, 16, 20, 24, 32); entry points check it before
+// any launch
+bool gb_knn_instantiated(int k);
 gb_status gb_voxelgrid_sampling_impl(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, double resolution, double* out_xyzw, double* out_times, double* out_intensities, size_t* num_out);
 
 // ---------------------------------------------------------------------------------------------
