@@ -512,15 +512,15 @@ static int env_int(const char* name, int dflt) {
   return v && *v ? atoi(v) : dflt;
 }
 
-// The work-item table of a sweep (descs[f].num_tiles / first_tile and the (factor, offset) list).
-//   contiguous: items of tile_size consecutive points, factor-major (drawn from the queue by the persistent warps);
-//   strided   : about one item per warp in total; factor f gets J_f items in proportion to its expected cost
+// The work-item table of a sweep (descs[f].num_tiles / first_tile and the (factor, offset) list); it follows the kernel.
+//   sweep3: items of tile_size consecutive points, factor-major (drawn from the queue by the persistent warps);
+//   sweep5: strided items, about one item per warp in total; factor f gets J_f items in proportion to its expected cost
 //               n_f * (1 + 1.25 r_f) (r_f = inlier fraction of its last linearization, 0.5 if unknown; a hit costs ~2.2x a
 //               miss), item j owning the 32-point rows j, j + J_f, ... of the source cloud.
 static void build_items(gb_sweep* s, FactorDesc* descs, std::vector<int2>& tiles) {
   tiles.clear();
   const size_t F = s->F;
-  if (!s->strided) {
+  if (s->kernel_version == 3) {
     // TAIL TAPERING (guided self-scheduling): the last wave of a sweep leaves warps idle for up to one 2048-point item time --
     // little of a single-GPU sweep but a large share of one of 8 ranks' shard.  The factors that
     // hold the last ~1.5 item-times of work per warp get items of a quarter of the size, the last 0.4 a sixteenth.
@@ -577,14 +577,14 @@ static void build_items(gb_sweep* s, FactorDesc* descs, std::vector<int2>& tiles
   }
 }
 
-// After results have been fetched (the stream is idle): remember every factor's inlier fraction, and -- once per strided
+// After results have been fetched (the stream is idle): remember every factor's inlier fraction, and -- once per sweep5
 // sweep -- re-size its item table from them.
 static gb_status sweep_learn_inliers(gb_sweep* s) {
   for (size_t f = 0; f < s->F; f++) {
     gb_factor* fa = s->factors[f];
     if (fa && fa->source->n) fa->inlier_frac = (float)(s->h_out[f * GB_OUT_DOUBLES + 121] / (double)fa->source->n);
   }
-  if (!s->strided || s->calibrated || s->stale) return GB_OK;
+  if (s->kernel_version != 5 || s->calibrated || s->stale) return GB_OK;
   s->calibrated = true;
   std::vector<int> old(s->F);
   for (size_t f = 0; f < s->F; f++) old[f] = s->h_descs[f].num_tiles;
@@ -668,15 +668,14 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   // Kernel policy (A/B runs of the kernels, scripts/ab_sweep.py): small sweeps -- about one item per warp: an odometry
   // frame, a single pair -- run k_vgicp_sweep5 with one wave of equally expensive STRIDED items (faster on the odometry
   // workload); large sweeps run k_vgicp_sweep3 with contiguous 2048-point items drawn from the queue (its simpler hot loops
-  // are faster there).  GB_KERNEL = 3 / 5 forces one kernel.
+  // are faster there).  GB_KERNEL = 3 / 5 forces one kernel, with its own kind of items.
   const int kv = env_int("GB_KERNEL", 0);
   s->capacity = ctx->num_sms * 2;
   const uint64_t warps = (uint64_t)s->capacity * 8;
   const bool small = F > 0 && total_pts <= warps * 2048;
   s->kernel_version = (kv == 3 || kv == 5) ? kv : (small ? 5 : 3);
-  s->strided = (s->kernel_version == 5 && small && env_int("GB_STRIDED", 1)) ? 1 : 0;
   {
-    // contiguous items: ~6 items per warp (first one static, the rest drawn dynamically), between 128 and 2048 points each,
+    // sweep3's items: ~6 items per warp (first one static, the rest drawn dynamically), between 128 and 2048 points each,
     // in whole rows of 32 points
     constexpr uint64_t kItemsPerWarp = 6, kMinItem = 128, kMaxItem = 2048;
     const uint64_t want = total_pts / (warps * kItemsPerWarp) + 1;
@@ -716,7 +715,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
 
   if (F > 0) {
     // one device block, one pinned block -- taken from the context's pool when a retired sweep left a fitting one
-    s->tiles_cap = std::max<size_t>(tiles.size(), s->strided ? (size_t)warps + F : 0);
+    s->tiles_cap = std::max<size_t>(tiles.size(), s->kernel_version == 5 ? (size_t)warps + F : 0);
     const size_t b_desc = align_up(sizeof(FactorDesc) * F, 256), b_tiles = align_up(sizeof(int2) * s->tiles_cap, 256), b_pose = align_up(sizeof(double) * 16 * F, 256);
     const size_t b_acc = align_up(sizeof(double) * GB_ACC_STRIDE * F * s->acc_slots, 256), b_done = align_up(sizeof(unsigned) * F + 16, 256), b_out = align_up(sizeof(double) * GB_OUT_DOUBLES * F, 256);
     const size_t total = b_desc + b_tiles + 2 * b_pose + b_acc + b_done + b_out;
@@ -855,7 +854,7 @@ static gb_status cached_sweep(gb_ctx* ctx, size_t F, gb_factor* const* factors, 
 // as a CUDA graph, every linearization is then ONE launch call instead of three API calls (the online odometry path calls this
 // ~10 times per frame: odometry_estimation_gpu.cpp:383-386).
 static bool graph_eligible(const gb_sweep* s) {
-  return s->graph_state >= 0 && s->strided && !s->peer && !s->d_slab && (unsigned long long)s->num_tiles <= (unsigned long long)s->grid * 8ull && s->F > 0;
+  return s->graph_state >= 0 && s->kernel_version == 5 && !s->peer && !s->d_slab && (unsigned long long)s->num_tiles <= (unsigned long long)s->grid * 8ull && s->F > 0;
 }
 static gb_status sweep_linearize(gb_sweep* s, const double* T, gb_linearized6* out) {
   if (!graph_eligible(s)) {

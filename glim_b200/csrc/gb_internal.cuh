@@ -96,7 +96,7 @@ struct FactorDesc {
   int pair;
   int flags;
   int num_tiles;
-  int chunk;       // contiguous items: points per item of THIS factor (the last factors of a sweep get smaller items: tail tapering)
+  int chunk;       // sweep3: points per item of THIS factor (the last factors of a sweep get smaller items: tail tapering)
 };
 static_assert(sizeof(FactorDesc) == 80, "FactorDesc size");
 
@@ -169,11 +169,12 @@ struct gb_sweep {
   unsigned* d_pair_done = nullptr;
   PeerPush* d_peer_tables = nullptr;  // [2]: one per step parity
   std::vector<int> h_pair;            // pair id per factor
-  int num_tiles = 0, tile_size = 0, grid = 0;  // work items, points per item, CTAs
-  int kernel_version = 0;           // 5 = small sweeps (one wave of strided items); 3 = large sweeps (queue of contiguous items) (GB_KERNEL=3/5 forces one)
+  int num_tiles = 0, tile_size = 0, grid = 0;  // work items, points per sweep3 item, CTAs
+  // 5 = small sweeps: strided items, item j of a factor owns its rows j, j + J, ... (about one item per warp; see k_vgicp_sweep5);
+  // 3 = large sweeps: a queue of contiguous items.  GB_KERNEL=3/5 forces one; the item table follows the kernel.
+  int kernel_version = 0;
   bool any_sv = false;              // some factor of the sweep has surface validation on
-  int strided = 0;                  // v5, about one item per warp: item j of a factor owns the rows j, j + J, ... (see k_vgicp_sweep5)
-  bool calibrated = false;          // strided: the item table has been re-sized from measured inlier fractions
+  bool calibrated = false;          // sweep5: the item table has been re-sized from measured inlier fractions
   int capacity = 0;                 // CTAs of a full grid
   FactorDesc* h_descs = nullptr;    // pinned copies (re-uploaded when the item table is re-sized)
   int2* h_tiles = nullptr;

@@ -6,10 +6,13 @@
 // gtsam_points::overlap_gpu (odometry_estimation_gpu.cpp:231,248).  Math: SURVEY.md Appendix A;
 // oracle: go_vgicp_linearize_gpumap / go_vgicp_error_gpumap / go_overlap_gpumap (oracle/glim_oracle.c).
 //
-// One launch covers a whole factor set.  Work unit = an item of up to `chunk` consecutive source
-// points of one factor; items are laid out factor-major and processed by the warps of a persistent grid
-// (first item = warp index, further items from a global queue), so at any instant the grid works on a
+// One launch covers a whole factor set.  Work unit = an item: a set of source points of one factor (consecutive points
+// in sweep3, strided rows in sweep5, below); items are laid out factor-major and processed by the warps of a persistent
+// grid (first item = warp index, further items from a global queue), so at any instant the grid works on a
 // window of a few consecutive factors whose source cloud and voxel tables stay L2 resident.
+// Both kernels run the same steps, written once below: phase A (probe_issue, probe_compact) resolves a round of points
+// into the warp's shared-memory queue of hits, phase B (accumulate_queue) accumulates them, then reduce_item and the
+// item's ticket (ticket_last); the warp that draws a factor's last ticket retires it (retire_factor).
 // Per inlier (one lane):
 //   q = R a + t -> voxel coord -> hash probe (16-byte buckets) -> 48-byte voxel record ->
 //   S = C_B + R C_A R^T, M = S^-1 (symmetric 3x3) -> accumulate the 21 unique entries of
@@ -38,7 +41,24 @@ static_assert(GB_MODE_LINEARIZE == GB_MODE_LINEARIZE_VALUE, "gb_vgicp_math.cuh m
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
-// probe result of one point given its first two buckets (b, b1 fetched together: adjacent 16-byte slots, one round trip)
+// A point's hash probe in flight: its voxel coordinates, hash and first two buckets.
+struct Probe {
+  int cx, cy, cz;
+  uint32_t h;
+  int4 b, b1;
+};
+
+// phase A, issue: transform one source point, and fetch its first two buckets together (adjacent 16-byte slots, one round trip)
+__device__ __forceinline__ void probe_issue(const FactorDesc& D, const PoseF& P, float ax, float ay, float az, Probe& p) {
+  float qx, qy, qz;
+  transform(P, ax, ay, az, qx, qy, qz);
+  p.cx = gb_coord(qx, D.inv_res); p.cy = gb_coord(qy, D.inv_res); p.cz = gb_coord(qz, D.inv_res);
+  p.h = gb_hash(p.cx, p.cy, p.cz);
+  p.b = __ldg(&D.buckets[p.h & D.mask]);
+  p.b1 = __ldg(&D.buckets[(p.h + 1u) & D.mask]);
+}
+
+// voxel index of a probed point, -1 for a miss
 __device__ __forceinline__ int resolve_probe(const FactorDesc& D, const int4 b, const int4 b1, uint32_t h, int cx, int cy, int cz) {
   int v = -1;
   if (b.w >= 0) {
@@ -57,6 +77,16 @@ __device__ __forceinline__ int resolve_probe(const FactorDesc& D, const int4 b, 
     }
   }
   return v;
+}
+
+// phase A, compaction: a hit of point i (none when i >= limit) is appended to the warp's queue as (point, voxel), in lane order.
+// nq: the warp-uniform queue length.
+__device__ __forceinline__ void probe_compact(const FactorDesc& D, const Probe& p, int i, int limit, uint2* __restrict__ q, int& nq, unsigned lt_mask) {
+  int v = resolve_probe(D, p.b, p.b1, p.h, p.cx, p.cy, p.cz);
+  if (i >= limit) v = -1;
+  const unsigned m = __ballot_sync(0xffffffffu, v >= 0);
+  if (v >= 0) q[nq + __popc(m & lt_mask)] = make_uint2((unsigned)i, (unsigned)v);
+  nq += __popc(m);
 }
 
 // Transposing warp reduction: on return lane l holds sum over the warp of v[l] (in v[0]).
@@ -118,6 +148,7 @@ __device__ __noinline__ void pair_push(const FactorDesc& D, const double* __rest
 // fp64 epilogue of one factor, executed (all 32 lanes in parallel) by the warp that retired the factor's last item.
 // sm: >= 104 doubles of shared memory (A[32] | Ad[36] | X[36]).
 constexpr int kEpilogueDoubles = 104;
+constexpr int kPairRowOffset = 2 * kEpilogueDoubles;  // floats: pair_push's row follows the epilogue's scratch in the warp's queue
 __device__ __noinline__ void factor_epilogue(int f, const FactorDesc& D, const double* __restrict__ poses, double* __restrict__ accum, int acc_slots, double* __restrict__ out, float* __restrict__ slab, double* sm) {
   const int lane = threadIdx.x & 31;
   double* A = sm;        // 32 accumulators
@@ -196,6 +227,62 @@ __device__ __noinline__ void factor_epilogue(int f, const FactorDesc& D, const d
   __syncwarp();
 }
 
+// phase B: the lanes walk the nq queued hits, so the warp stays full whatever the inlier rate.  SV = false compiles the
+// surface validation out (no factor of the sweep has it on).
+template <int MODE, bool SV>
+__device__ __forceinline__ void accumulate_queue(float (&acc)[32], const FactorDesc& D, const PoseF& P, const PoseF& Pe, const uint2* __restrict__ q, int nq, int lane) {
+#pragma unroll 2
+  for (int k = lane; k < nq; k += 32) {
+    const uint2 e = q[k];
+    const int i = (int)e.x;
+    const float4 a0 = __ldg(&D.p0[i]);
+    const float4 a1 = __ldg(&D.p1[i]);
+    const float a2 = __ldg(&D.p2[i]);
+    const float4 v0 = __ldg(&D.voxels[3 * (size_t)e.y + 0]);
+    const float4 v1 = __ldg(&D.voxels[3 * (size_t)e.y + 1]);
+    const float4 v2 = __ldg(&D.voxels[3 * (size_t)e.y + 2]);
+    if (!SV || D.normals == nullptr || surface_ok(P, __ldg(&D.normals[i]), v0.w, v1.x, v1.y, v1.z, v1.w, v2.x)) accumulate_hit<MODE>(acc, Pe, a0, a1, a2, v0, v1, v2);
+  }
+}
+
+// An item's sums into its factor's accumulator copy (item mod acc_slots): all 29 (linearize) or the error and the inlier
+// count (error).
+template <int MODE>
+__device__ __forceinline__ void reduce_item(float (&acc)[32], double* __restrict__ accum, int f, int acc_slots, int item, int lane) {
+  double* __restrict__ my_acc = accum + ((size_t)f * acc_slots + (size_t)(item & (acc_slots - 1))) * GB_ACC_STRIDE;
+  if (MODE == GB_MODE_LINEARIZE) {
+    const float r = warp_reduce_scatter32(acc, lane);
+    if (lane < 29) atomicAdd(&my_acc[lane], (double)r);
+  } else {
+    float e = acc[27], n = acc[28];
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) { e += __shfl_xor_sync(0xffffffffu, e, o); n += __shfl_xor_sync(0xffffffffu, n, o); }
+    if (lane == 27) atomicAdd(&my_acc[27], (double)e);
+    if (lane == 28) atomicAdd(&my_acc[28], (double)n);
+  }
+}
+
+// Lane 0, after a __syncwarp: publishes the completion of one of factor f's items.  Returns whether it was the last of the
+// factor's num_tiles() items; its drawer re-zeroes the ticket for the next sweep (self-cleaning).  num_tiles() is evaluated
+// after the release: sweep5 reads it from its descriptors, and reading it ahead of the release measured slower there.
+template <class NumTiles>
+__device__ __forceinline__ int ticket_last(unsigned* __restrict__ done, int f, const NumTiles& num_tiles) {
+  const unsigned t = ticket_release(&done[f]);
+  const int last = (t == (unsigned)num_tiles() - 1u);
+  if (last) done[f] = 0u;
+  return last;
+}
+
+// Retires factor f, by the warp that drew its last ticket: fp64 epilogue, then the pair push when a peer slab is attached.
+// The warp's queue q is free at this point and serves as scratch.  The caller issues fence_acquire() and then copies D: a
+// copy taken in here lands ahead of acc[] in sweep3's stack frame, which changed its code and measured slower.
+template <int MODE, bool PEER>
+__device__ __forceinline__ void retire_factor(int f, const FactorDesc& D, const double* __restrict__ poses, const double* __restrict__ poses_eval,
+                                              double* __restrict__ accum, int acc_slots, double* __restrict__ out, float* __restrict__ slab, const PeerPush* __restrict__ peer, uint2* q) {
+  factor_epilogue(f, D, MODE == GB_MODE_ERROR ? poses_eval : poses, accum, acc_slots, out, slab, reinterpret_cast<double*>(q));
+  if (PEER && MODE == GB_MODE_LINEARIZE) pair_push(D, out, peer, reinterpret_cast<float*>(q) + kPairRowOffset);
+}
+
 // =============================================================================================
 // k_vgicp_sweep3 -- the large-sweep kernel: register-staged loads, contiguous items drawn from a global queue (the atomic
 // for the next item is issued at the start of the current one).  An item's completion ticket is published LAZILY: an
@@ -212,14 +299,14 @@ constexpr int kLookupUnroll = 4;
 template <int MODE, bool PEER, bool SV>
 __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
   const FactorDesc* __restrict__ descs, const double* __restrict__ poses, const double* __restrict__ poses_eval,
-  const int2* __restrict__ items, int num_items, int chunk,
+  const int2* __restrict__ items, int num_items,
   unsigned long long* __restrict__ item_ctr, unsigned long long ctr_base,
   double* __restrict__ accum, int acc_slots, unsigned* __restrict__ done, double* __restrict__ out, float* __restrict__ slab, const PeerPush* __restrict__ peer) {
   __shared__ __align__(16) uint2 s_q[kWarps][kSubMax];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned lt_mask = (1u << lane) - 1u;
   uint2* __restrict__ q = s_q[warp];
-  (void)chunk;
+  auto desc_of = [&](int f) { return descs[f]; };  // a copy, for retire_factor
 
   // first item: static (warp id); further items (only when there are more items than warps) come from the global queue
   const int total_warps = gridDim.x * kWarps;
@@ -227,12 +314,8 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
   int item = blockIdx.x * kWarps + warp;
   if (item >= num_items) return;
   int2 it = __ldg(&items[item]);
-  int pend_f = -1, pend_last = 0, pend_tiles = 0;
-  auto publish = [&]() {  // lane 0, after a __syncwarp: the previous item's ticket
-    const unsigned t = ticket_release(&done[pend_f]);
-    pend_last = (t == (unsigned)pend_tiles - 1u);
-    if (pend_last) done[pend_f] = 0u;  // self-cleaning
-  };
+  int pend_f = -1, pend_last = 0, pend_tiles = 0;  // the previous item: its factor, whether it was the last, the factor's items
+  auto pend_count = [&] { return pend_tiles; };
 
   while (true) {
     int next_item = 0x7fffffff;
@@ -252,72 +335,34 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
       const int we = min(wb + kSubMax, item_end);
       int nq = 0;  // warp-uniform queue length
       for (int i0 = wb; i0 < we; i0 += 32 * kLookupUnroll) {
-        int cx[kLookupUnroll], cy[kLookupUnroll], cz[kLookupUnroll];
-        uint32_t h[kLookupUnroll];
-        int4 b[kLookupUnroll], b1[kLookupUnroll];
+        Probe p[kLookupUnroll];
 #pragma unroll
         for (int u = 0; u < kLookupUnroll; u++) {
-          const int i = i0 + u * 32 + lane;
-          const float4 a0 = __ldg(&D.p0[min(i, we - 1)]);
-          float qx, qy, qz;
-          transform(P, a0.x, a0.y, a0.z, qx, qy, qz);
-          cx[u] = gb_coord(qx, D.inv_res); cy[u] = gb_coord(qy, D.inv_res); cz[u] = gb_coord(qz, D.inv_res);
-          h[u] = gb_hash(cx[u], cy[u], cz[u]);
-          b[u] = __ldg(&D.buckets[h[u] & D.mask]);
-          b1[u] = __ldg(&D.buckets[(h[u] + 1u) & D.mask]);
+          const float4 a0 = __ldg(&D.p0[min(i0 + u * 32 + lane, we - 1)]);
+          probe_issue(D, P, a0.x, a0.y, a0.z, p[u]);
         }
         if (!published) {  // the MEMBAR of the release overlaps with the loads above
           published = true;
           __syncwarp();
-          if (lane == 0) publish();
+          if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
         }
 #pragma unroll
-        for (int u = 0; u < kLookupUnroll; u++) {
-          const int i = i0 + u * 32 + lane;
-          int v = resolve_probe(D, b[u], b1[u], h[u], cx[u], cy[u], cz[u]);
-          if (i >= we) v = -1;
-          const unsigned m = __ballot_sync(0xffffffffu, v >= 0);
-          if (v >= 0) q[nq + __popc(m & lt_mask)] = make_uint2((unsigned)i, (unsigned)v);
-          nq += __popc(m);
-        }
+        for (int u = 0; u < kLookupUnroll; u++) probe_compact(D, p[u], i0 + u * 32 + lane, we, q, nq, lt_mask);
       }
       __syncwarp();
-#pragma unroll 2
-      for (int k = lane; k < nq; k += 32) {
-        const uint2 e = q[k];
-        const int i = (int)e.x;
-        const float4 a0 = __ldg(&D.p0[i]);
-        const float4 a1 = __ldg(&D.p1[i]);
-        const float a2 = __ldg(&D.p2[i]);
-        const float4 v0 = __ldg(&D.voxels[3 * (size_t)e.y + 0]);
-        const float4 v1 = __ldg(&D.voxels[3 * (size_t)e.y + 1]);
-        const float4 v2 = __ldg(&D.voxels[3 * (size_t)e.y + 2]);
-        // surface validation is a compile-time variant here (GLIM enables it for odometry factors only, which run sweep5)
-        if (!SV || D.normals == nullptr || surface_ok(P, __ldg(&D.normals[i]), v0.w, v1.x, v1.y, v1.z, v1.w, v2.x)) accumulate_hit<MODE>(acc, Pe, a0, a1, a2, v0, v1, v2);
-      }
+      // surface validation is a compile-time variant here (GLIM enables it for odometry factors only, which run sweep5)
+      accumulate_queue<MODE, SV>(acc, D, P, Pe, q, nq, lane);
       __syncwarp();  // the queue is overwritten by the next round
     }
     if (!published) {  // the item had no lookup group (empty factor)
       __syncwarp();
-      if (lane == 0) publish();
+      if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
     }
 
-    double* __restrict__ my_acc = accum + ((size_t)f * acc_slots + (size_t)(item & (acc_slots - 1))) * GB_ACC_STRIDE;
-    if (MODE == GB_MODE_LINEARIZE) {
-      const float r = warp_reduce_scatter32(acc, lane);
-      if (lane < 29) atomicAdd(&my_acc[lane], (double)r);
-    } else {
-      float e = acc[27], n = acc[28];
-#pragma unroll
-      for (int o = 16; o >= 1; o >>= 1) { e += __shfl_xor_sync(0xffffffffu, e, o); n += __shfl_xor_sync(0xffffffffu, n, o); }
-      if (lane == 27) atomicAdd(&my_acc[27], (double)e);
-      if (lane == 28) atomicAdd(&my_acc[28], (double)n);
-    }
+    reduce_item<MODE>(acc, accum, f, acc_slots, item, lane);
     if (pend_f >= 0 && __shfl_sync(0xffffffffu, pend_last, 0)) {  // the PREVIOUS item completed its factor
       fence_acquire();
-      const FactorDesc Dp = descs[pend_f];
-      factor_epilogue(pend_f, Dp, MODE == GB_MODE_ERROR ? poses_eval : poses, accum, acc_slots, out, slab, reinterpret_cast<double*>(q));
-      if (PEER && MODE == GB_MODE_LINEARIZE) pair_push(Dp, out, peer, reinterpret_cast<float*>(q) + 512);
+      retire_factor<MODE, PEER>(pend_f, desc_of(pend_f), poses, poses_eval, accum, acc_slots, out, slab, peer, q);
       __syncwarp();
     }
     pend_f = f; pend_tiles = D.num_tiles; pend_last = 0;
@@ -326,12 +371,10 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
     it = __ldg(&items[item]);
   }
   __syncwarp();
-  if (lane == 0) publish();
+  if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
   if (__shfl_sync(0xffffffffu, pend_last, 0)) {
     fence_acquire();
-    const FactorDesc Dp = descs[pend_f];
-    factor_epilogue(pend_f, Dp, MODE == GB_MODE_ERROR ? poses_eval : poses, accum, acc_slots, out, slab, reinterpret_cast<double*>(q));
-    if (PEER && MODE == GB_MODE_LINEARIZE) pair_push(Dp, out, peer, reinterpret_cast<float*>(q) + 512);
+    retire_factor<MODE, PEER>(pend_f, desc_of(pend_f), poses, poses_eval, accum, acc_slots, out, slab, peer, q);
   }
 }
 
@@ -347,7 +390,7 @@ struct CtaCache {
 // with the per-item latency chain cut and the one-wave regime balanced:
 //   * descriptor / fp32-pose cache in shared memory for small factor sets (an odometry graph), one-item look-ahead of the
 //     work queue, lazily published release tickets (atom.release: no __threadfence, no L1 flush per item);
-//   * STRIDED items for sweeps of about one item per warp (odometry, single pair): item j of a factor with J items owns
+//   * STRIDED items, about one per warp in a small sweep (odometry, single pair): item j of a factor with J items owns
 //     the 32-point rows j, j + J, j + 2J, ... of the source cloud, so every item of a factor samples the whole (Morton-
 //     ordered) cloud and sees the same inlier rate; the host sizes J per factor from the factor's last inlier fraction
 //     (a hit costs ~2.2x a miss).  One wave of equally expensive items instead of a tail of all-inlier items.
@@ -355,7 +398,7 @@ struct CtaCache {
 template <int MODE, bool PEER>
 __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
   const FactorDesc* __restrict__ descs, int num_factors, const double* __restrict__ poses, const double* __restrict__ poses_eval,
-  const int2* __restrict__ items, int num_items, int chunk, int strided,
+  const int2* __restrict__ items, int num_items,
   unsigned long long* __restrict__ item_ctr, unsigned long long ctr_base,
   double* __restrict__ accum, int acc_slots, unsigned* __restrict__ done, double* __restrict__ out, float* __restrict__ slab, const PeerPush* __restrict__ peer) {
   __shared__ __align__(16) uint2 s_q[kWarps][kSubMax];
@@ -378,12 +421,6 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
   }
   // descriptor reads keep their address space (LDS from the cache or LDG from the table)
   auto desc_of = [&](int f) -> FactorDesc { FactorDesc d; if (cached) d = cache->desc[f]; else d = descs[f]; return d; };
-  auto publish = [&](int pf) -> int {  // lane 0, after a __syncwarp
-    const unsigned t = ticket_release(&done[pf]);
-    const int last = (t == (unsigned)(cached ? cache->desc[pf].num_tiles : descs[pf].num_tiles) - 1u);
-    if (last) done[pf] = 0u;
-    return last;
-  };
 
   const int total_warps = gridDim.x * kWarps;
   const bool dynamic = num_items > total_warps;
@@ -396,6 +433,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
   }
   int2 it = __ldg(&items[item]);
   int pend_f = -1, pend_last = 0;
+  auto pend_count = [&] { return desc_of(pend_f).num_tiles; };
 
   while (true) {
     int nxt2 = 0x7fffffff;
@@ -409,14 +447,13 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
     PoseF Pe = P;
     if (MODE == GB_MODE_ERROR) { if (cached) Pe = cache->pose_eval[f]; else Pe = pose_from_colmajor(poses_eval + (size_t)f * 16); }
 
-    // the item's points: contiguous [it.y, it.y + chunk) or the rows it.y, it.y + J, ... (32 points each) of the cloud
-    const int limit = strided ? D.n : min(it.y + D.chunk, D.n);
-    (void)chunk;
-    const int row_stride = strided ? D.num_tiles * 32 : 32;
-    const int first = strided ? it.y * 32 : it.y;
+    // the item's points: the rows it.y, it.y + J, ... (32 points each) of the cloud, J = the factor's item count
+    const int limit = D.n;
+    const int row_stride = D.num_tiles * 32;
+    const int first = it.y * 32;
     int ngroups = 0;
     if (first < limit) {
-      const int rows = (limit - first + row_stride - 1) / row_stride;  // strided: ceil((R - j) / J); contiguous: ceil(len / 32)
+      const int rows = (limit - first + row_stride - 1) / row_stride;  // ceil((R - j) / J)
       ngroups = (rows + U - 1) / U;
     }
 
@@ -437,32 +474,16 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
         ax[u] = a0.x; ay[u] = a0.y; az[u] = a0.z;
       }
       for (int g = g0; g < g1; g++) {
-        int cx[U], cy[U], cz[U];
-        uint32_t h[U];
-        int4 b[U], b1[U];
+        Probe p[U];
 #pragma unroll
-        for (int u = 0; u < U; u++) {
-          float qx, qy, qz;
-          transform(P, ax[u], ay[u], az[u], qx, qy, qz);
-          cx[u] = gb_coord(qx, D.inv_res); cy[u] = gb_coord(qy, D.inv_res); cz[u] = gb_coord(qz, D.inv_res);
-          h[u] = gb_hash(cx[u], cy[u], cz[u]);
-          b[u] = __ldg(&D.buckets[h[u] & D.mask]);
-          b1[u] = __ldg(&D.buckets[(h[u] + 1u) & D.mask]);
-        }
+        for (int u = 0; u < U; u++) probe_issue(D, P, ax[u], ay[u], az[u], p[u]);
         if (!published) {  // the previous item's ticket: the MEMBAR of the release overlaps with the loads above
           published = true;
           __syncwarp();
-          if (lane == 0) pend_last = publish(pend_f);
+          if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
         }
 #pragma unroll
-        for (int u = 0; u < U; u++) {
-          const int i = first + (g * U + u) * row_stride + lane;
-          int v = resolve_probe(D, b[u], b1[u], h[u], cx[u], cy[u], cz[u]);
-          if (i >= limit) v = -1;
-          const unsigned m = __ballot_sync(0xffffffffu, v >= 0);
-          if (v >= 0) q[nq + __popc(m & lt_mask)] = make_uint2((unsigned)i, (unsigned)v);
-          nq += __popc(m);
-        }
+        for (int u = 0; u < U; u++) probe_compact(D, p[u], first + (g * U + u) * row_stride + lane, limit, q, nq, lt_mask);
         if (g + 1 < g1) {  // the next group's points, loaded after this group is resolved
 #pragma unroll
           for (int u = 0; u < U; u++) {
@@ -473,42 +494,19 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
         }
       }
       __syncwarp();
-      // ---------------- phase B ----------------
-#pragma unroll 2
-      for (int k = lane; k < nq; k += 32) {
-        const uint2 e = q[k];
-        const float4 a0 = __ldg(&D.p0[e.x]);
-        const float4 a1 = __ldg(&D.p1[e.x]);
-        const float a2 = __ldg(&D.p2[e.x]);
-        const float4 v0 = __ldg(&D.voxels[3 * (size_t)e.y + 0]);
-        const float4 v1 = __ldg(&D.voxels[3 * (size_t)e.y + 1]);
-        const float4 v2 = __ldg(&D.voxels[3 * (size_t)e.y + 2]);
-        if (D.normals == nullptr || surface_ok(P, __ldg(&D.normals[e.x]), v0.w, v1.x, v1.y, v1.z, v1.w, v2.x)) accumulate_hit<MODE>(acc, Pe, a0, a1, a2, v0, v1, v2);
-      }
+      accumulate_queue<MODE, true>(acc, D, P, Pe, q, nq, lane);
       __syncwarp();  // the queue is overwritten by the next round
     }
     if (!published) {  // empty item
       __syncwarp();
-      if (lane == 0) pend_last = publish(pend_f);
+      if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
     }
 
-    double* __restrict__ my_acc = accum + ((size_t)f * acc_slots + (size_t)(item & (acc_slots - 1))) * GB_ACC_STRIDE;
-    if (MODE == GB_MODE_LINEARIZE) {
-      const float r = warp_reduce_scatter32(acc, lane);
-      if (lane < 29) atomicAdd(&my_acc[lane], (double)r);
-    } else {
-      float e = acc[27], n = acc[28];
-#pragma unroll
-      for (int o = 16; o >= 1; o >>= 1) { e += __shfl_xor_sync(0xffffffffu, e, o); n += __shfl_xor_sync(0xffffffffu, n, o); }
-      if (lane == 27) atomicAdd(&my_acc[27], (double)e);
-      if (lane == 28) atomicAdd(&my_acc[28], (double)n);
-    }
+    reduce_item<MODE>(acc, accum, f, acc_slots, item, lane);
     // epilogue of the PREVIOUS item's factor, if that item was its last
     if (pend_f >= 0 && __shfl_sync(0xffffffffu, pend_last, 0)) {
       fence_acquire();
-      const FactorDesc Dp = desc_of(pend_f);
-      factor_epilogue(pend_f, Dp, MODE == GB_MODE_ERROR ? poses_eval : poses, accum, acc_slots, out, slab, reinterpret_cast<double*>(q));
-      if (PEER && MODE == GB_MODE_LINEARIZE) pair_push(Dp, out, peer, reinterpret_cast<float*>(q) + 2 * kEpilogueDoubles);
+      retire_factor<MODE, PEER>(pend_f, desc_of(pend_f), poses, poses_eval, accum, acc_slots, out, slab, peer, q);
       __syncwarp();
     }
     pend_f = f;
@@ -519,12 +517,10 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
     if (item >= num_items) break;
   }
   __syncwarp();
-  if (lane == 0) pend_last = publish(pend_f);
+  if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
   if (__shfl_sync(0xffffffffu, pend_last, 0)) {
     fence_acquire();
-    const FactorDesc Dp = desc_of(pend_f);
-    factor_epilogue(pend_f, Dp, MODE == GB_MODE_ERROR ? poses_eval : poses, accum, acc_slots, out, slab, reinterpret_cast<double*>(q));
-    if (PEER && MODE == GB_MODE_LINEARIZE) pair_push(Dp, out, peer, reinterpret_cast<float*>(q) + 2 * kEpilogueDoubles);
+    retire_factor<MODE, PEER>(pend_f, desc_of(pend_f), poses, poses_eval, accum, acc_slots, out, slab, peer, q);
   }
 }
 
@@ -564,13 +560,13 @@ __global__ void __launch_bounds__(256) k_overlap(int num_targets, const FactorDe
 // ---------------------------------------------------------------------------------------------
 template <int MODE, bool PEER>
 static cudaError_t launch5(gb_sweep* s, const double* poses_eval, float* slab, const PeerPush* pp) {
-  k_vgicp_sweep5<MODE, PEER><<<s->grid, kThreads, 0, s->ctx->stream>>>(s->d_descs, (int)s->F, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->tile_size, s->strided, s->d_tile_ctr, s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
+  k_vgicp_sweep5<MODE, PEER><<<s->grid, kThreads, 0, s->ctx->stream>>>(s->d_descs, (int)s->F, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr, s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
   return cudaGetLastError();
 }
 
 template <int MODE, bool PEER, bool SV>
 static cudaError_t launch3(gb_sweep* s, const double* poses_eval, float* slab, const PeerPush* pp) {
-  k_vgicp_sweep3<MODE, PEER, SV><<<s->grid, kThreads, 0, s->ctx->stream>>>(s->d_descs, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->tile_size, s->d_tile_ctr, s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
+  k_vgicp_sweep3<MODE, PEER, SV><<<s->grid, kThreads, 0, s->ctx->stream>>>(s->d_descs, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr, s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
   return cudaGetLastError();
 }
 

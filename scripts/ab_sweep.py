@@ -16,9 +16,8 @@ CONFIGS = [
     ("v3", {"GB_KERNEL": "3"}),
     ("auto", {}),
     ("v5", {"GB_KERNEL": "5"}),
-    ("v5 nostride", {"GB_KERNEL": "5", "GB_STRIDED": "0"}),
 ]
-KEYS = ["GB_KERNEL", "GB_STRIDED"]
+KEYS = ["GB_KERNEL"]
 
 
 def main():

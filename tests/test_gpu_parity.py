@@ -390,26 +390,22 @@ def test_nan_points_and_singular_covariances_match_oracle(ctx, dev, pair):
 
 
 def test_kernel_generations_agree(ctx, dev, monkeypatch):
-    """k_vgicp_sweep3 (large sweeps) and k_vgicp_sweep5 (small sweeps, strided and contiguous items) on the same factor set:
-    identical inlier counts, blocks equal to fp32 summation-order noise."""
+    """k_vgicp_sweep3 (large sweeps, contiguous items) and k_vgicp_sweep5 (small sweeps, strided items) on the same factor
+    set: identical inlier counts, blocks equal to fp32 summation-order noise."""
     maps0 = [gpu.GaussianVoxelMapGPU(r, ctx=ctx).insert(dev["cloud"][0]) for r in (0.25, 0.5)]
     T = dev["T_gt"]
     outs = {}
-    for name, env in (("v3", {"GB_KERNEL": "3"}), ("v5", {"GB_KERNEL": "5"}), ("v5_contiguous", {"GB_KERNEL": "5", "GB_STRIDED": "0"})):
-        for k in ("GB_KERNEL", "GB_STRIDED"):
-            monkeypatch.delenv(k, raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, v)
+    for name, kernel in (("v3", "3"), ("v5", "5")):
+        monkeypatch.setenv("GB_KERNEL", kernel)
         facs = [gpu.IntegratedVGICPFactorGPU(0, 1, m, dev["cloud"][1], ctx=ctx) for m in maps0]
         fs = gpu.NonlinearFactorSetGPU(ctx).add(facs)
         outs[name] = fs.linearize_deltas(np.stack([T, T]))
         e = fs.error_deltas(np.stack([T, T]), np.stack([T, T]))
         assert np.allclose(e, outs[name]["error"], rtol=1e-5)
-    for name in ("v5", "v5_contiguous"):
-        for i in range(2):
-            assert outs[name][i]["num_inliers"] == outs["v3"][i]["num_inliers"]
-            for k in ("H_tt", "H_ss", "H_ts"):
-                assert util.rel_err(outs[name][i][k], outs["v3"][i][k]) < 1e-5, (name, k)
+    for i in range(2):
+        assert outs["v5"][i]["num_inliers"] == outs["v3"][i]["num_inliers"]
+        for k in ("H_tt", "H_ss", "H_ts"):
+            assert util.rel_err(outs["v5"][i][k], outs["v3"][i][k]) < 1e-5, k
 
 
 def test_large_sweep_matches_oracle(ctx):
@@ -464,21 +460,22 @@ def _oracle_check_factors(ctx, w, fset, picks, tol=REL_TOL):
     return sw, rec, worst
 
 
-@pytest.mark.parametrize("strided", ["1", "0"])
-def test_global_mapping_factors_match_oracle(ctx, monkeypatch, strided):
-    """M4 data distribution at full submap size (50 k points, 0.5 / 1.0 m voxels, ~35 % inliers) on a short loop.  strided=0:
-    the batched sweep runs through the dynamic item queue (items > warps) and replicated accumulators; strided=1 (what a
-    sweep of this size gets by default): one wave of strided items, re-sized after the first fetch.  Picked factors vs the oracle."""
+@pytest.mark.parametrize("kernel", ["auto", "3"])
+def test_global_mapping_factors_match_oracle(ctx, monkeypatch, kernel):
+    """M4 data distribution at full submap size (50 k points, 0.5 / 1.0 m voxels, ~35 % inliers) on a short loop.  kernel=3:
+    the batched sweep runs sweep3 through the dynamic item queue (items > warps) and replicated accumulators; kernel=auto
+    (sweep5, what a sweep of this size gets by default): one wave of strided items, re-sized after the first fetch.  Picked
+    factors vs the oracle."""
     from glim_b200 import workloads
 
-    monkeypatch.setenv("GB_STRIDED", strided)
+    monkeypatch.setenv("GB_KERNEL", kernel)
     w = workloads.global_mapping(ctx, n_submaps=12, laps=1, side=60.0, use_gpu=True)
     fset = w.sets[0]
     assert len(fset.factors) >= 10 and min(len(c[0]) for c in w.host_clouds) == 50000
     rng = np.random.default_rng(5)
     picks = sorted(rng.choice(len(fset.factors), 6, replace=False).tolist())
     sw, rec, worst = _oracle_check_factors(ctx, w, fset, picks)
-    if strided == "0":
+    if kernel == "3":
         assert sw.num_tiles > sw.grid * 8  # the queue path
     else:
         assert sw.num_tiles <= sw.grid * 8  # one wave
