@@ -116,8 +116,7 @@ extern "C" gb_status gb_vgicp_align(gb_ctx* ctx, size_t P, const size_t* off, gb
   GB_REQUIRE(results, "null results");
   GB_CHECK(validate(P, off, factors, T_init, prm));
   const size_t F = off[P];
-  GB_LOCK(ctx);
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   gb_sweep* s = nullptr;
   GB_CHECK(gb_sweep_create(ctx, F, factors, nullptr, &s));
   gb_status st = GB_OK;
@@ -152,13 +151,9 @@ extern "C" gb_status gb_vgicp_align(gb_ctx* ctx, size_t P, const size_t* off, gb
   bool need_lin = true;
   for (;;) {
     if (need_lin && (st = gb_launch_sweep(s, GB_MODE_LINEARIZE)) != GB_OK) return finish(st);
-    k_align_step<<<grid, kAlignThreads, 0, stream>>>(d_st, d_off, (int)P, s->d_out, s->d_poses_eval, d_ctr);
-    if ((e = cudaGetLastError()) != cudaSuccess) { gb_set_error("k_align_step: %s", cudaGetErrorString(e)); return finish(GB_ERR_CUDA); }
-    ctx->launches++;
+    if ((st = gb_launch(ctx, "k_align_step", k_align_step, grid, kAlignThreads, 0, d_st, d_off, (int)P, s->d_out, s->d_poses_eval, d_ctr)) != GB_OK) return finish(st);
     if ((st = gb_launch_sweep(s, GB_MODE_ERROR)) != GB_OK) return finish(st);
-    k_align_accept<<<grid, kAlignThreads, 0, stream>>>(d_st, d_off, (int)P, s->d_out, s->d_poses, *prm, d_ctr);
-    if ((e = cudaGetLastError()) != cudaSuccess) { gb_set_error("k_align_accept: %s", cudaGetErrorString(e)); return finish(GB_ERR_CUDA); }
-    ctx->launches++;
+    if ((st = gb_launch(ctx, "k_align_accept", k_align_accept, grid, kAlignThreads, 0, d_st, d_off, (int)P, s->d_out, s->d_poses, *prm, d_ctr)) != GB_OK) return finish(st);
     e = cudaMemcpyAsync((void*)h_ctr, d_ctr, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
     if (e != cudaSuccess) { gb_set_error("align round: %s", cudaGetErrorString(e)); return finish(GB_ERR_CUDA); }

@@ -189,6 +189,7 @@ extern "C" gb_status gb_ctx_destroy(gb_ctx* ctx) {
 }
 extern "C" gb_status gb_ctx_synchronize(gb_ctx* ctx) {
   GB_REQUIRE(ctx, "null ctx");
+  GB_ENTER(ctx);
   GB_CUDA(cudaStreamSynchronize(ctx->stream));
   return GB_OK;
 }
@@ -279,7 +280,7 @@ extern "C" gb_status gb_cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, 
   GB_REQUIRE(n == 0 || xyzw, "null points");
   GB_REQUIRE(n < (size_t)1 << 30, "too many points");
   *out = nullptr;
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   gb_cloud* c = new (std::nothrow) gb_cloud();
   if (!c) return GB_ERR_INTERNAL;
   c->device = ctx->device;
@@ -336,7 +337,7 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
   GB_REQUIRE(init_num_buckets > 0 && (init_num_buckets & (init_num_buckets - 1)) == 0, "init_num_buckets must be a power of two");
   GB_REQUIRE(max_bucket_scan_count > 0, "max_bucket_scan_count must be positive");
   *out = nullptr;
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   gb_voxelmap* m = new (std::nothrow) gb_voxelmap();
   if (!m) return GB_ERR_INTERNAL;
   gb_status st = gb_voxelmap_build_impl(ctx, cloud, resolution, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, m);
@@ -357,8 +358,7 @@ extern "C" gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolutio
   GB_REQUIRE(max_bucket_scan_count > 0, "max_bucket_scan_count must be positive");
   GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
   *out = nullptr;
-  GB_LOCK(ctx);
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   gb_voxelmap* m = new (std::nothrow) gb_voxelmap();
   if (!m) return GB_ERR_INTERNAL;
   m->resolution = resolution;
@@ -386,8 +386,7 @@ extern "C" gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_
   const double* T = T_map_cloud ? T_map_cloud : kIdentity;
   for (int k = 0; k < 16; k++) GB_REQUIRE(std::isfinite(T[k]), "T_map_cloud must be finite");
   GB_REQUIRE((uint64_t)map->num_voxels + (uint64_t)cloud->n < (1ull << 31) - 1, "map voxels + cloud points exceed 2^31");
-  GB_LOCK(ctx);
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   return gb_voxelmap_insert_impl(ctx, map, cloud, T, sampling_rate, (unsigned long long)seed);
 }
 extern "C" gb_status gb_voxelmap_info(const gb_voxelmap* m, int* num_voxels, int* num_buckets, float* resolution) {
@@ -657,8 +656,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     GB_REQUIRE(factors[f]->source->device == ctx->device && factors[f]->target->device == ctx->device, "factor lives on another device");
     total_pts += factors[f]->source->n;
   }
-  GB_LOCK(ctx);
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   gb_sweep* s = new (std::nothrow) gb_sweep();
   if (!s) return GB_ERR_INTERNAL;
   ctx_retain(ctx);
@@ -775,7 +773,7 @@ extern "C" gb_status gb_sweep_attach_slab(gb_sweep* s, void* device_slab_f32, si
 extern "C" gb_status gb_sweep_set_poses(gb_sweep* s, const double* T) {
   GB_REQUIRE(s && (s->F == 0 || T), "null argument");
   if (s->F == 0) return GB_OK;
-  GB_LOCK(s->ctx);
+  GB_ENTER(s->ctx);
   // double-buffered pinned staging: wait only for the H2D that read THIS slot two calls ago (normally long finished)
   const int k = s->pose_slot;
   s->pose_slot ^= 1;
@@ -794,19 +792,18 @@ static gb_status sweep_set_eval_poses(gb_sweep* s, const double* T) {
 }
 static gb_status sweep_launch(gb_sweep* s, int mode) {
   if (s->stale) { gb_set_error("a factor of this sweep has been destroyed"); return GB_ERR_INVALID_ARGUMENT; }
-  GB_CUDA(cudaSetDevice(s->ctx->device));
   GB_CHECK(sweep_follow_targets(s));
   return gb_launch_sweep(s, mode);
 }
 extern "C" gb_status gb_sweep_launch(gb_sweep* s) {
   GB_REQUIRE(s, "null sweep");
-  GB_LOCK(s->ctx);
+  GB_ENTER(s->ctx);
   return sweep_launch(s, GB_MODE_LINEARIZE);
 }
 extern "C" gb_status gb_sweep_fetch(gb_sweep* s, gb_linearized6* out) {
   GB_REQUIRE(s && (s->F == 0 || out), "null argument");
   if (s->F == 0) return GB_OK;
-  GB_LOCK(s->ctx);
+  GB_ENTER(s->ctx);
   static_assert(sizeof(gb_linearized6) == sizeof(double) * GB_OUT_DOUBLES, "gb_linearized6 layout");
   GB_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(double) * GB_OUT_DOUBLES * s->F, cudaMemcpyDeviceToHost, s->ctx->stream));
   GB_CUDA(cudaStreamSynchronize(s->ctx->stream));
@@ -864,7 +861,6 @@ static gb_status sweep_linearize(gb_sweep* s, const double* T, gb_linearized6* o
   }
   if (s->stale) { gb_set_error("a factor of this sweep has been destroyed"); return GB_ERR_INVALID_ARGUMENT; }
   gb_ctx* ctx = s->ctx;
-  GB_CUDA(cudaSetDevice(ctx->device));
   GB_CHECK(sweep_follow_targets(s));  // the graph's kernel reads the descriptors from HBM
   cudaStream_t st = ctx->stream;
   const size_t pose_bytes = sizeof(double) * 16 * s->F, out_bytes = sizeof(double) * GB_OUT_DOUBLES * s->F;
@@ -902,7 +898,7 @@ static gb_status sweep_linearize(gb_sweep* s, const double* T, gb_linearized6* o
 extern "C" gb_status gb_sweep_linearize(gb_sweep* s, const double* T, gb_linearized6* out) {
   GB_REQUIRE(s && (s->F == 0 || (T && out)), "null argument");
   if (s->F == 0) return GB_OK;
-  GB_LOCK(s->ctx);
+  GB_ENTER(s->ctx);
   return sweep_linearize(s, T, out);
 }
 
@@ -910,7 +906,7 @@ extern "C" gb_status gb_factor_set_linearize(gb_ctx* ctx, size_t F, gb_factor* c
   GB_REQUIRE(ctx, "null ctx");
   if (F == 0) return GB_OK;
   GB_REQUIRE(factors && T && out, "null argument");
-  GB_LOCK(ctx);
+  GB_ENTER(ctx);
   gb_sweep* s = nullptr;
   GB_CHECK(cached_sweep(ctx, F, factors, &s));
   return sweep_linearize(s, T, out);
@@ -920,7 +916,7 @@ extern "C" gb_status gb_factor_set_error(gb_ctx* ctx, size_t F, gb_factor* const
   GB_REQUIRE(ctx, "null ctx");
   if (F == 0) return GB_OK;
   GB_REQUIRE(factors && T_lin && T_eval && errors, "null argument");
-  GB_LOCK(ctx);
+  GB_ENTER(ctx);
   gb_sweep* s = nullptr;
   GB_CHECK(cached_sweep(ctx, F, factors, &s));
   GB_CHECK(gb_sweep_set_poses(s, T_lin));
@@ -939,14 +935,14 @@ static gb_status single_sweep(gb_factor* f, gb_sweep** out) {
 }
 extern "C" gb_status gb_vgicp_linearize(gb_factor* f, const double T[16], gb_linearized6* out) {
   GB_REQUIRE(f && T && out, "null argument");
-  GB_LOCK(f->ctx);
+  GB_ENTER(f->ctx);
   gb_sweep* s = nullptr;
   GB_CHECK(single_sweep(f, &s));
   return sweep_linearize(s, T, out);
 }
 extern "C" gb_status gb_vgicp_error(gb_factor* f, const double T_lin[16], const double T_eval[16], double* error) {
   GB_REQUIRE(f && T_lin && T_eval && error, "null argument");
-  GB_LOCK(f->ctx);
+  GB_ENTER(f->ctx);
   gb_sweep* s = nullptr;
   GB_CHECK(single_sweep(f, &s));
   GB_CHECK(gb_sweep_set_poses(s, T_lin));
@@ -1004,7 +1000,7 @@ extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int worl
   GB_REQUIRE(world >= 1 && world <= GB_MAX_PEERS && rank >= 0 && rank < world, "world must be 1..8 and rank < world");
   GB_REQUIRE(num_pairs > 0, "num_pairs must be positive");
   *out = nullptr;
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   gb_peer_slab* ps = new (std::nothrow) gb_peer_slab();
   if (!ps) return GB_ERR_INTERNAL;
   ps->ctx = ctx; ps->num_pairs = num_pairs; ps->world = world; ps->rank = rank;
@@ -1037,6 +1033,7 @@ extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int worl
 extern "C" gb_status gb_peer_slab_export(gb_peer_slab* ps, void* handle) {
   GB_REQUIRE(ps && handle, "null argument");
   static_assert(sizeof(cudaIpcMemHandle_t) == GB_IPC_HANDLE_BYTES, "IPC handle size");
+  GB_ENTER(ps->ctx);
   cudaIpcMemHandle_t h;
   GB_CUDA(cudaIpcGetMemHandle(&h, ps->local));
   memcpy(handle, &h, sizeof(h));
@@ -1045,7 +1042,7 @@ extern "C" gb_status gb_peer_slab_export(gb_peer_slab* ps, void* handle) {
 
 extern "C" gb_status gb_peer_slab_connect(gb_peer_slab* ps, const void* handles) {
   GB_REQUIRE(ps && handles, "null argument");
-  GB_CUDA(cudaSetDevice(ps->ctx->device));
+  GB_ENTER(ps->ctx);
   for (int p = 0; p < ps->world; p++) {
     if (p == ps->rank || ps->opened[p]) continue;
     cudaIpcMemHandle_t h;
@@ -1061,16 +1058,18 @@ extern "C" gb_status gb_peer_slab_connect(gb_peer_slab* ps, const void* handles)
 
 extern "C" gb_status gb_peer_slab_destroy(gb_peer_slab* ps) {
   if (!ps) return GB_OK;
-  cudaSetDevice(ps->ctx->device);
-  cudaStreamSynchronize(ps->ctx->stream);
-  for (int p = 0; p < ps->world; p++)
-    if (ps->opened[p]) cudaIpcCloseMemHandle(ps->peer[p]);
-  if (ps->local) cudaFree(ps->local);
-  if (ps->d_my_pairs) cudaFree(ps->d_my_pairs);
-  if (ps->h_pinned) cudaFreeHost(ps->h_pinned);
   gb_ctx* ctx = ps->ctx;
-  delete ps;
-  ctx_release(ctx);
+  {
+    GB_ENTER(ctx);
+    cudaStreamSynchronize(ctx->stream);
+    for (int p = 0; p < ps->world; p++)
+      if (ps->opened[p]) cudaIpcCloseMemHandle(ps->peer[p]);
+    if (ps->local) cudaFree(ps->local);
+    if (ps->d_my_pairs) cudaFree(ps->d_my_pairs);
+    if (ps->h_pinned) cudaFreeHost(ps->h_pinned);
+    delete ps;
+  }
+  ctx_release(ctx);  // outside the lock: it may delete the context
   return GB_OK;
 }
 
@@ -1089,7 +1088,7 @@ extern "C" gb_status gb_sweep_attach_peer_slab(gb_sweep* s, gb_peer_slab* ps) {
   for (size_t k = 0; k < P; k++) ptr[k + 1] += ptr[k];
   std::vector<int> fill(ptr.begin(), ptr.end() - 1);
   for (size_t f = 0; f < s->F; f++) fac[fill[s->h_pair[f]]++] = (int)f;
-  GB_CUDA(cudaSetDevice(s->ctx->device));
+  GB_ENTER(s->ctx);
   GB_CUDA(cudaStreamSynchronize(s->ctx->stream));
   if (s->d_pair_ptr) { GB_CUDA(cudaFree(s->d_pair_ptr)); s->d_pair_ptr = nullptr; }
   const size_t b_ptr = align_up(sizeof(int) * (P + 1), 256), b_fac = align_up(sizeof(int) * std::max<size_t>(1, s->F), 256), b_done = align_up(sizeof(unsigned) * P, 256);
@@ -1129,7 +1128,7 @@ extern "C" gb_status gb_sweep_attach_peer_slab(gb_sweep* s, gb_peer_slab* ps) {
 extern "C" gb_status gb_peer_slab_signal_wait(gb_peer_slab* ps) {
   GB_REQUIRE(ps, "null peer slab");
   GB_REQUIRE(ps->connected, "gb_peer_slab_connect has not been called");
-  GB_CUDA(cudaSetDevice(ps->ctx->device));
+  GB_ENTER(ps->ctx);
   ps->step++;
   GB_CHECK(gb_launch_peer_signal_wait(ps));
   ps->completed_parity = ps->parity;
@@ -1145,6 +1144,7 @@ extern "C" gb_status gb_peer_slab_device_ptr(gb_peer_slab* ps, void** device_ptr
 
 extern "C" gb_status gb_peer_slab_fetch_async(gb_peer_slab* ps, const float** host_ptr) {
   GB_REQUIRE(ps, "null peer slab");
+  GB_ENTER(ps->ctx);
   const size_t bytes = ps->num_pairs * GB_SLAB_STRIDE * sizeof(float);
   GB_CUDA(cudaMemcpyAsync(ps->h_pinned, ps->local + (size_t)ps->completed_parity * ps->buf_floats * sizeof(float), bytes, cudaMemcpyDeviceToHost, ps->ctx->stream));
   GB_CUDA(cudaMemcpyAsync((char*)ps->h_pinned + bytes, ps->d_timeout, sizeof(int), cudaMemcpyDeviceToHost, ps->ctx->stream));
@@ -1154,6 +1154,7 @@ extern "C" gb_status gb_peer_slab_fetch_async(gb_peer_slab* ps, const float** ho
 
 extern "C" gb_status gb_peer_slab_fetch(gb_peer_slab* ps, float* host) {
   GB_REQUIRE(ps && host, "null argument");
+  GB_ENTER(ps->ctx);
   const size_t bytes = ps->num_pairs * GB_SLAB_STRIDE * sizeof(float);
   GB_CHECK(gb_peer_slab_fetch_async(ps, nullptr));
   GB_CUDA(cudaStreamSynchronize(ps->ctx->stream));
@@ -1172,7 +1173,7 @@ extern "C" gb_status gb_overlap(gb_ctx* ctx, size_t T, const gb_voxelmap* const*
   *overlap = 0.0;
   if (T == 0 || source->n == 0) return GB_OK;
   GB_REQUIRE(targets && deltas, "null targets / deltas");
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   const size_t b_desc = align_up(sizeof(FactorDesc) * T, 256), b_pose = align_up(sizeof(double) * 16 * T, 256);
   char* h = nullptr;
   char* d = nullptr;
@@ -1215,7 +1216,7 @@ extern "C" gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, c
       const int32_t q = neighbors[i * (size_t)k_correspondences + j];
       GB_REQUIRE(q >= 0 && (size_t)q < n, "neighbour index out of range [0, n)");
     }
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   return gb_covariances_impl(ctx, n, xyzw, neighbors, k_correspondences, k_neighbors, normals4, cov4x4);
 }
 extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors) {
@@ -1223,8 +1224,7 @@ extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n, const double* xyzw
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw && neighbors && k > 0, "null argument");
   GB_REQUIRE(gb_knn_instantiated(k), "k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
-  GB_LOCK(ctx);
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   // >= 4096 points: exact search on a pyramid of hash grids (one Morton sort, cell size 0.25 m x 4^level); fewer: the tiled
   // brute force.  GB_KNN=pyramid / brute forces one.
   const char* mode = getenv("GB_KNN");
@@ -1246,8 +1246,7 @@ extern "C" gb_status gb_merge_frames(gb_ctx* ctx, size_t K, const gb_cloud* cons
     total += frames[k]->n;
   }
   GB_REQUIRE(total < (size_t)1 << 30 && K < 65536, "too many points / frames");
-  GB_LOCK(ctx);
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   gb_cloud* c = nullptr;
   if (out_cloud) {
     c = new (std::nothrow) gb_cloud();
@@ -1291,8 +1290,7 @@ extern "C" gb_status gb_preprocess(gb_ctx* ctx, size_t n, const double* xyzw, co
   GB_REQUIRE(P->crop_bbox_frame >= 0 && P->crop_bbox_frame <= 2, "crop_bbox_frame must be 0 (off), 1 (lidar) or 2 (imu)");
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw, "null points");
-  GB_LOCK(ctx);
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   gb_cloud* c = nullptr;
   if (P->estimate_covariances) {
     c = new (std::nothrow) gb_cloud();
@@ -1313,6 +1311,6 @@ extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* 
   *num_out = 0;
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw && out_xyzw && resolution > 0.0, "null argument");
-  GB_CUDA(cudaSetDevice(ctx->device));
+  GB_ENTER(ctx);
   return gb_voxelgrid_sampling_impl(ctx, n, xyzw, times, intensities, resolution, out_xyzw, out_times, out_intensities, num_out);
 }

@@ -173,7 +173,6 @@ extern "C" gb_status gb_deskew(gb_ctx* ctx, const double T_imu_lidar[16], const 
   GB_REQUIRE(ctx, "null ctx");
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw && out_xyzw && times, "null argument");
-  GB_CUDA(cudaSetDevice(ctx->device));
   std::vector<int32_t> idx(n);
   std::vector<double> table(16 * n > 16 * 4096 ? 16 * 4096 : 16 * n);
   // the table has at most (t_max - t_min) / 1e-4 + 1 entries; size it for the worst case of this scan
@@ -185,6 +184,7 @@ extern "C" gb_status gb_deskew(gb_ctx* ctx, const double T_imu_lidar[16], const 
   table.resize(16 * worst);
   size_t m = 0;
   GB_CHECK(gb_deskew_pose_table(T_imu_lidar, linear_vel, angular_vel, n_imu, imu_times, imu_poses, stamp, n, times, idx.data(), table.data(), &m));
+  GB_ENTER(ctx);
   cudaStream_t st = ctx->stream;
   double4 *d_pts, *d_out;
   int* d_idx;
@@ -200,9 +200,7 @@ extern "C" gb_status gb_deskew(gb_ctx* ctx, const double T_imu_lidar[16], const 
   GB_CUDA(cudaMemcpyAsync(d_idx, idx.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(d_tab, table.data(), sizeof(double) * 16 * m, cudaMemcpyHostToDevice, st));
   if (T_post) GB_CUDA(cudaMemcpyAsync(d_post, T_post, sizeof(double) * 16, cudaMemcpyHostToDevice, st));
-  k_deskew<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((int)n, d_pts, d_idx, d_tab, d_post, d_out);
-  GB_CUDA(cudaGetLastError());
-  ctx->launches++;
+  GB_CHECK(gb_launch(ctx, "k_deskew", k_deskew, (unsigned)((n + 255) / 256), 256, 0, (int)n, d_pts, d_idx, d_tab, d_post, d_out));
   GB_CUDA(cudaMemcpyAsync(out_xyzw, d_out, sizeof(double4) * n, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));  // idx / table are locals; out_xyzw is the caller's
   return GB_OK;

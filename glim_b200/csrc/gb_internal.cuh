@@ -6,6 +6,7 @@
 #include <atomic>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/glim_b200.h"
@@ -204,15 +205,47 @@ struct gb_ctx {
   size_t scratch_cap = 0;
   void* pinned = nullptr;
   size_t pinned_cap = 0;
-  uint64_t launches = 0;
+  uint64_t launches = 0;     // gb_ctx_kernel_launches: written by gb_launch, GB_CUB and the graph path of sweep_linearize only
   std::atomic<int> refs{0};  // owner + live factors / sweeps / peer slabs; the context is torn down when the last one lets go
   std::vector<gb_sweep*> sweep_cache;
   std::vector<gb_pool_block> pool;  // device + pinned blocks of retired sweeps, reused by the next gb_sweep_create
   // A context may be driven from more than one host thread (a frame cloned by the odometry thread is later used by the
-  // sub-mapping thread): every entry point that touches the stream, the scratch arena or the caches takes this lock.
+  // sub-mapping thread): every entry point that touches the stream, the scratch arena, the caches or the launch counter
+  // enters through GB_ENTER, which takes this lock.  Recursive: an entry point may call another (gb_vgicp_align creates a
+  // sweep).  No entry point holds the locks of two contexts.
   std::recursive_mutex mu;
 };
 #define GB_LOCK(ctx) std::lock_guard<std::recursive_mutex> gb_lock__((ctx)->mu)
+// The first statement of an entry point after its argument checks: the context's lock for the rest of the call, and the
+// context's device as the thread's current device.
+#define GB_ENTER(ctx) \
+  GB_LOCK(ctx);       \
+  GB_CUDA(cudaSetDevice((ctx)->device))
+
+// Every kernel launch of the library: kernel<<<grid, block, smem, ctx->stream>>>(args...), its launch error read at once
+// (an invalid configuration or a missing image is reported by the call that made it, naming the kernel) and, on success,
+// one count in ctx->launches.  The triple-chevron launch converts each argument to the kernel's parameter type, as a
+// direct launch would.
+template <typename... P, typename... A>
+gb_status gb_launch(gb_ctx* ctx, const char* name, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+  kernel<<<grid, block, smem, ctx->stream>>>(std::forward<A>(args)...);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    gb_set_error("launch of %s failed: %s", name, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? GB_ERR_OUT_OF_MEMORY : GB_ERR_CUDA;
+  }
+  ctx->launches++;
+  return GB_OK;
+}
+// Every cub device-wide call of the library with temporary storage: fn(storage, bytes, args..., ctx->stream), counted as
+// one launch (a radix sort is several kernels; the counter's unit is the call).  The size queries of gb_cub_temp_bytes
+// launch nothing and do not come here.
+#define GB_CUB(ctx, fn, storage, bytes, ...)                         \
+  do {                                                               \
+    size_t cub_bytes__ = (bytes);                                    \
+    GB_CUDA(fn(storage, cub_bytes__, __VA_ARGS__, (ctx)->stream));   \
+    (ctx)->launches++;                                               \
+  } while (0)
 
 // Device blocks of clouds / voxel maps come from a process-wide pool (a frame costs one cloud + two maps = five allocations;
 // cudaMalloc / cudaFree are 50-200 us each and cudaFree synchronises the device).  gb_dev_free waits for the streams of
@@ -272,9 +305,9 @@ inline gb_sort_tmp gb_take_sort_tmp(Carver& cv, size_t n, void* cub, size_t cub_
 // caller writes one packed key per point (~0 = no voxel) and idx[i] = i; gb_group_by_key sorts the pairs into keys_s /
 // idx_s, flags the first slot of every voxel and scans the flags: pos[s] = number of voxels up to sorted slot s, so
 // pos[n - 1] is the voxel count.  gb_group_starts then writes starts[v] = first sorted slot of voxel v and
-// starts[V] = number of valid points.  Each counts its own launches.
+// starts[V] = number of valid points.
 gb_status gb_group_by_key(gb_ctx* ctx, int n, const gb_sort_tmp& t, int* flags, int* pos);
-void gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* flags, const int* pos, int* starts);
+gb_status gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* flags, const int* pos, int* starts);
 
 // Device cloud construction.  gb_cloud_planes lays out the planes of n points (p0, p1, p2, optional normals) at the
 // carver's position; the planes staged in the caller's point order use the same layout as the cloud's own.
@@ -311,7 +344,7 @@ gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* c
 gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T_colmajor, void* d_frame, double4* pts, double* cov6);
 // k_grid_keys of the voxel-grid paths: key = packed floor(p * inv_res) in fp64 (~0 for non-finite / out-of-range points),
 // idx[i] = i.  One launch.
-void gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx);
+gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx);
 gb_status gb_covariances_impl(gb_ctx* ctx, size_t n, const double* xyzw, const int32_t* neighbors, int kc, int k, double* normals4, double* cov4x4);
 gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out, gb_cloud* cloud_out);
 gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out);

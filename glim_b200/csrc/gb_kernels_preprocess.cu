@@ -131,15 +131,14 @@ __global__ void k_grid_means_counted(const int* __restrict__ num_voxels, const i
 
 }  // namespace
 
-void gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx) {
-  k_grid_keys<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, pts, inv_res, keys, idx);
-  ctx->launches++;
+gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx) {
+  return gb_launch(ctx, "k_grid_keys", k_grid_keys, (n + 255) / 256, 256, 0, n, pts, inv_res, keys, idx);
 }
 
-// Calls launch(std::integral_constant<int, K>()) for the instantiated neighbour counts K of the k-NN kernels.
+// Returns launch(std::integral_constant<int, K>()) for the instantiated neighbour counts K of the k-NN kernels.
 template <typename Launch> static gb_status knn_dispatch(int k, Launch&& launch) {
   switch (k) {
-#define GB_KNN_CASE(K) case K: launch(std::integral_constant<int, K>()); return GB_OK;
+#define GB_KNN_CASE(K) case K: return launch(std::integral_constant<int, K>());
     GB_KNN_CASE(1) GB_KNN_CASE(2) GB_KNN_CASE(3) GB_KNN_CASE(4) GB_KNN_CASE(5) GB_KNN_CASE(6) GB_KNN_CASE(7) GB_KNN_CASE(8)
     GB_KNN_CASE(9) GB_KNN_CASE(10) GB_KNN_CASE(12) GB_KNN_CASE(15) GB_KNN_CASE(16) GB_KNN_CASE(20) GB_KNN_CASE(24) GB_KNN_CASE(32)
 #undef GB_KNN_CASE
@@ -148,7 +147,7 @@ template <typename Launch> static gb_status knn_dispatch(int k, Launch&& launch)
   return GB_ERR_INVALID_ARGUMENT;
 }
 bool gb_knn_instantiated(int k) {
-  return knn_dispatch(k, [](auto) {}) == GB_OK;
+  return knn_dispatch(k, [](auto) { return GB_OK; }) == GB_OK;
 }
 
 size_t gb_cub_temp_bytes(size_t n_) {
@@ -172,9 +171,7 @@ gb_status gb_find_neighbors_impl(gb_ctx* ctx, size_t n_, const double* xyzw, int
     d_nb = cv.take<int>((size_t)n * k);
   }));
   GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * (size_t)n, cudaMemcpyHostToDevice, st));
-  GB_CHECK(knn_dispatch(k, [&](auto K) { k_knn_bruteforce<decltype(K)::value><<<(n + 127) / 128, 128, 0, st>>>(n, d_pts, d_nb); }));
-  GB_CUDA(cudaGetLastError());
-  ctx->launches++;
+  GB_CHECK(knn_dispatch(k, [&](auto K) { return gb_launch(ctx, "k_knn_bruteforce", k_knn_bruteforce<decltype(K)::value>, (n + 127) / 128, 128, 0, n, d_pts, d_nb); }));
   GB_CUDA(cudaMemcpyAsync(neighbors, d_nb, sizeof(int) * (size_t)n * k, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
   return GB_OK;
@@ -195,9 +192,7 @@ gb_status gb_covariances_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const 
   }));
   GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * (size_t)n, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(d_nb, neighbors, sizeof(int) * (size_t)n * kc, cudaMemcpyHostToDevice, st));
-  k_covariances<<<(n + 127) / 128, 128, 0, st>>>(n, d_pts, d_nb, kc, k, d_nrm, d_cov);
-  GB_CUDA(cudaGetLastError());
-  ctx->launches++;
+  GB_CHECK(gb_launch(ctx, "k_covariances", k_covariances, (n + 127) / 128, 128, 0, n, d_pts, d_nb, kc, k, d_nrm, d_cov));
   GB_CUDA(cudaMemcpyAsync(normals4, d_nrm, sizeof(double4) * (size_t)n, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaMemcpyAsync(cov4x4, d_cov, sizeof(double) * 16 * (size_t)n, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
@@ -229,17 +224,15 @@ gb_status gb_voxelgrid_sampling_impl(gb_ctx* ctx, size_t n_, const double* xyzw,
   GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * N, cudaMemcpyHostToDevice, st));
   if (times) GB_CUDA(cudaMemcpyAsync(d_t, times, sizeof(double) * N, cudaMemcpyHostToDevice, st));
   if (intensities) GB_CUDA(cudaMemcpyAsync(d_i, intensities, sizeof(double) * N, cudaMemcpyHostToDevice, st));
-  k_grid_keys<<<(n + 255) / 256, 256, 0, st>>>(n, d_pts, 1.0 / resolution, t.keys, t.idx);
-  ctx->launches++;
+  GB_CHECK(gb_grid_keys(ctx, n, d_pts, 1.0 / resolution, t.keys, t.idx));
   GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
   int V = 0;
   GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
   if (V > 0) {
-    gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts);
-    k_grid_means_counted<<<(n + 127) / 128, 128, 0, st>>>(d_pos + (n - 1), d_starts, t.idx_s, d_pts, times ? d_t : nullptr, intensities ? d_i : nullptr, d_opts, d_ot, d_oi);
-    GB_CUDA(cudaGetLastError());
-    ctx->launches++;
+    GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
+    GB_CHECK(gb_launch(ctx, "k_grid_means_counted", k_grid_means_counted, (n + 127) / 128, 128, 0, d_pos + (n - 1), d_starts, t.idx_s, d_pts, times ? d_t : nullptr,
+                       intensities ? d_i : nullptr, d_opts, d_ot, d_oi));
     GB_CUDA(cudaMemcpyAsync(out_xyzw, d_opts, sizeof(double4) * (size_t)V, cudaMemcpyDeviceToHost, st));
     if (times && out_times) GB_CUDA(cudaMemcpyAsync(out_times, d_ot, sizeof(double) * (size_t)V, cudaMemcpyDeviceToHost, st));
     if (intensities && out_intensities) GB_CUDA(cudaMemcpyAsync(out_intensities, d_oi, sizeof(double) * (size_t)V, cudaMemcpyDeviceToHost, st));
@@ -593,21 +586,16 @@ static KnnTmp take_knn_tmp(Carver& cv, int n, void* cub, size_t cub_bytes) {
 
 // exact k-NN of the first *d_count points of d_pts (device resident); neighbors[i * k + j]
 static gb_status knn_device(gb_ctx* ctx, int n, const int* d_count, const double4* d_pts, int k, double h0, int* d_nb, const KnnTmp& t) {
-  cudaStream_t st = ctx->stream;
   const int tb = 256, gb = (n + tb - 1) / tb;
-  k_fill_self<<<(int)(((size_t)n * k + 255) / 256), 256, 0, st>>>(n, k, d_nb);
-  k_ml_keys<<<gb, tb, 0, st>>>(n, d_count, d_pts, 1.0 / h0, t.s.keys, t.s.idx);
-  size_t tmp = t.s.cub_bytes;
-  GB_CUDA(cub::DeviceRadixSort::SortPairs(t.s.cub, tmp, t.s.keys, t.s.keys_s, t.s.idx, t.s.idx_s, n, 0, 64, st));
-  k_ml_gather<<<gb, tb, 0, st>>>(n, t.s.keys_s, t.s.idx_s, d_pts, t.pts_s);
-  GB_CUDA(cudaMemsetAsync(t.tables, 0xff, sizeof(MlCell) * (size_t)kMlLevels * t.ts, st));
-  k_ml_cells<<<gb, tb, 0, st>>>(n, t.s.keys_s, t.tables, t.ts);
-  GB_CHECK(knn_dispatch(k, [&](auto K) {
-    k_knn_pyramid<decltype(K)::value><<<(n + 127) / 128, 128, 0, st>>>(n, t.pts_s, t.s.keys_s, t.s.idx_s, t.tables, t.ts, 1.0 / h0, h0, d_nb);
-  }));
-  GB_CUDA(cudaGetLastError());
-  ctx->launches += 6;
-  return GB_OK;
+  GB_CHECK(gb_launch(ctx, "k_fill_self", k_fill_self, (int)(((size_t)n * k + 255) / 256), 256, 0, n, k, d_nb));
+  GB_CHECK(gb_launch(ctx, "k_ml_keys", k_ml_keys, gb, tb, 0, n, d_count, d_pts, 1.0 / h0, t.s.keys, t.s.idx));
+  GB_CUB(ctx, cub::DeviceRadixSort::SortPairs, t.s.cub, t.s.cub_bytes, t.s.keys, t.s.keys_s, t.s.idx, t.s.idx_s, n, 0, 64);
+  GB_CHECK(gb_launch(ctx, "k_ml_gather", k_ml_gather, gb, tb, 0, n, t.s.keys_s, t.s.idx_s, d_pts, t.pts_s));
+  GB_CUDA(cudaMemsetAsync(t.tables, 0xff, sizeof(MlCell) * (size_t)kMlLevels * t.ts, ctx->stream));
+  GB_CHECK(gb_launch(ctx, "k_ml_cells", k_ml_cells, gb, tb, 0, n, t.s.keys_s, t.tables, t.ts));
+  return knn_dispatch(k, [&](auto K) {
+    return gb_launch(ctx, "k_knn_pyramid", k_knn_pyramid<decltype(K)::value>, (n + 127) / 128, 128, 0, n, t.pts_s, t.s.keys_s, t.s.idx_s, t.tables, t.ts, 1.0 / h0, h0, d_nb);
+  });
 }
 
 gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out, gb_cloud* cloud_out) {
@@ -659,7 +647,7 @@ gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const d
   if (times) GB_CUDA(cudaMemcpyAsync(d_t, times, sizeof(double) * N, cudaMemcpyHostToDevice, st));
   if (intensities) GB_CUDA(cudaMemcpyAsync(d_i, intensities, sizeof(double) * N, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemsetAsync(d_cnt, 0, 256, st));
-  k_set_int<<<1, 1, 0, st>>>(d_cnt + 0, n);
+  GB_CHECK(gb_launch(ctx, "k_set_int", k_set_int, 1, 1, 0, d_cnt + 0, n));
 
   // ---- downsampling ----
   const double4* cur_pts = d_raw;
@@ -668,30 +656,25 @@ gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const d
   const int* cur_cnt = d_cnt + 0;
   const int* keep = nullptr;
   if (P->downsample_resolution > 0.0) {
-    k_grid_keys<<<gb, tb, 0, st>>>(n, d_raw, 1.0 / P->downsample_resolution, t.keys, t.idx);
-    ctx->launches++;
+    GB_CHECK(gb_grid_keys(ctx, n, d_raw, 1.0 / P->downsample_resolution, t.keys, t.idx));
     GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
-    k_copy_last_pos<<<1, 1, 0, st>>>(n, d_pos, d_cnt + 3);  // V
-    gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts);
+    GB_CHECK(gb_launch(ctx, "k_copy_last_pos", k_copy_last_pos, 1, 1, 0, n, d_pos, d_cnt + 3));  // V
+    GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
     if (P->use_random_grid_downsampling) {
       const double rate = P->downsample_target > 0 ? (double)P->downsample_target / (double)n : P->downsample_rate;  // :105
       if (rate < 0.99) {
         GB_CUDA(cudaMemsetAsync(d_keep, 0, sizeof(int) * N, st));
-        k_randomgrid_select<<<gb, tb, 0, st>>>(n, d_cnt + 3, d_starts, t.idx_s, rate, P->seed, d_keep);
+        GB_CHECK(gb_launch(ctx, "k_randomgrid_select", k_randomgrid_select, gb, tb, 0, n, d_cnt + 3, d_starts, t.idx_s, rate, P->seed, d_keep));
         const int cap = (int)((double)n * rate * 1.2);
         if (cap > 0 && cap < n) {  // thin the survivors to 1.2 * rate * N: the smallest hashes stay
-          k_rg_hash_keys<<<gb, tb, 0, st>>>(n, d_keep, P->seed, t.keys);
-          size_t tmp = cub_b;
-          GB_CUDA(cub::DeviceRadixSort::SortKeys(t.cub, tmp, t.keys, t.keys_s, n, 0, 64, st));
-          k_rg_cap<<<gb, tb, 0, st>>>(n, cap, t.keys_s, P->seed, d_keep);
-          ctx->launches += 3;
+          GB_CHECK(gb_launch(ctx, "k_rg_hash_keys", k_rg_hash_keys, gb, tb, 0, n, d_keep, P->seed, t.keys));
+          GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, cub_b, t.keys, t.keys_s, n, 0, 64);
+          GB_CHECK(gb_launch(ctx, "k_rg_cap", k_rg_cap, gb, tb, 0, n, cap, t.keys_s, P->seed, d_keep));
         }
-        ctx->launches++;
         keep = d_keep;  // original order is kept; the gates below drop the rest
       }
     } else {
-      k_grid_means_counted<<<(n + 127) / 128, 128, 0, st>>>(d_cnt + 3, d_starts, t.idx_s, d_raw, cur_t, cur_i, d_ds, d_dst, d_dsi);
-      ctx->launches++;
+      GB_CHECK(gb_launch(ctx, "k_grid_means_counted", k_grid_means_counted, (n + 127) / 128, 128, 0, d_cnt + 3, d_starts, t.idx_s, d_raw, cur_t, cur_i, d_ds, d_dst, d_dsi));
       cur_pts = d_ds; cur_t = times ? d_dst : nullptr; cur_i = intensities ? d_dsi : nullptr; cur_cnt = d_cnt + 3;
     }
   }
@@ -703,29 +686,21 @@ gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const d
   for (int a = 0; a < 3; a++) { ff.bmin[a] = P->crop_bbox_min[a]; ff.bmax[a] = P->crop_bbox_max[a]; }
   for (int r = 0; r < 3; r++) for (int c = 0; c < 4; c++) ff.T[r * 4 + c] = P->T_imu_lidar[c * 4 + r];
   ff.global_shutter = P->global_shutter;
-  k_filter_time_keys<<<gb, tb, 0, st>>>(n, cur_cnt, keep, cur_pts, cur_t, ff, t.keys, t.idx, d_cnt + 2);
-  {
-    size_t tmp = cub_b;
-    GB_CUDA(cub::DeviceRadixSort::SortPairs(t.cub, tmp, t.keys, t.keys_s, t.idx, t.idx_s, n, 0, 64, st));
-  }
-  k_gather_frame<<<gb, tb, 0, st>>>(n, d_cnt + 2, t.idx_s, cur_pts, cur_t, cur_i, P->global_shutter, d_fr, d_frt, d_fri);
-  ctx->launches += 3;
+  GB_CHECK(gb_launch(ctx, "k_filter_time_keys", k_filter_time_keys, gb, tb, 0, n, cur_cnt, keep, cur_pts, cur_t, ff, t.keys, t.idx, d_cnt + 2));
+  GB_CUB(ctx, cub::DeviceRadixSort::SortPairs, t.cub, cub_b, t.keys, t.keys_s, t.idx, t.idx_s, n, 0, 64);
+  GB_CHECK(gb_launch(ctx, "k_gather_frame", k_gather_frame, gb, tb, 0, n, d_cnt + 2, t.idx_s, cur_pts, cur_t, cur_i, P->global_shutter, d_fr, d_frt, d_fri));
   const double h0 = P->knn_cell_size > 0.0 ? P->knn_cell_size : 0.25;
   const int* frame_cnt = d_cnt + 2;
   // ---- statistical outlier removal (optional) ----
   if (P->enable_outlier_removal) {
     const int ko = P->outlier_removal_k;
     GB_CHECK(knn_device(ctx, n, d_cnt + 2, d_fr, ko, h0, d_nbo, knn));
-    k_sor_dists<<<gb, tb, 0, st>>>(n, d_cnt + 2, d_fr, d_nbo, ko, d_dist, d_dist2);
-    size_t tmp = cub_b;
-    GB_CUDA(cub::DeviceReduce::Sum(t.cub, tmp, d_dist, d_sums, n, st));
-    tmp = cub_b;
-    GB_CUDA(cub::DeviceReduce::Sum(t.cub, tmp, d_dist2, d_sums + 1, n, st));
-    k_sor_flags<<<gb, tb, 0, st>>>(n, d_cnt + 2, d_dist, d_sums, P->outlier_std_mul_factor, d_keep);
-    tmp = cub_b;
-    GB_CUDA(cub::DeviceScan::InclusiveSum(t.cub, tmp, d_keep, d_pos, n, st));
-    k_sor_compact<<<gb, tb, 0, st>>>(n, d_keep, d_pos, d_fr, d_frt, intensities ? d_fri : nullptr, d_fr2, d_frt2, d_fri2, d_cnt + 4);
-    ctx->launches += 6;
+    GB_CHECK(gb_launch(ctx, "k_sor_dists", k_sor_dists, gb, tb, 0, n, d_cnt + 2, d_fr, d_nbo, ko, d_dist, d_dist2));
+    GB_CUB(ctx, cub::DeviceReduce::Sum, t.cub, cub_b, d_dist, d_sums, n);
+    GB_CUB(ctx, cub::DeviceReduce::Sum, t.cub, cub_b, d_dist2, d_sums + 1, n);
+    GB_CHECK(gb_launch(ctx, "k_sor_flags", k_sor_flags, gb, tb, 0, n, d_cnt + 2, d_dist, d_sums, P->outlier_std_mul_factor, d_keep));
+    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_keep, d_pos, n);
+    GB_CHECK(gb_launch(ctx, "k_sor_compact", k_sor_compact, gb, tb, 0, n, d_keep, d_pos, d_fr, d_frt, intensities ? d_fri : nullptr, d_fr2, d_frt2, d_fri2, d_cnt + 4));
     d_fr = d_fr2; d_frt = d_frt2; d_fri = d_fri2;
     frame_cnt = d_cnt + 4;
   }
@@ -738,9 +713,8 @@ gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const d
   out->num_points = (size_t)M;
   // ---- covariances, written straight into the staged fp32 planes of the cloud (PointCloudGPU::clone on the device) ----
   if (P->estimate_covariances && M > 0) {
-    k_covariances_planes<<<(M + 127) / 128, 128, 0, st>>>(M, frame_cnt, d_fr, d_nb, k, P->k_neighbors_cov > 0 ? P->k_neighbors_cov : k, d_nrm, d_cov, staged.p0, staged.p1, staged.p2, staged.normals);
-    GB_CUDA(cudaGetLastError());
-    ctx->launches++;
+    GB_CHECK(gb_launch(ctx, "k_covariances_planes", k_covariances_planes, (M + 127) / 128, 128, 0, M, frame_cnt, d_fr, d_nb, k, P->k_neighbors_cov > 0 ? P->k_neighbors_cov : k, d_nrm, d_cov,
+                       staged.p0, staged.p1, staged.p2, staged.normals));
     if (cloud_out) GB_CHECK(gb_cloud_build(ctx, cloud_out, (size_t)M, staged, t));  // the frame is gathered: t is free again
   }
   // ---- host products: D2H into the context's pinned staging (full PCIe rate), then one memcpy each into the caller's arrays ----
@@ -790,7 +764,7 @@ gb_status gb_find_neighbors_pyramid_impl(gb_ctx* ctx, size_t n_, const double* x
     d_nb = cv.take<int>(N * (size_t)k);
   }));
   GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * N, cudaMemcpyHostToDevice, st));
-  k_set_int<<<1, 1, 0, st>>>(d_cnt, n);
+  GB_CHECK(gb_launch(ctx, "k_set_int", k_set_int, 1, 1, 0, d_cnt, n));
   GB_CHECK(knn_device(ctx, n, d_cnt, d_pts, k, 0.25, d_nb, knn));
   GB_CUDA(cudaMemcpyAsync(neighbors, d_nb, sizeof(int) * N * (size_t)k, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
@@ -892,9 +866,7 @@ gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T, vo
   memcpy(h, &F, sizeof(MergeFrame));
   GB_CUDA(cudaMemcpyAsync(d_frame, h, sizeof(MergeFrame), cudaMemcpyHostToDevice, ctx->stream));
   const int n = (int)c->n;
-  k_merge_transform<<<(n + 255) / 256, 256, 0, ctx->stream>>>(1, (const MergeFrame*)d_frame, n, pts, cov6);
-  ctx->launches++;
-  return GB_OK;
+  return gb_launch(ctx, "k_merge_transform", k_merge_transform, (n + 255) / 256, 256, 0, 1, (const MergeFrame*)d_frame, n, pts, cov6);
 }
 
 gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out) {
@@ -939,28 +911,23 @@ gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames
   GB_CUDA(cudaMemcpyAsync(d_mf, h_mf, sizeof(MergeFrame) * (size_t)K, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemsetAsync(d_cnt, 0, 256, st));
   const int tb = 256, gb = (n + tb - 1) / tb;
-  k_merge_transform<<<gb, tb, 0, st>>>(K, d_mf, n, d_pts, d_cov);
-  k_grid_keys<<<gb, tb, 0, st>>>(n, d_pts, 1.0 / resolution, t.keys, t.idx);
+  GB_CHECK(gb_launch(ctx, "k_merge_transform", k_merge_transform, gb, tb, 0, K, d_mf, n, d_pts, d_cov));
+  GB_CHECK(gb_grid_keys(ctx, n, d_pts, 1.0 / resolution, t.keys, t.idx));
   GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
-  k_copy_last_pos<<<1, 1, 0, st>>>(n, d_pos, d_cnt);  // V
-  gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts);
-  k_merge_means<<<(n + 127) / 128, 128, 0, st>>>(d_cnt, d_starts, t.idx_s, d_pts, d_cov, d_vpts, d_vcov);
+  GB_CHECK(gb_launch(ctx, "k_copy_last_pos", k_copy_last_pos, 1, 1, 0, n, d_pos, d_cnt));  // V
+  GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
+  GB_CHECK(gb_launch(ctx, "k_merge_means", k_merge_means, (n + 127) / 128, 128, 0, d_cnt, d_starts, t.idx_s, d_pts, d_cov, d_vpts, d_vcov));
   // thinning to target_num_points
-  k_merge_hash_keys<<<gb, tb, 0, st>>>(n, d_cnt, seed, t.keys);
-  size_t tmp = cub_b;
-  GB_CUDA(cub::DeviceRadixSort::SortKeys(t.cub, tmp, t.keys, t.keys_s, n, 0, 64, st));
-  k_merge_keep<<<gb, tb, 0, st>>>(n, d_cnt, target, t.keys_s, seed, d_keep);
-  tmp = cub_b;
-  GB_CUDA(cub::DeviceScan::InclusiveSum(t.cub, tmp, d_keep, d_pos, n, st));
+  GB_CHECK(gb_launch(ctx, "k_merge_hash_keys", k_merge_hash_keys, gb, tb, 0, n, d_cnt, seed, t.keys));
+  GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, cub_b, t.keys, t.keys_s, n, 0, 64);
+  GB_CHECK(gb_launch(ctx, "k_merge_keep", k_merge_keep, gb, tb, 0, n, d_cnt, target, t.keys_s, seed, d_keep));
+  GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_keep, d_pos, n);
   int M = 0;
   GB_CUDA(cudaMemcpyAsync(&M, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
-  ctx->launches += 8;
   *num_out = (size_t)M;
   if (M == 0) return GB_OK;
-  k_merge_emit<<<gb, tb, 0, st>>>(n, d_keep, d_pos, d_vpts, d_vcov, d_pts /* reused: emitted points */, d_ocov, staged.p0, staged.p1, staged.p2);
-  GB_CUDA(cudaGetLastError());
-  ctx->launches++;
+  GB_CHECK(gb_launch(ctx, "k_merge_emit", k_merge_emit, gb, tb, 0, n, d_keep, d_pos, d_vpts, d_vcov, d_pts /* reused: emitted points */, d_ocov, staged.p0, staged.p1, staged.p2));
   if (cloud_out) GB_CHECK(gb_cloud_build(ctx, cloud_out, (size_t)M, staged, t));
   if (out_xyzw) GB_CUDA(cudaMemcpyAsync(out_xyzw, d_pts, sizeof(double4) * (size_t)M, cudaMemcpyDeviceToHost, st));
   if (out_cov4x4) GB_CUDA(cudaMemcpyAsync(out_cov4x4, d_ocov, sizeof(double) * 16 * (size_t)M, cudaMemcpyDeviceToHost, st));

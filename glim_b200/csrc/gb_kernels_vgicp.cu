@@ -559,15 +559,15 @@ __global__ void __launch_bounds__(256) k_overlap(int num_targets, const FactorDe
 // launchers
 // ---------------------------------------------------------------------------------------------
 template <int MODE, bool PEER>
-static cudaError_t launch5(gb_sweep* s, const double* poses_eval, float* slab, const PeerPush* pp) {
-  k_vgicp_sweep5<MODE, PEER><<<s->grid, kThreads, 0, s->ctx->stream>>>(s->d_descs, (int)s->F, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr, s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
-  return cudaGetLastError();
+static gb_status launch5(gb_sweep* s, const double* poses_eval, float* slab, const PeerPush* pp) {
+  return gb_launch(s->ctx, "k_vgicp_sweep5", k_vgicp_sweep5<MODE, PEER>, s->grid, kThreads, 0, s->d_descs, (int)s->F, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr,
+                   s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
 }
 
 template <int MODE, bool PEER, bool SV>
-static cudaError_t launch3(gb_sweep* s, const double* poses_eval, float* slab, const PeerPush* pp) {
-  k_vgicp_sweep3<MODE, PEER, SV><<<s->grid, kThreads, 0, s->ctx->stream>>>(s->d_descs, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr, s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
-  return cudaGetLastError();
+static gb_status launch3(gb_sweep* s, const double* poses_eval, float* slab, const PeerPush* pp) {
+  return gb_launch(s->ctx, "k_vgicp_sweep3", k_vgicp_sweep3<MODE, PEER, SV>, s->grid, kThreads, 0, s->d_descs, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr,
+                   s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
 }
 
 // completion flags of the fused exchange: one thread per rank publishes this rank's step to that peer, then waits for the
@@ -591,31 +591,29 @@ __global__ void k_peer_signal_wait(PeerFlags pf, int world, int rank, unsigned s
 
 gb_status gb_launch_sweep(gb_sweep* s, int mode) {
   if (s->num_tiles == 0) return GB_OK;
-  gb_ctx* ctx = s->ctx;
   // the table for the buffer of the current step parity (both were written to the device when the slab was attached)
   const bool peer = (mode == GB_MODE_LINEARIZE) && s->peer != nullptr;
   const PeerPush* pp = peer ? s->d_peer_tables + s->peer->parity : nullptr;
   float* slab = mode == GB_MODE_LINEARIZE ? s->d_slab : nullptr;
   const double* pe = mode == GB_MODE_ERROR ? s->d_poses_eval : nullptr;
-  cudaError_t e;
+  gb_status st;
   if (s->kernel_version == 3) {
     if (s->any_sv) {
-      if (mode == GB_MODE_LINEARIZE) e = peer ? launch3<GB_MODE_LINEARIZE, true, true>(s, pe, slab, pp) : launch3<GB_MODE_LINEARIZE, false, true>(s, pe, slab, pp);
-      else e = launch3<GB_MODE_ERROR, false, true>(s, pe, slab, pp);
+      if (mode == GB_MODE_LINEARIZE) st = peer ? launch3<GB_MODE_LINEARIZE, true, true>(s, pe, slab, pp) : launch3<GB_MODE_LINEARIZE, false, true>(s, pe, slab, pp);
+      else st = launch3<GB_MODE_ERROR, false, true>(s, pe, slab, pp);
     } else {
-      if (mode == GB_MODE_LINEARIZE) e = peer ? launch3<GB_MODE_LINEARIZE, true, false>(s, pe, slab, pp) : launch3<GB_MODE_LINEARIZE, false, false>(s, pe, slab, pp);
-      else e = launch3<GB_MODE_ERROR, false, false>(s, pe, slab, pp);
+      if (mode == GB_MODE_LINEARIZE) st = peer ? launch3<GB_MODE_LINEARIZE, true, false>(s, pe, slab, pp) : launch3<GB_MODE_LINEARIZE, false, false>(s, pe, slab, pp);
+      else st = launch3<GB_MODE_ERROR, false, false>(s, pe, slab, pp);
     }
   } else {
-    if (mode == GB_MODE_LINEARIZE) e = peer ? launch5<GB_MODE_LINEARIZE, true>(s, pe, slab, pp) : launch5<GB_MODE_LINEARIZE, false>(s, pe, slab, pp);
-    else e = launch5<GB_MODE_ERROR, false>(s, pe, slab, pp);
+    if (mode == GB_MODE_LINEARIZE) st = peer ? launch5<GB_MODE_LINEARIZE, true>(s, pe, slab, pp) : launch5<GB_MODE_LINEARIZE, false>(s, pe, slab, pp);
+    else st = launch5<GB_MODE_ERROR, false>(s, pe, slab, pp);
   }
-  if (e != cudaSuccess) { gb_set_error("sweep launch failed: %s", cudaGetErrorString(e)); return GB_ERR_CUDA; }
+  GB_CHECK(st);
   // queue bookkeeping: a sweep with more items than warps draws one ticket per processed item, plus, for sweep5, one per warp
   // for its one-item look-ahead
   const unsigned long long warps = (unsigned long long)s->grid * kWarps;
   if ((unsigned long long)s->num_tiles > warps) s->ctr_base += (s->kernel_version == 3 ? 0ull : warps) + (unsigned long long)s->num_tiles;
-  ctx->launches++;
   return GB_OK;
 }
 
@@ -689,25 +687,16 @@ gb_status gb_launch_peer_signal_wait(gb_peer_slab* ps) {
     px.my_pairs = ps->d_my_pairs;
     px.num_my_pairs = ps->num_my_pairs;
     px.arrivals = reinterpret_cast<unsigned*>(ps->d_timeout) + 16;  // zeroed at creation, self-cleaning
-    k_peer_exchange<<<ps->world * kExchangeCtasPerPeer, kExchangeThreads, 0, ps->ctx->stream>>>(px, ps->world, ps->rank, ps->step, ps->d_timeout);
-    GB_CUDA(cudaGetLastError());
-    ps->ctx->launches++;
-    return GB_OK;
+    return gb_launch(ps->ctx, "k_peer_exchange", k_peer_exchange, ps->world * kExchangeCtasPerPeer, kExchangeThreads, 0, px, ps->world, ps->rank, ps->step, ps->d_timeout);
   }
   PeerFlags pf;
   memset(&pf, 0, sizeof(pf));
   for (int p = 0; p < ps->world; p++) pf.flags[p] = reinterpret_cast<unsigned*>(ps->peer[p] + 2 * ps->buf_floats * sizeof(float));
-  k_peer_signal_wait<<<1, 32, 0, ps->ctx->stream>>>(pf, ps->world, ps->rank, ps->step, ps->d_timeout);
-  GB_CUDA(cudaGetLastError());
-  ps->ctx->launches++;
-  return GB_OK;
+  return gb_launch(ps->ctx, "k_peer_signal_wait", k_peer_signal_wait, 1, 32, 0, pf, ps->world, ps->rank, ps->step, ps->d_timeout);
 }
 
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count) {
   if (n <= 0 || num_targets <= 0) return GB_OK;
   const int grid = min((n + 255) / 256, ctx->num_sms * 8);
-  k_overlap<<<grid, 256, (size_t)num_targets * 12 * sizeof(float), ctx->stream>>>(num_targets, d_descs, d_poses, n, d_count);
-  GB_CUDA(cudaGetLastError());
-  ctx->launches++;
-  return GB_OK;
+  return gb_launch(ctx, "k_overlap", k_overlap, grid, 256, (size_t)num_targets * 12 * sizeof(float), num_targets, d_descs, d_poses, n, d_count);
 }

@@ -132,19 +132,14 @@ __global__ void k_table_finalize(int nb, const int4* __restrict__ vcoord, int4* 
 }  // namespace
 
 gb_status gb_group_by_key(gb_ctx* ctx, int n, const gb_sort_tmp& t, int* flags, int* pos) {
-  cudaStream_t st = ctx->stream;
-  size_t tmp = t.cub_bytes;
-  GB_CUDA(cub::DeviceRadixSort::SortPairs(t.cub, tmp, t.keys, t.keys_s, t.idx, t.idx_s, n, 0, 64, st));
-  k_head_flags<<<(n + 255) / 256, 256, 0, st>>>(n, t.keys_s, flags);
-  tmp = t.cub_bytes;
-  GB_CUDA(cub::DeviceScan::InclusiveSum(t.cub, tmp, flags, pos, n, st));
-  ctx->launches += 3;
+  GB_CUB(ctx, cub::DeviceRadixSort::SortPairs, t.cub, t.cub_bytes, t.keys, t.keys_s, t.idx, t.idx_s, n, 0, 64);
+  GB_CHECK(gb_launch(ctx, "k_head_flags", k_head_flags, (n + 255) / 256, 256, 0, n, t.keys_s, flags));
+  GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, t.cub_bytes, flags, pos, n);
   return GB_OK;
 }
 
-void gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* flags, const int* pos, int* starts) {
-  k_voxel_starts<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, t.keys_s, flags, pos, starts);
-  ctx->launches++;
+gb_status gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* flags, const int* pos, int* starts) {
+  return gb_launch(ctx, "k_voxel_starts", k_voxel_starts, (n + 255) / 256, 256, 0, n, t.keys_s, flags, pos, starts);
 }
 
 // The hash table of V voxels (vcoord[v] = {x, y, z, points}; d_dropped: one int of scratch, unused when V = 0): num_buckets =
@@ -159,21 +154,15 @@ static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dr
                                                              // same rule as the oracle
   for (;;) {
     GB_CUDA(gb_dev_malloc(ctx->device, sizeof(int4) * (size_t)nb, (void**)buckets));
-    k_table_clear<<<(nb + 255) / 256, 256, 0, st>>>(nb, *buckets);
-    ctx->launches++;
+    GB_CHECK(gb_launch(ctx, "k_table_clear", k_table_clear, (nb + 255) / 256, 256, 0, nb, *buckets));
     int dropped = 0;
     if (V > 0) {
       GB_CUDA(cudaMemsetAsync(d_dropped, 0, sizeof(int), st));
-      k_table_insert<<<(V + 255) / 256, 256, 0, st>>>(V, d_vcoord, *buckets, (uint32_t)nb - 1u, max_scan, d_dropped);
-      k_table_finalize<<<(nb + 255) / 256, 256, 0, st>>>(nb, d_vcoord, *buckets);
-      ctx->launches += 2;
-      GB_CUDA(cudaMemcpyAsync(&dropped, d_dropped, sizeof(int), cudaMemcpyDeviceToHost, st));
-    } else {
-      k_table_finalize<<<(nb + 255) / 256, 256, 0, st>>>(nb, d_vcoord, *buckets);
-      ctx->launches++;
+      GB_CHECK(gb_launch(ctx, "k_table_insert", k_table_insert, (V + 255) / 256, 256, 0, V, d_vcoord, *buckets, (uint32_t)nb - 1u, max_scan, d_dropped));
     }
+    GB_CHECK(gb_launch(ctx, "k_table_finalize", k_table_finalize, (nb + 255) / 256, 256, 0, nb, d_vcoord, *buckets));
+    if (V > 0) GB_CUDA(cudaMemcpyAsync(&dropped, d_dropped, sizeof(int), cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
-    GB_CUDA(cudaGetLastError());
     *num_buckets = nb;
     *num_dropped_points = dropped;
     if ((double)dropped <= drop_rate * total_points || nb >= (1 << 28)) break;
@@ -207,17 +196,15 @@ gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resol
       d_vcoord = cv.take<int4>(n);
       d_dropped = cv.take<int>(1);
     }));
-    k_point_keys<<<(n + 255) / 256, 256, 0, st>>>(n, cloud->p0, cloud->inv_perm, m->inv_res, t.keys, t.idx);
-    ctx->launches++;
+    GB_CHECK(gb_launch(ctx, "k_point_keys", k_point_keys, (n + 255) / 256, 256, 0, n, cloud->p0, cloud->inv_perm, m->inv_res, t.keys, t.idx));
     GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
     GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
     if (V > 0) {
       GB_CUDA(gb_dev_malloc(ctx->device, sizeof(float4) * 3 * (size_t)V, &m->base));
       m->voxels = (float4*)m->base;
-      gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts);
-      k_voxel_reduce<<<(V + 127) / 128, 128, 0, st>>>(V, d_starts, t.keys_s, t.idx_s, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm, m->voxels, d_vcoord);
-      ctx->launches++;
+      GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
+      GB_CHECK(gb_launch(ctx, "k_voxel_reduce", k_voxel_reduce, (V + 127) / 128, 128, 0, V, d_starts, t.keys_s, t.idx_s, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm, m->voxels, d_vcoord));
     }
   }
   m->num_voxels = V;
@@ -381,29 +368,24 @@ gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* c
     }));
     const int tb = 256;
     if (Vo > 0) {
-      k_ins_old_keys<<<(Vo + tb - 1) / tb, tb, 0, st>>>(Vo, m->vkeys, t.keys, t.idx);
-      ctx->launches++;
+      GB_CHECK(gb_launch(ctx, "k_ins_old_keys", k_ins_old_keys, (Vo + tb - 1) / tb, tb, 0, Vo, m->vkeys, t.keys, t.idx));
     }
     if (np > 0) {
       GB_CHECK(gb_transform_frame(ctx, cloud, T, d_frame, d_pts, d_cov));
-      gb_grid_keys(ctx, np, d_pts, 1.0 / (double)m->resolution, t.keys + Vo, t.idx + Vo);
+      GB_CHECK(gb_grid_keys(ctx, np, d_pts, 1.0 / (double)m->resolution, t.keys + Vo, t.idx + Vo));
       if (kept < n) {
-        k_ins_sample_hash<<<(np + tb - 1) / tb, tb, 0, st>>>(np, seed, t.keys_s);
-        size_t tmp = cub_b;
-        GB_CUDA(cub::DeviceRadixSort::SortKeys(t.cub, tmp, t.keys_s, d_hash, np, 0, 64, st));
-        k_ins_sample_drop<<<(np + tb - 1) / tb, tb, 0, st>>>(np, kept, seed, d_hash, t.keys + Vo);
-        ctx->launches += 3;
+        GB_CHECK(gb_launch(ctx, "k_ins_sample_hash", k_ins_sample_hash, (np + tb - 1) / tb, tb, 0, np, seed, t.keys_s));
+        GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, cub_b, t.keys_s, d_hash, np, 0, 64);
+        GB_CHECK(gb_launch(ctx, "k_ins_sample_drop", k_ins_sample_drop, (np + tb - 1) / tb, tb, 0, np, kept, seed, d_hash, t.keys + Vo));
       }
     }
     GB_CUDA(cudaMemsetAsync(d_info, 0, 2 * sizeof(unsigned long long), st));
     GB_CHECK(gb_group_by_key(ctx, N, t, d_flags, d_pos));
-    gb_group_starts(ctx, N, t, d_flags, d_pos, d_starts);
-    k_ins_merge<<<(N + 127) / 128, 128, 0, st>>>(N, d_pos + (N - 1), d_starts, t.idx_s, m->vn, m->vstamp, m->vsums, d_pts, d_cov, m->lru_counter,
-                                                  m->lru_horizon, m->lru_clear_cycle, d_mn, d_mstamp, d_msums, d_keep, d_info);
-    size_t tmp = cub_b;
-    GB_CUDA(cub::DeviceScan::InclusiveSum(t.cub, tmp, d_keep, d_kpos, N, st));
-    k_ins_count<<<1, 1, 0, st>>>(N, d_kpos, d_info + 1);
-    ctx->launches += 3;
+    GB_CHECK(gb_group_starts(ctx, N, t, d_flags, d_pos, d_starts));
+    GB_CHECK(gb_launch(ctx, "k_ins_merge", k_ins_merge, (N + 127) / 128, 128, 0, N, d_pos + (N - 1), d_starts, t.idx_s, m->vn, m->vstamp, m->vsums, d_pts, d_cov, m->lru_counter,
+                       m->lru_horizon, m->lru_clear_cycle, d_mn, d_mstamp, d_msums, d_keep, d_info));
+    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_keep, d_kpos, N);
+    GB_CHECK(gb_launch(ctx, "k_ins_count", k_ins_count, 1, 1, 0, N, d_kpos, d_info + 1));
     unsigned long long info[2] = {0, 0};
     GB_CUDA(cudaMemcpyAsync(info, d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
@@ -418,9 +400,9 @@ gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* c
       GB_CUDA(gb_dev_malloc(ctx->device, size.off, &next.base));
       Carver cv{(char*)next.base};
       state_layout(cv, (size_t)V, &next);
-      k_ins_emit<<<(N + tb - 1) / tb, tb, 0, st>>>(N, d_pos + (N - 1), d_keep, d_kpos, d_starts, t.keys_s, d_mn, d_mstamp, d_msums,
-                                                   next.vkeys, next.vn, next.vstamp, next.vsums, next.voxels, d_vcoord);
-      ctx->launches++;
+      gb_status s = gb_launch(ctx, "k_ins_emit", k_ins_emit, (N + tb - 1) / tb, tb, 0, N, d_pos + (N - 1), d_keep, d_kpos, d_starts, t.keys_s, d_mn, d_mstamp, d_msums,
+                              next.vkeys, next.vn, next.vstamp, next.vsums, next.voxels, d_vcoord);
+      if (s != GB_OK) { gb_dev_free(ctx->device, next.base); return s; }
     } else {
       next.voxels = nullptr; next.vkeys = nullptr; next.vn = nullptr; next.vstamp = nullptr; next.vsums = nullptr;
     }
@@ -480,7 +462,6 @@ __global__ void k_permute_cloud(int n, const int* __restrict__ perm, const float
 
 gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n_, const gb_planes& s, const gb_sort_tmp& t) {
   const int n = (int)n_;
-  cudaStream_t st = ctx->stream;
   gb_planes d;
   auto layout = [&](Carver& cv) {
     d = gb_cloud_planes(cv, n_, s.normals != nullptr);
@@ -496,11 +477,7 @@ gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n_, const gb_planes& s
   layout(cv);
   c->p0 = d.p0; c->p1 = d.p1; c->p2 = d.p2; c->normals = d.normals;
   const int tb = 256, gb = (n + tb - 1) / tb;
-  k_morton_keys<<<gb, tb, 0, st>>>(n, s.p0, t.keys, t.idx);
-  size_t tmp = t.cub_bytes;
-  GB_CUDA(cub::DeviceRadixSort::SortPairs(t.cub, tmp, t.keys, t.keys_s, t.idx, c->perm, n, 0, 64, st));
-  k_permute_cloud<<<gb, tb, 0, st>>>(n, c->perm, s.p0, s.p1, s.p2, s.normals, c->p0, c->p1, c->p2, c->normals, c->inv_perm);
-  GB_CUDA(cudaGetLastError());
-  ctx->launches += 3;
-  return GB_OK;
+  GB_CHECK(gb_launch(ctx, "k_morton_keys", k_morton_keys, gb, tb, 0, n, s.p0, t.keys, t.idx));
+  GB_CUB(ctx, cub::DeviceRadixSort::SortPairs, t.cub, t.cub_bytes, t.keys, t.keys_s, t.idx, c->perm, n, 0, 64);
+  return gb_launch(ctx, "k_permute_cloud", k_permute_cloud, gb, tb, 0, n, c->perm, s.p0, s.p1, s.p2, s.normals, c->p0, c->p1, c->p2, c->normals, c->inv_perm);
 }

@@ -87,7 +87,9 @@ GB_API gb_status gb_ctx_create_on_stream(int device, void* cuda_stream, gb_ctx**
 GB_API gb_status gb_ctx_destroy(gb_ctx* ctx);
 GB_API gb_status gb_ctx_synchronize(gb_ctx* ctx);
 GB_API void* gb_ctx_stream(gb_ctx* ctx); /* the cudaStream_t */
-GB_API uint64_t gb_ctx_kernel_launches(gb_ctx* ctx); /* kernels of this library launched so far */
+/* launches made through ctx so far: one per kernel launch and one per cub device-wide call (a sort or scan of several
+ * kernels) of this library, one per launch of a captured sweep graph; memsets and copies are not counted */
+GB_API uint64_t gb_ctx_kernel_launches(gb_ctx* ctx);
 
 /* ---- PointCloudGPU::clone(frame[, stream]) (odometry_estimation_gpu.cpp:96; sub_mapping.cpp:168,393;
  *      global_mapping.cpp:253,260,743).  Host layout as the reference's PointCloudCPU:

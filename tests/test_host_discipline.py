@@ -1,0 +1,218 @@
+"""Host-side rules of the native library, checked on its sources (glim_b200/csrc/*.cu, *.cuh):
+
+1. Every kernel launch goes through gb_launch: no triple-chevron launch anywhere else.
+2. The launch counter (gb_ctx_kernel_launches) is written only by gb_launch, GB_CUB and the graph path of sweep_linearize.
+3. Every cub device-wide call with temporary storage goes through GB_CUB (the size queries pass nullptr storage).
+4. Every C-ABI entry point that takes a context, sweep, factor or peer slab enters through GB_ENTER (the context's lock and
+   device), unless it is listed below with its reason; the lock and cudaSetDevice appear nowhere else but in GB_ENTER and
+   the context lifetime and teardown functions.
+
+The function bodies are found by brace matching on the sources with comments, strings and preprocessor lines removed."""
+import os
+import re
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CSRC = os.path.join(ROOT, "glim_b200", "csrc")
+
+HANDLE_PARAM = re.compile(r"\b(gb_ctx|gb_sweep|gb_factor|gb_peer_slab)\s*\*(?!\s*\*)")  # a handle taken, not a created one returned
+# C-ABI entry points that take a handle but do not enter its context
+NO_ENTER = {
+    "gb_ctx_stream": "getter of a field fixed at creation",
+    "gb_ctx_kernel_launches": "getter of the counter; no CUDA call",
+    "gb_sweep_results_device": "getter of a pointer fixed at creation",
+    "gb_sweep_stats": "getter of host fields",
+    "gb_peer_slab_device_ptr": "getter: pointer arithmetic on the slab's own fields",
+    "gb_vgicp_factor_create": "only retains the context (an atomic increment); no CUDA call",
+    "gb_sweep_attach_slab": "host-only: records the caller's slab pointer",
+    "gb_ctx_destroy": "teardown: locks the context itself, then releases it outside the lock",
+    "gb_vgicp_factor_destroy": "teardown: sweep_free locks the context; the registry mutex guards the factor links",
+    "gb_sweep_destroy": "teardown: sweep_free locks the context, then releases it outside the lock",
+}
+# the only functions that may take the lock or set the device by hand: context lifetime, teardown, and calls on objects
+# that keep no context (a device number only)
+LOCK_OR_DEVICE_BY_HAND = {"ctx_create", "ctx_release", "gb_ctx_destroy", "sweep_free", "gb_mem_info", "gb_cloud_destroy", "gb_voxelmap_destroy",
+                          "gb_cloud_download", "gb_voxelmap_download"}
+COUNTER_WRITERS = {"gb_launch", "sweep_linearize"}  # and the GB_CUB macro
+
+
+def strip_source(text):
+    """Comments, string and character literals blanked (same length, newlines kept) and preprocessor lines split off:
+    returns (code, [preprocessor directives with their continuation lines joined])."""
+    out = []
+    i, n = 0, len(text)
+    while i < n:
+        c = text[i]
+        if text.startswith("//", i):
+            j = text.find("\n", i)
+            j = n if j < 0 else j
+            out.append(" " * (j - i))
+            i = j
+        elif text.startswith("/*", i):
+            j = text.find("*/", i + 2)
+            j = n if j < 0 else j + 2
+            out.append(re.sub(r"[^\n]", " ", text[i:j]))
+            i = j
+        elif c in "\"'":
+            j = i + 1
+            while j < n and text[j] != c:
+                j += 2 if text[j] == "\\" else 1
+            out.append(c + " " * (j - i - 1) + c)
+            i = j + 1
+        else:
+            out.append(c)
+            i += 1
+    code = "".join(out)
+    lines = code.split("\n")
+    directives, k = [], 0
+    while k < len(lines):
+        if lines[k].lstrip().startswith("#"):
+            start = k
+            while lines[k].rstrip().endswith("\\") and k + 1 < len(lines):
+                k += 1
+            directives.append("\n".join(lines[start:k + 1]))
+            for m in range(start, k + 1):
+                lines[m] = " " * len(lines[m])
+        k += 1
+    return "\n".join(lines), directives
+
+
+def match_brace(code, i):
+    depth = 0
+    for j in range(i, len(code)):
+        if code[j] == "{":
+            depth += 1
+        elif code[j] == "}":
+            depth -= 1
+            if depth == 0:
+                return j
+    raise ValueError("unbalanced braces")
+
+
+def function_name(header):
+    """Name of the function a block header defines (the identifier before its last parenthesised group), else None."""
+    h = re.sub(r"\b(const|noexcept|override)\s*$", "", header.rstrip()).rstrip()
+    if not h.endswith(")"):
+        return None
+    depth = 0
+    for j in range(len(h) - 1, -1, -1):
+        depth += h[j] == ")"
+        depth -= h[j] == "("
+        if depth == 0:
+            m = re.search(r"([A-Za-z_]\w*)\s*(<[^()]*>)?\s*$", h[:j])
+            return m.group(1) if m else None
+    return None
+
+
+def functions(code):
+    """[(name, header, body_start, body_end)] of the function definitions outside other functions (namespaces are transparent)."""
+    found, seg, i = [], 0, 0
+    while i < len(code):
+        c = code[i]
+        if c == "{":
+            header = code[seg:i]
+            if re.search(r"\bnamespace\b[\w\s]*$", header):
+                seg = i = i + 1
+                continue
+            end = match_brace(code, i)
+            name = function_name(header)
+            if name:
+                found.append((name, header, i, end))
+            seg = i = end + 1
+            continue
+        if c in ";}":
+            seg = i + 1
+        i += 1
+    return found
+
+
+def sources(csrc):
+    out = []
+    for f in sorted(os.listdir(csrc)):
+        if f.endswith((".cu", ".cuh")):
+            code, directives = strip_source(open(os.path.join(csrc, f)).read())
+            out.append((f, code, directives, functions(code)))
+    return out
+
+
+def enclosing(funcs, pos):
+    for name, _, b, e in funcs:
+        if b <= pos <= e:
+            return name
+    return None
+
+
+def line_of(code, pos):
+    return code.count("\n", 0, pos) + 1
+
+
+def violations(csrc):
+    """{rule: [offending site]} for rules 1-4 of this module's docstring."""
+    bad = {1: [], 2: [], 3: [], 4: []}
+    enters = 0
+    for f, code, directives, funcs in sources(csrc):
+        where = lambda pos: f"{f}:{line_of(code, pos)} ({enclosing(funcs, pos)})"
+        for m in re.finditer(r"<<<", code):
+            if enclosing(funcs, m.start()) != "gb_launch":
+                bad[1].append(where(m.start()))
+        for m in re.finditer(r"(->|\.)\s*launches\s*(\+\+|--|[-+]?=(?!=))|(\+\+|--)\s*[\w()]+\s*->\s*launches\b", code):
+            if enclosing(funcs, m.start()) not in COUNTER_WRITERS:
+                bad[2].append(where(m.start()))
+        for d in directives:
+            if re.search(r"\blaunches\b", d) and not re.match(r"\s*#\s*define\s+GB_CUB\(", d):
+                bad[2].append(f"{f}: {d.splitlines()[0].strip()}")
+            if re.search(r"\bGB_LOCK\s*\(|\bcudaSetDevice\s*\(", d) and not re.match(r"\s*#\s*define\s+(GB_ENTER|GB_LOCK)\(", d):
+                bad[4].append(f"{f}: {d.splitlines()[0].strip()}")
+        for m in re.finditer(r"\bcub\s*::\s*Device\w+\s*::\s*\w+", code):
+            through_wrapper = re.search(r"\bGB_CUB\s*\(\s*[^,;]+,\s*$", code[max(0, m.start() - 200):m.start()])
+            size_query = re.match(r"\s*\(\s*nullptr\s*,", code[m.end():])
+            if not (through_wrapper or size_query):
+                bad[3].append(where(m.start()))
+        for name, header, b, e in funcs:
+            if not re.match(r"\s*extern\s*\"\s*\"", header):
+                continue
+            params = header[header.index(name) + len(name):]
+            if not HANDLE_PARAM.search(params):
+                continue
+            if "GB_ENTER(" in code[b:e]:
+                enters += 1
+            elif name not in NO_ENTER:
+                bad[4].append(f"{f}: {name} does not enter through GB_ENTER")
+        for m in re.finditer(r"\bGB_LOCK\s*\(|\bcudaSetDevice\s*\(", code):
+            if enclosing(funcs, m.start()) not in LOCK_OR_DEVICE_BY_HAND:
+                bad[4].append(where(m.start()))
+    return bad, enters
+
+
+def parsed_inventory(csrc):
+    """Sanity numbers of the parse, so that a rule cannot pass because the parser found nothing."""
+    names, launches_in_helper, cub_calls = set(), 0, 0
+    for f, code, _, funcs in sources(csrc):
+        names.update(n for n, *_ in funcs)
+        launches_in_helper += sum(1 for m in re.finditer(r"<<<", code) if enclosing(funcs, m.start()) == "gb_launch")
+        cub_calls += len(re.findall(r"\bGB_CUB\s*\(", code))
+    return names, launches_in_helper, cub_calls
+
+
+def test_parser_sees_the_library():
+    names, launches_in_helper, cub_calls = parsed_inventory(CSRC)
+    assert {"gb_launch", "sweep_linearize", "gb_preprocess", "gb_vgicp_align", "gb_deskew", "knn_device", "table_build"} <= names
+    assert launches_in_helper == 1
+    assert cub_calls >= 10
+    _, enters = violations(CSRC)
+    assert enters >= 30
+
+
+def test_every_kernel_launch_goes_through_gb_launch():
+    assert violations(CSRC)[0][1] == []
+
+
+def test_launch_counter_written_only_by_the_helpers_and_the_graph_path():
+    assert violations(CSRC)[0][2] == []
+
+
+def test_every_cub_call_goes_through_gb_cub():
+    assert violations(CSRC)[0][3] == []
+
+
+def test_every_context_bound_entry_point_enters_its_context():
+    assert violations(CSRC)[0][4] == []
