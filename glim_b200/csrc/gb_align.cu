@@ -117,54 +117,47 @@ extern "C" gb_status gb_vgicp_align(gb_ctx* ctx, size_t P, const size_t* off, gb
   GB_CHECK(validate(P, off, factors, T_init, prm));
   const size_t F = off[P];
   GB_ENTER(ctx);
-  gb_sweep* s = nullptr;
-  GB_CHECK(gb_sweep_create(ctx, F, factors, nullptr, &s));
-  gb_status st = GB_OK;
-  auto finish = [&](gb_status e) { gb_sweep_destroy(s); return e; };  // the sweep's blocks go back to the context's pool
-  // device: states | offsets | status word;  pinned host: states | offsets | status word (the same layout)
-  const size_t b_st = sizeof(AlignState) * P, b_off = (sizeof(int) * (P + 1) + 15) / 16 * 16, bytes = b_st + b_off + 16;
-  char *d = nullptr, *h = nullptr;
-  if ((st = gb_ctx_scratch(ctx, bytes, (void**)&d)) != GB_OK) return finish(st);
-  if ((st = gb_ctx_pinned(ctx, std::max(bytes, sizeof(double) * 16 * F), (void**)&h)) != GB_OK) return finish(st);
-  AlignState* h_st = (AlignState*)h;
-  int* h_off = (int*)(h + b_st);
-  for (size_t p = 0; p < P; p++) align_init(h_st[p], T_init + 16 * p, prm->lambda_initial);
-  for (size_t p = 0; p <= P; p++) h_off[p] = (int)off[p];
-  AlignState* d_st = (AlignState*)d;
-  const int* d_off = (const int*)(d + b_st);
-  unsigned* d_ctr = (unsigned*)(d + b_st + b_off);
-  const unsigned* h_ctr = (const unsigned*)(h + b_st + b_off);
+  gb_sweep* sweep = nullptr;
+  GB_CHECK(gb_sweep_create(ctx, F, factors, nullptr, &sweep));
+  const gb_owned<gb_sweep> s(sweep, sweep_free);  // its blocks go back to the context's pool on every exit
+  // the same layout in scratch and in pinned staging: states | offsets | status word; the pinned side also stages the poses
+  struct Block { AlignState* st; int* off; unsigned* ctr; } d, h;
+  auto layout = [&](Carver& cv, Block& b) {
+    b.st = cv.take<AlignState>(P);
+    b.off = cv.take<int>(P + 1);
+    b.ctr = cv.take<unsigned>(2);
+  };
+  double* h_poses = nullptr;
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) { layout(cv, d); }));
+  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) {
+    layout(cv, h);
+    h_poses = cv.take<double>(16 * F);
+  }));
+  for (size_t p = 0; p < P; p++) align_init(h.st[p], T_init + 16 * p, prm->lambda_initial);
+  for (size_t p = 0; p <= P; p++) h.off[p] = (int)off[p];
+  for (size_t p = 0; p < P; p++)
+    for (size_t f = off[p]; f < off[p + 1]; f++) memcpy(h_poses + 16 * f, T_init + 16 * p, sizeof(double) * 16);
   cudaStream_t stream = ctx->stream;
-  cudaError_t e = cudaMemcpyAsync(d, h, b_st + b_off, cudaMemcpyHostToDevice, stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);  // the pinned buffer is reused for the poses below
-  if (e != cudaSuccess) { gb_set_error("align setup: %s", cudaGetErrorString(e)); return finish(GB_ERR_CUDA); }
-  {
-    double* hp = (double*)h;
-    for (size_t p = 0; p < P; p++)
-      for (size_t f = off[p]; f < off[p + 1]; f++) memcpy(hp + 16 * f, T_init + 16 * p, sizeof(double) * 16);
-    e = cudaMemcpyAsync(s->d_poses, hp, sizeof(double) * 16 * F, cudaMemcpyHostToDevice, stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_poses_eval, hp, sizeof(double) * 16 * F, cudaMemcpyHostToDevice, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    if (e != cudaSuccess) { gb_set_error("align setup: %s", cudaGetErrorString(e)); return finish(GB_ERR_CUDA); }
-  }
+  GB_CUDA(cudaMemcpyAsync(d.st, h.st, (char*)h.ctr - (char*)h.st, cudaMemcpyHostToDevice, stream));  // states and offsets
+  GB_CUDA(cudaMemcpyAsync(s->d_poses, h_poses, sizeof(double) * 16 * F, cudaMemcpyHostToDevice, stream));
+  GB_CUDA(cudaMemcpyAsync(s->d_poses_eval, h_poses, sizeof(double) * 16 * F, cudaMemcpyHostToDevice, stream));
+  GB_CUDA(cudaStreamSynchronize(stream));
   const int grid = (int)((P * 32 + kAlignThreads - 1) / kAlignThreads);
   bool need_lin = true;
   for (;;) {
-    if (need_lin && (st = gb_launch_sweep(s, GB_MODE_LINEARIZE)) != GB_OK) return finish(st);
-    if ((st = gb_launch(ctx, "k_align_step", k_align_step, grid, kAlignThreads, 0, d_st, d_off, (int)P, s->d_out, s->d_poses_eval, d_ctr)) != GB_OK) return finish(st);
-    if ((st = gb_launch_sweep(s, GB_MODE_ERROR)) != GB_OK) return finish(st);
-    if ((st = gb_launch(ctx, "k_align_accept", k_align_accept, grid, kAlignThreads, 0, d_st, d_off, (int)P, s->d_out, s->d_poses, *prm, d_ctr)) != GB_OK) return finish(st);
-    e = cudaMemcpyAsync((void*)h_ctr, d_ctr, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    if (e != cudaSuccess) { gb_set_error("align round: %s", cudaGetErrorString(e)); return finish(GB_ERR_CUDA); }
-    if (h_ctr[0] == 0) break;
-    need_lin = h_ctr[1] > 0;
+    if (need_lin) GB_CHECK(gb_launch_sweep(s.get(), GB_MODE_LINEARIZE));
+    GB_CHECK(gb_launch(ctx, "k_align_step", k_align_step, grid, kAlignThreads, 0, d.st, d.off, (int)P, s->d_out, s->d_poses_eval, d.ctr));
+    GB_CHECK(gb_launch_sweep(s.get(), GB_MODE_ERROR));
+    GB_CHECK(gb_launch(ctx, "k_align_accept", k_align_accept, grid, kAlignThreads, 0, d.st, d.off, (int)P, s->d_out, s->d_poses, *prm, d.ctr));
+    GB_CUDA(cudaMemcpyAsync(h.ctr, d.ctr, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+    GB_CUDA(cudaStreamSynchronize(stream));
+    if (h.ctr[0] == 0) break;
+    need_lin = h.ctr[1] > 0;
   }
-  e = cudaMemcpyAsync(h_st, d_st, b_st, cudaMemcpyDeviceToHost, stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-  if (e != cudaSuccess) { gb_set_error("align results: %s", cudaGetErrorString(e)); return finish(GB_ERR_CUDA); }
+  GB_CUDA(cudaMemcpyAsync(h.st, d.st, sizeof(AlignState) * P, cudaMemcpyDeviceToHost, stream));
+  GB_CUDA(cudaStreamSynchronize(stream));
   for (size_t p = 0; p < P; p++) {
-    const AlignState& a = h_st[p];
+    const AlignState& a = h.st[p];
     gb_align_result& r = results[p];
     memcpy(r.T_target_source, a.T, sizeof(double) * 16);
     r.error = a.e;
@@ -174,5 +167,5 @@ extern "C" gb_status gb_vgicp_align(gb_ctx* ctx, size_t P, const size_t* off, gb
     r.trials = a.trials;
     r.status = a.status;
   }
-  return finish(GB_OK);
+  return GB_OK;
 }

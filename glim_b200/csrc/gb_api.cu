@@ -109,7 +109,7 @@ void gb_dev_free(int device, void* p) {
     if (it != P.live.end()) { cap = it->second; P.live.erase(it); }
     for (gb_ctx* c : P.ctxs) streams.push_back(c->stream);
   }
-  if (cap == 0 || getenv("GB_NO_POOL")) { cudaFree(p); return; }
+  if (cap == 0) { cudaFree(p); return; }
   for (cudaStream_t st : streams) cudaStreamSynchronize(st);  // nobody may still be reading the block (cudaFree's implicit guarantee)
   std::lock_guard<std::mutex> lock(P.mu);
   if (P.free_bytes + cap > kPoolMaxFreeBytes) { cudaFree(p); return; }
@@ -120,6 +120,7 @@ void gb_dev_free(int device, void* p) {
 // ---------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------
+static void ctx_release(gb_ctx* ctx);
 static gb_status ctx_create(int device, cudaStream_t stream, bool own, gb_ctx** out) {
   GB_REQUIRE(out, "null output");
   *out = nullptr;
@@ -135,29 +136,31 @@ static gb_status ctx_create(int device, cudaStream_t stream, bool own, gb_ctx** 
     gb_set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     return GB_ERR_NO_DEVICE;
   }
-  gb_ctx* c = new (std::nothrow) gb_ctx();
+  gb_owned<gb_ctx> c(new (std::nothrow) gb_ctx(), ctx_release);
   if (!c) return GB_ERR_INTERNAL;
+  c->refs.store(1);
   c->device = device;
-  c->own_stream = own;
   c->stream = stream;
   if (own) {
-    cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) { delete c; gb_set_error("cudaStreamCreate: %s", cudaGetErrorString(e)); return GB_ERR_CUDA; }
+    GB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+    c->own_stream = true;
   }
   c->num_sms = prop.multiProcessorCount;
-  c->refs.store(1);
-  { DevPool& P = g_pools[device & 15]; std::lock_guard<std::mutex> lock(P.mu); P.ctxs.push_back(c); }
-  *out = c;
+  { DevPool& P = g_pools[device & 15]; std::lock_guard<std::mutex> lock(P.mu); P.ctxs.push_back(c.get()); }
+  *out = c.release();
   return GB_OK;
 }
 extern "C" gb_status gb_ctx_create(int device, gb_ctx** out) { return ctx_create(device, nullptr, true, out); }
 extern "C" gb_status gb_ctx_create_on_stream(int device, void* cuda_stream, gb_ctx** out) { return ctx_create(device, (cudaStream_t)cuda_stream, false, out); }
 
-static void sweep_free(gb_sweep* s);
-
 // Cross links factor <-> sweep (a factor may sit in cached sweeps of several contexts): guarded by one registry mutex.
 static std::mutex g_registry_mu;
 static std::atomic<uint64_t> g_next_factor_id{1};
+
+static void pool_block_free(const gb_pool_block& b) {
+  if (b.d) cudaFree(b.d);
+  if (b.h) cudaFreeHost(b.h);
+}
 
 // Contexts are reference counted: factors, sweeps and peer slabs hold one; gb_ctx_destroy drops the owner's.  A module may
 // therefore destroy its CUDAStream while factors created on it are still alive (member destruction order, thread exit).
@@ -167,10 +170,9 @@ static void ctx_release(gb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   { DevPool& P = g_pools[ctx->device & 15]; std::lock_guard<std::mutex> lock(P.mu); P.ctxs.erase(std::remove(P.ctxs.begin(), P.ctxs.end(), ctx), P.ctxs.end()); }
-  for (gb_pool_block& b : ctx->pool) { if (b.d) cudaFree(b.d); if (b.h) cudaFreeHost(b.h); }
-  ctx->pool.clear();
-  if (ctx->scratch) cudaFree(ctx->scratch);
-  if (ctx->pinned) cudaFreeHost(ctx->pinned);
+  for (const gb_pool_block& b : ctx->pool) pool_block_free(b);
+  if (ctx->scratch.base) cudaFree(ctx->scratch.base);
+  if (ctx->pinned.base) cudaFreeHost(ctx->pinned.base);
   if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
 }
@@ -196,28 +198,15 @@ extern "C" gb_status gb_ctx_synchronize(gb_ctx* ctx) {
 extern "C" void* gb_ctx_stream(gb_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
 extern "C" uint64_t gb_ctx_kernel_launches(gb_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
-gb_status gb_ctx_scratch(gb_ctx* ctx, size_t bytes, void** out) {
-  if (bytes > ctx->scratch_cap) {
-    GB_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (ctx->scratch) GB_CUDA(cudaFree(ctx->scratch));
-    ctx->scratch = nullptr; ctx->scratch_cap = 0;
-    const size_t cap = bytes + bytes / 4;
-    GB_CUDA(cudaMalloc(&ctx->scratch, cap));
-    ctx->scratch_cap = cap;
-  }
-  *out = ctx->scratch;
-  return GB_OK;
-}
-gb_status gb_ctx_pinned(gb_ctx* ctx, size_t bytes, void** out) {
-  if (bytes > ctx->pinned_cap) {
-    GB_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (ctx->pinned) GB_CUDA(cudaFreeHost(ctx->pinned));
-    ctx->pinned = nullptr; ctx->pinned_cap = 0;
-    const size_t cap = bytes + bytes / 4;
-    GB_CUDA(cudaMallocHost(&ctx->pinned, cap));
-    ctx->pinned_cap = cap;
-  }
-  *out = ctx->pinned;
+gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes) {
+  if (bytes <= a.cap) return GB_OK;
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (a.base) GB_CUDA(a.host ? cudaFreeHost(a.base) : cudaFree(a.base));
+  a.base = nullptr;
+  a.cap = 0;
+  const size_t cap = bytes + bytes / 4;
+  GB_CUDA(a.host ? cudaMallocHost(&a.base, cap) : cudaMalloc(&a.base, cap));
+  a.cap = cap;
   return GB_OK;
 }
 
@@ -226,13 +215,19 @@ gb_status gb_ctx_pinned(gb_ctx* ctx, size_t bytes, void** out) {
 // ---------------------------------------------------------------------------------------------
 // the reference casts Vector4d / Matrix4d to float on the host before the copy (SURVEY K1); so do we, straight into the
 // plane layout in pinned memory, then stage the planes in scratch and Morton-sort them into the cloud on the device
+// (the caller has made the cloud's device current)
+static void cloud_free(gb_cloud* c) {
+  gb_dev_free(c->device, c->base);  // waits for every stream that may still read the cloud, then recycles the block
+  delete c;
+}
+
 static gb_status cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, const double* cov4x4, const double* normals4, gb_cloud* c) {
-  Carver size;
-  gb_cloud_planes(size, n, normals4 != nullptr);
-  const size_t planes_b = size.off;
-  Carver hc;
-  GB_CHECK(gb_ctx_pinned(ctx, planes_b, (void**)&hc.base));
-  const gb_planes h = gb_cloud_planes(hc, n, normals4 != nullptr);
+  gb_planes h;
+  size_t planes_b = 0;
+  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) {
+    h = gb_cloud_planes(cv, n, normals4 != nullptr);
+    planes_b = cv.off;
+  }));
   // fp64 -> fp32 cast straight into the plane layout; split over a few host threads for large clouds (the single-threaded
   // loop was 1.6 ms for 60 k points and 25 ms for 500 k: more than everything the GPU does per frame)
   auto pack = [&](size_t i0, size_t i1) {
@@ -265,7 +260,7 @@ static gb_status cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, const d
   const size_t cub_b = gb_cub_temp_bytes(n);
   gb_planes staged;
   gb_sort_tmp t;
-  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     staged = gb_cloud_planes(cv, n, normals4 != nullptr);
     t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
   }));
@@ -281,12 +276,11 @@ extern "C" gb_status gb_cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, 
   GB_REQUIRE(n < (size_t)1 << 30, "too many points");
   *out = nullptr;
   GB_ENTER(ctx);
-  gb_cloud* c = new (std::nothrow) gb_cloud();
+  gb_owned<gb_cloud> c(new (std::nothrow) gb_cloud(), cloud_free);
   if (!c) return GB_ERR_INTERNAL;
   c->device = ctx->device;
-  const gb_status st = n > 0 ? cloud_upload(ctx, n, xyzw, cov4x4, normals4, c) : GB_OK;
-  if (st != GB_OK) { gb_dev_free(ctx->device, c->base); delete c; return st; }
-  *out = c;
+  if (n > 0) GB_CHECK(cloud_upload(ctx, n, xyzw, cov4x4, normals4, c.get()));
+  *out = c.release();
   return GB_OK;
 }
 extern "C" gb_status gb_cloud_size(const gb_cloud* cloud, size_t* n) {
@@ -323,14 +317,20 @@ extern "C" gb_status gb_cloud_device_ptrs(const gb_cloud* c, void** p0, void** p
 extern "C" gb_status gb_cloud_destroy(gb_cloud* c) {
   if (!c) return GB_OK;
   cudaSetDevice(c->device);
-  gb_dev_free(c->device, c->base);  // waits for every stream that may still read the cloud, then recycles the block
-  delete c;
+  cloud_free(c);
   return GB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
 // voxel maps
 // ---------------------------------------------------------------------------------------------
+// (the caller has made the map's device current)
+static void voxelmap_free(gb_voxelmap* m) {
+  gb_dev_free(m->device, m->base);
+  gb_dev_free(m->device, m->buckets);
+  delete m;
+}
+
 extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_num_buckets, int max_bucket_scan_count, double target_points_drop_rate, gb_voxelmap** out) {
   GB_REQUIRE(ctx && cloud && out, "null argument");
   GB_REQUIRE(resolution > 0.f, "resolution must be positive");
@@ -338,16 +338,10 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
   GB_REQUIRE(max_bucket_scan_count > 0, "max_bucket_scan_count must be positive");
   *out = nullptr;
   GB_ENTER(ctx);
-  gb_voxelmap* m = new (std::nothrow) gb_voxelmap();
+  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(), voxelmap_free);
   if (!m) return GB_ERR_INTERNAL;
-  gb_status st = gb_voxelmap_build_impl(ctx, cloud, resolution, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, m);
-  if (st != GB_OK) {
-    gb_dev_free(ctx->device, m->base);
-    gb_dev_free(ctx->device, m->buckets);
-    delete m;
-    return st;
-  }
-  *out = m;
+  GB_CHECK(gb_voxelmap_build_impl(ctx, cloud, resolution, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, m.get()));
+  *out = m.release();
   return GB_OK;
 }
 extern "C" gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolution, int init_num_buckets, int max_bucket_scan_count, double target_points_drop_rate,
@@ -359,7 +353,7 @@ extern "C" gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolutio
   GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
   *out = nullptr;
   GB_ENTER(ctx);
-  gb_voxelmap* m = new (std::nothrow) gb_voxelmap();
+  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(), voxelmap_free);
   if (!m) return GB_ERR_INTERNAL;
   m->resolution = resolution;
   m->inv_res = 1.0f / resolution;
@@ -368,13 +362,8 @@ extern "C" gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolutio
   m->drop_rate = target_points_drop_rate;
   m->lru_horizon = lru_horizon;
   m->lru_clear_cycle = lru_clear_cycle;
-  gb_status st = gb_voxelmap_create_incremental_impl(ctx, m);
-  if (st != GB_OK) {
-    gb_dev_free(ctx->device, m->buckets);
-    delete m;
-    return st;
-  }
-  *out = m;
+  GB_CHECK(gb_voxelmap_create_incremental_impl(ctx, m.get()));
+  *out = m.release();
   return GB_OK;
 }
 extern "C" gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
@@ -415,9 +404,7 @@ extern "C" gb_status gb_voxelmap_download(const gb_voxelmap* m, int32_t* buckets
 extern "C" gb_status gb_voxelmap_destroy(gb_voxelmap* m) {
   if (!m) return GB_OK;
   cudaSetDevice(m->device);
-  gb_dev_free(m->device, m->base);
-  gb_dev_free(m->device, m->buckets);
-  delete m;
+  voxelmap_free(m);
   return GB_OK;
 }
 
@@ -433,23 +420,22 @@ extern "C" gb_status gb_vgicp_factor_create(gb_ctx* ctx, const gb_voxelmap* targ
     GB_REQUIRE(source->normals != nullptr, "surface validation needs the source frame's normals on the device (PointCloudGPU::clone of a frame that has normals)");
   gb_factor* f = new (std::nothrow) gb_factor();
   if (!f) return GB_ERR_INTERNAL;
-  f->ctx = ctx; f->target = target; f->source = source; f->flags = flags; f->single = nullptr; f->inlier_frac = -1.f; f->id = g_next_factor_id.fetch_add(1);
+  f->ctx = ctx; f->target = target; f->source = source; f->flags = flags; f->id = g_next_factor_id.fetch_add(1);
   ctx_retain(ctx);
   *out = f;
   return GB_OK;
 }
 
 // return a retired sweep's blocks to its context's pool (the caller holds the context lock and has drained the stream)
-static void pool_put(gb_ctx* ctx, void* d, size_t d_cap, void* h, size_t h_cap) {
-  if (!d && !h) return;
+static void pool_put(gb_ctx* ctx, const gb_pool_block& b) {
+  if (!b.d || !b.h) { pool_block_free(b); return; }  // no block, or half of one (its pinned allocation failed): not kept
   if (ctx->pool.size() >= 64) {  // bounded: drop the smallest block
     size_t k = 0;
     for (size_t i = 1; i < ctx->pool.size(); i++) if (ctx->pool[i].d_cap < ctx->pool[k].d_cap) k = i;
-    if (ctx->pool[k].d) cudaFree(ctx->pool[k].d);
-    if (ctx->pool[k].h) cudaFreeHost(ctx->pool[k].h);
+    pool_block_free(ctx->pool[k]);
     ctx->pool.erase(ctx->pool.begin() + k);
   }
-  ctx->pool.push_back({d, d_cap, h, h_cap});
+  ctx->pool.push_back(b);
 }
 static bool pool_get(gb_ctx* ctx, size_t d_need, size_t h_need, gb_pool_block* out) {
   int best = -1;
@@ -463,7 +449,7 @@ static bool pool_get(gb_ctx* ctx, size_t d_need, size_t h_need, gb_pool_block* o
   return true;
 }
 
-static void sweep_free(gb_sweep* s) {
+void sweep_free(gb_sweep* s) {
   if (!s) return;
   gb_ctx* ctx = s->ctx;
   {
@@ -481,7 +467,7 @@ static void sweep_free(gb_sweep* s) {
     for (int k = 0; k < 2; k++) if (s->pose_ev[k]) cudaEventDestroy(s->pose_ev[k]);
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
     if (s->d_pair_ptr) cudaFree(s->d_pair_ptr);
-    pool_put(ctx, s->pool_d, s->pool_d_cap, s->pool_h, s->pool_h_cap);
+    pool_put(ctx, s->blk);
     delete s;
   }
   ctx_release(ctx);
@@ -645,6 +631,29 @@ static gb_status sweep_follow_targets(gb_sweep* s) {
   return GB_OK;
 }
 
+// The sweep's device and pinned blocks (a pooled block may be larger than this layout measures).  The accumulators, tickets
+// and queue head are adjacent: one memset zeroes them at creation, over the byte count returned.
+static size_t sweep_layout(gb_sweep* s, Carver& d, Carver& h) {
+  const size_t F = s->F;
+  s->d_descs = d.take<FactorDesc>(F);
+  s->d_tiles = d.take<int2>(s->tiles_cap);
+  s->d_poses = d.take<double>(16 * F);
+  s->d_poses_eval = d.take<double>(16 * F);
+  const size_t zero_from = d.off;
+  s->d_accum = d.take<double>(GB_ACC_STRIDE * F * s->acc_slots);
+  s->d_done = d.take<unsigned>(F);
+  s->d_tile_ctr = d.take<unsigned long long>(1);
+  const size_t zero_bytes = d.off - zero_from;
+  s->d_out = d.take<double>(GB_OUT_DOUBLES * F);
+  s->h_pose_slot[0] = h.take<double>(16 * F);
+  s->h_pose_slot[1] = h.take<double>(16 * F);
+  s->h_poses_eval = h.take<double>(16 * F);
+  s->h_out = h.take<double>(GB_OUT_DOUBLES * F);
+  s->h_descs = h.take<FactorDesc>(F);
+  s->h_tiles = h.take<int2>(s->tiles_cap);
+  return zero_bytes;
+}
+
 extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* factors, const int32_t* pair_index, gb_sweep** out) {
   GB_REQUIRE(ctx && out, "null argument");
   GB_REQUIRE(F == 0 || factors, "null factor list");
@@ -657,7 +666,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     total_pts += factors[f]->source->n;
   }
   GB_ENTER(ctx);
-  gb_sweep* s = new (std::nothrow) gb_sweep();
+  gb_owned<gb_sweep> s(new (std::nothrow) gb_sweep(), sweep_free);
   if (!s) return GB_ERR_INTERNAL;
   ctx_retain(ctx);
   s->ctx = ctx; s->F = F; s->factors.assign(factors, factors + F);
@@ -703,7 +712,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     s->algorithmic_bytes += factor_bytes(fa);
   }
   s->any_sv = any_sv;
-  build_items(s, descs.data(), tiles);
+  build_items(s.get(), descs.data(), tiles);
   s->num_tiles = (int)tiles.size();
   s->grid = std::max(1, std::min((s->num_tiles + 7) / 8, s->capacity));
   // ~64 items per accumulator copy: sweeps with few factors (an odometry frame, a single pair) would otherwise
@@ -714,49 +723,31 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   if (F > 0) {
     // one device block, one pinned block -- taken from the context's pool when a retired sweep left a fitting one
     s->tiles_cap = std::max<size_t>(tiles.size(), s->kernel_version == 5 ? (size_t)warps + F : 0);
-    const size_t b_desc = align_up(sizeof(FactorDesc) * F, 256), b_tiles = align_up(sizeof(int2) * s->tiles_cap, 256), b_pose = align_up(sizeof(double) * 16 * F, 256);
-    const size_t b_acc = align_up(sizeof(double) * GB_ACC_STRIDE * F * s->acc_slots, 256), b_done = align_up(sizeof(unsigned) * F + 16, 256), b_out = align_up(sizeof(double) * GB_OUT_DOUBLES * F, 256);
-    const size_t total = b_desc + b_tiles + 2 * b_pose + b_acc + b_done + b_out;
-    const size_t h_total = 3 * b_pose + b_out + b_desc + b_tiles;
-    gb_pool_block blk{nullptr, 0, nullptr, 0};
-    if (!pool_get(ctx, total, h_total, &blk)) {
-      cudaError_t e = cudaMalloc(&blk.d, total);
-      if (e != cudaSuccess) { delete s; ctx_release(ctx); gb_set_error("cudaMalloc(%zu): %s", total, cudaGetErrorString(e)); return GB_ERR_OUT_OF_MEMORY; }
-      blk.d_cap = total;
-      e = cudaMallocHost(&blk.h, h_total);
-      if (e != cudaSuccess) { cudaFree(blk.d); delete s; ctx_release(ctx); gb_set_error("cudaMallocHost: %s", cudaGetErrorString(e)); return GB_ERR_OUT_OF_MEMORY; }
-      blk.h_cap = h_total;
+    Carver d, h;
+    sweep_layout(s.get(), d, h);
+    if (!pool_get(ctx, d.off, h.off, &s->blk)) {
+      GB_CUDA(cudaMalloc(&s->blk.d, d.off));
+      s->blk.d_cap = d.off;
+      GB_CUDA(cudaMallocHost(&s->blk.h, h.off));
+      s->blk.h_cap = h.off;
     }
-    s->pool_d = blk.d; s->pool_d_cap = blk.d_cap; s->pool_h = blk.h; s->pool_h_cap = blk.h_cap;
-    char* d = (char*)blk.d;
-    s->d_descs = (FactorDesc*)d; d += b_desc;
-    s->d_tiles = (int2*)d; d += b_tiles;
-    s->d_poses = (double*)d; d += b_pose;
-    s->d_poses_eval = (double*)d; d += b_pose;
-    s->d_accum = (double*)d; d += b_acc;
-    s->d_done = (unsigned*)d;
-    s->d_tile_ctr = (unsigned long long*)(d + align_up(sizeof(unsigned) * F, 8));
-    d += b_done;
-    s->d_out = (double*)d;
-    char* h = (char*)blk.h;
-    s->h_pose_slot[0] = (double*)h; s->h_pose_slot[1] = (double*)(h + b_pose); s->h_poses_eval = (double*)(h + 2 * b_pose); s->h_out = (double*)(h + 3 * b_pose);
-    s->h_descs = (FactorDesc*)(h + 3 * b_pose + b_out);
-    s->h_tiles = (int2*)(h + 3 * b_pose + b_out + b_desc);
+    d = Carver{(char*)s->blk.d};
+    h = Carver{(char*)s->blk.h};
+    const size_t zero_bytes = sweep_layout(s.get(), d, h);
     memcpy(s->h_descs, descs.data(), sizeof(FactorDesc) * F);
     memcpy(s->h_tiles, tiles.data(), sizeof(int2) * tiles.size());
     cudaStream_t st = ctx->stream;
-    cudaError_t e = cudaMemcpyAsync(s->d_descs, s->h_descs, sizeof(FactorDesc) * F, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_tiles, s->h_tiles, sizeof(int2) * tiles.size(), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(s->d_accum, 0, b_acc + b_done, st);
-    for (int k = 0; k < 2 && e == cudaSuccess; k++) e = cudaEventCreateWithFlags(&s->pose_ev[k], cudaEventDisableTiming);
-    if (e != cudaSuccess) { sweep_free(s); gb_set_error("sweep setup: %s", cudaGetErrorString(e)); return GB_ERR_CUDA; }
+    GB_CUDA(cudaMemcpyAsync(s->d_descs, s->h_descs, sizeof(FactorDesc) * F, cudaMemcpyHostToDevice, st));
+    GB_CUDA(cudaMemcpyAsync(s->d_tiles, s->h_tiles, sizeof(int2) * tiles.size(), cudaMemcpyHostToDevice, st));
+    GB_CUDA(cudaMemsetAsync(s->d_accum, 0, zero_bytes, st));
+    for (int k = 0; k < 2; k++) GB_CUDA(cudaEventCreateWithFlags(&s->pose_ev[k], cudaEventDisableTiming));
     // no synchronisation: the staging lives in the sweep's own pinned block, and everything that follows is stream ordered
   }
   {
     std::lock_guard<std::mutex> reg(g_registry_mu);
-    for (gb_factor* f : s->factors) f->users.push_back(s);
+    for (gb_factor* f : s->factors) f->users.push_back(s.get());
   }
-  *out = s;
+  *out = s.release();
   return GB_OK;
 }
 extern "C" gb_status gb_sweep_destroy(gb_sweep* s) { sweep_free(s); return GB_OK; }
@@ -783,17 +774,22 @@ extern "C" gb_status gb_sweep_set_poses(gb_sweep* s, const double* T) {
   GB_CUDA(cudaEventRecord(s->pose_ev[k], s->ctx->stream));
   return GB_OK;
 }
-static gb_status sweep_set_eval_poses(gb_sweep* s, const double* T) {
-  if (s->F == 0) return GB_OK;
-  // the eval poses are only used by the blocking error calls (each ends with a stream sync): single buffer is safe
-  memcpy(s->h_poses_eval, T, sizeof(double) * 16 * s->F);
-  GB_CUDA(cudaMemcpyAsync(s->d_poses_eval, s->h_poses_eval, sizeof(double) * 16 * s->F, cudaMemcpyHostToDevice, s->ctx->stream));
-  return GB_OK;
-}
 static gb_status sweep_launch(gb_sweep* s, int mode) {
   if (s->stale) { gb_set_error("a factor of this sweep has been destroyed"); return GB_ERR_INVALID_ARGUMENT; }
   GB_CHECK(sweep_follow_targets(s));
   return gb_launch_sweep(s, mode);
+}
+// errors[f] = factor f's error at T_eval[f], with its correspondences found at T_lin[f] (F > 0)
+static gb_status sweep_error(gb_sweep* s, const double* T_lin, const double* T_eval, double* errors) {
+  GB_CHECK(gb_sweep_set_poses(s, T_lin));
+  // the eval poses are only used by this blocking call (it ends with a stream sync): single buffer is safe
+  memcpy(s->h_poses_eval, T_eval, sizeof(double) * 16 * s->F);
+  GB_CUDA(cudaMemcpyAsync(s->d_poses_eval, s->h_poses_eval, sizeof(double) * 16 * s->F, cudaMemcpyHostToDevice, s->ctx->stream));
+  GB_CHECK(sweep_launch(s, GB_MODE_ERROR));
+  GB_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(double) * GB_OUT_DOUBLES * s->F, cudaMemcpyDeviceToHost, s->ctx->stream));
+  GB_CUDA(cudaStreamSynchronize(s->ctx->stream));
+  for (size_t f = 0; f < s->F; f++) errors[f] = s->h_out[f * GB_OUT_DOUBLES + 120];
+  return GB_OK;
 }
 extern "C" gb_status gb_sweep_launch(gb_sweep* s) {
   GB_REQUIRE(s, "null sweep");
@@ -919,13 +915,7 @@ extern "C" gb_status gb_factor_set_error(gb_ctx* ctx, size_t F, gb_factor* const
   GB_ENTER(ctx);
   gb_sweep* s = nullptr;
   GB_CHECK(cached_sweep(ctx, F, factors, &s));
-  GB_CHECK(gb_sweep_set_poses(s, T_lin));
-  GB_CHECK(sweep_set_eval_poses(s, T_eval));
-  GB_CHECK(sweep_launch(s, GB_MODE_ERROR));
-  GB_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(double) * GB_OUT_DOUBLES * F, cudaMemcpyDeviceToHost, ctx->stream));
-  GB_CUDA(cudaStreamSynchronize(ctx->stream));
-  for (size_t f = 0; f < F; f++) errors[f] = s->h_out[f * GB_OUT_DOUBLES + 120];
-  return GB_OK;
+  return sweep_error(s, T_lin, T_eval, errors);
 }
 
 static gb_status single_sweep(gb_factor* f, gb_sweep** out) {
@@ -945,13 +935,7 @@ extern "C" gb_status gb_vgicp_error(gb_factor* f, const double T_lin[16], const 
   GB_ENTER(f->ctx);
   gb_sweep* s = nullptr;
   GB_CHECK(single_sweep(f, &s));
-  GB_CHECK(gb_sweep_set_poses(s, T_lin));
-  GB_CHECK(sweep_set_eval_poses(s, T_eval));
-  GB_CHECK(sweep_launch(s, GB_MODE_ERROR));
-  GB_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(double) * GB_OUT_DOUBLES, cudaMemcpyDeviceToHost, f->ctx->stream));
-  GB_CUDA(cudaStreamSynchronize(f->ctx->stream));
-  *error = s->h_out[120];
-  return GB_OK;
+  return sweep_error(s, T_lin, T_eval, error);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -991,8 +975,20 @@ extern "C" gb_status gb_slab_row_hessian_blocks(const float* row, double error_s
 // ---------------------------------------------------------------------------------------------
 // fused multi-GPU result exchange (peer slabs over CUDA IPC)
 // ---------------------------------------------------------------------------------------------
-static size_t peer_alloc_bytes(size_t num_pairs, int world) {
-  return 2 * align_up(num_pairs * GB_SLAB_STRIDE * sizeof(float), 256) + align_up(sizeof(unsigned) * (size_t)world, 256);
+static void peer_slab_free(gb_peer_slab* ps) {
+  gb_ctx* ctx = ps->ctx;
+  {
+    GB_LOCK(ctx);
+    cudaSetDevice(ctx->device);
+    cudaStreamSynchronize(ctx->stream);
+    for (int p = 0; p < ps->world; p++)
+      if (ps->opened[p]) cudaIpcCloseMemHandle(ps->peer[p]);
+    if (ps->local) cudaFree(ps->local);
+    if (ps->d_my_pairs) cudaFree(ps->d_my_pairs);
+    if (ps->h_pinned) cudaFreeHost(ps->h_pinned);
+    delete ps;
+  }
+  ctx_release(ctx);  // outside the lock: it may delete the context
 }
 
 extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int world, int rank, gb_peer_slab** out) {
@@ -1001,10 +997,10 @@ extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int worl
   GB_REQUIRE(num_pairs > 0, "num_pairs must be positive");
   *out = nullptr;
   GB_ENTER(ctx);
-  gb_peer_slab* ps = new (std::nothrow) gb_peer_slab();
+  gb_owned<gb_peer_slab> ps(new (std::nothrow) gb_peer_slab(), peer_slab_free);
   if (!ps) return GB_ERR_INTERNAL;
+  ctx_retain(ctx);
   ps->ctx = ctx; ps->num_pairs = num_pairs; ps->world = world; ps->rank = rank;
-  ps->buf_floats = align_up(num_pairs * GB_SLAB_STRIDE * sizeof(float), 256) / sizeof(float);
   ps->connected = (world == 1);
   // fused: the sweep's epilogue stores every finished row straight into all peers; deferred: rows go to the local buffer and
   // the exchange kernel pushes them (see gb_launch_peer_signal_wait).  The peer stores' cost to the sweep grows with the
@@ -1015,18 +1011,14 @@ extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int worl
     if (e && !strcmp(e, "fused")) ps->deferred = false;
     if (e && !strcmp(e, "deferred")) ps->deferred = true;
   }
-  const size_t bytes = peer_alloc_bytes(num_pairs, world);
-  cudaError_t e = cudaMalloc((void**)&ps->local, bytes + 256);
-  if (e != cudaSuccess) { delete ps; gb_set_error("cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e)); return GB_ERR_OUT_OF_MEMORY; }
-  e = cudaMemsetAsync(ps->local, 0, bytes + 256, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) { cudaFree(ps->local); delete ps; gb_set_error("peer slab init: %s", cudaGetErrorString(e)); return GB_ERR_CUDA; }
-  ps->d_timeout = (int*)(ps->local + bytes);
+  Carver size;
+  gb_peer_layout(size, num_pairs, world);
+  GB_CUDA(cudaMalloc((void**)&ps->local, size.off));
   ps->peer[rank] = ps->local;
-  e = cudaMallocHost((void**)&ps->h_pinned, num_pairs * GB_SLAB_STRIDE * sizeof(float) + 64);
-  if (e != cudaSuccess) { cudaFree(ps->local); delete ps; gb_set_error("cudaMallocHost: %s", cudaGetErrorString(e)); return GB_ERR_OUT_OF_MEMORY; }
-  ctx_retain(ctx);
-  *out = ps;
+  GB_CUDA(cudaMemsetAsync(ps->local, 0, size.off, ctx->stream));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  GB_CUDA(cudaMallocHost((void**)&ps->h_pinned, num_pairs * GB_SLAB_STRIDE * sizeof(float) + 64));
+  *out = ps.release();
   return GB_OK;
 }
 
@@ -1057,19 +1049,19 @@ extern "C" gb_status gb_peer_slab_connect(gb_peer_slab* ps, const void* handles)
 }
 
 extern "C" gb_status gb_peer_slab_destroy(gb_peer_slab* ps) {
-  if (!ps) return GB_OK;
-  gb_ctx* ctx = ps->ctx;
-  {
-    GB_ENTER(ctx);
-    cudaStreamSynchronize(ctx->stream);
-    for (int p = 0; p < ps->world; p++)
-      if (ps->opened[p]) cudaIpcCloseMemHandle(ps->peer[p]);
-    if (ps->local) cudaFree(ps->local);
-    if (ps->d_my_pairs) cudaFree(ps->d_my_pairs);
-    if (ps->h_pinned) cudaFreeHost(ps->h_pinned);
-    delete ps;
-  }
-  ctx_release(ctx);  // outside the lock: it may delete the context
+  if (ps) peer_slab_free(ps);
+  return GB_OK;
+}
+
+// Replaces the device block *block (nullptr: none yet; the stream has drained) with a fresh cudaMalloc block of the layout.
+// *block is the layout's first array: measuring sets it to nullptr, so it never points at a freed block.
+template <typename Layout> static gb_status dev_block_realloc(void** block, Layout&& layout) {
+  if (*block) GB_CUDA(cudaFree(*block));
+  Carver size;
+  layout(size);
+  Carver cv;
+  GB_CUDA(cudaMalloc((void**)&cv.base, size.off));
+  layout(cv);
   return GB_OK;
 }
 
@@ -1088,39 +1080,36 @@ extern "C" gb_status gb_sweep_attach_peer_slab(gb_sweep* s, gb_peer_slab* ps) {
   for (size_t k = 0; k < P; k++) ptr[k + 1] += ptr[k];
   std::vector<int> fill(ptr.begin(), ptr.end() - 1);
   for (size_t f = 0; f < s->F; f++) fac[fill[s->h_pair[f]]++] = (int)f;
+  // the pairs this sweep owns (one sweep per peer slab): the rows the exchange kernel copies to the peers
+  std::vector<int> mine;
+  for (size_t k = 0; k < P; k++) if (ptr[k + 1] > ptr[k]) mine.push_back((int)k);
   GB_ENTER(s->ctx);
   GB_CUDA(cudaStreamSynchronize(s->ctx->stream));
-  if (s->d_pair_ptr) { GB_CUDA(cudaFree(s->d_pair_ptr)); s->d_pair_ptr = nullptr; }
-  const size_t b_ptr = align_up(sizeof(int) * (P + 1), 256), b_fac = align_up(sizeof(int) * std::max<size_t>(1, s->F), 256), b_done = align_up(sizeof(unsigned) * P, 256);
-  char* d = nullptr;
-  GB_CUDA(cudaMalloc((void**)&d, b_ptr + b_fac + b_done + 2 * sizeof(PeerPush)));
-  s->d_pair_ptr = (int*)d; s->d_pair_factors = (int*)(d + b_ptr); s->d_pair_done = (unsigned*)(d + b_ptr + b_fac);
-  s->d_peer_tables = (PeerPush*)(d + b_ptr + b_fac + b_done);
+  GB_CHECK(dev_block_realloc((void**)&s->d_pair_ptr, [&](Carver& cv) {
+    s->d_pair_ptr = cv.take<int>(P + 1);
+    s->d_pair_factors = cv.take<int>(std::max<size_t>(1, s->F));
+    s->d_pair_done = cv.take<unsigned>(P);
+    s->d_peer_tables = cv.take<PeerPush>(2);
+  }));
+  GB_CHECK(dev_block_realloc((void**)&ps->d_my_pairs, [&](Carver& cv) { ps->d_my_pairs = cv.take<int>(std::max<size_t>(1, mine.size())); }));
   PeerPush tabs[2];
   memset(tabs, 0, sizeof(tabs));
   for (int par = 0; par < 2; par++) {
     if (ps->deferred) {  // the sweep writes this rank's buffer only
       tabs[par].world = 1;
-      tabs[par].base[0] = reinterpret_cast<float*>(ps->local) + (size_t)par * ps->buf_floats;
+      tabs[par].base[0] = gb_peer_regions_of(ps, ps->rank).buf[par];
     } else {
       tabs[par].world = ps->world;
-      for (int p = 0; p < ps->world; p++) tabs[par].base[p] = reinterpret_cast<float*>(ps->peer[p]) + (size_t)par * ps->buf_floats;
+      for (int p = 0; p < ps->world; p++) tabs[par].base[p] = gb_peer_regions_of(ps, p).buf[par];
     }
     tabs[par].pair_ptr = s->d_pair_ptr; tabs[par].pair_factors = s->d_pair_factors; tabs[par].pair_done = s->d_pair_done;
   }
   GB_CUDA(cudaMemcpy(s->d_peer_tables, tabs, sizeof(tabs), cudaMemcpyHostToDevice));
   GB_CUDA(cudaMemcpy(s->d_pair_ptr, ptr.data(), sizeof(int) * (P + 1), cudaMemcpyHostToDevice));
   if (s->F) GB_CUDA(cudaMemcpy(s->d_pair_factors, fac.data(), sizeof(int) * s->F, cudaMemcpyHostToDevice));
-  GB_CUDA(cudaMemset(s->d_pair_done, 0, b_done));
-  // the pairs this sweep owns (one sweep per peer slab): the rows the exchange kernel copies to the peers
-  std::vector<int> mine;
-  for (size_t k = 0; k < P; k++) if (ptr[k + 1] > ptr[k]) mine.push_back((int)k);
-  if (ps->d_my_pairs) { GB_CUDA(cudaFree(ps->d_my_pairs)); ps->d_my_pairs = nullptr; }
+  GB_CUDA(cudaMemset(s->d_pair_done, 0, sizeof(unsigned) * P));
   ps->num_my_pairs = (int)mine.size();
-  if (!mine.empty()) {
-    GB_CUDA(cudaMalloc((void**)&ps->d_my_pairs, sizeof(int) * mine.size()));
-    GB_CUDA(cudaMemcpy(ps->d_my_pairs, mine.data(), sizeof(int) * mine.size(), cudaMemcpyHostToDevice));
-  }
+  if (!mine.empty()) GB_CUDA(cudaMemcpy(ps->d_my_pairs, mine.data(), sizeof(int) * mine.size(), cudaMemcpyHostToDevice));
   s->peer = ps;
   return GB_OK;
 }
@@ -1138,7 +1127,7 @@ extern "C" gb_status gb_peer_slab_signal_wait(gb_peer_slab* ps) {
 
 extern "C" gb_status gb_peer_slab_device_ptr(gb_peer_slab* ps, void** device_ptr) {
   GB_REQUIRE(ps && device_ptr, "null argument");
-  *device_ptr = ps->local + (size_t)ps->completed_parity * ps->buf_floats * sizeof(float);
+  *device_ptr = gb_peer_regions_of(ps, ps->rank).buf[ps->completed_parity];
   return GB_OK;
 }
 
@@ -1146,8 +1135,9 @@ extern "C" gb_status gb_peer_slab_fetch_async(gb_peer_slab* ps, const float** ho
   GB_REQUIRE(ps, "null peer slab");
   GB_ENTER(ps->ctx);
   const size_t bytes = ps->num_pairs * GB_SLAB_STRIDE * sizeof(float);
-  GB_CUDA(cudaMemcpyAsync(ps->h_pinned, ps->local + (size_t)ps->completed_parity * ps->buf_floats * sizeof(float), bytes, cudaMemcpyDeviceToHost, ps->ctx->stream));
-  GB_CUDA(cudaMemcpyAsync((char*)ps->h_pinned + bytes, ps->d_timeout, sizeof(int), cudaMemcpyDeviceToHost, ps->ctx->stream));
+  const gb_peer_regions r = gb_peer_regions_of(ps, ps->rank);
+  GB_CUDA(cudaMemcpyAsync(ps->h_pinned, r.buf[ps->completed_parity], bytes, cudaMemcpyDeviceToHost, ps->ctx->stream));
+  GB_CUDA(cudaMemcpyAsync((char*)ps->h_pinned + bytes, r.timeout, sizeof(int), cudaMemcpyDeviceToHost, ps->ctx->stream));
   if (host_ptr) *host_ptr = ps->h_pinned;
   return GB_OK;
 }
@@ -1174,29 +1164,30 @@ extern "C" gb_status gb_overlap(gb_ctx* ctx, size_t T, const gb_voxelmap* const*
   if (T == 0 || source->n == 0) return GB_OK;
   GB_REQUIRE(targets && deltas, "null targets / deltas");
   GB_ENTER(ctx);
-  const size_t b_desc = align_up(sizeof(FactorDesc) * T, 256), b_pose = align_up(sizeof(double) * 16 * T, 256);
-  char* h = nullptr;
-  char* d = nullptr;
-  GB_CHECK(gb_ctx_pinned(ctx, b_desc + b_pose + 256, (void**)&h));
-  GB_CHECK(gb_ctx_scratch(ctx, b_desc + b_pose + 256, (void**)&d));
-  FactorDesc* hd = (FactorDesc*)h;
+  // the same layout in pinned staging and in scratch: descriptors | poses | count
+  struct Staging { FactorDesc* descs; double* poses; int* count; } h, d;
+  auto layout = [&](Carver& cv, Staging& b) {
+    b.descs = cv.take<FactorDesc>(T);
+    b.poses = cv.take<double>(16 * T);
+    b.count = cv.take<int>(1);
+  };
+  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { layout(cv, h); }));
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) { layout(cv, d); }));
   for (size_t t = 0; t < T; t++) {
     GB_REQUIRE(targets[t], "null target");
-    FactorDesc& D = hd[t];
+    FactorDesc& D = h.descs[t];
     memset(&D, 0, sizeof(D));
     D.p0 = source->p0; D.p1 = source->p1; D.p2 = source->p2;
     D.buckets = targets[t]->buckets; D.voxels = targets[t]->voxels;
     D.mask = (uint32_t)targets[t]->num_buckets - 1u; D.max_scan = targets[t]->max_scan; D.inv_res = targets[t]->inv_res; D.n = (int)source->n;
   }
-  memcpy(h + b_desc, deltas, sizeof(double) * 16 * T);
-  int* h_count = (int*)(h + b_desc + b_pose);
-  int* d_count = (int*)(d + b_desc + b_pose);
-  GB_CUDA(cudaMemcpyAsync(d, h, b_desc + b_pose, cudaMemcpyHostToDevice, ctx->stream));
-  GB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(int), ctx->stream));
-  GB_CHECK(gb_launch_overlap(ctx, (int)T, (const FactorDesc*)d, (const double*)(d + b_desc), (int)source->n, d_count));
-  GB_CUDA(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  memcpy(h.poses, deltas, sizeof(double) * 16 * T);
+  GB_CUDA(cudaMemcpyAsync(d.descs, h.descs, (char*)h.count - (char*)h.descs, cudaMemcpyHostToDevice, ctx->stream));  // descriptors and poses
+  GB_CUDA(cudaMemsetAsync(d.count, 0, sizeof(int), ctx->stream));
+  GB_CHECK(gb_launch_overlap(ctx, (int)T, d.descs, d.poses, (int)source->n, d.count));
+  GB_CUDA(cudaMemcpyAsync(h.count, d.count, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(cudaStreamSynchronize(ctx->stream));
-  *overlap = (double)*h_count / (double)source->n;
+  *overlap = (double)*h.count / (double)source->n;
   return GB_OK;
 }
 
@@ -1247,19 +1238,12 @@ extern "C" gb_status gb_merge_frames(gb_ctx* ctx, size_t K, const gb_cloud* cons
   }
   GB_REQUIRE(total < (size_t)1 << 30 && K < 65536, "too many points / frames");
   GB_ENTER(ctx);
-  gb_cloud* c = nullptr;
-  if (out_cloud) {
-    c = new (std::nothrow) gb_cloud();
-    if (!c) return GB_ERR_INTERNAL;
-    c->device = ctx->device;
-  }
-  gb_status st = gb_merge_frames_impl(ctx, (int)K, frames, poses, resolution, target, seed, out_xyzw, out_cov4x4, num_out, c);
-  if (st == GB_OK) {
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { gb_set_error("gb_merge_frames: %s", cudaGetErrorString(e)); st = GB_ERR_CUDA; }
-  }
-  if (st != GB_OK) { if (c) { gb_dev_free(ctx->device, c->base); delete c; } return st; }
-  if (out_cloud) *out_cloud = c;
+  gb_owned<gb_cloud> c(out_cloud ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
+  if (out_cloud && !c) return GB_ERR_INTERNAL;
+  if (c) c->device = ctx->device;
+  GB_CHECK(gb_merge_frames_impl(ctx, (int)K, frames, poses, resolution, target, seed, out_xyzw, out_cov4x4, num_out, c.get()));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (out_cloud) *out_cloud = c.release();
   return GB_OK;
 }
 
@@ -1291,19 +1275,12 @@ extern "C" gb_status gb_preprocess(gb_ctx* ctx, size_t n, const double* xyzw, co
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw, "null points");
   GB_ENTER(ctx);
-  gb_cloud* c = nullptr;
-  if (P->estimate_covariances) {
-    c = new (std::nothrow) gb_cloud();
-    if (!c) return GB_ERR_INTERNAL;
-    c->device = ctx->device;
-  }
-  gb_status st = gb_preprocess_impl(ctx, n, xyzw, times, intensities, P, out, c);
-  if (st == GB_OK) {
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);  // the cloud is complete when the call returns (it may be used from another context)
-    if (e != cudaSuccess) { gb_set_error("gb_preprocess: %s", cudaGetErrorString(e)); st = GB_ERR_CUDA; }
-  }
-  if (st != GB_OK) { if (c) { gb_dev_free(ctx->device, c->base); delete c; } return st; }
-  out->cloud = c;
+  gb_owned<gb_cloud> c(P->estimate_covariances ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
+  if (P->estimate_covariances && !c) return GB_ERR_INTERNAL;
+  if (c) c->device = ctx->device;
+  GB_CHECK(gb_preprocess_impl(ctx, n, xyzw, times, intensities, P, out, c.get()));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));  // the cloud is complete when the call returns (it may be used from another context)
+  out->cloud = c.release();
   return GB_OK;
 }
 extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, double resolution, double* out_xyzw, double* out_times, double* out_intensities, size_t* num_out) {

@@ -189,7 +189,7 @@ extern "C" gb_status gb_deskew(gb_ctx* ctx, const double T_imu_lidar[16], const 
   double4 *d_pts, *d_out;
   int* d_idx;
   double* d_tab;
-  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     d_pts = cv.take<double4>(n);
     d_out = cv.take<double4>(n);
     d_idx = cv.take<int>(n);

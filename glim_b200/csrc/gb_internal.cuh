@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stddef.h>
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <utility>
@@ -102,13 +103,13 @@ struct FactorDesc {
 static_assert(sizeof(FactorDesc) == 80, "FactorDesc size");
 
 struct gb_factor {
-  gb_ctx* ctx;
-  const gb_voxelmap* target;
-  const gb_cloud* source;
-  int flags;
-  gb_sweep* single;  // lazily created 1-factor sweep
-  float inlier_frac; // inlier fraction of the last linearization (< 0: unknown) -- sizes the work items of the next sweep
-  uint64_t id;       // process-wide unique
+  gb_ctx* ctx = nullptr;
+  const gb_voxelmap* target = nullptr;
+  const gb_cloud* source = nullptr;
+  int flags = 0;
+  gb_sweep* single = nullptr;  // lazily created 1-factor sweep
+  float inlier_frac = -1.f;    // inlier fraction of the last linearization (< 0: unknown) -- sizes the work items of the next sweep
+  uint64_t id = 0;             // process-wide unique
   std::vector<gb_sweep*> users;  // sweeps (of any context) that reference this factor; guarded by the registry mutex
 };
 
@@ -126,15 +127,13 @@ struct gb_peer_slab {
   gb_ctx* ctx = nullptr;
   size_t num_pairs = 0;
   int world = 0, rank = 0;
-  size_t buf_floats = 0;          // floats per buffer
-  char* local = nullptr;          // cudaMalloc: [buffer 0][buffer 1][flags: world x u32, padded]
+  char* local = nullptr;          // cudaMalloc, laid out by gb_peer_layout
   char* peer[GB_MAX_PEERS] = {};  // every rank's allocation as mapped here (peer[rank] == local)
   bool opened[GB_MAX_PEERS] = {};
   unsigned step = 0;              // last launched step
   int parity = 0;                 // buffer written by the NEXT launch
   int completed_parity = 0;       // buffer completed by the last signal_wait
-  int* d_timeout = nullptr;
-  float* h_pinned = nullptr;      // num_pairs x GB_SLAB_STRIDE, for the fetches
+  float* h_pinned = nullptr;      // num_pairs x GB_SLAB_STRIDE + the timeout word, for the fetches
   bool connected = false;
   // deferred exchange (default): the sweep stores finished pair rows into the LOCAL buffer only; the exchange kernel that
   // follows it copies this rank's rows to every peer (one CTA per peer) before it publishes the completion flags
@@ -145,6 +144,8 @@ struct gb_peer_slab {
 
 #define GB_ACC_STRIDE 32      // doubles per factor in the accumulation buffer (29 used)
 #define GB_OUT_DOUBLES 122    // gb_linearized6
+
+struct gb_pool_block { void* d = nullptr; size_t d_cap = 0; void* h = nullptr; size_t h_cap = 0; };
 
 struct gb_sweep {
   gb_ctx* ctx = nullptr;
@@ -188,23 +189,25 @@ struct gb_sweep {
   int pose_slot = 0;
   cudaGraphExec_t graph_exec = nullptr;  // small sweeps: poses H2D -> kernel -> records D2H as ONE graph launch (gb_factor_set_linearize)
   int graph_state = 0;              // 0 = not built, 1 = valid, -1 = capture failed (plain launches from then on)
-  void* pool_d = nullptr; size_t pool_d_cap = 0;  // the blocks this sweep took from its context's pool
-  void* pool_h = nullptr; size_t pool_h_cap = 0;
+  gb_pool_block blk;                // the device and pinned blocks, laid out by sweep_layout; back to the context's pool at the end
   bool any_incremental = false;     // some target is an incremental map: its descriptor may go stale (gb_voxelmap_insert)
   std::vector<uint64_t> target_versions;  // per factor: the target version its descriptor was written from
 };
 
-struct gb_pool_block { void* d; size_t d_cap; void* h; size_t h_cap; };
+// A context's grow-only buffer: device scratch or pinned host staging.  What it holds is valid until the next gb_carve on it.
+struct gb_arena {
+  bool host = false;  // cudaMallocHost, else cudaMalloc
+  void* base = nullptr;
+  size_t cap = 0;
+};
 
 struct gb_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   int num_sms = 0;
-  void* scratch = nullptr;
-  size_t scratch_cap = 0;
-  void* pinned = nullptr;
-  size_t pinned_cap = 0;
+  gb_arena scratch;
+  gb_arena pinned{true};
   uint64_t launches = 0;     // gb_ctx_kernel_launches: written by gb_launch, GB_CUB and the graph path of sweep_linearize only
   std::atomic<int> refs{0};  // owner + live factors / sweeps / peer slabs; the context is torn down when the last one lets go
   std::vector<gb_sweep*> sweep_cache;
@@ -252,13 +255,18 @@ gb_status gb_launch(gb_ctx* ctx, const char* name, void (*kernel)(P...), dim3 gr
 // every live context of the device (what the implicit synchronisation of cudaFree used to guarantee) and keeps the block.
 cudaError_t gb_dev_malloc(int device, size_t bytes, void** out);
 void gb_dev_free(int device, void* p);
-gb_status gb_ctx_scratch(gb_ctx* ctx, size_t bytes, void** out);  // device scratch, valid until the next call
-gb_status gb_ctx_pinned(gb_ctx* ctx, size_t bytes, void** out);   // pinned host staging, same lifetime rule
+gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes);  // a.base holds at least `bytes` afterwards
+
+// The one free function of each handle that owns memory (cloud_free, voxelmap_free, sweep_free, peer_slab_free,
+// ctx_release): it releases everything the handle owns, never returns early, and ends with the delete.  A creation holds
+// its partial handle in a gb_owned with that function, so that every failure exit frees it, and releases it on success.
+template <typename T> using gb_owned = std::unique_ptr<T, void (*)(T*)>;
+void sweep_free(gb_sweep* s);
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Carves 256-byte aligned arrays out of one buffer.  Without a base it only measures: a layout is written once, as a
-// function of a Carver, and run first to size the buffer and then to hand out the pointers (gb_carve_scratch).
+// Carves 256-byte aligned arrays out of one buffer.  Without a base it only measures: every block the host lays out is
+// written once, as a function of a Carver, and run first to size the buffer and then to hand out the pointers (gb_carve).
 struct Carver {
   char* base = nullptr;
   size_t off = 0;
@@ -268,13 +276,37 @@ struct Carver {
     return p;
   }
 };
-template <typename Layout> gb_status gb_carve_scratch(gb_ctx* ctx, Layout&& layout) {
+// A layout carved out of one of the context's arenas (ctx->scratch or ctx->pinned).
+template <typename Layout> gb_status gb_carve(gb_ctx* ctx, gb_arena& arena, Layout&& layout) {
   Carver size;
   layout(size);
-  Carver cv;
-  GB_CHECK(gb_ctx_scratch(ctx, size.off, (void**)&cv.base));
+  GB_CHECK(gb_arena_reserve(ctx, arena, size.off));
+  Carver cv{(char*)arena.base};
   layout(cv);
   return GB_OK;
+}
+
+// The peer slab's allocation, the same on every rank (so a peer's regions are found at the same offsets of its mapping).
+// All of it is zero at creation.
+struct gb_peer_regions {
+  float* buf[2];       // the step-parity buffers: num_pairs x GB_SLAB_STRIDE floats each
+  unsigned* flags;     // [world] completion flags, written by the peers
+  int* timeout;        // set by the exchange kernels when a peer misses its flag
+  unsigned* arrivals;  // [world] CTA arrival counters of the deferred exchange (self-cleaning)
+};
+inline gb_peer_regions gb_peer_layout(Carver& cv, size_t num_pairs, int world) {
+  gb_peer_regions r;
+  r.buf[0] = cv.take<float>(num_pairs * GB_SLAB_STRIDE);
+  r.buf[1] = cv.take<float>(num_pairs * GB_SLAB_STRIDE);
+  r.flags = cv.take<unsigned>((size_t)world);
+  r.timeout = cv.take<int>(1);
+  r.arrivals = cv.take<unsigned>((size_t)world);
+  return r;
+}
+// rank p's regions as mapped on this device
+inline gb_peer_regions gb_peer_regions_of(const gb_peer_slab* ps, int p) {
+  Carver cv{ps->peer[p]};
+  return gb_peer_layout(cv, ps->num_pairs, ps->world);
 }
 
 // The largest temporary storage of the cub calls the library makes on n items (radix sorts of 64-bit keys with or

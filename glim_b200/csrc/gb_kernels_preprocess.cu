@@ -166,7 +166,7 @@ gb_status gb_find_neighbors_impl(gb_ctx* ctx, size_t n_, const double* xyzw, int
   cudaStream_t st = ctx->stream;
   double4* d_pts;
   int* d_nb;
-  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     d_pts = cv.take<double4>(n);
     d_nb = cv.take<int>((size_t)n * k);
   }));
@@ -184,7 +184,7 @@ gb_status gb_covariances_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const 
   double4 *d_pts, *d_nrm;
   int* d_nb;
   double* d_cov;
-  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     d_pts = cv.take<double4>(n);
     d_nb = cv.take<int>((size_t)n * kc);
     d_nrm = cv.take<double4>(n);
@@ -209,7 +209,7 @@ gb_status gb_voxelgrid_sampling_impl(gb_ctx* ctx, size_t n_, const double* xyzw,
   double4 *d_pts, *d_opts;
   double *d_t, *d_i, *d_ot, *d_oi;
   int *d_flags, *d_pos, *d_starts;
-  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     t = gb_take_sort_tmp(cv, N, cv.take<char>(cub_b), cub_b);
     d_pts = cv.take<double4>(N);
     d_opts = cv.take<double4>(N);
@@ -609,7 +609,7 @@ gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const d
   int *d_cnt, *d_flags, *d_pos, *d_starts, *d_keep, *d_nb, *d_nbo;
   double4 *d_raw, *d_ds, *d_fr, *d_nrm, *d_fr2;
   double *d_t, *d_i, *d_dst, *d_dsi, *d_frt, *d_fri, *d_cov, *d_dist, *d_dist2, *d_sums, *d_frt2, *d_fri2;
-  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     staged = gb_cloud_planes(cv, N, true);
     void* d_cub = cv.take<char>(cub_b);
     t = gb_take_sort_tmp(cv, N, d_cub, cub_b);
@@ -721,28 +721,21 @@ gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const d
   if (M > 0) {
     const size_t m = (size_t)M;
     const bool cov_out = P->estimate_covariances != 0;
-    struct Part { void* dst; const void* src; size_t bytes; };
+    struct Part { void* dst; const void* src; size_t bytes; char* staged; };
     Part parts[6] = {{out->xyzw, d_fr, sizeof(double4) * m}, {out->times, d_frt, sizeof(double) * m}, {(out->intensities && intensities) ? out->intensities : nullptr, d_fri, sizeof(double) * m},
                      {out->neighbors, d_nb, sizeof(int) * m * (size_t)k}, {(cov_out ? out->normals4 : nullptr), d_nrm, sizeof(double4) * m}, {(cov_out ? out->cov4x4 : nullptr), d_cov, sizeof(double) * 16 * m}};
-    size_t total_h = 64;
-    for (const Part& q : parts) if (q.dst) total_h += align_up(q.bytes, 64);
-    char* h = nullptr;
-    GB_CHECK(gb_ctx_pinned(ctx, total_h, (void**)&h));
-    size_t off = 64;
-    GB_CUDA(cudaMemcpyAsync(h, d_frt + (M - 1), sizeof(double), cudaMemcpyDeviceToHost, st));
-    for (const Part& q : parts) {
-      if (!q.dst) continue;
-      GB_CUDA(cudaMemcpyAsync(h + off, q.src, q.bytes, cudaMemcpyDeviceToHost, st));
-      off += align_up(q.bytes, 64);
-    }
+    double* h_last_time = nullptr;
+    GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) {
+      h_last_time = cv.take<double>(1);
+      for (Part& q : parts) q.staged = q.dst ? cv.take<char>(q.bytes) : nullptr;
+    }));
+    GB_CUDA(cudaMemcpyAsync(h_last_time, d_frt + (M - 1), sizeof(double), cudaMemcpyDeviceToHost, st));
+    for (const Part& q : parts)
+      if (q.dst) GB_CUDA(cudaMemcpyAsync(q.staged, q.src, q.bytes, cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
-    memcpy(&out->last_time, h, sizeof(double));
-    off = 64;
-    for (const Part& q : parts) {
-      if (!q.dst) continue;
-      memcpy(q.dst, h + off, q.bytes);
-      off += align_up(q.bytes, 64);
-    }
+    out->last_time = *h_last_time;
+    for (const Part& q : parts)
+      if (q.dst) memcpy(q.dst, q.staged, q.bytes);
   } else {
     out->last_time = 0.0;
   }
@@ -757,7 +750,7 @@ gb_status gb_find_neighbors_pyramid_impl(gb_ctx* ctx, size_t n_, const double* x
   KnnTmp knn;
   int *d_cnt, *d_nb;
   double4* d_pts;
-  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     knn = take_knn_tmp(cv, n, cv.take<char>(cub_b), cub_b);
     d_cnt = cv.take<int>(64);
     d_pts = cv.take<double4>(N);
@@ -861,9 +854,9 @@ gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T, vo
   MergeFrame F;
   F.p0 = c->p0; F.p1 = c->p1; F.p2 = c->p2; F.inv_perm = c->inv_perm; F.n = (int)c->n; F.offset = 0;
   for (int r = 0; r < 3; r++) for (int cc = 0; cc < 4; cc++) F.T[r * 4 + cc] = T[cc * 4 + r];
-  void* h = nullptr;
-  GB_CHECK(gb_ctx_pinned(ctx, sizeof(MergeFrame), &h));
-  memcpy(h, &F, sizeof(MergeFrame));
+  MergeFrame* h = nullptr;
+  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h = cv.take<MergeFrame>(1); }));
+  *h = F;
   GB_CUDA(cudaMemcpyAsync(d_frame, h, sizeof(MergeFrame), cudaMemcpyHostToDevice, ctx->stream));
   const int n = (int)c->n;
   return gb_launch(ctx, "k_merge_transform", k_merge_transform, (n + 255) / 256, 256, 0, 1, (const MergeFrame*)d_frame, n, pts, cov6);
@@ -890,7 +883,7 @@ gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames
   MergeFrame* d_mf;
   double4 *d_pts, *d_vpts;
   double *d_cov, *d_vcov, *d_ocov;
-  GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     staged = gb_cloud_planes(cv, N, false);
     t = gb_take_sort_tmp(cv, N, cv.take<char>(cub_b), cub_b);
     d_cnt = cv.take<int>(64);
@@ -905,8 +898,8 @@ gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames
     d_starts = cv.take<int>(N + 1);
     d_keep = cv.take<int>(N + 1);
   }));
-  void* h_mf = nullptr;
-  GB_CHECK(gb_ctx_pinned(ctx, sizeof(MergeFrame) * (size_t)K, &h_mf));
+  MergeFrame* h_mf = nullptr;
+  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h_mf = cv.take<MergeFrame>((size_t)K); }));
   memcpy(h_mf, mf.data(), sizeof(MergeFrame) * (size_t)K);
   GB_CUDA(cudaMemcpyAsync(d_mf, h_mf, sizeof(MergeFrame) * (size_t)K, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemsetAsync(d_cnt, 0, 256, st));

@@ -676,23 +676,25 @@ __global__ void __launch_bounds__(kExchangeThreads) k_peer_exchange(PeerExchange
 }
 
 gb_status gb_launch_peer_signal_wait(gb_peer_slab* ps) {
+  const gb_peer_regions mine = gb_peer_regions_of(ps, ps->rank);
   if (ps->deferred) {
     PeerExchange px;
     memset(&px, 0, sizeof(px));
     for (int p = 0; p < ps->world; p++) {
-      px.dst[p] = reinterpret_cast<float*>(ps->peer[p]) + (size_t)ps->parity * ps->buf_floats;
-      px.flags[p] = reinterpret_cast<unsigned*>(ps->peer[p] + 2 * ps->buf_floats * sizeof(float));
+      const gb_peer_regions r = gb_peer_regions_of(ps, p);
+      px.dst[p] = r.buf[ps->parity];
+      px.flags[p] = r.flags;
     }
-    px.src = reinterpret_cast<const float*>(ps->local) + (size_t)ps->parity * ps->buf_floats;
+    px.src = mine.buf[ps->parity];
     px.my_pairs = ps->d_my_pairs;
     px.num_my_pairs = ps->num_my_pairs;
-    px.arrivals = reinterpret_cast<unsigned*>(ps->d_timeout) + 16;  // zeroed at creation, self-cleaning
-    return gb_launch(ps->ctx, "k_peer_exchange", k_peer_exchange, ps->world * kExchangeCtasPerPeer, kExchangeThreads, 0, px, ps->world, ps->rank, ps->step, ps->d_timeout);
+    px.arrivals = mine.arrivals;
+    return gb_launch(ps->ctx, "k_peer_exchange", k_peer_exchange, ps->world * kExchangeCtasPerPeer, kExchangeThreads, 0, px, ps->world, ps->rank, ps->step, mine.timeout);
   }
   PeerFlags pf;
   memset(&pf, 0, sizeof(pf));
-  for (int p = 0; p < ps->world; p++) pf.flags[p] = reinterpret_cast<unsigned*>(ps->peer[p] + 2 * ps->buf_floats * sizeof(float));
-  return gb_launch(ps->ctx, "k_peer_signal_wait", k_peer_signal_wait, 1, 32, 0, pf, ps->world, ps->rank, ps->step, ps->d_timeout);
+  for (int p = 0; p < ps->world; p++) pf.flags[p] = gb_peer_regions_of(ps, p).flags;
+  return gb_launch(ps->ctx, "k_peer_signal_wait", k_peer_signal_wait, 1, 32, 0, pf, ps->world, ps->rank, ps->step, mine.timeout);
 }
 
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count) {

@@ -188,7 +188,7 @@ gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resol
     const size_t cub_b = gb_cub_temp_bytes(n);
     gb_sort_tmp t;
     int *d_flags, *d_pos, *d_starts;
-    GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
       t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
       d_flags = cv.take<int>(n + 1);
       d_pos = cv.take<int>(n + 1);
@@ -346,7 +346,7 @@ gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* c
     unsigned long long *d_hash = nullptr, *d_info;
     void* d_frame;
     int4* d_vcoord;
-    GB_CHECK(gb_carve_scratch(ctx, [&](Carver& cv) {
+    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
       t = gb_take_sort_tmp(cv, (size_t)N, cv.take<char>(cub_b), cub_b);
       d_flags = cv.take<int>(N + 1);
       d_pos = cv.take<int>(N + 1);

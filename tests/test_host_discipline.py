@@ -6,6 +6,9 @@
 4. Every C-ABI entry point that takes a context, sweep, factor or peer slab enters through GB_ENTER (the context's lock and
    device), unless it is listed below with its reason; the lock and cudaSetDevice appear nowhere else but in GB_ENTER and
    the context lifetime and teardown functions.
+5. align_up is called only by Carver: every block the host lays out is a Carver layout, run once to size and once to carve.
+6. delete (of a handle) and cudaFree / cudaFreeHost appear only in the free and release functions listed below: each
+   handle has one free function, which every destroy entry point and every failed creation calls.
 
 The function bodies are found by brace matching on the sources with comments, strings and preprocessor lines removed."""
 import os
@@ -27,12 +30,27 @@ NO_ENTER = {
     "gb_ctx_destroy": "teardown: locks the context itself, then releases it outside the lock",
     "gb_vgicp_factor_destroy": "teardown: sweep_free locks the context; the registry mutex guards the factor links",
     "gb_sweep_destroy": "teardown: sweep_free locks the context, then releases it outside the lock",
+    "gb_peer_slab_destroy": "teardown: peer_slab_free locks the context, then releases it outside the lock",
 }
 # the only functions that may take the lock or set the device by hand: context lifetime, teardown, and calls on objects
 # that keep no context (a device number only)
-LOCK_OR_DEVICE_BY_HAND = {"ctx_create", "ctx_release", "gb_ctx_destroy", "sweep_free", "gb_mem_info", "gb_cloud_destroy", "gb_voxelmap_destroy",
-                          "gb_cloud_download", "gb_voxelmap_download"}
+LOCK_OR_DEVICE_BY_HAND = {"ctx_create", "ctx_release", "gb_ctx_destroy", "sweep_free", "peer_slab_free", "gb_mem_info", "gb_cloud_destroy",
+                          "gb_voxelmap_destroy", "gb_cloud_download", "gb_voxelmap_download"}
 COUNTER_WRITERS = {"gb_launch", "sweep_linearize"}  # and the GB_CUB macro
+# the only functions that may delete a handle or call cudaFree / cudaFreeHost
+FREE_FUNCTIONS = {
+    "cloud_free": "free function of gb_cloud",
+    "voxelmap_free": "free function of gb_voxelmap",
+    "sweep_free": "free function of gb_sweep",
+    "peer_slab_free": "free function of gb_peer_slab",
+    "ctx_release": "free function of gb_ctx (the last reference lets go)",
+    "gb_vgicp_factor_destroy": "free function of gb_factor, which owns no device memory",
+    "gb_dev_malloc": "the device pool gives its free blocks back to the driver when an allocation fails",
+    "gb_dev_free": "the device pool frees a block it does not keep",
+    "gb_arena_reserve": "the context's grow routine replaces its scratch / pinned buffer",
+    "pool_block_free": "a sweep block evicted from the context's pool, or not kept by it",
+    "dev_block_realloc": "a sweep's pair CSR block and a peer slab's pair list, replaced when a slab is attached",
+}
 
 
 def strip_source(text):
@@ -145,12 +163,29 @@ def line_of(code, pos):
     return code.count("\n", 0, pos) + 1
 
 
+def struct_body(code, name):
+    """(start, end) of the body of struct `name` in code, or None."""
+    m = re.search(r"\bstruct\s+" + name + r"\s*\{", code)
+    return (m.end() - 1, match_brace(code, m.end() - 1)) if m else None
+
+
 def violations(csrc):
-    """{rule: [offending site]} for rules 1-4 of this module's docstring."""
-    bad = {1: [], 2: [], 3: [], 4: []}
+    """{rule: [offending site]} for rules 1-6 of this module's docstring."""
+    bad = {1: [], 2: [], 3: [], 4: [], 5: [], 6: []}
     enters = 0
     for f, code, directives, funcs in sources(csrc):
         where = lambda pos: f"{f}:{line_of(code, pos)} ({enclosing(funcs, pos)})"
+        carver = struct_body(code, "Carver")
+        for m in re.finditer(r"\balign_up\b", code):
+            definition = re.search(r"\bsize_t\s+$", code[max(0, m.start() - 40):m.start()])
+            if not (definition or (carver and carver[0] < m.start() < carver[1])):
+                bad[5].append(where(m.start()))
+        for m in re.finditer(r"\bdelete\b|\bcudaFree(Host)?\s*\(", code):
+            if enclosing(funcs, m.start()) not in FREE_FUNCTIONS:
+                bad[6].append(where(m.start()))
+        for d in directives:
+            if re.search(r"\balign_up\b|\bdelete\b|\bcudaFree", d):
+                bad[5 if "align_up" in d else 6].append(f"{f}: {d.splitlines()[0].strip()}")
         for m in re.finditer(r"<<<", code):
             if enclosing(funcs, m.start()) != "gb_launch":
                 bad[1].append(where(m.start()))
@@ -185,21 +220,28 @@ def violations(csrc):
 
 def parsed_inventory(csrc):
     """Sanity numbers of the parse, so that a rule cannot pass because the parser found nothing."""
-    names, launches_in_helper, cub_calls = set(), 0, 0
+    names, launches_in_helper, cub_calls, carver_align, frees = set(), 0, 0, 0, 0
     for f, code, _, funcs in sources(csrc):
         names.update(n for n, *_ in funcs)
         launches_in_helper += sum(1 for m in re.finditer(r"<<<", code) if enclosing(funcs, m.start()) == "gb_launch")
         cub_calls += len(re.findall(r"\bGB_CUB\s*\(", code))
-    return names, launches_in_helper, cub_calls
+        carver = struct_body(code, "Carver")
+        if carver:
+            carver_align += len(re.findall(r"\balign_up\s*\(", code[carver[0]:carver[1]]))
+        frees += sum(1 for m in re.finditer(r"\bdelete\b|\bcudaFree(Host)?\s*\(", code) if enclosing(funcs, m.start()) in FREE_FUNCTIONS)
+    return names, launches_in_helper, cub_calls, carver_align, frees
 
 
 def test_parser_sees_the_library():
-    names, launches_in_helper, cub_calls = parsed_inventory(CSRC)
+    names, launches_in_helper, cub_calls, carver_align, frees = parsed_inventory(CSRC)
     assert {"gb_launch", "sweep_linearize", "gb_preprocess", "gb_vgicp_align", "gb_deskew", "knn_device", "table_build"} <= names
+    assert set(FREE_FUNCTIONS) <= names
     assert launches_in_helper == 1
     assert cub_calls >= 10
+    assert carver_align == 1
+    assert frees >= len(FREE_FUNCTIONS)
     _, enters = violations(CSRC)
-    assert enters >= 30
+    assert enters >= 29  # gb_peer_slab_destroy is teardown now: peer_slab_free locks the context by hand
 
 
 def test_every_kernel_launch_goes_through_gb_launch():
@@ -216,3 +258,11 @@ def test_every_cub_call_goes_through_gb_cub():
 
 def test_every_context_bound_entry_point_enters_its_context():
     assert violations(CSRC)[0][4] == []
+
+
+def test_align_up_only_in_carver():
+    assert violations(CSRC)[0][5] == []
+
+
+def test_handles_freed_only_by_their_free_functions():
+    assert violations(CSRC)[0][6] == []
