@@ -28,6 +28,7 @@ SYMBOLS = [
     "gb_overlap", "gb_covariances", "gb_find_neighbors", "gb_voxelgrid_sampling", "gb_preprocess_default_params", "gb_preprocess", "gb_merge_frames",
     "gb_deskew_pose_table", "gb_deskew",
     "gb_align_default_params", "gb_vgicp_align",
+    "gb_ivox_create", "gb_ivox_insert", "gb_ivox_info", "gb_ivox_download", "gb_ivox_destroy", "gb_gicp_factor_create",
 ]
 
 GB_SLAB_STRIDE = 96
@@ -142,6 +143,12 @@ def lib():
     L.gb_deskew.argtypes = [vp, vp, vp, vp, sz, vp, vp, f64, sz, vp, vp, vp, vp]
     L.gb_align_default_params.argtypes = [vp]
     L.gb_vgicp_align.argtypes = [vp, sz, vp, vp, vp, vp, vp]
+    L.gb_ivox_create.argtypes = [vp, f64, f64, i32, i32, i32, i32, vp]
+    L.gb_ivox_insert.argtypes = [vp, vp, vp, vp, f64, u64]
+    L.gb_ivox_info.argtypes = [vp, vp, vp, vp]
+    L.gb_ivox_download.argtypes = [vp, vp, vp, vp, vp]
+    L.gb_ivox_destroy.argtypes = [vp]
+    L.gb_gicp_factor_create.argtypes = [vp, vp, vp, f64, vp]
     for name in SYMBOLS:
         getattr(L, name)  # AttributeError here means the library and include/glim_b200.h are out of sync
     _lib = L

@@ -328,6 +328,7 @@ extern "C" gb_status gb_cloud_destroy(gb_cloud* c) {
 static void voxelmap_free(gb_voxelmap* m) {
   gb_dev_free(m->device, m->base);
   gb_dev_free(m->device, m->buckets);
+  delete m->ivox;
   delete m;
 }
 
@@ -409,6 +410,86 @@ extern "C" gb_status gb_voxelmap_destroy(gb_voxelmap* m) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// iVox: a gb_voxelmap with iVox state (gb_internal.cuh); voxelmap_free and gb_voxelmap_destroy release it
+// ---------------------------------------------------------------------------------------------
+extern "C" gb_status gb_ivox_create(gb_ctx* ctx, double resolution, double min_dist_in_cell, int max_points_in_cell, int neighbor_voxel_mode, int lru_horizon,
+                                    int lru_clear_cycle, gb_ivox** out) {
+  GB_REQUIRE(ctx && out, "null argument");
+  GB_REQUIRE(std::isfinite(resolution) && resolution > 0.0, "resolution must be positive and finite");
+  GB_REQUIRE(min_dist_in_cell >= 0.0, "min_dist_in_cell must be >= 0");
+  GB_REQUIRE(max_points_in_cell >= 1 && max_points_in_cell <= 64, "max_points_in_cell must be in [1, 64]");
+  GB_REQUIRE(neighbor_voxel_mode == 1 || neighbor_voxel_mode == 7 || neighbor_voxel_mode == 19 || neighbor_voxel_mode == 27, "neighbor_voxel_mode must be 1, 7, 19 or 27");
+  GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
+  *out = nullptr;
+  GB_ENTER(ctx);
+  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(), voxelmap_free);
+  if (!m) return GB_ERR_INTERNAL;
+  m->ivox = new (std::nothrow) gb_ivox_state();
+  if (!m->ivox) return GB_ERR_INTERNAL;
+  m->ivox->resolution = resolution;
+  m->ivox->min_dist = min_dist_in_cell;
+  m->ivox->max_points = max_points_in_cell;
+  m->ivox->mode = neighbor_voxel_mode;
+  m->resolution = (float)resolution;
+  m->inv_res = (float)(1.0 / resolution);
+  m->lru_horizon = lru_horizon;
+  m->lru_clear_cycle = lru_clear_cycle;
+  GB_CHECK(gb_ivox_create_impl(ctx, m.get()));
+  *out = reinterpret_cast<gb_ivox*>(m.release());
+  return GB_OK;
+}
+extern "C" gb_status gb_ivox_insert(gb_ctx* ctx, gb_ivox* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
+  GB_REQUIRE(ctx && map && cloud, "null argument");
+  GB_REQUIRE(sampling_rate > 0.0 && sampling_rate <= 1.0, "sampling_rate must be in (0, 1]");
+  static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  const double* T = T_map_cloud ? T_map_cloud : kIdentity;
+  for (int k = 0; k < 16; k++) GB_REQUIRE(std::isfinite(T[k]), "T_map_cloud must be finite");
+  gb_voxelmap* m = ivox_map(map);
+  GB_REQUIRE(m->device == ctx->device && cloud->device == ctx->device, "cloud / iVox live on another device");
+  GB_REQUIRE((uint64_t)m->ivox->num_points + (uint64_t)cloud->n < (1ull << 31) - 1, "stored points + cloud points exceed 2^31");
+  GB_ENTER(ctx);
+  return gb_ivox_insert_impl(ctx, m, cloud, T, sampling_rate, (unsigned long long)seed);
+}
+extern "C" gb_status gb_ivox_info(const gb_ivox* map, int* num_voxels, size_t* num_points, double* resolution) {
+  GB_REQUIRE(map, "null iVox");
+  const gb_voxelmap* m = ivox_map(map);
+  if (num_voxels) *num_voxels = m->num_voxels;
+  if (num_points) *num_points = m->ivox->num_points;
+  if (resolution) *resolution = m->ivox->resolution;
+  return GB_OK;
+}
+// plain copies, their direction taken from the unified address space (the map may live on another device than the current
+// one); the insert returned after its stream had drained
+extern "C" gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords, int32_t* voxel_counts, float* xyz, float* cov6) {
+  GB_REQUIRE(map, "null iVox");
+  const gb_voxelmap* m = ivox_map(map);
+  const size_t V = (size_t)m->num_voxels, P = m->ivox->num_points;
+  if (V == 0) return GB_OK;
+  if (voxel_coords || voxel_counts) {
+    std::vector<unsigned long long> keys(V);
+    std::vector<int2> cells(V);
+    GB_CUDA(cudaMemcpy(keys.data(), m->vkeys, sizeof(unsigned long long) * V, cudaMemcpyDefault));
+    GB_CUDA(cudaMemcpy(cells.data(), m->ivox->cells, sizeof(int2) * V, cudaMemcpyDefault));
+    for (size_t v = 0; v < V; v++) {
+      if (voxel_coords)
+        for (int a = 0; a < 3; a++) voxel_coords[3 * v + a] = (int32_t)((keys[v] >> (42 - 21 * a)) & 0x1FFFFF) - (1 << 20);
+      if (voxel_counts) voxel_counts[v] = cells[v].y;
+    }
+  }
+  if (xyz || cov6) {
+    std::vector<float4> h(3 * P);
+    GB_CUDA(cudaMemcpy(h.data(), m->voxels, sizeof(float4) * h.size(), cudaMemcpyDefault));
+    for (size_t p = 0; p < P; p++) {
+      const float4 a = h[3 * p], b = h[3 * p + 1], c = h[3 * p + 2];
+      if (xyz) { xyz[3 * p] = a.x; xyz[3 * p + 1] = a.y; xyz[3 * p + 2] = a.z; }
+      if (cov6) { cov6[6 * p] = a.w; cov6[6 * p + 1] = b.x; cov6[6 * p + 2] = b.y; cov6[6 * p + 3] = b.z; cov6[6 * p + 4] = b.w; cov6[6 * p + 5] = c.x; }
+    }
+  }
+  return GB_OK;
+}
+extern "C" gb_status gb_ivox_destroy(gb_ivox* map) { return gb_voxelmap_destroy(ivox_map(map)); }
+
+// ---------------------------------------------------------------------------------------------
 // factors and sweeps
 // ---------------------------------------------------------------------------------------------
 extern "C" gb_status gb_vgicp_factor_create(gb_ctx* ctx, const gb_voxelmap* target, const gb_cloud* source, int flags, gb_factor** out) {
@@ -421,6 +502,20 @@ extern "C" gb_status gb_vgicp_factor_create(gb_ctx* ctx, const gb_voxelmap* targ
   gb_factor* f = new (std::nothrow) gb_factor();
   if (!f) return GB_ERR_INTERNAL;
   f->ctx = ctx; f->target = target; f->source = source; f->flags = flags; f->id = g_next_factor_id.fetch_add(1);
+  ctx_retain(ctx);
+  *out = f;
+  return GB_OK;
+}
+extern "C" gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out) {
+  GB_REQUIRE(ctx && target && source && out, "null argument");
+  GB_REQUIRE(std::isfinite(max_correspondence_distance) && max_correspondence_distance > 0.0, "max_correspondence_distance must be positive and finite");
+  const gb_voxelmap* m = ivox_map(target);
+  GB_REQUIRE(m->device == ctx->device && source->device == ctx->device, "cloud / iVox live on another device");
+  GB_ENTER(ctx);
+  gb_factor* f = new (std::nothrow) gb_factor();
+  if (!f) return GB_ERR_INTERNAL;
+  f->ctx = ctx; f->target = m; f->source = source; f->id = g_next_factor_id.fetch_add(1);
+  f->max_corr2 = (float)(max_correspondence_distance * max_correspondence_distance);
   ctx_retain(ctx);
   *out = f;
   return GB_OK;
@@ -598,18 +693,29 @@ static void desc_target(FactorDesc& D, const gb_voxelmap* t) {
   D.max_scan = t->max_scan;
   D.inv_res = t->inv_res;
 }
+// a GICP factor's target part: the iVox's table and point records in the FactorDesc, the rest in its GicpDesc
+static void desc_target_ivox(FactorDesc& D, GicpDesc& G, const gb_factor* fa) {
+  desc_target(D, fa->target);
+  G.cells = fa->target->ivox->cells;
+  G.max_corr2 = fa->max_corr2;
+  G.num_offsets = fa->target->ivox->mode;
+}
 // B_f of SURVEY 8(d): 48 B per source point, 48 B per target voxel, 16 B per bucket, pose in + record out.
 // The bucket term is charged at the SMALLEST table that could hold the voxels (16384 doubled until >= V), not at
 // our deliberately sparse table (>= 8 V): padding we added for speed must not inflate the achieved-GB/s figure.
+// A GICP factor is charged 48 B per STORED target point in place of the voxel records (its voxels' buckets the same way).
 static uint64_t factor_bytes(const gb_factor* fa) {
   const bool sv = (fa->flags & GB_FACTOR_SURFACE_VALIDATION) != 0;
+  const uint64_t V = (uint64_t)fa->target->num_voxels;
+  const uint64_t records = fa->target->ivox ? (uint64_t)fa->target->ivox->num_points : V;
   uint64_t nb_ref = 16384;
-  while (nb_ref < (uint64_t)fa->target->num_voxels) nb_ref *= 2;
-  return (uint64_t)fa->source->n * (48 + (sv ? 12 : 0)) + (uint64_t)fa->target->num_voxels * 48 + nb_ref * 16 + 64 + 488;  // +12 B / point: the normals, when they are read
+  while (nb_ref < V) nb_ref *= 2;
+  return (uint64_t)fa->source->n * (48 + (sv ? 12 : 0)) + records * 48 + nb_ref * 16 + 64 + 488;  // +12 B / point: the normals, when they are read
 }
 
-// Before every launch: a factor whose target is an incremental map that gb_voxelmap_insert changed since its descriptor was
-// written gets that descriptor re-written (buckets, records, mask) and re-uploaded.  Sweeps over built maps return at once.
+// Before every launch: a factor whose target is an incremental map that gb_voxelmap_insert changed (or an iVox that
+// gb_ivox_insert changed) since its descriptor was written gets that descriptor re-written (buckets, records, mask; for
+// GICP the cells too) and re-uploaded.  Sweeps over built maps return at once.
 static gb_status sweep_follow_targets(gb_sweep* s) {
   if (!s->any_incremental) return GB_OK;
   bool synced = false;
@@ -620,8 +726,13 @@ static gb_status sweep_follow_targets(gb_sweep* s) {
       GB_CUDA(cudaStreamSynchronize(s->ctx->stream));
       synced = true;
     }
-    desc_target(s->h_descs[f], fa->target);
     s->target_versions[f] = fa->target->version;
+    if (fa->target->ivox) {
+      desc_target_ivox(s->h_descs[f], s->h_gdescs[f], fa);
+      GB_CUDA(cudaMemcpyAsync(s->d_gdescs + f, s->h_gdescs + f, sizeof(GicpDesc), cudaMemcpyHostToDevice, s->ctx->stream));
+    } else {
+      desc_target(s->h_descs[f], fa->target);
+    }
     GB_CUDA(cudaMemcpyAsync(s->d_descs + f, s->h_descs + f, sizeof(FactorDesc), cudaMemcpyHostToDevice, s->ctx->stream));
   }
   if (synced) {
@@ -651,6 +762,8 @@ static size_t sweep_layout(gb_sweep* s, Carver& d, Carver& h) {
   s->h_out = h.take<double>(GB_OUT_DOUBLES * F);
   s->h_descs = h.take<FactorDesc>(F);
   s->h_tiles = h.take<int2>(s->tiles_cap);
+  s->d_gdescs = s->gicp ? d.take<GicpDesc>(F) : nullptr;
+  s->h_gdescs = s->gicp ? h.take<GicpDesc>(F) : nullptr;
   return zero_bytes;
 }
 
@@ -663,13 +776,17 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   for (size_t f = 0; f < F; f++) {
     GB_REQUIRE(factors[f], "null factor");
     GB_REQUIRE(factors[f]->source->device == ctx->device && factors[f]->target->device == ctx->device, "factor lives on another device");
+    GB_REQUIRE((factors[f]->target->ivox != nullptr) == (factors[0]->target->ivox != nullptr), "the factors of one sweep must all be VGICP or all GICP factors");
     total_pts += factors[f]->source->n;
   }
+  const bool gicp = F > 0 && factors[0]->target->ivox != nullptr;
+  GB_REQUIRE(!gicp || !pair_index, "GICP sweeps take no pair_index (no slab can be attached to them)");
   GB_ENTER(ctx);
   gb_owned<gb_sweep> s(new (std::nothrow) gb_sweep(), sweep_free);
   if (!s) return GB_ERR_INTERNAL;
   ctx_retain(ctx);
   s->ctx = ctx; s->F = F; s->factors.assign(factors, factors + F);
+  s->gicp = gicp;
 
   // kernel generation and work-item policy
   // Kernel policy (A/B runs of the kernels, scripts/ab_sweep.py): small sweeps -- about one item per warp: an odometry
@@ -681,6 +798,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   const uint64_t warps = (uint64_t)s->capacity * 8;
   const bool small = F > 0 && total_pts <= warps * 2048;
   s->kernel_version = (kv == 3 || kv == 5) ? kv : (small ? 5 : 3);
+  if (gicp) s->kernel_version = 5;  // k_gicp_sweep runs sweep5's strided items at every size
   {
     // sweep3's items: ~6 items per warp (first one static, the rest drawn dynamically), between 128 and 2048 points each,
     // in whole rows of 32 points
@@ -691,6 +809,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   }
 
   std::vector<FactorDesc> descs(F);
+  std::vector<GicpDesc> gdescs(gicp ? F : 0);
   std::vector<int2> tiles;
   bool any_sv = false;
   for (size_t f = 0; f < F; f++) {
@@ -700,9 +819,9 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     const bool sv = (fa->flags & GB_FACTOR_SURFACE_VALIDATION) != 0;
     D.normals = sv ? fa->source->normals : nullptr;
     any_sv = any_sv || sv;
-    desc_target(D, fa->target);
+    if (gicp) desc_target_ivox(D, gdescs[f], fa); else desc_target(D, fa->target);
     s->target_versions.push_back(fa->target->version);
-    s->any_incremental = s->any_incremental || fa->target->incremental;
+    s->any_incremental = s->any_incremental || gicp || fa->target->incremental;
     D.n = (int)fa->source->n;
     D.pair = pair_index ? pair_index[f] : (int)f;
     s->h_pair.push_back(D.pair);
@@ -738,6 +857,10 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     memcpy(s->h_tiles, tiles.data(), sizeof(int2) * tiles.size());
     cudaStream_t st = ctx->stream;
     GB_CUDA(cudaMemcpyAsync(s->d_descs, s->h_descs, sizeof(FactorDesc) * F, cudaMemcpyHostToDevice, st));
+    if (gicp) {
+      memcpy(s->h_gdescs, gdescs.data(), sizeof(GicpDesc) * F);
+      GB_CUDA(cudaMemcpyAsync(s->d_gdescs, s->h_gdescs, sizeof(GicpDesc) * F, cudaMemcpyHostToDevice, st));
+    }
     GB_CUDA(cudaMemcpyAsync(s->d_tiles, s->h_tiles, sizeof(int2) * tiles.size(), cudaMemcpyHostToDevice, st));
     GB_CUDA(cudaMemsetAsync(s->d_accum, 0, zero_bytes, st));
     for (int k = 0; k < 2; k++) GB_CUDA(cudaEventCreateWithFlags(&s->pose_ev[k], cudaEventDisableTiming));
@@ -754,6 +877,7 @@ extern "C" gb_status gb_sweep_destroy(gb_sweep* s) { sweep_free(s); return GB_OK
 
 extern "C" gb_status gb_sweep_attach_slab(gb_sweep* s, void* device_slab_f32, size_t num_pairs) {
   GB_REQUIRE(s, "null sweep");
+  GB_REQUIRE(!s->gicp || !device_slab_f32, "no slab can be attached to a GICP sweep");
   for (size_t f = 0; f < s->F && device_slab_f32; f++)
     GB_REQUIRE(s->h_pair[f] >= 0 && (size_t)s->h_pair[f] < num_pairs, "pair index out of range for this slab");
   s->d_slab = (float*)device_slab_f32;
@@ -1068,6 +1192,7 @@ template <typename Layout> static gb_status dev_block_realloc(void** block, Layo
 extern "C" gb_status gb_sweep_attach_peer_slab(gb_sweep* s, gb_peer_slab* ps) {
   GB_REQUIRE(s, "null sweep");
   if (!ps) { s->peer = nullptr; return GB_OK; }
+  GB_REQUIRE(!s->gicp, "no peer slab can be attached to a GICP sweep");
   GB_REQUIRE(ps->ctx == s->ctx, "peer slab belongs to another context");
   GB_REQUIRE(ps->connected, "connect the peer slab (gb_peer_slab_connect) before attaching it");
   // CSR: global pair id -> this sweep's factor indices

@@ -81,7 +81,22 @@ struct gb_voxelmap {
   int* vn = nullptr;
   int* vstamp = nullptr;
   double* vsums = nullptr;     // 9 per voxel: q.x q.y q.z c00 c01 c02 c11 c12 c22
+  // A device iVox (gb_ivox_create / gb_ivox_insert) is a gb_voxelmap with this state: the gb_ivox handle is the map itself,
+  // so one free function, one device and one table serve both.  Its block in `base` holds the stored points as 48-byte
+  // records in `voxels` (3 float4 each, the voxel-record layout: {x y z c00} {c01 c02 c11 c12} {c22, 1, 0, 0}), voxel-major
+  // in ascending packed-key order, then per voxel its cell {first point, count} (ivox->cells), key (vkeys) and stamp (vstamp);
+  // lru_* and version are the incremental map's.  nullptr for every voxel map.
+  struct gb_ivox_state* ivox = nullptr;
 };
+struct gb_ivox_state {
+  double resolution = 0.0, min_dist = 0.0;  // the map's float resolution / inv_res: (float) of these, inv_res = (float)(1 / r)
+  int max_points = 10, mode = 1;
+  size_t num_points = 0;
+  int2* cells = nullptr;
+};
+// the handle of an iVox is its gb_voxelmap (gb_ivox stays an incomplete type)
+inline gb_voxelmap* ivox_map(gb_ivox* h) { return reinterpret_cast<gb_voxelmap*>(h); }
+inline const gb_voxelmap* ivox_map(const gb_ivox* h) { return reinterpret_cast<const gb_voxelmap*>(h); }
 
 // device-side factor descriptor (80 B)
 struct FactorDesc {
@@ -101,10 +116,19 @@ struct FactorDesc {
   int chunk;       // sweep3: points per item of THIS factor (the last factors of a sweep get smaller items: tail tapering)
 };
 static_assert(sizeof(FactorDesc) == 80, "FactorDesc size");
+// The rest of a GICP factor's descriptor (k_gicp_sweep): its FactorDesc carries the iVox's table (buckets, mask, max_scan,
+// inv_res) and its point records (voxels); this adds the cells, the correspondence bound and the searched offsets.
+struct GicpDesc {
+  const int2* cells;
+  float max_corr2;   // (float)(max_correspondence_distance^2)
+  int num_offsets;   // neighbor_voxel_mode
+};
+static_assert(sizeof(GicpDesc) == 16, "GicpDesc size");
 
 struct gb_factor {
   gb_ctx* ctx = nullptr;
-  const gb_voxelmap* target = nullptr;
+  const gb_voxelmap* target = nullptr;  // the voxel map, or the iVox of a GICP factor (target->ivox != nullptr)
+  float max_corr2 = 0.f;                // GICP: (float)(max_correspondence_distance^2)
   const gb_cloud* source = nullptr;
   int flags = 0;
   gb_sweep* single = nullptr;  // lazily created 1-factor sweep
@@ -192,6 +216,11 @@ struct gb_sweep {
   gb_pool_block blk;                // the device and pinned blocks, laid out by sweep_layout; back to the context's pool at the end
   bool any_incremental = false;     // some target is an incremental map: its descriptor may go stale (gb_voxelmap_insert)
   std::vector<uint64_t> target_versions;  // per factor: the target version its descriptor was written from
+  // GICP sweeps (every factor on an iVox; a sweep holds one kind): k_gicp_sweep over sweep5's strided items, with the
+  // GICP half of each descriptor next to the FactorDesc table
+  bool gicp = false;
+  GicpDesc* d_gdescs = nullptr;
+  GicpDesc* h_gdescs = nullptr;
 };
 
 // A context's grow-only buffer: device scratch or pinned host staging.  What it holds is valid until the next gb_carve on it.
@@ -364,11 +393,14 @@ gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n, const gb_planes& st
 // kernel launchers (gb_kernels_*.cu)
 enum { GB_MODE_LINEARIZE = 0, GB_MODE_ERROR = 1 };
 gb_status gb_launch_sweep(gb_sweep* s, int mode);
+gb_status gb_launch_gicp_sweep(gb_sweep* s, int mode);  // gb_launch_sweep of a GICP sweep
 gb_status gb_launch_peer_signal_wait(gb_peer_slab* ps);
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count);
 gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_buckets, int max_scan, double drop_rate, gb_voxelmap* out);
 gb_status gb_voxelmap_create_incremental_impl(gb_ctx* ctx, gb_voxelmap* m);
 gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, unsigned long long seed);
+gb_status gb_ivox_create_impl(gb_ctx* ctx, gb_voxelmap* m);
+gb_status gb_ivox_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, unsigned long long seed);
 // Shared with gb_merge_frames (gb_kernels_preprocess.cu): one frame's points q = R a + t and covariances R C R^T in
 // un-contracted fp64, in the caller's point order (pts: n x double4, cov6: n x 6 upper triangle).  d_frame: GB_FRAME_DESC_BYTES
 // of device scratch for the frame descriptor.  One launch.

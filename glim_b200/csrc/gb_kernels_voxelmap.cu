@@ -425,6 +425,253 @@ gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* c
   return GB_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// The device iVox (gb_ivox_create / gb_ivox_insert; the rule is written once in include/glim_b200.h).  One insert:
+//   1. k_ivox_old_keys     one entry per STORED point (idx = -1 - record), ahead of the frame's points
+//   2. the voxel map's steps 1-2 (transform, fp64 keys, sampling) and gb_group_by_key: a voxel's group is its stored points
+//      in slot order, then its new points in index order
+//   3. k_ivox_merge        one thread per merged voxel: the sequential admission, the stamp, the eviction
+//   4. two scans + k_ivox_count: surviving voxels and points (one host synchronisation)
+//   5. k_ivox_emit         the survivors into a new block: cells, keys, stamps and the point records
+//   6. table_build         the build's table kernels, with drop rate 0: every voxel is found
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+constexpr int kIvoxInitBuckets = 16384;
+
+__global__ void k_ivox_old_keys(int V, const unsigned long long* __restrict__ vkeys, const int2* __restrict__ cells, unsigned long long* __restrict__ keys, int* __restrict__ idx) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  const int2 c = cells[v];
+  const unsigned long long key = vkeys[v];
+  for (int s = 0; s < c.y; s++) {
+    keys[c.x + s] = key;
+    idx[c.x + s] = -1 - (c.x + s);
+  }
+}
+
+// the fp32 position of a group entry: a stored record (ref < 0) or a new point
+__device__ __forceinline__ float3 ivox_entry_pos(int ref, const float4* __restrict__ opoints, const double4* __restrict__ pts) {
+  if (ref < 0) {
+    const float4 p = opoints[3 * (size_t)(-1 - ref)];
+    return make_float3(p.x, p.y, p.z);
+  }
+  const double4 q = pts[ref];
+  return make_float3((float)q.x, (float)q.y, (float)q.z);
+}
+
+// mref[b .. b + mcount[v]) = the entries voxel v keeps (stored ones first, then the admitted new points in index order)
+__global__ void k_ivox_merge(int N, const int* __restrict__ num_merged, const int* __restrict__ starts, const unsigned long long* __restrict__ keys_s, const int* __restrict__ idx_s,
+                             int Vo, const unsigned long long* __restrict__ ovkeys, const int* __restrict__ ostamp, const float4* __restrict__ opoints,
+                             const double4* __restrict__ pts, int max_points, double min_d2, int counter, int horizon, int cycle,
+                             int* __restrict__ mref, int* __restrict__ mcount, int* __restrict__ mstamp, int* __restrict__ keep) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= N) return;
+  if (v >= *num_merged) { keep[v] = 0; mcount[v] = 0; return; }
+  const int b = starts[v], e = starts[v + 1];
+  int cnt = 0, stamp = counter;
+  bool touched = false;
+  if (idx_s[b] < 0) {  // a stored voxel: its stamp (the stored keys are ascending)
+    const unsigned long long key = keys_s[b];
+    int lo = 0, hi = Vo;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (ovkeys[mid] < key) lo = mid + 1; else hi = mid;
+    }
+    stamp = ostamp[lo];
+  }
+  for (int j = b; j < e; j++) {
+    const int i = idx_s[j];
+    if (i < 0) { mref[b + cnt++] = i; continue; }
+    touched = true;
+    if (cnt >= max_points) continue;
+    const float3 a = ivox_entry_pos(i, opoints, pts);
+    bool ok = true;
+    for (int k = 0; k < cnt && ok; k++) {
+      const float3 p = ivox_entry_pos(mref[b + k], opoints, pts);
+      const double dx = (double)p.x - (double)a.x, dy = (double)p.y - (double)a.y, dz = (double)p.z - (double)a.z;
+      const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+      ok = d2 >= min_d2;
+    }
+    if (ok) mref[b + cnt++] = i;
+  }
+  if (touched) stamp = counter;
+  const int c1 = counter + 1;
+  const bool evict = horizon > 0 && c1 % cycle == 0 && stamp + horizon < c1;
+  keep[v] = evict ? 0 : 1;
+  mcount[v] = evict ? 0 : cnt;
+  mstamp[v] = stamp;
+}
+__global__ void k_ivox_count(int N, const int* __restrict__ kpos, const int* __restrict__ ppos, unsigned long long* __restrict__ info) {
+  info[0] = (unsigned long long)ppos[N - 1];
+  info[1] = (unsigned long long)kpos[N - 1];
+}
+
+__global__ void k_ivox_emit(int N, const int* __restrict__ num_merged, const int* __restrict__ keep, const int* __restrict__ kpos, const int* __restrict__ ppos,
+                            const int* __restrict__ starts, const unsigned long long* __restrict__ keys_s, const int* __restrict__ mref, const int* __restrict__ mcount,
+                            const int* __restrict__ mstamp, const float4* __restrict__ opoints, const double4* __restrict__ pts, const double* __restrict__ cov6,
+                            unsigned long long* __restrict__ vkeys, int* __restrict__ vstamp, int2* __restrict__ cells, float4* __restrict__ points, int4* __restrict__ vcoord) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= N || v >= *num_merged || !keep[v]) return;
+  const int o = kpos[v] - 1;
+  const int cnt = mcount[v];
+  const int first = ppos[v] - cnt;
+  const int b = starts[v];
+  const unsigned long long key = keys_s[b];
+  vkeys[o] = key;
+  vstamp[o] = mstamp[v];
+  cells[o] = make_int2(first, cnt);
+  int x, y, z;
+  gb_unpack_key(key, x, y, z);
+  vcoord[o] = make_int4(x, y, z, cnt);
+  for (int k = 0; k < cnt; k++) {
+    const int ref = mref[b + k];
+    float4* dst = points + 3 * (size_t)(first + k);
+    if (ref < 0) {
+      const float4* src = opoints + 3 * (size_t)(-1 - ref);
+      dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
+    } else {
+      const double4 q = pts[ref];
+      const double* c = cov6 + 6 * (size_t)ref;
+      dst[0] = make_float4((float)q.x, (float)q.y, (float)q.z, (float)c[0]);
+      dst[1] = make_float4((float)c[1], (float)c[2], (float)c[3], (float)c[4]);
+      dst[2] = make_float4((float)c[5], 1.f, 0.f, 0.f);
+    }
+  }
+}
+
+// the state block of V voxels and P points: point records first (gb_voxelmap::voxels), then cells, keys and stamps
+void ivox_layout(Carver& cv, size_t V, size_t P, gb_voxelmap* m, int2** cells) {
+  m->voxels = cv.take<float4>(3 * P);
+  *cells = cv.take<int2>(V);
+  m->vkeys = cv.take<unsigned long long>(V);
+  m->vstamp = cv.take<int>(V);
+}
+
+}  // namespace
+
+gb_status gb_ivox_create_impl(gb_ctx* ctx, gb_voxelmap* m) {
+  m->device = ctx->device;
+  m->max_scan = 10;
+  m->init_buckets = kIvoxInitBuckets;
+  int dropped = 0;
+  GB_CHECK(table_build(ctx, 0, nullptr, nullptr, kIvoxInitBuckets, m->max_scan, 0.0, 0.0, &m->buckets, &m->num_buckets, &dropped));
+  m->bytes = sizeof(int4) * (size_t)m->num_buckets;
+  return GB_OK;
+}
+
+gb_status gb_ivox_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T, double sampling_rate, unsigned long long seed) {
+  cudaStream_t st = ctx->stream;
+  gb_ivox_state* iv = m->ivox;
+  const int n = (int)cloud->n;
+  const int Vo = m->num_voxels;
+  const int Po = (int)iv->num_points;
+  const int kept = sampling_rate < 1.0 ? (int)(size_t)((double)n * sampling_rate) : n;  // random_sampling's count
+  const int np = kept > 0 ? n : 0;
+  const int N = Po + np;
+  gb_voxelmap next = *m;  // the map after this insert (with next_cells / next_points); m is replaced only when everything has succeeded
+  int2* next_cells = iv->cells;
+  size_t next_points = iv->num_points;
+  next.lru_counter = m->lru_counter + 1;
+  next.version = m->version + 1;
+  if (N > 0) {
+    const size_t cub_b = gb_cub_temp_bytes((size_t)N);
+    gb_sort_tmp t;
+    int *d_flags, *d_pos, *d_starts, *d_keep, *d_kpos, *d_ppos, *d_mcount, *d_mstamp, *d_mref, *d_dropped;
+    double4* d_pts = nullptr;
+    double* d_cov = nullptr;
+    unsigned long long *d_hash = nullptr, *d_info;
+    void* d_frame;
+    int4* d_vcoord;
+    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+      t = gb_take_sort_tmp(cv, (size_t)N, cv.take<char>(cub_b), cub_b);
+      d_flags = cv.take<int>(N + 1);
+      d_pos = cv.take<int>(N + 1);
+      d_starts = cv.take<int>(N + 1);
+      d_keep = cv.take<int>(N + 1);
+      d_kpos = cv.take<int>(N + 1);
+      d_ppos = cv.take<int>(N + 1);
+      d_mcount = cv.take<int>(N + 1);
+      d_mstamp = cv.take<int>(N);
+      d_mref = cv.take<int>(N);
+      d_vcoord = cv.take<int4>(N);
+      d_dropped = cv.take<int>(1);
+      d_info = cv.take<unsigned long long>(2);  // {surviving points, surviving voxels}
+      d_frame = cv.take<char>(GB_FRAME_DESC_BYTES);
+      if (np > 0) {
+        d_pts = cv.take<double4>(np);
+        d_cov = cv.take<double>(6 * (size_t)np);
+        if (kept < n) d_hash = cv.take<unsigned long long>(np);
+      }
+    }));
+    const int tb = 256;
+    if (Vo > 0) {
+      GB_CHECK(gb_launch(ctx, "k_ivox_old_keys", k_ivox_old_keys, (Vo + tb - 1) / tb, tb, 0, Vo, m->vkeys, iv->cells, t.keys, t.idx));
+    }
+    if (np > 0) {
+      GB_CHECK(gb_transform_frame(ctx, cloud, T, d_frame, d_pts, d_cov));
+      GB_CHECK(gb_grid_keys(ctx, np, d_pts, 1.0 / iv->resolution, t.keys + Po, t.idx + Po));
+      if (kept < n) {
+        GB_CHECK(gb_launch(ctx, "k_ins_sample_hash", k_ins_sample_hash, (np + tb - 1) / tb, tb, 0, np, seed, t.keys_s));
+        GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, cub_b, t.keys_s, d_hash, np, 0, 64);
+        GB_CHECK(gb_launch(ctx, "k_ins_sample_drop", k_ins_sample_drop, (np + tb - 1) / tb, tb, 0, np, kept, seed, d_hash, t.keys + Po));
+      }
+    }
+    GB_CHECK(gb_group_by_key(ctx, N, t, d_flags, d_pos));
+    GB_CHECK(gb_group_starts(ctx, N, t, d_flags, d_pos, d_starts));
+    GB_CHECK(gb_launch(ctx, "k_ivox_merge", k_ivox_merge, (N + 127) / 128, 128, 0, N, d_pos + (N - 1), d_starts, t.keys_s, t.idx_s, Vo, m->vkeys, m->vstamp, m->voxels, d_pts,
+                       iv->max_points, iv->min_dist * iv->min_dist, m->lru_counter, m->lru_horizon, m->lru_clear_cycle, d_mref, d_mcount, d_mstamp, d_keep));
+    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_keep, d_kpos, N);
+    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_mcount, d_ppos, N);
+    GB_CHECK(gb_launch(ctx, "k_ivox_count", k_ivox_count, 1, 1, 0, N, d_kpos, d_ppos, d_info));
+    unsigned long long info[2] = {0, 0};
+    GB_CUDA(cudaMemcpyAsync(info, d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaStreamSynchronize(st));
+    const int V = (int)info[1];
+    const size_t P = (size_t)info[0];
+    next.base = nullptr;
+    next.buckets = nullptr;
+    next.num_voxels = V;
+    next_points = P;
+    Carver size;
+    ivox_layout(size, (size_t)V, P, &next, &next_cells);
+    next.bytes = V > 0 ? size.off : 0;
+    if (V > 0) {
+      GB_CUDA(gb_dev_malloc(ctx->device, size.off, &next.base));
+      Carver cv{(char*)next.base};
+      ivox_layout(cv, (size_t)V, P, &next, &next_cells);
+      gb_status s = gb_launch(ctx, "k_ivox_emit", k_ivox_emit, (N + tb - 1) / tb, tb, 0, N, d_pos + (N - 1), d_keep, d_kpos, d_ppos, d_starts, t.keys_s, d_mref, d_mcount, d_mstamp,
+                              m->voxels, d_pts, d_cov, next.vkeys, next.vstamp, next_cells, next.voxels, d_vcoord);
+      if (s != GB_OK) { gb_dev_free(ctx->device, next.base); return s; }
+    } else {
+      next.voxels = nullptr; next_cells = nullptr; next.vkeys = nullptr; next.vstamp = nullptr;
+    }
+    int dropped = 0;
+    gb_status s = table_build(ctx, V, d_vcoord, d_dropped, kIvoxInitBuckets, m->max_scan, 0.0, (double)P, &next.buckets, &next.num_buckets, &dropped);
+    if (s == GB_OK && dropped != 0) {
+      gb_set_error("iVox table: %d points left out of a table of %d buckets", dropped, next.num_buckets);
+      s = GB_ERR_INTERNAL;
+    }
+    if (s != GB_OK) {
+      gb_dev_free(ctx->device, next.base);
+      gb_dev_free(ctx->device, next.buckets);
+      return s;
+    }
+    next.bytes += sizeof(int4) * (size_t)next.num_buckets;
+  }
+  void* old_base = m->base;
+  int4* old_buckets = m->buckets;
+  const bool replaced = N > 0;
+  *m = next;
+  iv->cells = next_cells;
+  iv->num_points = next_points;
+  if (replaced) {
+    gb_dev_free(ctx->device, old_base);
+    gb_dev_free(ctx->device, old_buckets);
+  }
+  return GB_OK;
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Morton reordering of a new cloud (PointCloudGPU::clone keeps the caller's order on the host side of the

@@ -9,6 +9,8 @@ include/glim_b200/gtsam_points_compat.hpp.
     IntegratedVGICPFactorGPU(target_key | fixed_target_pose, source_key, voxelmap, source)   :144, :161
     NonlinearFactorSetGPU.add(...) / .linearize(values)     odometry_estimation_gpu.cpp:383-386
     overlap_gpu(voxelmap(s), source, delta(s))              odometry_estimation_gpu.cpp:231, :248
+    IVoxGPU(resolution, min_dist, ...).insert(cloud, T, rate)   gtsam_points::iVox, odometry_estimation_cpu.cpp:57-61, :177-191
+    IntegratedGICPFactorGPU(target, source_key, ivox, source, max_corr)   odometry_estimation_cpu.cpp:95-104
     align_vgicp(problems, T_init, params)                   the LM loop of odometry_estimation_cpu.cpp:105-150 /
                                                             global_mapping_pose_graph.cpp:405-417, many problems per call
 """
@@ -273,6 +275,75 @@ class IntegratedVGICPFactorGPU:
         if getattr(self, "h", None) and self.ctx.h:
             lib().gb_vgicp_factor_destroy(self.h)
             self.h = None
+
+
+class IVoxGPU:
+    """gtsam_points::iVox kept on the device (gb_ivox_create / gb_ivox_insert): the GICP target of GLIM's CPU odometry
+    (odometry_estimation_cpu.cpp:57-61, update_target :177-191).  Factors and sweeps on it follow its inserts."""
+
+    def __init__(self, resolution: float, min_dist_in_cell: float = 0.1, max_points_in_cell: int = 10, neighbor_voxel_mode: int = 1,
+                 lru_horizon: int = 100, lru_clear_cycle: int = 10, ctx: Context | None = None):
+        self.ctx = ctx or default_context()
+        self.resolution = float(resolution)
+        self.h = None
+        h = C.c_void_p()
+        check(lib().gb_ivox_create(self.ctx.h, self.resolution, float(min_dist_in_cell), int(max_points_in_cell), int(neighbor_voxel_mode),
+                                   int(lru_horizon), int(lru_clear_cycle), C.byref(h)))
+        self.h = h
+        self.info()
+
+    def info(self):
+        """-> (num_voxels, num_points, resolution)"""
+        nv, npt, res = C.c_int(), C.c_size_t(), C.c_double()
+        check(lib().gb_ivox_info(self.h, C.byref(nv), C.byref(npt), C.byref(res)))
+        self.num_voxels, self.num_points = nv.value, npt.value
+        return nv.value, npt.value, res.value
+
+    def insert(self, cloud: PointCloudGPU, T=None, sampling_rate: float = 1.0, seed: int = 0):
+        """Insert `cloud` at T_map_cloud (4x4, None = identity), keeping a sampling_rate share of its points."""
+        Tc = pose16(np.asarray(T, dtype=np.float64).reshape(4, 4)) if T is not None else None
+        check(lib().gb_ivox_insert(self.ctx.h, self.h, cloud.h, ptr(Tc), float(sampling_rate), int(seed)))
+        self.info()
+        return self
+
+    def voxel_resolution(self) -> float:
+        return self.resolution
+
+    def download(self):
+        """-> voxel coords (V,3) int32 in ascending key order, counts (V,) int32, points (P,3) f32 and covariances (P,6) f32
+        voxel-major in slot order"""
+        V, P = self.num_voxels, self.num_points
+        coords, counts = np.empty((V, 3), np.int32), np.empty(V, np.int32)
+        xyz, cov6 = np.empty((P, 3), np.float32), np.empty((P, 6), np.float32)
+        check(lib().gb_ivox_download(self.h, ptr(coords), ptr(counts), ptr(xyz), ptr(cov6)))
+        return coords, counts, xyz, cov6
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx and self.ctx.h:
+            lib().gb_ivox_destroy(self.h)
+            self.h = None
+
+
+class IntegratedGICPFactorGPU(IntegratedVGICPFactorGPU):
+    """IntegratedGICPFactor_<iVox, PointCloud>(target, source_key, ivox, source) + set_max_correspondence_distance
+    (odometry_estimation_cpu.cpp:95-104) on the device: a gb_factor like the VGICP one, so NonlinearFactorSetGPU, Sweep and
+    align_vgicp take it (one kind of factor per set, sweep or call)."""
+
+    def __init__(self, target, source_key, ivox: IVoxGPU, source: PointCloudGPU, max_correspondence_distance: float, ctx: Context | None = None):
+        super().__init__(target, source_key, ivox, source, ctx=ctx)
+        self.ivox = ivox
+        self.max_correspondence_distance = float(max_correspondence_distance)
+
+    def set_enable_surface_validation(self, enable: bool):
+        if enable:
+            raise capi.GlimB200Error("surface validation is a VGICP factor option")
+
+    def _handle(self):
+        if self.h is None:
+            h = C.c_void_p()
+            check(lib().gb_gicp_factor_create(self.ctx.h, self.ivox.h, self.source.h, self.max_correspondence_distance, C.byref(h)))
+            self.h = h
+        return self.h
 
 
 class NonlinearFactorSetGPU:

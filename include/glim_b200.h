@@ -51,6 +51,7 @@ typedef struct gb_cloud gb_cloud;       /* gtsam_points::PointCloudGPU          
 typedef struct gb_voxelmap gb_voxelmap; /* gtsam_points::GaussianVoxelMapGPU                                        */
 typedef struct gb_factor gb_factor;     /* gtsam_points::IntegratedVGICPFactorGPU                                   */
 typedef struct gb_sweep gb_sweep;       /* gtsam_points::NonlinearFactorSetGPU (a prepared batch of factors)        */
+typedef struct gb_ivox gb_ivox;         /* gtsam_points::iVox (odometry_estimation_cpu.cpp:57-61), kept on the device */
 #define GB_SLAB_STRIDE 96               /* floats per row of the per-pair Hessian slab (layout below, at gb_sweep_create) */
 
 /* LinearizedSystem6 of the reference GPU factor, widened to fp64 (SURVEY.md 8(a) a4, A.3).
@@ -154,6 +155,42 @@ GB_API gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolution, i
 GB_API gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_cloud* cloud, const double* T_map_cloud /* 16, col-major */,
                                     double sampling_rate, uint64_t seed);
 
+/* ---- iVox: the scan-to-map target of GLIM's odometry with registration_type "GICP" (odometry_estimation_cpu.cpp:57-61:
+ *      gtsam_points::iVox(ivox_resolution = 1.0), set_min_dist_in_cell(ivox_min_dist = 0.1), set_lru_horizon(lru_thresh = 100),
+ *      set_neighbor_voxel_mode(1); update_target :177-191 inserts 10 % of each frame from frame 5 on), kept on the device.
+ *      Each voxel holds a few actual points with their covariances.
+ *
+ *      The insert rule.  Per voxel the map keeps its packed key, its points in slot order and its stamp; per map the insert
+ *      counter c, h = lru_horizon and k = lru_clear_cycle.  One insert:
+ *        1-3. sample, transform and key exactly as gb_voxelmap_insert steps 1-3, with the key floor(q * (1.0 / resolution)) in
+ *           fp64 (resolution is a double here).
+ *        4. per touched voxel, sequentially: the stored points keep their slots; the new points are offered in original index
+ *           order, and a point is admitted iff the voxel holds fewer than max_points_in_cell points and its squared distance to
+ *           every point the voxel holds is >= min_dist_in_cell^2.  Stored values are the fp32 roundings of q and C'; the
+ *           admission distance is computed in fp64 from the fp32-rounded positions, d2 = (dx^2 + dy^2) + dz^2, uncontracted.
+ *           Every touched voxel gets stamp = c, also one whose new points were all refused.
+ *        5. evict as gb_voxelmap_insert step 5: c += 1; if h > 0 and c % k == 0, the voxels with stamp + h < c are dropped; an
+ *           insert that keeps no points still advances c.
+ *        6. voxels in ascending packed-key order; the table is the build's (16384 buckets doubled until >= 8 V, 10 probes)
+ *           with drop rate 0: every voxel is found.
+ *      [EXT] gtsam_points is not vendored: the cell capacity 10 (max_points_in_cell default, recalled), the admission test of
+ *      step 4 and the neighbour offsets below are this library's statement of it.
+ *      Threading and lifetime as for incremental voxel maps: two host synchronisations per insert (one more per extra table
+ *      attempt), sweeps created before an insert follow it, do not insert while another thread uses the map. ---- */
+/* neighbor_voxel_mode: 1 (centre), 7 (+ the faces), 19 (+ the edges), 27 (+ the corners).  lru_horizon <= 0: no eviction.
+ * GB_ERR_INVALID_ARGUMENT for a non-finite or non-positive resolution, min_dist_in_cell < 0, max_points_in_cell outside
+ * [1, 64], another mode or lru_clear_cycle < 1. */
+GB_API gb_status gb_ivox_create(gb_ctx* ctx, double resolution, double min_dist_in_cell, int max_points_in_cell, int neighbor_voxel_mode,
+                                int lru_horizon, int lru_clear_cycle, gb_ivox** out);
+/* validated before any launch: T finite, sampling_rate in (0, 1], cloud and map on ctx's device */
+GB_API gb_status gb_ivox_insert(gb_ctx* ctx, gb_ivox* map, const gb_cloud* cloud, const double* T_map_cloud /* 16 col-major, NULL = I */,
+                                double sampling_rate, uint64_t seed);
+GB_API gb_status gb_ivox_info(const gb_ivox* map, int* num_voxels, size_t* num_points, double* resolution);
+/* voxels in ascending packed-key order; points voxel-major, in slot order; any pointer may be NULL */
+GB_API gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords /* V x 3 */, int32_t* voxel_counts /* V */,
+                                  float* xyz /* P x 3 */, float* cov6 /* P x 6 */);
+GB_API gb_status gb_ivox_destroy(gb_ivox* map);
+
 /* ---- IntegratedVGICPFactorGPU(target_key | fixed_target_pose, source_key, voxelmap, source, stream, buffer)
  *      (odometry_estimation_gpu.cpp:144,161; sub_mapping.cpp:307; global_mapping.cpp:335,466,860).
  *      Keys and the binary/unary distinction stay on the host side of the boundary: the device only
@@ -166,6 +203,28 @@ GB_API gb_status gb_vgicp_linearize(gb_factor* factor, const double T_target_sou
 GB_API gb_status gb_vgicp_error(gb_factor* factor, const double T_lin[16], const double T_eval[16], double* error);
 /* num_inliers() / inlier_fraction() come back in gb_linearized6::num_inliers */
 
+/* ---- IntegratedGICPFactor_<iVox, PointCloud>(Pose3(), X(current), ivox, frame, ivox) + set_max_correspondence_distance
+ *      (odometry_estimation_cpu.cpp:95-104, max_correspondence_distance = 2 * ivox_resolution).  The source must carry
+ *      covariances, as for VGICP.  The result is an ordinary gb_factor: gb_vgicp_linearize / _error / _factor_destroy,
+ *      gb_factor_set_*, gb_sweep_* and gb_vgicp_align take it.  The factors of one sweep or call must all be VGICP or all GICP
+ *      (GB_ERR_INVALID_ARGUMENT before any launch); GICP sweeps take no pair_index, slab or peer slab; gb_overlap stays
+ *      voxel-map only.
+ *
+ *      The correspondence rule.  q = the source point transformed with the sweep's fp32 pose (the lookup transform of every
+ *      sweep), keyed with the fp32 rule (float)(1 / resolution) of every lookup (a point on a voxel face may key to its
+ *      neighbour).  The voxels (cx, cy, cz) + o are searched for o in the mode's offset list, in order: the centre; the faces
+ *      -x +x -y +y -z +z; the edges (zero axis x, y, z; the other two signs --, -+, +-, ++); the corners ((dx, dy, dz) in
+ *      {-1, 1}^3, lexicographic).  The fp32 squared distance d2 = (dx^2 + dy^2) + dz^2 (d = p - q, uncontracted) to every
+ *      stored point is formed; the nearest point with d2 < (float)(max_correspondence_distance^2) is the correspondence, ties
+ *      to the earlier offset, then the earlier slot.  The per-point arithmetic is the VGICP factor's with the matched point's
+ *      position and covariance in place of the voxel's mean and covariance: r = p - q, M = (C_p + R C_a R^T)^-1,
+ *      error = sum r^T M r (no 1/2), and error() takes its correspondences at T_lin and evaluates at T_eval.
+ *      [EXT] "nearest stored point within the maximum distance" and this error convention are this library's statement of the
+ *      un-vendored gtsam_points factor.
+ *      gb_sweep_stats of a GICP sweep: 48 B per source point, 48 B per stored target point, 16 B per bucket of the smallest
+ *      power-of-two table >= 16384 holding the voxels, plus pose and record. ---- */
+GB_API gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out);
+
 /* ---- NonlinearFactorSetGPU::add(graph) / ::linearize(values) (odometry_estimation_gpu.cpp:383-386;
  *      hook at src/glim/viewer/offline_viewer.cpp:29): F x 64 B of poses down, one launch over all
  *      factors, F records up. ---- */
@@ -176,7 +235,8 @@ GB_API gb_status gb_factor_set_error(gb_ctx* ctx, size_t num_factors, gb_factor*
  *      (odometry_estimation_cpu.cpp:105-150: one unary IntegratedVGICPFactor(Pose3(), X(current), voxelmap, frame) per level,
  *      LevenbergMarquardtOptimizerExt; global_mapping_pose_graph.cpp:405-417: loop candidates, 10 iterations each).
  *      A problem is the set of factors (levels) that share one unknown T_target_source, the target pose fixed to identity;
- *      the factors of problem p are factors[factor_offsets[p] .. factor_offsets[p+1]).  Factors keep their flags.
+ *      the factors of problem p are factors[factor_offsets[p] .. factor_offsets[p+1]).  Factors keep their flags.  The factors
+ *      may be VGICP (gb_vgicp_factor_create) or GICP (gb_gicp_factor_create) factors, all of one kind per call.
  *
  *      The rule (gtsam_points' LevenbergMarquardtOptimizerExt is not vendored: GTSAM's documented LM defaults plus GLIM's
  *      termination callback, DESIGN.md section 7 [EXT]).  Per problem, T = T_init, lambda = lambda_initial, need_lin = 1;

@@ -8,7 +8,10 @@
       frame with the maps kept on the host: the frame is sampled and transformed on the host, inserted into the oracle's
       GaussianVoxelMapCPU (go_cpumap), and the map is uploaded again as a cloud of its voxels and rebuilt with
       gb_voxelmap_build.  The uploaded content is the device map's voxel set, which is the host map's up to key rounding:
-      the upload and build costs depend only on its size.
+      the upload and build costs depend only on its size;
+  (d) the GICP configuration GLIM ships (registration_type "GICP"): a 1.0 m device iVox grown over the warm frames, then per
+      frame one device odometry frame -- gb_vgicp_align on one GICP factor (max_iterations 8) plus the insert at rate 0.1 --
+      with the insert also reported on its own.
 
 Times are a host clock around synchronised calls, median over the timed frames.  Launch counts come from
 gb_ctx_kernel_launches.  Every line carries the card's name and power limit, read in the same run.
@@ -134,6 +137,35 @@ def main():
     emit(leg="odometry_frame/device_maps", median_ms=round(d, 3), runs_ms=[round(t * 1e3, 3) for t in dev_ms], kernel_launches=int(np.median(dev_launches)))
     emit(leg="odometry_frame/host_maps", median_ms=round(h, 3), runs_ms=[round(t * 1e3, 3) for t in host_ms])
     emit(odometry_frame_speedup_device_vs_host=round(h / d, 2))
+
+    # (d) the GICP configuration GLIM ships: a 1.0 m iVox (min_dist 0.1, mode 1, LRU 100 / 10) grown over the warm frames,
+    #     then per frame one device odometry frame (GICP align, max_iterations 8, max_correspondence_distance 2.0, then the
+    #     insert at rate 0.1), with the insert also timed on its own
+    ivox = gpu.IVoxGPU(1.0, 0.1, 10, 1, 100, 10, ctx=ctx)
+    for k in range(args.warm):
+        ivox.insert(clouds[k], gt[k], rate_of(k), seed=k)
+    ins_ms, ins_launches, frame_ms, frame_launches = [], [], [], []
+    est = gt[args.warm - 1]
+    rng = synth.rng_for(523)
+    for k in range(args.warm, n_frames):
+        inc = synth.perturb(synth.inv_pose(gt[k - 1]) @ gt[k], rng, 0.01, 0.1)
+        l0 = ctx.kernel_launches
+        t0 = time.perf_counter()
+        fac = gpu.IntegratedGICPFactorGPU(np.eye(4), 0, ivox, clouds[k], 2.0, ctx=ctx)
+        T = gpu.align_vgicp([[fac]], [est @ inc], params=gpu.align_params(max_iterations=8))[0]["T_target_source"]
+        l1 = ctx.kernel_launches
+        t1 = time.perf_counter()
+        ivox.insert(clouds[k], T, 0.1, seed=k)
+        t2 = time.perf_counter()
+        ins_ms.append(t2 - t1)
+        ins_launches.append(ctx.kernel_launches - l1)
+        frame_ms.append(t2 - t0)
+        frame_launches.append(ctx.kernel_launches - l0)
+        est = T
+    emit(leg="gicp/insert/hdl32/1.0m", median_ms=round(float(np.median(ins_ms[1:])) * 1e3, 3), runs_ms=[round(t * 1e3, 3) for t in ins_ms],
+         kernel_launches=int(np.median(ins_launches)), frame_points=int(clouds[-1].n), sampling_rate=0.1)
+    emit(leg="gicp/odometry_frame/device_ivox", median_ms=round(float(np.median(frame_ms[1:])) * 1e3, 3), runs_ms=[round(t * 1e3, 3) for t in frame_ms],
+         kernel_launches=int(np.median(frame_launches)), ivox_voxels=ivox.num_voxels, ivox_points=ivox.num_points)
 
 
 if __name__ == "__main__":
