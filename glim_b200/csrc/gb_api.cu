@@ -328,8 +328,43 @@ extern "C" gb_status gb_cloud_destroy(gb_cloud* c) {
 static void voxelmap_free(gb_voxelmap* m) {
   gb_dev_free(m->device, m->base);
   gb_dev_free(m->device, m->buckets);
-  delete m->ivox;
   delete m;
+}
+// an empty incremental map or iVox of the parameters in `init` (the caller has entered ctx)
+static gb_status map_create_empty(gb_ctx* ctx, const gb_voxelmap& init, gb_voxelmap** out) {
+  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(init), voxelmap_free);
+  if (!m) return GB_ERR_INTERNAL;
+  GB_CHECK(gb_map_create_empty_impl(ctx, m.get()));
+  *out = m.release();
+  return GB_OK;
+}
+// The checks both inserts make before any launch, the handles read last; *T is the pose to insert at.
+static gb_status insert_args(gb_ctx* ctx, const gb_voxelmap* m, gb_map_kind kind, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, const double** T) {
+  GB_REQUIRE(ctx && m && cloud, "null argument");
+  GB_REQUIRE(sampling_rate > 0.0 && sampling_rate <= 1.0, "sampling_rate must be in (0, 1]");
+  static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  *T = T_map_cloud ? T_map_cloud : kIdentity;
+  for (int k = 0; k < 16; k++) GB_REQUIRE(std::isfinite((*T)[k]), "T_map_cloud must be finite");
+  GB_REQUIRE(m->kind == kind, kind == GB_MAP_IVOX ? "the map is not an iVox: create it with gb_ivox_create"
+                                                  : "the map is not incremental: create it with gb_voxelmap_create_incremental");
+  GB_REQUIRE(m->device == ctx->device && cloud->device == ctx->device, "cloud / map live on another device");
+  GB_REQUIRE((uint64_t)gb_stored_entries(m) + (uint64_t)cloud->n < (1ull << 31) - 1, "stored entries + cloud points exceed 2^31");
+  return GB_OK;
+}
+// 48-byte records (a voxel's or a stored point's) to the host; any output may be null.  A plain copy, its direction taken
+// from the unified address space: the map may live on another device than the current one, and every producer call
+// returned after its stream had drained.
+static gb_status download_records(const float4* records, size_t count, int32_t* num_points, float* xyz, float* cov6) {
+  if (count == 0 || !(num_points || xyz || cov6)) return GB_OK;
+  std::vector<float4> h(3 * count);
+  GB_CUDA(cudaMemcpy(h.data(), records, sizeof(float4) * h.size(), cudaMemcpyDefault));
+  for (size_t r = 0; r < count; r++) {
+    const float4 a = h[3 * r], b = h[3 * r + 1], c = h[3 * r + 2];
+    if (num_points) num_points[r] = (int32_t)c.y;
+    if (xyz) { xyz[3 * r] = a.x; xyz[3 * r + 1] = a.y; xyz[3 * r + 2] = a.z; }
+    if (cov6) { cov6[6 * r] = a.w; cov6[6 * r + 1] = b.x; cov6[6 * r + 2] = b.y; cov6[6 * r + 3] = b.z; cov6[6 * r + 4] = b.w; cov6[6 * r + 5] = c.x; }
+  }
+  return GB_OK;
 }
 
 extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_num_buckets, int max_bucket_scan_count, double target_points_drop_rate, gb_voxelmap** out) {
@@ -354,30 +389,23 @@ extern "C" gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolutio
   GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
   *out = nullptr;
   GB_ENTER(ctx);
-  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(), voxelmap_free);
-  if (!m) return GB_ERR_INTERNAL;
-  m->resolution = resolution;
-  m->inv_res = 1.0f / resolution;
-  m->max_scan = max_bucket_scan_count;
-  m->init_buckets = init_num_buckets;
-  m->drop_rate = target_points_drop_rate;
-  m->lru_horizon = lru_horizon;
-  m->lru_clear_cycle = lru_clear_cycle;
-  GB_CHECK(gb_voxelmap_create_incremental_impl(ctx, m.get()));
-  *out = m.release();
-  return GB_OK;
+  gb_voxelmap m;
+  m.kind = GB_MAP_INCREMENTAL;
+  m.resolution = resolution;
+  m.inv_res = 1.0f / resolution;
+  m.key_inv_res = 1.0 / (double)resolution;
+  m.max_scan = max_bucket_scan_count;
+  m.init_buckets = init_num_buckets;
+  m.drop_rate = target_points_drop_rate;
+  m.lru_horizon = lru_horizon;
+  m.lru_clear_cycle = lru_clear_cycle;
+  return map_create_empty(ctx, m, out);
 }
 extern "C" gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
-  GB_REQUIRE(ctx && map && cloud, "null argument");
-  GB_REQUIRE(map->incremental, "the map comes from gb_voxelmap_build, which keeps no sums: create it with gb_voxelmap_create_incremental");
-  GB_REQUIRE(map->device == ctx->device && cloud->device == ctx->device, "cloud / voxel map live on another device");
-  GB_REQUIRE(sampling_rate > 0.0 && sampling_rate <= 1.0, "sampling_rate must be in (0, 1]");
-  static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-  const double* T = T_map_cloud ? T_map_cloud : kIdentity;
-  for (int k = 0; k < 16; k++) GB_REQUIRE(std::isfinite(T[k]), "T_map_cloud must be finite");
-  GB_REQUIRE((uint64_t)map->num_voxels + (uint64_t)cloud->n < (1ull << 31) - 1, "map voxels + cloud points exceed 2^31");
+  const double* T;
+  GB_CHECK(insert_args(ctx, map, GB_MAP_INCREMENTAL, cloud, T_map_cloud, sampling_rate, &T));
   GB_ENTER(ctx);
-  return gb_voxelmap_insert_impl(ctx, map, cloud, T, sampling_rate, (unsigned long long)seed);
+  return gb_map_insert_impl(ctx, map, cloud, T, sampling_rate, (unsigned long long)seed);
 }
 extern "C" gb_status gb_voxelmap_info(const gb_voxelmap* m, int* num_voxels, int* num_buckets, float* resolution) {
   GB_REQUIRE(m, "null map");
@@ -388,19 +416,9 @@ extern "C" gb_status gb_voxelmap_info(const gb_voxelmap* m, int* num_voxels, int
 }
 extern "C" gb_status gb_voxelmap_download(const gb_voxelmap* m, int32_t* buckets, int32_t* num_points, float* means, float* cov6) {
   GB_REQUIRE(m, "null map");
-  GB_CUDA(cudaSetDevice(m->device));
-  if (buckets) GB_CUDA(cudaMemcpy(buckets, m->buckets, sizeof(int4) * (size_t)m->num_buckets, cudaMemcpyDeviceToHost));
-  if ((num_points || means || cov6) && m->num_voxels > 0) {
-    std::vector<float4> h(3 * (size_t)m->num_voxels);
-    GB_CUDA(cudaMemcpy(h.data(), m->voxels, sizeof(float4) * h.size(), cudaMemcpyDeviceToHost));
-    for (size_t v = 0; v < (size_t)m->num_voxels; v++) {
-      const float4 a = h[3 * v], b = h[3 * v + 1], c = h[3 * v + 2];
-      if (num_points) num_points[v] = (int32_t)c.y;
-      if (means) { means[3 * v] = a.x; means[3 * v + 1] = a.y; means[3 * v + 2] = a.z; }
-      if (cov6) { cov6[6 * v] = a.w; cov6[6 * v + 1] = b.x; cov6[6 * v + 2] = b.y; cov6[6 * v + 3] = b.z; cov6[6 * v + 4] = b.w; cov6[6 * v + 5] = c.x; }
-    }
-  }
-  return GB_OK;
+  GB_REQUIRE(m->kind != GB_MAP_IVOX, "an iVox holds points, not voxels: use gb_ivox_download");
+  if (buckets) GB_CUDA(cudaMemcpy(buckets, m->buckets, sizeof(int4) * (size_t)m->num_buckets, cudaMemcpyDefault));
+  return download_records(m->voxels, (size_t)m->num_voxels, num_points, means, cov6);
 }
 extern "C" gb_status gb_voxelmap_destroy(gb_voxelmap* m) {
   if (!m) return GB_OK;
@@ -410,7 +428,7 @@ extern "C" gb_status gb_voxelmap_destroy(gb_voxelmap* m) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// iVox: a gb_voxelmap with iVox state (gb_internal.cuh); voxelmap_free and gb_voxelmap_destroy release it
+// iVox: a gb_voxelmap of kind GB_MAP_IVOX (gb_internal.cuh); voxelmap_free and gb_voxelmap_destroy release it
 // ---------------------------------------------------------------------------------------------
 extern "C" gb_status gb_ivox_create(gb_ctx* ctx, double resolution, double min_dist_in_cell, int max_points_in_cell, int neighbor_voxel_mode, int lru_horizon,
                                     int lru_clear_cycle, gb_ivox** out) {
@@ -422,70 +440,55 @@ extern "C" gb_status gb_ivox_create(gb_ctx* ctx, double resolution, double min_d
   GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
   *out = nullptr;
   GB_ENTER(ctx);
-  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(), voxelmap_free);
-  if (!m) return GB_ERR_INTERNAL;
-  m->ivox = new (std::nothrow) gb_ivox_state();
-  if (!m->ivox) return GB_ERR_INTERNAL;
-  m->ivox->resolution = resolution;
-  m->ivox->min_dist = min_dist_in_cell;
-  m->ivox->max_points = max_points_in_cell;
-  m->ivox->mode = neighbor_voxel_mode;
-  m->resolution = (float)resolution;
-  m->inv_res = (float)(1.0 / resolution);
-  m->lru_horizon = lru_horizon;
-  m->lru_clear_cycle = lru_clear_cycle;
-  GB_CHECK(gb_ivox_create_impl(ctx, m.get()));
-  *out = reinterpret_cast<gb_ivox*>(m.release());
+  gb_voxelmap m;
+  m.kind = GB_MAP_IVOX;
+  m.ivox_resolution = resolution;
+  m.min_dist = min_dist_in_cell;
+  m.max_points = max_points_in_cell;
+  m.mode = neighbor_voxel_mode;
+  m.resolution = (float)resolution;
+  m.inv_res = (float)(1.0 / resolution);
+  m.key_inv_res = 1.0 / resolution;
+  m.max_scan = 10;          // the build's table (16384 buckets doubled until >= 8 V, 10 probes) with drop rate 0
+  m.init_buckets = 16384;
+  m.lru_horizon = lru_horizon;
+  m.lru_clear_cycle = lru_clear_cycle;
+  gb_voxelmap* h = nullptr;
+  GB_CHECK(map_create_empty(ctx, m, &h));
+  *out = reinterpret_cast<gb_ivox*>(h);
   return GB_OK;
 }
 extern "C" gb_status gb_ivox_insert(gb_ctx* ctx, gb_ivox* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
-  GB_REQUIRE(ctx && map && cloud, "null argument");
-  GB_REQUIRE(sampling_rate > 0.0 && sampling_rate <= 1.0, "sampling_rate must be in (0, 1]");
-  static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-  const double* T = T_map_cloud ? T_map_cloud : kIdentity;
-  for (int k = 0; k < 16; k++) GB_REQUIRE(std::isfinite(T[k]), "T_map_cloud must be finite");
   gb_voxelmap* m = ivox_map(map);
-  GB_REQUIRE(m->device == ctx->device && cloud->device == ctx->device, "cloud / iVox live on another device");
-  GB_REQUIRE((uint64_t)m->ivox->num_points + (uint64_t)cloud->n < (1ull << 31) - 1, "stored points + cloud points exceed 2^31");
+  const double* T;
+  GB_CHECK(insert_args(ctx, m, GB_MAP_IVOX, cloud, T_map_cloud, sampling_rate, &T));
   GB_ENTER(ctx);
-  return gb_ivox_insert_impl(ctx, m, cloud, T, sampling_rate, (unsigned long long)seed);
+  return gb_map_insert_impl(ctx, m, cloud, T, sampling_rate, (unsigned long long)seed);
 }
 extern "C" gb_status gb_ivox_info(const gb_ivox* map, int* num_voxels, size_t* num_points, double* resolution) {
-  GB_REQUIRE(map, "null iVox");
   const gb_voxelmap* m = ivox_map(map);
+  GB_REQUIRE(m && m->kind == GB_MAP_IVOX, "null map, or not an iVox");
   if (num_voxels) *num_voxels = m->num_voxels;
-  if (num_points) *num_points = m->ivox->num_points;
-  if (resolution) *resolution = m->ivox->resolution;
+  if (num_points) *num_points = m->num_points;
+  if (resolution) *resolution = m->ivox_resolution;
   return GB_OK;
 }
-// plain copies, their direction taken from the unified address space (the map may live on another device than the current
-// one); the insert returned after its stream had drained
 extern "C" gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords, int32_t* voxel_counts, float* xyz, float* cov6) {
-  GB_REQUIRE(map, "null iVox");
   const gb_voxelmap* m = ivox_map(map);
-  const size_t V = (size_t)m->num_voxels, P = m->ivox->num_points;
-  if (V == 0) return GB_OK;
-  if (voxel_coords || voxel_counts) {
+  GB_REQUIRE(m && m->kind == GB_MAP_IVOX, "null map, or not an iVox");
+  const size_t V = (size_t)m->num_voxels;
+  if (V > 0 && (voxel_coords || voxel_counts)) {
     std::vector<unsigned long long> keys(V);
     std::vector<int2> cells(V);
     GB_CUDA(cudaMemcpy(keys.data(), m->vkeys, sizeof(unsigned long long) * V, cudaMemcpyDefault));
-    GB_CUDA(cudaMemcpy(cells.data(), m->ivox->cells, sizeof(int2) * V, cudaMemcpyDefault));
+    GB_CUDA(cudaMemcpy(cells.data(), m->cells, sizeof(int2) * V, cudaMemcpyDefault));
     for (size_t v = 0; v < V; v++) {
       if (voxel_coords)
         for (int a = 0; a < 3; a++) voxel_coords[3 * v + a] = (int32_t)((keys[v] >> (42 - 21 * a)) & 0x1FFFFF) - (1 << 20);
       if (voxel_counts) voxel_counts[v] = cells[v].y;
     }
   }
-  if (xyz || cov6) {
-    std::vector<float4> h(3 * P);
-    GB_CUDA(cudaMemcpy(h.data(), m->voxels, sizeof(float4) * h.size(), cudaMemcpyDefault));
-    for (size_t p = 0; p < P; p++) {
-      const float4 a = h[3 * p], b = h[3 * p + 1], c = h[3 * p + 2];
-      if (xyz) { xyz[3 * p] = a.x; xyz[3 * p + 1] = a.y; xyz[3 * p + 2] = a.z; }
-      if (cov6) { cov6[6 * p] = a.w; cov6[6 * p + 1] = b.x; cov6[6 * p + 2] = b.y; cov6[6 * p + 3] = b.z; cov6[6 * p + 4] = b.w; cov6[6 * p + 5] = c.x; }
-    }
-  }
-  return GB_OK;
+  return download_records(m->voxels, m->num_points, nullptr, xyz, cov6);
 }
 extern "C" gb_status gb_ivox_destroy(gb_ivox* map) { return gb_voxelmap_destroy(ivox_map(map)); }
 
@@ -494,6 +497,7 @@ extern "C" gb_status gb_ivox_destroy(gb_ivox* map) { return gb_voxelmap_destroy(
 // ---------------------------------------------------------------------------------------------
 extern "C" gb_status gb_vgicp_factor_create(gb_ctx* ctx, const gb_voxelmap* target, const gb_cloud* source, int flags, gb_factor** out) {
   GB_REQUIRE(ctx && target && source && out, "null argument");
+  GB_REQUIRE(target->kind != GB_MAP_IVOX, "the target is an iVox: GICP factors on it come from gb_gicp_factor_create");
   // clouds / voxel maps may have been uploaded through another context (another module thread): device memory is shared,
   // and every producer call returns only after its stream has drained, so only the DEVICE has to match
   GB_REQUIRE(target->device == ctx->device && source->device == ctx->device, "cloud / voxel map live on another device");
@@ -510,6 +514,7 @@ extern "C" gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, c
   GB_REQUIRE(ctx && target && source && out, "null argument");
   GB_REQUIRE(std::isfinite(max_correspondence_distance) && max_correspondence_distance > 0.0, "max_correspondence_distance must be positive and finite");
   const gb_voxelmap* m = ivox_map(target);
+  GB_REQUIRE(m->kind == GB_MAP_IVOX, "the target is not an iVox: VGICP factors on voxel maps come from gb_vgicp_factor_create");
   GB_REQUIRE(m->device == ctx->device && source->device == ctx->device, "cloud / iVox live on another device");
   GB_ENTER(ctx);
   gb_factor* f = new (std::nothrow) gb_factor();
@@ -696,9 +701,9 @@ static void desc_target(FactorDesc& D, const gb_voxelmap* t) {
 // a GICP factor's target part: the iVox's table and point records in the FactorDesc, the rest in its GicpDesc
 static void desc_target_ivox(FactorDesc& D, GicpDesc& G, const gb_factor* fa) {
   desc_target(D, fa->target);
-  G.cells = fa->target->ivox->cells;
+  G.cells = fa->target->cells;
   G.max_corr2 = fa->max_corr2;
-  G.num_offsets = fa->target->ivox->mode;
+  G.num_offsets = fa->target->mode;
 }
 // B_f of SURVEY 8(d): 48 B per source point, 48 B per target voxel, 16 B per bucket, pose in + record out.
 // The bucket term is charged at the SMALLEST table that could hold the voxels (16384 doubled until >= V), not at
@@ -707,7 +712,7 @@ static void desc_target_ivox(FactorDesc& D, GicpDesc& G, const gb_factor* fa) {
 static uint64_t factor_bytes(const gb_factor* fa) {
   const bool sv = (fa->flags & GB_FACTOR_SURFACE_VALIDATION) != 0;
   const uint64_t V = (uint64_t)fa->target->num_voxels;
-  const uint64_t records = fa->target->ivox ? (uint64_t)fa->target->ivox->num_points : V;
+  const uint64_t records = fa->target->kind == GB_MAP_IVOX ? (uint64_t)fa->target->num_points : V;
   uint64_t nb_ref = 16384;
   while (nb_ref < V) nb_ref *= 2;
   return (uint64_t)fa->source->n * (48 + (sv ? 12 : 0)) + records * 48 + nb_ref * 16 + 64 + 488;  // +12 B / point: the normals, when they are read
@@ -727,7 +732,7 @@ static gb_status sweep_follow_targets(gb_sweep* s) {
       synced = true;
     }
     s->target_versions[f] = fa->target->version;
-    if (fa->target->ivox) {
+    if (fa->target->kind == GB_MAP_IVOX) {
       desc_target_ivox(s->h_descs[f], s->h_gdescs[f], fa);
       GB_CUDA(cudaMemcpyAsync(s->d_gdescs + f, s->h_gdescs + f, sizeof(GicpDesc), cudaMemcpyHostToDevice, s->ctx->stream));
     } else {
@@ -776,10 +781,10 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   for (size_t f = 0; f < F; f++) {
     GB_REQUIRE(factors[f], "null factor");
     GB_REQUIRE(factors[f]->source->device == ctx->device && factors[f]->target->device == ctx->device, "factor lives on another device");
-    GB_REQUIRE((factors[f]->target->ivox != nullptr) == (factors[0]->target->ivox != nullptr), "the factors of one sweep must all be VGICP or all GICP factors");
+    GB_REQUIRE((factors[f]->target->kind == GB_MAP_IVOX) == (factors[0]->target->kind == GB_MAP_IVOX), "the factors of one sweep must all be VGICP or all GICP factors");
     total_pts += factors[f]->source->n;
   }
-  const bool gicp = F > 0 && factors[0]->target->ivox != nullptr;
+  const bool gicp = F > 0 && factors[0]->target->kind == GB_MAP_IVOX;
   GB_REQUIRE(!gicp || !pair_index, "GICP sweeps take no pair_index (no slab can be attached to them)");
   GB_ENTER(ctx);
   gb_owned<gb_sweep> s(new (std::nothrow) gb_sweep(), sweep_free);
@@ -821,7 +826,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     any_sv = any_sv || sv;
     if (gicp) desc_target_ivox(D, gdescs[f], fa); else desc_target(D, fa->target);
     s->target_versions.push_back(fa->target->version);
-    s->any_incremental = s->any_incremental || gicp || fa->target->incremental;
+    s->any_incremental = s->any_incremental || fa->target->kind != GB_MAP_BUILT;
     D.n = (int)fa->source->n;
     D.pair = pair_index ? pair_index[f] : (int)f;
     s->h_pair.push_back(D.pair);
@@ -1303,8 +1308,8 @@ extern "C" gb_status gb_overlap(gb_ctx* ctx, size_t T, const gb_voxelmap* const*
     FactorDesc& D = h.descs[t];
     memset(&D, 0, sizeof(D));
     D.p0 = source->p0; D.p1 = source->p1; D.p2 = source->p2;
-    D.buckets = targets[t]->buckets; D.voxels = targets[t]->voxels;
-    D.mask = (uint32_t)targets[t]->num_buckets - 1u; D.max_scan = targets[t]->max_scan; D.inv_res = targets[t]->inv_res; D.n = (int)source->n;
+    desc_target(D, targets[t]);
+    D.n = (int)source->n;
   }
   memcpy(h.poses, deltas, sizeof(double) * 16 * T);
   GB_CUDA(cudaMemcpyAsync(d.descs, h.descs, (char*)h.count - (char*)h.descs, cudaMemcpyHostToDevice, ctx->stream));  // descriptors and poses

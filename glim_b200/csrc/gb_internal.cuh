@@ -59,41 +59,44 @@ struct gb_cloud {
   size_t bytes = 0;
 };
 
+// A map is one of three kinds, fixed at creation.  Every entry point that takes a map checks the kind it accepts.
+enum gb_map_kind {
+  GB_MAP_BUILT,        // gb_voxelmap_build: records and table only
+  GB_MAP_INCREMENTAL,  // gb_voxelmap_create_incremental / gb_voxelmap_insert
+  GB_MAP_IVOX,         // gb_ivox_create / gb_ivox_insert: the gb_ivox handle is the map itself
+};
 struct gb_voxelmap {
   int device = 0;
-  float resolution = 0.f, inv_res = 0.f;
+  gb_map_kind kind = GB_MAP_BUILT;
+  float resolution = 0.f, inv_res = 0.f;  // the fp32 lookup rule of every sweep and overlap
   int max_scan = 0;
   int num_voxels = 0, num_buckets = 0;
   int num_dropped_points = 0;
   int4* buckets = nullptr;
-  float4* voxels = nullptr;   // 3 float4 per voxel
+  float4* voxels = nullptr;   // 3 float4 per record: one record per voxel, or per stored point of an iVox
   void* base = nullptr;
   size_t bytes = 0;
-  // Incremental maps (gb_voxelmap_create_incremental / gb_voxelmap_insert) also keep, in `base` behind the records, each
-  // voxel's packed key, point count, fp64 sums (Sigma q: 3, Sigma C: 6 unique entries) and the insert that last touched it.
-  // A built map keeps none of this and its version stays 0.
-  bool incremental = false;
+  // Incremental maps and iVoxes also keep, in `base` behind the records, each voxel's packed key and the insert that last
+  // touched it.  An incremental map adds each voxel's point count and fp64 sums (Sigma q: 3, Sigma C: 6 unique entries).  An
+  // iVox's records are its stored points ({x y z c00} {c01 c02 c11 c12} {c22, 1, 0, 0}), voxel-major in ascending packed-key
+  // order, and it adds each voxel's cell {first point, count}.  A built map keeps none of this and its version stays 0.
   uint64_t version = 0;        // bumped by every insert: sweeps re-read the target's buckets / records when it changed
+  double key_inv_res = 0.0;    // an insert's fp64 key rule floor(q * key_inv_res), fixed at creation
   int init_buckets = 0;
-  double drop_rate = 0.0;
+  double drop_rate = 0.0;      // 0 for an iVox: every voxel is found
   int lru_horizon = 0, lru_clear_cycle = 10, lru_counter = 0;
+  size_t num_points = 0;       // the points the voxels hold
   unsigned long long* vkeys = nullptr;  // ascending: the voxel numbering
-  int* vn = nullptr;
   int* vstamp = nullptr;
-  double* vsums = nullptr;     // 9 per voxel: q.x q.y q.z c00 c01 c02 c11 c12 c22
-  // A device iVox (gb_ivox_create / gb_ivox_insert) is a gb_voxelmap with this state: the gb_ivox handle is the map itself,
-  // so one free function, one device and one table serve both.  Its block in `base` holds the stored points as 48-byte
-  // records in `voxels` (3 float4 each, the voxel-record layout: {x y z c00} {c01 c02 c11 c12} {c22, 1, 0, 0}), voxel-major
-  // in ascending packed-key order, then per voxel its cell {first point, count} (ivox->cells), key (vkeys) and stamp (vstamp);
-  // lru_* and version are the incremental map's.  nullptr for every voxel map.
-  struct gb_ivox_state* ivox = nullptr;
-};
-struct gb_ivox_state {
-  double resolution = 0.0, min_dist = 0.0;  // the map's float resolution / inv_res: (float) of these, inv_res = (float)(1 / r)
+  int* vn = nullptr;           // incremental
+  double* vsums = nullptr;     // incremental, 9 per voxel: q.x q.y q.z c00 c01 c02 c11 c12 c22
+  int2* cells = nullptr;       // iVox
+  // iVox parameters: resolution and inv_res are (float)ivox_resolution and (float)(1 / ivox_resolution)
+  double ivox_resolution = 0.0, min_dist = 0.0;
   int max_points = 10, mode = 1;
-  size_t num_points = 0;
-  int2* cells = nullptr;
 };
+// the stored entries an insert groups ahead of the frame's points: one per voxel, or one per stored point of an iVox
+inline size_t gb_stored_entries(const gb_voxelmap* m) { return m->kind == GB_MAP_IVOX ? m->num_points : (size_t)m->num_voxels; }
 // the handle of an iVox is its gb_voxelmap (gb_ivox stays an incomplete type)
 inline gb_voxelmap* ivox_map(gb_ivox* h) { return reinterpret_cast<gb_voxelmap*>(h); }
 inline const gb_voxelmap* ivox_map(const gb_ivox* h) { return reinterpret_cast<const gb_voxelmap*>(h); }
@@ -127,7 +130,7 @@ static_assert(sizeof(GicpDesc) == 16, "GicpDesc size");
 
 struct gb_factor {
   gb_ctx* ctx = nullptr;
-  const gb_voxelmap* target = nullptr;  // the voxel map, or the iVox of a GICP factor (target->ivox != nullptr)
+  const gb_voxelmap* target = nullptr;  // a built or incremental map (VGICP), or an iVox (GICP: target->kind == GB_MAP_IVOX)
   float max_corr2 = 0.f;                // GICP: (float)(max_correspondence_distance^2)
   const gb_cloud* source = nullptr;
   int flags = 0;
@@ -214,7 +217,7 @@ struct gb_sweep {
   cudaGraphExec_t graph_exec = nullptr;  // small sweeps: poses H2D -> kernel -> records D2H as ONE graph launch (gb_factor_set_linearize)
   int graph_state = 0;              // 0 = not built, 1 = valid, -1 = capture failed (plain launches from then on)
   gb_pool_block blk;                // the device and pinned blocks, laid out by sweep_layout; back to the context's pool at the end
-  bool any_incremental = false;     // some target is an incremental map: its descriptor may go stale (gb_voxelmap_insert)
+  bool any_incremental = false;     // some target is not a built map: its descriptor may go stale (gb_voxelmap_insert, gb_ivox_insert)
   std::vector<uint64_t> target_versions;  // per factor: the target version its descriptor was written from
   // GICP sweeps (every factor on an iVox; a sweep holds one kind): k_gicp_sweep over sweep5's strided items, with the
   // GICP half of each descriptor next to the FactorDesc table
@@ -397,10 +400,10 @@ gb_status gb_launch_gicp_sweep(gb_sweep* s, int mode);  // gb_launch_sweep of a 
 gb_status gb_launch_peer_signal_wait(gb_peer_slab* ps);
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count);
 gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_buckets, int max_scan, double drop_rate, gb_voxelmap* out);
-gb_status gb_voxelmap_create_incremental_impl(gb_ctx* ctx, gb_voxelmap* m);
-gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, unsigned long long seed);
-gb_status gb_ivox_create_impl(gb_ctx* ctx, gb_voxelmap* m);
-gb_status gb_ivox_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, unsigned long long seed);
+// An incremental map or iVox whose parameters are set: its device and empty table.
+gb_status gb_map_create_empty_impl(gb_ctx* ctx, gb_voxelmap* m);
+// One insert into an incremental map or an iVox, by its kind.
+gb_status gb_map_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, unsigned long long seed);
 // Shared with gb_merge_frames (gb_kernels_preprocess.cu): one frame's points q = R a + t and covariances R C R^T in
 // un-contracted fp64, in the caller's point order (pts: n x double4, cov6: n x 6 upper triangle).  d_frame: GB_FRAME_DESC_BYTES
 // of device scratch for the frame descriptor.  One launch.

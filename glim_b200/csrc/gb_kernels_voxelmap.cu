@@ -21,7 +21,7 @@
 //   6. host loop         num_buckets = init doubled until >= 8 V (load factor <= 1/8), then doubled again while
 //                        dropped points > drop_rate * N
 // Steps 2-3 (+ k_voxel_starts) are gb_group_by_key / gb_group_starts, shared with the voxel-grid downsampling and the frame
-// merge of gb_kernels_preprocess.cu.  Step 6 (table_build) also serves the incremental maps of gb_voxelmap_insert, whose
+// merge of gb_kernels_preprocess.cu.  Step 6 (table_build) also serves the incremental maps and iVoxes, whose one insert
 // pipeline is described below.  This file also builds every device cloud (gb_cloud_build: Morton reorder of staged
 // planes), for gb_cloud_upload, gb_preprocess and gb_merge_frames.
 #include "gb_internal.cuh"
@@ -215,18 +215,26 @@ gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resol
 }
 
 // ---------------------------------------------------------------------------------------------
-// Incremental maps (gb_voxelmap_create_incremental / gb_voxelmap_insert; the rule is written once in include/glim_b200.h).
-// One insert is one pass over (the map's voxels, the frame's points):
-//   1. k_merge_transform   (gb_transform_frame, shared with gb_merge_frames) q = R a + t, R C R^T in un-contracted fp64
-//   2. k_grid_keys         (gb_grid_keys) packed floor(q * (1 / r)) in fp64; with sampling_rate < 1 the points whose
+// Incremental maps and iVoxes (gb_voxelmap_insert / gb_ivox_insert; both rules are written once in include/glim_b200.h).
+// One insert is one pass over (the map's stored entries, the frame's points), the same steps for both kinds:
+//   1. old keys            the stored entries, tagged old (idx = -1 - entry), ahead of the points: one per voxel
+//                          (k_ins_old_keys) or one per stored iVox point (k_ivox_old_keys)
+//   2. k_merge_transform   (gb_transform_frame, shared with gb_merge_frames) q = R a + t, R C R^T in un-contracted fp64
+//   3. k_grid_keys         (gb_grid_keys) packed floor(q * key_inv_res) in fp64; with sampling_rate < 1 the points whose
 //                          rg_hash(seed, index) is not among the m smallest lose their key (k_ins_sample_*, one radix sort)
-//   3. k_ins_old_keys      the map's voxel keys, tagged old (idx = -1 - v), ahead of the points: after the stable
-//                          gb_group_by_key a voxel's group is its old entry first, then its new points in index order
-//   4. k_ins_merge         one thread per merged voxel: stored sums + the new points one at a time, n, stamp, eviction
-//   5. scan + k_ins_emit   the survivors, in ascending key order, into a new state block (keys, n, stamps, sums, fp32 records)
-//   6. table_build         the build's table kernels and sizing rule
-// Two host synchronisations (survivor count; dropped points of each table attempt).  The old blocks go back to the pool
-// through gb_dev_free, which waits for every stream of the device: a sweep of another context still reading them is safe.
+//   4. gb_group_by_key     stable: a voxel's group is its old entries first, then its new points in index order
+//   5. merge               one thread per merged voxel: the kind's per-voxel rule, then the LRU eviction (the same
+//                          expression in both merge kernels: a shared helper changes k_ivox_merge's SASS)
+//                            incremental  stored sums + the new points one at a time, n, stamp (k_ins_merge, a scan, k_ins_count)
+//                            iVox         the stored points, then the sequential admission of the new ones (k_ivox_merge,
+//                                         two scans, k_ivox_count)
+//   6. read back           surviving points and voxels
+//   7. emit                the survivors, in ascending key order, into a new state block of the kind's layout (k_ins_emit:
+//                          keys, n, stamps, sums, fp32 records; k_ivox_emit: point records, cells, keys, stamps)
+//   8. table_build         the build's table kernels and sizing rule; an iVox has drop rate 0 and fails if a voxel is left out
+// Two host synchronisations (survivor count; dropped points of each table attempt).  The map is replaced only when every
+// step has succeeded.  The old blocks go back to the pool through gb_dev_free, which waits for every stream of the device:
+// a sweep of another context still reading them is safe.
 // ---------------------------------------------------------------------------------------------
 namespace {
 
@@ -307,137 +315,6 @@ __global__ void k_ins_emit(int N, const int* __restrict__ num_merged, const int*
   gb_unpack_key(key, x, y, z);
   vcoord[o] = make_int4(x, y, z, cnt);
 }
-
-// the state block of V voxels: fp32 records first (gb_voxelmap::voxels), then keys, counts, stamps and sums
-void state_layout(Carver& cv, size_t V, gb_voxelmap* m) {
-  m->voxels = cv.take<float4>(3 * V);
-  m->vkeys = cv.take<unsigned long long>(V);
-  m->vn = cv.take<int>(V);
-  m->vstamp = cv.take<int>(V);
-  m->vsums = cv.take<double>(9 * V);
-}
-
-}  // namespace
-
-gb_status gb_voxelmap_create_incremental_impl(gb_ctx* ctx, gb_voxelmap* m) {
-  m->device = ctx->device;
-  m->incremental = true;
-  GB_CHECK(table_build(ctx, 0, nullptr, nullptr, m->init_buckets, m->max_scan, m->drop_rate, 0.0, &m->buckets, &m->num_buckets, &m->num_dropped_points));
-  m->bytes = sizeof(int4) * (size_t)m->num_buckets;
-  return GB_OK;
-}
-
-gb_status gb_voxelmap_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T, double sampling_rate, unsigned long long seed) {
-  cudaStream_t st = ctx->stream;
-  const int n = (int)cloud->n;
-  const int Vo = m->num_voxels;
-  const int kept = sampling_rate < 1.0 ? (int)(size_t)((double)n * sampling_rate) : n;  // random_sampling's count
-  const int np = kept > 0 ? n : 0;  // points that take part (the unsampled ones get no key)
-  const int N = Vo + np;
-  gb_voxelmap next = *m;  // the map after this insert; m is replaced only when everything has succeeded
-  next.lru_counter = m->lru_counter + 1;
-  next.version = m->version + 1;
-  if (N > 0) {
-    const size_t cub_b = gb_cub_temp_bytes((size_t)N);
-    gb_sort_tmp t;
-    int *d_flags, *d_pos, *d_starts, *d_keep, *d_kpos, *d_mn, *d_mstamp, *d_dropped;
-    double4* d_pts = nullptr;
-    double *d_cov = nullptr, *d_msums;
-    unsigned long long *d_hash = nullptr, *d_info;
-    void* d_frame;
-    int4* d_vcoord;
-    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
-      t = gb_take_sort_tmp(cv, (size_t)N, cv.take<char>(cub_b), cub_b);
-      d_flags = cv.take<int>(N + 1);
-      d_pos = cv.take<int>(N + 1);
-      d_starts = cv.take<int>(N + 1);
-      d_keep = cv.take<int>(N + 1);
-      d_kpos = cv.take<int>(N + 1);
-      d_mn = cv.take<int>(N);
-      d_mstamp = cv.take<int>(N);
-      d_msums = cv.take<double>(9 * (size_t)N);
-      d_vcoord = cv.take<int4>(N);
-      d_dropped = cv.take<int>(1);
-      d_info = cv.take<unsigned long long>(2);  // {points in the surviving voxels, surviving voxels}
-      d_frame = cv.take<char>(GB_FRAME_DESC_BYTES);
-      if (np > 0) {
-        d_pts = cv.take<double4>(np);
-        d_cov = cv.take<double>(6 * (size_t)np);
-        if (kept < n) d_hash = cv.take<unsigned long long>(np);
-      }
-    }));
-    const int tb = 256;
-    if (Vo > 0) {
-      GB_CHECK(gb_launch(ctx, "k_ins_old_keys", k_ins_old_keys, (Vo + tb - 1) / tb, tb, 0, Vo, m->vkeys, t.keys, t.idx));
-    }
-    if (np > 0) {
-      GB_CHECK(gb_transform_frame(ctx, cloud, T, d_frame, d_pts, d_cov));
-      GB_CHECK(gb_grid_keys(ctx, np, d_pts, 1.0 / (double)m->resolution, t.keys + Vo, t.idx + Vo));
-      if (kept < n) {
-        GB_CHECK(gb_launch(ctx, "k_ins_sample_hash", k_ins_sample_hash, (np + tb - 1) / tb, tb, 0, np, seed, t.keys_s));
-        GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, cub_b, t.keys_s, d_hash, np, 0, 64);
-        GB_CHECK(gb_launch(ctx, "k_ins_sample_drop", k_ins_sample_drop, (np + tb - 1) / tb, tb, 0, np, kept, seed, d_hash, t.keys + Vo));
-      }
-    }
-    GB_CUDA(cudaMemsetAsync(d_info, 0, 2 * sizeof(unsigned long long), st));
-    GB_CHECK(gb_group_by_key(ctx, N, t, d_flags, d_pos));
-    GB_CHECK(gb_group_starts(ctx, N, t, d_flags, d_pos, d_starts));
-    GB_CHECK(gb_launch(ctx, "k_ins_merge", k_ins_merge, (N + 127) / 128, 128, 0, N, d_pos + (N - 1), d_starts, t.idx_s, m->vn, m->vstamp, m->vsums, d_pts, d_cov, m->lru_counter,
-                       m->lru_horizon, m->lru_clear_cycle, d_mn, d_mstamp, d_msums, d_keep, d_info));
-    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_keep, d_kpos, N);
-    GB_CHECK(gb_launch(ctx, "k_ins_count", k_ins_count, 1, 1, 0, N, d_kpos, d_info + 1));
-    unsigned long long info[2] = {0, 0};
-    GB_CUDA(cudaMemcpyAsync(info, d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    const int V = (int)info[1];
-    next.base = nullptr;
-    next.buckets = nullptr;
-    next.num_voxels = V;
-    Carver size;
-    state_layout(size, (size_t)V, &next);
-    next.bytes = V > 0 ? size.off : 0;
-    if (V > 0) {
-      GB_CUDA(gb_dev_malloc(ctx->device, size.off, &next.base));
-      Carver cv{(char*)next.base};
-      state_layout(cv, (size_t)V, &next);
-      gb_status s = gb_launch(ctx, "k_ins_emit", k_ins_emit, (N + tb - 1) / tb, tb, 0, N, d_pos + (N - 1), d_keep, d_kpos, d_starts, t.keys_s, d_mn, d_mstamp, d_msums,
-                              next.vkeys, next.vn, next.vstamp, next.vsums, next.voxels, d_vcoord);
-      if (s != GB_OK) { gb_dev_free(ctx->device, next.base); return s; }
-    } else {
-      next.voxels = nullptr; next.vkeys = nullptr; next.vn = nullptr; next.vstamp = nullptr; next.vsums = nullptr;
-    }
-    gb_status s = table_build(ctx, V, d_vcoord, d_dropped, m->init_buckets, m->max_scan, m->drop_rate, (double)info[0], &next.buckets, &next.num_buckets, &next.num_dropped_points);
-    if (s != GB_OK) {
-      gb_dev_free(ctx->device, next.base);
-      gb_dev_free(ctx->device, next.buckets);
-      return s;
-    }
-    next.bytes += sizeof(int4) * (size_t)next.num_buckets;
-  }
-  void* old_base = m->base;
-  int4* old_buckets = m->buckets;
-  const bool replaced = N > 0;
-  *m = next;
-  if (replaced) {
-    gb_dev_free(ctx->device, old_base);
-    gb_dev_free(ctx->device, old_buckets);
-  }
-  return GB_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// The device iVox (gb_ivox_create / gb_ivox_insert; the rule is written once in include/glim_b200.h).  One insert:
-//   1. k_ivox_old_keys     one entry per STORED point (idx = -1 - record), ahead of the frame's points
-//   2. the voxel map's steps 1-2 (transform, fp64 keys, sampling) and gb_group_by_key: a voxel's group is its stored points
-//      in slot order, then its new points in index order
-//   3. k_ivox_merge        one thread per merged voxel: the sequential admission, the stamp, the eviction
-//   4. two scans + k_ivox_count: surviving voxels and points (one host synchronisation)
-//   5. k_ivox_emit         the survivors into a new block: cells, keys, stamps and the point records
-//   6. table_build         the build's table kernels, with drop rate 0: every voxel is found
-// ---------------------------------------------------------------------------------------------
-namespace {
-
-constexpr int kIvoxInitBuckets = 16384;
 
 __global__ void k_ivox_old_keys(int V, const unsigned long long* __restrict__ vkeys, const int2* __restrict__ cells, unsigned long long* __restrict__ keys, int* __restrict__ idx) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
@@ -540,138 +417,194 @@ __global__ void k_ivox_emit(int N, const int* __restrict__ num_merged, const int
   }
 }
 
-// the state block of V voxels and P points: point records first (gb_voxelmap::voxels), then cells, keys and stamps
-void ivox_layout(Carver& cv, size_t V, size_t P, gb_voxelmap* m, int2** cells) {
-  m->voxels = cv.take<float4>(3 * P);
-  *cells = cv.take<int2>(V);
-  m->vkeys = cv.take<unsigned long long>(V);
-  m->vstamp = cv.take<int>(V);
-}
+// The scratch of steps 1-8 that both kinds use: the grouping of N entries, the frame's fp64 points and covariances, the
+// survivors' table coordinates and the read-back {points in the surviving voxels, surviving voxels}.
+struct InsertScratch {
+  gb_sort_tmp t;
+  int *flags, *pos, *starts, *keep, *kpos, *dropped;
+  int4* vcoord;
+  unsigned long long* info;
+  void* frame;
+  double4* pts = nullptr;
+  double* cov = nullptr;
+  unsigned long long* hash = nullptr;
+};
 
-}  // namespace
+// The per-voxel part of an incremental map: one stored entry per voxel, whose fp64 sums the new points continue.
+struct VoxelRule {
+  const gb_voxelmap* m;
+  int *mn, *mstamp;
+  double* msums;
+  void scratch(Carver& cv, size_t N) {
+    mn = cv.take<int>(N);
+    mstamp = cv.take<int>(N);
+    msums = cv.take<double>(9 * N);
+  }
+  gb_status old_keys(gb_ctx* ctx, const gb_sort_tmp& t) const {
+    const int Vo = m->num_voxels;
+    return gb_launch(ctx, "k_ins_old_keys", k_ins_old_keys, (Vo + 255) / 256, 256, 0, Vo, m->vkeys, t.keys, t.idx);
+  }
+  gb_status merge(gb_ctx* ctx, const InsertScratch& s, int N) const {
+    GB_CUDA(cudaMemsetAsync(s.info, 0, 2 * sizeof(unsigned long long), ctx->stream));  // k_ins_merge adds up info[0]
+    GB_CHECK(gb_launch(ctx, "k_ins_merge", k_ins_merge, (N + 127) / 128, 128, 0, N, s.pos + (N - 1), s.starts, s.t.idx_s, m->vn, m->vstamp, m->vsums, s.pts, s.cov,
+                       m->lru_counter, m->lru_horizon, m->lru_clear_cycle, mn, mstamp, msums, s.keep, s.info));
+    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, s.t.cub, s.t.cub_bytes, s.keep, s.kpos, N);
+    return gb_launch(ctx, "k_ins_count", k_ins_count, 1, 1, 0, N, s.kpos, s.info + 1);
+  }
+  // the state block: fp32 records first (gb_voxelmap::voxels), then keys, counts, stamps and sums
+  static void layout(Carver& cv, gb_voxelmap* next) {
+    const size_t V = (size_t)next->num_voxels;
+    next->voxels = cv.take<float4>(3 * V);
+    next->vkeys = cv.take<unsigned long long>(V);
+    next->vn = cv.take<int>(V);
+    next->vstamp = cv.take<int>(V);
+    next->vsums = cv.take<double>(9 * V);
+  }
+  gb_status emit(gb_ctx* ctx, const InsertScratch& s, int N, const gb_voxelmap& next) const {
+    return gb_launch(ctx, "k_ins_emit", k_ins_emit, (N + 255) / 256, 256, 0, N, s.pos + (N - 1), s.keep, s.kpos, s.starts, s.t.keys_s, mn, mstamp, msums,
+                     next.vkeys, next.vn, next.vstamp, next.vsums, next.voxels, s.vcoord);
+  }
+  gb_status check_table(const gb_voxelmap&) const { return GB_OK; }
+};
 
-gb_status gb_ivox_create_impl(gb_ctx* ctx, gb_voxelmap* m) {
-  m->device = ctx->device;
-  m->max_scan = 10;
-  m->init_buckets = kIvoxInitBuckets;
-  int dropped = 0;
-  GB_CHECK(table_build(ctx, 0, nullptr, nullptr, kIvoxInitBuckets, m->max_scan, 0.0, 0.0, &m->buckets, &m->num_buckets, &dropped));
-  m->bytes = sizeof(int4) * (size_t)m->num_buckets;
-  return GB_OK;
-}
+// The per-voxel part of an iVox: one stored entry per stored point; a voxel keeps its points and admits new ones.
+struct IvoxRule {
+  const gb_voxelmap* m;
+  int *ppos, *mcount, *mstamp, *mref;
+  void scratch(Carver& cv, size_t N) {
+    ppos = cv.take<int>(N + 1);
+    mcount = cv.take<int>(N + 1);
+    mstamp = cv.take<int>(N);
+    mref = cv.take<int>(N);
+  }
+  gb_status old_keys(gb_ctx* ctx, const gb_sort_tmp& t) const {
+    const int Vo = m->num_voxels;
+    return gb_launch(ctx, "k_ivox_old_keys", k_ivox_old_keys, (Vo + 255) / 256, 256, 0, Vo, m->vkeys, m->cells, t.keys, t.idx);
+  }
+  gb_status merge(gb_ctx* ctx, const InsertScratch& s, int N) const {
+    GB_CHECK(gb_launch(ctx, "k_ivox_merge", k_ivox_merge, (N + 127) / 128, 128, 0, N, s.pos + (N - 1), s.starts, s.t.keys_s, s.t.idx_s, m->num_voxels, m->vkeys, m->vstamp,
+                       m->voxels, s.pts, m->max_points, m->min_dist * m->min_dist, m->lru_counter, m->lru_horizon, m->lru_clear_cycle, mref, mcount, mstamp, s.keep));
+    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, s.t.cub, s.t.cub_bytes, s.keep, s.kpos, N);
+    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, s.t.cub, s.t.cub_bytes, mcount, ppos, N);
+    return gb_launch(ctx, "k_ivox_count", k_ivox_count, 1, 1, 0, N, s.kpos, ppos, s.info);
+  }
+  // the state block of V voxels and P points: point records first (gb_voxelmap::voxels), then cells, keys and stamps
+  static void layout(Carver& cv, gb_voxelmap* next) {
+    const size_t V = (size_t)next->num_voxels;
+    next->voxels = cv.take<float4>(3 * next->num_points);
+    next->cells = cv.take<int2>(V);
+    next->vkeys = cv.take<unsigned long long>(V);
+    next->vstamp = cv.take<int>(V);
+  }
+  gb_status emit(gb_ctx* ctx, const InsertScratch& s, int N, const gb_voxelmap& next) const {
+    return gb_launch(ctx, "k_ivox_emit", k_ivox_emit, (N + 255) / 256, 256, 0, N, s.pos + (N - 1), s.keep, s.kpos, ppos, s.starts, s.t.keys_s, mref, mcount, mstamp,
+                     m->voxels, s.pts, s.cov, next.vkeys, next.vstamp, next.cells, next.voxels, s.vcoord);
+  }
+  gb_status check_table(const gb_voxelmap& next) const {
+    if (next.num_dropped_points == 0) return GB_OK;
+    gb_set_error("iVox table: %d points left out of a table of %d buckets", next.num_dropped_points, next.num_buckets);
+    return GB_ERR_INTERNAL;
+  }
+};
 
-gb_status gb_ivox_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T, double sampling_rate, unsigned long long seed) {
+// Steps 1-8 for either kind; `rule` is the kind's per-voxel part.
+template <typename Rule>
+gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T, double sampling_rate, unsigned long long seed, Rule rule) {
   cudaStream_t st = ctx->stream;
-  gb_ivox_state* iv = m->ivox;
   const int n = (int)cloud->n;
-  const int Vo = m->num_voxels;
-  const int Po = (int)iv->num_points;
+  const int No = (int)gb_stored_entries(m);
   const int kept = sampling_rate < 1.0 ? (int)(size_t)((double)n * sampling_rate) : n;  // random_sampling's count
-  const int np = kept > 0 ? n : 0;
-  const int N = Po + np;
-  gb_voxelmap next = *m;  // the map after this insert (with next_cells / next_points); m is replaced only when everything has succeeded
-  int2* next_cells = iv->cells;
-  size_t next_points = iv->num_points;
+  const int np = kept > 0 ? n : 0;  // points that take part (the unsampled ones get no key)
+  const int N = No + np;
+  gb_voxelmap next = *m;  // the map after this insert; m is replaced only when every step has succeeded
   next.lru_counter = m->lru_counter + 1;
   next.version = m->version + 1;
   if (N > 0) {
     const size_t cub_b = gb_cub_temp_bytes((size_t)N);
-    gb_sort_tmp t;
-    int *d_flags, *d_pos, *d_starts, *d_keep, *d_kpos, *d_ppos, *d_mcount, *d_mstamp, *d_mref, *d_dropped;
-    double4* d_pts = nullptr;
-    double* d_cov = nullptr;
-    unsigned long long *d_hash = nullptr, *d_info;
-    void* d_frame;
-    int4* d_vcoord;
+    InsertScratch s;
     GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
-      t = gb_take_sort_tmp(cv, (size_t)N, cv.take<char>(cub_b), cub_b);
-      d_flags = cv.take<int>(N + 1);
-      d_pos = cv.take<int>(N + 1);
-      d_starts = cv.take<int>(N + 1);
-      d_keep = cv.take<int>(N + 1);
-      d_kpos = cv.take<int>(N + 1);
-      d_ppos = cv.take<int>(N + 1);
-      d_mcount = cv.take<int>(N + 1);
-      d_mstamp = cv.take<int>(N);
-      d_mref = cv.take<int>(N);
-      d_vcoord = cv.take<int4>(N);
-      d_dropped = cv.take<int>(1);
-      d_info = cv.take<unsigned long long>(2);  // {surviving points, surviving voxels}
-      d_frame = cv.take<char>(GB_FRAME_DESC_BYTES);
+      s.t = gb_take_sort_tmp(cv, (size_t)N, cv.take<char>(cub_b), cub_b);
+      s.flags = cv.take<int>(N + 1);
+      s.pos = cv.take<int>(N + 1);
+      s.starts = cv.take<int>(N + 1);
+      s.keep = cv.take<int>(N + 1);
+      s.kpos = cv.take<int>(N + 1);
+      s.vcoord = cv.take<int4>(N);
+      s.dropped = cv.take<int>(1);
+      s.info = cv.take<unsigned long long>(2);
+      s.frame = cv.take<char>(GB_FRAME_DESC_BYTES);
       if (np > 0) {
-        d_pts = cv.take<double4>(np);
-        d_cov = cv.take<double>(6 * (size_t)np);
-        if (kept < n) d_hash = cv.take<unsigned long long>(np);
+        s.pts = cv.take<double4>(np);
+        s.cov = cv.take<double>(6 * (size_t)np);
+        if (kept < n) s.hash = cv.take<unsigned long long>(np);
       }
+      rule.scratch(cv, (size_t)N);
     }));
     const int tb = 256;
-    if (Vo > 0) {
-      GB_CHECK(gb_launch(ctx, "k_ivox_old_keys", k_ivox_old_keys, (Vo + tb - 1) / tb, tb, 0, Vo, m->vkeys, iv->cells, t.keys, t.idx));
-    }
+    if (m->num_voxels > 0) GB_CHECK(rule.old_keys(ctx, s.t));
     if (np > 0) {
-      GB_CHECK(gb_transform_frame(ctx, cloud, T, d_frame, d_pts, d_cov));
-      GB_CHECK(gb_grid_keys(ctx, np, d_pts, 1.0 / iv->resolution, t.keys + Po, t.idx + Po));
+      GB_CHECK(gb_transform_frame(ctx, cloud, T, s.frame, s.pts, s.cov));
+      GB_CHECK(gb_grid_keys(ctx, np, s.pts, m->key_inv_res, s.t.keys + No, s.t.idx + No));
       if (kept < n) {
-        GB_CHECK(gb_launch(ctx, "k_ins_sample_hash", k_ins_sample_hash, (np + tb - 1) / tb, tb, 0, np, seed, t.keys_s));
-        GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, cub_b, t.keys_s, d_hash, np, 0, 64);
-        GB_CHECK(gb_launch(ctx, "k_ins_sample_drop", k_ins_sample_drop, (np + tb - 1) / tb, tb, 0, np, kept, seed, d_hash, t.keys + Po));
+        GB_CHECK(gb_launch(ctx, "k_ins_sample_hash", k_ins_sample_hash, (np + tb - 1) / tb, tb, 0, np, seed, s.t.keys_s));
+        GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, s.t.cub, cub_b, s.t.keys_s, s.hash, np, 0, 64);
+        GB_CHECK(gb_launch(ctx, "k_ins_sample_drop", k_ins_sample_drop, (np + tb - 1) / tb, tb, 0, np, kept, seed, s.hash, s.t.keys + No));
       }
     }
-    GB_CHECK(gb_group_by_key(ctx, N, t, d_flags, d_pos));
-    GB_CHECK(gb_group_starts(ctx, N, t, d_flags, d_pos, d_starts));
-    GB_CHECK(gb_launch(ctx, "k_ivox_merge", k_ivox_merge, (N + 127) / 128, 128, 0, N, d_pos + (N - 1), d_starts, t.keys_s, t.idx_s, Vo, m->vkeys, m->vstamp, m->voxels, d_pts,
-                       iv->max_points, iv->min_dist * iv->min_dist, m->lru_counter, m->lru_horizon, m->lru_clear_cycle, d_mref, d_mcount, d_mstamp, d_keep));
-    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_keep, d_kpos, N);
-    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_mcount, d_ppos, N);
-    GB_CHECK(gb_launch(ctx, "k_ivox_count", k_ivox_count, 1, 1, 0, N, d_kpos, d_ppos, d_info));
+    GB_CHECK(gb_group_by_key(ctx, N, s.t, s.flags, s.pos));
+    GB_CHECK(gb_group_starts(ctx, N, s.t, s.flags, s.pos, s.starts));
+    GB_CHECK(rule.merge(ctx, s, N));
     unsigned long long info[2] = {0, 0};
-    GB_CUDA(cudaMemcpyAsync(info, d_info, sizeof(info), cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaMemcpyAsync(info, s.info, sizeof(info), cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
     const int V = (int)info[1];
-    const size_t P = (size_t)info[0];
+    next.num_voxels = V;
+    next.num_points = (size_t)info[0];
     next.base = nullptr;
     next.buckets = nullptr;
-    next.num_voxels = V;
-    next_points = P;
     Carver size;
-    ivox_layout(size, (size_t)V, P, &next, &next_cells);
+    Rule::layout(size, &next);  // measures, and leaves every state pointer null
     next.bytes = V > 0 ? size.off : 0;
+    gb_status r = GB_OK;
     if (V > 0) {
       GB_CUDA(gb_dev_malloc(ctx->device, size.off, &next.base));
       Carver cv{(char*)next.base};
-      ivox_layout(cv, (size_t)V, P, &next, &next_cells);
-      gb_status s = gb_launch(ctx, "k_ivox_emit", k_ivox_emit, (N + tb - 1) / tb, tb, 0, N, d_pos + (N - 1), d_keep, d_kpos, d_ppos, d_starts, t.keys_s, d_mref, d_mcount, d_mstamp,
-                              m->voxels, d_pts, d_cov, next.vkeys, next.vstamp, next_cells, next.voxels, d_vcoord);
-      if (s != GB_OK) { gb_dev_free(ctx->device, next.base); return s; }
-    } else {
-      next.voxels = nullptr; next_cells = nullptr; next.vkeys = nullptr; next.vstamp = nullptr;
+      Rule::layout(cv, &next);
+      r = rule.emit(ctx, s, N, next);
     }
-    int dropped = 0;
-    gb_status s = table_build(ctx, V, d_vcoord, d_dropped, kIvoxInitBuckets, m->max_scan, 0.0, (double)P, &next.buckets, &next.num_buckets, &dropped);
-    if (s == GB_OK && dropped != 0) {
-      gb_set_error("iVox table: %d points left out of a table of %d buckets", dropped, next.num_buckets);
-      s = GB_ERR_INTERNAL;
-    }
-    if (s != GB_OK) {
+    if (r == GB_OK)
+      r = table_build(ctx, V, s.vcoord, s.dropped, m->init_buckets, m->max_scan, m->drop_rate, (double)info[0], &next.buckets, &next.num_buckets, &next.num_dropped_points);
+    if (r == GB_OK) r = rule.check_table(next);
+    if (r != GB_OK) {  // the insert's one failure exit once its block exists: m is unchanged
       gb_dev_free(ctx->device, next.base);
       gb_dev_free(ctx->device, next.buckets);
-      return s;
+      return r;
     }
     next.bytes += sizeof(int4) * (size_t)next.num_buckets;
   }
   void* old_base = m->base;
   int4* old_buckets = m->buckets;
-  const bool replaced = N > 0;
   *m = next;
-  iv->cells = next_cells;
-  iv->num_points = next_points;
-  if (replaced) {
+  if (N > 0) {
     gb_dev_free(ctx->device, old_base);
     gb_dev_free(ctx->device, old_buckets);
   }
   return GB_OK;
 }
 
+}  // namespace
+
+gb_status gb_map_create_empty_impl(gb_ctx* ctx, gb_voxelmap* m) {
+  m->device = ctx->device;
+  GB_CHECK(table_build(ctx, 0, nullptr, nullptr, m->init_buckets, m->max_scan, m->drop_rate, 0.0, &m->buckets, &m->num_buckets, &m->num_dropped_points));
+  m->bytes = sizeof(int4) * (size_t)m->num_buckets;
+  return GB_OK;
+}
+
+gb_status gb_map_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T, double sampling_rate, unsigned long long seed) {
+  if (m->kind == GB_MAP_IVOX) return map_insert(ctx, m, cloud, T, sampling_rate, seed, IvoxRule{m});
+  return map_insert(ctx, m, cloud, T, sampling_rate, seed, VoxelRule{m});
+}
 
 // ---------------------------------------------------------------------------------------------
 // Morton reordering of a new cloud (PointCloudGPU::clone keeps the caller's order on the host side of the

@@ -114,7 +114,7 @@ GB_API gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float res
 /* voxel_resolution(), voxelmap_info.{num_voxels,num_buckets} (standard_viewer_callbacks.cpp:117; standard_viewer_mem.cpp:76-77) */
 GB_API gb_status gb_voxelmap_info(const gb_voxelmap* map, int* num_voxels, int* num_buckets, float* resolution);
 /* device -> host: buckets NB x 4 int32 (x y z index, index -1 = empty), per voxel num_points, mean (V x 3),
- * cov6 (V x 6); any pointer may be NULL */
+ * cov6 (V x 6); any pointer may be NULL.  GB_ERR_INVALID_ARGUMENT for an iVox (gb_ivox_download). */
 GB_API gb_status gb_voxelmap_download(const gb_voxelmap* map, int32_t* buckets, int32_t* num_points, float* means, float* cov6);
 GB_API gb_status gb_voxelmap_destroy(gb_voxelmap* map);
 
@@ -150,8 +150,8 @@ GB_API gb_status gb_voxelmap_destroy(gb_voxelmap* map);
 GB_API gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolution, int init_num_buckets, int max_bucket_scan_count,
                                                 double target_points_drop_rate, int lru_horizon, int lru_clear_cycle, gb_voxelmap** out);
 /* Insert `cloud` at T_map_cloud (NULL = identity), keeping a sampling_rate share of its points (1 = all).  Every input is
- * validated before any launch: GB_ERR_INVALID_ARGUMENT for a map from gb_voxelmap_build (it keeps no sums), a non-finite
- * T, sampling_rate outside (0, 1], or a cloud / map on another device than ctx. */
+ * validated before any launch: GB_ERR_INVALID_ARGUMENT for a map that is not incremental (from gb_voxelmap_build, which
+ * keeps no sums, or an iVox), a non-finite T, sampling_rate outside (0, 1], or a cloud / map on another device than ctx. */
 GB_API gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_cloud* cloud, const double* T_map_cloud /* 16, col-major */,
                                     double sampling_rate, uint64_t seed);
 
@@ -177,12 +177,17 @@ GB_API gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_clou
  *      step 4 and the neighbour offsets below are this library's statement of it.
  *      Threading and lifetime as for incremental voxel maps: two host synchronisations per insert (one more per extra table
  *      attempt), sweeps created before an insert follow it, do not insert while another thread uses the map. ---- */
-/* neighbor_voxel_mode: 1 (centre), 7 (+ the faces), 19 (+ the edges), 27 (+ the corners).  lru_horizon <= 0: no eviction.
+/* An iVox handle and a voxel-map handle are not interchangeable.  gb_ivox_insert, gb_ivox_info, gb_ivox_download and
+ * gb_gicp_factor_create take an iVox only; gb_vgicp_factor_create and gb_voxelmap_download refuse one, and gb_voxelmap_insert
+ * takes an incremental map only.  Each refuses another kind with GB_ERR_INVALID_ARGUMENT before any launch.  These
+ * refusals are the only change of behaviour from earlier builds, which read a handle of the wrong kind as the other kind.
+ * gb_overlap takes every kind: it tests occupancy only.
+ * neighbor_voxel_mode: 1 (centre), 7 (+ the faces), 19 (+ the edges), 27 (+ the corners).  lru_horizon <= 0: no eviction.
  * GB_ERR_INVALID_ARGUMENT for a non-finite or non-positive resolution, min_dist_in_cell < 0, max_points_in_cell outside
  * [1, 64], another mode or lru_clear_cycle < 1. */
 GB_API gb_status gb_ivox_create(gb_ctx* ctx, double resolution, double min_dist_in_cell, int max_points_in_cell, int neighbor_voxel_mode,
                                 int lru_horizon, int lru_clear_cycle, gb_ivox** out);
-/* validated before any launch: T finite, sampling_rate in (0, 1], cloud and map on ctx's device */
+/* validated before any launch: T finite, sampling_rate in (0, 1], an iVox, cloud and map on ctx's device */
 GB_API gb_status gb_ivox_insert(gb_ctx* ctx, gb_ivox* map, const gb_cloud* cloud, const double* T_map_cloud /* 16 col-major, NULL = I */,
                                 double sampling_rate, uint64_t seed);
 GB_API gb_status gb_ivox_info(const gb_ivox* map, int* num_voxels, size_t* num_points, double* resolution);
@@ -207,8 +212,8 @@ GB_API gb_status gb_vgicp_error(gb_factor* factor, const double T_lin[16], const
  *      (odometry_estimation_cpu.cpp:95-104, max_correspondence_distance = 2 * ivox_resolution).  The source must carry
  *      covariances, as for VGICP.  The result is an ordinary gb_factor: gb_vgicp_linearize / _error / _factor_destroy,
  *      gb_factor_set_*, gb_sweep_* and gb_vgicp_align take it.  The factors of one sweep or call must all be VGICP or all GICP
- *      (GB_ERR_INVALID_ARGUMENT before any launch); GICP sweeps take no pair_index, slab or peer slab; gb_overlap stays
- *      voxel-map only.
+ *      (GB_ERR_INVALID_ARGUMENT before any launch); GICP sweeps take no pair_index, slab or peer slab; gb_overlap takes
+ *      maps, not factors.
  *
  *      The correspondence rule.  q = the source point transformed with the sweep's fp32 pose (the lookup transform of every
  *      sweep), keyed with the fp32 rule (float)(1 / resolution) of every lookup (a point on a voxel face may key to its

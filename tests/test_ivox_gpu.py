@@ -228,6 +228,7 @@ def test_invalid_and_mixed_inputs_are_rejected_before_any_launch(ctx, frames):
     m = gpu.IVoxGPU(1.0, ctx=ctx)
     m.insert(cloud, T)
     vmap = gpu.IncrementalVoxelMapGPU(1.0, ctx=ctx).insert(cloud, T)
+    built = gpu.GaussianVoxelMapGPU(1.0, ctx=ctx).insert(cloud)
     g = gpu.IntegratedGICPFactorGPU(np.eye(4), 0, m, cloud, MAX_CORR, ctx=ctx)
     v = gpu.IntegratedVGICPFactorGPU(np.eye(4), 0, vmap, cloud, ctx=ctx)
     good = capi.pose16(T)
@@ -262,6 +263,15 @@ def test_invalid_and_mixed_inputs_are_rejected_before_any_launch(ctx, frames):
     for args in ((0.0, 0.1, 10, 1), (1.0, -0.1, 10, 1), (1.0, 0.1, 0, 1), (1.0, 0.1, 65, 1), (1.0, 0.1, 10, 5)):
         assert L.gb_ivox_create(ctx.h, *args, 100, 10, C.byref(h)) == 1 and not h.value
     assert L.gb_ivox_create(ctx.h, 1.0, 0.1, 10, 1, 100, 0, C.byref(h)) == 1 and not h.value
+    # a map of another kind: each entry point takes only the kinds it serves
+    for other in (vmap.h, built.h):
+        assert L.gb_ivox_insert(ctx.h, other, cloud.h, capi.ptr(good), 1.0, 0) == 1
+        assert L.gb_ivox_info(other, None, None, None) == 1
+        assert L.gb_ivox_download(other, None, None, None, None) == 1
+        assert L.gb_gicp_factor_create(ctx.h, other, cloud.h, MAX_CORR, C.byref(h)) == 1 and not h.value
+    assert L.gb_voxelmap_insert(ctx.h, m.h, cloud.h, capi.ptr(good), 1.0, 0) == 1
+    assert L.gb_vgicp_factor_create(ctx.h, m.h, cloud.h, 0, C.byref(h)) == 1 and not h.value
+    assert L.gb_voxelmap_download(m.h, None, None, None, None) == 1
     assert ctx.kernel_launches == launches
     if L.gb_device_count() > 1:
         ctx1 = gpu.Context(1)
