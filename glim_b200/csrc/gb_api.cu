@@ -1,4 +1,6 @@
-// gb_api.cu -- implementation of the C-ABI declared in include/glim_b200.h (host side of libglim_b200.so).
+// gb_api.cu -- the shared host side of the C-ABI declared in include/glim_b200.h: errors, the device pool, contexts and
+// arenas, clouds, factors, sweeps and overlap.  The map, preprocess and peer-slab entry points are defined next to their
+// work, in gb_kernels_voxelmap.cu, gb_kernels_preprocess.cu and gb_peer.cu.
 #include "gb_internal.cuh"
 
 #include <stdarg.h>
@@ -120,7 +122,6 @@ void gb_dev_free(int device, void* p) {
 // ---------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------
-static void ctx_release(gb_ctx* ctx);
 static gb_status ctx_create(int device, cudaStream_t stream, bool own, gb_ctx** out) {
   GB_REQUIRE(out, "null output");
   *out = nullptr;
@@ -164,8 +165,8 @@ static void pool_block_free(const gb_pool_block& b) {
 
 // Contexts are reference counted: factors, sweeps and peer slabs hold one; gb_ctx_destroy drops the owner's.  A module may
 // therefore destroy its CUDAStream while factors created on it are still alive (member destruction order, thread exit).
-static void ctx_retain(gb_ctx* ctx) { ctx->refs.fetch_add(1); }
-static void ctx_release(gb_ctx* ctx) {
+void ctx_retain(gb_ctx* ctx) { ctx->refs.fetch_add(1); }
+void ctx_release(gb_ctx* ctx) {
   if (ctx->refs.fetch_sub(1) != 1) return;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
@@ -216,7 +217,7 @@ gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes) {
 // the reference casts Vector4d / Matrix4d to float on the host before the copy (SURVEY K1); so do we, straight into the
 // plane layout in pinned memory, then stage the planes in scratch and Morton-sort them into the cloud on the device
 // (the caller has made the cloud's device current)
-static void cloud_free(gb_cloud* c) {
+void cloud_free(gb_cloud* c) {
   gb_dev_free(c->device, c->base);  // waits for every stream that may still read the cloud, then recycles the block
   delete c;
 }
@@ -320,177 +321,6 @@ extern "C" gb_status gb_cloud_destroy(gb_cloud* c) {
   cloud_free(c);
   return GB_OK;
 }
-
-// ---------------------------------------------------------------------------------------------
-// voxel maps
-// ---------------------------------------------------------------------------------------------
-// (the caller has made the map's device current)
-static void voxelmap_free(gb_voxelmap* m) {
-  gb_dev_free(m->device, m->base);
-  gb_dev_free(m->device, m->buckets);
-  delete m;
-}
-// an empty incremental map or iVox of the parameters in `init` (the caller has entered ctx)
-static gb_status map_create_empty(gb_ctx* ctx, const gb_voxelmap& init, gb_voxelmap** out) {
-  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(init), voxelmap_free);
-  if (!m) return GB_ERR_INTERNAL;
-  GB_CHECK(gb_map_create_empty_impl(ctx, m.get()));
-  *out = m.release();
-  return GB_OK;
-}
-// The checks both inserts make before any launch, the handles read last; *T is the pose to insert at.
-static gb_status insert_args(gb_ctx* ctx, const gb_voxelmap* m, gb_map_kind kind, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, const double** T) {
-  GB_REQUIRE(ctx && m && cloud, "null argument");
-  GB_REQUIRE(sampling_rate > 0.0 && sampling_rate <= 1.0, "sampling_rate must be in (0, 1]");
-  static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-  *T = T_map_cloud ? T_map_cloud : kIdentity;
-  for (int k = 0; k < 16; k++) GB_REQUIRE(std::isfinite((*T)[k]), "T_map_cloud must be finite");
-  GB_REQUIRE(m->kind == kind, kind == GB_MAP_IVOX ? "the map is not an iVox: create it with gb_ivox_create"
-                                                  : "the map is not incremental: create it with gb_voxelmap_create_incremental");
-  GB_REQUIRE(m->device == ctx->device && cloud->device == ctx->device, "cloud / map live on another device");
-  GB_REQUIRE((uint64_t)gb_stored_entries(m) + (uint64_t)cloud->n < (1ull << 31) - 1, "stored entries + cloud points exceed 2^31");
-  return GB_OK;
-}
-// 48-byte records (a voxel's or a stored point's) to the host; any output may be null.  A plain copy, its direction taken
-// from the unified address space: the map may live on another device than the current one, and every producer call
-// returned after its stream had drained.
-static gb_status download_records(const float4* records, size_t count, int32_t* num_points, float* xyz, float* cov6) {
-  if (count == 0 || !(num_points || xyz || cov6)) return GB_OK;
-  std::vector<float4> h(3 * count);
-  GB_CUDA(cudaMemcpy(h.data(), records, sizeof(float4) * h.size(), cudaMemcpyDefault));
-  for (size_t r = 0; r < count; r++) {
-    const float4 a = h[3 * r], b = h[3 * r + 1], c = h[3 * r + 2];
-    if (num_points) num_points[r] = (int32_t)c.y;
-    if (xyz) { xyz[3 * r] = a.x; xyz[3 * r + 1] = a.y; xyz[3 * r + 2] = a.z; }
-    if (cov6) { cov6[6 * r] = a.w; cov6[6 * r + 1] = b.x; cov6[6 * r + 2] = b.y; cov6[6 * r + 3] = b.z; cov6[6 * r + 4] = b.w; cov6[6 * r + 5] = c.x; }
-  }
-  return GB_OK;
-}
-
-extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_num_buckets, int max_bucket_scan_count, double target_points_drop_rate, gb_voxelmap** out) {
-  GB_REQUIRE(ctx && cloud && out, "null argument");
-  GB_REQUIRE(resolution > 0.f, "resolution must be positive");
-  GB_REQUIRE(init_num_buckets > 0 && (init_num_buckets & (init_num_buckets - 1)) == 0, "init_num_buckets must be a power of two");
-  GB_REQUIRE(max_bucket_scan_count > 0, "max_bucket_scan_count must be positive");
-  *out = nullptr;
-  GB_ENTER(ctx);
-  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(), voxelmap_free);
-  if (!m) return GB_ERR_INTERNAL;
-  GB_CHECK(gb_voxelmap_build_impl(ctx, cloud, resolution, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, m.get()));
-  *out = m.release();
-  return GB_OK;
-}
-extern "C" gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolution, int init_num_buckets, int max_bucket_scan_count, double target_points_drop_rate,
-                                                    int lru_horizon, int lru_clear_cycle, gb_voxelmap** out) {
-  GB_REQUIRE(ctx && out, "null argument");
-  GB_REQUIRE(resolution > 0.f && std::isfinite(resolution), "resolution must be positive and finite");
-  GB_REQUIRE(init_num_buckets > 0 && (init_num_buckets & (init_num_buckets - 1)) == 0, "init_num_buckets must be a power of two");
-  GB_REQUIRE(max_bucket_scan_count > 0, "max_bucket_scan_count must be positive");
-  GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
-  *out = nullptr;
-  GB_ENTER(ctx);
-  gb_voxelmap m;
-  m.kind = GB_MAP_INCREMENTAL;
-  m.resolution = resolution;
-  m.inv_res = 1.0f / resolution;
-  m.key_inv_res = 1.0 / (double)resolution;
-  m.max_scan = max_bucket_scan_count;
-  m.init_buckets = init_num_buckets;
-  m.drop_rate = target_points_drop_rate;
-  m.lru_horizon = lru_horizon;
-  m.lru_clear_cycle = lru_clear_cycle;
-  return map_create_empty(ctx, m, out);
-}
-extern "C" gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
-  const double* T;
-  GB_CHECK(insert_args(ctx, map, GB_MAP_INCREMENTAL, cloud, T_map_cloud, sampling_rate, &T));
-  GB_ENTER(ctx);
-  return gb_map_insert_impl(ctx, map, cloud, T, sampling_rate, (unsigned long long)seed);
-}
-extern "C" gb_status gb_voxelmap_info(const gb_voxelmap* m, int* num_voxels, int* num_buckets, float* resolution) {
-  GB_REQUIRE(m, "null map");
-  if (num_voxels) *num_voxels = m->num_voxels;
-  if (num_buckets) *num_buckets = m->num_buckets;
-  if (resolution) *resolution = m->resolution;
-  return GB_OK;
-}
-extern "C" gb_status gb_voxelmap_download(const gb_voxelmap* m, int32_t* buckets, int32_t* num_points, float* means, float* cov6) {
-  GB_REQUIRE(m, "null map");
-  GB_REQUIRE(m->kind != GB_MAP_IVOX, "an iVox holds points, not voxels: use gb_ivox_download");
-  if (buckets) GB_CUDA(cudaMemcpy(buckets, m->buckets, sizeof(int4) * (size_t)m->num_buckets, cudaMemcpyDefault));
-  return download_records(m->voxels, (size_t)m->num_voxels, num_points, means, cov6);
-}
-extern "C" gb_status gb_voxelmap_destroy(gb_voxelmap* m) {
-  if (!m) return GB_OK;
-  cudaSetDevice(m->device);
-  voxelmap_free(m);
-  return GB_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// iVox: a gb_voxelmap of kind GB_MAP_IVOX (gb_internal.cuh); voxelmap_free and gb_voxelmap_destroy release it
-// ---------------------------------------------------------------------------------------------
-extern "C" gb_status gb_ivox_create(gb_ctx* ctx, double resolution, double min_dist_in_cell, int max_points_in_cell, int neighbor_voxel_mode, int lru_horizon,
-                                    int lru_clear_cycle, gb_ivox** out) {
-  GB_REQUIRE(ctx && out, "null argument");
-  GB_REQUIRE(std::isfinite(resolution) && resolution > 0.0, "resolution must be positive and finite");
-  GB_REQUIRE(min_dist_in_cell >= 0.0, "min_dist_in_cell must be >= 0");
-  GB_REQUIRE(max_points_in_cell >= 1 && max_points_in_cell <= 64, "max_points_in_cell must be in [1, 64]");
-  GB_REQUIRE(neighbor_voxel_mode == 1 || neighbor_voxel_mode == 7 || neighbor_voxel_mode == 19 || neighbor_voxel_mode == 27, "neighbor_voxel_mode must be 1, 7, 19 or 27");
-  GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
-  *out = nullptr;
-  GB_ENTER(ctx);
-  gb_voxelmap m;
-  m.kind = GB_MAP_IVOX;
-  m.ivox_resolution = resolution;
-  m.min_dist = min_dist_in_cell;
-  m.max_points = max_points_in_cell;
-  m.mode = neighbor_voxel_mode;
-  m.resolution = (float)resolution;
-  m.inv_res = (float)(1.0 / resolution);
-  m.key_inv_res = 1.0 / resolution;
-  m.max_scan = 10;          // the build's table (16384 buckets doubled until >= 8 V, 10 probes) with drop rate 0
-  m.init_buckets = 16384;
-  m.lru_horizon = lru_horizon;
-  m.lru_clear_cycle = lru_clear_cycle;
-  gb_voxelmap* h = nullptr;
-  GB_CHECK(map_create_empty(ctx, m, &h));
-  *out = reinterpret_cast<gb_ivox*>(h);
-  return GB_OK;
-}
-extern "C" gb_status gb_ivox_insert(gb_ctx* ctx, gb_ivox* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
-  gb_voxelmap* m = ivox_map(map);
-  const double* T;
-  GB_CHECK(insert_args(ctx, m, GB_MAP_IVOX, cloud, T_map_cloud, sampling_rate, &T));
-  GB_ENTER(ctx);
-  return gb_map_insert_impl(ctx, m, cloud, T, sampling_rate, (unsigned long long)seed);
-}
-extern "C" gb_status gb_ivox_info(const gb_ivox* map, int* num_voxels, size_t* num_points, double* resolution) {
-  const gb_voxelmap* m = ivox_map(map);
-  GB_REQUIRE(m && m->kind == GB_MAP_IVOX, "null map, or not an iVox");
-  if (num_voxels) *num_voxels = m->num_voxels;
-  if (num_points) *num_points = m->num_points;
-  if (resolution) *resolution = m->ivox_resolution;
-  return GB_OK;
-}
-extern "C" gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords, int32_t* voxel_counts, float* xyz, float* cov6) {
-  const gb_voxelmap* m = ivox_map(map);
-  GB_REQUIRE(m && m->kind == GB_MAP_IVOX, "null map, or not an iVox");
-  const size_t V = (size_t)m->num_voxels;
-  if (V > 0 && (voxel_coords || voxel_counts)) {
-    std::vector<unsigned long long> keys(V);
-    std::vector<int2> cells(V);
-    GB_CUDA(cudaMemcpy(keys.data(), m->vkeys, sizeof(unsigned long long) * V, cudaMemcpyDefault));
-    GB_CUDA(cudaMemcpy(cells.data(), m->cells, sizeof(int2) * V, cudaMemcpyDefault));
-    for (size_t v = 0; v < V; v++) {
-      if (voxel_coords)
-        for (int a = 0; a < 3; a++) voxel_coords[3 * v + a] = (int32_t)((keys[v] >> (42 - 21 * a)) & 0x1FFFFF) - (1 << 20);
-      if (voxel_counts) voxel_counts[v] = cells[v].y;
-    }
-  }
-  return download_records(m->voxels, m->num_points, nullptr, xyz, cov6);
-}
-extern "C" gb_status gb_ivox_destroy(gb_ivox* map) { return gb_voxelmap_destroy(ivox_map(map)); }
 
 // ---------------------------------------------------------------------------------------------
 // factors and sweeps
@@ -1102,190 +932,6 @@ extern "C" gb_status gb_slab_row_hessian_blocks(const float* row, double error_s
 }
 
 // ---------------------------------------------------------------------------------------------
-// fused multi-GPU result exchange (peer slabs over CUDA IPC)
-// ---------------------------------------------------------------------------------------------
-static void peer_slab_free(gb_peer_slab* ps) {
-  gb_ctx* ctx = ps->ctx;
-  {
-    GB_LOCK(ctx);
-    cudaSetDevice(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-    for (int p = 0; p < ps->world; p++)
-      if (ps->opened[p]) cudaIpcCloseMemHandle(ps->peer[p]);
-    if (ps->local) cudaFree(ps->local);
-    if (ps->d_my_pairs) cudaFree(ps->d_my_pairs);
-    if (ps->h_pinned) cudaFreeHost(ps->h_pinned);
-    delete ps;
-  }
-  ctx_release(ctx);  // outside the lock: it may delete the context
-}
-
-extern "C" gb_status gb_peer_slab_create(gb_ctx* ctx, size_t num_pairs, int world, int rank, gb_peer_slab** out) {
-  GB_REQUIRE(ctx && out, "null argument");
-  GB_REQUIRE(world >= 1 && world <= GB_MAX_PEERS && rank >= 0 && rank < world, "world must be 1..8 and rank < world");
-  GB_REQUIRE(num_pairs > 0, "num_pairs must be positive");
-  *out = nullptr;
-  GB_ENTER(ctx);
-  gb_owned<gb_peer_slab> ps(new (std::nothrow) gb_peer_slab(), peer_slab_free);
-  if (!ps) return GB_ERR_INTERNAL;
-  ctx_retain(ctx);
-  ps->ctx = ctx; ps->num_pairs = num_pairs; ps->world = world; ps->rank = rank;
-  ps->connected = (world == 1);
-  // fused: the sweep's epilogue stores every finished row straight into all peers; deferred: rows go to the local buffer and
-  // the exchange kernel pushes them (see gb_launch_peer_signal_wait).  The peer stores' cost to the sweep grows with the
-  // rank count faster than the exchange kernel's extra time -> fused up to 4 ranks, deferred above.  GB_PEER_PUSH=fused|deferred forces one.
-  {
-    const char* e = getenv("GB_PEER_PUSH");
-    ps->deferred = world > 4;
-    if (e && !strcmp(e, "fused")) ps->deferred = false;
-    if (e && !strcmp(e, "deferred")) ps->deferred = true;
-  }
-  Carver size;
-  gb_peer_layout(size, num_pairs, world);
-  GB_CUDA(cudaMalloc((void**)&ps->local, size.off));
-  ps->peer[rank] = ps->local;
-  GB_CUDA(cudaMemsetAsync(ps->local, 0, size.off, ctx->stream));
-  GB_CUDA(cudaStreamSynchronize(ctx->stream));
-  GB_CUDA(cudaMallocHost((void**)&ps->h_pinned, num_pairs * GB_SLAB_STRIDE * sizeof(float) + 64));
-  *out = ps.release();
-  return GB_OK;
-}
-
-extern "C" gb_status gb_peer_slab_export(gb_peer_slab* ps, void* handle) {
-  GB_REQUIRE(ps && handle, "null argument");
-  static_assert(sizeof(cudaIpcMemHandle_t) == GB_IPC_HANDLE_BYTES, "IPC handle size");
-  GB_ENTER(ps->ctx);
-  cudaIpcMemHandle_t h;
-  GB_CUDA(cudaIpcGetMemHandle(&h, ps->local));
-  memcpy(handle, &h, sizeof(h));
-  return GB_OK;
-}
-
-extern "C" gb_status gb_peer_slab_connect(gb_peer_slab* ps, const void* handles) {
-  GB_REQUIRE(ps && handles, "null argument");
-  GB_ENTER(ps->ctx);
-  for (int p = 0; p < ps->world; p++) {
-    if (p == ps->rank || ps->opened[p]) continue;
-    cudaIpcMemHandle_t h;
-    memcpy(&h, (const char*)handles + (size_t)p * GB_IPC_HANDLE_BYTES, sizeof(h));
-    void* ptr = nullptr;
-    GB_CUDA(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
-    ps->peer[p] = (char*)ptr;
-    ps->opened[p] = true;
-  }
-  ps->connected = true;
-  return GB_OK;
-}
-
-extern "C" gb_status gb_peer_slab_destroy(gb_peer_slab* ps) {
-  if (ps) peer_slab_free(ps);
-  return GB_OK;
-}
-
-// Replaces the device block *block (nullptr: none yet; the stream has drained) with a fresh cudaMalloc block of the layout.
-// *block is the layout's first array: measuring sets it to nullptr, so it never points at a freed block.
-template <typename Layout> static gb_status dev_block_realloc(void** block, Layout&& layout) {
-  if (*block) GB_CUDA(cudaFree(*block));
-  Carver size;
-  layout(size);
-  Carver cv;
-  GB_CUDA(cudaMalloc((void**)&cv.base, size.off));
-  layout(cv);
-  return GB_OK;
-}
-
-extern "C" gb_status gb_sweep_attach_peer_slab(gb_sweep* s, gb_peer_slab* ps) {
-  GB_REQUIRE(s, "null sweep");
-  if (!ps) { s->peer = nullptr; return GB_OK; }
-  GB_REQUIRE(!s->gicp, "no peer slab can be attached to a GICP sweep");
-  GB_REQUIRE(ps->ctx == s->ctx, "peer slab belongs to another context");
-  GB_REQUIRE(ps->connected, "connect the peer slab (gb_peer_slab_connect) before attaching it");
-  // CSR: global pair id -> this sweep's factor indices
-  const size_t P = ps->num_pairs;
-  std::vector<int> ptr(P + 1, 0), fac(s->F);
-  for (size_t f = 0; f < s->F; f++) {
-    GB_REQUIRE(s->h_pair[f] >= 0 && (size_t)s->h_pair[f] < P, "pair index out of range for this peer slab");
-    ptr[s->h_pair[f] + 1]++;
-  }
-  for (size_t k = 0; k < P; k++) ptr[k + 1] += ptr[k];
-  std::vector<int> fill(ptr.begin(), ptr.end() - 1);
-  for (size_t f = 0; f < s->F; f++) fac[fill[s->h_pair[f]]++] = (int)f;
-  // the pairs this sweep owns (one sweep per peer slab): the rows the exchange kernel copies to the peers
-  std::vector<int> mine;
-  for (size_t k = 0; k < P; k++) if (ptr[k + 1] > ptr[k]) mine.push_back((int)k);
-  GB_ENTER(s->ctx);
-  GB_CUDA(cudaStreamSynchronize(s->ctx->stream));
-  GB_CHECK(dev_block_realloc((void**)&s->d_pair_ptr, [&](Carver& cv) {
-    s->d_pair_ptr = cv.take<int>(P + 1);
-    s->d_pair_factors = cv.take<int>(std::max<size_t>(1, s->F));
-    s->d_pair_done = cv.take<unsigned>(P);
-    s->d_peer_tables = cv.take<PeerPush>(2);
-  }));
-  GB_CHECK(dev_block_realloc((void**)&ps->d_my_pairs, [&](Carver& cv) { ps->d_my_pairs = cv.take<int>(std::max<size_t>(1, mine.size())); }));
-  PeerPush tabs[2];
-  memset(tabs, 0, sizeof(tabs));
-  for (int par = 0; par < 2; par++) {
-    if (ps->deferred) {  // the sweep writes this rank's buffer only
-      tabs[par].world = 1;
-      tabs[par].base[0] = gb_peer_regions_of(ps, ps->rank).buf[par];
-    } else {
-      tabs[par].world = ps->world;
-      for (int p = 0; p < ps->world; p++) tabs[par].base[p] = gb_peer_regions_of(ps, p).buf[par];
-    }
-    tabs[par].pair_ptr = s->d_pair_ptr; tabs[par].pair_factors = s->d_pair_factors; tabs[par].pair_done = s->d_pair_done;
-  }
-  GB_CUDA(cudaMemcpy(s->d_peer_tables, tabs, sizeof(tabs), cudaMemcpyHostToDevice));
-  GB_CUDA(cudaMemcpy(s->d_pair_ptr, ptr.data(), sizeof(int) * (P + 1), cudaMemcpyHostToDevice));
-  if (s->F) GB_CUDA(cudaMemcpy(s->d_pair_factors, fac.data(), sizeof(int) * s->F, cudaMemcpyHostToDevice));
-  GB_CUDA(cudaMemset(s->d_pair_done, 0, sizeof(unsigned) * P));
-  ps->num_my_pairs = (int)mine.size();
-  if (!mine.empty()) GB_CUDA(cudaMemcpy(ps->d_my_pairs, mine.data(), sizeof(int) * mine.size(), cudaMemcpyHostToDevice));
-  s->peer = ps;
-  return GB_OK;
-}
-
-extern "C" gb_status gb_peer_slab_signal_wait(gb_peer_slab* ps) {
-  GB_REQUIRE(ps, "null peer slab");
-  GB_REQUIRE(ps->connected, "gb_peer_slab_connect has not been called");
-  GB_ENTER(ps->ctx);
-  ps->step++;
-  GB_CHECK(gb_launch_peer_signal_wait(ps));
-  ps->completed_parity = ps->parity;
-  ps->parity ^= 1;
-  return GB_OK;
-}
-
-extern "C" gb_status gb_peer_slab_device_ptr(gb_peer_slab* ps, void** device_ptr) {
-  GB_REQUIRE(ps && device_ptr, "null argument");
-  *device_ptr = gb_peer_regions_of(ps, ps->rank).buf[ps->completed_parity];
-  return GB_OK;
-}
-
-extern "C" gb_status gb_peer_slab_fetch_async(gb_peer_slab* ps, const float** host_ptr) {
-  GB_REQUIRE(ps, "null peer slab");
-  GB_ENTER(ps->ctx);
-  const size_t bytes = ps->num_pairs * GB_SLAB_STRIDE * sizeof(float);
-  const gb_peer_regions r = gb_peer_regions_of(ps, ps->rank);
-  GB_CUDA(cudaMemcpyAsync(ps->h_pinned, r.buf[ps->completed_parity], bytes, cudaMemcpyDeviceToHost, ps->ctx->stream));
-  GB_CUDA(cudaMemcpyAsync((char*)ps->h_pinned + bytes, r.timeout, sizeof(int), cudaMemcpyDeviceToHost, ps->ctx->stream));
-  if (host_ptr) *host_ptr = ps->h_pinned;
-  return GB_OK;
-}
-
-extern "C" gb_status gb_peer_slab_fetch(gb_peer_slab* ps, float* host) {
-  GB_REQUIRE(ps && host, "null argument");
-  GB_ENTER(ps->ctx);
-  const size_t bytes = ps->num_pairs * GB_SLAB_STRIDE * sizeof(float);
-  GB_CHECK(gb_peer_slab_fetch_async(ps, nullptr));
-  GB_CUDA(cudaStreamSynchronize(ps->ctx->stream));
-  int timeout = 0;
-  memcpy(&timeout, (char*)ps->h_pinned + bytes, sizeof(int));
-  if (timeout) { gb_set_error("peer slab: a peer did not publish its completion flag within the timeout"); return GB_ERR_INTERNAL; }
-  memcpy(host, ps->h_pinned, bytes);
-  return GB_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
 // overlap
 // ---------------------------------------------------------------------------------------------
 extern "C" gb_status gb_overlap(gb_ctx* ctx, size_t T, const gb_voxelmap* const* targets, const gb_cloud* source, const double* deltas, double* overlap) {
@@ -1319,105 +965,4 @@ extern "C" gb_status gb_overlap(gb_ctx* ctx, size_t T, const gb_voxelmap* const*
   GB_CUDA(cudaStreamSynchronize(ctx->stream));
   *overlap = (double)*h.count / (double)source->n;
   return GB_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// preprocess
-// ---------------------------------------------------------------------------------------------
-extern "C" gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, const int32_t* neighbors, int k_correspondences, int k_neighbors, double* normals4, double* cov4x4) {
-  GB_REQUIRE(ctx, "null ctx");
-  if (n == 0) return GB_OK;
-  GB_REQUIRE(xyzw && neighbors && normals4 && cov4x4, "null argument");
-  GB_REQUIRE(k_neighbors > 0 && k_neighbors <= k_correspondences, "k_neighbors must be in [1, k_correspondences]");
-  GB_REQUIRE(n < (size_t)1 << 30, "too many points");
-  // the kernel gathers the points of the first k_neighbors entries of every row: an index outside [0, n) would be an
-  // out-of-bounds device read
-  for (size_t i = 0; i < n; i++)
-    for (int j = 0; j < k_neighbors; j++) {
-      const int32_t q = neighbors[i * (size_t)k_correspondences + j];
-      GB_REQUIRE(q >= 0 && (size_t)q < n, "neighbour index out of range [0, n)");
-    }
-  GB_ENTER(ctx);
-  return gb_covariances_impl(ctx, n, xyzw, neighbors, k_correspondences, k_neighbors, normals4, cov4x4);
-}
-extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors) {
-  GB_REQUIRE(ctx, "null ctx");
-  if (n == 0) return GB_OK;
-  GB_REQUIRE(xyzw && neighbors && k > 0, "null argument");
-  GB_REQUIRE(gb_knn_instantiated(k), "k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
-  GB_ENTER(ctx);
-  // >= 4096 points: exact search on a pyramid of hash grids (one Morton sort, cell size 0.25 m x 4^level); fewer: the tiled
-  // brute force.  GB_KNN=pyramid / brute forces one.
-  const char* mode = getenv("GB_KNN");
-  const bool pyramid = mode ? (strcmp(mode, "pyramid") == 0) : (n >= 4096);
-  if (pyramid) return gb_find_neighbors_pyramid_impl(ctx, n, xyzw, k, neighbors);
-  return gb_find_neighbors_impl(ctx, n, xyzw, k, neighbors);
-}
-
-extern "C" gb_status gb_merge_frames(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, double resolution, int target, uint64_t seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud** out_cloud) {
-  GB_REQUIRE(ctx && num_out, "null argument");
-  *num_out = 0;
-  if (out_cloud) *out_cloud = nullptr;
-  if (K == 0) return GB_OK;
-  GB_REQUIRE(frames && poses, "null frames / poses");
-  GB_REQUIRE(resolution > 0.0, "downsample_resolution must be positive");
-  size_t total = 0;
-  for (size_t k = 0; k < K; k++) {
-    GB_REQUIRE(frames[k] && frames[k]->device == ctx->device, "null frame / frame on another device");
-    total += frames[k]->n;
-  }
-  GB_REQUIRE(total < (size_t)1 << 30 && K < 65536, "too many points / frames");
-  GB_ENTER(ctx);
-  gb_owned<gb_cloud> c(out_cloud ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
-  if (out_cloud && !c) return GB_ERR_INTERNAL;
-  if (c) c->device = ctx->device;
-  GB_CHECK(gb_merge_frames_impl(ctx, (int)K, frames, poses, resolution, target, seed, out_xyzw, out_cov4x4, num_out, c.get()));
-  GB_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (out_cloud) *out_cloud = c.release();
-  return GB_OK;
-}
-
-extern "C" gb_status gb_preprocess_default_params(gb_preprocess_params* p) {
-  GB_REQUIRE(p, "null params");
-  memset(p, 0, sizeof(*p));
-  p->distance_near_thresh = 0.5;      // config_preprocess.json:20
-  p->distance_far_thresh = 100.0;     // :21
-  p->use_random_grid_downsampling = 1;  // :22
-  p->downsample_resolution = 1.0;     // :23
-  p->downsample_target = 10000;       // :24
-  p->downsample_rate = 0.1;           // :25
-  p->seed = 0;
-  p->outlier_removal_k = 10;          // :27
-  p->outlier_std_mul_factor = 1.0;    // :28
-  p->k_correspondences = 10;          // :33
-  p->estimate_covariances = 1;
-  for (int i = 0; i < 4; i++) p->T_imu_lidar[i * 5] = 1.0;
-  return GB_OK;
-}
-extern "C" gb_status gb_preprocess(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out) {
-  GB_REQUIRE(ctx && P && out, "null argument");
-  out->num_points = 0; out->last_time = 0.0; out->cloud = nullptr;
-  GB_REQUIRE(n < (size_t)1 << 30, "too many points");
-  GB_REQUIRE(gb_knn_instantiated(P->k_correspondences), "k_correspondences is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
-  GB_REQUIRE(P->k_neighbors_cov >= 0 && P->k_neighbors_cov <= P->k_correspondences, "k_neighbors_cov must be in [0, k_correspondences]");
-  GB_REQUIRE(!P->enable_outlier_removal || gb_knn_instantiated(P->outlier_removal_k), "outlier_removal_k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
-  GB_REQUIRE(P->crop_bbox_frame >= 0 && P->crop_bbox_frame <= 2, "crop_bbox_frame must be 0 (off), 1 (lidar) or 2 (imu)");
-  if (n == 0) return GB_OK;
-  GB_REQUIRE(xyzw, "null points");
-  GB_ENTER(ctx);
-  gb_owned<gb_cloud> c(P->estimate_covariances ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
-  if (P->estimate_covariances && !c) return GB_ERR_INTERNAL;
-  if (c) c->device = ctx->device;
-  GB_CHECK(gb_preprocess_impl(ctx, n, xyzw, times, intensities, P, out, c.get()));
-  GB_CUDA(cudaStreamSynchronize(ctx->stream));  // the cloud is complete when the call returns (it may be used from another context)
-  out->cloud = c.release();
-  return GB_OK;
-}
-extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, double resolution, double* out_xyzw, double* out_times, double* out_intensities, size_t* num_out) {
-  GB_REQUIRE(ctx && num_out, "null argument");
-  *num_out = 0;
-  if (n == 0) return GB_OK;
-  GB_REQUIRE(xyzw && out_xyzw && resolution > 0.0, "null argument");
-  GB_ENTER(ctx);
-  return gb_voxelgrid_sampling_impl(ctx, n, xyzw, times, intensities, resolution, out_xyzw, out_times, out_intensities, num_out);
 }

@@ -160,7 +160,7 @@ struct gb_peer_slab {
   unsigned step = 0;              // last launched step
   int parity = 0;                 // buffer written by the NEXT launch
   int completed_parity = 0;       // buffer completed by the last signal_wait
-  float* h_pinned = nullptr;      // num_pairs x GB_SLAB_STRIDE + the timeout word, for the fetches
+  float* h_pinned = nullptr;      // the rows and the timeout word of the fetches (peer_fetch_layout, gb_peer.cu)
   bool connected = false;
   // deferred exchange (default): the sweep stores finished pair rows into the LOCAL buffer only; the exchange kernel that
   // follows it copies this rank's rows to every peer (one CTA per peer) before it publishes the completion flags
@@ -293,7 +293,10 @@ gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes);  // a.base h
 // ctx_release): it releases everything the handle owns, never returns early, and ends with the delete.  A creation holds
 // its partial handle in a gb_owned with that function, so that every failure exit frees it, and releases it on success.
 template <typename T> using gb_owned = std::unique_ptr<T, void (*)(T*)>;
+void cloud_free(gb_cloud* c);
 void sweep_free(gb_sweep* s);
+void ctx_retain(gb_ctx* ctx);
+void ctx_release(gb_ctx* ctx);
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
@@ -397,13 +400,7 @@ gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n, const gb_planes& st
 enum { GB_MODE_LINEARIZE = 0, GB_MODE_ERROR = 1 };
 gb_status gb_launch_sweep(gb_sweep* s, int mode);
 gb_status gb_launch_gicp_sweep(gb_sweep* s, int mode);  // gb_launch_sweep of a GICP sweep
-gb_status gb_launch_peer_signal_wait(gb_peer_slab* ps);
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count);
-gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_buckets, int max_scan, double drop_rate, gb_voxelmap* out);
-// An incremental map or iVox whose parameters are set: its device and empty table.
-gb_status gb_map_create_empty_impl(gb_ctx* ctx, gb_voxelmap* m);
-// One insert into an incremental map or an iVox, by its kind.
-gb_status gb_map_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, unsigned long long seed);
 // Shared with gb_merge_frames (gb_kernels_preprocess.cu): one frame's points q = R a + t and covariances R C R^T in
 // un-contracted fp64, in the caller's point order (pts: n x double4, cov6: n x 6 upper triangle).  d_frame: GB_FRAME_DESC_BYTES
 // of device scratch for the frame descriptor.  One launch.
@@ -412,15 +409,6 @@ gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T_col
 // k_grid_keys of the voxel-grid paths: key = packed floor(p * inv_res) in fp64 (~0 for non-finite / out-of-range points),
 // idx[i] = i.  One launch.
 gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx);
-gb_status gb_covariances_impl(gb_ctx* ctx, size_t n, const double* xyzw, const int32_t* neighbors, int kc, int k, double* normals4, double* cov4x4);
-gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out, gb_cloud* cloud_out);
-gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out);
-gb_status gb_find_neighbors_pyramid_impl(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors);
-gb_status gb_find_neighbors_impl(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors);
-// true iff the k-NN kernels are instantiated for k neighbours (1-10, 12, 15, 16, 20, 24, 32); entry points check it before
-// any launch
-bool gb_knn_instantiated(int k);
-gb_status gb_voxelgrid_sampling_impl(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, double resolution, double* out_xyzw, double* out_times, double* out_intensities, size_t* num_out);
 
 // ---------------------------------------------------------------------------------------------
 // device helpers shared by kernels

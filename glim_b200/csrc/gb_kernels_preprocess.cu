@@ -9,6 +9,7 @@
 // All three work in fp64 like the reference's host code (Vector4d / Matrix4d).
 // The voxel grouping (sort, head flags, scan, voxel starts) and the device cloud build are shared with the voxel-map build
 // (gb_group_by_key, gb_group_starts, gb_cloud_build in gb_kernels_voxelmap.cu); only the fp64 key kernel is this file's.
+// The entry points gb_covariances, gb_find_neighbors, gb_voxelgrid_sampling, gb_preprocess and gb_merge_frames are defined here.
 #include "gb_internal.cuh"
 #include "gb_cov_math.cuh"  // plane_covariance (shared with the host-compiled CPU test of the covariance arithmetic)
 
@@ -17,6 +18,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <new>
 #include <type_traits>
 
 namespace {
@@ -146,7 +148,8 @@ template <typename Launch> static gb_status knn_dispatch(int k, Launch&& launch)
   gb_set_error("k = %d is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)", k);
   return GB_ERR_INVALID_ARGUMENT;
 }
-bool gb_knn_instantiated(int k) {
+// true iff the k-NN kernels are instantiated for k neighbours; entry points check it before any launch
+static bool gb_knn_instantiated(int k) {
   return knn_dispatch(k, [](auto) { return GB_OK; }) == GB_OK;
 }
 
@@ -160,9 +163,9 @@ size_t gb_cub_temp_bytes(size_t n_) {
   return std::max({sort_pairs, sort_keys, scan, sum});
 }
 
-gb_status gb_find_neighbors_impl(gb_ctx* ctx, size_t n_, const double* xyzw, int k, int32_t* neighbors) {
+// gb_find_neighbors by brute force
+static gb_status find_neighbors_brute(gb_ctx* ctx, size_t n_, const double* xyzw, int k, int32_t* neighbors) {
   const int n = (int)n_;
-  if (n == 0) return GB_OK;
   cudaStream_t st = ctx->stream;
   double4* d_pts;
   int* d_nb;
@@ -177,60 +180,73 @@ gb_status gb_find_neighbors_impl(gb_ctx* ctx, size_t n_, const double* xyzw, int
   return GB_OK;
 }
 
-gb_status gb_covariances_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const int32_t* neighbors, int kc, int k, double* normals4, double* cov4x4) {
-  const int n = (int)n_;
+extern "C" gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, const int32_t* neighbors, int k_correspondences, int k_neighbors, double* normals4, double* cov4x4) {
+  GB_REQUIRE(ctx, "null ctx");
   if (n == 0) return GB_OK;  // cloud_covariance_estimation.cpp:49-51
+  GB_REQUIRE(xyzw && neighbors && normals4 && cov4x4, "null argument");
+  GB_REQUIRE(k_neighbors > 0 && k_neighbors <= k_correspondences, "k_neighbors must be in [1, k_correspondences]");
+  GB_REQUIRE(n < (size_t)1 << 30, "too many points");
+  // the kernel gathers the points of the first k_neighbors entries of every row: an index outside [0, n) would be an
+  // out-of-bounds device read
+  for (size_t i = 0; i < n; i++)
+    for (int j = 0; j < k_neighbors; j++) {
+      const int32_t q = neighbors[i * (size_t)k_correspondences + j];
+      GB_REQUIRE(q >= 0 && (size_t)q < n, "neighbour index out of range [0, n)");
+    }
+  GB_ENTER(ctx);
   cudaStream_t st = ctx->stream;
   double4 *d_pts, *d_nrm;
   int* d_nb;
   double* d_cov;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     d_pts = cv.take<double4>(n);
-    d_nb = cv.take<int>((size_t)n * kc);
+    d_nb = cv.take<int>(n * k_correspondences);
     d_nrm = cv.take<double4>(n);
-    d_cov = cv.take<double>(16 * (size_t)n);
+    d_cov = cv.take<double>(16 * n);
   }));
-  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * (size_t)n, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(d_nb, neighbors, sizeof(int) * (size_t)n * kc, cudaMemcpyHostToDevice, st));
-  GB_CHECK(gb_launch(ctx, "k_covariances", k_covariances, (n + 127) / 128, 128, 0, n, d_pts, d_nb, kc, k, d_nrm, d_cov));
-  GB_CUDA(cudaMemcpyAsync(normals4, d_nrm, sizeof(double4) * (size_t)n, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaMemcpyAsync(cov4x4, d_cov, sizeof(double) * 16 * (size_t)n, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * n, cudaMemcpyHostToDevice, st));
+  GB_CUDA(cudaMemcpyAsync(d_nb, neighbors, sizeof(int) * n * k_correspondences, cudaMemcpyHostToDevice, st));
+  GB_CHECK(gb_launch(ctx, "k_covariances", k_covariances, (n + 127) / 128, 128, 0, (int)n, d_pts, d_nb, k_correspondences, k_neighbors, d_nrm, d_cov));
+  GB_CUDA(cudaMemcpyAsync(normals4, d_nrm, sizeof(double4) * n, cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaMemcpyAsync(cov4x4, d_cov, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
   return GB_OK;
 }
 
-gb_status gb_voxelgrid_sampling_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const double* times, const double* intensities, double resolution, double* out_xyzw, double* out_times, double* out_intensities, size_t* num_out) {
-  const int n = (int)n_;
+extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, double resolution, double* out_xyzw, double* out_times, double* out_intensities, size_t* num_out) {
+  GB_REQUIRE(ctx && num_out, "null argument");
   *num_out = 0;
   if (n == 0) return GB_OK;
+  GB_REQUIRE(xyzw && out_xyzw && resolution > 0.0, "null argument");
+  GB_ENTER(ctx);
   cudaStream_t st = ctx->stream;
-  const size_t N = (size_t)n, cub_b = gb_cub_temp_bytes(N);
+  const size_t cub_b = gb_cub_temp_bytes(n);
   gb_sort_tmp t;
   double4 *d_pts, *d_opts;
   double *d_t, *d_i, *d_ot, *d_oi;
   int *d_flags, *d_pos, *d_starts;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
-    t = gb_take_sort_tmp(cv, N, cv.take<char>(cub_b), cub_b);
-    d_pts = cv.take<double4>(N);
-    d_opts = cv.take<double4>(N);
-    d_t = cv.take<double>(N);
-    d_i = cv.take<double>(N);
-    d_ot = cv.take<double>(N);
-    d_oi = cv.take<double>(N);
-    d_flags = cv.take<int>(N + 1);
-    d_pos = cv.take<int>(N + 1);
-    d_starts = cv.take<int>(N + 1);
+    t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
+    d_pts = cv.take<double4>(n);
+    d_opts = cv.take<double4>(n);
+    d_t = cv.take<double>(n);
+    d_i = cv.take<double>(n);
+    d_ot = cv.take<double>(n);
+    d_oi = cv.take<double>(n);
+    d_flags = cv.take<int>(n + 1);
+    d_pos = cv.take<int>(n + 1);
+    d_starts = cv.take<int>(n + 1);
   }));
-  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * N, cudaMemcpyHostToDevice, st));
-  if (times) GB_CUDA(cudaMemcpyAsync(d_t, times, sizeof(double) * N, cudaMemcpyHostToDevice, st));
-  if (intensities) GB_CUDA(cudaMemcpyAsync(d_i, intensities, sizeof(double) * N, cudaMemcpyHostToDevice, st));
-  GB_CHECK(gb_grid_keys(ctx, n, d_pts, 1.0 / resolution, t.keys, t.idx));
-  GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
+  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * n, cudaMemcpyHostToDevice, st));
+  if (times) GB_CUDA(cudaMemcpyAsync(d_t, times, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  if (intensities) GB_CUDA(cudaMemcpyAsync(d_i, intensities, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  GB_CHECK(gb_grid_keys(ctx, (int)n, d_pts, 1.0 / resolution, t.keys, t.idx));
+  GB_CHECK(gb_group_by_key(ctx, (int)n, t, d_flags, d_pos));
   int V = 0;
   GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
   if (V > 0) {
-    GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
+    GB_CHECK(gb_group_starts(ctx, (int)n, t, d_flags, d_pos, d_starts));
     GB_CHECK(gb_launch(ctx, "k_grid_means_counted", k_grid_means_counted, (n + 127) / 128, 128, 0, d_pos + (n - 1), d_starts, t.idx_s, d_pts, times ? d_t : nullptr,
                        intensities ? d_i : nullptr, d_opts, d_ot, d_oi));
     GB_CUDA(cudaMemcpyAsync(out_xyzw, d_opts, sizeof(double4) * (size_t)V, cudaMemcpyDeviceToHost, st));
@@ -598,7 +614,7 @@ static gb_status knn_device(gb_ctx* ctx, int n, const int* d_count, const double
   });
 }
 
-gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out, gb_cloud* cloud_out) {
+static gb_status preprocess(gb_ctx* ctx, size_t n_, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out, gb_cloud* cloud_out) {
   const int n = (int)n_;
   cudaStream_t st = ctx->stream;
   const int k = P->k_correspondences;
@@ -742,8 +758,45 @@ gb_status gb_preprocess_impl(gb_ctx* ctx, size_t n_, const double* xyzw, const d
   return GB_OK;
 }
 
+extern "C" gb_status gb_preprocess_default_params(gb_preprocess_params* p) {
+  GB_REQUIRE(p, "null params");
+  memset(p, 0, sizeof(*p));
+  p->distance_near_thresh = 0.5;      // config_preprocess.json:20
+  p->distance_far_thresh = 100.0;     // :21
+  p->use_random_grid_downsampling = 1;  // :22
+  p->downsample_resolution = 1.0;     // :23
+  p->downsample_target = 10000;       // :24
+  p->downsample_rate = 0.1;           // :25
+  p->seed = 0;
+  p->outlier_removal_k = 10;          // :27
+  p->outlier_std_mul_factor = 1.0;    // :28
+  p->k_correspondences = 10;          // :33
+  p->estimate_covariances = 1;
+  for (int i = 0; i < 4; i++) p->T_imu_lidar[i * 5] = 1.0;
+  return GB_OK;
+}
+extern "C" gb_status gb_preprocess(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, const gb_preprocess_params* P, gb_preprocessed* out) {
+  GB_REQUIRE(ctx && P && out, "null argument");
+  out->num_points = 0; out->last_time = 0.0; out->cloud = nullptr;
+  GB_REQUIRE(n < (size_t)1 << 30, "too many points");
+  GB_REQUIRE(gb_knn_instantiated(P->k_correspondences), "k_correspondences is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
+  GB_REQUIRE(P->k_neighbors_cov >= 0 && P->k_neighbors_cov <= P->k_correspondences, "k_neighbors_cov must be in [0, k_correspondences]");
+  GB_REQUIRE(!P->enable_outlier_removal || gb_knn_instantiated(P->outlier_removal_k), "outlier_removal_k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
+  GB_REQUIRE(P->crop_bbox_frame >= 0 && P->crop_bbox_frame <= 2, "crop_bbox_frame must be 0 (off), 1 (lidar) or 2 (imu)");
+  if (n == 0) return GB_OK;
+  GB_REQUIRE(xyzw, "null points");
+  GB_ENTER(ctx);
+  gb_owned<gb_cloud> c(P->estimate_covariances ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
+  if (P->estimate_covariances && !c) return GB_ERR_INTERNAL;
+  if (c) c->device = ctx->device;
+  GB_CHECK(preprocess(ctx, n, xyzw, times, intensities, P, out, c.get()));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));  // the cloud is complete when the call returns (it may be used from another context)
+  out->cloud = c.release();
+  return GB_OK;
+}
+
 // gb_find_neighbors on the pyramid (host arrays in / out; the device-resident entry is inside gb_preprocess)
-gb_status gb_find_neighbors_pyramid_impl(gb_ctx* ctx, size_t n_, const double* xyzw, int k, int32_t* neighbors) {
+static gb_status find_neighbors_pyramid(gb_ctx* ctx, size_t n_, const double* xyzw, int k, int32_t* neighbors) {
   const int n = (int)n_;
   cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n, cub_b = gb_cub_temp_bytes(N);
@@ -762,6 +815,20 @@ gb_status gb_find_neighbors_pyramid_impl(gb_ctx* ctx, size_t n_, const double* x
   GB_CUDA(cudaMemcpyAsync(neighbors, d_nb, sizeof(int) * N * (size_t)k, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
   return GB_OK;
+}
+
+extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors) {
+  GB_REQUIRE(ctx, "null ctx");
+  if (n == 0) return GB_OK;
+  GB_REQUIRE(xyzw && neighbors && k > 0, "null argument");
+  GB_REQUIRE(gb_knn_instantiated(k), "k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
+  GB_ENTER(ctx);
+  // >= 4096 points: exact search on a pyramid of hash grids (one Morton sort, cell size 0.25 m x 4^level); fewer: the tiled
+  // brute force.  GB_KNN=pyramid / brute forces one.
+  const char* mode = getenv("GB_KNN");
+  const bool pyramid = mode ? (strcmp(mode, "pyramid") == 0) : (n >= 4096);
+  if (pyramid) return find_neighbors_pyramid(ctx, n, xyzw, k, neighbors);
+  return find_neighbors_brute(ctx, n, xyzw, k, neighbors);
 }
 
 // =============================================================================================
@@ -862,7 +929,7 @@ gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T, vo
   return gb_launch(ctx, "k_merge_transform", k_merge_transform, (n + 255) / 256, 256, 0, 1, (const MergeFrame*)d_frame, n, pts, cov6);
 }
 
-gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out) {
+static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out) {
   cudaStream_t st = ctx->stream;
   size_t total = 0;
   std::vector<MergeFrame> mf((size_t)K);
@@ -925,5 +992,28 @@ gb_status gb_merge_frames_impl(gb_ctx* ctx, int K, const gb_cloud* const* frames
   if (out_xyzw) GB_CUDA(cudaMemcpyAsync(out_xyzw, d_pts, sizeof(double4) * (size_t)M, cudaMemcpyDeviceToHost, st));
   if (out_cov4x4) GB_CUDA(cudaMemcpyAsync(out_cov4x4, d_ocov, sizeof(double) * 16 * (size_t)M, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
+  return GB_OK;
+}
+
+extern "C" gb_status gb_merge_frames(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, double resolution, int target, uint64_t seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud** out_cloud) {
+  GB_REQUIRE(ctx && num_out, "null argument");
+  *num_out = 0;
+  if (out_cloud) *out_cloud = nullptr;
+  if (K == 0) return GB_OK;
+  GB_REQUIRE(frames && poses, "null frames / poses");
+  GB_REQUIRE(resolution > 0.0, "downsample_resolution must be positive");
+  size_t total = 0;
+  for (size_t k = 0; k < K; k++) {
+    GB_REQUIRE(frames[k] && frames[k]->device == ctx->device, "null frame / frame on another device");
+    total += frames[k]->n;
+  }
+  GB_REQUIRE(total < (size_t)1 << 30 && K < 65536, "too many points / frames");
+  GB_ENTER(ctx);
+  gb_owned<gb_cloud> c(out_cloud ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
+  if (out_cloud && !c) return GB_ERR_INTERNAL;
+  if (c) c->device = ctx->device;
+  GB_CHECK(merge_frames(ctx, (int)K, frames, poses, resolution, target, seed, out_xyzw, out_cov4x4, num_out, c.get()));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (out_cloud) *out_cloud = c.release();
   return GB_OK;
 }

@@ -32,9 +32,6 @@
 #include "gb_internal.cuh"
 #include "gb_vgicp_math.cuh"  // PoseF, transform, fused_mahalanobis, accumulate_hit, surface_ok, slab_to_record (also compiled for the host by the CPU test)
 
-#include <stdlib.h>
-#include <string.h>
-
 #include "gb_sweep_steps.cuh"  // the steps every sweep kernel runs (shared with k_gicp_sweep, gb_kernels_gicp.cu)
 
 namespace {
@@ -326,25 +323,6 @@ static gb_status launch3(gb_sweep* s, const double* poses_eval, float* slab, con
                    s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
 }
 
-// completion flags of the fused exchange: one thread per rank publishes this rank's step to that peer, then waits for the
-// peer's flag.  The preceding sweep kernel has completed (stream order), so all its peer stores have been performed.
-struct PeerFlags { unsigned* flags[GB_MAX_PEERS]; };
-__global__ void k_peer_signal_wait(PeerFlags pf, int world, int rank, unsigned step, int* timeout) {
-  const int t = threadIdx.x;
-  if (t >= world) return;
-  __threadfence_system();
-  volatile unsigned* remote = pf.flags[t] + rank;
-  *remote = step;
-  __threadfence_system();
-  volatile unsigned* mine = pf.flags[rank] + t;
-  const long long t0 = clock64();
-  while ((int)(*mine - step) < 0) {
-    __nanosleep(200);
-    if (clock64() - t0 > 4000000000ll) { *timeout = 1; break; }  // ~2 s: a peer died; do not hold the GPU
-  }
-  __threadfence_system();
-}
-
 gb_status gb_launch_sweep(gb_sweep* s, int mode) {
   if (s->num_tiles == 0) return GB_OK;
   if (s->gicp) return gb_launch_gicp_sweep(s, mode);  // gb_kernels_gicp.cu
@@ -372,86 +350,6 @@ gb_status gb_launch_sweep(gb_sweep* s, int mode) {
   const unsigned long long warps = (unsigned long long)s->grid * kWarps;
   if ((unsigned long long)s->num_tiles > warps) s->ctr_base += (s->kernel_version == 3 ? 0ull : warps) + (unsigned long long)s->num_tiles;
   return GB_OK;
-}
-
-// Deferred exchange: the four CTAs of peer p copy this rank's finished rows (written by the sweep into the local buffer of the step
-// parity) into peer p's buffer -- 128-bit stores through the IPC mapping, ~164 KB per peer at 8 ranks -- then publishes this
-// rank's step to that peer and waits for the peer's flag.  The CTAs are independent (one per peer): no ordering between them.
-// Why not from the sweep's epilogue (GB_PEER_PUSH=fused, the round-1 design): stores to peer memory issued from all the busy
-// SMs slow the sweep down at 8 ranks (against the same shard without the peer stores) while the whole exchange is ~1 MB per rank
-// and step.
-struct PeerExchange {
-  float* dst[GB_MAX_PEERS];   // every rank's buffer of the step parity, as mapped here
-  unsigned* flags[GB_MAX_PEERS];
-  const float* src;           // this rank's buffer of the step parity
-  const int* my_pairs;
-  int num_my_pairs;
-  unsigned* arrivals;         // [world] CTA arrival counters (self-cleaning)
-};
-constexpr int kExchangeCtasPerPeer = 4;
-constexpr int kExchangeThreads = 512;
-__global__ void __launch_bounds__(kExchangeThreads) k_peer_exchange(PeerExchange px, int world, int rank, unsigned step, int* timeout) {
-  const int p = blockIdx.x / kExchangeCtasPerPeer, c = blockIdx.x % kExchangeCtasPerPeer;
-  if (p != rank) {
-    float4* __restrict__ dst = reinterpret_cast<float4*>(px.dst[p]);
-    const float4* __restrict__ src = reinterpret_cast<const float4*>(px.src);
-    constexpr int kVec = GB_SLAB_STRIDE / 4;
-    const int total = px.num_my_pairs * kVec;
-    const int stride = kExchangeCtasPerPeer * kExchangeThreads;
-    // four independent 16-byte loads in flight per thread: the copy is latency-, not bandwidth-bound (~1 MB per rank and step)
-    for (int e0 = c * kExchangeThreads + threadIdx.x; e0 < total; e0 += 4 * stride) {
-      float4 v[4];
-      size_t at[4];
-#pragma unroll
-      for (int u = 0; u < 4; u++) {
-        const int e = min(e0 + u * stride, total - 1);
-        at[u] = (size_t)px.my_pairs[e / kVec] * kVec + (size_t)(e % kVec);
-        v[u] = __ldcg(&src[at[u]]);
-      }
-#pragma unroll
-      for (int u = 0; u < 4; u++)
-        if (e0 + u * stride < total) dst[at[u]] = v[u];
-    }
-  }
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x != 0) return;
-  // the last of this peer's CTAs publishes the flag and waits for the peer's
-  const unsigned arrived = atomicAdd(&px.arrivals[p], 1u);
-  if (arrived != (unsigned)kExchangeCtasPerPeer - 1u) return;
-  px.arrivals[p] = 0u;
-  __threadfence_system();
-  volatile unsigned* remote = px.flags[p] + rank;
-  *remote = step;
-  volatile unsigned* mine = px.flags[rank] + p;
-  const long long t0 = clock64();
-  while ((int)(*mine - step) < 0) {
-    __nanosleep(100);
-    if (clock64() - t0 > 4000000000ll) { *timeout = 1; break; }  // ~2 s: a peer died; do not hold the GPU
-  }
-  __threadfence_system();
-}
-
-gb_status gb_launch_peer_signal_wait(gb_peer_slab* ps) {
-  const gb_peer_regions mine = gb_peer_regions_of(ps, ps->rank);
-  if (ps->deferred) {
-    PeerExchange px;
-    memset(&px, 0, sizeof(px));
-    for (int p = 0; p < ps->world; p++) {
-      const gb_peer_regions r = gb_peer_regions_of(ps, p);
-      px.dst[p] = r.buf[ps->parity];
-      px.flags[p] = r.flags;
-    }
-    px.src = mine.buf[ps->parity];
-    px.my_pairs = ps->d_my_pairs;
-    px.num_my_pairs = ps->num_my_pairs;
-    px.arrivals = mine.arrivals;
-    return gb_launch(ps->ctx, "k_peer_exchange", k_peer_exchange, ps->world * kExchangeCtasPerPeer, kExchangeThreads, 0, px, ps->world, ps->rank, ps->step, mine.timeout);
-  }
-  PeerFlags pf;
-  memset(&pf, 0, sizeof(pf));
-  for (int p = 0; p < ps->world; p++) pf.flags[p] = gb_peer_regions_of(ps, p).flags;
-  return gb_launch(ps->ctx, "k_peer_signal_wait", k_peer_signal_wait, 1, 32, 0, pf, ps->world, ps->rank, ps->step, mine.timeout);
 }
 
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count) {

@@ -22,11 +22,15 @@
 //                        dropped points > drop_rate * N
 // Steps 2-3 (+ k_voxel_starts) are gb_group_by_key / gb_group_starts, shared with the voxel-grid downsampling and the frame
 // merge of gb_kernels_preprocess.cu.  Step 6 (table_build) also serves the incremental maps and iVoxes, whose one insert
-// pipeline is described below.  This file also builds every device cloud (gb_cloud_build: Morton reorder of staged
-// planes), for gb_cloud_upload, gb_preprocess and gb_merge_frames.
+// pipeline is described below.  The map entry points (gb_voxelmap_*, gb_ivox_*) are defined here too.  This file also builds
+// every device cloud (gb_cloud_build: Morton reorder of staged planes), for gb_cloud_upload, gb_preprocess and gb_merge_frames.
 #include "gb_internal.cuh"
 
 #include <cub/cub.cuh>
+
+#include <cmath>
+#include <new>
+#include <vector>
 
 namespace {
 
@@ -173,13 +177,28 @@ static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dr
   return GB_OK;
 }
 
-gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_buckets, int max_scan, double drop_rate, gb_voxelmap* m) {
+// (the caller has made the map's device current)
+static void voxelmap_free(gb_voxelmap* m) {
+  gb_dev_free(m->device, m->base);
+  gb_dev_free(m->device, m->buckets);
+  delete m;
+}
+
+extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float resolution, int init_num_buckets, int max_bucket_scan_count, double target_points_drop_rate, gb_voxelmap** out) {
+  GB_REQUIRE(ctx && cloud && out, "null argument");
+  GB_REQUIRE(resolution > 0.f, "resolution must be positive");
+  GB_REQUIRE(init_num_buckets > 0 && (init_num_buckets & (init_num_buckets - 1)) == 0, "init_num_buckets must be a power of two");
+  GB_REQUIRE(max_bucket_scan_count > 0, "max_bucket_scan_count must be positive");
+  *out = nullptr;
+  GB_ENTER(ctx);
+  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(), voxelmap_free);
+  if (!m) return GB_ERR_INTERNAL;
   const int n = (int)cloud->n;
   cudaStream_t st = ctx->stream;
   m->device = ctx->device;
   m->resolution = resolution;
   m->inv_res = 1.0f / resolution;
-  m->max_scan = max_scan;
+  m->max_scan = max_bucket_scan_count;
 
   int V = 0;
   int4* d_vcoord = nullptr;
@@ -209,8 +228,10 @@ gb_status gb_voxelmap_build_impl(gb_ctx* ctx, const gb_cloud* cloud, float resol
   }
   m->num_voxels = V;
   m->bytes = sizeof(float4) * 3 * (size_t)V;
-  GB_CHECK(table_build(ctx, V, d_vcoord, d_dropped, init_buckets, max_scan, drop_rate, (double)n, &m->buckets, &m->num_buckets, &m->num_dropped_points));
+  GB_CHECK(table_build(ctx, V, d_vcoord, d_dropped, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, (double)n, &m->buckets, &m->num_buckets,
+                       &m->num_dropped_points));
   m->bytes += sizeof(int4) * (size_t)m->num_buckets;
+  *out = m.release();
   return GB_OK;
 }
 
@@ -594,17 +615,154 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
 
 }  // namespace
 
-gb_status gb_map_create_empty_impl(gb_ctx* ctx, gb_voxelmap* m) {
+// an empty incremental map or iVox of the parameters in `init` (the caller has entered ctx)
+static gb_status map_create_empty(gb_ctx* ctx, const gb_voxelmap& init, gb_voxelmap** out) {
+  gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(init), voxelmap_free);
+  if (!m) return GB_ERR_INTERNAL;
   m->device = ctx->device;
   GB_CHECK(table_build(ctx, 0, nullptr, nullptr, m->init_buckets, m->max_scan, m->drop_rate, 0.0, &m->buckets, &m->num_buckets, &m->num_dropped_points));
   m->bytes = sizeof(int4) * (size_t)m->num_buckets;
+  *out = m.release();
+  return GB_OK;
+}
+// The checks both inserts make before any launch, the handles read last; *T is the pose to insert at.
+static gb_status insert_args(gb_ctx* ctx, const gb_voxelmap* m, gb_map_kind kind, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, const double** T) {
+  GB_REQUIRE(ctx && m && cloud, "null argument");
+  GB_REQUIRE(sampling_rate > 0.0 && sampling_rate <= 1.0, "sampling_rate must be in (0, 1]");
+  static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  *T = T_map_cloud ? T_map_cloud : kIdentity;
+  for (int k = 0; k < 16; k++) GB_REQUIRE(std::isfinite((*T)[k]), "T_map_cloud must be finite");
+  GB_REQUIRE(m->kind == kind, kind == GB_MAP_IVOX ? "the map is not an iVox: create it with gb_ivox_create"
+                                                  : "the map is not incremental: create it with gb_voxelmap_create_incremental");
+  GB_REQUIRE(m->device == ctx->device && cloud->device == ctx->device, "cloud / map live on another device");
+  GB_REQUIRE((uint64_t)gb_stored_entries(m) + (uint64_t)cloud->n < (1ull << 31) - 1, "stored entries + cloud points exceed 2^31");
+  return GB_OK;
+}
+// 48-byte records (a voxel's or a stored point's) to the host; any output may be null.  A plain copy, its direction taken
+// from the unified address space: the map may live on another device than the current one, and every producer call
+// returned after its stream had drained.
+static gb_status download_records(const float4* records, size_t count, int32_t* num_points, float* xyz, float* cov6) {
+  if (count == 0 || !(num_points || xyz || cov6)) return GB_OK;
+  std::vector<float4> h(3 * count);
+  GB_CUDA(cudaMemcpy(h.data(), records, sizeof(float4) * h.size(), cudaMemcpyDefault));
+  for (size_t r = 0; r < count; r++) {
+    const float4 a = h[3 * r], b = h[3 * r + 1], c = h[3 * r + 2];
+    if (num_points) num_points[r] = (int32_t)c.y;
+    if (xyz) { xyz[3 * r] = a.x; xyz[3 * r + 1] = a.y; xyz[3 * r + 2] = a.z; }
+    if (cov6) { cov6[6 * r] = a.w; cov6[6 * r + 1] = b.x; cov6[6 * r + 2] = b.y; cov6[6 * r + 3] = b.z; cov6[6 * r + 4] = b.w; cov6[6 * r + 5] = c.x; }
+  }
   return GB_OK;
 }
 
-gb_status gb_map_insert_impl(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T, double sampling_rate, unsigned long long seed) {
-  if (m->kind == GB_MAP_IVOX) return map_insert(ctx, m, cloud, T, sampling_rate, seed, IvoxRule{m});
-  return map_insert(ctx, m, cloud, T, sampling_rate, seed, VoxelRule{m});
+extern "C" gb_status gb_voxelmap_create_incremental(gb_ctx* ctx, float resolution, int init_num_buckets, int max_bucket_scan_count, double target_points_drop_rate,
+                                                    int lru_horizon, int lru_clear_cycle, gb_voxelmap** out) {
+  GB_REQUIRE(ctx && out, "null argument");
+  GB_REQUIRE(resolution > 0.f && std::isfinite(resolution), "resolution must be positive and finite");
+  GB_REQUIRE(init_num_buckets > 0 && (init_num_buckets & (init_num_buckets - 1)) == 0, "init_num_buckets must be a power of two");
+  GB_REQUIRE(max_bucket_scan_count > 0, "max_bucket_scan_count must be positive");
+  GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
+  *out = nullptr;
+  GB_ENTER(ctx);
+  gb_voxelmap m;
+  m.kind = GB_MAP_INCREMENTAL;
+  m.resolution = resolution;
+  m.inv_res = 1.0f / resolution;
+  m.key_inv_res = 1.0 / (double)resolution;
+  m.max_scan = max_bucket_scan_count;
+  m.init_buckets = init_num_buckets;
+  m.drop_rate = target_points_drop_rate;
+  m.lru_horizon = lru_horizon;
+  m.lru_clear_cycle = lru_clear_cycle;
+  return map_create_empty(ctx, m, out);
 }
+extern "C" gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
+  const double* T;
+  GB_CHECK(insert_args(ctx, map, GB_MAP_INCREMENTAL, cloud, T_map_cloud, sampling_rate, &T));
+  GB_ENTER(ctx);
+  return map_insert(ctx, map, cloud, T, sampling_rate, (unsigned long long)seed, VoxelRule{map});
+}
+extern "C" gb_status gb_voxelmap_info(const gb_voxelmap* m, int* num_voxels, int* num_buckets, float* resolution) {
+  GB_REQUIRE(m, "null map");
+  if (num_voxels) *num_voxels = m->num_voxels;
+  if (num_buckets) *num_buckets = m->num_buckets;
+  if (resolution) *resolution = m->resolution;
+  return GB_OK;
+}
+extern "C" gb_status gb_voxelmap_download(const gb_voxelmap* m, int32_t* buckets, int32_t* num_points, float* means, float* cov6) {
+  GB_REQUIRE(m, "null map");
+  GB_REQUIRE(m->kind != GB_MAP_IVOX, "an iVox holds points, not voxels: use gb_ivox_download");
+  if (buckets) GB_CUDA(cudaMemcpy(buckets, m->buckets, sizeof(int4) * (size_t)m->num_buckets, cudaMemcpyDefault));
+  return download_records(m->voxels, (size_t)m->num_voxels, num_points, means, cov6);
+}
+extern "C" gb_status gb_voxelmap_destroy(gb_voxelmap* m) {
+  if (!m) return GB_OK;
+  cudaSetDevice(m->device);
+  voxelmap_free(m);
+  return GB_OK;
+}
+
+// iVox: a gb_voxelmap of kind GB_MAP_IVOX (gb_internal.cuh); voxelmap_free and gb_voxelmap_destroy release it
+extern "C" gb_status gb_ivox_create(gb_ctx* ctx, double resolution, double min_dist_in_cell, int max_points_in_cell, int neighbor_voxel_mode, int lru_horizon,
+                                    int lru_clear_cycle, gb_ivox** out) {
+  GB_REQUIRE(ctx && out, "null argument");
+  GB_REQUIRE(std::isfinite(resolution) && resolution > 0.0, "resolution must be positive and finite");
+  GB_REQUIRE(min_dist_in_cell >= 0.0, "min_dist_in_cell must be >= 0");
+  GB_REQUIRE(max_points_in_cell >= 1 && max_points_in_cell <= 64, "max_points_in_cell must be in [1, 64]");
+  GB_REQUIRE(neighbor_voxel_mode == 1 || neighbor_voxel_mode == 7 || neighbor_voxel_mode == 19 || neighbor_voxel_mode == 27, "neighbor_voxel_mode must be 1, 7, 19 or 27");
+  GB_REQUIRE(lru_clear_cycle >= 1, "lru_clear_cycle must be at least 1");
+  *out = nullptr;
+  GB_ENTER(ctx);
+  gb_voxelmap m;
+  m.kind = GB_MAP_IVOX;
+  m.ivox_resolution = resolution;
+  m.min_dist = min_dist_in_cell;
+  m.max_points = max_points_in_cell;
+  m.mode = neighbor_voxel_mode;
+  m.resolution = (float)resolution;
+  m.inv_res = (float)(1.0 / resolution);
+  m.key_inv_res = 1.0 / resolution;
+  m.max_scan = 10;          // the build's table (16384 buckets doubled until >= 8 V, 10 probes) with drop rate 0
+  m.init_buckets = 16384;
+  m.lru_horizon = lru_horizon;
+  m.lru_clear_cycle = lru_clear_cycle;
+  gb_voxelmap* h = nullptr;
+  GB_CHECK(map_create_empty(ctx, m, &h));
+  *out = reinterpret_cast<gb_ivox*>(h);
+  return GB_OK;
+}
+extern "C" gb_status gb_ivox_insert(gb_ctx* ctx, gb_ivox* map, const gb_cloud* cloud, const double* T_map_cloud, double sampling_rate, uint64_t seed) {
+  gb_voxelmap* m = ivox_map(map);
+  const double* T;
+  GB_CHECK(insert_args(ctx, m, GB_MAP_IVOX, cloud, T_map_cloud, sampling_rate, &T));
+  GB_ENTER(ctx);
+  return map_insert(ctx, m, cloud, T, sampling_rate, (unsigned long long)seed, IvoxRule{m});
+}
+extern "C" gb_status gb_ivox_info(const gb_ivox* map, int* num_voxels, size_t* num_points, double* resolution) {
+  const gb_voxelmap* m = ivox_map(map);
+  GB_REQUIRE(m && m->kind == GB_MAP_IVOX, "null map, or not an iVox");
+  if (num_voxels) *num_voxels = m->num_voxels;
+  if (num_points) *num_points = m->num_points;
+  if (resolution) *resolution = m->ivox_resolution;
+  return GB_OK;
+}
+extern "C" gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords, int32_t* voxel_counts, float* xyz, float* cov6) {
+  const gb_voxelmap* m = ivox_map(map);
+  GB_REQUIRE(m && m->kind == GB_MAP_IVOX, "null map, or not an iVox");
+  const size_t V = (size_t)m->num_voxels;
+  if (V > 0 && (voxel_coords || voxel_counts)) {
+    std::vector<unsigned long long> keys(V);
+    std::vector<int2> cells(V);
+    GB_CUDA(cudaMemcpy(keys.data(), m->vkeys, sizeof(unsigned long long) * V, cudaMemcpyDefault));
+    GB_CUDA(cudaMemcpy(cells.data(), m->cells, sizeof(int2) * V, cudaMemcpyDefault));
+    for (size_t v = 0; v < V; v++) {
+      if (voxel_coords)
+        for (int a = 0; a < 3; a++) voxel_coords[3 * v + a] = (int32_t)((keys[v] >> (42 - 21 * a)) & 0x1FFFFF) - (1 << 20);
+      if (voxel_counts) voxel_counts[v] = cells[v].y;
+    }
+  }
+  return download_records(m->voxels, m->num_points, nullptr, xyz, cov6);
+}
+extern "C" gb_status gb_ivox_destroy(gb_ivox* map) { return gb_voxelmap_destroy(ivox_map(map)); }
 
 // ---------------------------------------------------------------------------------------------
 // Morton reordering of a new cloud (PointCloudGPU::clone keeps the caller's order on the host side of the
