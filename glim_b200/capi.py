@@ -29,6 +29,8 @@ SYMBOLS = [
     "gb_deskew_pose_table", "gb_deskew",
     "gb_align_default_params", "gb_vgicp_align",
     "gb_ivox_create", "gb_ivox_insert", "gb_ivox_info", "gb_ivox_download", "gb_ivox_destroy", "gb_gicp_factor_create",
+    "gb_cloud_add_times", "gb_cloud_time_table", "gb_ct_gicp_factor_create", "gb_ct_gicp_linearize", "gb_ct_gicp_error",
+    "gb_ct_default_params", "gb_ct_gicp_align", "gb_ct_deskew",
 ]
 
 GB_SLAB_STRIDE = 96
@@ -63,6 +65,17 @@ class AlignParams(C.Structure):
 class AlignResult(C.Structure):
     """gb_align_result (include/glim_b200.h)."""
     _fields_ = [("T_target_source", C.c_double * 16), ("error", C.c_double), ("num_inliers", C.c_double), ("lambda_", C.c_double),
+                ("iterations", C.c_int), ("trials", C.c_int), ("status", C.c_int)]
+
+
+class CtParams(C.Structure):
+    """gb_ct_params (include/glim_b200.h)."""
+    _fields_ = [("lm", AlignParams), ("location_consistency_inf_scale", C.c_double), ("constant_velocity_inf_scale", C.c_double)]
+
+
+class CtResult(C.Structure):
+    """gb_ct_result (include/glim_b200.h)."""
+    _fields_ = [("X", C.c_double * 16), ("Y", C.c_double * 16), ("error", C.c_double), ("num_inliers", C.c_double), ("lambda_", C.c_double),
                 ("iterations", C.c_int), ("trials", C.c_int), ("status", C.c_int)]
 
 
@@ -149,6 +162,14 @@ def lib():
     L.gb_ivox_download.argtypes = [vp, vp, vp, vp, vp]
     L.gb_ivox_destroy.argtypes = [vp]
     L.gb_gicp_factor_create.argtypes = [vp, vp, vp, f64, vp]
+    L.gb_cloud_add_times.argtypes = [vp, vp, sz, vp]
+    L.gb_cloud_time_table.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.gb_ct_gicp_factor_create.argtypes = [vp, vp, vp, f64, vp]
+    L.gb_ct_gicp_linearize.argtypes = [vp, vp, vp, vp]
+    L.gb_ct_gicp_error.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.gb_ct_default_params.argtypes = [vp]
+    L.gb_ct_gicp_align.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp]
+    L.gb_ct_deskew.argtypes = [vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]
     for name in SYMBOLS:
         getattr(L, name)  # AttributeError here means the library and include/glim_b200.h are out of sync
     _lib = L

@@ -84,6 +84,13 @@ gb_status validate(size_t P, const size_t* off, gb_factor* const* factors, const
   GB_REQUIRE(factors, "null factor list");
   for (size_t f = 0; f < off[P]; f++) GB_REQUIRE(factors[f], "null factor");
   for (size_t k = 0; k < 16 * P; k++) GB_REQUIRE(isfinite(T_init[k]), "T_init must be finite");
+  return gb_align_params_check(prm);
+}
+
+}  // namespace
+
+gb_status gb_align_params_check(const gb_align_params* prm) {
+  GB_REQUIRE(prm, "null params");
   GB_REQUIRE(prm->max_iterations >= 1, "max_iterations must be >= 1");
   GB_REQUIRE(prm->lambda_factor > 1.0 && isfinite(prm->lambda_factor), "lambda_factor must be a finite number > 1");
   GB_REQUIRE(prm->lambda_initial > 0.0 && isfinite(prm->lambda_initial), "lambda_initial must be a finite number > 0");
@@ -94,8 +101,6 @@ gb_status validate(size_t P, const size_t* off, gb_factor* const* factors, const
   GB_REQUIRE(!isnan(prm->relative_error_tol) && !isnan(prm->absolute_error_tol) && !isnan(prm->step_translation_tol) && !isnan(prm->step_rotation_tol), "NaN tolerance");
   return GB_OK;
 }
-
-}  // namespace
 
 extern "C" gb_status gb_align_default_params(gb_align_params* p) {
   GB_REQUIRE(p, "null params");

@@ -219,6 +219,7 @@ gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes) {
 // (the caller has made the cloud's device current)
 void cloud_free(gb_cloud* c) {
   gb_dev_free(c->device, c->base);  // waits for every stream that may still read the cloud, then recycles the block
+  gb_dev_free(c->device, c->t_base);
   delete c;
 }
 
@@ -610,6 +611,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   uint64_t total_pts = 0;
   for (size_t f = 0; f < F; f++) {
     GB_REQUIRE(factors[f], "null factor");
+    GB_REQUIRE(factors[f]->kind != GB_FACTOR_CT, "a CT factor has two poses: only the gb_ct_* entry points take it");
     GB_REQUIRE(factors[f]->source->device == ctx->device && factors[f]->target->device == ctx->device, "factor lives on another device");
     GB_REQUIRE((factors[f]->target->kind == GB_MAP_IVOX) == (factors[0]->target->kind == GB_MAP_IVOX), "the factors of one sweep must all be VGICP or all GICP factors");
     total_pts += factors[f]->source->n;

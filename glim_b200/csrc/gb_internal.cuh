@@ -57,6 +57,16 @@ struct gb_cloud {
   int* inv_perm = nullptr;
   void* base = nullptr;       // one allocation
   size_t bytes = 0;
+  // The time table of gb_cloud_add_times (gb_kernels_ct.cu), or none (num_entries == 0).  Entry b holds the original indices
+  // [t_starts[b], t_starts[b + 1]) at normalized time t_tau[b]; the stored slots are reached through inv_perm.  The device
+  // copy is one block of its own (ct_table_layout), from the device pool; only the CT factor reads it.
+  int num_entries = 0;
+  double t_first = 0.0, t_last = 0.0;  // t_0 and t_{B-1}
+  std::vector<int> h_starts;           // host copies
+  std::vector<double> h_tau;
+  int* t_starts = nullptr;
+  double* t_tau = nullptr;
+  void* t_base = nullptr;
 };
 
 // A map is one of three kinds, fixed at creation.  Every entry point that takes a map checks the kind it accepts.
@@ -128,7 +138,15 @@ struct GicpDesc {
 };
 static_assert(sizeof(GicpDesc) == 16, "GicpDesc size");
 
+// A factor is one of two kinds, fixed at creation.  A pose factor (gb_vgicp_factor_create, gb_gicp_factor_create) has one
+// unknown pose and goes through sweeps; a CT factor (gb_ct_gicp_factor_create) has two and only the gb_ct_* entry points
+// take it: gb_sweep_create refuses it, and so every consumer of sweeps.
+enum gb_factor_kind {
+  GB_FACTOR_POSE,
+  GB_FACTOR_CT,
+};
 struct gb_factor {
+  gb_factor_kind kind = GB_FACTOR_POSE;
   gb_ctx* ctx = nullptr;
   const gb_voxelmap* target = nullptr;  // a built or incremental map (VGICP), or an iVox (GICP: target->kind == GB_MAP_IVOX)
   float max_corr2 = 0.f;                // GICP: (float)(max_correspondence_distance^2)
@@ -288,6 +306,8 @@ gb_status gb_launch(gb_ctx* ctx, const char* name, void (*kernel)(P...), dim3 gr
 cudaError_t gb_dev_malloc(int device, size_t bytes, void** out);
 void gb_dev_free(int device, void* p);
 gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes);  // a.base holds at least `bytes` afterwards
+// the parameter bounds of gb_vgicp_align (gb_align.cu), shared by gb_ct_gicp_align
+gb_status gb_align_params_check(const gb_align_params* prm);
 
 // The one free function of each handle that owns memory (cloud_free, voxelmap_free, sweep_free, peer_slab_free,
 // ctx_release): it releases everything the handle owns, never returns early, and ends with the delete.  A creation holds
@@ -395,6 +415,12 @@ inline gb_planes gb_cloud_planes(Carver& cv, size_t n, bool normals) {
   return p;
 }
 gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n, const gb_planes& staged, const gb_sort_tmp& t);
+// The covariance stage of gb_preprocess (gb_kernels_preprocess.cu), shared with gb_ct_deskew: plane_covariance of the first
+// *d_count of M points (pts, neighbors[i * kc + j], the first k of each row) into the fp64 normals (M x double4) and covs
+// (M x 16, column-major), and the fp32 planes staged for the cloud; then, when cloud_out is given, the cloud (gb_cloud_build
+// with t).  One launch plus the build's.
+gb_status gb_covariance_cloud(gb_ctx* ctx, int M, const int* d_count, const double4* pts, const int* neighbors, int kc, int k, double4* normals, double* covs,
+                              const gb_planes& staged, const gb_sort_tmp& t, gb_cloud* cloud_out);
 
 // kernel launchers (gb_kernels_*.cu)
 enum { GB_MODE_LINEARIZE = 0, GB_MODE_ERROR = 1 };

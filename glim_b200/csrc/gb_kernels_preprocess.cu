@@ -582,6 +582,14 @@ __global__ void k_sor_compact(int n_upper, const int* __restrict__ keep, const i
 
 }  // namespace
 
+gb_status gb_covariance_cloud(gb_ctx* ctx, int M, const int* d_count, const double4* pts, const int* neighbors, int kc, int k, double4* normals, double* covs,
+                              const gb_planes& staged, const gb_sort_tmp& t, gb_cloud* cloud_out) {
+  GB_CHECK(gb_launch(ctx, "k_covariances_planes", k_covariances_planes, (M + 127) / 128, 128, 0, M, d_count, pts, neighbors, kc, k, normals, covs, staged.p0, staged.p1, staged.p2,
+                     staged.normals));
+  if (cloud_out) GB_CHECK(gb_cloud_build(ctx, cloud_out, (size_t)M, staged, t));
+  return GB_OK;
+}
+
 // Temporaries of knn_device for up to n points.  The outlier removal's k-NN and the frame's k-NN run one after the other
 // on the same stream and share them.
 struct KnnTmp {
@@ -728,11 +736,8 @@ static gb_status preprocess(gb_ctx* ctx, size_t n_, const double* xyzw, const do
   GB_CUDA(cudaStreamSynchronize(st));
   out->num_points = (size_t)M;
   // ---- covariances, written straight into the staged fp32 planes of the cloud (PointCloudGPU::clone on the device) ----
-  if (P->estimate_covariances && M > 0) {
-    GB_CHECK(gb_launch(ctx, "k_covariances_planes", k_covariances_planes, (M + 127) / 128, 128, 0, M, frame_cnt, d_fr, d_nb, k, P->k_neighbors_cov > 0 ? P->k_neighbors_cov : k, d_nrm, d_cov,
-                       staged.p0, staged.p1, staged.p2, staged.normals));
-    if (cloud_out) GB_CHECK(gb_cloud_build(ctx, cloud_out, (size_t)M, staged, t));  // the frame is gathered: t is free again
-  }
+  if (P->estimate_covariances && M > 0)  // the frame is gathered: t is free again
+    GB_CHECK(gb_covariance_cloud(ctx, M, frame_cnt, d_fr, d_nb, k, P->k_neighbors_cov > 0 ? P->k_neighbors_cov : k, d_nrm, d_cov, staged, t, cloud_out));
   // ---- host products: D2H into the context's pinned staging (full PCIe rate), then one memcpy each into the caller's arrays ----
   if (M > 0) {
     const size_t m = (size_t)M;

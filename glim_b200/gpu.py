@@ -13,6 +13,10 @@ include/glim_b200/gtsam_points_compat.hpp.
     IntegratedGICPFactorGPU(target, source_key, ivox, source, max_corr)   odometry_estimation_cpu.cpp:95-104
     align_vgicp(problems, T_init, params)                   the LM loop of odometry_estimation_cpu.cpp:105-150 /
                                                             global_mapping_pose_graph.cpp:405-417, many problems per call
+    PointCloudGPU.add_times(times)                          PointCloud::add_times, odometry_estimation_ct.cpp:101
+    IntegratedCT_GICPFactorGPU(key_X, key_Y, ivox, source, max_corr)   odometry_estimation_ct.cpp:159-163
+    align_ct_gicp(factors, X_init, Y_init, X_prior, params) the CT LM solve with its motion priors, odometry_estimation_ct.cpp:166-182
+    deskew_ct(cloud, X, Y, neighbors, k_neighbors)          deskewed_source_points + covariances, odometry_estimation_ct.cpp:199-204
 """
 from __future__ import annotations
 
@@ -101,6 +105,22 @@ class PointCloudGPU:
         cov6 = np.empty((self.n, 6), np.float32)
         check(lib().gb_cloud_download(self.h, ptr(xyz), ptr(cov6)))
         return xyz, cov6
+
+    def add_times(self, times):
+        """PointCloud::add_times (odometry_estimation_ct.cpp:101): the cloud's time table (gb_cloud_add_times); times (n,) in
+        the original point order, finite and non-decreasing."""
+        t = f64(times).reshape(-1)
+        check(lib().gb_cloud_add_times(self.ctx.h, self.h, t.shape[0], ptr(t)))
+        return self
+
+    def time_table(self):
+        """-> (starts (B+1,) int32, tau (B,) float64, t_first, t_last); B = 0 without times"""
+        B = C.c_int()
+        check(lib().gb_cloud_time_table(self.h, C.byref(B), None, None, None, None))
+        starts, tau = np.empty(B.value + 1, np.int32), np.empty(B.value, np.float64)
+        t0, t1 = C.c_double(), C.c_double()
+        check(lib().gb_cloud_time_table(self.h, None, ptr(starts), ptr(tau), C.byref(t0), C.byref(t1)))
+        return (starts if B.value else np.zeros(0, np.int32)), tau, t0.value, t1.value
 
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:
@@ -344,6 +364,111 @@ class IntegratedGICPFactorGPU(IntegratedVGICPFactorGPU):
             check(lib().gb_gicp_factor_create(self.ctx.h, self.ivox.h, self.source.h, self.max_correspondence_distance, C.byref(h)))
             self.h = h
         return self.h
+
+
+class IntegratedCT_GICPFactorGPU:
+    """IntegratedCT_GICPFactor_<iVox, PointCloud>(X, Y, ivox, frame, ivox) + max_correspondence_distance
+    (odometry_estimation_ct.cpp:159-163) on the device.  Its two keys are the poses at the scan's first and last time-table
+    entries; the source must carry times (PointCloudGPU.add_times).  linearize(values) returns the usual dict with X in the
+    target slot (H_tt = H_XX, b_t = b_X) and Y in the source slot (H_ss = H_YY, b_s = b_Y), H_ts = H_XY."""
+
+    def __init__(self, key_X, key_Y, ivox: IVoxGPU, source: PointCloudGPU, max_correspondence_distance: float, ctx: Context | None = None):
+        self.ctx = ctx or source.ctx
+        self.key_X, self.key_Y = key_X, key_Y
+        self.ivox, self.source = ivox, source  # keep alive
+        self.max_correspondence_distance = float(max_correspondence_distance)
+        self.h = None
+        self._lin_point = None
+        h = C.c_void_p()
+        check(lib().gb_ct_gicp_factor_create(self.ctx.h, ivox.h, source.h, self.max_correspondence_distance, C.byref(h)))
+        self.h = h
+
+    def keys(self):
+        return [self.key_X, self.key_Y]
+
+    def _handle(self):
+        return self.h
+
+    def poses(self, values):
+        return np.asarray(values[self.key_X], dtype=np.float64).reshape(4, 4), np.asarray(values[self.key_Y], dtype=np.float64).reshape(4, 4)
+
+    def linearize(self, values) -> dict:
+        X, Y = self.poses(values)
+        self._lin_point = (X, Y)
+        out = np.zeros(1, LIN_DTYPE)
+        check(lib().gb_ct_gicp_linearize(self.h, ptr(pose16(X)), ptr(pose16(Y)), ptr(out)))
+        return unpack_linearized(out[0])
+
+    def error(self, values) -> float:
+        """error at `values` with the correspondences of the last linearization point"""
+        X, Y = self.poses(values)
+        Xl, Yl = self._lin_point if self._lin_point is not None else (X, Y)
+        e = C.c_double()
+        check(lib().gb_ct_gicp_error(self.h, ptr(pose16(Xl)), ptr(pose16(Yl)), ptr(pose16(X)), ptr(pose16(Y)), C.byref(e)))
+        return e.value
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            lib().gb_vgicp_factor_destroy(self.h)
+            self.h = None
+
+
+def ct_params(**overrides) -> capi.CtParams:
+    """gb_ct_default_params (GLIM's shipped CT settings) with the given fields replaced; fields of gb_align_params may be
+    given by name as well (max_iterations=..., ...)."""
+    p = capi.CtParams()
+    check(lib().gb_ct_default_params(C.byref(p)))
+    lm_fields = dict(capi.AlignParams._fields_)
+    for k, v in overrides.items():
+        if k in lm_fields:
+            setattr(p.lm, k, v)
+        elif k in ("location_consistency_inf_scale", "constant_velocity_inf_scale"):
+            setattr(p, k, v)
+        else:
+            raise capi.GlimB200Error(f"gb_ct_params has no field {k!r}")
+    return p
+
+
+def align_ct_gicp(factors: list[IntegratedCT_GICPFactorGPU], X_init, Y_init, X_prior, params=None, ctx: Context | None = None) -> list[dict]:
+    """gb_ct_gicp_align: the per-frame LM solve of GLIM's CT odometry (odometry_estimation_ct.cpp:159-182) for every problem
+    in one call.  factors[p] is problem p's CT factor; X_init, Y_init, X_prior: (P,4,4); params: None (defaults), a dict of
+    overrides or a capi.CtParams.  -> per problem {X, Y (4,4), error, num_inliers, lambda, iterations, trials, status, status_name}"""
+    P = len(factors)
+    if P == 0:
+        return []
+    if params is None or isinstance(params, dict):
+        params = ct_params(**(params or {}))
+    ctx = ctx or factors[0].ctx
+    arr = (C.c_void_p * P)(*[f._handle() for f in factors])
+    X0, Y0, Xp = (pose16(np.asarray(a, dtype=np.float64).reshape(P, 4, 4)) for a in (X_init, Y_init, X_prior))
+    res = (capi.CtResult * P)()
+    check(lib().gb_ct_gicp_align(ctx.h, P, C.cast(arr, C.c_void_p), ptr(X0), ptr(Y0), ptr(Xp), C.byref(params), C.cast(res, C.c_void_p)))
+    return [{
+        "X": np.array(r.X[:]).reshape(4, 4).T.copy(), "Y": np.array(r.Y[:]).reshape(4, 4).T.copy(),
+        "error": r.error, "num_inliers": r.num_inliers, "lambda": r.lambda_,
+        "iterations": r.iterations, "trials": r.trials, "status": r.status, "status_name": capi.ALIGN_STATUS_NAMES.get(r.status, "?"),
+    } for r in res]
+
+
+def deskew_ct(cloud: PointCloudGPU, X, Y, neighbors, k_neighbors: int, host_outputs: bool = True, ctx: Context | None = None):
+    """gb_ct_deskew: the deskewed frame of GLIM's CT odometry (deskewed_source_points(values, true) + covariance re-estimation
+    with the same neighbour indices, odometry_estimation_ct.cpp:199-204).  cloud carries times; neighbors (n, k_correspondences)
+    int32 in the original order.  -> (points (n,4), covs (n,4,4) [i,row,col], normals (n,4), PointCloudGPU); the host arrays are
+    None unless host_outputs."""
+    ctx = ctx or cloud.ctx
+    nb = np.ascontiguousarray(neighbors, dtype=np.int32)
+    n = cloud.n
+    kc = nb.shape[1] if nb.ndim == 2 else 0
+    pts = np.empty((n, 4)) if host_outputs else None
+    cov = np.empty((n, 16)) if host_outputs else None
+    nrm = np.empty((n, 4)) if host_outputs else None
+    h = C.c_void_p()
+    check(lib().gb_ct_deskew(ctx.h, cloud.h, ptr(pose16(np.asarray(X, dtype=np.float64).reshape(4, 4))), ptr(pose16(np.asarray(Y, dtype=np.float64).reshape(4, 4))), ptr(nb),
+                             int(kc), int(k_neighbors), ptr(pts), ptr(cov), ptr(nrm), C.byref(h)))
+    out = PointCloudGPU(ctx, h, n)
+    if not host_outputs:
+        return None, None, None, out
+    return pts, cov.reshape(n, 4, 4).transpose(0, 2, 1).copy(), nrm, out
 
 
 class NonlinearFactorSetGPU:

@@ -287,6 +287,89 @@ GB_API gb_status gb_align_default_params(gb_align_params* params); /* the odomet
 GB_API gb_status gb_vgicp_align(gb_ctx* ctx, size_t num_problems, const size_t* factor_offsets /* P + 1 */, gb_factor* const* factors,
                                 const double* T_init /* P x 16 */, const gb_align_params* params, gb_align_result* results /* P */);
 
+/* ---- Continuous-time GICP: GLIM's LiDAR-only odometry (OdometryEstimationCT, src/glim/odometry/odometry_estimation_ct.cpp,
+ *      config/config_odometry_ct.json) on the device: the time table of a frame (:101), IntegratedCT_GICPFactor_<iVox,
+ *      PointCloud>(X, Y, ivox, frame, ivox) with max_correspondence_distance (:159-163) and the Levenberg-Marquardt solve with
+ *      the two motion priors (:166-182).  X is the pose at the scan's first time-table entry, Y at its last.
+ *      [EXT] gtsam_points is not vendored: the time table, the interpolation, the error convention and the weighting of the
+ *      objective below are this library's statement of the un-vendored factor, written from GLIM's call site.
+ *
+ *      The time table (PointCloud::add_times).  The points are walked in their original order; a point opens a new entry iff
+ *      its time exceeds the current entry's time by more than time_eps = 1e-3 s; an entry's time t_b is the time of its first
+ *      point and every point takes the time of its entry.  tau_b = (t_b - t_0) / (t_{B-1} - t_0), or 0 when B == 1.  So Y is
+ *      the pose at the LAST ENTRY's time, which may precede the last point's time by up to time_eps.
+ *
+ *      The factor.  With xi = Log(X^-1 Y), the pose of entry b is T_b = X Exp(tau_b xi) (Pose3 Expmap chart, tangent
+ *      [rot; trans], perturbations on the right).  Each point is matched exactly as by gb_gicp_factor_create, with the fp32
+ *      cast of its entry's pose as the lookup transform; residual, M and error as there: r = q - T_b p,
+ *      M = (C_q + R_b C_p R_b^T)^-1, error = sum r^T M r (no 1/2); error() takes the correspondences at (X_lin, Y_lin) and
+ *      evaluates at (X_eval, Y_eval).  Per entry, (H_b, b_b) are the blocks the GICP factor's record holds as H_ss / b_s at the
+ *      pose T_b; they are chained to (X, Y) in fp64, entry by entry, by
+ *        D0_b = Ad(Exp(-tau_b xi)) - tau_b J_r(tau_b xi) J_r^-1(xi) Ad(Y^-1 X),   D1_b = tau_b J_r(tau_b xi) J_r^-1(xi),
+ *        H = sum_b [D0_b D1_b]^T H_b [D0_b D1_b],   b = sum_b [D0_b D1_b]^T b_b
+ *      (J_r the SE(3) right Jacobian; exact, the pose being constant within an entry).  The 12x12 system goes into a
+ *      gb_linearized6 with X IN THE TARGET SLOT and Y IN THE SOURCE SLOT: H_tt = H_XX, H_ss = H_YY, H_ts = H_XY (rows X),
+ *      b_t = b_X, b_s = b_Y; so gb_hessian_blocks yields HessianFactor(X, Y, ...) unchanged.
+ *
+ *      A CT factor is a gb_factor of its own kind, destroyed by gb_vgicp_factor_destroy.  gb_vgicp_linearize, gb_vgicp_error,
+ *      gb_factor_set_*, gb_sweep_create and gb_vgicp_align refuse it, and the gb_ct_* entry points refuse every other factor,
+ *      with GB_ERR_INVALID_ARGUMENT before any launch; these refusals are the only change of behaviour of earlier entry points.
+ *      A CT factor reads its source's time table at every call: do not set times while another thread uses the factor. ---- */
+/* The time table of `cloud` from its n times (the cloud's original point order), built on the host and stored with the cloud
+ * on the device (entry starts and tau_b; t_0 and t_{B-1} on the host as well); setting times again replaces it.  Validated
+ * before any launch: times finite and non-decreasing, n equal to the cloud's size (>= 1), the cloud on ctx's device.
+ * Every consumer of clouds other than the CT factor ignores the table. */
+GB_API gb_status gb_cloud_add_times(gb_ctx* ctx, gb_cloud* cloud, size_t n, const double* times);
+/* host copy of a cloud's time table: B, starts (B + 1, original indices), tau (B), t_0, t_{B-1}; any pointer may be NULL.
+ * B = 0 for a cloud without times. */
+GB_API gb_status gb_cloud_time_table(const gb_cloud* cloud, int* num_entries, int32_t* starts, double* tau, double* t_first, double* t_last);
+/* The source must carry times (and covariances, as for GICP); the target must be an iVox. */
+GB_API gb_status gb_ct_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out);
+/* Two launches: the sweep over the work items and the per-problem chain rule. */
+GB_API gb_status gb_ct_gicp_linearize(gb_factor* factor, const double X[16], const double Y[16], gb_linearized6* out);
+GB_API gb_status gb_ct_gicp_error(gb_factor* factor, const double X_lin[16], const double Y_lin[16], const double X_eval[16], const double Y_eval[16], double* error);
+
+/* The per-frame solve (odometry_estimation_ct.cpp:159-182), many problems in one call.  Problem p has one CT factor and the
+ *      objective  E(X, Y) = e_ct(X, Y) + l |Log(X_prior^-1 X)|^2 + c |Log(X^-1 Y)|^2
+ *      (l = location_consistency_inf_scale, c = constant_velocity_inf_scale; PriorFactor(X, last_T_world_lidar_end) and
+ *      BetweenFactor(X, Y, identity) with isotropic precisions).  The small terms carry no 1/2 because the CT error carries
+ *      none: the relative weight GTSAM gives HessianFactor(H, -b, e) next to a NoiseModelFactor.  Their Jacobians are
+ *      J_r^-1(e), and -J_r^-1(e) Ad(Y^-1 X) for X in the between term.  The CT error takes the inliers of the linearization
+ *      poses.
+ *      The iteration rule is gb_vgicp_align's at 12 dof: (H + lambda I) delta = -b by a 12x12 fp64 Cholesky, trial poses
+ *      X Exp(delta_X), Y Exp(delta_Y), the same accept, reject and termination steps (the step tests read the larger of the
+ *      two poses' steps), DEGENERATE when the first linearization has no inliers.
+ *      Each round is at most four launches for the whole batch (linearize sweep if any problem needs it, step, error sweep,
+ *      accept) and one 8-byte device-to-host copy, whatever the number of problems. */
+typedef struct gb_ct_params {
+  gb_align_params lm;                     /* max_iterations 8 (lm_max_iterations), lambda_initial 1e-10, absolute_error_tol 1e-2,
+                                             relative_error_tol 1e-5, lambda_factor 10, lambda_upper_bound 1e5, step tests off (<= 0) */
+  double location_consistency_inf_scale;  /* 1e-3 (config_odometry_ct.json:25) */
+  double constant_velocity_inf_scale;     /* 1e3  (config_odometry_ct.json:26; the code default at :44 is 1e-3) */
+} gb_ct_params;
+typedef struct gb_ct_result {
+  double X[16], Y[16];                    /* column-major */
+  double error, num_inliers, lambda;      /* as gb_align_result; error = the objective E */
+  int iterations, trials, status;         /* GB_ALIGN_* */
+} gb_ct_result;
+GB_API gb_status gb_ct_default_params(gb_ct_params* params);
+/* Validated before any launch: CT factors on ctx's device, finite poses, the bounds of gb_vgicp_align's parameters, finite
+ * non-negative precisions. */
+GB_API gb_status gb_ct_gicp_align(gb_ctx* ctx, size_t num_problems, gb_factor* const* factors /* P CT factors */, const double* X_init /* P x 16 */,
+                                  const double* Y_init /* P x 16 */, const double* X_prior /* P x 16: last_T_world_lidar_end */,
+                                  const gb_ct_params* params, gb_ct_result* results /* P */);
+/* The deskewed frame (factor->deskewed_source_points(values, true) and the covariance re-estimation of
+ * odometry_estimation_ct.cpp:199-204): every point becomes Exp(tau_b xi) p (= X^-1 T_b p) in fp64, computed from the cloud's fp32
+ * position; covariances and normals are then re-estimated from the deskewed points with the caller's neighbour indices by
+ * gb_preprocess's covariance stage (plane_covariance).  Outputs, each n x ... in the original point order, or NULL: points
+ * (n x 4, w = 1), covariances (n x 16, column-major) and normals (n x 4); out_cloud: a new device cloud of the deskewed frame
+ * with its covariances and normals, ready for gb_ivox_insert(ivox, cloud, X, 1, seed); it carries no times.
+ * Validated before any launch as gb_covariances: 1 <= k_neighbors <= k_correspondences, the first k_neighbors indices of every
+ * row in [0, n); X and Y finite; a source with times on ctx's device. */
+GB_API gb_status gb_ct_deskew(gb_ctx* ctx, const gb_cloud* source, const double X[16], const double Y[16],
+                              const int32_t* neighbors /* n x k_correspondences, original order, as gb_preprocess returns them */,
+                              int k_correspondences, int k_neighbors, double* out_xyzw, double* out_cov4x4, double* out_normals4, gb_cloud** out_cloud);
+
 /* ---- Solver hand-off (SURVEY A.3; global_mapping.cpp:492-501 feeds these to isam2->update): the blocks of
  *      gtsam::HessianFactor(k_t, k_s, G11 = H_tt, G12 = H_ts, g1 = -b_t, G22 = H_ss, g2 = -b_s, f = error_scale * error),
  *      6x6 blocks column-major, from one factor record or from one fp32 row of the pair slab (levels pre-summed on the

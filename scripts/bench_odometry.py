@@ -11,12 +11,17 @@
       the upload and build costs depend only on its size;
   (d) the GICP configuration GLIM ships (registration_type "GICP"): a 1.0 m device iVox grown over the warm frames, then per
       frame one device odometry frame -- gb_vgicp_align on one GICP factor (max_iterations 8) plus the insert at rate 0.1 --
-      with the insert also reported on its own.
+      with the insert also reported on its own;
+  (e) the CT configuration GLIM ships for LiDAR-only odometry (odometry_estimation_ct.cpp, config_odometry_ct.json):
+      motion-distorted hdl32 frames (60 000 rays, 10 m/s, 0.6 rad/s; tests/ct_oracle.distorted_frame), a 1.0 m iVox (min_dist
+      0.1, mode 1, LRU 200) grown over --ct-warm frames deskewed at ground truth, then per frame gb_cloud_add_times, the CT
+      factor, gb_ct_gicp_align (default gb_ct_params, max_correspondence_distance 2.0), gb_ct_deskew and the insert of every
+      deskewed point at X.  The twist prediction is host arithmetic outside the timed span; frames are uploaded beforehand.
 
 Times are a host clock around synchronised calls, median over the timed frames.  Launch counts come from
 gb_ctx_kernel_launches.  Every line carries the card's name and power limit, read in the same run.
 
-    python scripts/bench_odometry.py [--warm 40] [--frames 20]
+    python scripts/bench_odometry.py [--warm 40] [--frames 20] [--ct-warm 10]
 """
 import argparse
 import json
@@ -47,6 +52,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--warm", type=int, default=40)
     ap.add_argument("--frames", type=int, default=20)
+    ap.add_argument("--ct-warm", type=int, default=10)
     args = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip().splitlines()
     CARD = card[0] if card else "unknown"
@@ -166,6 +172,44 @@ def main():
          kernel_launches=int(np.median(ins_launches)), frame_points=int(clouds[-1].n), sampling_rate=0.1)
     emit(leg="gicp/odometry_frame/device_ivox", median_ms=round(float(np.median(frame_ms[1:])) * 1e3, 3), runs_ms=[round(t * 1e3, 3) for t in frame_ms],
          kernel_launches=int(np.median(frame_launches)), ivox_voxels=ivox.num_voxels, ivox_points=ivox.num_points)
+
+    # (e) the CT configuration: per frame add_times + CT factor + gb_ct_gicp_align + gb_ct_deskew + insert
+    from tests import ct_oracle as co
+
+    n_ct = args.ct_warm + args.frames
+    frames = []
+    for k in range(n_ct):
+        pts, tms = co.distorted_frame(sc, k, 32 * 1875, synth.rng_for(524, k))
+        nb = synth.knn(pts, 10)
+        cov = synth.plane_covariances(pts, nb)[1]
+        frames.append((gpu.PointCloudGPU.clone(pts, cov, ctx=ctx), nb, tms))
+    ivox = gpu.IVoxGPU(1.0, 0.1, 10, 1, 200, 10, ctx=ctx)
+    ms, launches, iters = [], [], []
+    X_last = Y_last = span = None
+    for k, (cloud, nb, tms) in enumerate(frames):
+        t_first, t_last = 0.1 * k + tms[0], 0.1 * k + tms[co.time_table(tms)[0][-2]]  # t_0 and t_{B-1}
+        if k < args.ct_warm:
+            X, Y = co.gt_pose(t_first), co.gt_pose(t_last)
+            cloud.add_times(tms)
+            ivox.insert(gpu.deskew_ct(cloud, X, Y, nb, 10, host_outputs=False)[3], X, 1.0, seed=k)
+        else:
+            v = co.motion(X_last, Y_last) / (span[1] - span[0])
+            X0 = Y_last @ co.se3_exp(v * (t_first - span[1]))
+            Y0 = X0 @ co.se3_exp(v * (t_last - t_first))
+            l0 = ctx.kernel_launches
+            t0 = time.perf_counter()
+            cloud.add_times(tms)
+            fac = gpu.IntegratedCT_GICPFactorGPU(0, 1, ivox, cloud, 2.0, ctx=ctx)
+            r = gpu.align_ct_gicp([fac], [X0], [Y0], [Y_last])[0]
+            X, Y = r["X"], r["Y"]
+            ivox.insert(gpu.deskew_ct(cloud, X, Y, nb, 10, host_outputs=False)[3], X, 1.0, seed=k)
+            ms.append(time.perf_counter() - t0)
+            launches.append(ctx.kernel_launches - l0)
+            iters.append(r["iterations"])
+        X_last, Y_last, span = X, Y, (t_first, t_last)
+    emit(leg="ct/odometry_frame/device_ivox", median_ms=round(float(np.median(ms[1:])) * 1e3, 3), runs_ms=[round(t * 1e3, 3) for t in ms],
+         kernel_launches=int(np.median(launches)), lm_iterations=int(np.median(iters)), frame_points=int(frames[-1][0].n), ivox_voxels=ivox.num_voxels,
+         ivox_points=ivox.num_points)
 
 
 if __name__ == "__main__":
