@@ -31,6 +31,8 @@ SYMBOLS = [
     "gb_ivox_create", "gb_ivox_insert", "gb_ivox_info", "gb_ivox_download", "gb_ivox_destroy", "gb_gicp_factor_create",
     "gb_cloud_add_times", "gb_cloud_time_table", "gb_ct_gicp_factor_create", "gb_ct_gicp_linearize", "gb_ct_gicp_error",
     "gb_ct_default_params", "gb_ct_gicp_align", "gb_ct_deskew",
+    "gb_point_grid_build", "gb_point_grid_info", "gb_point_grid_download", "gb_point_grid_destroy", "gb_gicp_grid_factor_create",
+    "gb_gicp_grid_factor_half_width",
 ]
 
 GB_SLAB_STRIDE = 96
@@ -170,6 +172,12 @@ def lib():
     L.gb_ct_default_params.argtypes = [vp]
     L.gb_ct_gicp_align.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp]
     L.gb_ct_deskew.argtypes = [vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]
+    L.gb_point_grid_build.argtypes = [vp, vp, f64, vp]
+    L.gb_point_grid_info.argtypes = [vp, vp, vp, vp]
+    L.gb_point_grid_download.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.gb_point_grid_destroy.argtypes = [vp]
+    L.gb_gicp_grid_factor_create.argtypes = [vp, vp, vp, f64, vp]
+    L.gb_gicp_grid_factor_half_width.argtypes = [vp, vp]
     for name in SYMBOLS:
         getattr(L, name)  # AttributeError here means the library and include/glim_b200.h are out of sync
     _lib = L

@@ -2,6 +2,7 @@
 // arenas, clouds, factors, sweeps and overlap.  The map, preprocess and peer-slab entry points are defined next to their
 // work, in gb_kernels_voxelmap.cu, gb_kernels_preprocess.cu and gb_peer.cu.
 #include "gb_internal.cuh"
+#include "gb_grid_math.cuh"  // grid_half_width
 
 #include <stdarg.h>
 #include <stdio.h>
@@ -281,6 +282,7 @@ extern "C" gb_status gb_cloud_upload(gb_ctx* ctx, size_t n, const double* xyzw, 
   gb_owned<gb_cloud> c(new (std::nothrow) gb_cloud(), cloud_free);
   if (!c) return GB_ERR_INTERNAL;
   c->device = ctx->device;
+  c->covs = cov4x4 != nullptr;
   if (n > 0) GB_CHECK(cloud_upload(ctx, n, xyzw, cov4x4, normals4, c.get()));
   *out = c.release();
   return GB_OK;
@@ -329,6 +331,7 @@ extern "C" gb_status gb_cloud_destroy(gb_cloud* c) {
 extern "C" gb_status gb_vgicp_factor_create(gb_ctx* ctx, const gb_voxelmap* target, const gb_cloud* source, int flags, gb_factor** out) {
   GB_REQUIRE(ctx && target && source && out, "null argument");
   GB_REQUIRE(target->kind != GB_MAP_IVOX, "the target is an iVox: GICP factors on it come from gb_gicp_factor_create");
+  GB_REQUIRE(target->kind != GB_MAP_POINTS, "the target is a point grid: GICP factors on it come from gb_gicp_grid_factor_create");
   // clouds / voxel maps may have been uploaded through another context (another module thread): device memory is shared,
   // and every producer call returns only after its stream has drained, so only the DEVICE has to match
   GB_REQUIRE(target->device == ctx->device && source->device == ctx->device, "cloud / voxel map live on another device");
@@ -354,6 +357,34 @@ extern "C" gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, c
   f->max_corr2 = (float)(max_correspondence_distance * max_correspondence_distance);
   ctx_retain(ctx);
   *out = f;
+  return GB_OK;
+}
+
+extern "C" gb_status gb_gicp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out) {
+  GB_REQUIRE(ctx && target && source && out, "null argument");
+  *out = nullptr;
+  GB_REQUIRE(std::isfinite(max_correspondence_distance) && max_correspondence_distance > 0.0, "max_correspondence_distance must be positive and finite");
+  const gb_voxelmap* m = grid_map(target);
+  GB_REQUIRE(m->kind == GB_MAP_POINTS, "the target is not a point grid (gb_point_grid_build)");
+  GB_REQUIRE(m->device == ctx->device && source->device == ctx->device, "cloud / point grid live on another device");
+  GB_REQUIRE(source->covs, "the source carries no covariances");
+  const float max_corr2 = (float)(max_correspondence_distance * max_correspondence_distance);
+  const int half_width = grid_half_width(m->inv_res, max_corr2, m->key_extent);
+  GB_REQUIRE(half_width <= kGridMaxHalfWidth, "max_correspondence_distance / cell_size too large: the search would span more than 17^3 cells");
+  GB_ENTER(ctx);
+  gb_factor* f = new (std::nothrow) gb_factor();
+  if (!f) return GB_ERR_INTERNAL;
+  f->ctx = ctx; f->target = m; f->source = source; f->id = g_next_factor_id.fetch_add(1);
+  f->max_corr2 = max_corr2;
+  f->grid_m = half_width;
+  ctx_retain(ctx);
+  *out = f;
+  return GB_OK;
+}
+extern "C" gb_status gb_gicp_grid_factor_half_width(const gb_factor* f, int* m) {
+  GB_REQUIRE(f && m, "null argument");
+  GB_ENTER(f->ctx);
+  *m = f->grid_m;
   return GB_OK;
 }
 
@@ -529,21 +560,22 @@ static void desc_target(FactorDesc& D, const gb_voxelmap* t) {
   D.max_scan = t->max_scan;
   D.inv_res = t->inv_res;
 }
-// a GICP factor's target part: the iVox's table and point records in the FactorDesc, the rest in its GicpDesc
-static void desc_target_ivox(FactorDesc& D, GicpDesc& G, const gb_factor* fa) {
+// a GICP factor's target part: the iVox's or point grid's table and point records in the FactorDesc, the rest in its GicpDesc
+static void desc_target_gicp(FactorDesc& D, GicpDesc& G, const gb_factor* fa) {
   desc_target(D, fa->target);
   G.cells = fa->target->cells;
   G.max_corr2 = fa->max_corr2;
-  G.num_offsets = fa->target->mode;
+  G.num_offsets = fa->target->kind == GB_MAP_POINTS ? fa->grid_m : fa->target->mode;
 }
 // B_f of SURVEY 8(d): 48 B per source point, 48 B per target voxel, 16 B per bucket, pose in + record out.
 // The bucket term is charged at the SMALLEST table that could hold the voxels (16384 doubled until >= V), not at
 // our deliberately sparse table (>= 8 V): padding we added for speed must not inflate the achieved-GB/s figure.
-// A GICP factor is charged 48 B per STORED target point in place of the voxel records (its voxels' buckets the same way).
+// A GICP factor is charged 48 B per STORED target point in place of the voxel records (its voxels' or cells' buckets the
+// same way).
 static uint64_t factor_bytes(const gb_factor* fa) {
   const bool sv = (fa->flags & GB_FACTOR_SURFACE_VALIDATION) != 0;
   const uint64_t V = (uint64_t)fa->target->num_voxels;
-  const uint64_t records = fa->target->kind == GB_MAP_IVOX ? (uint64_t)fa->target->num_points : V;
+  const uint64_t records = gb_target_class(fa->target) != 0 ? (uint64_t)fa->target->num_points : V;
   uint64_t nb_ref = 16384;
   while (nb_ref < V) nb_ref *= 2;
   return (uint64_t)fa->source->n * (48 + (sv ? 12 : 0)) + records * 48 + nb_ref * 16 + 64 + 488;  // +12 B / point: the normals, when they are read
@@ -563,8 +595,8 @@ static gb_status sweep_follow_targets(gb_sweep* s) {
       synced = true;
     }
     s->target_versions[f] = fa->target->version;
-    if (fa->target->kind == GB_MAP_IVOX) {
-      desc_target_ivox(s->h_descs[f], s->h_gdescs[f], fa);
+    if (s->gicp) {
+      desc_target_gicp(s->h_descs[f], s->h_gdescs[f], fa);
       GB_CUDA(cudaMemcpyAsync(s->d_gdescs + f, s->h_gdescs + f, sizeof(GicpDesc), cudaMemcpyHostToDevice, s->ctx->stream));
     } else {
       desc_target(s->h_descs[f], fa->target);
@@ -613,10 +645,12 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     GB_REQUIRE(factors[f], "null factor");
     GB_REQUIRE(factors[f]->kind != GB_FACTOR_CT, "a CT factor has two poses: only the gb_ct_* entry points take it");
     GB_REQUIRE(factors[f]->source->device == ctx->device && factors[f]->target->device == ctx->device, "factor lives on another device");
-    GB_REQUIRE((factors[f]->target->kind == GB_MAP_IVOX) == (factors[0]->target->kind == GB_MAP_IVOX), "the factors of one sweep must all be VGICP or all GICP factors");
+    GB_REQUIRE(gb_target_class(factors[f]->target) == gb_target_class(factors[0]->target),
+               "the factors of one sweep must all be VGICP factors, all GICP factors on iVoxes or all GICP factors on point grids");
     total_pts += factors[f]->source->n;
   }
-  const bool gicp = F > 0 && factors[0]->target->kind == GB_MAP_IVOX;
+  const int target_class = F > 0 ? gb_target_class(factors[0]->target) : 0;
+  const bool gicp = target_class != 0;
   GB_REQUIRE(!gicp || !pair_index, "GICP sweeps take no pair_index (no slab can be attached to them)");
   GB_ENTER(ctx);
   gb_owned<gb_sweep> s(new (std::nothrow) gb_sweep(), sweep_free);
@@ -624,6 +658,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   ctx_retain(ctx);
   s->ctx = ctx; s->F = F; s->factors.assign(factors, factors + F);
   s->gicp = gicp;
+  s->point_grid = target_class == 2;
 
   // kernel generation and work-item policy
   // Kernel policy (A/B runs of the kernels, scripts/ab_sweep.py): small sweeps -- about one item per warp: an odometry
@@ -635,7 +670,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   const uint64_t warps = (uint64_t)s->capacity * 8;
   const bool small = F > 0 && total_pts <= warps * 2048;
   s->kernel_version = (kv == 3 || kv == 5) ? kv : (small ? 5 : 3);
-  if (gicp) s->kernel_version = 5;  // k_gicp_sweep runs sweep5's strided items at every size
+  if (gicp) s->kernel_version = 5;  // k_gicp_sweep and k_gicp_grid_sweep run sweep5's strided items at every size
   {
     // sweep3's items: ~6 items per warp (first one static, the rest drawn dynamically), between 128 and 2048 points each,
     // in whole rows of 32 points
@@ -656,9 +691,9 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     const bool sv = (fa->flags & GB_FACTOR_SURFACE_VALIDATION) != 0;
     D.normals = sv ? fa->source->normals : nullptr;
     any_sv = any_sv || sv;
-    if (gicp) desc_target_ivox(D, gdescs[f], fa); else desc_target(D, fa->target);
+    if (gicp) desc_target_gicp(D, gdescs[f], fa); else desc_target(D, fa->target);
     s->target_versions.push_back(fa->target->version);
-    s->any_incremental = s->any_incremental || fa->target->kind != GB_MAP_BUILT;
+    s->any_incremental = s->any_incremental || (fa->target->kind != GB_MAP_BUILT && fa->target->kind != GB_MAP_POINTS);
     D.n = (int)fa->source->n;
     D.pair = pair_index ? pair_index[f] : (int)f;
     s->h_pair.push_back(D.pair);
@@ -941,6 +976,7 @@ extern "C" gb_status gb_overlap(gb_ctx* ctx, size_t T, const gb_voxelmap* const*
   *overlap = 0.0;
   if (T == 0 || source->n == 0) return GB_OK;
   GB_REQUIRE(targets && deltas, "null targets / deltas");
+  for (size_t t = 0; t < T; t++) GB_REQUIRE(!targets[t] || targets[t]->kind != GB_MAP_POINTS, "a point grid is not an occupancy target");
   GB_ENTER(ctx);
   // the same layout in pinned staging and in scratch: descriptors | poses | count
   struct Staging { FactorDesc* descs; double* poses; int* count; } h, d;

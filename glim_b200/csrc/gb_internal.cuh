@@ -67,13 +67,15 @@ struct gb_cloud {
   int* t_starts = nullptr;
   double* t_tau = nullptr;
   void* t_base = nullptr;
+  bool covs = false;  // the cloud carries covariances (an upload with cov4x4, a preprocessed, merged or deskewed frame)
 };
 
-// A map is one of three kinds, fixed at creation.  Every entry point that takes a map checks the kind it accepts.
+// A map is one of four kinds, fixed at creation.  Every entry point that takes a map checks the kind it accepts.
 enum gb_map_kind {
   GB_MAP_BUILT,        // gb_voxelmap_build: records and table only
   GB_MAP_INCREMENTAL,  // gb_voxelmap_create_incremental / gb_voxelmap_insert
   GB_MAP_IVOX,         // gb_ivox_create / gb_ivox_insert: the gb_ivox handle is the map itself
+  GB_MAP_POINTS,       // gb_point_grid_build: every point of a cloud; the gb_point_grid handle is the map itself
 };
 struct gb_voxelmap {
   int device = 0;
@@ -104,12 +106,23 @@ struct gb_voxelmap {
   // iVox parameters: resolution and inv_res are (float)ivox_resolution and (float)(1 / ivox_resolution)
   double ivox_resolution = 0.0, min_dist = 0.0;
   int max_points = 10, mode = 1;
+  // A point grid's records are every point of its cloud ({x y z c00} {c01 c02 c11 c12} {c22, 1, original index bits, 0}) in
+  // ascending (packed key, original index) order, the points without a key last; it keeps cells and keys like an iVox (in
+  // `base`, laid out by grid_layout) and is never inserted into: its version stays 0.  resolution and inv_res are
+  // (float)cell_size and (float)(1 / cell_size).
+  double cell_size = 0.0;
+  int key_extent = 0;          // max over cells and axes of max(|k|, |k + 1|): bounds |q * inv_res| for the search width
 };
 // the stored entries an insert groups ahead of the frame's points: one per voxel, or one per stored point of an iVox
 inline size_t gb_stored_entries(const gb_voxelmap* m) { return m->kind == GB_MAP_IVOX ? m->num_points : (size_t)m->num_voxels; }
 // the handle of an iVox is its gb_voxelmap (gb_ivox stays an incomplete type)
 inline gb_voxelmap* ivox_map(gb_ivox* h) { return reinterpret_cast<gb_voxelmap*>(h); }
 inline const gb_voxelmap* ivox_map(const gb_ivox* h) { return reinterpret_cast<const gb_voxelmap*>(h); }
+// likewise for a point grid (gb_point_grid stays an incomplete type)
+inline gb_voxelmap* grid_map(gb_point_grid* h) { return reinterpret_cast<gb_voxelmap*>(h); }
+inline const gb_voxelmap* grid_map(const gb_point_grid* h) { return reinterpret_cast<const gb_voxelmap*>(h); }
+// The target class of a pose factor: a sweep or call holds one.  0: voxel maps (VGICP), 1: iVoxes (GICP), 2: point grids (GICP).
+inline int gb_target_class(const gb_voxelmap* m) { return m->kind == GB_MAP_IVOX ? 1 : (m->kind == GB_MAP_POINTS ? 2 : 0); }
 
 // device-side factor descriptor (80 B)
 struct FactorDesc {
@@ -129,12 +142,13 @@ struct FactorDesc {
   int chunk;       // sweep3: points per item of THIS factor (the last factors of a sweep get smaller items: tail tapering)
 };
 static_assert(sizeof(FactorDesc) == 80, "FactorDesc size");
-// The rest of a GICP factor's descriptor (k_gicp_sweep): its FactorDesc carries the iVox's table (buckets, mask, max_scan,
-// inv_res) and its point records (voxels); this adds the cells, the correspondence bound and the searched offsets.
+// The rest of a GICP factor's descriptor (k_gicp_sweep, k_gicp_grid_sweep): its FactorDesc carries the iVox's or point grid's
+// table (buckets, mask, max_scan, inv_res) and its point records (voxels); this adds the cells, the correspondence bound and
+// the searched offsets.
 struct GicpDesc {
   const int2* cells;
   float max_corr2;   // (float)(max_correspondence_distance^2)
-  int num_offsets;   // neighbor_voxel_mode
+  int num_offsets;   // neighbor_voxel_mode (iVox), or the search half-width m (point grid)
 };
 static_assert(sizeof(GicpDesc) == 16, "GicpDesc size");
 
@@ -148,8 +162,9 @@ enum gb_factor_kind {
 struct gb_factor {
   gb_factor_kind kind = GB_FACTOR_POSE;
   gb_ctx* ctx = nullptr;
-  const gb_voxelmap* target = nullptr;  // a built or incremental map (VGICP), or an iVox (GICP: target->kind == GB_MAP_IVOX)
+  const gb_voxelmap* target = nullptr;  // a built or incremental map (VGICP), an iVox or a point grid (GICP)
   float max_corr2 = 0.f;                // GICP: (float)(max_correspondence_distance^2)
+  int grid_m = 0;                       // GICP on a point grid: the search half-width m (grid_half_width)
   const gb_cloud* source = nullptr;
   int flags = 0;
   gb_sweep* single = nullptr;  // lazily created 1-factor sweep
@@ -237,9 +252,10 @@ struct gb_sweep {
   gb_pool_block blk;                // the device and pinned blocks, laid out by sweep_layout; back to the context's pool at the end
   bool any_incremental = false;     // some target is not a built map: its descriptor may go stale (gb_voxelmap_insert, gb_ivox_insert)
   std::vector<uint64_t> target_versions;  // per factor: the target version its descriptor was written from
-  // GICP sweeps (every factor on an iVox; a sweep holds one kind): k_gicp_sweep over sweep5's strided items, with the
-  // GICP half of each descriptor next to the FactorDesc table
+  // GICP sweeps (every factor on an iVox, or every factor on a point grid; a sweep holds one target class): k_gicp_sweep or
+  // k_gicp_grid_sweep over sweep5's strided items, with the GICP half of each descriptor next to the FactorDesc table
   bool gicp = false;
+  bool point_grid = false;          // a GICP sweep over point grids
   GicpDesc* d_gdescs = nullptr;
   GicpDesc* h_gdescs = nullptr;
 };

@@ -621,7 +621,7 @@ extern "C" gb_status gb_ct_deskew(gb_ctx* ctx, const gb_cloud* source, const dou
   GB_ENTER(ctx);
   gb_owned<gb_cloud> c(out_cloud ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
   if (out_cloud && !c) return GB_ERR_INTERNAL;
-  if (c) c->device = ctx->device;
+  if (c) { c->device = ctx->device; c->covs = true; }
   const size_t cub_b = gb_cub_temp_bytes(n);
   gb_planes staged;
   gb_sort_tmp t;

@@ -793,7 +793,7 @@ extern "C" gb_status gb_preprocess(gb_ctx* ctx, size_t n, const double* xyzw, co
   GB_ENTER(ctx);
   gb_owned<gb_cloud> c(P->estimate_covariances ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
   if (P->estimate_covariances && !c) return GB_ERR_INTERNAL;
-  if (c) c->device = ctx->device;
+  if (c) { c->device = ctx->device; c->covs = true; }
   GB_CHECK(preprocess(ctx, n, xyzw, times, intensities, P, out, c.get()));
   GB_CUDA(cudaStreamSynchronize(ctx->stream));  // the cloud is complete when the call returns (it may be used from another context)
   out->cloud = c.release();
@@ -1016,7 +1016,7 @@ extern "C" gb_status gb_merge_frames(gb_ctx* ctx, size_t K, const gb_cloud* cons
   GB_ENTER(ctx);
   gb_owned<gb_cloud> c(out_cloud ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
   if (out_cloud && !c) return GB_ERR_INTERNAL;
-  if (c) c->device = ctx->device;
+  if (c) { c->device = ctx->device; c->covs = true; }
   GB_CHECK(merge_frames(ctx, (int)K, frames, poses, resolution, target, seed, out_xyzw, out_cov4x4, num_out, c.get()));
   GB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (out_cloud) *out_cloud = c.release();

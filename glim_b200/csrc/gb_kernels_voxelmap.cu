@@ -29,6 +29,7 @@
 #include <cub/cub.cuh>
 
 #include <cmath>
+#include <cstring>
 #include <new>
 #include <vector>
 
@@ -691,6 +692,7 @@ extern "C" gb_status gb_voxelmap_info(const gb_voxelmap* m, int* num_voxels, int
 extern "C" gb_status gb_voxelmap_download(const gb_voxelmap* m, int32_t* buckets, int32_t* num_points, float* means, float* cov6) {
   GB_REQUIRE(m, "null map");
   GB_REQUIRE(m->kind != GB_MAP_IVOX, "an iVox holds points, not voxels: use gb_ivox_download");
+  GB_REQUIRE(m->kind != GB_MAP_POINTS, "a point grid holds points, not voxels: use gb_point_grid_download");
   if (buckets) GB_CUDA(cudaMemcpy(buckets, m->buckets, sizeof(int4) * (size_t)m->num_buckets, cudaMemcpyDefault));
   return download_records(m->voxels, (size_t)m->num_voxels, num_points, means, cov6);
 }
@@ -763,6 +765,141 @@ extern "C" gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords,
   return download_records(m->voxels, m->num_points, nullptr, xyz, cov6);
 }
 extern "C" gb_status gb_ivox_destroy(gb_ivox* map) { return gb_voxelmap_destroy(ivox_map(map)); }
+
+// ---------------------------------------------------------------------------------------------
+// Point grid (gb_point_grid_build; the rule is written once in include/glim_b200.h): every point of a cloud, grouped by its
+// fp32 lookup key.  k_point_keys (the build's fp32 key per original index), gb_group_by_key / gb_group_starts (stable: a cell's
+// points in original index order, the points without a key last), k_grid_emit (records, cells, keys, table coordinates and the
+// key extent), table_build with drop rate 0.  One host synchronisation for the cell count, one per table attempt.
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+// one thread per sorted slot s: record s is the cloud point of original index idx_s[s]; the first slot of a cell writes the cell
+__global__ void k_grid_emit(int n, const unsigned long long* __restrict__ keys_s, const int* __restrict__ idx_s, const int* __restrict__ flags, const int* __restrict__ pos,
+                            const int* __restrict__ starts, const float4* __restrict__ p0, const float4* __restrict__ p1, const float* __restrict__ p2, const int* __restrict__ inv_perm,
+                            float4* __restrict__ points, int2* __restrict__ cells, unsigned long long* __restrict__ vkeys, int4* __restrict__ vcoord, int* __restrict__ extent) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  const int i = idx_s[s];
+  const int j = inv_perm ? inv_perm[i] : i;
+  const float4 a0 = __ldg(&p0[j]);
+  float4* dst = points + 3 * (size_t)s;
+  dst[0] = a0;
+  dst[1] = __ldg(&p1[j]);
+  dst[2] = make_float4(__ldg(&p2[j]), 1.f, __int_as_float(i), 0.f);
+  if (!flags[s]) return;
+  const int v = pos[s] - 1;
+  const unsigned long long key = keys_s[s];
+  const int cnt = starts[v + 1] - s;
+  int x, y, z;
+  gb_unpack_key(key, x, y, z);
+  cells[v] = make_int2(s, cnt);
+  vkeys[v] = key;
+  vcoord[v] = make_int4(x, y, z, cnt);
+  const int e = max(max(max(-x, x + 1), max(-y, y + 1)), max(-z, z + 1));
+  atomicMax(extent, e);
+}
+
+// the grid's block of P points and V cells: point records first (gb_voxelmap::voxels), then cells and keys
+void grid_layout(Carver& cv, gb_voxelmap* g) {
+  g->voxels = cv.take<float4>(3 * g->num_points);
+  g->cells = cv.take<int2>((size_t)g->num_voxels);
+  g->vkeys = cv.take<unsigned long long>((size_t)g->num_voxels);
+}
+
+}  // namespace
+
+extern "C" gb_status gb_point_grid_build(gb_ctx* ctx, const gb_cloud* cloud, double cell_size, gb_point_grid** out) {
+  GB_REQUIRE(ctx && cloud && out, "null argument");
+  *out = nullptr;
+  GB_REQUIRE(std::isfinite(cell_size) && cell_size > 0.0, "cell_size must be positive and finite");
+  GB_REQUIRE(cloud->device == ctx->device, "the cloud lives on another device");
+  GB_ENTER(ctx);
+  gb_owned<gb_voxelmap> g(new (std::nothrow) gb_voxelmap(), voxelmap_free);
+  if (!g) return GB_ERR_INTERNAL;
+  g->device = ctx->device;
+  g->kind = GB_MAP_POINTS;
+  g->cell_size = cell_size;
+  g->resolution = (float)cell_size;
+  g->inv_res = (float)(1.0 / cell_size);
+  g->max_scan = 10;  // the build's table (16384 buckets doubled until >= 8 cells, 10 probes) with drop rate 0
+  g->init_buckets = 16384;
+  const int n = (int)cloud->n;
+  cudaStream_t st = ctx->stream;
+  int V = 0;
+  int4* d_vcoord = nullptr;
+  int* d_dropped = nullptr;
+  if (n > 0) {
+    const size_t cub_b = gb_cub_temp_bytes(n);
+    gb_sort_tmp t;
+    int *d_flags, *d_pos, *d_starts, *d_extent;
+    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+      t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
+      d_flags = cv.take<int>(n + 1);
+      d_pos = cv.take<int>(n + 1);
+      d_starts = cv.take<int>(n + 1);
+      d_vcoord = cv.take<int4>(n);
+      d_dropped = cv.take<int>(1);
+      d_extent = cv.take<int>(1);
+    }));
+    GB_CHECK(gb_launch(ctx, "k_point_keys", k_point_keys, (n + 255) / 256, 256, 0, n, cloud->p0, cloud->inv_perm, g->inv_res, t.keys, t.idx));
+    GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
+    GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+    GB_CUDA(cudaStreamSynchronize(st));
+    g->num_voxels = V;
+    g->num_points = (size_t)n;
+    Carver size;
+    grid_layout(size, g.get());
+    GB_CUDA(gb_dev_malloc(ctx->device, size.off, &g->base));
+    g->bytes = size.off;
+    Carver cv{(char*)g->base};
+    grid_layout(cv, g.get());
+    GB_CUDA(cudaMemsetAsync(d_extent, 0, sizeof(int), st));
+    GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
+    GB_CHECK(gb_launch(ctx, "k_grid_emit", k_grid_emit, (n + 255) / 256, 256, 0, n, t.keys_s, t.idx_s, d_flags, d_pos, d_starts, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm,
+                       g->voxels, g->cells, g->vkeys, d_vcoord, d_extent));
+    GB_CUDA(cudaMemcpyAsync(&g->key_extent, d_extent, sizeof(int), cudaMemcpyDeviceToHost, st));  // read by table_build's synchronisation
+  }
+  GB_CHECK(table_build(ctx, V, d_vcoord, d_dropped, g->init_buckets, g->max_scan, 0.0, (double)n, &g->buckets, &g->num_buckets, &g->num_dropped_points));
+  g->bytes += sizeof(int4) * (size_t)g->num_buckets;
+  if (g->num_dropped_points != 0) {
+    gb_set_error("point grid table: %d points left out of a table of %d buckets", g->num_dropped_points, g->num_buckets);
+    return GB_ERR_INTERNAL;
+  }
+  *out = reinterpret_cast<gb_point_grid*>(g.release());
+  return GB_OK;
+}
+extern "C" gb_status gb_point_grid_info(const gb_point_grid* grid, int* num_cells, size_t* num_points, double* cell_size) {
+  const gb_voxelmap* g = grid_map(grid);
+  GB_REQUIRE(g && g->kind == GB_MAP_POINTS, "null grid, or not a point grid");
+  if (num_cells) *num_cells = g->num_voxels;
+  if (num_points) *num_points = g->num_points;
+  if (cell_size) *cell_size = g->cell_size;
+  return GB_OK;
+}
+extern "C" gb_status gb_point_grid_download(const gb_point_grid* grid, int32_t* cell_coords, int32_t* cell_counts, int32_t* indices, float* xyz, float* cov6) {
+  const gb_voxelmap* g = grid_map(grid);
+  GB_REQUIRE(g && g->kind == GB_MAP_POINTS, "null grid, or not a point grid");
+  const size_t V = (size_t)g->num_voxels, P = g->num_points;
+  if (V > 0 && (cell_coords || cell_counts)) {
+    std::vector<unsigned long long> keys(V);
+    std::vector<int2> cells(V);
+    GB_CUDA(cudaMemcpy(keys.data(), g->vkeys, sizeof(unsigned long long) * V, cudaMemcpyDefault));
+    GB_CUDA(cudaMemcpy(cells.data(), g->cells, sizeof(int2) * V, cudaMemcpyDefault));
+    for (size_t v = 0; v < V; v++) {
+      if (cell_coords)
+        for (int a = 0; a < 3; a++) cell_coords[3 * v + a] = (int32_t)((keys[v] >> (42 - 21 * a)) & 0x1FFFFF) - (1 << 20);
+      if (cell_counts) cell_counts[v] = cells[v].y;
+    }
+  }
+  if (P > 0 && indices) {
+    std::vector<float4> h(3 * P);
+    GB_CUDA(cudaMemcpy(h.data(), g->voxels, sizeof(float4) * h.size(), cudaMemcpyDefault));
+    for (size_t r = 0; r < P; r++) memcpy(&indices[r], &h[3 * r + 2].z, sizeof(int32_t));
+  }
+  return download_records(g->voxels, P, nullptr, xyz, cov6);
+}
+extern "C" gb_status gb_point_grid_destroy(gb_point_grid* grid) { return gb_voxelmap_destroy(grid_map(grid)); }
 
 // ---------------------------------------------------------------------------------------------
 // Morton reordering of a new cloud (PointCloudGPU::clone keeps the caller's order on the host side of the

@@ -52,6 +52,7 @@ typedef struct gb_voxelmap gb_voxelmap; /* gtsam_points::GaussianVoxelMapGPU    
 typedef struct gb_factor gb_factor;     /* gtsam_points::IntegratedVGICPFactorGPU                                   */
 typedef struct gb_sweep gb_sweep;       /* gtsam_points::NonlinearFactorSetGPU (a prepared batch of factors)        */
 typedef struct gb_ivox gb_ivox;         /* gtsam_points::iVox (odometry_estimation_cpu.cpp:57-61), kept on the device */
+typedef struct gb_point_grid gb_point_grid; /* a whole frame's points on the device: the KdTree target of IntegratedGICPFactor  */
 #define GB_SLAB_STRIDE 96               /* floats per row of the per-pair Hessian slab (layout below, at gb_sweep_create) */
 
 /* LinearizedSystem6 of the reference GPU factor, widened to fp64 (SURVEY.md 8(a) a4, A.3).
@@ -177,11 +178,11 @@ GB_API gb_status gb_voxelmap_insert(gb_ctx* ctx, gb_voxelmap* map, const gb_clou
  *      step 4 and the neighbour offsets below are this library's statement of it.
  *      Threading and lifetime as for incremental voxel maps: two host synchronisations per insert (one more per extra table
  *      attempt), sweeps created before an insert follow it, do not insert while another thread uses the map. ---- */
-/* An iVox handle and a voxel-map handle are not interchangeable.  gb_ivox_insert, gb_ivox_info, gb_ivox_download and
+/* An iVox handle, a point-grid handle and a voxel-map handle are not interchangeable.  gb_ivox_insert, gb_ivox_info, gb_ivox_download and
  * gb_gicp_factor_create take an iVox only; gb_vgicp_factor_create and gb_voxelmap_download refuse one, and gb_voxelmap_insert
  * takes an incremental map only.  Each refuses another kind with GB_ERR_INVALID_ARGUMENT before any launch.  These
  * refusals are the only change of behaviour from earlier builds, which read a handle of the wrong kind as the other kind.
- * gb_overlap takes every kind: it tests occupancy only.
+ * gb_overlap takes voxel maps and iVoxes: it tests occupancy only (point grids: see gb_point_grid_build).
  * neighbor_voxel_mode: 1 (centre), 7 (+ the faces), 19 (+ the edges), 27 (+ the corners).  lru_horizon <= 0: no eviction.
  * GB_ERR_INVALID_ARGUMENT for a non-finite or non-positive resolution, min_dist_in_cell < 0, max_points_in_cell outside
  * [1, 64], another mode or lru_clear_cycle < 1. */
@@ -230,6 +231,55 @@ GB_API gb_status gb_vgicp_error(gb_factor* factor, const double T_lin[16], const
  *      power-of-two table >= 16384 holding the voxels, plus pose and record. ---- */
 GB_API gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out);
 
+/* ---- IntegratedGICPFactor(target_key, source_key, target_frame, source_frame) with the target's KdTree: GICP between two whole
+ *      point clouds, the nearest target point of each source point its correspondence (sub_mapping.cpp:189-211 between factors,
+ *      global_mapping.cpp:379-428 submap between factors, global_mapping_pose_graph.cpp:391-405 loop candidates), on the device.
+ *      An exact KdTree returns the brute-force nearest neighbour; here a uniform grid over the target's points finds the same
+ *      point by a bounded cell search.
+ *
+ *      The point grid.  gb_point_grid_build copies every point of a device cloud (position and covariance) into a map of its
+ *      own kind.  Each point with finite x, y, z is keyed with the fp32 lookup rule k = floor((float)(p * (float)(1 / cell_size)))
+ *      per axis (as every sweep keys its queries); points that are not finite, or whose key is outside the 21-bit range
+ *      (+-2^20 cells), are stored but never match.  Cells are in ascending packed-key order, and the points of a cell in
+ *      ascending original index (the cloud's caller order); a cell is {first point, count}.  Records have the iVox's layout
+ *      {x y z c00} {c01 c02 c11 c12} {c22, 1, ., .}.  The table is the build's (16384 buckets doubled until >= 8 cells, 10
+ *      probes) with drop rate 0: every cell is found.  The grid is built once (no insert) and owns its memory, so the cloud
+ *      may be destroyed after the build.  An empty cloud gives an empty grid.  GB_ERR_INVALID_ARGUMENT before any launch for
+ *      a non-finite or non-positive cell_size or a cloud on another device than ctx.
+ *
+ *      The correspondence.  q = the source point transformed with the sweep's fp32 pose, c = its cell.  The cells c + o are
+ *      searched for o in [-m, m]^3, where m is the smallest integer that provably holds every stored point with
+ *      d2 < (float)(r^2) given the fp32 rounding of 1 / cell_size, of q * inv and of r^2 (the proof is at grid_half_width,
+ *      gb_grid_math.cuh; m depends on r / cell_size and, by a few ulps, on the grid's extent; gb_gicp_grid_factor_half_width
+ *      reports it).  The match is the stored point with the smallest fp32 d2 = (dx^2 + dy^2) + dz^2 (d = p - q, uncontracted)
+ *      subject to d2 < (float)(r^2), ties to the smaller original index: the brute-force argmin over all target points,
+ *      whatever the search order (unlike the iVox rule, whose ties follow the offset order).  A query whose key saturates
+ *      finds nothing.  Per point the factor is the iVox GICP factor's: r = p - q, M = (C_p + R C_a R^T)^-1, error = sum
+ *      r^T M r (no 1/2); error() takes its correspondences at T_lin and evaluates at T_eval.  [EXT] the un-vendored
+ *      IntegratedGICPFactor's KdTree search and error convention are this library's statement of them.
+ *
+ *      A grid factor is an ordinary pose gb_factor: gb_vgicp_linearize / _error / _factor_destroy, gb_factor_set_*, gb_sweep_*
+ *      and gb_vgicp_align take it.  A sweep or call holds one target class -- voxel maps, iVoxes or point grids -- and a mix is
+ *      GB_ERR_INVALID_ARGUMENT before any launch; grid sweeps take no pair_index, slab or peer slab.  gb_sweep_stats of a grid
+ *      sweep: 48 B per source point, 48 B per stored target point, 16 B per bucket of the smallest power-of-two table >= 16384
+ *      holding the cells, plus pose and record.
+ *      A grid is not a voxel map and not an iVox: gb_vgicp_factor_create, gb_gicp_factor_create, gb_ct_gicp_factor_create,
+ *      gb_voxelmap_insert, gb_voxelmap_download, the gb_ivox_* calls and gb_overlap refuse it with GB_ERR_INVALID_ARGUMENT
+ *      before any launch, and gb_point_grid_info / _download / gb_gicp_grid_factor_create refuse every other kind.  These are
+ *      refusals of the new kind only: no call valid before changes. ---- */
+GB_API gb_status gb_point_grid_build(gb_ctx* ctx, const gb_cloud* cloud, double cell_size, gb_point_grid** out);
+GB_API gb_status gb_point_grid_info(const gb_point_grid* grid, int* num_cells, size_t* num_points, double* cell_size);
+/* cells in ascending packed-key order: cell_coords (C x 3), cell_counts (C); points in record order (the keyed ones cell-major,
+ * then those that never match): original indices (P), xyz (P x 3), cov6 (P x 6); any pointer may be NULL */
+GB_API gb_status gb_point_grid_download(const gb_point_grid* grid, int32_t* cell_coords, int32_t* cell_counts, int32_t* indices, float* xyz, float* cov6);
+GB_API gb_status gb_point_grid_destroy(gb_point_grid* grid);
+/* A GICP factor on a point grid.  GB_ERR_INVALID_ARGUMENT before any launch, creating nothing, for a non-finite or
+ * non-positive max_correspondence_distance, a target that is not a point grid, a source without covariances, a grid or
+ * source on another device than ctx, or a search half-width m above 8 (r more than about 8 cell sizes). */
+GB_API gb_status gb_gicp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out);
+/* the factor's search half-width m (0 for a factor of another kind) */
+GB_API gb_status gb_gicp_grid_factor_half_width(const gb_factor* factor, int* m);
+
 /* ---- NonlinearFactorSetGPU::add(graph) / ::linearize(values) (odometry_estimation_gpu.cpp:383-386;
  *      hook at src/glim/viewer/offline_viewer.cpp:29): F x 64 B of poses down, one launch over all
  *      factors, F records up. ---- */
@@ -241,7 +291,8 @@ GB_API gb_status gb_factor_set_error(gb_ctx* ctx, size_t num_factors, gb_factor*
  *      LevenbergMarquardtOptimizerExt; global_mapping_pose_graph.cpp:405-417: loop candidates, 10 iterations each).
  *      A problem is the set of factors (levels) that share one unknown T_target_source, the target pose fixed to identity;
  *      the factors of problem p are factors[factor_offsets[p] .. factor_offsets[p+1]).  Factors keep their flags.  The factors
- *      may be VGICP (gb_vgicp_factor_create) or GICP (gb_gicp_factor_create) factors, all of one kind per call.
+ *      may be VGICP (gb_vgicp_factor_create), GICP on iVoxes (gb_gicp_factor_create) or GICP on point grids
+ *      (gb_gicp_grid_factor_create) factors, all of one target class per call.
  *
  *      The rule (gtsam_points' LevenbergMarquardtOptimizerExt is not vendored: GTSAM's documented LM defaults plus GLIM's
  *      termination callback, DESIGN.md section 7 [EXT]).  Per problem, T = T_init, lambda = lambda_initial, need_lin = 1;
