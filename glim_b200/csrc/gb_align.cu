@@ -2,7 +2,8 @@
 //
 // Replaces the loop LevenbergMarquardtOptimizerExt runs around IntegratedVGICPFactor(Pose3(), X(current), voxelmap, frame)
 // (odometry_estimation_cpu.cpp:105-150; global_mapping_pose_graph.cpp:405-417).  The rule is stated once, in
-// include/glim_b200.h; its per-problem arithmetic lives in gb_align_math.cuh (also compiled for the host by the CPU test).
+// include/glim_b200.h; its per-problem arithmetic lives in gb_align_math.cuh (also compiled for the host by the CPU test) and
+// its round loop is gb_align_rounds (gb_internal.cuh), both shared with gb_ct_gicp_align.
 //
 // One private gb_sweep covers every factor of every problem, in CSR order.  A round is at most four launches:
 //   linearize sweep (if any problem needs a linearization) -> k_align_step -> error sweep -> k_align_accept,
@@ -26,7 +27,7 @@ constexpr int kAlignThreads = 256;  // 8 problems (one warp each) per CTA
 // them), solve, form T' and write it into the eval-pose rows of the problem's factors.  Block 0 clears the status word.
 __global__ void __launch_bounds__(kAlignThreads) k_align_step(AlignState* __restrict__ st, const int* __restrict__ off, int P, const double* __restrict__ out,
                                                                double* __restrict__ poses_eval, unsigned* __restrict__ counters) {
-  if (blockIdx.x == 0 && threadIdx.x < 2) counters[threadIdx.x] = 0u;
+  align_status_clear(counters);
   const int p = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
   if (p >= P) return;
@@ -34,13 +35,7 @@ __global__ void __launch_bounds__(kAlignThreads) k_align_step(AlignState* __rest
   if (s.status != GB_ALIGN_ACTIVE) return;
   const int f0 = off[p], f1 = off[p + 1];
   if (s.need_lin) {
-    for (int k = lane; k < GB_ALIGN_STATE_ENTRIES; k += 32) {
-      const double v = align_record_entry(out, f0, f1, k);
-      if (k < 36) s.H[k] = v;
-      else if (k < 42) s.b[k - 36] = v;
-      else if (k == 42) s.e = v;
-      else s.n = v;
-    }
+    for (int k = lane; k < GB_ALIGN_STATE_ENTRIES; k += 32) align_set_entry(s, k, align_record_entry(out, f0, f1, k));
     __syncwarp();
     int active = 0;
     if (lane == 0) {
@@ -67,9 +62,7 @@ __global__ void __launch_bounds__(kAlignThreads) k_align_accept(AlignState* __re
   int flags = 0;
   if (lane == 0) {
     align_conclude(s, prm, align_record_entry(out, f0, f1, 42));
-    flags = (s.need_lin ? 1 : 0) | (s.status == GB_ALIGN_ACTIVE ? 2 : 0);
-    if (flags & 2) atomicAdd(&counters[0], 1u);
-    if (flags == 3) atomicAdd(&counters[1], 1u);
+    flags = align_status_tally(s, counters);
   }
   flags = __shfl_sync(0xffffffffu, flags, 0);
   if (flags & 1)
@@ -148,29 +141,17 @@ extern "C" gb_status gb_vgicp_align(gb_ctx* ctx, size_t P, const size_t* off, gb
   GB_CUDA(cudaMemcpyAsync(s->d_poses_eval, h_poses, sizeof(double) * 16 * F, cudaMemcpyHostToDevice, stream));
   GB_CUDA(cudaStreamSynchronize(stream));
   const int grid = (int)((P * 32 + kAlignThreads - 1) / kAlignThreads);
-  bool need_lin = true;
-  for (;;) {
+  GB_CHECK(gb_align_rounds(ctx, d.ctr, h.ctr, [&](bool need_lin) -> gb_status {
     if (need_lin) GB_CHECK(gb_launch_sweep(s.get(), GB_MODE_LINEARIZE));
     GB_CHECK(gb_launch(ctx, "k_align_step", k_align_step, grid, kAlignThreads, 0, d.st, d.off, (int)P, s->d_out, s->d_poses_eval, d.ctr));
     GB_CHECK(gb_launch_sweep(s.get(), GB_MODE_ERROR));
-    GB_CHECK(gb_launch(ctx, "k_align_accept", k_align_accept, grid, kAlignThreads, 0, d.st, d.off, (int)P, s->d_out, s->d_poses, *prm, d.ctr));
-    GB_CUDA(cudaMemcpyAsync(h.ctr, d.ctr, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
-    GB_CUDA(cudaStreamSynchronize(stream));
-    if (h.ctr[0] == 0) break;
-    need_lin = h.ctr[1] > 0;
-  }
+    return gb_launch(ctx, "k_align_accept", k_align_accept, grid, kAlignThreads, 0, d.st, d.off, (int)P, s->d_out, s->d_poses, *prm, d.ctr);
+  }));
   GB_CUDA(cudaMemcpyAsync(h.st, d.st, sizeof(AlignState) * P, cudaMemcpyDeviceToHost, stream));
   GB_CUDA(cudaStreamSynchronize(stream));
   for (size_t p = 0; p < P; p++) {
-    const AlignState& a = h.st[p];
-    gb_align_result& r = results[p];
-    memcpy(r.T_target_source, a.T, sizeof(double) * 16);
-    r.error = a.e;
-    r.num_inliers = a.n;
-    r.lambda = a.lambda;
-    r.iterations = a.iterations;
-    r.trials = a.trials;
-    r.status = a.status;
+    memcpy(results[p].T_target_source, h.st[p].T, sizeof(double) * 16);
+    align_result(h.st[p], results[p]);
   }
   return GB_OK;
 }

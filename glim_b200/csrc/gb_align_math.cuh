@@ -1,9 +1,10 @@
-// gb_align_math.cuh -- the per-problem arithmetic of gb_vgicp_align (gb_align.cu): record sum, 6x6 Cholesky solve, Exp,
-// compose, step norms and the Levenberg-Marquardt accept / terminate rule of include/glim_b200.h.  Like gb_vgicp_math.cuh it
-// holds nothing that only exists on the device, so the SAME TEXT compiles for the host: tests/cpp/align_math_host.cpp builds
-// it with g++ and tests/test_align_math_host.py checks it against numpy, synth.se3_exp and the rule's restatement in
-// tests/align_oracle.py.
-// All poses are 4x4 column-major doubles; tangent order [rot; trans] (GTSAM Pose3, SURVEY A.3).
+// gb_align_math.cuh -- the per-problem Levenberg-Marquardt arithmetic of gb_vgicp_align (gb_align.cu) and gb_ct_gicp_align
+// (gb_kernels_ct.cu): record sum, the N x N Cholesky solve, 3x3 helpers, the SE(3) Exp tail, compose, step norms, the accept /
+// terminate rule of include/glim_b200.h, the round's status word and the result fields.  Like gb_vgicp_math.cuh it holds
+// nothing that only exists on the device (the status-word helpers excepted), so the SAME TEXT compiles for the host:
+// tests/cpp/align_math_host.cpp builds it with g++ and tests/test_align_math_host.py checks it against numpy, synth.se3_exp
+// and the rule's restatement in tests/lm_oracle.py.
+// All poses are 4x4 column-major doubles; tangent order [rot; trans] (GTSAM Pose3, SURVEY A.3); square matrices are ROW-major.
 #pragma once
 #ifdef __CUDACC__
 #define GB_AHD __host__ __device__ inline
@@ -15,7 +16,7 @@
 #include "../../include/glim_b200.h"
 
 #define GB_ALIGN_ACTIVE (-1)       // status of a problem that is still iterating
-#define GB_ALIGN_STATE_ENTRIES 44  // H (36, column-major) | b (6) | error | num_inliers
+#define GB_ALIGN_STATE_ENTRIES 44  // H_ss (36, column-major in the record) | b (6) | error | num_inliers
 
 namespace {
 
@@ -23,7 +24,7 @@ namespace {
 struct AlignState {
   double T[16];      // current pose
   double Tn[16];     // trial pose T * Exp(delta)
-  double H[36];      // sum of H_ss of the last linearization (column-major)
+  double H[36];      // sum of H_ss of the last linearization (row-major)
   double b[6];       // sum of b_s
   double e;          // error: of the last linearization, then of the accepted trial pose
   double n;          // inliers of the last linearization
@@ -37,7 +38,7 @@ struct AlignState {
   int pad;
 };
 
-// entry k of the state vector (H column-major | b | error | num_inliers) summed over the records [f0, f1) of a
+// entry k of the state vector (H_ss column-major | b | error | num_inliers) summed over the records [f0, f1) of a
 // F x GB_OUT_DOUBLES (122) record array, in record order
 GB_AHD double align_record_entry(const double* out, int f0, int f1, int k) {
   const int r = k < 36 ? 36 + k : (k < 42 ? 114 + (k - 36) : 120 + (k - 42));  // H_ss | b_s | error | num_inliers
@@ -45,50 +46,62 @@ GB_AHD double align_record_entry(const double* out, int f0, int f1, int k) {
   for (int f = f0; f < f1; f++) s += out[(size_t)f * 122 + r];
   return s;
 }
+// entry k of the state vector into the state (H_ss transposed into the row-major H)
+GB_AHD void align_set_entry(AlignState& s, int k, double v) {
+  if (k < 36) s.H[(k % 6) * 6 + k / 6] = v;
+  else if (k < 42) s.b[k - 36] = v;
+  else if (k == 42) s.e = v;
+  else s.n = v;
+}
 
-// (H + lambda I) delta = -b by Cholesky (lower, row by row).  false: not positive definite (or not finite).
+// (H + lambda I) delta = -b for an N x N row-major H by Cholesky (lower, row by row; only H(i, j <= i) is read).  N is 6
+// for a pose problem (the default) and 12 for a CT problem (ct_solve12).  false: not positive definite (or not finite).
+template <int N = 6>
 GB_AHD bool align_solve(const double* H, const double* b, double lambda, double* delta) {
-  double L[36];
-  for (int i = 0; i < 6; i++) {
+  double L[N * N];
+  for (int i = 0; i < N; i++) {
     for (int j = 0; j <= i; j++) {
-      double s = H[j * 6 + i] + (i == j ? lambda : 0.0);
-      for (int k = 0; k < j; k++) s -= L[i * 6 + k] * L[j * 6 + k];
+      double s = H[i * N + j] + (i == j ? lambda : 0.0);
+      for (int k = 0; k < j; k++) s -= L[i * N + k] * L[j * N + k];
       if (i == j) {
         if (!(s > 0.0) || !(s < INFINITY)) return false;
-        L[i * 6 + i] = sqrt(s);
+        L[i * N + i] = sqrt(s);
       } else {
-        L[i * 6 + j] = s / L[j * 6 + j];
+        L[i * N + j] = s / L[j * N + j];
       }
     }
   }
-  double y[6];
-  for (int i = 0; i < 6; i++) {
+  double y[N];
+  for (int i = 0; i < N; i++) {
     double s = -b[i];
-    for (int k = 0; k < i; k++) s -= L[i * 6 + k] * y[k];
-    y[i] = s / L[i * 6 + i];
+    for (int k = 0; k < i; k++) s -= L[i * N + k] * y[k];
+    y[i] = s / L[i * N + i];
   }
-  for (int i = 5; i >= 0; i--) {
+  for (int i = N - 1; i >= 0; i--) {
     double s = y[i];
-    for (int k = i + 1; k < 6; k++) s -= L[k * 6 + i] * delta[k];
-    delta[i] = s / L[i * 6 + i];
+    for (int k = i + 1; k < N; k++) s -= L[k * N + i] * delta[k];
+    delta[i] = s / L[i * N + i];
   }
   return true;
 }
 
-// Pose3::Expmap([w; v]) as a column-major 4x4 (the formulas of synth.se3_exp)
-GB_AHD void align_exp(const double* xi, double* E) {
-  const double wx = xi[0], wy = xi[1], wz = xi[2];
-  const double th2 = wx * wx + wy * wy + wz * wz, th = sqrt(th2);
-  double a, bb, c;  // R = I + a K + bb K^2,  V = I + bb K + c K^2 (second-order series below 1e-10 rad)
-  if (th < 1e-10) {
-    a = 1.0; bb = 0.5; c = 0.0;
-  } else {
-    a = sin(th) / th; bb = (1.0 - cos(th)) / th2; c = (th - sin(th)) / (th2 * th);
-  }
-  const double K[9] = {0.0, -wz, wy, wz, 0.0, -wx, -wy, wx, 0.0};  // row-major hat(w)
-  double K2[9];
+// ---- 3x3 helpers (row-major) ----
+GB_AHD void mat3_hat(const double* w, double* K) {
+  K[0] = 0.0; K[1] = -w[2]; K[2] = w[1];
+  K[3] = w[2]; K[4] = 0.0; K[5] = -w[0];
+  K[6] = -w[1]; K[7] = w[0]; K[8] = 0.0;
+}
+GB_AHD void mat3_mul(const double* A, const double* B, double* C) {
   for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) K2[i * 3 + j] = K[i * 3 + 0] * K[0 * 3 + j] + K[i * 3 + 1] * K[1 * 3 + j] + K[i * 3 + 2] * K[2 * 3 + j];
+    for (int j = 0; j < 3; j++) C[i * 3 + j] = A[i * 3 + 0] * B[0 * 3 + j] + A[i * 3 + 1] * B[1 * 3 + j] + A[i * 3 + 2] * B[2 * 3 + j];
+}
+
+// Pose3::Expmap([w; v]) as a column-major 4x4 from its coefficients: R = I + a K + bb K^2, V = I + bb K + c K^2, t = V v
+// (K = hat(w)).  align_exp and ct_exp choose a, bb, c by their own rules.
+GB_AHD void se3_exp_coeffs(const double* xi, double a, double bb, double c, double* E) {
+  double K[9], K2[9];
+  mat3_hat(xi, K);
+  mat3_mul(K, K, K2);
   double V[9];
   for (int i = 0; i < 3; i++)
     for (int j = 0; j < 3; j++) {
@@ -101,6 +114,18 @@ GB_AHD void align_exp(const double* xi, double* E) {
     E[i * 4 + 3] = 0.0;
   }
   E[15] = 1.0;
+}
+
+// Pose3::Expmap([w; v]) as a column-major 4x4 (the formulas of synth.se3_exp; second-order series below 1e-10 rad)
+GB_AHD void align_exp(const double* xi, double* E) {
+  const double th2 = xi[0] * xi[0] + xi[1] * xi[1] + xi[2] * xi[2], th = sqrt(th2);
+  double a, bb, c;
+  if (th < 1e-10) {
+    a = 1.0; bb = 0.5; c = 0.0;
+  } else {
+    a = sin(th) / th; bb = (1.0 - cos(th)) / th2; c = (th - sin(th)) / (th2 * th);
+  }
+  se3_exp_coeffs(xi, a, bb, c, E);
 }
 
 // C = A B (column-major 4x4 rigid transforms)
@@ -168,5 +193,30 @@ GB_AHD void align_conclude(AlignState& s, const gb_align_params& P, double e_new
     if (s.lambda > P.lambda_upper_bound) s.status = GB_ALIGN_LAMBDA_EXCEEDED;
   }
 }
+
+// the result fields every solve reports (gb_align_result, gb_ct_result) from a concluded state
+template <class Result>
+GB_AHD void align_result(const AlignState& s, Result& r) {
+  r.error = s.e;
+  r.num_inliers = s.n;
+  r.lambda = s.lambda;
+  r.iterations = s.iterations;
+  r.trials = s.trials;
+  r.status = s.status;
+}
+
+#ifdef __CUDACC__
+// The status word of a round: [0] the active problems, [1] those of them that need a linearization.  Block 0 of the step
+// kernel clears it; the accept kernel tallies every problem it concludes and gets its flags back (1: need_lin, 2: active).
+__device__ __forceinline__ void align_status_clear(unsigned* ctr) {
+  if (blockIdx.x == 0 && threadIdx.x < 2) ctr[threadIdx.x] = 0u;
+}
+__device__ __forceinline__ int align_status_tally(const AlignState& s, unsigned* ctr) {
+  const int flags = (s.need_lin ? 1 : 0) | (s.status == GB_ALIGN_ACTIVE ? 2 : 0);
+  if (flags & 2) atomicAdd(&ctr[0], 1u);
+  if (flags == 3) atomicAdd(&ctr[1], 1u);
+  return flags;
+}
+#endif
 
 }  // namespace

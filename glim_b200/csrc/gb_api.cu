@@ -328,8 +328,18 @@ extern "C" gb_status gb_cloud_destroy(gb_cloud* c) {
 // ---------------------------------------------------------------------------------------------
 // factors and sweeps
 // ---------------------------------------------------------------------------------------------
+gb_factor* factor_new(gb_ctx* ctx, gb_factor_kind kind, const gb_voxelmap* target, const gb_cloud* source) {
+  gb_factor* f = new (std::nothrow) gb_factor();
+  if (!f) return nullptr;
+  f->kind = kind;
+  f->ctx = ctx; f->target = target; f->source = source; f->id = g_next_factor_id.fetch_add(1);
+  ctx_retain(ctx);
+  return f;
+}
+
 extern "C" gb_status gb_vgicp_factor_create(gb_ctx* ctx, const gb_voxelmap* target, const gb_cloud* source, int flags, gb_factor** out) {
   GB_REQUIRE(ctx && target && source && out, "null argument");
+  *out = nullptr;
   GB_REQUIRE(target->kind != GB_MAP_IVOX, "the target is an iVox: GICP factors on it come from gb_gicp_factor_create");
   GB_REQUIRE(target->kind != GB_MAP_POINTS, "the target is a point grid: GICP factors on it come from gb_gicp_grid_factor_create");
   // clouds / voxel maps may have been uploaded through another context (another module thread): device memory is shared,
@@ -337,25 +347,23 @@ extern "C" gb_status gb_vgicp_factor_create(gb_ctx* ctx, const gb_voxelmap* targ
   GB_REQUIRE(target->device == ctx->device && source->device == ctx->device, "cloud / voxel map live on another device");
   if (flags & GB_FACTOR_SURFACE_VALIDATION)
     GB_REQUIRE(source->normals != nullptr, "surface validation needs the source frame's normals on the device (PointCloudGPU::clone of a frame that has normals)");
-  gb_factor* f = new (std::nothrow) gb_factor();
+  gb_factor* f = factor_new(ctx, GB_FACTOR_POSE, target, source);
   if (!f) return GB_ERR_INTERNAL;
-  f->ctx = ctx; f->target = target; f->source = source; f->flags = flags; f->id = g_next_factor_id.fetch_add(1);
-  ctx_retain(ctx);
+  f->flags = flags;
   *out = f;
   return GB_OK;
 }
 extern "C" gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out) {
   GB_REQUIRE(ctx && target && source && out, "null argument");
+  *out = nullptr;
   GB_REQUIRE(std::isfinite(max_correspondence_distance) && max_correspondence_distance > 0.0, "max_correspondence_distance must be positive and finite");
   const gb_voxelmap* m = ivox_map(target);
   GB_REQUIRE(m->kind == GB_MAP_IVOX, "the target is not an iVox: VGICP factors on voxel maps come from gb_vgicp_factor_create");
   GB_REQUIRE(m->device == ctx->device && source->device == ctx->device, "cloud / iVox live on another device");
   GB_ENTER(ctx);
-  gb_factor* f = new (std::nothrow) gb_factor();
+  gb_factor* f = factor_new(ctx, GB_FACTOR_POSE, m, source);
   if (!f) return GB_ERR_INTERNAL;
-  f->ctx = ctx; f->target = m; f->source = source; f->id = g_next_factor_id.fetch_add(1);
   f->max_corr2 = (float)(max_correspondence_distance * max_correspondence_distance);
-  ctx_retain(ctx);
   *out = f;
   return GB_OK;
 }
@@ -372,12 +380,10 @@ extern "C" gb_status gb_gicp_grid_factor_create(gb_ctx* ctx, const gb_point_grid
   const int half_width = grid_half_width(m->inv_res, max_corr2, m->key_extent);
   GB_REQUIRE(half_width <= kGridMaxHalfWidth, "max_correspondence_distance / cell_size too large: the search would span more than 17^3 cells");
   GB_ENTER(ctx);
-  gb_factor* f = new (std::nothrow) gb_factor();
+  gb_factor* f = factor_new(ctx, GB_FACTOR_POSE, m, source);
   if (!f) return GB_ERR_INTERNAL;
-  f->ctx = ctx; f->target = m; f->source = source; f->id = g_next_factor_id.fetch_add(1);
   f->max_corr2 = max_corr2;
   f->grid_m = half_width;
-  ctx_retain(ctx);
   *out = f;
   return GB_OK;
 }
@@ -560,8 +566,7 @@ static void desc_target(FactorDesc& D, const gb_voxelmap* t) {
   D.max_scan = t->max_scan;
   D.inv_res = t->inv_res;
 }
-// a GICP factor's target part: the iVox's or point grid's table and point records in the FactorDesc, the rest in its GicpDesc
-static void desc_target_gicp(FactorDesc& D, GicpDesc& G, const gb_factor* fa) {
+void desc_target_gicp(FactorDesc& D, GicpDesc& G, const gb_factor* fa) {
   desc_target(D, fa->target);
   G.cells = fa->target->cells;
   G.max_corr2 = fa->max_corr2;

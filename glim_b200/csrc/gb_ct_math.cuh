@@ -1,12 +1,12 @@
 // gb_ct_math.cuh -- the arithmetic of the continuous-time GICP factor and its solve (gb_kernels_ct.cu): the time table of
 // gb_cloud_add_times, SE(3) Exp / Log / right Jacobian / its inverse / adjoint, the entry poses and their chain-rule blocks
-// D0 / D1, the prior and between terms of gb_ct_gicp_align, and its 12x12 Cholesky solve and trial step.  Like
+// D0 / D1, the prior and between terms of gb_ct_gicp_align, and its trial step (ct_solve12 is align_solve at 12 dof).  Like
 // gb_align_math.cuh it holds nothing that only exists on the device, so the SAME TEXT compiles for the host:
 // tests/cpp/ct_math_host.cpp builds it with g++ and tests/test_ct_host.py checks it against tests/ct_oracle.py.
 // The rule is written once, in include/glim_b200.h.  Poses are 4x4 column-major doubles, tangent order [rot; trans] with
 // perturbations on the right (GTSAM Pose3, Expmap chart); 6x6 and 12x12 matrices here are ROW-major.
 #pragma once
-#include "gb_align_math.cuh"  // GB_AHD, AlignState, align_compose, align_step_norms, align_linearized, align_conclude
+#include "gb_align_math.cuh"  // GB_AHD, AlignState, align_solve, mat3_*, se3_exp_coeffs, align_compose, align_step_norms, align_linearized, align_conclude
 
 #define GB_CT_TIME_EPS 1e-3  // s: a point opens a new time-table entry iff it is later than the entry's time by more than this
 
@@ -31,23 +31,12 @@ GB_AHD int ct_time_table(const double* times, int n, int* starts, double* tau) {
   return B;
 }
 
-// ---- 3x3 helpers (row-major) ----
-GB_AHD void ct_hat(const double* w, double* K) {
-  K[0] = 0.0; K[1] = -w[2]; K[2] = w[1];
-  K[3] = w[2]; K[4] = 0.0; K[5] = -w[0];
-  K[6] = -w[1]; K[7] = w[0]; K[8] = 0.0;
-}
-GB_AHD void ct_mul3(const double* A, const double* B, double* C) {
-  for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) C[i * 3 + j] = A[i * 3 + 0] * B[0 * 3 + j] + A[i * 3 + 1] * B[1 * 3 + j] + A[i * 3 + 2] * B[2 * 3 + j];
-}
-
 // SO(3) left Jacobian J_l(w) = I + a K + c K^2 and its inverse I - K / 2 + d K^2 (series below 1e-2 rad)
 GB_AHD void ct_so3_jl(const double* w, bool inverse, double* J) {
   const double th2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2], th = sqrt(th2);
   double K[9], K2[9];
-  ct_hat(w, K);
-  ct_mul3(K, K, K2);
+  mat3_hat(w, K);
+  mat3_mul(K, K, K2);
   double a, c;
   if (inverse) {
     a = -0.5;
@@ -81,16 +70,16 @@ GB_AHD void ct_se3_jl(const double* xi, bool inverse, double* J6) {
     c3 = (2.0 * th - 3.0 * s + th * c) / (2.0 * th2 * th2 * th);
   }
   double P[9], R[9], PR[9], RP[9], PRP[9], PP[9], PPR[9], RPP[9], PRPP[9], PPRP[9], Q[9];
-  ct_hat(w, P);
-  ct_hat(v, R);
-  ct_mul3(P, R, PR);
-  ct_mul3(R, P, RP);
-  ct_mul3(PR, P, PRP);
-  ct_mul3(P, P, PP);
-  ct_mul3(PP, R, PPR);
-  ct_mul3(RP, P, RPP);
-  ct_mul3(PRP, P, PRPP);
-  ct_mul3(P, PRP, PPRP);
+  mat3_hat(w, P);
+  mat3_hat(v, R);
+  mat3_mul(P, R, PR);
+  mat3_mul(R, P, RP);
+  mat3_mul(PR, P, PRP);
+  mat3_mul(P, P, PP);
+  mat3_mul(PP, R, PPR);
+  mat3_mul(RP, P, RPP);
+  mat3_mul(PRP, P, PRPP);
+  mat3_mul(P, PRP, PPRP);
   for (int e = 0; e < 9; e++)
     Q[e] = 0.5 * R[e] + c1 * (PR[e] + RP[e] + PRP[e]) + c2 * (PPR[e] + RPP[e] - 3.0 * PRP[e]) + c3 * (PRPP[e] + PPRP[e]);
   double J[9];
@@ -98,8 +87,8 @@ GB_AHD void ct_se3_jl(const double* xi, bool inverse, double* J6) {
   double B[9];
   if (inverse) {
     double T[9];
-    ct_mul3(J, Q, T);
-    ct_mul3(T, J, B);
+    mat3_mul(J, Q, T);
+    mat3_mul(T, J, B);
     for (int e = 0; e < 9; e++) B[e] = -B[e];
   } else {
     for (int e = 0; e < 9; e++) B[e] = Q[e];
@@ -117,12 +106,12 @@ GB_AHD void ct_se3_jr(const double* xi, bool inverse, double* J6) {
   ct_se3_jl(m, inverse, J6);
 }
 
-// Pose3::Expmap and Pose3::Logmap of a column-major rigid transform.  ct_exp is align_exp's formula with series below 1e-2 rad
-// (align_exp's closed form loses the K^2 coefficient of V at tiny angles, which the entry poses of a slow scan reach); Exp(0) is
-// exactly the identity.
+// Pose3::Expmap and Pose3::Logmap of a column-major rigid transform.  ct_exp is se3_exp_coeffs with series coefficients below
+// 1e-2 rad (align_exp's closed form loses the K^2 coefficient of V at tiny angles, which the entry poses of a slow scan reach);
+// Exp(0) is exactly the identity.
 GB_AHD void ct_exp(const double* xi, double* E) {
   const double th2 = xi[0] * xi[0] + xi[1] * xi[1] + xi[2] * xi[2], th = sqrt(th2);
-  double a, bb, c;  // R = I + a K + bb K^2,  V = I + bb K + c K^2
+  double a, bb, c;
   if (th < 1e-2) {
     a = 1.0 - th2 / 6.0 + th2 * th2 / 120.0;
     bb = 0.5 - th2 / 24.0 + th2 * th2 / 720.0;
@@ -130,21 +119,7 @@ GB_AHD void ct_exp(const double* xi, double* E) {
   } else {
     a = sin(th) / th; bb = (1.0 - cos(th)) / th2; c = (th - sin(th)) / (th2 * th);
   }
-  double K[9], K2[9];
-  ct_hat(xi, K);
-  ct_mul3(K, K, K2);
-  double V[9];
-  for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) {
-      const double I = i == j ? 1.0 : 0.0;
-      E[j * 4 + i] = I + a * K[i * 3 + j] + bb * K2[i * 3 + j];
-      V[i * 3 + j] = I + bb * K[i * 3 + j] + c * K2[i * 3 + j];
-    }
-  for (int i = 0; i < 3; i++) {
-    E[12 + i] = V[i * 3 + 0] * xi[3] + V[i * 3 + 1] * xi[4] + V[i * 3 + 2] * xi[5];
-    E[i * 4 + 3] = 0.0;
-  }
-  E[15] = 1.0;
+  se3_exp_coeffs(xi, a, bb, c, E);
 }
 GB_AHD void ct_log(const double* T, double* xi) {
   // R(i, j) = T[j * 4 + i]
@@ -199,8 +174,8 @@ GB_AHD void ct_adjoint(const double* T, double* A) {
   double R[9], K[9], KR[9];
   for (int i = 0; i < 3; i++)
     for (int j = 0; j < 3; j++) R[i * 3 + j] = T[j * 4 + i];
-  ct_hat(T + 12, K);
-  ct_mul3(K, R, KR);
+  mat3_hat(T + 12, K);
+  mat3_mul(K, R, KR);
   for (int i = 0; i < 6; i++)
     for (int j = 0; j < 6; j++) {
       const int r = i % 3, c = j % 3;
@@ -302,34 +277,8 @@ GB_AHD double ct_small_terms(const double* X, const double* Y, const double* Xp,
   return e;
 }
 
-// (H + lambda I) delta = -b, 12x12 row-major, by Cholesky (the rule of align_solve at 12 dof).  false: not positive definite.
-GB_AHD bool ct_solve12(const double* H, const double* b, double lambda, double* delta) {
-  double L[144];
-  for (int i = 0; i < 12; i++) {
-    for (int j = 0; j <= i; j++) {
-      double s = H[i * 12 + j] + (i == j ? lambda : 0.0);
-      for (int k = 0; k < j; k++) s -= L[i * 12 + k] * L[j * 12 + k];
-      if (i == j) {
-        if (!(s > 0.0) || !(s < INFINITY)) return false;
-        L[i * 12 + i] = sqrt(s);
-      } else {
-        L[i * 12 + j] = s / L[j * 12 + j];
-      }
-    }
-  }
-  double y[12];
-  for (int i = 0; i < 12; i++) {
-    double s = -b[i];
-    for (int k = 0; k < i; k++) s -= L[i * 12 + k] * y[k];
-    y[i] = s / L[i * 12 + i];
-  }
-  for (int i = 11; i >= 0; i--) {
-    double s = y[i];
-    for (int k = i + 1; k < 12; k++) s -= L[k * 12 + i] * delta[k];
-    delta[i] = s / L[i * 12 + i];
-  }
-  return true;
-}
+// the 12x12 solve of a CT problem over [X; Y] (row-major H): align_solve at 12 dof
+GB_AHD bool ct_solve12(const double* H, const double* b, double lambda, double* delta) { return align_solve<12>(H, b, lambda, delta); }
 
 // Everything gb_ct_gicp_align keeps for one problem.  The accept / terminate rule is gb_vgicp_align's (align_conclude on
 // `a`): a.T / a.Tn hold X and its trial, Y / Yn the scan-end pose and its trial; a.H and a.b are unused.

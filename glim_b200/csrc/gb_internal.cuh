@@ -151,6 +151,8 @@ struct GicpDesc {
   int num_offsets;   // neighbor_voxel_mode (iVox), or the search half-width m (point grid)
 };
 static_assert(sizeof(GicpDesc) == 16, "GicpDesc size");
+// a GICP factor's target part (gb_api.cu): the iVox's or point grid's table and point records in D, the rest in G
+void desc_target_gicp(FactorDesc& D, GicpDesc& G, const gb_factor* fa);
 
 // A factor is one of two kinds, fixed at creation.  A pose factor (gb_vgicp_factor_create, gb_gicp_factor_create) has one
 // unknown pose and goes through sweeps; a CT factor (gb_ct_gicp_factor_create) has two and only the gb_ct_* entry points
@@ -324,6 +326,21 @@ void gb_dev_free(int device, void* p);
 gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes);  // a.base holds at least `bytes` afterwards
 // the parameter bounds of gb_vgicp_align (gb_align.cu), shared by gb_ct_gicp_align
 gb_status gb_align_params_check(const gb_align_params* prm);
+// The round loop of gb_vgicp_align and gb_ct_gicp_align.  round(need_lin) launches one round for every problem: the
+// linearize sweep when need_lin, the step kernel, the error sweep and the accept kernel, which leave the status word (active
+// problems | those that need a linearization) in d_ctr.  After each round one 8-byte copy of it into h_ctr (pinned) and a
+// stream sync; the loop ends when no problem is active.
+template <typename Round>
+gb_status gb_align_rounds(gb_ctx* ctx, const unsigned* d_ctr, unsigned* h_ctr, Round&& round) {
+  bool need_lin = true;
+  for (;;) {
+    GB_CHECK(round(need_lin));
+    GB_CUDA(cudaMemcpyAsync(h_ctr, d_ctr, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+    GB_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (h_ctr[0] == 0) return GB_OK;
+    need_lin = h_ctr[1] > 0;
+  }
+}
 
 // The one free function of each handle that owns memory (cloud_free, voxelmap_free, sweep_free, peer_slab_free,
 // ctx_release): it releases everything the handle owns, never returns early, and ends with the delete.  A creation holds
@@ -333,6 +350,9 @@ void cloud_free(gb_cloud* c);
 void sweep_free(gb_sweep* s);
 void ctx_retain(gb_ctx* ctx);
 void ctx_release(gb_ctx* ctx);
+// A new factor of `kind` on (target, source) with its context retained and a process-wide unique id; nullptr when out of
+// host memory.  Every *_factor_create calls it after its own argument checks.
+gb_factor* factor_new(gb_ctx* ctx, gb_factor_kind kind, const gb_voxelmap* target, const gb_cloud* source);
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 

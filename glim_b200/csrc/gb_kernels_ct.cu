@@ -235,7 +235,7 @@ __global__ void __launch_bounds__(kCtThreads) k_ct_step(CtState* __restrict__ st
                                                         double w_prior, double w_between, unsigned* __restrict__ counters) {
   __shared__ double sys[kCtSystem];
   __shared__ int active;
-  if (blockIdx.x == 0 && threadIdx.x < 2) counters[threadIdx.x] = 0u;
+  align_status_clear(counters);
   const int p = blockIdx.x;
   CtState& s = st[p];
   if (s.a.status != GB_ALIGN_ACTIVE) return;
@@ -270,10 +270,7 @@ __global__ void __launch_bounds__(kCtThreads) k_ct_accept(CtState* __restrict__ 
   if (threadIdx.x == 0) {
     const double e_new = sys[156] + ct_small_terms(s.a.Tn, s.Yn, s.Xp, w_prior, w_between, nullptr, nullptr);
     ct_conclude(s, prm, e_new);
-    const int flags = (s.a.need_lin ? 1 : 0) | (s.a.status == GB_ALIGN_ACTIVE ? 2 : 0);
-    if (flags & 2) atomicAdd(&counters[0], 1u);
-    if (flags == 3) atomicAdd(&counters[1], 1u);
-    if (flags & 1)
+    if (align_status_tally(s.a, counters) & 1)
       for (int k = 0; k < 16; k++) { XY[(size_t)p * 32 + k] = s.a.T[k]; XY[(size_t)p * 32 + 16 + k] = s.Y[k]; }
   }
 }
@@ -375,18 +372,11 @@ gb_status ct_prepare(gb_ctx* ctx, size_t P, gb_factor* const* factors, bool alig
   for (size_t p = 0; p < P; p++) {
     const gb_factor* fa = factors[p];
     const gb_cloud* src = fa->source;
-    const gb_voxelmap* m = fa->target;
     CtDesc& C = c.h.descs[p];
     memset(&C, 0, sizeof(C));
     C.D.p0 = src->p0; C.D.p1 = src->p1; C.D.p2 = src->p2;
-    C.D.buckets = m->buckets; C.D.voxels = m->voxels;
-    C.D.mask = (uint32_t)m->num_buckets - 1u;
-    C.D.max_scan = m->max_scan;
-    C.D.inv_res = m->inv_res;
     C.D.n = (int)src->n;
-    C.G.cells = m->cells;
-    C.G.max_corr2 = fa->max_corr2;
-    C.G.num_offsets = m->mode;
+    desc_target_gicp(C.D, C.G, fa);
     C.inv_perm = src->inv_perm;
     C.tau = src->t_tau;
     C.entry_items = c.d.entry_items + e;
@@ -512,12 +502,9 @@ extern "C" gb_status gb_ct_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target
   GB_REQUIRE(m->device == ctx->device && source->device == ctx->device, "cloud / iVox live on another device");
   GB_REQUIRE(source->num_entries > 0, "the source has no times (gb_cloud_add_times)");
   GB_ENTER(ctx);
-  gb_factor* f = new (std::nothrow) gb_factor();
+  gb_factor* f = factor_new(ctx, GB_FACTOR_CT, m, source);
   if (!f) return GB_ERR_INTERNAL;
-  f->kind = GB_FACTOR_CT;
-  f->ctx = ctx; f->target = m; f->source = source;
   f->max_corr2 = (float)(max_correspondence_distance * max_correspondence_distance);
-  ctx_retain(ctx);
   *out = f;
   return GB_OK;
 }
@@ -576,30 +563,18 @@ extern "C" gb_status gb_ct_gicp_align(gb_ctx* ctx, size_t P, gb_factor* const* f
   cudaStream_t stream = ctx->stream;
   GB_CUDA(cudaStreamSynchronize(stream));
   const double wl = prm->location_consistency_inf_scale, wc = prm->constant_velocity_inf_scale;
-  bool need_lin = true;
-  for (;;) {
+  GB_CHECK(gb_align_rounds(ctx, c.d.ctr, c.h.ctr, [&](bool need_lin) -> gb_status {
     if (need_lin) GB_CHECK(ct_launch_sweep(c, GB_MODE_LINEARIZE));
     GB_CHECK(gb_launch(ctx, "k_ct_step", k_ct_step, (int)P, kCtThreads, 0, c.d.st, c.d.descs, c.d.slots, c.d.XYe, wl, wc, c.d.ctr));
     GB_CHECK(ct_launch_sweep(c, GB_MODE_ERROR));
-    GB_CHECK(gb_launch(ctx, "k_ct_accept", k_ct_accept, (int)P, kCtThreads, 0, c.d.st, c.d.descs, c.d.slots, c.d.XY, prm->lm, wl, wc, c.d.ctr));
-    GB_CUDA(cudaMemcpyAsync(c.h.ctr, c.d.ctr, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
-    GB_CUDA(cudaStreamSynchronize(stream));
-    if (c.h.ctr[0] == 0) break;
-    need_lin = c.h.ctr[1] > 0;
-  }
+    return gb_launch(ctx, "k_ct_accept", k_ct_accept, (int)P, kCtThreads, 0, c.d.st, c.d.descs, c.d.slots, c.d.XY, prm->lm, wl, wc, c.d.ctr);
+  }));
   GB_CUDA(cudaMemcpyAsync(c.h.st, c.d.st, sizeof(CtState) * P, cudaMemcpyDeviceToHost, stream));
   GB_CUDA(cudaStreamSynchronize(stream));
   for (size_t p = 0; p < P; p++) {
-    const CtState& s = c.h.st[p];
-    gb_ct_result& r = results[p];
-    memcpy(r.X, s.a.T, sizeof(double) * 16);
-    memcpy(r.Y, s.Y, sizeof(double) * 16);
-    r.error = s.a.e;
-    r.num_inliers = s.a.n;
-    r.lambda = s.a.lambda;
-    r.iterations = s.a.iterations;
-    r.trials = s.a.trials;
-    r.status = s.a.status;
+    memcpy(results[p].X, c.h.st[p].a.T, sizeof(double) * 16);
+    memcpy(results[p].Y, c.h.st[p].Y, sizeof(double) * 16);
+    align_result(c.h.st[p].a, results[p]);
   }
   return GB_OK;
 }

@@ -455,20 +455,32 @@ class IntegratedCT_GICPFactorGPU:
             self.h = None
 
 
+def _params(p, fill, name, overrides):
+    """p as fill (a gb_*_default_params) leaves it, with the given fields replaced; the fields of a nested gb_align_params `lm`
+    may be given by name"""
+    check(fill(C.byref(p)))
+    for k, v in overrides.items():
+        if hasattr(p, "lm") and k in dict(capi.AlignParams._fields_):
+            setattr(p.lm, k, v)
+        elif k in dict(type(p)._fields_) and k != "lm":
+            setattr(p, k, v)
+        else:
+            raise capi.GlimB200Error(f"{name} has no field {k!r}")
+    return p
+
+
+def _result(r, *poses) -> dict:
+    """a gb_align_result / gb_ct_result as a dict: the named poses (4,4), then the fields the two share"""
+    out = {k: np.array(getattr(r, k)[:]).reshape(4, 4).T.copy() for k in poses}
+    out.update({"error": r.error, "num_inliers": r.num_inliers, "lambda": r.lambda_, "iterations": r.iterations, "trials": r.trials,
+                "status": r.status, "status_name": capi.ALIGN_STATUS_NAMES.get(r.status, "?")})
+    return out
+
+
 def ct_params(**overrides) -> capi.CtParams:
     """gb_ct_default_params (GLIM's shipped CT settings) with the given fields replaced; fields of gb_align_params may be
     given by name as well (max_iterations=..., ...)."""
-    p = capi.CtParams()
-    check(lib().gb_ct_default_params(C.byref(p)))
-    lm_fields = dict(capi.AlignParams._fields_)
-    for k, v in overrides.items():
-        if k in lm_fields:
-            setattr(p.lm, k, v)
-        elif k in ("location_consistency_inf_scale", "constant_velocity_inf_scale"):
-            setattr(p, k, v)
-        else:
-            raise capi.GlimB200Error(f"gb_ct_params has no field {k!r}")
-    return p
+    return _params(capi.CtParams(), lib().gb_ct_default_params, "gb_ct_params", overrides)
 
 
 def align_ct_gicp(factors: list[IntegratedCT_GICPFactorGPU], X_init, Y_init, X_prior, params=None, ctx: Context | None = None) -> list[dict]:
@@ -485,11 +497,7 @@ def align_ct_gicp(factors: list[IntegratedCT_GICPFactorGPU], X_init, Y_init, X_p
     X0, Y0, Xp = (pose16(np.asarray(a, dtype=np.float64).reshape(P, 4, 4)) for a in (X_init, Y_init, X_prior))
     res = (capi.CtResult * P)()
     check(lib().gb_ct_gicp_align(ctx.h, P, C.cast(arr, C.c_void_p), ptr(X0), ptr(Y0), ptr(Xp), C.byref(params), C.cast(res, C.c_void_p)))
-    return [{
-        "X": np.array(r.X[:]).reshape(4, 4).T.copy(), "Y": np.array(r.Y[:]).reshape(4, 4).T.copy(),
-        "error": r.error, "num_inliers": r.num_inliers, "lambda": r.lambda_,
-        "iterations": r.iterations, "trials": r.trials, "status": r.status, "status_name": capi.ALIGN_STATUS_NAMES.get(r.status, "?"),
-    } for r in res]
+    return [_result(r, "X", "Y") for r in res]
 
 
 def deskew_ct(cloud: PointCloudGPU, X, Y, neighbors, k_neighbors: int, host_outputs: bool = True, ctx: Context | None = None):
@@ -663,13 +671,7 @@ class PeerSlab:
 
 def align_params(**overrides) -> capi.AlignParams:
     """gb_align_default_params (the odometry_estimation_cpu values) with the given fields replaced."""
-    p = capi.AlignParams()
-    check(lib().gb_align_default_params(C.byref(p)))
-    for k, v in overrides.items():
-        if k not in dict(capi.AlignParams._fields_):
-            raise capi.GlimB200Error(f"gb_align_params has no field {k!r}")
-        setattr(p, k, v)
-    return p
+    return _params(capi.AlignParams(), lib().gb_align_default_params, "gb_align_params", overrides)
 
 
 def align_vgicp(problems: list[list[IntegratedVGICPFactorGPU]], T_init, params=None, ctx: Context | None = None) -> list[dict]:
@@ -691,11 +693,7 @@ def align_vgicp(problems: list[list[IntegratedVGICPFactorGPU]], T_init, params=N
     arr = (C.c_void_p * max(1, len(flat)))(*[f._handle() for f in flat])
     res = (capi.AlignResult * P)()
     check(lib().gb_vgicp_align(ctx.h, P, ptr(off), C.cast(arr, C.c_void_p), ptr(T0), C.byref(params), C.cast(res, C.c_void_p)))
-    return [{
-        "T_target_source": np.array(r.T_target_source[:]).reshape(4, 4).T.copy(),
-        "error": r.error, "num_inliers": r.num_inliers, "lambda": r.lambda_,
-        "iterations": r.iterations, "trials": r.trials, "status": r.status, "status_name": capi.ALIGN_STATUS_NAMES.get(r.status, "?"),
-    } for r in res]
+    return [_result(r, "T_target_source") for r in res]
 
 
 def overlap_gpu(voxelmaps, source: PointCloudGPU, deltas, ctx: Context | None = None) -> float:

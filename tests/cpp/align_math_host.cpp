@@ -1,7 +1,7 @@
 // Host build of gb_vgicp_align's per-problem arithmetic (glim_b200/csrc/gb_align_math.cuh -- the SAME text k_align_step /
 // k_align_accept compile) and of its round structure for one problem: linearize -> gather -> trial -> error -> conclude.
 // TEST INFRASTRUCTURE: built by tests/test_align_math_host.py with g++ and compared with numpy, synth.se3_exp and
-// tests/align_oracle.py (align_gpumap) on the CPU-only box; nothing in the product links it.
+// tests/lm_oracle.py (through tests/align_oracle.py's align_gpumap) on the CPU-only box; nothing in the product links it.
 #include <stdlib.h>
 #include <string.h>
 
@@ -43,13 +43,7 @@ extern "C" int am_align(const gb_align_params* P, int F, const double* T_init, l
   while (s.status == GB_ALIGN_ACTIVE) {
     if (s.need_lin) {
       lin(s.T, out.data());
-      for (int k = 0; k < GB_ALIGN_STATE_ENTRIES; k++) {
-        const double v = align_record_entry(out.data(), 0, F, k);
-        if (k < 36) s.H[k] = v;
-        else if (k < 42) s.b[k - 36] = v;
-        else if (k == 42) s.e = v;
-        else s.n = v;
-      }
+      for (int k = 0; k < GB_ALIGN_STATE_ENTRIES; k++) align_set_entry(s, k, align_record_entry(out.data(), 0, F, k));
       align_linearized(s);
       if (s.status != GB_ALIGN_ACTIVE) break;
     }
@@ -58,11 +52,6 @@ extern "C" int am_align(const gb_align_params* P, int F, const double* T_init, l
     align_conclude(s, *P, align_record_entry(out.data(), 0, F, 42));
   }
   memcpy(r->T_target_source, s.T, sizeof(double) * 16);
-  r->error = s.e;
-  r->num_inliers = s.n;
-  r->lambda = s.lambda;
-  r->iterations = s.iterations;
-  r->trials = s.trials;
-  r->status = s.status;
+  align_result(s, *r);
   return 0;
 }

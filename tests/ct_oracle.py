@@ -2,16 +2,15 @@
 gb_ct_gicp_align), written from the rules in include/glim_b200.h and independently of the CUDA: the time table, SE(3) Exp / Log
 (matrix exponential and logarithm), the right Jacobian as the series of the adjoint, the entry poses, the factor at the device
 layout (fp32 lookup transform and fp32-cast residual pose per entry, as tests/ivox_oracle.py; fp64 after), the two small terms
-of the objective and the Levenberg-Marquardt loop at 12 dof."""
+of the objective and the Levenberg-Marquardt problem at 12 dof (the rule is tests/lm_oracle.py's)."""
 import numpy as np
 from scipy.linalg import expm
 
 from tests import ivox_oracle as io
+from tests import lm_oracle as lm
 
 F32, F64 = np.float32, np.float64
 TIME_EPS = 1e-3
-CT_DEFAULTS = dict(max_iterations=8, lambda_initial=1e-10, lambda_factor=10.0, lambda_upper_bound=1e5, relative_error_tol=1e-5,
-                   absolute_error_tol=1e-2, step_translation_tol=0.0, step_rotation_tol=0.0)
 W_PRIOR, W_BETWEEN = 1e-3, 1e3  # config_odometry_ct.json:25-26
 
 
@@ -200,54 +199,25 @@ def small_terms(X, Y, Xp, w_prior=W_PRIOR, w_between=W_BETWEEN):
 
 def align(m, xyz, cov6, starts, tau, X0, Y0, Xp, max_corr, params=None, w_prior=W_PRIOR, w_between=W_BETWEEN):
     """gb_ct_gicp_align's rule on one problem in fp64 -> dict(X, Y, error, num_inliers, lambda, iterations, trials, status)"""
-    P = dict(CT_DEFAULTS, **(params or {}))
-    X, Y = np.asarray(X0, dtype=F64).copy(), np.asarray(Y0, dtype=F64).copy()
-    lam, need_lin, iterations, trials = P["lambda_initial"], True, 0, 0
-    H, b, e, n, corr = None, None, 0.0, 0.0, None
 
-    def result(status):
-        return {"X": X, "Y": Y, "error": e, "num_inliers": n, "lambda": lam, "iterations": iterations, "trials": trials, "status": status}
+    def lin(XY):
+        r, corr = linearize(m, xyz, cov6, starts, tau, *XY, max_corr)
+        es, Hs, bs = small_terms(*XY, Xp, w_prior, w_between)
+        return r["H"] + Hs, r["b"] + bs, r["error"] + es, r["num_inliers"], corr
 
-    while True:
-        if need_lin:
-            r, corr = linearize(m, xyz, cov6, starts, tau, X, Y, max_corr)
-            es, Hs, bs = small_terms(X, Y, Xp, w_prior, w_between)
-            H, b, e, n = r["H"] + Hs, r["b"] + bs, r["error"] + es, r["num_inliers"]
-            iterations += 1
-            need_lin = False
-            if n == 0 and iterations == 1:
-                return result(io.ALIGN_DEGENERATE)
-        trials += 1
-        A = H + lam * np.eye(12)
-        try:
-            np.linalg.cholesky(A)
-            d = np.linalg.solve(A, -b)
-            solved = bool(np.isfinite(d).all())
-        except np.linalg.LinAlgError:
-            solved = False
-        if solved:
-            EX, EY = se3_exp(d[:6]), se3_exp(d[6:])
-            Xn, Yn = X @ EX, Y @ EY
-            dt = max(np.linalg.norm(EX[:3, 3]), np.linalg.norm(EY[:3, 3]))
-            dr = max(np.linalg.norm(d[:3]), np.linalg.norm(d[6:9]))
-            e_new = linearize(m, xyz, cov6, starts, tau, Xn, Yn, max_corr, corr=corr)[0]["error"] + small_terms(Xn, Yn, Xp, w_prior, w_between)[0]
-        status = None
-        if solved and e_new < e:
-            X, Y, lam, need_lin = Xn, Yn, lam / P["lambda_factor"], True
-            de = e - e_new
-            if not (dt < 1e-10 and dr < 1e-10) and dt < P["step_translation_tol"] and dr < P["step_rotation_tol"]:
-                status = io.ALIGN_CONVERGED
-            elif de <= P["absolute_error_tol"] or de / e <= P["relative_error_tol"]:
-                status = io.ALIGN_CONVERGED
-            elif iterations >= P["max_iterations"]:
-                status = io.ALIGN_MAX_ITERATIONS
-            e = e_new
-        else:
-            lam *= P["lambda_factor"]
-            if lam > P["lambda_upper_bound"]:
-                status = io.ALIGN_LAMBDA_EXCEEDED
-        if status is not None:
-            return result(status)
+    def error(corr, XY):
+        return linearize(m, xyz, cov6, starts, tau, *XY, max_corr, corr=corr)[0]["error"] + small_terms(*XY, Xp, w_prior, w_between)[0]
+
+    def retract(XY, d):  # the step size is the larger of the two poses' steps
+        EX, EY = se3_exp(d[:6]), se3_exp(d[6:])
+        dt = max(np.linalg.norm(EX[:3, 3]), np.linalg.norm(EY[:3, 3]))
+        dr = max(np.linalg.norm(d[:3]), np.linalg.norm(d[6:9]))
+        return (XY[0] @ EX, XY[1] @ EY), dt, dr
+
+    x0 = (np.asarray(X0, dtype=F64).copy(), np.asarray(Y0, dtype=F64).copy())
+    r = lm.levenberg_marquardt(lin, error, retract, x0, dict(lm.CT_DEFAULTS, **(params or {})))
+    r["X"], r["Y"] = r.pop("x")
+    return r
 
 
 # ---------------------------------------------------------------------------------------------------------------------

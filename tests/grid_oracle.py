@@ -1,12 +1,12 @@
 """numpy restatement of the device point grid and its GICP factor (gb_point_grid_build, gb_gicp_grid_factor_create), written
 from the rules in include/glim_b200.h and independently of the CUDA: the build (fp32 keys, cell order, record order, the table
 with drop rate 0), the correspondence as a brute-force fp32 argmin over every target point with the index tie, the search
-half-width's bound, and linearize / error / Levenberg-Marquardt over them.  The per-point fp64 arithmetic is
+half-width's bound, and linearize / error over them with the Levenberg-Marquardt rule of tests/lm_oracle.py.  The per-point fp64 arithmetic is
 tests/ivox_oracle.py's (residuals, linearize), fed this module's correspondences."""
 import numpy as np
 
-from glim_b200 import synth
 from tests import ivox_oracle as io
+from tests import lm_oracle as lm
 from tests import voxelmap_oracle as vo
 
 F32, F64 = np.float32, np.float64
@@ -110,51 +110,11 @@ def error(g: PointGrid, xyz, cov6, T_lin, T_eval, max_corr):
 
 
 def align(g: PointGrid, xyz, cov6, T0, max_corr, params=None):
-    """gb_vgicp_align's rule (include/glim_b200.h) on one grid factor, in fp64, restated as tests/align_oracle.py states it.
-    -> dict(T, error, num_inliers, lambda, iterations, trials, status)"""
-    P = dict(io.ALIGN_DEFAULTS, **(params or {}))
-    T = np.asarray(T0, dtype=F64).copy()
-    lam, need_lin, iterations, trials = P["lambda_initial"], True, 0, 0
-    H, b, e, n, corr = None, None, 0.0, 0.0, None
+    """gb_vgicp_align's rule (tests/lm_oracle.py) on one grid factor, in fp64.  -> dict(T, error, num_inliers, lambda,
+    iterations, trials, status)"""
 
-    def result(status):
-        return {"T": T, "error": e, "num_inliers": n, "lambda": lam, "iterations": iterations, "trials": trials, "status": status}
+    def lin(T):
+        r, corr = linearize(g, xyz, cov6, T, max_corr)
+        return r["H_ss"], r["b_s"], r["error"], r["num_inliers"], corr
 
-    while True:
-        if need_lin:
-            r, corr = linearize(g, xyz, cov6, T, max_corr)
-            H, b, e, n = r["H_ss"], r["b_s"], r["error"], r["num_inliers"]
-            iterations += 1
-            need_lin = False
-            if n == 0 and iterations == 1:
-                return result(io.ALIGN_DEGENERATE)
-        trials += 1
-        A = H + lam * np.eye(6)
-        try:
-            np.linalg.cholesky(A)
-            delta = np.linalg.solve(A, -b)
-            solved = bool(np.isfinite(delta).all())
-        except np.linalg.LinAlgError:
-            solved = False
-        if solved:
-            E = synth.se3_exp(delta)
-            Tn = T @ E
-            dt, dr = float(np.linalg.norm(E[:3, 3])), float(np.linalg.norm(delta[:3]))
-            e_new = linearize(g, xyz, cov6, Tn, max_corr, corr=corr)[0]["error"]
-        status = None
-        if solved and e_new < e:
-            T, lam, need_lin = Tn, lam / P["lambda_factor"], True
-            de = e - e_new
-            if not (dt < 1e-10 and dr < 1e-10) and dt < P["step_translation_tol"] and dr < P["step_rotation_tol"]:
-                status = io.ALIGN_CONVERGED
-            elif de <= P["absolute_error_tol"] or de / e <= P["relative_error_tol"]:
-                status = io.ALIGN_CONVERGED
-            elif iterations >= P["max_iterations"]:
-                status = io.ALIGN_MAX_ITERATIONS
-            e = e_new
-        else:
-            lam *= P["lambda_factor"]
-            if lam > P["lambda_upper_bound"]:
-                status = io.ALIGN_LAMBDA_EXCEEDED
-        if status is not None:
-            return result(status)
+    return lm.align_pose(lin, lambda corr, Tn: linearize(g, xyz, cov6, Tn, max_corr, corr=corr)[0]["error"], T0, params)

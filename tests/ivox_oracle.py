@@ -2,10 +2,10 @@
 include/glim_b200.h and independently of the CUDA: the insert (sampling, fp64 transform and keys as tests/voxelmap_oracle.py,
 sequential admission with fp32 storage, stamps, LRU eviction, ascending-key numbering, the table with drop rate 0), the
 correspondence search in fp32 (np.float32 wherever the device is fp32), an fp64 GICP linearize / error, and the
-Levenberg-Marquardt loop of gb_vgicp_align over them (restated like tests/align_oracle.py)."""
+Levenberg-Marquardt problem of gb_vgicp_align over them (the rule is tests/lm_oracle.py's)."""
 import numpy as np
 
-from glim_b200 import synth
+from tests import lm_oracle as lm
 from tests import voxelmap_oracle as vo
 
 F32, F64 = np.float32, np.float64
@@ -244,57 +244,12 @@ def error(m: IVox, xyz, cov6, T_lin, T_eval, max_corr):
     return linearize(m, xyz, cov6, T_eval, max_corr, corr=corr)[0]["error"]
 
 
-ALIGN_CONVERGED, ALIGN_MAX_ITERATIONS, ALIGN_LAMBDA_EXCEEDED, ALIGN_DEGENERATE = 0, 1, 2, 3
-ALIGN_DEFAULTS = dict(max_iterations=8, lambda_initial=1e-5, lambda_factor=10.0, lambda_upper_bound=1e5, relative_error_tol=1e-5,
-                      absolute_error_tol=0.1, step_translation_tol=1e-3, step_rotation_tol=1e-3 * np.pi / 180.0)
-
-
 def align(m: IVox, xyz, cov6, T0, max_corr, params=None):
-    """gb_vgicp_align's rule (include/glim_b200.h) on one GICP factor, in fp64.  -> dict(T, error, num_inliers, lambda,
+    """gb_vgicp_align's rule (tests/lm_oracle.py) on one GICP factor, in fp64.  -> dict(T, error, num_inliers, lambda,
     iterations, trials, status)"""
-    P = dict(ALIGN_DEFAULTS, **(params or {}))
-    T = np.asarray(T0, dtype=F64).copy()
-    lam, need_lin, iterations, trials = P["lambda_initial"], True, 0, 0
-    H, b, e, n, corr = None, None, 0.0, 0.0, None
 
-    def result(status):
-        return {"T": T, "error": e, "num_inliers": n, "lambda": lam, "iterations": iterations, "trials": trials, "status": status}
+    def lin(T):
+        r, corr = linearize(m, xyz, cov6, T, max_corr)
+        return r["H_ss"], r["b_s"], r["error"], r["num_inliers"], corr
 
-    while True:
-        if need_lin:
-            r, corr = linearize(m, xyz, cov6, T, max_corr)
-            H, b, e, n = r["H_ss"], r["b_s"], r["error"], r["num_inliers"]
-            iterations += 1
-            need_lin = False
-            if n == 0 and iterations == 1:
-                return result(ALIGN_DEGENERATE)
-        trials += 1
-        A = H + lam * np.eye(6)
-        try:
-            np.linalg.cholesky(A)
-            delta = np.linalg.solve(A, -b)
-            solved = bool(np.isfinite(delta).all())
-        except np.linalg.LinAlgError:
-            solved = False
-        if solved:
-            E = synth.se3_exp(delta)
-            Tn = T @ E
-            dt, dr = float(np.linalg.norm(E[:3, 3])), float(np.linalg.norm(delta[:3]))
-            e_new = linearize(m, xyz, cov6, Tn, max_corr, corr=corr)[0]["error"]
-        status = None
-        if solved and e_new < e:
-            T, lam, need_lin = Tn, lam / P["lambda_factor"], True
-            de = e - e_new
-            if not (dt < 1e-10 and dr < 1e-10) and dt < P["step_translation_tol"] and dr < P["step_rotation_tol"]:
-                status = ALIGN_CONVERGED
-            elif de <= P["absolute_error_tol"] or de / e <= P["relative_error_tol"]:
-                status = ALIGN_CONVERGED
-            elif iterations >= P["max_iterations"]:
-                status = ALIGN_MAX_ITERATIONS
-            e = e_new
-        else:
-            lam *= P["lambda_factor"]
-            if lam > P["lambda_upper_bound"]:
-                status = ALIGN_LAMBDA_EXCEEDED
-        if status is not None:
-            return result(status)
+    return lm.align_pose(lin, lambda corr, Tn: linearize(m, xyz, cov6, Tn, max_corr, corr=corr)[0]["error"], T0, params)

@@ -8,6 +8,7 @@ import pytest
 from glim_b200 import capi, gpu, synth, workloads
 from oracle import oracle
 from tests import align_oracle
+from tests import lm_oracle as lm
 from tests.util import cov_colmajor16, scan_pair
 
 pytestmark = pytest.mark.gpu
@@ -73,7 +74,7 @@ def test_one_iteration_matches_oracle(scene):
     ref = scene.oracle(T0, params={"max_iterations": 1})
     et, er = pose_error(got["T_target_source"], ref["T"])
     assert et < 1e-4 and er < 1e-5, (et, er)
-    assert (got["iterations"], got["trials"], got["status"]) == (ref["iterations"], ref["trials"], ref["status"]) == (1, 1, align_oracle.ALIGN_MAX_ITERATIONS)
+    assert (got["iterations"], got["trials"], got["status"]) == (ref["iterations"], ref["trials"], ref["status"]) == (1, 1, lm.ALIGN_MAX_ITERATIONS)
     assert got["num_inliers"] == ref["num_inliers"]
 
 
@@ -88,7 +89,7 @@ def test_full_run_matches_oracle_and_ground_truth(scene, monkeypatch, kernel):
         assert et < 2e-3 and er < 2e-3, (seed, et, er, got, ref)
         gt, gr = pose_error(got["T_target_source"], scene.T_gt)
         assert gt < 0.03 and gr < 2e-3, (seed, gt, gr)
-        assert got["status"] == ref["status"] == align_oracle.ALIGN_CONVERGED, (seed, got, ref)
+        assert got["status"] == ref["status"] == lm.ALIGN_CONVERGED, (seed, got, ref)
         assert got["iterations"] <= 8
 
 

@@ -3,7 +3,7 @@
 glim_b200/csrc/gb_align_math.cuh holds the text k_align_step / k_align_accept compile for the device (record sum, 6x6 Cholesky
 solve, Exp, compose, step norms, the accept / terminate rule).  Here the SAME text is compiled for the host with g++
 (tests/cpp/align_math_host.cpp) and checked against numpy, synth.se3_exp and the rule's independent restatement
-in tests/align_oracle.py (on the CPU oracle) -- so a change to the rule or its arithmetic is caught on the CPU-only box before the GPU tests run.
+in tests/lm_oracle.py (on the CPU oracle, through tests/align_oracle.py) -- so a change to the rule or its arithmetic is caught on the CPU-only box before the GPU tests run.
 """
 import ctypes as C
 import os
@@ -15,6 +15,7 @@ import pytest
 from glim_b200 import capi, synth
 from oracle import oracle
 from tests import align_oracle
+from tests import lm_oracle as lm
 from tests.util import cov_colmajor16, scan_pair
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -44,7 +45,7 @@ def _p(a):
 
 def params(**kw):
     p = capi.AlignParams()
-    for k, v in dict(align_oracle.ALIGN_DEFAULTS, **kw).items():
+    for k, v in dict(lm.ALIGN_DEFAULTS, **kw).items():
         setattr(p, k, v)
     return p
 
@@ -52,7 +53,7 @@ def params(**kw):
 def test_default_params_are_the_odometry_cpu_values():
     p = capi.AlignParams()
     assert capi.lib().gb_align_default_params(C.byref(p)) == 0  # host only: no device needed
-    for k, v in align_oracle.ALIGN_DEFAULTS.items():
+    for k, v in lm.ALIGN_DEFAULTS.items():
         assert getattr(p, k) == v, k
     assert capi.lib().gb_align_default_params(None) == 1
 
@@ -65,13 +66,13 @@ def test_cholesky_solve_matches_numpy(am):
         b = rng.normal(size=6) * 10.0 ** rng.uniform(-3, 3)
         lam = 10.0 ** rng.uniform(-8, 2)
         d = np.zeros(6)
-        assert am.am_solve(_p(np.asfortranarray(H).ravel(order="F")), _p(b), lam, _p(d)) == 1
+        assert am.am_solve(_p(np.ascontiguousarray(H).ravel()), _p(b), lam, _p(d)) == 1
         ref = np.linalg.solve(H + lam * np.eye(6), -b)
         assert np.linalg.norm(d - ref) <= 1e-14 * np.linalg.cond(H + lam * np.eye(6)) * np.linalg.norm(ref)
     # not positive definite (lambda = 0 on a rank-deficient H, or an indefinite H), or NaN: the trial is rejected
     v = rng.normal(size=(6, 1))
     for H, lam in ((v @ v.T, 0.0), (-np.eye(6), 1e-5), (np.full((6, 6), np.nan), 1.0)):
-        assert am.am_solve(_p(np.ascontiguousarray(H.T).ravel()), _p(np.ones(6)), lam, _p(np.zeros(6))) == 0
+        assert am.am_solve(_p(np.ascontiguousarray(H).ravel()), _p(np.ones(6)), lam, _p(np.zeros(6))) == 0
 
 
 def test_exp_compose_and_step_norms_match_synth(am):
@@ -95,21 +96,21 @@ def test_exp_compose_and_step_norms_match_synth(am):
 TOL_R = 1e-3 * np.pi / 180.0
 DECISIONS = [
     ("accept, keep going", {}, 1, 100.0, 50.0, 0.1, 0.01, 1, 1e-5, ACTIVE, 1, 1e-6, 50.0),
-    ("accept, small step converges", {}, 1, 100.0, 50.0, 5e-4, 0.5 * TOL_R, 1, 1e-5, align_oracle.ALIGN_CONVERGED, 1, 1e-6, 50.0),
+    ("accept, small step converges", {}, 1, 100.0, 50.0, 5e-4, 0.5 * TOL_R, 1, 1e-5, lm.ALIGN_CONVERGED, 1, 1e-6, 50.0),
     ("accept, small translation but large rotation", {}, 1, 100.0, 50.0, 5e-4, 2 * TOL_R, 1, 1e-5, ACTIVE, 1, 1e-6, 50.0),
     ("accept, step under 1e-10 does not count", {}, 1, 100.0, 50.0, 1e-11, 1e-11, 1, 1e-5, ACTIVE, 1, 1e-6, 50.0),
-    ("accept, only the translation under 1e-10 still counts", {}, 1, 100.0, 50.0, 1e-11, 0.5 * TOL_R, 1, 1e-5, align_oracle.ALIGN_CONVERGED, 1, 1e-6, 50.0),
+    ("accept, only the translation under 1e-10 still counts", {}, 1, 100.0, 50.0, 1e-11, 0.5 * TOL_R, 1, 1e-5, lm.ALIGN_CONVERGED, 1, 1e-6, 50.0),
     ("accept, step test off", dict(step_translation_tol=0.0, step_rotation_tol=0.0), 1, 100.0, 50.0, 5e-4, 0.5 * TOL_R, 1, 1e-5, ACTIVE, 1, 1e-6, 50.0),
-    ("accept, absolute decrease", {}, 1, 100.0, 99.95, 0.1, 0.01, 1, 1e-5, align_oracle.ALIGN_CONVERGED, 1, 1e-6, 99.95),
-    ("accept, absolute decrease at the bound", dict(absolute_error_tol=0.5), 1, 100.0, 99.5, 0.1, 0.01, 1, 1e-5, align_oracle.ALIGN_CONVERGED, 1, 1e-6, 99.5),
-    ("accept, relative decrease", dict(absolute_error_tol=0.0), 1, 1e9, 1e9 - 1e3, 0.1, 0.01, 1, 1e-5, align_oracle.ALIGN_CONVERGED, 1, 1e-6, 1e9 - 1e3),
-    ("accept, last iteration", dict(max_iterations=3), 1, 100.0, 50.0, 0.1, 0.01, 3, 1e-5, align_oracle.ALIGN_MAX_ITERATIONS, 1, 1e-6, 50.0),
-    ("accept, convergence wins over the last iteration", dict(max_iterations=3), 1, 100.0, 99.99, 0.1, 0.01, 3, 1e-5, align_oracle.ALIGN_CONVERGED, 1, 1e-6, 99.99),
+    ("accept, absolute decrease", {}, 1, 100.0, 99.95, 0.1, 0.01, 1, 1e-5, lm.ALIGN_CONVERGED, 1, 1e-6, 99.95),
+    ("accept, absolute decrease at the bound", dict(absolute_error_tol=0.5), 1, 100.0, 99.5, 0.1, 0.01, 1, 1e-5, lm.ALIGN_CONVERGED, 1, 1e-6, 99.5),
+    ("accept, relative decrease", dict(absolute_error_tol=0.0), 1, 1e9, 1e9 - 1e3, 0.1, 0.01, 1, 1e-5, lm.ALIGN_CONVERGED, 1, 1e-6, 1e9 - 1e3),
+    ("accept, last iteration", dict(max_iterations=3), 1, 100.0, 50.0, 0.1, 0.01, 3, 1e-5, lm.ALIGN_MAX_ITERATIONS, 1, 1e-6, 50.0),
+    ("accept, convergence wins over the last iteration", dict(max_iterations=3), 1, 100.0, 99.99, 0.1, 0.01, 3, 1e-5, lm.ALIGN_CONVERGED, 1, 1e-6, 99.99),
     ("reject, equal error", {}, 1, 100.0, 100.0, 0.1, 0.01, 1, 1e-5, ACTIVE, 0, 1e-4, 100.0),
     ("reject, larger error", {}, 1, 100.0, 200.0, 0.1, 0.01, 5, 1e-5, ACTIVE, 0, 1e-4, 100.0),
     ("reject, failed factorization", {}, 0, 100.0, 0.0, 0.0, 0.0, 1, 1e-5, ACTIVE, 0, 1e-4, 100.0),
     ("reject at the lambda bound", {}, 1, 100.0, 200.0, 0.1, 0.01, 1, 1e4, ACTIVE, 0, 1e5, 100.0),
-    ("reject over the lambda bound", {}, 1, 100.0, 200.0, 0.1, 0.01, 1, 1e5, align_oracle.ALIGN_LAMBDA_EXCEEDED, 0, 1e6, 100.0),
+    ("reject over the lambda bound", {}, 1, 100.0, 200.0, 0.1, 0.01, 1, 1e5, lm.ALIGN_LAMBDA_EXCEEDED, 0, 1e6, 100.0),
 ]
 
 
@@ -175,9 +176,9 @@ def test_oracle_registers_the_scan_pair(problem):
         r = align_oracle.align_gpumap(maps, xyz1, cov1, T0)
         et, er = pose_error(r["T"], T_gt)
         assert r["iterations"] <= 8 and et < 0.03 and er < 2e-3, (seed, et, er, r)
-        assert r["status"] in (align_oracle.ALIGN_CONVERGED, align_oracle.ALIGN_LAMBDA_EXCEEDED), r
+        assert r["status"] in (lm.ALIGN_CONVERGED, lm.ALIGN_LAMBDA_EXCEEDED), r
         statuses.append(r["status"])
-    assert statuses.count(align_oracle.ALIGN_CONVERGED) >= 3, statuses
+    assert statuses.count(lm.ALIGN_CONVERGED) >= 3, statuses
 
 
 @pytest.mark.parametrize("case", ["default", "one_iteration", "one_level", "surface_validation", "no_step_test", "degenerate", "lambda_bound"])
@@ -205,6 +206,6 @@ def test_host_state_machine_takes_the_oracles_decisions(am, problem, case):
     assert got["num_inliers"] == ref["num_inliers"]
     assert abs(got["error"] - ref["error"]) <= 1e-9 * max(ref["error"], 1.0)
     if case == "degenerate":
-        assert ref["status"] == align_oracle.ALIGN_DEGENERATE and np.array_equal(got["T"], T0) and got["trials"] == 0
+        assert ref["status"] == lm.ALIGN_DEGENERATE and np.array_equal(got["T"], T0) and got["trials"] == 0
     if case == "one_iteration":
         assert ref["iterations"] == 1

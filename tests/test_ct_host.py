@@ -14,6 +14,7 @@ import pytest
 from glim_b200 import capi, synth
 from oracle import oracle
 from tests import ct_oracle as co
+from tests import lm_oracle as lm
 from tests import ivox_oracle as io
 from tests import voxelmap_oracle as vo
 from tests.util import cov_colmajor16
@@ -216,7 +217,7 @@ def test_cholesky_12_matches_numpy(cm):
 def test_default_params_are_the_shipped_ct_values():
     p = capi.CtParams()
     assert capi.lib().gb_ct_default_params(C.byref(p)) == 0  # host only: no device needed
-    for k, v in co.CT_DEFAULTS.items():
+    for k, v in lm.CT_DEFAULTS.items():
         assert getattr(p.lm, k) == v, k
     assert (p.location_consistency_inf_scale, p.constant_velocity_inf_scale) == (co.W_PRIOR, co.W_BETWEEN)
     assert capi.lib().gb_ct_default_params(None) == 1
