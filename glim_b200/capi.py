@@ -33,6 +33,7 @@ SYMBOLS = [
     "gb_ct_default_params", "gb_ct_gicp_align", "gb_ct_deskew",
     "gb_point_grid_build", "gb_point_grid_info", "gb_point_grid_download", "gb_point_grid_destroy", "gb_gicp_grid_factor_create",
     "gb_gicp_grid_factor_half_width",
+    "gb_cloud_estimate_fpfh", "gb_cloud_fpfh", "gb_fpfh_match", "gb_ransac_default_params", "gb_ransac_align",
 ]
 
 GB_SLAB_STRIDE = 96
@@ -80,6 +81,22 @@ class CtResult(C.Structure):
     _fields_ = [("X", C.c_double * 16), ("Y", C.c_double * 16), ("error", C.c_double), ("num_inliers", C.c_double), ("lambda_", C.c_double),
                 ("iterations", C.c_int), ("trials", C.c_int), ("status", C.c_int)]
 
+
+class RansacParams(C.Structure):
+    """gb_ransac_params (include/glim_b200.h)."""
+    _fields_ = [("max_iterations", C.c_int), ("early_stop_inlier_rate", C.c_double), ("inlier_voxel_resolution", C.c_double), ("dof", C.c_int), ("seed", C.c_uint64)]
+
+
+class RansacResult(C.Structure):
+    """gb_ransac_result (include/glim_b200.h)."""
+    _fields_ = [("T_target_source", C.c_double * 16), ("inlier_rate", C.c_double), ("inliers", C.c_int), ("best_hypothesis", C.c_int), ("evaluated", C.c_int),
+                ("status", C.c_int)]
+
+
+# gb_ransac_result::status
+RANSAC_FOUND, RANSAC_EARLY_STOP, RANSAC_DEGENERATE = 0, 1, 2
+RANSAC_STATUS_NAMES = {0: "FOUND", 1: "EARLY_STOP", 2: "DEGENERATE"}
+FPFH_DIM = 33
 
 # gb_align_result::status
 ALIGN_CONVERGED, ALIGN_MAX_ITERATIONS, ALIGN_LAMBDA_EXCEEDED, ALIGN_DEGENERATE = 0, 1, 2, 3
@@ -178,6 +195,11 @@ def lib():
     L.gb_point_grid_destroy.argtypes = [vp]
     L.gb_gicp_grid_factor_create.argtypes = [vp, vp, vp, f64, vp]
     L.gb_gicp_grid_factor_half_width.argtypes = [vp, vp]
+    L.gb_cloud_estimate_fpfh.argtypes = [vp, vp, f64]
+    L.gb_cloud_fpfh.argtypes = [vp, vp]
+    L.gb_fpfh_match.argtypes = [vp, vp, vp, vp]
+    L.gb_ransac_default_params.argtypes = [vp]
+    L.gb_ransac_align.argtypes = [vp, vp, vp, vp, vp, vp]
     for name in SYMBOLS:
         getattr(L, name)  # AttributeError here means the library and include/glim_b200.h are out of sync
     _lib = L

@@ -221,6 +221,7 @@ gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes) {
 void cloud_free(gb_cloud* c) {
   gb_dev_free(c->device, c->base);  // waits for every stream that may still read the cloud, then recycles the block
   gb_dev_free(c->device, c->t_base);
+  gb_dev_free(c->device, c->f_base);
   delete c;
 }
 

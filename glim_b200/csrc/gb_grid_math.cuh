@@ -80,4 +80,29 @@ GB_HD int grid_nearest(const int4* __restrict__ buckets, uint32_t mask, int max_
   return best;
 }
 
+// Every stored point p with fp32 d2(p, q) < max_d2 (d2 as in grid_nearest): visit(record) for each, cells in offset order and
+// the points of a cell in ascending original index.  With m from grid_half_width this is exactly the brute-force set (the proof
+// above bounds every such point, not only the nearest).  The FPFH neighbourhood of gb_cloud_estimate_fpfh.
+template <typename Visit>
+GB_HD void grid_within(const int4* __restrict__ buckets, uint32_t mask, int max_scan, const int2* __restrict__ cells, const float4* __restrict__ points,
+                       int m, float inv, float max_d2, float qx, float qy, float qz, Visit&& visit) {
+  const int cx = gb_coord(qx, inv), cy = gb_coord(qy, inv), cz = gb_coord(qz, inv);
+  for (int ox = -m; ox <= m; ox++) {
+    for (int oy = -m; oy <= m; oy++) {
+      for (int oz = -m; oz <= m; oz++) {
+        const int v = ivox_find(buckets, mask, max_scan, (int)((uint32_t)cx + (uint32_t)ox), (int)((uint32_t)cy + (uint32_t)oy), (int)((uint32_t)cz + (uint32_t)oz));
+        if (v < 0) continue;
+        const int2 c = cells[v];
+        for (int s = 0; s < c.y; s++) {
+          const int r = c.x + s;
+          const float4 p = points[3 * (size_t)r];
+          const float ex = __fsub_rn(p.x, qx), ey = __fsub_rn(p.y, qy), ez = __fsub_rn(p.z, qz);
+          const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
+          if (d2 < max_d2) visit(r);
+        }
+      }
+    }
+  }
+}
+
 }  // namespace

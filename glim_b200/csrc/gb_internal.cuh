@@ -68,6 +68,10 @@ struct gb_cloud {
   double* t_tau = nullptr;
   void* t_base = nullptr;
   bool covs = false;  // the cloud carries covariances (an upload with cov4x4, a preprocessed, merged or deskewed frame)
+  // The FPFH features of gb_cloud_estimate_fpfh (gb_kernels_global.cu), or none (fpfh == nullptr): N x 33 fp32 in the caller's
+  // point order, one block of their own from the device pool; only the global registration entry points read them.
+  float* fpfh = nullptr;
+  void* f_base = nullptr;
 };
 
 // A map is one of four kinds, fixed at creation.  Every entry point that takes a map checks the kind it accepts.
@@ -489,14 +493,6 @@ __device__ __forceinline__ void gb_unpack_key(unsigned long long key, int& x, in
   x = (int)((key >> 42) & 0x1FFFFF) - GB_KEY_OFFSET;
   y = (int)((key >> 21) & 0x1FFFFF) - GB_KEY_OFFSET;
   z = (int)(key & 0x1FFFFF) - GB_KEY_OFFSET;
-}
-// the project's fixed pseudo-random pick ([EXT]: the reference draws with std::mt19937): the points / voxels with the smallest
-// rg_hash(seed, index) are kept (random-grid downsampling, frame-merge thinning, voxel-map insert sampling; the oracle shares it)
-__device__ __forceinline__ unsigned long long rg_hash(unsigned long long seed, unsigned i) {
-  unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(i + 1u);
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
 }
 // 21 bits -> every third bit (Morton interleaving)
 __device__ __forceinline__ unsigned long long gb_spread21(unsigned long long v) {

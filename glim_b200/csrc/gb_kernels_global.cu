@@ -1,0 +1,361 @@
+// gb_kernels_global.cu -- global registration on the device (sm_90a): FPFH features of a cloud (gb_cloud_estimate_fpfh), exact
+// feature matching (gb_fpfh_match) and RANSAC pose hypotheses (gb_ransac_align), the pieces of GLIM's manual loop closure
+// (ManualLoopCloseModal::align_global, manual_loop_close_modal.cpp:370-468) that run without an initial guess.  The rules are
+// written once in include/glim_b200.h; the per-pair and per-hypothesis arithmetic is gb_global_math.cuh, which the host test
+// build compiles as well.
+//
+//   gb_cloud_estimate_fpfh  a point grid of the cloud (gb_point_grid_build, cell 1.05 r), then k_fpfh_spfh (every point's SPFH,
+//                           fp64, in scratch) and k_fpfh_final (the weighted sum of the neighbours' SPFH plus the own, stored
+//                           fp32): the grid build's launches + 2.  Neighbour lists are never stored.
+//   gb_fpfh_match           k_fpfh_match: one launch.
+//   gb_ransac_align         a point grid of the target at the inlier resolution, the match, then per wave of kRansacWave
+//                           hypotheses k_ransac_pose and k_ransac_score and one copy of the wave's counts; the host applies the
+//                           selection rule and stops after the wave that holds the first hypothesis to reach the early-stop rate.
+#include "gb_internal.cuh"
+#include "gb_global_math.cuh"
+
+#include <cmath>
+#include <cstring>
+#include <new>
+#include <vector>
+
+namespace {
+
+constexpr int kFpfhThreads = 128;
+constexpr int kMatchThreads = 128;
+constexpr int kMatchTile = 128;     // target features per shared-memory tile
+constexpr int kMatchStride = 36;    // floats per staged feature: 33 padded to whole float4s
+constexpr int kRansacWave = 512;    // hypotheses per wave (include/glim_b200.h states it: `evaluated` depends on it)
+constexpr int kScoreThreads = 256;
+constexpr int kScorePerThread = 4;
+
+// the point grid of a cloud and the radius search over it
+struct FpfhGrid {
+  const int4* buckets;
+  const int2* cells;
+  const float4* points;
+  uint32_t mask;
+  int max_scan, m;
+  float inv, max_d2;
+};
+
+__device__ __forceinline__ void load3(const float4 p, double* x) { x[0] = p.x; x[1] = p.y; x[2] = p.z; }
+
+// one thread per grid record: the SPFH of the record's point, cnt_b * (100 / K) for the K neighbours, into spfh (caller order)
+__global__ void __launch_bounds__(kFpfhThreads) k_fpfh_spfh(int n, FpfhGrid G, const float4* __restrict__ normals, const int* __restrict__ inv_perm,
+                                                            double* __restrict__ spfh) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const float4 a = G.points[3 * (size_t)r];
+  const int i = grid_record_index(G.points, r);
+  double ps[3], ns[3];
+  load3(a, ps);
+  load3(normals[inv_perm ? inv_perm[i] : i], ns);
+  int cnt[kFpfhDim];
+#pragma unroll
+  for (int b = 0; b < kFpfhDim; b++) cnt[b] = 0;
+  int K = 0;
+  grid_within(G.buckets, G.mask, G.max_scan, G.cells, G.points, G.m, G.inv, G.max_d2, a.x, a.y, a.z, [&](int q) {
+    const int j = grid_record_index(G.points, q);
+    if (j == i) return;
+    double pt[3], nt[3], f[3];
+    load3(G.points[3 * (size_t)q], pt);
+    load3(normals[inv_perm ? inv_perm[j] : j], nt);
+    fpfh_pair(ps, ns, pt, nt, f);
+    int bins[3];
+    fpfh_bins(f, bins);
+    cnt[bins[0]]++;
+    cnt[bins[1]]++;
+    cnt[bins[2]]++;
+    K++;
+  });
+  const double inc = K > 0 ? 100.0 / (double)K : 0.0;
+  double* out = spfh + (size_t)i * kFpfhDim;
+#pragma unroll
+  for (int b = 0; b < kFpfhDim; b++) out[b] = __dmul_rn((double)cnt[b], inc);
+}
+
+// one thread per grid record: FPFH_b = (sum_j SPFH_j,b / d2_ij) * 100 / (its block's sum) + SPFH_i,b, fp64, stored fp32
+__global__ void __launch_bounds__(kFpfhThreads) k_fpfh_final(int n, FpfhGrid G, const double* __restrict__ spfh, float* __restrict__ fpfh) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const float4 a = G.points[3 * (size_t)r];
+  const int i = grid_record_index(G.points, r);
+  double ps[3];
+  load3(a, ps);
+  double acc[kFpfhDim], sum[3] = {0.0, 0.0, 0.0};
+#pragma unroll
+  for (int b = 0; b < kFpfhDim; b++) acc[b] = 0.0;
+  grid_within(G.buckets, G.mask, G.max_scan, G.cells, G.points, G.m, G.inv, G.max_d2, a.x, a.y, a.z, [&](int q) {
+    const int j = grid_record_index(G.points, q);
+    if (j == i) return;
+    double pt[3];
+    load3(G.points[3 * (size_t)q], pt);
+    const double d[3] = {__dsub_rn(pt[0], ps[0]), __dsub_rn(pt[1], ps[1]), __dsub_rn(pt[2], ps[2])};
+    const double dd = dot3(d, d);
+    if (dd == 0.0) return;
+    const double* sj = spfh + (size_t)j * kFpfhDim;
+#pragma unroll
+    for (int b = 0; b < kFpfhDim; b++) {
+      const double v = sj[b] / dd;
+      acc[b] = __dadd_rn(acc[b], v);
+      sum[b / kFpfhBins] = __dadd_rn(sum[b / kFpfhBins], v);
+    }
+  });
+  double scale[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++) scale[k] = sum[k] != 0.0 ? 100.0 / sum[k] : 0.0;
+  const double* si = spfh + (size_t)i * kFpfhDim;
+  float* out = fpfh + (size_t)i * kFpfhDim;
+#pragma unroll
+  for (int b = 0; b < kFpfhDim; b++) out[b] = (float)__dadd_rn(__dmul_rn(acc[b], scale[b / kFpfhBins]), si[b]);
+}
+
+// One thread per source feature, its 33 values in registers; target features staged through shared memory a tile at a time and
+// visited in ascending index: the running argmin of d2 = sum_k (a_k - b_k)^2, summed sequentially in fp32 without contraction,
+// keeps the first (smallest) index among equal distances.  NaN distances never win; -1 when nothing does.
+__global__ void __launch_bounds__(kMatchThreads) k_fpfh_match(int ns, const float* __restrict__ src, int nt, const float* __restrict__ tgt, int* __restrict__ nearest) {
+  __shared__ __align__(16) float tile[kMatchTile * kMatchStride];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  float a[kFpfhDim];
+#pragma unroll
+  for (int k = 0; k < kFpfhDim; k++) a[k] = i < ns ? src[(size_t)i * kFpfhDim + k] : 0.f;
+  float best = INFINITY;
+  int best_j = -1;
+  for (int t0 = 0; t0 < nt; t0 += kMatchTile) {
+    const int cnt = min(kMatchTile, nt - t0);
+    __syncthreads();
+    for (int e = threadIdx.x; e < cnt * kFpfhDim; e += blockDim.x) {
+      const int t = e / kFpfhDim, k = e - t * kFpfhDim;
+      tile[t * kMatchStride + k] = tgt[(size_t)t0 * kFpfhDim + e];
+    }
+    __syncthreads();
+    for (int t = 0; t < cnt; t++) {
+      const float4* b4 = reinterpret_cast<const float4*>(tile + t * kMatchStride);
+      float b[kMatchStride];
+#pragma unroll
+      for (int k = 0; k < kMatchStride / 4; k++) {
+        const float4 v = b4[k];
+        b[4 * k] = v.x; b[4 * k + 1] = v.y; b[4 * k + 2] = v.z; b[4 * k + 3] = v.w;
+      }
+      float e0 = __fsub_rn(a[0], b[0]);
+      float d2 = __fmul_rn(e0, e0);
+#pragma unroll
+      for (int k = 1; k < kFpfhDim; k++) {
+        const float e = __fsub_rn(a[k], b[k]);
+        d2 = __fadd_rn(d2, __fmul_rn(e, e));
+      }
+      if (d2 < best) {
+        best = d2;
+        best_j = t0 + t;
+      }
+    }
+  }
+  if (i < ns) nearest[i] = best_j;
+}
+
+// one thread per hypothesis h0 + k of the wave: the sample, its matches and the pose (T: 16 doubles per hypothesis, column-major);
+// counts[h] = 0 for a valid sample, -1 for an invalid one
+__global__ void k_ransac_pose(int h0, int w, unsigned long long seed, int ns, int dof, const int* __restrict__ nearest, const float4* __restrict__ sp0,
+                              const int* __restrict__ sinv, const float4* __restrict__ tp0, const int* __restrict__ tinv, double* __restrict__ T, int* __restrict__ counts) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= w) return;
+  const int h = h0 + k;
+  int s[3];
+  ransac_sample(seed, h, ns, s);
+  bool ok = s[0] != s[1] && s[0] != s[2] && s[1] != s[2];
+  double a[9], b[9];
+  for (int j = 0; j < 3 && ok; j++) {
+    const int t = nearest[s[j]];
+    if (t < 0) { ok = false; break; }
+    load3(sp0[sinv ? sinv[s[j]] : s[j]], a + 3 * j);
+    load3(tp0[tinv ? tinv[t] : t], b + 3 * j);
+  }
+  ok = ok && ransac_pose(a, b, dof, T + 16 * (size_t)h);
+  counts[h] = ok ? 0 : -1;
+}
+
+// blockIdx.y = hypothesis of the wave, x = a chunk of source points: the inliers of the chunk, one integer atomic per warp
+__global__ void __launch_bounds__(kScoreThreads) k_ransac_score(int h0, int ns, const float4* __restrict__ sp0, const double* __restrict__ T, const int4* __restrict__ buckets,
+                                                                uint32_t mask, int max_scan, float inv, int* __restrict__ counts) {
+  const int h = h0 + (int)blockIdx.y;
+  if (counts[h] < 0) return;
+  const PoseF P = pose_from_colmajor(T + 16 * (size_t)h);
+  int c = 0;
+  const int base = blockIdx.x * kScoreThreads * kScorePerThread + threadIdx.x;
+#pragma unroll
+  for (int u = 0; u < kScorePerThread; u++) {
+    const int j = base + u * kScoreThreads;
+    if (j < ns) {
+      const float4 a = sp0[j];
+      c += ransac_inlier(P, a.x, a.y, a.z, buckets, mask, max_scan, inv) ? 1 : 0;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  if ((threadIdx.x & 31) == 0 && c > 0) atomicAdd(&counts[h], c);
+}
+
+void grid_release(gb_point_grid* g) { gb_point_grid_destroy(g); }
+
+FpfhGrid fpfh_grid(const gb_voxelmap* g, int m, float max_d2) {
+  return FpfhGrid{g->buckets, g->cells, g->voxels, (uint32_t)(g->num_buckets - 1), g->max_scan, m, g->inv_res, max_d2};
+}
+
+gb_status match_launch(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source, int* d_nearest) {
+  if (source->n == 0) return GB_OK;
+  return gb_launch(ctx, "k_fpfh_match", k_fpfh_match, (int)((source->n + kMatchThreads - 1) / kMatchThreads), kMatchThreads, 0, (int)source->n, source->fpfh,
+                   (int)target->n, target->fpfh, d_nearest);
+}
+
+gb_status match_args(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source) {
+  GB_REQUIRE(ctx && target && source, "null argument");
+  GB_REQUIRE(target->fpfh && source->fpfh, "a cloud without FPFH features (gb_cloud_estimate_fpfh)");
+  GB_REQUIRE(target->device == ctx->device && source->device == ctx->device, "a cloud lives on another device");
+  return GB_OK;
+}
+
+}  // namespace
+
+// ---------------------------------------------------------------------------------------------
+// entry points
+// ---------------------------------------------------------------------------------------------
+extern "C" gb_status gb_cloud_estimate_fpfh(gb_ctx* ctx, gb_cloud* cloud, double search_radius) {
+  GB_REQUIRE(ctx && cloud, "null argument");
+  GB_REQUIRE(std::isfinite(search_radius) && search_radius > 0.0, "search_radius must be positive and finite");
+  GB_REQUIRE(cloud->device == ctx->device, "the cloud lives on another device");
+  GB_REQUIRE(cloud->n == 0 || cloud->normals, "FPFH needs the cloud's normals");
+  GB_ENTER(ctx);
+  const size_t n = cloud->n;
+  void* base = nullptr;
+  GB_CUDA(gb_dev_malloc(ctx->device, sizeof(float) * kFpfhDim * n, &base));  // replaces the old block only on success
+  if (n > 0) {
+    gb_point_grid* gh = nullptr;
+    const gb_status st = gb_point_grid_build(ctx, cloud, 1.05 * search_radius, &gh);
+    gb_owned<gb_point_grid> grid(gh, grid_release);
+    if (st != GB_OK) { gb_dev_free(ctx->device, base); return st; }
+    const gb_voxelmap* g = grid_map(gh);
+    const float max_d2 = (float)(search_radius * search_radius);
+    const int m = grid_half_width(g->inv_res, max_d2, g->key_extent);
+    double* spfh = nullptr;
+    gb_status s2 = m <= kGridMaxHalfWidth ? gb_carve(ctx, ctx->scratch, [&](Carver& cv) { spfh = cv.take<double>(kFpfhDim * n); }) : GB_ERR_INTERNAL;
+    const FpfhGrid G = fpfh_grid(g, m, max_d2);
+    const int blocks = (int)((n + kFpfhThreads - 1) / kFpfhThreads);
+    if (s2 == GB_OK) s2 = gb_launch(ctx, "k_fpfh_spfh", k_fpfh_spfh, blocks, kFpfhThreads, 0, (int)n, G, cloud->normals, cloud->inv_perm, spfh);
+    if (s2 == GB_OK) s2 = gb_launch(ctx, "k_fpfh_final", k_fpfh_final, blocks, kFpfhThreads, 0, (int)n, G, spfh, (float*)base);
+    if (s2 == GB_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
+      gb_set_error("FPFH estimation failed: %s", cudaGetErrorString(cudaGetLastError()));
+      s2 = GB_ERR_CUDA;
+    }
+    if (s2 != GB_OK) {
+      if (s2 == GB_ERR_INTERNAL) gb_set_error("FPFH search half-width %d exceeds %d", m, kGridMaxHalfWidth);
+      gb_dev_free(ctx->device, base);
+      return s2;
+    }
+  }
+  gb_dev_free(cloud->device, cloud->f_base);
+  cloud->f_base = base;
+  cloud->fpfh = (float*)base;
+  return GB_OK;
+}
+
+extern "C" gb_status gb_cloud_fpfh(const gb_cloud* cloud, float* out) {
+  GB_REQUIRE(cloud && out, "null argument");
+  GB_REQUIRE(cloud->fpfh, "the cloud has no FPFH features (gb_cloud_estimate_fpfh)");
+  if (cloud->n) GB_CUDA(cudaMemcpy(out, cloud->fpfh, sizeof(float) * kFpfhDim * cloud->n, cudaMemcpyDefault));
+  return GB_OK;
+}
+
+extern "C" gb_status gb_fpfh_match(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source, int32_t* nearest) {
+  GB_CHECK(match_args(ctx, target, source));
+  GB_REQUIRE(nearest || source->n == 0, "null output");
+  GB_ENTER(ctx);
+  const size_t ns = source->n;
+  if (ns == 0) return GB_OK;
+  int* d_nearest = nullptr;
+  int* h_nearest = nullptr;
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) { d_nearest = cv.take<int>(ns); }));
+  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h_nearest = cv.take<int>(ns); }));
+  GB_CHECK(match_launch(ctx, target, source, d_nearest));
+  GB_CUDA(cudaMemcpyAsync(h_nearest, d_nearest, sizeof(int) * ns, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(nearest, h_nearest, sizeof(int) * ns);
+  return GB_OK;
+}
+
+extern "C" gb_status gb_ransac_default_params(gb_ransac_params* p) {
+  GB_REQUIRE(p, "null argument");
+  p->max_iterations = 5000;
+  p->early_stop_inlier_rate = 0.9;
+  p->inlier_voxel_resolution = 1.0;
+  p->dof = 4;
+  p->seed = 53123;
+  return GB_OK;
+}
+
+extern "C" gb_status gb_ransac_align(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source, const gb_ransac_params* prm, gb_ransac_result* result,
+                                     int32_t* hypothesis_inliers) {
+  GB_REQUIRE(prm && result, "null argument");
+  GB_REQUIRE(prm->max_iterations >= 1 && prm->max_iterations <= (1 << 28), "max_iterations must be in [1, 2^28]");
+  GB_REQUIRE(std::isfinite(prm->early_stop_inlier_rate) && prm->early_stop_inlier_rate > 0.0, "early_stop_inlier_rate must be positive and finite");
+  GB_REQUIRE(std::isfinite(prm->inlier_voxel_resolution) && prm->inlier_voxel_resolution > 0.0, "inlier_voxel_resolution must be positive and finite");
+  GB_REQUIRE(prm->dof == 4 || prm->dof == 6, "dof must be 4 or 6");
+  GB_CHECK(match_args(ctx, target, source));
+  GB_REQUIRE(source->n >= 1 && target->n >= 1, "empty cloud");
+  GB_ENTER(ctx);
+  // the grid first: its build carves the context's scratch, which then holds this call's arrays
+  gb_point_grid* gh = nullptr;
+  GB_CHECK(gb_point_grid_build(ctx, target, prm->inlier_voxel_resolution, &gh));
+  gb_owned<gb_point_grid> grid(gh, grid_release);
+  const gb_voxelmap* g = grid_map(gh);
+  const int ns = (int)source->n, H = prm->max_iterations;
+  int *d_nearest, *d_counts, *h_counts;
+  double *d_T, *h_T;
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+    d_nearest = cv.take<int>((size_t)ns);
+    d_counts = cv.take<int>((size_t)H);
+    d_T = cv.take<double>(16 * (size_t)H);
+  }));
+  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) {
+    h_counts = cv.take<int>((size_t)H);
+    h_T = cv.take<double>(16);
+  }));
+  GB_CHECK(match_launch(ctx, target, source, d_nearest));
+  // the rule of include/glim_b200.h: the lowest h whose rate reaches the early-stop rate, else the most inliers (ties: lowest h)
+  int best = -1, best_count = 0, stop = -1, evaluated = 0;
+  for (int h0 = 0; h0 < H && stop < 0; h0 += kRansacWave) {
+    const int w = std::min(kRansacWave, H - h0);
+    GB_CHECK(gb_launch(ctx, "k_ransac_pose", k_ransac_pose, (w + 127) / 128, 128, 0, h0, w, (unsigned long long)prm->seed, ns, prm->dof, d_nearest, source->p0,
+                       source->inv_perm, target->p0, target->inv_perm, d_T, d_counts));
+    const dim3 sgrid((unsigned)((ns + kScoreThreads * kScorePerThread - 1) / (kScoreThreads * kScorePerThread)), (unsigned)w);
+    GB_CHECK(gb_launch(ctx, "k_ransac_score", k_ransac_score, sgrid, kScoreThreads, 0, h0, ns, source->p0, d_T, g->buckets, (uint32_t)(g->num_buckets - 1),
+                       g->max_scan, g->inv_res, d_counts));
+    GB_CUDA(cudaMemcpyAsync(h_counts + h0, d_counts + h0, sizeof(int) * w, cudaMemcpyDeviceToHost, ctx->stream));
+    GB_CUDA(cudaStreamSynchronize(ctx->stream));
+    evaluated = h0 + w;
+    for (int h = h0; h < h0 + w; h++) {
+      const int c = h_counts[h];
+      if (c > best_count) { best_count = c; best = h; }
+      if (stop < 0 && c >= 0 && (double)c / (double)ns >= prm->early_stop_inlier_rate) stop = h;
+    }
+  }
+  memset(result, 0, sizeof(*result));
+  for (int k = 0; k < 16; k++) result->T_target_source[k] = (k % 5 == 0) ? 1.0 : 0.0;
+  const int chosen = stop >= 0 ? stop : best;
+  result->evaluated = evaluated;
+  result->best_hypothesis = -1;
+  result->status = GB_RANSAC_DEGENERATE;
+  if (chosen >= 0) {
+    GB_CUDA(cudaMemcpyAsync(h_T, d_T + 16 * (size_t)chosen, sizeof(double) * 16, cudaMemcpyDeviceToHost, ctx->stream));
+    GB_CUDA(cudaStreamSynchronize(ctx->stream));
+    memcpy(result->T_target_source, h_T, sizeof(double) * 16);
+    result->best_hypothesis = chosen;
+    result->inliers = h_counts[chosen];
+    result->inlier_rate = (double)h_counts[chosen] / (double)ns;
+    result->status = stop >= 0 ? GB_RANSAC_EARLY_STOP : GB_RANSAC_FOUND;
+  }
+  if (hypothesis_inliers) {
+    for (int h = 0; h < H; h++) hypothesis_inliers[h] = h < evaluated ? h_counts[h] : -2;
+  }
+  return GB_OK;
+}

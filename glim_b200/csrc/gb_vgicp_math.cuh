@@ -28,6 +28,15 @@ GB_HD int gb_coord(float p, float inv_res) { return __float2int_rd(p * inv_res);
 GB_HD uint32_t gb_hash(int x, int y, int z) {
   return ((uint32_t)x * 73856093u) ^ ((uint32_t)y * 19349669u) ^ ((uint32_t)z * 83492791u);
 }
+// the project's fixed pseudo-random pick ([EXT]: the reference draws with std::mt19937): the points / voxels with the smallest
+// rg_hash(seed, index) are kept (random-grid downsampling, frame-merge thinning, voxel-map insert sampling; the oracle shares it),
+// and RANSAC draws its samples from it (gb_global_math.cuh)
+GB_HD unsigned long long rg_hash(unsigned long long seed, unsigned i) {
+  unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(i + 1u);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
 
 #ifndef GB_MODE_LINEARIZE_VALUE
 #define GB_MODE_LINEARIZE_VALUE 0  // == GB_MODE_LINEARIZE (gb_internal.cuh)

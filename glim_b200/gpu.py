@@ -20,6 +20,9 @@ include/glim_b200/gtsam_points_compat.hpp.
     IntegratedCT_GICPFactorGPU(key_X, key_Y, ivox, source, max_corr)   odometry_estimation_ct.cpp:159-163
     align_ct_gicp(factors, X_init, Y_init, X_prior, params) the CT LM solve with its motion priors, odometry_estimation_ct.cpp:166-182
     deskew_ct(cloud, X, Y, neighbors, k_neighbors)          deskewed_source_points + covariances, odometry_estimation_ct.cpp:199-204
+    PointCloudGPU.estimate_fpfh(radius) / .fpfh()           gtsam_points::estimate_fpfh, manual_loop_close_modal.cpp:382-397, :415
+    fpfh_match(target, source)                              the target's KdTreeX over FPFH features, manual_loop_close_modal.cpp:402
+    estimate_pose_ransac(target, source, **params)          gtsam_points::estimate_pose_ransac, manual_loop_close_modal.cpp:435-443
 """
 from __future__ import annotations
 
@@ -124,6 +127,18 @@ class PointCloudGPU:
         t0, t1 = C.c_double(), C.c_double()
         check(lib().gb_cloud_time_table(self.h, None, ptr(starts), ptr(tau), C.byref(t0), C.byref(t1)))
         return (starts if B.value else np.zeros(0, np.int32)), tau, t0.value, t1.value
+
+    def estimate_fpfh(self, radius: float):
+        """gtsam_points::estimate_fpfh with search_radius = radius (manual_loop_close_modal.cpp:382-397): the cloud's FPFH features,
+        kept on the device with it (gb_cloud_estimate_fpfh); the cloud must carry normals.  A second call replaces them."""
+        check(lib().gb_cloud_estimate_fpfh(self.ctx.h, self.h, float(radius)))
+        return self
+
+    def fpfh(self) -> np.ndarray:
+        """-> (n, 33) float32 features in the original point order"""
+        out = np.empty((self.n, capi.FPFH_DIM), np.float32)
+        check(lib().gb_cloud_fpfh(self.h, ptr(out)))
+        return out
 
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:
@@ -519,6 +534,37 @@ def deskew_ct(cloud: PointCloudGPU, X, Y, neighbors, k_neighbors: int, host_outp
     if not host_outputs:
         return None, None, None, out
     return pts, cov.reshape(n, 4, 4).transpose(0, 2, 1).copy(), nrm, out
+
+
+def fpfh_match(target: PointCloudGPU, source: PointCloudGPU, ctx: Context | None = None) -> np.ndarray:
+    """gb_fpfh_match: for every source feature the index of the nearest target feature (exact, ties to the smaller index),
+    -> (n_source,) int32"""
+    ctx = ctx or source.ctx
+    out = np.empty(source.n, np.int32)
+    check(lib().gb_fpfh_match(ctx.h, target.h, source.h, ptr(out)))
+    return out
+
+
+def ransac_params(**overrides) -> capi.RansacParams:
+    """gb_ransac_default_params (the manual loop-closure modal's values) with the given fields replaced."""
+    return _params(capi.RansacParams(), lib().gb_ransac_default_params, "gb_ransac_params", overrides)
+
+
+def estimate_pose_ransac(target: PointCloudGPU, source: PointCloudGPU, ctx: Context | None = None, hypothesis_inliers: bool = False, **params) -> dict:
+    """gtsam_points::estimate_pose_ransac (manual_loop_close_modal.cpp:435-443) on the device (gb_ransac_align): both clouds carry
+    FPFH features; params are fields of gb_ransac_params (max_iterations, early_stop_inlier_rate, inlier_voxel_resolution, dof,
+    seed).  -> {T_target_source (4,4), inliers, inlier_rate, best_hypothesis, evaluated, status, status_name} and, with
+    hypothesis_inliers, the per-hypothesis counts (max_iterations,) int32 (-1 invalid sample, -2 not evaluated)."""
+    ctx = ctx or source.ctx
+    p = ransac_params(**params)
+    r = capi.RansacResult()
+    counts = np.empty(p.max_iterations, np.int32) if hypothesis_inliers else None
+    check(lib().gb_ransac_align(ctx.h, target.h, source.h, C.byref(p), C.byref(r), ptr(counts)))
+    out = {"T_target_source": np.array(r.T_target_source[:]).reshape(4, 4).T.copy(), "inliers": r.inliers, "inlier_rate": r.inlier_rate,
+           "best_hypothesis": r.best_hypothesis, "evaluated": r.evaluated, "status": r.status, "status_name": capi.RANSAC_STATUS_NAMES.get(r.status, "?")}
+    if counts is not None:
+        out["hypothesis_inliers"] = counts
+    return out
 
 
 class NonlinearFactorSetGPU:

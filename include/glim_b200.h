@@ -280,6 +280,79 @@ GB_API gb_status gb_gicp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* ta
 /* the factor's search half-width m (0 for a factor of another kind) */
 GB_API gb_status gb_gicp_grid_factor_half_width(const gb_factor* factor, int* m);
 
+/* ---- Global registration: T_target_source between two clouds with no initial guess, as GLIM's manual loop closure runs it
+ *      (ManualLoopCloseModal::align_global, src/glim/viewer/interactive/manual_loop_close_modal.cpp:370-468): FPFH features of
+ *      both clouds (gtsam_points::estimate_fpfh, :382-397, :415), exact nearest-feature matching (the target's KdTreeX, :402)
+ *      and RANSAC (gtsam_points::estimate_pose_ransac, :435-443).  Refine the result with a GICP factor on a point grid and
+ *      gb_vgicp_align, the modal's fine registration (:470-520).  [EXT] gtsam_points is not vendored: the feature (PCL /
+ *      Open3D's FPFH), the sample draw, the estimators and the selection rule below are this library's statement of it.
+ *
+ *      FPFH.  The neighbours of point i are every other point j with fp32 d2 = (dx^2 + dy^2) + dz^2 (uncontracted) <
+ *      (float)(r^2): the brute-force set (no neighbour cap), found in a point grid of cell 1.05 r with the half-width
+ *      grid_half_width proves.  Pair features in fp64 from the stored fp32 positions and normals, with d = p_j - p_i:
+ *      |d| = 0 gives (0, 0, 0); the roles swap (n_s = n_j, n_t = n_i, d = -d, f3 = -n_j.d/|d|) when |n_i.d| < |n_j.d| (PCL's
+ *      acos test on the cosines), else n_s = n_i, n_t = n_j, f3 = n_i.d/|d|; v = d x n_s (|v| = 0 gives (0, 0, 0)), v /= |v|,
+ *      w = n_s x v, f2 = v.n_t, f1 = atan2(w.n_t, n_s.n_t).  Bins (Open3D): floor(11 (f1 + pi) / 2 pi), floor(11 (f2 + 1) / 2),
+ *      floor(11 (f3 + 1) / 2), clamped to [0, 10] (NaN to 0), at offsets 0, 11, 22.  SPFH_i = (pairs of i in the bin) x
+ *      (100 / K_i) for the K_i neighbours of i.  FPFH_i = A_b x 100 / (sum of A over b's 11-bin block) + SPFH_i,b with
+ *      A_b = sum_j SPFH_j,b / d2_ij, d2_ij = d.d in fp64, neighbours at d2_ij = 0 skipped and a zero block sum scaling by 0
+ *      (PCL and Open3D weight by the squared distance their radius search returns).  So every 11-bin block of a point with
+ *      neighbours sums to 200 (100 if every neighbour coincides with it), and a point with no neighbours (a NaN point) is zero.
+ *      fp64 throughout, stored once as fp32.  The SPFH counts do not depend on the visiting order; the fp64 sum A visits
+ *      cells in offset order and a cell's points in ascending original index, so it may differ from an ascending-index sum in
+ *      the last bits of fp64.
+ *
+ *      Matching.  nearest[i] = the target feature with the smallest fp32 d2 = (...((a_0 - b_0)^2 + (a_1 - b_1)^2) + ...) +
+ *      (a_32 - b_32)^2, summed sequentially and uncontracted; ties to the smaller target index (the brute-force argmin of an exact
+ *      KdTree); -1 when no distance is a number.  No ||a||^2 + ||b||^2 - 2 a.b shortcut: it would not give the exact argmin.
+ *
+ *      RANSAC, per hypothesis h = 0, 1, ...: s_j = rg_hash(seed, 3 h + j) mod N_s (j = 0, 1, 2; the hash of the random-grid
+ *      pick), each paired with its match.  Invalid (counts -1) when two s_j coincide or a match is -1, or when the doubled area
+ *      |(x_1 - x_0) x (x_2 - x_0)| of the source or the target triangle is below 1e-3 m^2 or not finite.  Pose in fp64 from the
+ *      fp32 positions: dof 6 is Horn's quaternion (the eigenvector of the largest eigenvalue of his 4x4, from 8 cyclic Jacobi
+ *      sweeps); dof 4 is yaw = atan2(sum a'_x b'_y - a'_y b'_x, sum a'_x b'_x + a'_y b'_y) over the centred points, R = Rz(yaw);
+ *      both t = centroid_b - R centroid_a.  A source point is an inlier iff q = R a + t under the fp32 cast of the pose
+ *      (((r0 a_x + r1 a_y) + r2 a_z) + t, uncontracted) is finite and keys (gb_coord at (float)(1 / inlier_voxel_resolution))
+ *      into a cell of a point grid of the target at that resolution; inlier_rate = inliers / N_s.  The result is the lowest h
+ *      with inlier_rate >= early_stop_inlier_rate (EARLY_STOP); else the h with the most inliers, ties to the lowest h (FOUND);
+ *      DEGENERATE, T = I, best_hypothesis = -1 when no hypothesis has an inlier.  This is what a sequential loop with early stop
+ *      returns, whatever the batching.  The device scores waves of 512 hypotheses and stops after the wave that holds the
+ *      early stop: `evaluated` = the hypotheses scored (a multiple of 512, or max_iterations).
+ *
+ *      Launches: gb_cloud_estimate_fpfh, the point grid build's (gb_point_grid_build) + 2; gb_fpfh_match, 1 (0 for an empty
+ *      source); gb_ransac_align, 1 (the match) + the target grid's build + 2 per wave, with one copy of the wave's counts and one
+ *      stream synchronisation per wave. ---- */
+/* The FPFH features of `cloud` with search radius r, kept on the device with the cloud (cloud_destroy releases them); a second
+ * call replaces them.  GB_ERR_INVALID_ARGUMENT before any launch for a cloud without normals, a non-finite or non-positive r,
+ * or a cloud on another device than ctx. */
+GB_API gb_status gb_cloud_estimate_fpfh(gb_ctx* ctx, gb_cloud* cloud, double search_radius);
+/* host copy of the features, N x 33 in the caller's point order; GB_ERR_INVALID_ARGUMENT for a cloud without features */
+GB_API gb_status gb_cloud_fpfh(const gb_cloud* cloud, float* out);
+/* nearest[i] (N_s, the source's caller order) = the target index of source feature i's nearest target feature.  Both clouds
+ * must carry features and live on ctx's device (GB_ERR_INVALID_ARGUMENT before any launch). */
+GB_API gb_status gb_fpfh_match(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source, int32_t* nearest);
+#define GB_RANSAC_FOUND 0
+#define GB_RANSAC_EARLY_STOP 1
+#define GB_RANSAC_DEGENERATE 2
+typedef struct gb_ransac_params {
+  int max_iterations;              /* 5000 (manual_loop_close_modal.cpp:47), in [1, 2^28] */
+  double early_stop_inlier_rate;   /* 0.9 (:48); > 0, above 1 never stops early */
+  double inlier_voxel_resolution;  /* 1.0 m (:49), > 0 */
+  int dof;                         /* 4 (:50, global_registration_4dof) or 6 */
+  uint64_t seed;                   /* 53123 (:42; the modal adds 4322 before each run) */
+} gb_ransac_params;
+typedef struct gb_ransac_result {
+  double T_target_source[16];      /* column-major */
+  double inlier_rate;
+  int inliers, best_hypothesis, evaluated, status; /* GB_RANSAC_* */
+} gb_ransac_result;
+GB_API gb_status gb_ransac_default_params(gb_ransac_params* params);
+/* hypothesis_inliers (max_iterations, or NULL): the inlier count of every evaluated hypothesis, -1 for an invalid sample, -2
+ * for one not evaluated.  Validated before any launch: both clouds with features and at least one point, on ctx's device; the
+ * parameter bounds above. */
+GB_API gb_status gb_ransac_align(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source, const gb_ransac_params* params, gb_ransac_result* result,
+                                 int32_t* hypothesis_inliers);
+
 /* ---- NonlinearFactorSetGPU::add(graph) / ::linearize(values) (odometry_estimation_gpu.cpp:383-386;
  *      hook at src/glim/viewer/offline_viewer.cpp:29): F x 64 B of poses down, one launch over all
  *      factors, F records up. ---- */
