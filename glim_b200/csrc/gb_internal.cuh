@@ -435,6 +435,13 @@ inline gb_sort_tmp gb_take_sort_tmp(Carver& cv, size_t n, void* cub, size_t cub_
 // starts[V] = number of valid points.
 gb_status gb_group_by_key(gb_ctx* ctx, int n, const gb_sort_tmp& t, int* flags, int* pos);
 gb_status gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* flags, const int* pos, int* starts);
+// Hash thinning (gb_kernels_voxelmap.cu), shared by the random-grid cap, the frame-merge thinning and the map-insert sampling:
+// of the candidates among n items (i with cand[i] != 0 when cand is given, and i < *count when count is given), the m with
+// the smallest rg_hash(seed, i) stay.  keep[i] = candidate(i) && rg_hash(seed, i) <= sorted[m - 1], where sorted holds the
+// candidates' hashes (~0 for the others) in ascending order; every candidate stays when m <= 0 or m >= *count (n without a
+// count).  keep may be cand itself.  The hashes go through t.keys into t.keys_s (t.cub for the sort), which it overwrites.
+// Three launches: k_thin_hash, cub SortKeys, k_thin_keep.
+gb_status gb_thin(gb_ctx* ctx, int n, const int* cand, const int* count, int m, unsigned long long seed, const gb_sort_tmp& t, int* keep);
 
 // Device cloud construction.  gb_cloud_planes lays out the planes of n points (p0, p1, p2, optional normals) at the
 // carver's position; the planes staged in the caller's point order use the same layout as the cloud's own.
@@ -472,9 +479,9 @@ gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_de
 // of device scratch for the frame descriptor.  One launch.
 #define GB_FRAME_DESC_BYTES 256
 gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T_colmajor, void* d_frame, double4* pts, double* cov6);
-// k_grid_keys of the voxel-grid paths: key = packed floor(p * inv_res) in fp64 (~0 for non-finite / out-of-range points),
-// idx[i] = i.  One launch.
-gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx);
+// k_grid_keys of the voxel-grid paths: key = packed floor(p * inv_res) in fp64 (~0 for non-finite / out-of-range points,
+// and for every point with keep[i] == 0 when keep is given), idx[i] = i.  One launch.
+gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, const int* keep, unsigned long long* keys, int* idx);
 
 // ---------------------------------------------------------------------------------------------
 // device helpers shared by kernels
@@ -489,7 +496,7 @@ __device__ __forceinline__ bool gb_pack_key(int x, int y, int z, unsigned long l
   *key = ((unsigned long long)(x + GB_KEY_OFFSET) << 42) | ((unsigned long long)(y + GB_KEY_OFFSET) << 21) | (unsigned long long)(z + GB_KEY_OFFSET);
   return true;
 }
-__device__ __forceinline__ void gb_unpack_key(unsigned long long key, int& x, int& y, int& z) {
+__host__ __device__ __forceinline__ void gb_unpack_key(unsigned long long key, int& x, int& y, int& z) {
   x = (int)((key >> 42) & 0x1FFFFF) - GB_KEY_OFFSET;
   y = (int)((key >> 21) & 0x1FFFFF) - GB_KEY_OFFSET;
   z = (int)(key & 0x1FFFFF) - GB_KEY_OFFSET;

@@ -7,8 +7,9 @@
 //   gtsam_points::voxelgrid_sampling             src/glim/preprocess/cloud_preprocessor.cpp:108
 // Oracles: go_knn_bruteforce, go_covariance_estimate, go_voxelgrid_sampling (oracle/glim_oracle.c).
 // All three work in fp64 like the reference's host code (Vector4d / Matrix4d).
-// The voxel grouping (sort, head flags, scan, voxel starts) and the device cloud build are shared with the voxel-map build
-// (gb_group_by_key, gb_group_starts, gb_cloud_build in gb_kernels_voxelmap.cu); only the fp64 key kernel is this file's.
+// The voxel grouping (sort, head flags, scan, voxel starts), the hash thinning and the device cloud build are shared with the
+// voxel-map paths (gb_group_by_key, gb_group_starts, gb_thin, gb_cloud_build in gb_kernels_voxelmap.cu); the fp64 key kernel
+// and the group means are this file's.
 // The entry points gb_covariances, gb_find_neighbors, gb_voxelgrid_sampling, gb_preprocess and gb_merge_frames are defined here.
 #include "gb_internal.cuh"
 #include "gb_cov_math.cuh"  // plane_covariance (shared with the host-compiled CPU test of the covariance arithmetic)
@@ -96,12 +97,12 @@ __global__ void __launch_bounds__(128) k_covariances(int n, const double4* __res
 // ---------------------------------------------------------------------------------------------
 // voxel-grid downsampling (fp64 coordinates, SURVEY C.2)
 // ---------------------------------------------------------------------------------------------
-__global__ void k_grid_keys(int n, const double4* __restrict__ pts, double inv_res, unsigned long long* __restrict__ keys, int* __restrict__ idx) {
+__global__ void k_grid_keys(int n, const double4* __restrict__ pts, double inv_res, const int* __restrict__ keep, unsigned long long* __restrict__ keys, int* __restrict__ idx) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const double4 p = pts[i];
   unsigned long long key = kInvalidKey;
-  if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
+  if ((!keep || keep[i]) && isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
     const double fx = floor(p.x * inv_res), fy = floor(p.y * inv_res), fz = floor(p.z * inv_res);
     if (fabs(fx) < 2e9 && fabs(fy) < 2e9 && fabs(fz) < 2e9) {
       unsigned long long k;
@@ -111,30 +112,36 @@ __global__ void k_grid_keys(int n, const double4* __restrict__ pts, double inv_r
   keys[i] = key;
   idx[i] = i;
 }
-// num_voxels = device count of voxels (the last element of the inclusive scan of gb_group_by_key)
+// The fp64 mean of each voxel's members in sorted-slot order, for the voxel-grid downsampling and the frame merge: points,
+// and the times, intensities and 6-entry covariances when given.  num_voxels = device count of voxels (the last element of
+// the inclusive scan of gb_group_by_key).
 __global__ void k_grid_means_counted(const int* __restrict__ num_voxels, const int* __restrict__ starts, const int* __restrict__ idx, const double4* __restrict__ pts, const double* __restrict__ times, const double* __restrict__ intens,
-                                     double4* __restrict__ out_pts, double* __restrict__ out_times, double* __restrict__ out_intens) {
+                                     const double* __restrict__ cov6, double4* __restrict__ out_pts, double* __restrict__ out_times, double* __restrict__ out_intens, double* __restrict__ out_cov6) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= *num_voxels) return;
   const int b = starts[v], e = starts[v + 1];
-  double sx = 0, sy = 0, sz = 0, sw = 0, st = 0, si = 0;
+  double sx = 0, sy = 0, sz = 0, sw = 0, st = 0, si = 0, c[6] = {0, 0, 0, 0, 0, 0};
   for (int s = b; s < e; s++) {  // same sums in the same order as the oracle
     const int i = idx[s];
     const double4 p = pts[i];
     sx += p.x; sy += p.y; sz += p.z; sw += p.w;
     if (times) st += times[i];
     if (intens) si += intens[i];
+    if (cov6)
+      for (int m = 0; m < 6; m++) c[m] += cov6[6 * (size_t)i + m];
   }
   const int cnt = e - b;
   out_pts[v] = make_double4(sx / cnt, sy / cnt, sz / cnt, sw / cnt);
   if (times) out_times[v] = st / cnt;
   if (intens) out_intens[v] = si / cnt;
+  if (cov6)
+    for (int m = 0; m < 6; m++) out_cov6[6 * (size_t)v + m] = c[m] / cnt;
 }
 
 }  // namespace
 
-gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, unsigned long long* keys, int* idx) {
-  return gb_launch(ctx, "k_grid_keys", k_grid_keys, (n + 255) / 256, 256, 0, n, pts, inv_res, keys, idx);
+gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, const int* keep, unsigned long long* keys, int* idx) {
+  return gb_launch(ctx, "k_grid_keys", k_grid_keys, (n + 255) / 256, 256, 0, n, pts, inv_res, keep, keys, idx);
 }
 
 // Returns launch(std::integral_constant<int, K>()) for the instantiated neighbour counts K of the k-NN kernels.
@@ -240,7 +247,7 @@ extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* 
   GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * n, cudaMemcpyHostToDevice, st));
   if (times) GB_CUDA(cudaMemcpyAsync(d_t, times, sizeof(double) * n, cudaMemcpyHostToDevice, st));
   if (intensities) GB_CUDA(cudaMemcpyAsync(d_i, intensities, sizeof(double) * n, cudaMemcpyHostToDevice, st));
-  GB_CHECK(gb_grid_keys(ctx, (int)n, d_pts, 1.0 / resolution, t.keys, t.idx));
+  GB_CHECK(gb_grid_keys(ctx, (int)n, d_pts, 1.0 / resolution, nullptr, t.keys, t.idx));
   GB_CHECK(gb_group_by_key(ctx, (int)n, t, d_flags, d_pos));
   int V = 0;
   GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -248,7 +255,7 @@ extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* 
   if (V > 0) {
     GB_CHECK(gb_group_starts(ctx, (int)n, t, d_flags, d_pos, d_starts));
     GB_CHECK(gb_launch(ctx, "k_grid_means_counted", k_grid_means_counted, (n + 127) / 128, 128, 0, d_pos + (n - 1), d_starts, t.idx_s, d_pts, times ? d_t : nullptr,
-                       intensities ? d_i : nullptr, d_opts, d_ot, d_oi));
+                       intensities ? d_i : nullptr, nullptr, d_opts, d_ot, d_oi, nullptr));
     GB_CUDA(cudaMemcpyAsync(out_xyzw, d_opts, sizeof(double4) * (size_t)V, cudaMemcpyDeviceToHost, st));
     if (times && out_times) GB_CUDA(cudaMemcpyAsync(out_times, d_ot, sizeof(double) * (size_t)V, cudaMemcpyDeviceToHost, st));
     if (intensities && out_intensities) GB_CUDA(cudaMemcpyAsync(out_intensities, d_oi, sizeof(double) * (size_t)V, cudaMemcpyDeviceToHost, st));
@@ -426,7 +433,7 @@ __global__ void k_fill_self(int n, int k, int* __restrict__ neighbors) {
 // ---- downsampling, filtering, time order ----
 // random grid (gtsam_points::randomgrid_sampling, cloud_preprocessor.cpp:104-106): every voxel keeps at most
 // ppv = ceil(rate * N / V) of its points.  Which ones is a draw from std::mt19937 in the reference (not reproducible, SURVEY
-// C.2); here it is the ppv points with the smallest rg_hash(seed, index) (gb_internal.cuh) -- a fixed pseudo-random choice the
+// C.2); here it is the ppv points with the smallest rg_hash(seed, index) (gb_vgicp_math.cuh) -- a fixed pseudo-random choice the
 // oracle shares.
 __global__ void k_randomgrid_select(int n, const int* __restrict__ num_voxels, const int* __restrict__ starts, const int* __restrict__ idx_s, double rate, unsigned long long seed, int* __restrict__ keep) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
@@ -456,14 +463,6 @@ __global__ void k_randomgrid_select(int n, const int* __restrict__ num_voxels, c
   }
 }
 
-__global__ void k_rg_hash_keys(int n, const int* __restrict__ keep, unsigned long long seed, unsigned long long* __restrict__ keys) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) keys[i] = keep[i] ? rg_hash(seed, (unsigned)i) : ~0ull;
-}
-__global__ void k_rg_cap(int n, int cap, const unsigned long long* __restrict__ sorted, unsigned long long seed, int* __restrict__ keep) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n && keep[i] && rg_hash(seed, (unsigned)i) > sorted[cap - 1]) keep[i] = 0;
-}
 
 struct FrameFilter {
   double near2, far2;
@@ -680,7 +679,7 @@ static gb_status preprocess(gb_ctx* ctx, size_t n_, const double* xyzw, const do
   const int* cur_cnt = d_cnt + 0;
   const int* keep = nullptr;
   if (P->downsample_resolution > 0.0) {
-    GB_CHECK(gb_grid_keys(ctx, n, d_raw, 1.0 / P->downsample_resolution, t.keys, t.idx));
+    GB_CHECK(gb_grid_keys(ctx, n, d_raw, 1.0 / P->downsample_resolution, nullptr, t.keys, t.idx));
     GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
     GB_CHECK(gb_launch(ctx, "k_copy_last_pos", k_copy_last_pos, 1, 1, 0, n, d_pos, d_cnt + 3));  // V
     GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
@@ -690,15 +689,13 @@ static gb_status preprocess(gb_ctx* ctx, size_t n_, const double* xyzw, const do
         GB_CUDA(cudaMemsetAsync(d_keep, 0, sizeof(int) * N, st));
         GB_CHECK(gb_launch(ctx, "k_randomgrid_select", k_randomgrid_select, gb, tb, 0, n, d_cnt + 3, d_starts, t.idx_s, rate, P->seed, d_keep));
         const int cap = (int)((double)n * rate * 1.2);
-        if (cap > 0 && cap < n) {  // thin the survivors to 1.2 * rate * N: the smallest hashes stay
-          GB_CHECK(gb_launch(ctx, "k_rg_hash_keys", k_rg_hash_keys, gb, tb, 0, n, d_keep, P->seed, t.keys));
-          GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, cub_b, t.keys, t.keys_s, n, 0, 64);
-          GB_CHECK(gb_launch(ctx, "k_rg_cap", k_rg_cap, gb, tb, 0, n, cap, t.keys_s, P->seed, d_keep));
-        }
+        if (cap > 0 && cap < n)  // thin the survivors to 1.2 * rate * N: the smallest hashes stay
+          GB_CHECK(gb_thin(ctx, n, d_keep, nullptr, cap, P->seed, t, d_keep));
         keep = d_keep;  // original order is kept; the gates below drop the rest
       }
     } else {
-      GB_CHECK(gb_launch(ctx, "k_grid_means_counted", k_grid_means_counted, (n + 127) / 128, 128, 0, d_cnt + 3, d_starts, t.idx_s, d_raw, cur_t, cur_i, d_ds, d_dst, d_dsi));
+      GB_CHECK(gb_launch(ctx, "k_grid_means_counted", k_grid_means_counted, (n + 127) / 128, 128, 0, d_cnt + 3, d_starts, t.idx_s, d_raw, cur_t, cur_i, nullptr, d_ds, d_dst, d_dsi,
+                         nullptr));
       cur_pts = d_ds; cur_t = times ? d_dst : nullptr; cur_i = intensities ? d_dsi : nullptr; cur_cnt = d_cnt + 3;
     }
   }
@@ -875,34 +872,6 @@ __global__ void k_merge_transform(int num_frames, const MergeFrame* __restrict__
   for (int r = 0; r < 3; r++)
     for (int c = r; c < 3; c++) o[e++] = __dadd_rn(__dadd_rn(__dmul_rn(RC[r * 3 + 0], T[c * 4 + 0]), __dmul_rn(RC[r * 3 + 1], T[c * 4 + 1])), __dmul_rn(RC[r * 3 + 2], T[c * 4 + 2]));
 }
-__global__ void k_merge_means(const int* __restrict__ num_voxels, const int* __restrict__ starts, const int* __restrict__ idx, const double4* __restrict__ pts, const double* __restrict__ cov6,
-                              double4* __restrict__ o_pts, double* __restrict__ o_cov6) {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= *num_voxels) return;
-  const int b = starts[v], e = starts[v + 1];
-  double s[4] = {0, 0, 0, 0}, c[6] = {0, 0, 0, 0, 0, 0};
-  for (int k = b; k < e; k++) {
-    const int i = idx[k];
-    const double4 p = pts[i];
-    s[0] += p.x; s[1] += p.y; s[2] += p.z; s[3] += p.w;
-    for (int m = 0; m < 6; m++) c[m] += cov6[6 * (size_t)i + m];
-  }
-  const int cnt = e - b;
-  o_pts[v] = make_double4(s[0] / cnt, s[1] / cnt, s[2] / cnt, s[3] / cnt);
-  for (int m = 0; m < 6; m++) o_cov6[6 * (size_t)v + m] = c[m] / cnt;
-}
-__global__ void k_merge_hash_keys(int n_upper, const int* __restrict__ num_voxels, unsigned long long seed, unsigned long long* __restrict__ keys) {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v < n_upper) keys[v] = v < *num_voxels ? rg_hash(seed, (unsigned)v) : ~0ull;
-}
-// keep flag per voxel (all, or the `target` smallest hashes), then an inclusive scan gives the output slot
-__global__ void k_merge_keep(int n_upper, const int* __restrict__ num_voxels, int target, const unsigned long long* __restrict__ sorted, unsigned long long seed, int* __restrict__ keep) {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= n_upper) return;
-  int k = v < *num_voxels;
-  if (k && target > 0 && target < *num_voxels) k = rg_hash(seed, (unsigned)v) <= sorted[target - 1];
-  keep[v] = k;
-}
 __global__ void k_merge_emit(int n_upper, const int* __restrict__ keep, const int* __restrict__ pos, const double4* __restrict__ pts, const double* __restrict__ cov6, double4* __restrict__ o_pts, double* __restrict__ o_cov16,
                              float4* __restrict__ s0, float4* __restrict__ s1, float* __restrict__ s2) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
@@ -911,9 +880,8 @@ __global__ void k_merge_emit(int n_upper, const int* __restrict__ keep, const in
   const double4 p = pts[v];
   const double* c = cov6 + 6 * (size_t)v;
   o_pts[o] = p;
-  double* C = o_cov16 + 16 * (size_t)o;
-  for (int e = 0; e < 16; e++) C[e] = 0.0;
-  C[0] = c[0]; C[4] = c[1]; C[8] = c[2]; C[1] = c[1]; C[5] = c[3]; C[9] = c[4]; C[2] = c[2]; C[6] = c[4]; C[10] = c[5];
+  const double C[9] = {c[0], c[1], c[2], c[1], c[3], c[4], c[2], c[4], c[5]};
+  store_cov4x4(o_cov16 + 16 * (size_t)o, C);
   s0[o] = make_float4((float)p.x, (float)p.y, (float)p.z, (float)c[0]);
   s1[o] = make_float4((float)c[1], (float)c[2], (float)c[3], (float)c[4]);
   s2[o] = (float)c[5];
@@ -921,14 +889,19 @@ __global__ void k_merge_emit(int n_upper, const int* __restrict__ keep, const in
 
 }  // namespace
 
+// the descriptor of cloud c at pose T (column-major 4x4) whose points are numbered from offset on
+static MergeFrame merge_frame(const gb_cloud* c, const double* T, int offset) {
+  MergeFrame F;
+  F.p0 = c->p0; F.p1 = c->p1; F.p2 = c->p2; F.inv_perm = c->inv_perm; F.n = (int)c->n; F.offset = offset;
+  for (int r = 0; r < 3; r++) for (int cc = 0; cc < 4; cc++) F.T[r * 4 + cc] = T[cc * 4 + r];
+  return F;
+}
+
 static_assert(sizeof(MergeFrame) <= GB_FRAME_DESC_BYTES, "frame descriptor scratch");
 gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T, void* d_frame, double4* pts, double* cov6) {
-  MergeFrame F;
-  F.p0 = c->p0; F.p1 = c->p1; F.p2 = c->p2; F.inv_perm = c->inv_perm; F.n = (int)c->n; F.offset = 0;
-  for (int r = 0; r < 3; r++) for (int cc = 0; cc < 4; cc++) F.T[r * 4 + cc] = T[cc * 4 + r];
   MergeFrame* h = nullptr;
   GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h = cv.take<MergeFrame>(1); }));
-  *h = F;
+  *h = merge_frame(c, T, 0);
   GB_CUDA(cudaMemcpyAsync(d_frame, h, sizeof(MergeFrame), cudaMemcpyHostToDevice, ctx->stream));
   const int n = (int)c->n;
   return gb_launch(ctx, "k_merge_transform", k_merge_transform, (n + 255) / 256, 256, 0, 1, (const MergeFrame*)d_frame, n, pts, cov6);
@@ -939,11 +912,8 @@ static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames,
   size_t total = 0;
   std::vector<MergeFrame> mf((size_t)K);
   for (int k = 0; k < K; k++) {
-    const gb_cloud* c = frames[k];
-    MergeFrame& F = mf[(size_t)k];
-    F.p0 = c->p0; F.p1 = c->p1; F.p2 = c->p2; F.inv_perm = c->inv_perm; F.n = (int)c->n; F.offset = (int)total;
-    for (int r = 0; r < 3; r++) for (int cc = 0; cc < 4; cc++) F.T[r * 4 + cc] = poses[(size_t)k * 16 + cc * 4 + r];
-    total += c->n;
+    mf[(size_t)k] = merge_frame(frames[k], poses + (size_t)k * 16, (int)total);
+    total += frames[k]->n;
   }
   *num_out = 0;
   if (total == 0) return GB_OK;
@@ -977,15 +947,14 @@ static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames,
   GB_CUDA(cudaMemsetAsync(d_cnt, 0, 256, st));
   const int tb = 256, gb = (n + tb - 1) / tb;
   GB_CHECK(gb_launch(ctx, "k_merge_transform", k_merge_transform, gb, tb, 0, K, d_mf, n, d_pts, d_cov));
-  GB_CHECK(gb_grid_keys(ctx, n, d_pts, 1.0 / resolution, t.keys, t.idx));
+  GB_CHECK(gb_grid_keys(ctx, n, d_pts, 1.0 / resolution, nullptr, t.keys, t.idx));
   GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
   GB_CHECK(gb_launch(ctx, "k_copy_last_pos", k_copy_last_pos, 1, 1, 0, n, d_pos, d_cnt));  // V
   GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
-  GB_CHECK(gb_launch(ctx, "k_merge_means", k_merge_means, (n + 127) / 128, 128, 0, d_cnt, d_starts, t.idx_s, d_pts, d_cov, d_vpts, d_vcov));
-  // thinning to target_num_points
-  GB_CHECK(gb_launch(ctx, "k_merge_hash_keys", k_merge_hash_keys, gb, tb, 0, n, d_cnt, seed, t.keys));
-  GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, cub_b, t.keys, t.keys_s, n, 0, 64);
-  GB_CHECK(gb_launch(ctx, "k_merge_keep", k_merge_keep, gb, tb, 0, n, d_cnt, target, t.keys_s, seed, d_keep));
+  GB_CHECK(gb_launch(ctx, "k_grid_means_counted", k_grid_means_counted, (n + 127) / 128, 128, 0, d_cnt, d_starts, t.idx_s, d_pts, nullptr, nullptr, d_cov, d_vpts, nullptr,
+                     nullptr, d_vcov));
+  // keep flag per voxel v < V (all, or the `target` smallest hashes), then an inclusive scan gives the output slot
+  GB_CHECK(gb_thin(ctx, n, nullptr, d_cnt, target, seed, t, d_keep));
   GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_keep, d_pos, n);
   int M = 0;
   GB_CUDA(cudaMemcpyAsync(&M, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));

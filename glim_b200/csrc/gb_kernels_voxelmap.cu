@@ -21,8 +21,9 @@
 //   6. host loop         num_buckets = init doubled until >= 8 V (load factor <= 1/8), then doubled again while
 //                        dropped points > drop_rate * N
 // Steps 2-3 (+ k_voxel_starts) are gb_group_by_key / gb_group_starts, shared with the voxel-grid downsampling and the frame
-// merge of gb_kernels_preprocess.cu.  Step 6 (table_build) also serves the incremental maps and iVoxes, whose one insert
-// pipeline is described below.  The map entry points (gb_voxelmap_*, gb_ivox_*) are defined here too.  This file also builds
+// merge of gb_kernels_preprocess.cu; the hash thinning of those paths and of the map insert (gb_thin) sits next to them.
+// Steps 1-3 with the voxel count are group_cloud, shared with the point grid.  Step 6 (table_build) also serves the
+// incremental maps and iVoxes, whose one insert pipeline is described below.  The map entry points (gb_voxelmap_*, gb_ivox_*) are defined here too.  This file also builds
 // every device cloud (gb_cloud_build: Morton reorder of staged planes), for gb_cloud_upload, gb_preprocess and gb_merge_frames.
 #include "gb_internal.cuh"
 
@@ -67,6 +68,21 @@ __global__ void k_voxel_starts(int n, const unsigned long long* __restrict__ key
   const bool valid = keys[i] != kInvalidKey;
   const bool next_valid = (i + 1 < n) && keys[i + 1] != kInvalidKey;
   if (valid && !next_valid) starts[pos[i]] = i + 1;
+}
+
+// the candidates of gb_thin: i with cand[i] != 0 (when given) and i < *count (when given)
+__device__ __forceinline__ bool thin_candidate(int i, const int* cand, const int* count) { return (!cand || cand[i]) && (!count || i < *count); }
+__global__ void k_thin_hash(int n, const int* __restrict__ cand, const int* __restrict__ count, unsigned long long seed, unsigned long long* __restrict__ hash) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) hash[i] = thin_candidate(i, cand, count) ? rg_hash(seed, (unsigned)i) : ~0ull;
+}
+// rg_hash is a bijection of the index for a fixed seed, so exactly the m smallest candidate hashes are <= sorted[m - 1]
+// (cand and keep may be the same array)
+__global__ void k_thin_keep(int n, const int* cand, const int* __restrict__ count, int m, unsigned long long seed, const unsigned long long* __restrict__ sorted, int* keep) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int c = count ? *count : n;
+  keep[i] = thin_candidate(i, cand, count) && (m <= 0 || m >= c || rg_hash(seed, (unsigned)i) <= sorted[m - 1]);
 }
 
 __global__ void k_voxel_reduce(int V, const int* __restrict__ starts, const unsigned long long* __restrict__ keys, const int* __restrict__ idx,
@@ -147,6 +163,13 @@ gb_status gb_group_starts(gb_ctx* ctx, int n, const gb_sort_tmp& t, const int* f
   return gb_launch(ctx, "k_voxel_starts", k_voxel_starts, (n + 255) / 256, 256, 0, n, t.keys_s, flags, pos, starts);
 }
 
+gb_status gb_thin(gb_ctx* ctx, int n, const int* cand, const int* count, int m, unsigned long long seed, const gb_sort_tmp& t, int* keep) {
+  const int blocks = (n + 255) / 256;
+  GB_CHECK(gb_launch(ctx, "k_thin_hash", k_thin_hash, blocks, 256, 0, n, cand, count, seed, t.keys));
+  GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, t.cub, t.cub_bytes, t.keys, t.keys_s, n, 0, 64);
+  return gb_launch(ctx, "k_thin_keep", k_thin_keep, blocks, 256, 0, n, cand, count, m, seed, t.keys_s, keep);
+}
+
 // The hash table of V voxels (vcoord[v] = {x, y, z, points}; d_dropped: one int of scratch, unused when V = 0): num_buckets =
 // init_buckets doubled until >= 8 V, then doubled again while more than drop_rate * total_points points fall out of it.
 // One host synchronisation per attempt.  On failure *buckets may hold a block the caller frees.
@@ -178,6 +201,34 @@ static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dr
   return GB_OK;
 }
 
+// The grouping of a cloud of n > 0 points by the build's fp32 key at inv_res, for the voxel-map build and the point grid: the
+// scratch, k_point_keys and gb_group_by_key, then the group count V read back (one host synchronisation).  starts is left for
+// gb_group_starts; vcoord and dropped are table_build's, extent the point grid's.
+struct CloudGroups {
+  gb_sort_tmp t;
+  int *flags, *pos, *starts, *dropped, *extent;
+  int4* vcoord;
+  int V = 0;
+};
+static gb_status group_cloud(gb_ctx* ctx, const gb_cloud* cloud, float inv_res, CloudGroups& g) {
+  const int n = (int)cloud->n;
+  const size_t cub_b = gb_cub_temp_bytes(n);
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+    g.t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
+    g.flags = cv.take<int>(n + 1);
+    g.pos = cv.take<int>(n + 1);
+    g.starts = cv.take<int>(n + 1);
+    g.vcoord = cv.take<int4>(n);
+    g.dropped = cv.take<int>(1);
+    g.extent = cv.take<int>(1);
+  }));
+  GB_CHECK(gb_launch(ctx, "k_point_keys", k_point_keys, (n + 255) / 256, 256, 0, n, cloud->p0, cloud->inv_perm, inv_res, g.t.keys, g.t.idx));
+  GB_CHECK(gb_group_by_key(ctx, n, g.t, g.flags, g.pos));
+  GB_CUDA(cudaMemcpyAsync(&g.V, g.pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return GB_OK;
+}
+
 // (the caller has made the map's device current)
 static void voxelmap_free(gb_voxelmap* m) {
   gb_dev_free(m->device, m->base);
@@ -195,41 +246,25 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
   gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(), voxelmap_free);
   if (!m) return GB_ERR_INTERNAL;
   const int n = (int)cloud->n;
-  cudaStream_t st = ctx->stream;
   m->device = ctx->device;
   m->resolution = resolution;
   m->inv_res = 1.0f / resolution;
   m->max_scan = max_bucket_scan_count;
 
-  int V = 0;
-  int4* d_vcoord = nullptr;
-  int* d_dropped = nullptr;
+  CloudGroups g{};
   if (n > 0) {
-    const size_t cub_b = gb_cub_temp_bytes(n);
-    gb_sort_tmp t;
-    int *d_flags, *d_pos, *d_starts;
-    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
-      t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
-      d_flags = cv.take<int>(n + 1);
-      d_pos = cv.take<int>(n + 1);
-      d_starts = cv.take<int>(n + 1);
-      d_vcoord = cv.take<int4>(n);
-      d_dropped = cv.take<int>(1);
-    }));
-    GB_CHECK(gb_launch(ctx, "k_point_keys", k_point_keys, (n + 255) / 256, 256, 0, n, cloud->p0, cloud->inv_perm, m->inv_res, t.keys, t.idx));
-    GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
-    GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    if (V > 0) {
-      GB_CUDA(gb_dev_malloc(ctx->device, sizeof(float4) * 3 * (size_t)V, &m->base));
+    GB_CHECK(group_cloud(ctx, cloud, m->inv_res, g));
+    if (g.V > 0) {
+      GB_CUDA(gb_dev_malloc(ctx->device, sizeof(float4) * 3 * (size_t)g.V, &m->base));
       m->voxels = (float4*)m->base;
-      GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
-      GB_CHECK(gb_launch(ctx, "k_voxel_reduce", k_voxel_reduce, (V + 127) / 128, 128, 0, V, d_starts, t.keys_s, t.idx_s, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm, m->voxels, d_vcoord));
+      GB_CHECK(gb_group_starts(ctx, n, g.t, g.flags, g.pos, g.starts));
+      GB_CHECK(gb_launch(ctx, "k_voxel_reduce", k_voxel_reduce, (g.V + 127) / 128, 128, 0, g.V, g.starts, g.t.keys_s, g.t.idx_s, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm,
+                         m->voxels, g.vcoord));
     }
   }
-  m->num_voxels = V;
-  m->bytes = sizeof(float4) * 3 * (size_t)V;
-  GB_CHECK(table_build(ctx, V, d_vcoord, d_dropped, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, (double)n, &m->buckets, &m->num_buckets,
+  m->num_voxels = g.V;
+  m->bytes = sizeof(float4) * 3 * (size_t)g.V;
+  GB_CHECK(table_build(ctx, g.V, g.vcoord, g.dropped, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, (double)n, &m->buckets, &m->num_buckets,
                        &m->num_dropped_points));
   m->bytes += sizeof(int4) * (size_t)m->num_buckets;
   *out = m.release();
@@ -242,8 +277,8 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
 //   1. old keys            the stored entries, tagged old (idx = -1 - entry), ahead of the points: one per voxel
 //                          (k_ins_old_keys) or one per stored iVox point (k_ivox_old_keys)
 //   2. k_merge_transform   (gb_transform_frame, shared with gb_merge_frames) q = R a + t, R C R^T in un-contracted fp64
-//   3. k_grid_keys         (gb_grid_keys) packed floor(q * key_inv_res) in fp64; with sampling_rate < 1 the points whose
-//                          rg_hash(seed, index) is not among the m smallest lose their key (k_ins_sample_*, one radix sort)
+//   3. k_grid_keys         (gb_grid_keys) packed floor(q * key_inv_res) in fp64; with sampling_rate < 1, gb_thin first keeps
+//                          the m points with the smallest rg_hash(seed, index) and the others get no key
 //   4. gb_group_by_key     stable: a voxel's group is its old entries first, then its new points in index order
 //   5. merge               one thread per merged voxel: the kind's per-voxel rule, then the LRU eviction (the same
 //                          expression in both merge kernels: a shared helper changes k_ivox_merge's SASS)
@@ -265,15 +300,6 @@ __global__ void k_ins_old_keys(int V, const unsigned long long* __restrict__ vke
   if (v >= V) return;
   keys[v] = vkeys[v];
   idx[v] = -1 - v;
-}
-__global__ void k_ins_sample_hash(int n, unsigned long long seed, unsigned long long* __restrict__ h) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) h[i] = rg_hash(seed, (unsigned)i);
-}
-// rg_hash is a bijection of the index for a fixed seed, so exactly the m smallest hashes are <= sorted[m - 1]
-__global__ void k_ins_sample_drop(int n, int m, unsigned long long seed, const unsigned long long* __restrict__ sorted, unsigned long long* __restrict__ keys) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n && rg_hash(seed, (unsigned)i) > sorted[m - 1]) keys[i] = kInvalidKey;
 }
 
 __global__ void k_ins_merge(int N, const int* __restrict__ num_merged, const int* __restrict__ starts, const int* __restrict__ idx_s,
@@ -449,7 +475,6 @@ struct InsertScratch {
   void* frame;
   double4* pts = nullptr;
   double* cov = nullptr;
-  unsigned long long* hash = nullptr;
 };
 
 // The per-voxel part of an incremental map: one stored entry per voxel, whose fp64 sums the new points continue.
@@ -558,20 +583,20 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
       if (np > 0) {
         s.pts = cv.take<double4>(np);
         s.cov = cv.take<double>(6 * (size_t)np);
-        if (kept < n) s.hash = cv.take<unsigned long long>(np);
       }
       rule.scratch(cv, (size_t)N);
     }));
-    const int tb = 256;
     if (m->num_voxels > 0) GB_CHECK(rule.old_keys(ctx, s.t));
     if (np > 0) {
       GB_CHECK(gb_transform_frame(ctx, cloud, T, s.frame, s.pts, s.cov));
-      GB_CHECK(gb_grid_keys(ctx, np, s.pts, m->key_inv_res, s.t.keys + No, s.t.idx + No));
+      const int* sampled = nullptr;  // the sampling's keep flags (in s.keep until the merge writes it)
       if (kept < n) {
-        GB_CHECK(gb_launch(ctx, "k_ins_sample_hash", k_ins_sample_hash, (np + tb - 1) / tb, tb, 0, np, seed, s.t.keys_s));
-        GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, s.t.cub, cub_b, s.t.keys_s, s.hash, np, 0, 64);
-        GB_CHECK(gb_launch(ctx, "k_ins_sample_drop", k_ins_sample_drop, (np + tb - 1) / tb, tb, 0, np, kept, seed, s.hash, s.t.keys + No));
+        gb_sort_tmp pt = s.t;  // the hashes pass through the points' keys, which k_grid_keys writes next
+        pt.keys += No;
+        GB_CHECK(gb_thin(ctx, np, nullptr, nullptr, kept, seed, pt, s.keep));
+        sampled = s.keep;
       }
+      GB_CHECK(gb_grid_keys(ctx, np, s.pts, m->key_inv_res, sampled, s.t.keys + No, s.t.idx + No));
     }
     GB_CHECK(gb_group_by_key(ctx, N, s.t, s.flags, s.pos));
     GB_CHECK(gb_group_starts(ctx, N, s.t, s.flags, s.pos, s.starts));
@@ -651,6 +676,21 @@ static gb_status download_records(const float4* records, size_t count, int32_t* 
     if (num_points) num_points[r] = (int32_t)c.y;
     if (xyz) { xyz[3 * r] = a.x; xyz[3 * r + 1] = a.y; xyz[3 * r + 2] = a.z; }
     if (cov6) { cov6[6 * r] = a.w; cov6[6 * r + 1] = b.x; cov6[6 * r + 2] = b.y; cov6[6 * r + 3] = b.z; cov6[6 * r + 4] = b.w; cov6[6 * r + 5] = c.x; }
+  }
+  return GB_OK;
+}
+// The cells of an iVox or a point grid to the host, as download_records copies: coords[3 v + a] decoded from the packed key,
+// counts[v] = the cell's points; either may be null.
+static gb_status download_cells(const gb_voxelmap* m, int32_t* coords, int32_t* counts) {
+  const size_t V = (size_t)m->num_voxels;
+  if (V == 0 || !(coords || counts)) return GB_OK;
+  std::vector<unsigned long long> keys(V);
+  std::vector<int2> cells(V);
+  GB_CUDA(cudaMemcpy(keys.data(), m->vkeys, sizeof(unsigned long long) * V, cudaMemcpyDefault));
+  GB_CUDA(cudaMemcpy(cells.data(), m->cells, sizeof(int2) * V, cudaMemcpyDefault));
+  for (size_t v = 0; v < V; v++) {
+    if (coords) gb_unpack_key(keys[v], coords[3 * v], coords[3 * v + 1], coords[3 * v + 2]);
+    if (counts) counts[v] = cells[v].y;
   }
   return GB_OK;
 }
@@ -750,25 +790,14 @@ extern "C" gb_status gb_ivox_info(const gb_ivox* map, int* num_voxels, size_t* n
 extern "C" gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords, int32_t* voxel_counts, float* xyz, float* cov6) {
   const gb_voxelmap* m = ivox_map(map);
   GB_REQUIRE(m && m->kind == GB_MAP_IVOX, "null map, or not an iVox");
-  const size_t V = (size_t)m->num_voxels;
-  if (V > 0 && (voxel_coords || voxel_counts)) {
-    std::vector<unsigned long long> keys(V);
-    std::vector<int2> cells(V);
-    GB_CUDA(cudaMemcpy(keys.data(), m->vkeys, sizeof(unsigned long long) * V, cudaMemcpyDefault));
-    GB_CUDA(cudaMemcpy(cells.data(), m->cells, sizeof(int2) * V, cudaMemcpyDefault));
-    for (size_t v = 0; v < V; v++) {
-      if (voxel_coords)
-        for (int a = 0; a < 3; a++) voxel_coords[3 * v + a] = (int32_t)((keys[v] >> (42 - 21 * a)) & 0x1FFFFF) - (1 << 20);
-      if (voxel_counts) voxel_counts[v] = cells[v].y;
-    }
-  }
+  GB_CHECK(download_cells(m, voxel_coords, voxel_counts));
   return download_records(m->voxels, m->num_points, nullptr, xyz, cov6);
 }
 extern "C" gb_status gb_ivox_destroy(gb_ivox* map) { return gb_voxelmap_destroy(ivox_map(map)); }
 
 // ---------------------------------------------------------------------------------------------
 // Point grid (gb_point_grid_build; the rule is written once in include/glim_b200.h): every point of a cloud, grouped by its
-// fp32 lookup key.  k_point_keys (the build's fp32 key per original index), gb_group_by_key / gb_group_starts (stable: a cell's
+// fp32 lookup key.  group_cloud (the build's fp32 key per original index, grouped) and gb_group_starts (stable: a cell's
 // points in original index order, the points without a key last), k_grid_emit (records, cells, keys, table coordinates and the
 // key extent), table_build with drop rate 0.  One host synchronisation for the cell count, one per table attempt.
 // ---------------------------------------------------------------------------------------------
@@ -826,27 +855,10 @@ extern "C" gb_status gb_point_grid_build(gb_ctx* ctx, const gb_cloud* cloud, dou
   g->init_buckets = 16384;
   const int n = (int)cloud->n;
   cudaStream_t st = ctx->stream;
-  int V = 0;
-  int4* d_vcoord = nullptr;
-  int* d_dropped = nullptr;
+  CloudGroups c{};
   if (n > 0) {
-    const size_t cub_b = gb_cub_temp_bytes(n);
-    gb_sort_tmp t;
-    int *d_flags, *d_pos, *d_starts, *d_extent;
-    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
-      t = gb_take_sort_tmp(cv, n, cv.take<char>(cub_b), cub_b);
-      d_flags = cv.take<int>(n + 1);
-      d_pos = cv.take<int>(n + 1);
-      d_starts = cv.take<int>(n + 1);
-      d_vcoord = cv.take<int4>(n);
-      d_dropped = cv.take<int>(1);
-      d_extent = cv.take<int>(1);
-    }));
-    GB_CHECK(gb_launch(ctx, "k_point_keys", k_point_keys, (n + 255) / 256, 256, 0, n, cloud->p0, cloud->inv_perm, g->inv_res, t.keys, t.idx));
-    GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
-    GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    g->num_voxels = V;
+    GB_CHECK(group_cloud(ctx, cloud, g->inv_res, c));
+    g->num_voxels = c.V;
     g->num_points = (size_t)n;
     Carver size;
     grid_layout(size, g.get());
@@ -854,13 +866,13 @@ extern "C" gb_status gb_point_grid_build(gb_ctx* ctx, const gb_cloud* cloud, dou
     g->bytes = size.off;
     Carver cv{(char*)g->base};
     grid_layout(cv, g.get());
-    GB_CUDA(cudaMemsetAsync(d_extent, 0, sizeof(int), st));
-    GB_CHECK(gb_group_starts(ctx, n, t, d_flags, d_pos, d_starts));
-    GB_CHECK(gb_launch(ctx, "k_grid_emit", k_grid_emit, (n + 255) / 256, 256, 0, n, t.keys_s, t.idx_s, d_flags, d_pos, d_starts, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm,
-                       g->voxels, g->cells, g->vkeys, d_vcoord, d_extent));
-    GB_CUDA(cudaMemcpyAsync(&g->key_extent, d_extent, sizeof(int), cudaMemcpyDeviceToHost, st));  // read by table_build's synchronisation
+    GB_CUDA(cudaMemsetAsync(c.extent, 0, sizeof(int), st));
+    GB_CHECK(gb_group_starts(ctx, n, c.t, c.flags, c.pos, c.starts));
+    GB_CHECK(gb_launch(ctx, "k_grid_emit", k_grid_emit, (n + 255) / 256, 256, 0, n, c.t.keys_s, c.t.idx_s, c.flags, c.pos, c.starts, cloud->p0, cloud->p1, cloud->p2,
+                       cloud->inv_perm, g->voxels, g->cells, g->vkeys, c.vcoord, c.extent));
+    GB_CUDA(cudaMemcpyAsync(&g->key_extent, c.extent, sizeof(int), cudaMemcpyDeviceToHost, st));  // read by table_build's synchronisation
   }
-  GB_CHECK(table_build(ctx, V, d_vcoord, d_dropped, g->init_buckets, g->max_scan, 0.0, (double)n, &g->buckets, &g->num_buckets, &g->num_dropped_points));
+  GB_CHECK(table_build(ctx, c.V, c.vcoord, c.dropped, g->init_buckets, g->max_scan, 0.0, (double)n, &g->buckets, &g->num_buckets, &g->num_dropped_points));
   g->bytes += sizeof(int4) * (size_t)g->num_buckets;
   if (g->num_dropped_points != 0) {
     gb_set_error("point grid table: %d points left out of a table of %d buckets", g->num_dropped_points, g->num_buckets);
@@ -880,18 +892,8 @@ extern "C" gb_status gb_point_grid_info(const gb_point_grid* grid, int* num_cell
 extern "C" gb_status gb_point_grid_download(const gb_point_grid* grid, int32_t* cell_coords, int32_t* cell_counts, int32_t* indices, float* xyz, float* cov6) {
   const gb_voxelmap* g = grid_map(grid);
   GB_REQUIRE(g && g->kind == GB_MAP_POINTS, "null grid, or not a point grid");
-  const size_t V = (size_t)g->num_voxels, P = g->num_points;
-  if (V > 0 && (cell_coords || cell_counts)) {
-    std::vector<unsigned long long> keys(V);
-    std::vector<int2> cells(V);
-    GB_CUDA(cudaMemcpy(keys.data(), g->vkeys, sizeof(unsigned long long) * V, cudaMemcpyDefault));
-    GB_CUDA(cudaMemcpy(cells.data(), g->cells, sizeof(int2) * V, cudaMemcpyDefault));
-    for (size_t v = 0; v < V; v++) {
-      if (cell_coords)
-        for (int a = 0; a < 3; a++) cell_coords[3 * v + a] = (int32_t)((keys[v] >> (42 - 21 * a)) & 0x1FFFFF) - (1 << 20);
-      if (cell_counts) cell_counts[v] = cells[v].y;
-    }
-  }
+  const size_t P = g->num_points;
+  GB_CHECK(download_cells(g, cell_coords, cell_counts));
   if (P > 0 && indices) {
     std::vector<float4> h(3 * P);
     GB_CUDA(cudaMemcpy(h.data(), g->voxels, sizeof(float4) * h.size(), cudaMemcpyDefault));

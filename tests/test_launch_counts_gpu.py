@@ -5,6 +5,7 @@ sweep graph; memsets and copies are not counted.  Each expected value below is w
 (and cub calls) of that path, so it can be read against the code.  Shared pieces:
     group    = gb_group_by_key: cub SortPairs + k_head_flags + cub InclusiveSum                   = 3
     starts   = gb_group_starts: k_voxel_starts                                                     = 1
+    thin     = gb_thin: k_thin_hash + cub SortKeys + k_thin_keep                                   = 3
     table    = one table_build attempt: k_table_clear + k_table_insert + k_table_finalize          = 3
     cloud    = gb_cloud_build: k_morton_keys + cub SortPairs + k_permute_cloud                     = 3
     knn      = knn_device: k_fill_self + k_ml_keys + cub SortPairs + k_ml_gather + k_ml_cells + k_knn_pyramid = 6"""
@@ -15,7 +16,7 @@ from glim_b200 import gpu, preprocess, synth
 
 pytestmark = pytest.mark.gpu
 
-GROUP, STARTS, TABLE, CLOUD, KNN = 3, 1, 3, 3, 6
+GROUP, STARTS, THIN, TABLE, CLOUD, KNN = 3, 1, 3, 3, 3, 6
 
 
 @pytest.fixture(scope="module")
@@ -60,9 +61,9 @@ def test_voxelmap_insert(ctx, scans):
     # k_ins_emit, table
     n, _ = launches(ctx, lambda: m.insert(c0))
     assert n == 2 + GROUP + STARTS + 3 + 1 + TABLE
-    # into a non-empty map, rate < 1: + k_ins_old_keys, + k_ins_sample_hash + cub SortKeys + k_ins_sample_drop
+    # into a non-empty map, rate < 1: + k_ins_old_keys, + thin
     n, _ = launches(ctx, lambda: m.insert(c1, scans[1], sampling_rate=0.1, seed=3))
-    assert n == 1 + 2 + 3 + GROUP + STARTS + 3 + 1 + TABLE
+    assert n == 1 + 2 + THIN + GROUP + STARTS + 3 + 1 + TABLE
 
 
 def test_overlap_covariances_and_deskew(ctx, scans):
@@ -98,7 +99,7 @@ PREPROCESS = {
     # k_set_int; downsampling; k_filter_time_keys + cub SortPairs + k_gather_frame; [outlier removal]; knn; k_covariances_planes; cloud
     "voxel_grid": (dict(downsample_resolution=0.5), 1 + (1 + GROUP + 1 + STARTS + 1) + 3 + KNN + 1 + CLOUD),  # k_grid_keys, group, k_copy_last_pos, starts, k_grid_means_counted
     "random_grid": (dict(downsample_resolution=0.5, use_random_grid_downsampling=True, downsample_rate=0.3),
-                    1 + (1 + GROUP + 1 + STARTS + 1 + 3) + 3 + KNN + 1 + CLOUD),  # ..., k_randomgrid_select, k_rg_hash_keys + cub SortKeys + k_rg_cap
+                    1 + (1 + GROUP + 1 + STARTS + 1 + THIN) + 3 + KNN + 1 + CLOUD),  # ..., k_randomgrid_select, thin
     "outlier_removal": (dict(downsample_resolution=0.5, enable_outlier_removal=True),
                         1 + (1 + GROUP + 1 + STARTS + 1) + 3 + (KNN + 6) + KNN + 1 + CLOUD),  # knn + k_sor_dists + 2 cub Sum + k_sor_flags + cub InclusiveSum + k_sor_compact
 }
@@ -119,9 +120,9 @@ def test_merge_frames(ctx, scans):
     frames = [gpu.PointCloudGPU.clone(pts0, cov0, ctx=ctx), gpu.PointCloudGPU.clone(pts1, cov1, ctx=ctx)]
     n, (out, _, cloud) = launches(ctx, lambda: gpu.merge_frames_gpu([np.eye(4), scans[1]], frames, 0.5, target_num_points=2000, seed=1, ctx=ctx))
     assert 0 < len(out) and cloud is not None
-    # k_merge_transform + k_grid_keys, group, k_copy_last_pos, starts, k_merge_means, k_merge_hash_keys + cub SortKeys +
-    # k_merge_keep + cub InclusiveSum, k_merge_emit, cloud
-    assert n == 2 + GROUP + 1 + STARTS + 1 + 4 + 1 + CLOUD
+    # k_merge_transform + k_grid_keys, group, k_copy_last_pos, starts, k_grid_means_counted, thin + cub InclusiveSum,
+    # k_merge_emit, cloud
+    assert n == 2 + GROUP + 1 + STARTS + 1 + THIN + 1 + 1 + CLOUD
 
 
 @pytest.mark.parametrize("path", ["graph", "plain"])
