@@ -1,5 +1,5 @@
 // gb_cov_math.cuh -- covariance and normal of one point (CloudCovarianceEstimation::estimate with PLANE regularisation,
-// cloud_covariance_estimation.cpp:80-102, :181-196), shared by k_covariances and k_covariances_planes.  Like
+// cloud_covariance_estimation.cpp:80-102, :181-196), the arithmetic of k_covariances_planes.  Like
 // gb_vgicp_math.cuh it holds nothing that only exists on the device, so the SAME TEXT compiles for the host:
 // tests/cpp/cov_math_host.cpp builds it with g++ and tests/test_cov_degenerate.py checks it bit for bit against the oracle.
 //

@@ -8,7 +8,7 @@
 // the host build agree bit for bit; division and sqrt are correctly rounded on both.  What remains between them is atan2 (the
 // pair feature f1 and the 4-DoF yaw), a few ulps apart: a bin can differ only for a feature within that distance of its edge.
 #pragma once
-#include "gb_grid_math.cuh"  // GB_HD, gb_coord, ivox_find, rg_hash, PoseF, the fp32 intrinsics' host shims
+#include "gb_grid_math.cuh"  // GB_HD, gb_coord, gb_lookup, rg_hash, PoseF, the fp32 intrinsics' host shims
 #include "gb_cov_math.cuh"   // cross3, dot3, the fp64 intrinsics' host shims
 
 namespace {
@@ -184,7 +184,7 @@ GB_HD bool ransac_inlier(const PoseF& P, float ax, float ay, float az, const int
   const float qy = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(P.r10, ax), __fmul_rn(P.r11, ay)), __fmul_rn(P.r12, az)), P.ty);
   const float qz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(P.r20, ax), __fmul_rn(P.r21, ay)), __fmul_rn(P.r22, az)), P.tz);
   if (!(isfinite(qx) && isfinite(qy) && isfinite(qz))) return false;
-  return ivox_find(buckets, mask, max_scan, gb_coord(qx, inv), gb_coord(qy, inv), gb_coord(qz, inv)) >= 0;
+  return gb_lookup(buckets, mask, max_scan, gb_coord(qx, inv), gb_coord(qy, inv), gb_coord(qz, inv)) >= 0;
 }
 
 }  // namespace

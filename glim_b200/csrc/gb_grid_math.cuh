@@ -4,7 +4,7 @@
 // rule (tests/grid_oracle.py) on the CPU-only box.  The rule is written once, in include/glim_b200.h (gb_point_grid_build,
 // gb_gicp_grid_factor_create).
 #pragma once
-#include "gb_ivox_math.cuh"  // GB_HD, gb_coord, gb_hash, ivox_find, the host shims of the fp32 intrinsics
+#include "gb_ivox_math.cuh"  // GB_HD, gb_coord, gb_lookup, point_d2, the host shims of the fp32 intrinsics
 
 #ifndef __CUDACC__
 #include <string.h>
@@ -46,11 +46,11 @@ inline int grid_half_width(float inv, float max_d2, int key_extent) {
 // The original index of a grid record (slot 2.z holds its bits).
 GB_HD int grid_record_index(const float4* __restrict__ points, int r) { return __float_as_int(points[3 * (size_t)r + 2].z); }
 
-// The correspondence of a transformed source point q: the stored point with the smallest fp32 d2 = (dx^2 + dy^2) + dz^2
-// (d = p - q, never contracted) among the cells c(q) + o, o in [-m, m]^3, if d2 < max_d2; ties go to the smaller original
-// index.  With m from grid_half_width this is the brute-force argmin over every stored point, whatever the visiting order.
-// Returns the record, -1 for none.  A NaN q keys to cell (0, 0, 0) and its distances are NaN: it never matches; a saturated
-// coordinate wraps out of the key range and finds nothing.
+// The correspondence of a transformed source point q: the stored point with the smallest fp32 d2 = point_d2(p, q) among the
+// cells c(q) + o, o in [-m, m]^3, if d2 < max_d2; ties go to the smaller original index.  With m from grid_half_width this is
+// the brute-force argmin over every stored point, whatever the visiting order.  Returns the record, -1 for none.  A NaN q keys
+// to cell (0, 0, 0) and its distances are NaN: it never matches; a saturated coordinate wraps out of the key range and finds
+// nothing.
 GB_HD int grid_nearest(const int4* __restrict__ buckets, uint32_t mask, int max_scan, const int2* __restrict__ cells, const float4* __restrict__ points,
                        int m, float inv, float max_d2, float qx, float qy, float qz) {
   const int cx = gb_coord(qx, inv), cy = gb_coord(qy, inv), cz = gb_coord(qz, inv);
@@ -59,14 +59,12 @@ GB_HD int grid_nearest(const int4* __restrict__ buckets, uint32_t mask, int max_
   for (int ox = -m; ox <= m; ox++) {
     for (int oy = -m; oy <= m; oy++) {
       for (int oz = -m; oz <= m; oz++) {
-        const int v = ivox_find(buckets, mask, max_scan, (int)((uint32_t)cx + (uint32_t)ox), (int)((uint32_t)cy + (uint32_t)oy), (int)((uint32_t)cz + (uint32_t)oz));
+        const int v = gb_lookup(buckets, mask, max_scan, (int)((uint32_t)cx + (uint32_t)ox), (int)((uint32_t)cy + (uint32_t)oy), (int)((uint32_t)cz + (uint32_t)oz));
         if (v < 0) continue;
         const int2 c = cells[v];
         for (int s = 0; s < c.y; s++) {
           const int r = c.x + s;
-          const float4 p = points[3 * (size_t)r];
-          const float ex = __fsub_rn(p.x, qx), ey = __fsub_rn(p.y, qy), ez = __fsub_rn(p.z, qz);
-          const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
+          const float d2 = point_d2(points[3 * (size_t)r], qx, qy, qz);
           if (d2 < best_d2) {
             best_d2 = d2;
             best = r;
@@ -80,7 +78,7 @@ GB_HD int grid_nearest(const int4* __restrict__ buckets, uint32_t mask, int max_
   return best;
 }
 
-// Every stored point p with fp32 d2(p, q) < max_d2 (d2 as in grid_nearest): visit(record) for each, cells in offset order and
+// Every stored point p with fp32 point_d2(p, q) < max_d2: visit(record) for each, cells in offset order and
 // the points of a cell in ascending original index.  With m from grid_half_width this is exactly the brute-force set (the proof
 // above bounds every such point, not only the nearest).  The FPFH neighbourhood of gb_cloud_estimate_fpfh.
 template <typename Visit>
@@ -90,14 +88,12 @@ GB_HD void grid_within(const int4* __restrict__ buckets, uint32_t mask, int max_
   for (int ox = -m; ox <= m; ox++) {
     for (int oy = -m; oy <= m; oy++) {
       for (int oz = -m; oz <= m; oz++) {
-        const int v = ivox_find(buckets, mask, max_scan, (int)((uint32_t)cx + (uint32_t)ox), (int)((uint32_t)cy + (uint32_t)oy), (int)((uint32_t)cz + (uint32_t)oz));
+        const int v = gb_lookup(buckets, mask, max_scan, (int)((uint32_t)cx + (uint32_t)ox), (int)((uint32_t)cy + (uint32_t)oy), (int)((uint32_t)cz + (uint32_t)oz));
         if (v < 0) continue;
         const int2 c = cells[v];
         for (int s = 0; s < c.y; s++) {
           const int r = c.x + s;
-          const float4 p = points[3 * (size_t)r];
-          const float ex = __fsub_rn(p.x, qx), ey = __fsub_rn(p.y, qy), ez = __fsub_rn(p.z, qz);
-          const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
+          const float d2 = point_d2(points[3 * (size_t)r], qx, qy, qz);
           if (d2 < max_d2) visit(r);
         }
       }

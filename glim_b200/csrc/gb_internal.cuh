@@ -462,10 +462,10 @@ inline gb_planes gb_cloud_planes(Carver& cv, size_t n, bool normals) {
   return p;
 }
 gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n, const gb_planes& staged, const gb_sort_tmp& t);
-// The covariance stage of gb_preprocess (gb_kernels_preprocess.cu), shared with gb_ct_deskew: plane_covariance of the first
-// *d_count of M points (pts, neighbors[i * kc + j], the first k of each row) into the fp64 normals (M x double4) and covs
-// (M x 16, column-major), and the fp32 planes staged for the cloud; then, when cloud_out is given, the cloud (gb_cloud_build
-// with t).  One launch plus the build's.
+// The covariance stage of gb_preprocess (gb_kernels_preprocess.cu), shared with gb_ct_deskew and gb_covariances:
+// plane_covariance of the first *d_count of M points (pts, neighbors[i * kc + j], the first k of each row) into the fp64
+// normals (M x double4) and covs (M x 16, column-major), and, when staged.p0 is given, the fp32 planes staged for the cloud;
+// then, when cloud_out is given, the cloud (gb_cloud_build with t).  One launch plus the build's.
 gb_status gb_covariance_cloud(gb_ctx* ctx, int M, const int* d_count, const double4* pts, const int* neighbors, int kc, int k, double4* normals, double* covs,
                               const gb_planes& staged, const gb_sort_tmp& t, gb_cloud* cloud_out);
 
@@ -487,7 +487,7 @@ gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, c
 // device helpers shared by kernels
 // ---------------------------------------------------------------------------------------------
 #ifdef __CUDACC__
-#include "gb_vgicp_math.cuh"  // gb_coord, gb_hash (shared with the host-compiled CPU test of the kernel arithmetic)
+#include "gb_vgicp_math.cuh"  // gb_coord, gb_hash, gb_lookup (shared with the host-compiled CPU test of the kernel arithmetic)
 // packed 3 x 21-bit voxel key (ascending key = canonical voxel order); false if out of range
 #define GB_KEY_OFFSET (1 << 20)
 constexpr unsigned long long kInvalidKey = ~0ull;  // the key of a point in no voxel: sorts last
@@ -510,15 +510,5 @@ __device__ __forceinline__ unsigned long long gb_spread21(unsigned long long v) 
   v = (v | (v << 4)) & 0x10C30C30C30C30C3ull;
   v = (v | (v << 2)) & 0x1249249249249249ull;
   return v;
-}
-// linear-probing lookup (SURVEY B.4)
-__device__ __forceinline__ int gb_lookup(const int4* __restrict__ buckets, uint32_t mask, int max_scan, int cx, int cy, int cz) {
-  const uint32_t h = gb_hash(cx, cy, cz);
-  for (int i = 0; i < max_scan; i++) {
-    const int4 b = __ldg(&buckets[(h + (uint32_t)i) & mask]);
-    if (b.w < 0) return -1;
-    if (b.x == cx && b.y == cy && b.z == cz) return b.w;
-  }
-  return -1;
 }
 #endif

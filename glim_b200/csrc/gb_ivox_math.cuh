@@ -3,7 +3,7 @@
 // tests/cpp/ivox_search_host.cpp builds it with g++ and tests/test_ivox_host.py checks it against the numpy restatement of the
 // rule (tests/ivox_oracle.py) on the CPU-only box.  The rule is written once, in include/glim_b200.h (gb_gicp_factor_create).
 #pragma once
-#include "gb_vgicp_math.cuh"  // GB_HD, gb_coord, gb_hash, PoseF, transform
+#include "gb_vgicp_math.cuh"  // GB_HD, gb_coord, gb_lookup, PoseF, transform
 
 #ifndef __CUDACC__
 struct int2 { int x, y; };
@@ -12,6 +12,13 @@ static inline float __fmul_rn(float a, float b) { return a * b; }
 static inline float __fadd_rn(float a, float b) { return a + b; }
 static inline float __fsub_rn(float a, float b) { return a - b; }
 #endif
+
+// fp32 squared distance of a stored point p to q in one fixed order, (ex * ex + ey * ey) + ez * ez with e = p - q, never
+// contracted
+GB_HD float point_d2(const float4 p, float qx, float qy, float qz) {
+  const float ex = __fsub_rn(p.x, qx), ey = __fsub_rn(p.y, qy), ez = __fsub_rn(p.z, qz);
+  return __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
+}
 
 namespace {
 
@@ -39,20 +46,8 @@ GB_HD void ivox_offset(int k, int& dx, int& dy, int& dz) {
   dx = (c & 4) ? 1 : -1; dy = (c & 2) ? 1 : -1; dz = (c & 1) ? 1 : -1;
 }
 
-// linear-probing lookup of voxel (cx, cy, cz) in the iVox's table: its index, -1 if absent
-GB_HD int ivox_find(const int4* __restrict__ buckets, uint32_t mask, int max_scan, int cx, int cy, int cz) {
-  const uint32_t h = gb_hash(cx, cy, cz);
-  for (int i = 0; i < max_scan; i++) {
-    const int4 b = buckets[(h + (uint32_t)i) & mask];
-    if (b.w < 0) return -1;
-    if (b.x == cx && b.y == cy && b.z == cz) return b.w;
-  }
-  return -1;
-}
-
 // The correspondence of a transformed source point q: the stored point nearest to q among the points of the searched voxels,
-// if its squared distance is below max_d2; -1 otherwise.  Distances are fp32 in one fixed order,
-// d2 = (dx * dx + dy * dy) + dz * dz with d = p - q, never contracted; a tie keeps the earlier offset, then the earlier slot.
+// if its squared distance (point_d2) is below max_d2; -1 otherwise.  A tie keeps the earlier offset, then the earlier slot.
 // A NaN q keys to voxel (0, 0, 0) and its distances are NaN: it never matches.
 GB_HD int ivox_nearest(const int4* __restrict__ buckets, uint32_t mask, int max_scan, const int2* __restrict__ cells, const float4* __restrict__ points,
                        int num_offsets, float inv_res, float max_d2, float qx, float qy, float qz) {
@@ -63,13 +58,11 @@ GB_HD int ivox_nearest(const int4* __restrict__ buckets, uint32_t mask, int max_
     int dx, dy, dz;
     ivox_offset(k, dx, dy, dz);
     // wrapping sums: a saturated coordinate (a point far outside the key range) finds nothing
-    const int v = ivox_find(buckets, mask, max_scan, (int)((uint32_t)cx + (uint32_t)dx), (int)((uint32_t)cy + (uint32_t)dy), (int)((uint32_t)cz + (uint32_t)dz));
+    const int v = gb_lookup(buckets, mask, max_scan, (int)((uint32_t)cx + (uint32_t)dx), (int)((uint32_t)cy + (uint32_t)dy), (int)((uint32_t)cz + (uint32_t)dz));
     if (v < 0) continue;
     const int2 c = cells[v];
     for (int s = 0; s < c.y; s++) {
-      const float4 p = points[3 * (size_t)(c.x + s)];
-      const float ex = __fsub_rn(p.x, qx), ey = __fsub_rn(p.y, qy), ez = __fsub_rn(p.z, qz);
-      const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
+      const float d2 = point_d2(points[3 * (size_t)(c.x + s)], qx, qy, qz);
       if (d2 < best_d2) { best_d2 = d2; best = c.x + s; }
     }
   }

@@ -16,7 +16,6 @@
 
 #include <cub/cub.cuh>
 #include <cmath>
-#include <stdlib.h>
 #include <string.h>
 #include <algorithm>
 #include <new>
@@ -24,74 +23,11 @@
 
 namespace {
 
-// ---------------------------------------------------------------------------------------------
-// exact k-NN, brute force over shared-memory tiles.  One query per thread, candidates streamed
-// in ascending index with a strict '<' insertion, so ties resolve to the lower index exactly as
-// in the oracle.  The query itself is a candidate (distance 0), as in the reference (:196).
-// ---------------------------------------------------------------------------------------------
-template <int K>
-__global__ void __launch_bounds__(128) k_knn_bruteforce(int n, const double4* __restrict__ pts, int* __restrict__ neighbors) {
-  constexpr int TILE = 256;
-  __shared__ double sx[TILE], sy[TILE], sz[TILE];
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  double px = 0, py = 0, pz = 0;
-  if (i < n) { const double4 p = pts[i]; px = p.x; py = p.y; pz = p.z; }
-  double bd[K];
-  int bi[K];
-#pragma unroll
-  for (int k = 0; k < K; k++) { bd[k] = 1e300; bi[k] = i; }
-  int cnt = 0;
-  for (int base = 0; base < n; base += TILE) {
-    __syncthreads();
-    for (int t = threadIdx.x; t < TILE; t += blockDim.x) {
-      const int j = base + t;
-      if (j < n) { const double4 q = pts[j]; sx[t] = q.x; sy[t] = q.y; sz[t] = q.z; }
-    }
-    __syncthreads();
-    const int m = min(TILE, n - base);
-    if (i < n) {
-      for (int t = 0; t < m; t++) {
-        const double dx = px - sx[t], dy = py - sy[t], dz = pz - sz[t];
-        // no FMA contraction: bit-identical to the oracle's (dx*dx + dy*dy) + dz*dz
-        const double d = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-        if (d < bd[K - 1]) {
-          // insert (d, base+t) keeping ascending (distance, index): equal distances stay behind lower indices, also for an
-          // entry pushed down by the insertion (a new nearer candidate must not drop a tied lower index at the tail)
-          double cd = d;
-          int ci = base + t;
-#pragma unroll
-          for (int k = 0; k < K; k++) {
-            if (cd < bd[k] || (cd == bd[k] && ci < bi[k])) {
-              const double td = bd[k]; const int ti = bi[k];
-              bd[k] = cd; bi[k] = ci; cd = td; ci = ti;
-            }
-          }
-          cnt++;
-        }
-      }
-    }
-  }
-  if (i < n) {
-    const int found = min(cnt, K);
-#pragma unroll
-    for (int k = 0; k < K; k++) neighbors[(size_t)i * K + k] = k < found ? bi[k] : i;
-  }
-}
-
 // fp64 4x4 column-major covariance of the host layout
 __device__ __forceinline__ void store_cov4x4(double* __restrict__ Co, const double (&C)[9]) {
   for (int e = 0; e < 16; e++) Co[e] = 0.0;
   for (int r = 0; r < 3; r++)
     for (int c = 0; c < 3; c++) Co[c * 4 + r] = C[r * 3 + c];
-}
-
-__global__ void __launch_bounds__(128) k_covariances(int n, const double4* __restrict__ pts, const int* __restrict__ neighbors, int kc, int k, double4* __restrict__ normals, double* __restrict__ covs) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  double C[9], nrm[3];
-  plane_covariance(i, pts, neighbors, kc, k, C, nrm);
-  store_cov4x4(covs + 16 * (size_t)i, C);
-  normals[i] = make_double4(nrm[0], nrm[1], nrm[2], 0.0);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -144,18 +80,18 @@ gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, c
   return gb_launch(ctx, "k_grid_keys", k_grid_keys, (n + 255) / 256, 256, 0, n, pts, inv_res, keep, keys, idx);
 }
 
-// Returns launch(std::integral_constant<int, K>()) for the instantiated neighbour counts K of the k-NN kernels.
+// Returns launch(std::integral_constant<int, K>()) for the instantiated neighbour counts K of k_knn_pyramid.
 template <typename Launch> static gb_status knn_dispatch(int k, Launch&& launch) {
   switch (k) {
-#define GB_KNN_CASE(K) case K: return launch(std::integral_constant<int, K>());
-    GB_KNN_CASE(1) GB_KNN_CASE(2) GB_KNN_CASE(3) GB_KNN_CASE(4) GB_KNN_CASE(5) GB_KNN_CASE(6) GB_KNN_CASE(7) GB_KNN_CASE(8)
-    GB_KNN_CASE(9) GB_KNN_CASE(10) GB_KNN_CASE(12) GB_KNN_CASE(15) GB_KNN_CASE(16) GB_KNN_CASE(20) GB_KNN_CASE(24) GB_KNN_CASE(32)
-#undef GB_KNN_CASE
+#define KNN_CASE(K) case K: return launch(std::integral_constant<int, K>());
+    KNN_CASE(1) KNN_CASE(2) KNN_CASE(3) KNN_CASE(4) KNN_CASE(5) KNN_CASE(6) KNN_CASE(7) KNN_CASE(8)
+    KNN_CASE(9) KNN_CASE(10) KNN_CASE(12) KNN_CASE(15) KNN_CASE(16) KNN_CASE(20) KNN_CASE(24) KNN_CASE(32)
+#undef KNN_CASE
   }
   gb_set_error("k = %d is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)", k);
   return GB_ERR_INVALID_ARGUMENT;
 }
-// true iff the k-NN kernels are instantiated for k neighbours; entry points check it before any launch
+// true iff k_knn_pyramid is instantiated for k neighbours; entry points check it before any launch
 static bool gb_knn_instantiated(int k) {
   return knn_dispatch(k, [](auto) { return GB_OK; }) == GB_OK;
 }
@@ -168,23 +104,6 @@ size_t gb_cub_temp_bytes(size_t n_) {
   cub::DeviceScan::InclusiveSum(nullptr, scan, (int*)nullptr, (int*)nullptr, n);
   cub::DeviceReduce::Sum(nullptr, sum, (double*)nullptr, (double*)nullptr, n);
   return std::max({sort_pairs, sort_keys, scan, sum});
-}
-
-// gb_find_neighbors by brute force
-static gb_status find_neighbors_brute(gb_ctx* ctx, size_t n_, const double* xyzw, int k, int32_t* neighbors) {
-  const int n = (int)n_;
-  cudaStream_t st = ctx->stream;
-  double4* d_pts;
-  int* d_nb;
-  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
-    d_pts = cv.take<double4>(n);
-    d_nb = cv.take<int>((size_t)n * k);
-  }));
-  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * (size_t)n, cudaMemcpyHostToDevice, st));
-  GB_CHECK(knn_dispatch(k, [&](auto K) { return gb_launch(ctx, "k_knn_bruteforce", k_knn_bruteforce<decltype(K)::value>, (n + 127) / 128, 128, 0, n, d_pts, d_nb); }));
-  GB_CUDA(cudaMemcpyAsync(neighbors, d_nb, sizeof(int) * (size_t)n * k, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  return GB_OK;
 }
 
 extern "C" gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, const int32_t* neighbors, int k_correspondences, int k_neighbors, double* normals4, double* cov4x4) {
@@ -203,17 +122,20 @@ extern "C" gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, c
   GB_ENTER(ctx);
   cudaStream_t st = ctx->stream;
   double4 *d_pts, *d_nrm;
-  int* d_nb;
+  int *d_nb, *d_cnt;
   double* d_cov;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     d_pts = cv.take<double4>(n);
     d_nb = cv.take<int>(n * k_correspondences);
     d_nrm = cv.take<double4>(n);
     d_cov = cv.take<double>(16 * n);
+    d_cnt = cv.take<int>(1);
   }));
+  const int count = (int)n;
+  GB_CUDA(cudaMemcpyAsync(d_cnt, &count, sizeof(int), cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * n, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemcpyAsync(d_nb, neighbors, sizeof(int) * n * k_correspondences, cudaMemcpyHostToDevice, st));
-  GB_CHECK(gb_launch(ctx, "k_covariances", k_covariances, (n + 127) / 128, 128, 0, (int)n, d_pts, d_nb, k_correspondences, k_neighbors, d_nrm, d_cov));
+  GB_CHECK(gb_covariance_cloud(ctx, count, d_cnt, d_pts, d_nb, k_correspondences, k_neighbors, d_nrm, d_cov, gb_planes{}, gb_sort_tmp{}, nullptr));
   GB_CUDA(cudaMemcpyAsync(normals4, d_nrm, sizeof(double4) * n, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaMemcpyAsync(cov4x4, d_cov, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
@@ -347,7 +269,7 @@ __device__ __forceinline__ void knn_insert(double (&bd)[K], int (&bi)[K], int& c
 // Exact k-NN on the pyramid: a query searches the 3x3x3 block of cells around it at the finest level; every unseen point is
 // then at least (1 + min(u, 1 - u)) * h away (u = position inside its cell), so the answer is complete as soon as the k-th
 // best distance is within that bound.  Otherwise the query moves one level up (4x larger cells); after the coarsest level it
-// scans all points.  Same un-contracted fp64 distance and (distance, index) tie rule as the brute-force kernel and the oracle.
+// scans all points.  Same un-contracted fp64 distance and (distance, index) tie rule as the oracle.
 template <int K>
 __global__ void __launch_bounds__(128) k_knn_pyramid(int n, const double4* __restrict__ pts_s, const unsigned long long* __restrict__ keys_s, const int* __restrict__ idx_s,
                                                      const MlCell* __restrict__ tables, unsigned table_size, double inv_h0, double h0, int* __restrict__ neighbors) {
@@ -519,7 +441,7 @@ __global__ void k_gather_frame(int n_upper, const int* __restrict__ count, const
 __global__ void k_set_int(int* p, int v) { *p = v; }
 __global__ void k_copy_last_pos(int n, const int* __restrict__ pos, int* __restrict__ out) { *out = n > 0 ? pos[n - 1] : 0; }
 
-// covariance estimation (plane_covariance, as k_covariances) writing the fp64 host-layout outputs AND the fp32 planes of the
+// covariance estimation (plane_covariance) writing the fp64 host-layout outputs and, when s0 is given, the fp32 planes of the
 // device cloud in the caller's point order (the Morton reorder of gb_cloud_upload follows)
 __global__ void __launch_bounds__(128) k_covariances_planes(int n_upper, const int* __restrict__ count, const double4* __restrict__ pts, const int* __restrict__ neighbors, int kc, int k,
                                                             double4* __restrict__ normals, double* __restrict__ covs, float4* __restrict__ s0, float4* __restrict__ s1, float* __restrict__ s2, float4* __restrict__ s3) {
@@ -530,6 +452,7 @@ __global__ void __launch_bounds__(128) k_covariances_planes(int n_upper, const i
   const double nx = nrm[0], ny = nrm[1], nz = nrm[2];
   if (normals) normals[i] = make_double4(nx, ny, nz, 0.0);
   if (covs) store_cov4x4(covs + 16 * (size_t)i, C);
+  if (!s0) return;
   // the host cast of PointCloudGPU::clone (fp64 -> fp32), upper triangle as gb_cloud_upload reads it from the column-major 4x4
   s0[i] = make_float4((float)p.x, (float)p.y, (float)p.z, (float)C[0]);
   s1[i] = make_float4((float)C[1], (float)C[2], (float)C[4], (float)C[5]);
@@ -797,8 +720,13 @@ extern "C" gb_status gb_preprocess(gb_ctx* ctx, size_t n, const double* xyzw, co
   return GB_OK;
 }
 
-// gb_find_neighbors on the pyramid (host arrays in / out; the device-resident entry is inside gb_preprocess)
-static gb_status find_neighbors_pyramid(gb_ctx* ctx, size_t n_, const double* xyzw, int k, int32_t* neighbors) {
+// knn_device with cell size 0.25 m on host arrays (the device-resident entry is inside gb_preprocess)
+extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n_, const double* xyzw, int k, int32_t* neighbors) {
+  GB_REQUIRE(ctx, "null ctx");
+  if (n_ == 0) return GB_OK;
+  GB_REQUIRE(xyzw && neighbors && k > 0, "null argument");
+  GB_REQUIRE(gb_knn_instantiated(k), "k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
+  GB_ENTER(ctx);
   const int n = (int)n_;
   cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n, cub_b = gb_cub_temp_bytes(N);
@@ -817,20 +745,6 @@ static gb_status find_neighbors_pyramid(gb_ctx* ctx, size_t n_, const double* xy
   GB_CUDA(cudaMemcpyAsync(neighbors, d_nb, sizeof(int) * N * (size_t)k, cudaMemcpyDeviceToHost, st));
   GB_CUDA(cudaStreamSynchronize(st));
   return GB_OK;
-}
-
-extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors) {
-  GB_REQUIRE(ctx, "null ctx");
-  if (n == 0) return GB_OK;
-  GB_REQUIRE(xyzw && neighbors && k > 0, "null argument");
-  GB_REQUIRE(gb_knn_instantiated(k), "k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
-  GB_ENTER(ctx);
-  // >= 4096 points: exact search on a pyramid of hash grids (one Morton sort, cell size 0.25 m x 4^level); fewer: the tiled
-  // brute force.  GB_KNN=pyramid / brute forces one.
-  const char* mode = getenv("GB_KNN");
-  const bool pyramid = mode ? (strcmp(mode, "pyramid") == 0) : (n >= 4096);
-  if (pyramid) return find_neighbors_pyramid(ctx, n, xyzw, k, neighbors);
-  return find_neighbors_brute(ctx, n, xyzw, k, neighbors);
 }
 
 // =============================================================================================

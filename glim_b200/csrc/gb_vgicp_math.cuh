@@ -28,6 +28,16 @@ GB_HD int gb_coord(float p, float inv_res) { return __float2int_rd(p * inv_res);
 GB_HD uint32_t gb_hash(int x, int y, int z) {
   return ((uint32_t)x * 73856093u) ^ ((uint32_t)y * 19349669u) ^ ((uint32_t)z * 83492791u);
 }
+// linear-probing lookup of voxel (cx, cy, cz) in a voxel table (SURVEY B.4): its index, -1 if absent
+GB_HD int gb_lookup(const int4* __restrict__ buckets, uint32_t mask, int max_scan, int cx, int cy, int cz) {
+  const uint32_t h = gb_hash(cx, cy, cz);
+  for (int i = 0; i < max_scan; i++) {
+    const int4 b = buckets[(h + (uint32_t)i) & mask];
+    if (b.w < 0) return -1;
+    if (b.x == cx && b.y == cy && b.z == cz) return b.w;
+  }
+  return -1;
+}
 // the project's fixed pseudo-random pick ([EXT]: the reference draws with std::mt19937): the points / voxels with the smallest
 // rg_hash(seed, index) are kept (random-grid downsampling, frame-merge thinning, voxel-map insert sampling; the oracle shares it),
 // and RANSAC draws its samples from it (gb_global_math.cuh)

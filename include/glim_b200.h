@@ -559,7 +559,10 @@ GB_API gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, const
 
 /* ---- CloudPreprocessor::find_neighbors (src/glim/preprocess/cloud_preprocessor.cpp:190-221): exact k-NN,
  *      query included, row-major neighbors[i*k + j].  k in {1-10, 12, 15, 16, 20, 24, 32}, else GB_ERR_INVALID_ARGUMENT
- *      before any launch (the same set for k_correspondences and outlier_removal_k of gb_preprocess) ---- */
+ *      before any launch (the same set for k_correspondences and outlier_removal_k of gb_preprocess).  The search is
+ *      gb_preprocess's grid pyramid with knn_cell_size 0.25 m: a point that is not finite, or whose 0.25 m cell lies outside
+ *      the 21-bit range (a coordinate outside [-262144, 262144) m), gets a row of its own index and is no point's neighbour,
+ *      at every cloud size ---- */
 GB_API gb_status gb_find_neighbors(gb_ctx* ctx, size_t n, const double* xyzw, int k, int32_t* neighbors);
 
 /* ---- gtsam_points::voxelgrid_sampling (cloud_preprocessor.cpp:108): one point per voxel = mean of

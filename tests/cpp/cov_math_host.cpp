@@ -1,5 +1,5 @@
-// Host build of the covariance kernels' per-point arithmetic (glim_b200/csrc/gb_cov_math.cuh -- the SAME text k_covariances
-// and k_covariances_planes compile), laid out like go_covariance_estimate.  TEST INFRASTRUCTURE: built by
+// Host build of the covariance kernel's per-point arithmetic (glim_b200/csrc/gb_cov_math.cuh -- the SAME text
+// k_covariances_planes compiles), laid out like go_covariance_estimate.  TEST INFRASTRUCTURE: built by
 // tests/test_cov_degenerate.py with g++ -ffp-contract=off and compared bit for bit with the CPU oracle; nothing in the product
 // links it.
 #include <stddef.h>

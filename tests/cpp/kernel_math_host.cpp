@@ -9,17 +9,6 @@
 
 namespace {
 
-// linear probing exactly as gb_lookup / resolve_probe (gb_internal.cuh, gb_kernels_vgicp.cu)
-int lookup(const int4* buckets, uint32_t mask, int max_scan, int cx, int cy, int cz) {
-  const uint32_t h = gb_hash(cx, cy, cz);
-  for (int i = 0; i < max_scan; i++) {
-    const int4 b = buckets[(h + (uint32_t)i) & mask];
-    if (b.w < 0) return -1;
-    if (b.x == cx && b.y == cy && b.z == cz) return b.w;
-  }
-  return -1;
-}
-
 // warp_reduce_scatter32 of the kernel, lanes as an array index: on return v[l][0] = sum over lanes of v[.][l]
 void reduce_scatter32(float (*v)[32]) {
   for (int step = 16; step >= 1; step >>= 1) {
@@ -67,7 +56,7 @@ extern "C" int km_sweep(int n, const float* p0, const float* p1, const float* p2
       for (int i = wb; i < we; i++) {  // phase A
         float qx, qy, qz;
         transform(P, P0[i].x, P0[i].y, P0[i].z, qx, qy, qz);
-        const int v = lookup(B, mask, max_scan, gb_coord(qx, inv_res), gb_coord(qy, inv_res), gb_coord(qz, inv_res));
+        const int v = gb_lookup(B, mask, max_scan, gb_coord(qx, inv_res), gb_coord(qy, inv_res), gb_coord(qz, inv_res));
         if (corr) corr[i] = v;
         if (v >= 0) { qi[nq] = i; qv[nq] = v; nq++; }
       }

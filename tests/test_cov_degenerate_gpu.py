@@ -148,20 +148,18 @@ def _knn_clouds():
     return {"lattice": lattice, "duplicates": dup}
 
 
-@pytest.mark.parametrize("mode", ["brute", "pyramid"])
-def test_knn_is_exact_at_every_instantiated_k(ctx, monkeypatch, mode):
-    monkeypatch.setenv("GB_KNN", mode)
-    for name, cloud in _knn_clouds().items():
-        for k in KNN_KS:
-            nb = preprocess.find_neighbors(cloud, k, ctx=ctx).reshape(len(cloud), k)
-            ref, _ = oracle.knn_bruteforce(cloud, k)
-            assert np.array_equal(nb, ref), (name, k)
+@pytest.mark.parametrize("name", ["lattice", "duplicates"])
+def test_knn_is_exact_at_every_instantiated_k(ctx, name):
+    cloud = _knn_clouds()[name]
+    for k in KNN_KS:
+        nb = preprocess.find_neighbors(cloud, k, ctx=ctx).reshape(len(cloud), k)
+        ref, _ = oracle.knn_bruteforce(cloud, k)
+        assert np.array_equal(nb, ref), (name, k)
 
 
-@pytest.mark.parametrize("mode", ["brute", "pyramid"])
-def test_uninstantiated_k_and_bad_indices_are_rejected_before_any_launch(ctx, monkeypatch, mode):
-    monkeypatch.setenv("GB_KNN", mode)
-    P = _knn_clouds()["lattice"]
+@pytest.mark.parametrize("name", ["lattice", "duplicates"])
+def test_uninstantiated_k_and_bad_indices_are_rejected_before_any_launch(ctx, name):
+    P = _knn_clouds()[name]
     n = len(P)
     L = lib()
     before = ctx.kernel_launches

@@ -579,11 +579,11 @@ def test_gb_preprocess_matches_oracle_pipeline(ctx, mode):
     assert np.array_equal(fr2.points, fr.points) and np.array_equal(fr2.neighbors, fr.neighbors)
 
 
-def test_pyramid_knn_is_exact_on_hard_clouds(ctx, monkeypatch):
-    """The grid-pyramid k-NN on duplicated points, far outliers (coarsest-level / full-scan fallback), tiny clouds."""
+def test_pyramid_knn_is_exact_on_hard_clouds(ctx):
+    """The grid-pyramid k-NN on duplicated points, far outliers (coarsest-level / full-scan fallback), tiny clouds; a point
+    whose 0.25 m cell is outside the 21-bit key range gets a row of itself and is no point's neighbour, whatever the size."""
     from glim_b200 import preprocess
 
-    monkeypatch.setenv("GB_KNN", "pyramid")
     P = util.scan_pair(n_rays=32 * 100)["points"][0]
     rng = synth.rng_for(31)
     dup = np.concatenate([P[:500], P[:500], P[100:200] + [1e-9, 0, 0, 0], [[500.0, -300.0, 20.0, 1.0], [-800.0, 10.0, 5.0, 1.0]], rng.normal(0, 0.01, (64, 4)) * [1, 1, 1, 0] + [3, 3, 3, 1]])
@@ -592,6 +592,9 @@ def test_pyramid_knn_is_exact_on_hard_clouds(ctx, monkeypatch):
             nb = preprocess.find_neighbors(cloud, k, ctx=ctx).reshape(len(cloud), k)
             ref, _ = oracle.knn_bruteforce(cloud, k)
             assert np.array_equal(nb, ref)
+    far = np.concatenate([P[:300], [[3e5, 0.0, 0.0, 1.0]]])
+    nb = preprocess.find_neighbors(far, 10, ctx=ctx).reshape(len(far), 10)
+    assert np.array_equal(nb[:300], oracle.knn_bruteforce(P[:300], 10)[0]) and (nb[300] == 300).all()
 
 
 def test_merge_frames_gpu_matches_oracle(ctx):

@@ -75,17 +75,17 @@ def test_overlap_covariances_and_deskew(ctx, scans):
     assert n == 1  # k_overlap
     nb = synth.knn(pts, 10)
     n, _ = launches(ctx, lambda: preprocess.CloudCovarianceEstimation(ctx=ctx).estimate(pts, nb))
-    assert n == 1  # k_covariances
+    assert n == 1  # k_covariances_planes
     n, _ = launches(ctx, lambda: preprocess.CloudDeskewing(ctx=ctx).deskew(np.eye(4), times, pts, linear_vel=[1.0, 0.0, 0.0], angular_vel=[0.0, 0.0, 0.3]))
     assert n == 1  # k_deskew
 
 
-@pytest.mark.parametrize("mode", ["brute", "pyramid"])
-def test_find_neighbors(ctx, scans, monkeypatch, mode):
-    monkeypatch.setenv("GB_KNN", mode)
-    pts = scans[0][0][0]
+@pytest.mark.parametrize("size", [500, 6400])
+def test_find_neighbors(ctx, scans, size):
+    pts = scans[0][0][0][:size]
+    assert len(pts) == size
     n, _ = launches(ctx, lambda: preprocess.find_neighbors(pts, 10, ctx=ctx))
-    assert n == (1 if mode == "brute" else 1 + KNN)  # k_knn_bruteforce | k_set_int + knn
+    assert n == 1 + KNN  # k_set_int + knn
 
 
 def test_voxelgrid_sampling(ctx, scans):
