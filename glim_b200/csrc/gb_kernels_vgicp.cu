@@ -10,7 +10,7 @@
 // in sweep3, strided rows in sweep5, below); items are laid out factor-major and processed by the warps of a persistent
 // grid (first item = warp index, further items from a global queue), so at any instant the grid works on a
 // window of a few consecutive factors whose source cloud and voxel tables stay L2 resident.
-// Both kernels run the same steps, written once in gb_sweep_steps.cuh (k_gicp_sweep of gb_kernels_gicp.cu runs them too): phase A (probe_issue, probe_compact) resolves a round of points
+// Both kernels run the same steps, written once in gb_sweep_steps.cuh (k_gicp_sweep of gb_kernels_gicp.cu runs them too): phase A (probe_issue, probe_resolve, probe_compact) resolves a round of points
 // into the warp's shared-memory queue of hits, phase B (accumulate_queue) accumulates them, then reduce_item and the
 // item's ticket (ticket_last); the warp that draws a factor's last ticket retires it (retire_factor).
 // Per inlier (one lane):
@@ -47,7 +47,9 @@ namespace {
 // three dependent L2 round trips between two items are already covered by the other 15 warps of the SM).
 // =============================================================================================
 constexpr int kSubMax = 512;   // queue capacity per warp (points per round)
-constexpr int kLookupUnroll = 4;
+constexpr int kLookupUnroll3 = 5;  // probes per lane in flight (4: 2 % slower on the global-mapping sweep; 6: spills)
+constexpr int kRound3 = 32 * kLookupUnroll3 * ((kSubMax - 31) / (32 * kLookupUnroll3));  // points per round: whole lookup groups
+static_assert(kRound3 + 31 <= kSubMax, "a round's hits and the up to 31 carried from the previous round fit the queue");
 
 template <int MODE, bool PEER, bool SV>
 __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
@@ -84,13 +86,13 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
 #pragma unroll
     for (int k = 0; k < 32; k++) acc[k] = 0.f;
 
-    for (int wb = it.y; wb < item_end; wb += kSubMax) {
-      const int we = min(wb + kSubMax, item_end);
-      int nq = 0;  // warp-uniform queue length
-      for (int i0 = wb; i0 < we; i0 += 32 * kLookupUnroll) {
-        Probe p[kLookupUnroll];
+    int nq = 0;  // warp-uniform queue length
+    for (int wb = it.y; wb < item_end; wb += kRound3) {
+      const int we = min(wb + kRound3, item_end);
+      for (int i0 = wb; i0 < we; i0 += 32 * kLookupUnroll3) {
+        Probe p[kLookupUnroll3];
 #pragma unroll
-        for (int u = 0; u < kLookupUnroll; u++) {
+        for (int u = 0; u < kLookupUnroll3; u++) {
           const float4 a0 = __ldg(&D.p0[min(i0 + u * 32 + lane, we - 1)]);
           probe_issue(D, P, a0.x, a0.y, a0.z, p[u]);
         }
@@ -99,13 +101,21 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
           __syncwarp();
           if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
         }
+        int v[kLookupUnroll3];
+        probe_resolve(D, p, v);
 #pragma unroll
-        for (int u = 0; u < kLookupUnroll; u++) probe_compact(D, p[u], i0 + u * 32 + lane, we, q, nq, lt_mask);
+        for (int u = 0; u < kLookupUnroll3; u++) probe_compact(v[u], i0 + u * 32 + lane, we, q, nq, lt_mask);
       }
       __syncwarp();
+      // Whole passes of 32 hits only: the last nq % 32 hits are carried to the front of the queue for the next round (a
+      // pass costs a round trip however few lanes it fills), except in the item's last round.
+      const int nacc = we == item_end ? nq : (nq & ~31);
       // surface validation is a compile-time variant here (GLIM enables it for odometry factors only, which run sweep5)
-      accumulate_queue<MODE, SV>(acc, D, P, Pe, q, nq, lane);
+      accumulate_queue<MODE, SV>(acc, D, P, Pe, q, nacc, lane);
       __syncwarp();  // the queue is overwritten by the next round
+      nq -= nacc;
+      if (nacc > 0 && lane < nq) q[lane] = q[nacc + lane];  // nacc >= 32 > nq: the ranges do not overlap
+      __syncwarp();
     }
     if (!published) {  // the item had no lookup group (empty factor)
       __syncwarp();
@@ -131,6 +141,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
   }
 }
 
+constexpr int kLookupUnroll5 = 4;  // probes per lane in flight (5 spills)
 constexpr int kDescCache = 40;  // factors whose descriptor + fp32 pose are cached in shared memory (an odometry graph has <= 34)
 struct CtaCache {
   FactorDesc desc[kDescCache];
@@ -157,7 +168,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
   __shared__ __align__(16) uint2 s_q[kWarps][kSubMax];
   __shared__ CtaCache cache_s;
   CtaCache* const cache = &cache_s;
-  constexpr int U = kLookupUnroll;
+  constexpr int U = kLookupUnroll5;
   constexpr int kGroupsPerRound = kSubMax / (32 * U);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned lt_mask = (1u << lane) - 1u;
@@ -235,8 +246,10 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
           __syncwarp();
           if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
         }
+        int v[U];
+        probe_resolve(D, p, v);
 #pragma unroll
-        for (int u = 0; u < U; u++) probe_compact(D, p[u], first + (g * U + u) * row_stride + lane, limit, q, nq, lt_mask);
+        for (int u = 0; u < U; u++) probe_compact(v[u], first + (g * U + u) * row_stride + lane, limit, q, nq, lt_mask);
         if (g + 1 < g1) {  // the next group's points, loaded after this group is resolved
 #pragma unroll
           for (int u = 0; u < U; u++) {

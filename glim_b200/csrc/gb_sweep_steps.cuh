@@ -11,48 +11,60 @@ static_assert(GB_MODE_LINEARIZE == GB_MODE_LINEARIZE_VALUE, "gb_vgicp_math.cuh m
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
-// A point's hash probe in flight: its voxel coordinates, hash and first two buckets.
+// A point's hash probe in flight: its voxel coordinates, hash and the last bucket gathered for it.
 struct Probe {
   int cx, cy, cz;
   uint32_t h;
-  int4 b, b1;
+  int4 b;
 };
 
-// phase A, issue: transform one source point, and fetch its first two buckets together (adjacent 16-byte slots, one round trip)
+__device__ __forceinline__ bool bucket_holds(const int4 b, const Probe& p) { return b.w >= 0 && b.x == p.cx && b.y == p.cy && b.z == p.cz; }
+
+// phase A, issue: transform one source point and gather its first bucket.  The second bucket is gathered by probe_resolve,
+// only for the lanes whose first bucket holds another voxel: 12-35 % of the points of the global-mapping sweep, by level and
+// pair kind (scripts/probe_stats.py), so gathering it up front for every point wasted a 16-byte gather on most of them.
 __device__ __forceinline__ void probe_issue(const FactorDesc& D, const PoseF& P, float ax, float ay, float az, Probe& p) {
   float qx, qy, qz;
   transform(P, ax, ay, az, qx, qy, qz);
   p.cx = gb_coord(qx, D.inv_res); p.cy = gb_coord(qy, D.inv_res); p.cz = gb_coord(qz, D.inv_res);
   p.h = gb_hash(p.cx, p.cy, p.cz);
   p.b = __ldg(&D.buckets[p.h & D.mask]);
-  p.b1 = __ldg(&D.buckets[(p.h + 1u) & D.mask]);
 }
 
-// voxel index of a probed point, -1 for a miss
-__device__ __forceinline__ int resolve_probe(const FactorDesc& D, const int4 b, const int4 b1, uint32_t h, int cx, int cy, int cz) {
-  int v = -1;
-  if (b.w >= 0) {
-    if (b.x == cx && b.y == cy && b.z == cz) {
-      v = b.w;
-    } else if (D.max_scan > 1 && b1.w >= 0) {
-      if (b1.x == cx && b1.y == cy && b1.z == cz) {
-        v = b1.w;
+// phase A, resolve: the voxel index of each probe of a group (as gb_lookup: -1 for a miss), from the first buckets issued by
+// probe_issue.  The lanes whose first bucket holds another voxel gather their second bucket in ONE predicated round for the
+// whole group, so a group waits for at most one more round trip; inactive lanes issue no wavefronts.  Chains longer than two
+// buckets are walked one bucket at a time (rare: tables are at most 1/8 full).
+template <int U>
+__device__ __forceinline__ void probe_resolve(const FactorDesc& D, Probe (&p)[U], int (&v)[U]) {
+  bool next[U];
+#pragma unroll
+  for (int u = 0; u < U; u++) {
+    v[u] = bucket_holds(p[u].b, p[u]) ? p[u].b.w : -1;
+    next[u] = p[u].b.w >= 0 && v[u] < 0 && D.max_scan > 1;
+  }
+#pragma unroll
+  for (int u = 0; u < U; u++)
+    if (next[u]) p[u].b = __ldg(&D.buckets[(p[u].h + 1u) & D.mask]);
+#pragma unroll
+  for (int u = 0; u < U; u++) {
+    if (next[u] && p[u].b.w >= 0) {
+      if (bucket_holds(p[u].b, p[u])) {
+        v[u] = p[u].b.w;
       } else {
         for (int k = 2; k < D.max_scan; k++) {  // rare: longer collision chain
-          const int4 bb = __ldg(&D.buckets[(h + (uint32_t)k) & D.mask]);
+          const int4 bb = __ldg(&D.buckets[(p[u].h + (uint32_t)k) & D.mask]);
           if (bb.w < 0) break;
-          if (bb.x == cx && bb.y == cy && bb.z == cz) { v = bb.w; break; }
+          if (bucket_holds(bb, p[u])) { v[u] = bb.w; break; }
         }
       }
     }
   }
-  return v;
 }
 
-// phase A, compaction: a hit of point i (none when i >= limit) is appended to the warp's queue as (point, voxel), in lane order.
-// nq: the warp-uniform queue length.
-__device__ __forceinline__ void probe_compact(const FactorDesc& D, const Probe& p, int i, int limit, uint2* __restrict__ q, int& nq, unsigned lt_mask) {
-  int v = resolve_probe(D, p.b, p.b1, p.h, p.cx, p.cy, p.cz);
+// phase A, compaction: a hit v >= 0 of point i (none when i >= limit) is appended to the warp's queue as (point, voxel), in
+// lane order.  nq: the warp-uniform queue length.
+__device__ __forceinline__ void probe_compact(int v, int i, int limit, uint2* __restrict__ q, int& nq, unsigned lt_mask) {
   if (i >= limit) v = -1;
   const unsigned m = __ballot_sync(0xffffffffu, v >= 0);
   if (v >= 0) q[nq + __popc(m & lt_mask)] = make_uint2((unsigned)i, (unsigned)v);
