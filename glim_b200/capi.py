@@ -34,6 +34,7 @@ SYMBOLS = [
     "gb_point_grid_build", "gb_point_grid_info", "gb_point_grid_download", "gb_point_grid_destroy", "gb_gicp_grid_factor_create",
     "gb_gicp_grid_factor_half_width",
     "gb_cloud_estimate_fpfh", "gb_cloud_fpfh", "gb_fpfh_match", "gb_ransac_default_params", "gb_ransac_align",
+    "gb_gnc_default_params", "gb_gnc_align",
 ]
 
 GB_SLAB_STRIDE = 96
@@ -93,10 +94,25 @@ class RansacResult(C.Structure):
                 ("status", C.c_int)]
 
 
+class GncParams(C.Structure):
+    """gb_gnc_params (include/glim_b200.h)."""
+    _fields_ = [("max_init_samples", C.c_int), ("dof", C.c_int), ("seed", C.c_uint64)]
+
+
+class GncResult(C.Structure):
+    """gb_gnc_result (include/glim_b200.h)."""
+    _fields_ = [("T_target_source", C.c_double * 16), ("inlier_rate", C.c_double), ("inliers", C.c_int), ("samples", C.c_int), ("correspondences", C.c_int),
+                ("iterations", C.c_int), ("status", C.c_int)]
+
+
 # gb_ransac_result::status
 RANSAC_FOUND, RANSAC_EARLY_STOP, RANSAC_DEGENERATE = 0, 1, 2
 RANSAC_STATUS_NAMES = {0: "FOUND", 1: "EARLY_STOP", 2: "DEGENERATE"}
 FPFH_DIM = 33
+
+# gb_gnc_result::status
+GNC_FOUND, GNC_DEGENERATE = 0, 1
+GNC_STATUS_NAMES = {0: "FOUND", 1: "DEGENERATE"}
 
 # gb_align_result::status
 ALIGN_CONVERGED, ALIGN_MAX_ITERATIONS, ALIGN_LAMBDA_EXCEEDED, ALIGN_DEGENERATE = 0, 1, 2, 3
@@ -200,6 +216,8 @@ def lib():
     L.gb_fpfh_match.argtypes = [vp, vp, vp, vp]
     L.gb_ransac_default_params.argtypes = [vp]
     L.gb_ransac_align.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.gb_gnc_default_params.argtypes = [vp]
+    L.gb_gnc_align.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     for name in SYMBOLS:
         getattr(L, name)  # AttributeError here means the library and include/glim_b200.h are out of sync
     _lib = L

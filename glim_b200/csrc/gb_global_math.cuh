@@ -1,8 +1,10 @@
 // gb_global_math.cuh -- the per-pair and per-hypothesis arithmetic of global registration (gb_kernels_global.cu): FPFH pair
-// features and their bins, the RANSAC sample draw, and the 6-DoF (Horn) and 4-DoF pose estimators.  Like gb_cov_math.cuh it
-// holds nothing that only exists on the device, so the SAME TEXT compiles for the host: tests/cpp/global_math_host.cpp builds
-// it with g++ -ffp-contract=off and tests/test_global_host.py checks it against the numpy restatement (tests/global_oracle.py).
-// The rules are written once, in include/glim_b200.h (gb_cloud_estimate_fpfh, gb_ransac_align).
+// features and their bins, the RANSAC sample draw, the 6-DoF (Horn) and 4-DoF pose estimators, and GNC's weighted closed form
+// and Geman-McClure schedule.  Like gb_cov_math.cuh it holds nothing that only exists on the device, so the SAME TEXT compiles
+// for the host: tests/cpp/global_math_host.cpp and tests/cpp/gnc_math_host.cpp build it with g++ -ffp-contract=off and
+// tests/test_global_host.py / tests/test_gnc_host.py check it against the numpy restatements (tests/global_oracle.py,
+// tests/gnc_oracle.py).
+// The rules are written once, in include/glim_b200.h (gb_cloud_estimate_fpfh, gb_ransac_align, gb_gnc_align).
 //
 // Every fp64 multiply, add and subtract that could be contracted is an explicit round-to-nearest operation, so the device and
 // the host build agree bit for bit; division and sqrt are correctly rounded on both.  What remains between them is atan2 (the
@@ -113,12 +115,61 @@ GB_CHD void jacobi_rotate(double* A, double* V, int p, int q) {
 }
 constexpr int kJacobiSweeps = 8;  // fixed: a 4x4 converges to fp64 rounding in fewer
 
+// Horn's closed form: R (3 x 3 row-major) from S[3 r + c] = sum_i a'_i[r] b'_i[c] (source a', target b', centred).  The unit
+// quaternion (w, x, y, z) is the eigenvector of the largest eigenvalue of Horn's 4x4 N built from S, found by kJacobiSweeps
+// cyclic Jacobi sweeps over the pairs (0,1) (0,2) (0,3) (1,2) (1,3) (2,3) (the largest diagonal entry after the sweeps, ties to
+// the lower index).
+GB_CHD void horn_rotation(const double* S, double* R) {
+  const double sxx = S[0], sxy = S[1], sxz = S[2], syx = S[3], syy = S[4], syz = S[5], szx = S[6], szy = S[7], szz = S[8];
+  double N[16] = {
+      __dadd_rn(__dadd_rn(sxx, syy), szz), __dsub_rn(syz, szy), __dsub_rn(szx, sxz), __dsub_rn(sxy, syx),
+      __dsub_rn(syz, szy), __dsub_rn(__dsub_rn(sxx, syy), szz), __dadd_rn(sxy, syx), __dadd_rn(szx, sxz),
+      __dsub_rn(szx, sxz), __dadd_rn(sxy, syx), __dsub_rn(__dsub_rn(syy, sxx), szz), __dadd_rn(syz, szy),
+      __dsub_rn(sxy, syx), __dadd_rn(szx, sxz), __dadd_rn(syz, szy), __dsub_rn(__dsub_rn(szz, sxx), syy)};
+  double V[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  for (int sweep = 0; sweep < kJacobiSweeps; sweep++)
+    for (int p = 0; p < 3; p++)
+      for (int q = p + 1; q < 4; q++) jacobi_rotate(N, V, p, q);
+  int k = 0;
+  for (int j = 1; j < 4; j++)
+    if (N[5 * j] > N[5 * k]) k = j;
+  double w = V[k], x = V[4 + k], y = V[8 + k], z = V[12 + k];
+  const double qn = sqrt(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(w, w), __dmul_rn(x, x)), __dmul_rn(y, y)), __dmul_rn(z, z)));
+  w = w / qn; x = x / qn; y = y / qn; z = z / qn;
+  R[0] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(__dmul_rn(y, y), __dmul_rn(z, z))));
+  R[1] = __dmul_rn(2.0, __dsub_rn(__dmul_rn(x, y), __dmul_rn(w, z)));
+  R[2] = __dmul_rn(2.0, __dadd_rn(__dmul_rn(x, z), __dmul_rn(w, y)));
+  R[3] = __dmul_rn(2.0, __dadd_rn(__dmul_rn(x, y), __dmul_rn(w, z)));
+  R[4] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(__dmul_rn(x, x), __dmul_rn(z, z))));
+  R[5] = __dmul_rn(2.0, __dsub_rn(__dmul_rn(y, z), __dmul_rn(w, x)));
+  R[6] = __dmul_rn(2.0, __dsub_rn(__dmul_rn(x, z), __dmul_rn(w, y)));
+  R[7] = __dmul_rn(2.0, __dadd_rn(__dmul_rn(y, z), __dmul_rn(w, x)));
+  R[8] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y))));
+}
+
+// The 4-DoF estimator: R = Rz(atan2(sn, cs)) for sn = sum a'_x b'_y - a'_y b'_x, cs = sum a'_x b'_x + a'_y b'_y.
+GB_CHD void yaw_rotation(double sn, double cs, double* R) {
+  const double yaw = atan2(sn, cs), c = cos(yaw), s = sin(yaw);
+  R[0] = c; R[1] = -s; R[2] = 0.0;
+  R[3] = s; R[4] = c;  R[5] = 0.0;
+  R[6] = 0.0; R[7] = 0.0; R[8] = 1.0;
+}
+
+// T (16, column-major) = [R | cb - R ca], R ca taken row by row as ((R0 ca_x + R1 ca_y) + R2 ca_z)
+GB_CHD void pose_from_rotation(const double* R, const double* ca, const double* cb, double* T) {
+  for (int r = 0; r < 3; r++) {
+    const double ra = __dadd_rn(__dadd_rn(__dmul_rn(R[3 * r], ca[0]), __dmul_rn(R[3 * r + 1], ca[1])), __dmul_rn(R[3 * r + 2], ca[2]));
+    for (int c = 0; c < 3; c++) T[4 * c + r] = R[3 * r + c];
+    T[12 + r] = __dsub_rn(cb[r], ra);
+    T[3 + 4 * r] = 0.0;
+  }
+  T[15] = 1.0;
+}
+
 // T (16, column-major) with target ~ R source + t from three pairs (a: source, b: target; 3 x 3 row-major each).  dof 6:
-// Horn's closed form -- the unit quaternion (w, x, y, z) is the eigenvector of the largest eigenvalue of Horn's 4x4 N built
-// from S = sum_i a'_i b'_i^T (centred points), found by kJacobiSweeps cyclic Jacobi sweeps over the pairs (0,1) (0,2) (0,3)
-// (1,2) (1,3) (2,3) (the largest diagonal entry after the sweeps, ties to the lower index).  dof 4: yaw = atan2(sum a'_x b'_y -
-// a'_y b'_x, sum a'_x b'_x + a'_y b'_y), R = Rz(yaw).  Both: t = b_centroid - R a_centroid.  Returns false (T untouched) for an
-// invalid sample (tri_area2 of either triangle below kRansacMinArea2 or not finite).
+// horn_rotation of S = sum_i a'_i b'_i^T (centred points).  dof 4: yaw_rotation of the centred xy cross terms.  Both: t =
+// b_centroid - R a_centroid.  Returns false (T untouched) for an invalid sample (tri_area2 of either triangle below
+// kRansacMinArea2 or not finite).
 GB_CHD bool ransac_pose(const double* a, const double* b, int dof, double* T) {
   if (!(tri_area2(a) >= kRansacMinArea2) || !(tri_area2(b) >= kRansacMinArea2)) return false;
   double ca[3], cb[3], ac[9], bc[9], R[9];
@@ -132,50 +183,73 @@ GB_CHD bool ransac_pose(const double* a, const double* b, int dof, double* T) {
       sn = __dadd_rn(sn, __dsub_rn(__dmul_rn(p[0], q[1]), __dmul_rn(p[1], q[0])));
       cs = __dadd_rn(cs, __dadd_rn(__dmul_rn(p[0], q[0]), __dmul_rn(p[1], q[1])));
     }
-    const double yaw = atan2(sn, cs), c = cos(yaw), s = sin(yaw);
-    R[0] = c; R[1] = -s; R[2] = 0.0;
-    R[3] = s; R[4] = c;  R[5] = 0.0;
-    R[6] = 0.0; R[7] = 0.0; R[8] = 1.0;
+    yaw_rotation(sn, cs, R);
   } else {
     double S[9];  // S[3 r + c] = sum_i a'_i[r] b'_i[c]
     for (int r = 0; r < 3; r++)
       for (int c = 0; c < 3; c++)
         S[3 * r + c] = __dadd_rn(__dadd_rn(__dmul_rn(ac[r], bc[c]), __dmul_rn(ac[3 + r], bc[3 + c])), __dmul_rn(ac[6 + r], bc[6 + c]));
-    const double sxx = S[0], sxy = S[1], sxz = S[2], syx = S[3], syy = S[4], syz = S[5], szx = S[6], szy = S[7], szz = S[8];
-    double N[16] = {
-        __dadd_rn(__dadd_rn(sxx, syy), szz), __dsub_rn(syz, szy), __dsub_rn(szx, sxz), __dsub_rn(sxy, syx),
-        __dsub_rn(syz, szy), __dsub_rn(__dsub_rn(sxx, syy), szz), __dadd_rn(sxy, syx), __dadd_rn(szx, sxz),
-        __dsub_rn(szx, sxz), __dadd_rn(sxy, syx), __dsub_rn(__dsub_rn(syy, sxx), szz), __dadd_rn(syz, szy),
-        __dsub_rn(sxy, syx), __dadd_rn(szx, sxz), __dadd_rn(syz, szy), __dsub_rn(__dsub_rn(szz, sxx), syy)};
-    double V[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    for (int sweep = 0; sweep < kJacobiSweeps; sweep++)
-      for (int p = 0; p < 3; p++)
-        for (int q = p + 1; q < 4; q++) jacobi_rotate(N, V, p, q);
-    int k = 0;
-    for (int j = 1; j < 4; j++)
-      if (N[5 * j] > N[5 * k]) k = j;
-    double w = V[k], x = V[4 + k], y = V[8 + k], z = V[12 + k];
-    const double qn = sqrt(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(w, w), __dmul_rn(x, x)), __dmul_rn(y, y)), __dmul_rn(z, z)));
-    w = w / qn; x = x / qn; y = y / qn; z = z / qn;
-    R[0] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(__dmul_rn(y, y), __dmul_rn(z, z))));
-    R[1] = __dmul_rn(2.0, __dsub_rn(__dmul_rn(x, y), __dmul_rn(w, z)));
-    R[2] = __dmul_rn(2.0, __dadd_rn(__dmul_rn(x, z), __dmul_rn(w, y)));
-    R[3] = __dmul_rn(2.0, __dadd_rn(__dmul_rn(x, y), __dmul_rn(w, z)));
-    R[4] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(__dmul_rn(x, x), __dmul_rn(z, z))));
-    R[5] = __dmul_rn(2.0, __dsub_rn(__dmul_rn(y, z), __dmul_rn(w, x)));
-    R[6] = __dmul_rn(2.0, __dsub_rn(__dmul_rn(x, z), __dmul_rn(w, y)));
-    R[7] = __dmul_rn(2.0, __dadd_rn(__dmul_rn(y, z), __dmul_rn(w, x)));
-    R[8] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y))));
+    horn_rotation(S, R);
   }
-  for (int r = 0; r < 3; r++) {
-    const double ra = __dadd_rn(__dadd_rn(__dmul_rn(R[3 * r], ca[0]), __dmul_rn(R[3 * r + 1], ca[1])), __dmul_rn(R[3 * r + 2], ca[2]));
-    for (int c = 0; c < 3; c++) T[4 * c + r] = R[3 * r + c];
-    T[12 + r] = __dsub_rn(cb[r], ra);
-    T[3 + 4 * r] = 0.0;
-  }
-  T[15] = 1.0;
+  pose_from_rotation(R, ca, cb, T);
   return true;
 }
+
+// ---- GNC (gb_gnc_align): the weighted closed form and the Geman-McClure schedule of include/glim_b200.h ----
+constexpr double kGncDivFactor = 1.4;   // mu's update factor (Yang et al., "Graduated Non-Convexity for Robust Spatial Perception", 2020)
+constexpr double kGncMinScale = 1.0;    // m^2: the last mu, at which the schedule ends
+constexpr double kGncMaxScale = 1e3;    // m^2: the cap on the first mu
+constexpr double kGncInlierVoxel = 1.0; // m: the score's target grid (RANSAC's default inlier_voxel_resolution)
+constexpr int kGncSums = 16;            // W, p (3), q (3), M (9)
+
+// the sums of one pair (a' = a - a_shift, b' = b - b_shift) at weight w: s[0] += w, s[1 + r] += w a'_r, s[4 + c] += w b'_c,
+// s[7 + 3 r + c] += (w a'_r) b'_c
+GB_CHD void gnc_accumulate(double* s, double w, const double* ac, const double* bc) {
+  s[0] = __dadd_rn(s[0], w);
+  for (int r = 0; r < 3; r++) {
+    const double wa = __dmul_rn(w, ac[r]);
+    s[1 + r] = __dadd_rn(s[1 + r], wa);
+    s[4 + r] = __dadd_rn(s[4 + r], __dmul_rn(w, bc[r]));
+    for (int c = 0; c < 3; c++) s[7 + 3 * r + c] = __dadd_rn(s[7 + 3 * r + c], __dmul_rn(wa, bc[c]));
+  }
+}
+
+// T (16, column-major) from the sums s (gnc_accumulate) about the shifts a_shift, b_shift: c_a = a_shift + p / W, c_b = b_shift
+// + q / W, S = M - p q^T / W; dof 6 horn_rotation(S), dof 4 yaw_rotation(S01 - S10, S00 + S11); t = c_b - R c_a.
+GB_CHD void gnc_pose(const double* s, const double* a_shift, const double* b_shift, int dof, double* T) {
+  const double W = s[0];
+  double ca[3], cb[3], S[9], R[9];
+  for (int r = 0; r < 3; r++) {
+    ca[r] = __dadd_rn(a_shift[r], s[1 + r] / W);
+    cb[r] = __dadd_rn(b_shift[r], s[4 + r] / W);
+    for (int c = 0; c < 3; c++) S[3 * r + c] = __dsub_rn(s[7 + 3 * r + c], __dmul_rn(s[1 + r], s[4 + c]) / W);
+  }
+  if (dof == 4)
+    yaw_rotation(__dsub_rn(S[1], S[3]), __dadd_rn(S[0], S[4]), R);
+  else
+    horn_rotation(S, R);
+  pose_from_rotation(R, ca, cb, T);
+}
+
+// r^2 = (e_x^2 + e_y^2) + e_z^2 with e = b - (R a + t), R a row by row as ((R0 a_x + R1 a_y) + R2 a_z); T column-major
+GB_CHD double gnc_residual2(const double* T, const double* a, const double* b) {
+  double e[3];
+  for (int r = 0; r < 3; r++) {
+    const double ra = __dadd_rn(__dadd_rn(__dmul_rn(T[r], a[0]), __dmul_rn(T[4 + r], a[1])), __dmul_rn(T[8 + r], a[2]));
+    e[r] = __dsub_rn(b[r], __dadd_rn(ra, T[12 + r]));
+  }
+  return __dadd_rn(__dadd_rn(__dmul_rn(e[0], e[0]), __dmul_rn(e[1], e[1])), __dmul_rn(e[2], e[2]));
+}
+
+// the Geman-McClure weight (mu / (mu + r^2))^2
+GB_CHD double gnc_weight(double mu, double r2) {
+  const double u = mu / __dadd_rn(mu, r2);
+  return __dmul_rn(u, u);
+}
+// the first mu from the largest r^2 at the unit-weight pose, and the step after an iteration at mu (the schedule ends after
+// the iteration at mu == kGncMinScale)
+GB_CHD double gnc_initial_scale(double max_r2) { return fmin(fmax(max_r2, kGncMinScale), kGncMaxScale); }
+GB_CHD double gnc_next_scale(double mu) { return fmax(mu / kGncDivFactor, kGncMinScale); }
 
 // The RANSAC inlier test of source point (ax, ay, az) under P (the fp32 cast of the hypothesis): q = R a + t uncontracted,
 // ((r0 ax + r1 ay) + r2 az) + t per row; an inlier iff q is finite and its cell (gb_coord at inv) holds a target point.

@@ -23,6 +23,7 @@ include/glim_b200/gtsam_points_compat.hpp.
     PointCloudGPU.estimate_fpfh(radius) / .fpfh()           gtsam_points::estimate_fpfh, manual_loop_close_modal.cpp:382-397, :415
     fpfh_match(target, source)                              the target's KdTreeX over FPFH features, manual_loop_close_modal.cpp:402
     estimate_pose_ransac(target, source, **params)          gtsam_points::estimate_pose_ransac, manual_loop_close_modal.cpp:435-443
+    estimate_pose_gnc(target, source, **params)             gtsam_points::estimate_pose_gnc, manual_loop_close_modal.cpp:446-458
 """
 from __future__ import annotations
 
@@ -788,3 +789,29 @@ def median_distance(points, max_scan_count: int = 256) -> float:
     d = np.linalg.norm(points[::step, :3], axis=1)
     d = np.sort(d)
     return float(d[len(d) // 2])
+
+
+def gnc_params(**overrides) -> capi.GncParams:
+    """gb_gnc_default_params (the manual loop-closure modal's values) with the given fields replaced."""
+    return _params(capi.GncParams(), lib().gb_gnc_default_params, "gb_gnc_params", overrides)
+
+
+def estimate_pose_gnc(target: PointCloudGPU, source: PointCloudGPU, ctx: Context | None = None, correspondences: bool = False, **params) -> dict:
+    """gtsam_points::estimate_pose_gnc as the modal runs it (manual_loop_close_modal.cpp:446-458: reciprocal matches, no tuple
+    check) on the device (gb_gnc_align): both clouds carry FPFH features; params are fields of gb_gnc_params (max_init_samples,
+    dof, seed).  -> {T_target_source (4,4), inliers, inlier_rate, samples, correspondences, iterations, status, status_name} and,
+    with correspondences, pairs (K,2) int32 (source index, target index) and their final weights (K,)."""
+    ctx = ctx or source.ctx
+    p = gnc_params(**params)
+    r = capi.GncResult()
+    m = min(source.n, p.max_init_samples)
+    pairs = np.empty((m, 2), np.int32) if correspondences else None
+    weights = np.empty(m) if correspondences else None
+    check(lib().gb_gnc_align(ctx.h, target.h, source.h, C.byref(p), C.byref(r), ptr(pairs), ptr(weights)))
+    out = {"T_target_source": np.array(r.T_target_source[:]).reshape(4, 4).T.copy(), "inliers": r.inliers, "inlier_rate": r.inlier_rate,
+           "samples": r.samples, "correspondences": r.correspondences, "iterations": r.iterations, "status": r.status,
+           "status_name": capi.GNC_STATUS_NAMES.get(r.status, "?")}
+    if correspondences:
+        out["pairs"] = pairs[:r.correspondences].copy()
+        out["weights"] = weights[:r.correspondences].copy()
+    return out

@@ -353,6 +353,48 @@ GB_API gb_status gb_ransac_default_params(gb_ransac_params* params);
 GB_API gb_status gb_ransac_align(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source, const gb_ransac_params* params, gb_ransac_result* result,
                                  int32_t* hypothesis_inliers);
 
+/* ---- GNC: the modal's other global method (gtsam_points::estimate_pose_gnc, manual_loop_close_modal.cpp:446-458), with its
+ *      settings fixed as the modal fixes them (reciprocal_check = true, tuple_check = false).  [EXT] the rule below is this
+ *      library's statement of it.
+ *
+ *      1. Samples, m = min(N_s, max_init_samples): every source index when N_s <= max_init_samples, else the m indices with the
+ *      smallest rg_hash(seed, i) (the hash thinning of the random-grid pick; reference: an std::mt19937 shuffle), in ascending i.
+ *      2. j(i) = the target feature nearest to sample i by gb_fpfh_match's rule.  3. Sample i keeps the pair (i, j(i)) iff j(i)
+ *      >= 0, the source feature nearest to target feature j(i) over all N_s source features (same rule) is i, and both fp32
+ *      positions are finite; pairs in ascending i, K of them.  K < 3: DEGENERATE, T = I, 0 iterations.
+ *      4. Weighted closed form, fp64 from the fp32 positions (a source, b target), every operation rounded separately: once
+ *      per call the shifts a_s = sum a / K, b_s = sum b / K; for weights w, W = sum w, p = sum w (a - a_s), q = sum w (b - b_s),
+ *      M = sum w (a - a_s)(b - b_s)^T; c_a = a_s + p / W, c_b = b_s + q / W, S = M - p q^T / W; dof 6 Horn's rotation of S (as
+ *      RANSAC's: 8 cyclic Jacobi sweeps), dof 4 R = Rz(atan2(S01 - S10, S00 + S11)); t = c_b - R c_a.
+ *      5. Graduated non-convexity, Geman-McClure: r_k^2 = (e_x^2 + e_y^2) + e_z^2, e = b_k - (R a_k + t) (R a row by row as
+ *      ((R0 a_x + R1 a_y) + R2 a_z)); T = pose(w = 1); mu = min(max(max_k r_k^2(T), 1 m^2), 1e3 m^2); then repeat: w_k =
+ *      (mu / (mu + r_k^2(T)))^2, T = pose(w), iterations += 1, stop if mu == 1 m^2, else mu = max(mu / 1.4, 1 m^2).  At most 22
+ *      iterations.  The reported weights are the last iteration's.
+ *      6. inliers: RANSAC's inlier test of all N_s source points under T against a point grid of the target at 1.0 m (RANSAC's
+ *      default inlier_voxel_resolution), inlier_rate = inliers / N_s, also for a DEGENERATE result (T = I).
+ *
+ *      Launches: the target grid's build (gb_point_grid_build at 1.0 m) + 7 (two matches, the gather of the matched target
+ *      rows, the pair flags, the pair compaction, the solve, the score), + 5 when N_s > max_init_samples (the hash thinning's 3,
+ *      the sample compaction, the gather of the sampled source rows).  One stream synchronisation, at the end. ---- */
+#define GB_GNC_FOUND 0
+#define GB_GNC_DEGENERATE 1
+typedef struct gb_gnc_params {
+  int max_init_samples;  /* 10000 (manual_loop_close_modal.cpp:52, gnc_max_samples), in [1, 2^28] */
+  int dof;               /* 4 (:50, global_registration_4dof) or 6 */
+  uint64_t seed;         /* 53123 (:42; the modal adds 4322 before each run) */
+} gb_gnc_params;
+typedef struct gb_gnc_result {
+  double T_target_source[16];  /* column-major */
+  double inlier_rate;
+  int inliers, samples, correspondences, iterations, status; /* samples = m, correspondences = K; GB_GNC_* */
+} gb_gnc_result;
+GB_API gb_status gb_gnc_default_params(gb_gnc_params* params);
+/* pairs (K x 2: source index, target index) and weights (K) may be NULL; their capacity is m = min(N_s, max_init_samples) rows,
+ * of which the first K are written (a DEGENERATE result's weights are 0).  Validated before any launch: both clouds with
+ * features and at least one point, on ctx's device; the parameter bounds above. */
+GB_API gb_status gb_gnc_align(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source, const gb_gnc_params* params, gb_gnc_result* result, int32_t* pairs,
+                              double* weights);
+
 /* ---- NonlinearFactorSetGPU::add(graph) / ::linearize(values) (odometry_estimation_gpu.cpp:383-386;
  *      hook at src/glim/viewer/offline_viewer.cpp:29): F x 64 B of poses down, one launch over all
  *      factors, F records up. ---- */
