@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
+#include <cassert>
 #include <atomic>
 #include <memory>
 #include <mutex>
@@ -56,7 +57,6 @@ struct gb_cloud {
   int* perm = nullptr;
   int* inv_perm = nullptr;
   void* base = nullptr;       // one allocation
-  size_t bytes = 0;
   // The time table of gb_cloud_add_times (gb_kernels_ct.cu), or none (num_entries == 0).  Entry b holds the original indices
   // [t_starts[b], t_starts[b + 1]) at normalized time t_tau[b]; the stored slots are reached through inv_perm.  The device
   // copy is one block of its own (ct_table_layout), from the device pool; only the CT factor reads it.
@@ -91,7 +91,6 @@ struct gb_voxelmap {
   int4* buckets = nullptr;
   float4* voxels = nullptr;   // 3 float4 per record: one record per voxel, or per stored point of an iVox
   void* base = nullptr;
-  size_t bytes = 0;
   // Incremental maps and iVoxes also keep, in `base` behind the records, each voxel's packed key and the insert that last
   // touched it.  An incremental map adds each voxel's point count and fp64 sums (Sigma q: 3, Sigma C: 6 unique entries).  An
   // iVox's records are its stored points ({x y z c00} {c01 c02 c11 c12} {c22, 1, 0, 0}), voxel-major in ascending packed-key
@@ -327,6 +326,18 @@ gb_status gb_launch(gb_ctx* ctx, const char* name, void (*kernel)(P...), dim3 gr
 // every live context of the device (what the implicit synchronisation of cudaFree used to guarantee) and keeps the block.
 cudaError_t gb_dev_malloc(int device, size_t bytes, void** out);
 void gb_dev_free(int device, void* p);
+// A pool block is taken only by gb_dev_carve, into an owner made for its device, which returns it to the pool on every exit
+// before hand_over(field).  That swaps it into a handle's field on the same device, and the owner returns the field's old block
+// instead.  Only cloud_free and voxelmap_free return a handle's blocks.  An owner assigned to returns the block it held.
+struct gb_dev_block {
+  int device;
+  void* base = nullptr;
+  explicit gb_dev_block(int device) : device(device) {}
+  gb_dev_block(gb_dev_block&& o) noexcept : device(o.device), base(std::exchange(o.base, nullptr)) {}
+  gb_dev_block& operator=(gb_dev_block o) noexcept { std::swap(device, o.device); std::swap(base, o.base); return *this; }  // o returns the old block
+  ~gb_dev_block() { gb_dev_free(device, base); }
+  template <typename T> void hand_over(T*& field) { void* old = field; field = (T*)base; base = old; }
+};
 gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes);  // a.base holds at least `bytes` afterwards
 // the parameter bounds of gb_vgicp_align (gb_align.cu), shared by gb_ct_gicp_align
 gb_status gb_align_params_check(const gb_align_params* prm);
@@ -377,6 +388,18 @@ template <typename Layout> gb_status gb_carve(gb_ctx* ctx, gb_arena& arena, Layo
   layout(size);
   GB_CHECK(gb_arena_reserve(ctx, arena, size.off));
   Carver cv{(char*)arena.base};
+  layout(cv);
+  return GB_OK;
+}
+// A layout carved out of a new block of the device pool, which `block` (an empty owner of ctx's device) owns afterwards.
+template <typename Layout> gb_status gb_dev_carve(gb_ctx* ctx, gb_dev_block& block, Layout&& layout) {
+  assert(!block.base && block.device == ctx->device);
+  Carver size;
+  layout(size);
+  void* base = nullptr;
+  GB_CUDA(gb_dev_malloc(ctx->device, size.off, &base));
+  block.base = base;
+  Carver cv{(char*)base};
   layout(cv);
   return GB_OK;
 }

@@ -451,7 +451,7 @@ extern "C" gb_status gb_cloud_add_times(gb_ctx* ctx, gb_cloud* cloud, size_t n, 
   const int B = ct_time_table(times, (int)n, starts.data(), tau.data());
   starts.resize((size_t)B + 1);
   tau.resize((size_t)B);
-  // stage in pinned memory, then one device block of the pool that replaces the old table
+  // stage in pinned memory, then one device block of the pool that replaces the old table once the upload has succeeded
   CtTable h;
   size_t bytes = 0;
   GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) {
@@ -460,19 +460,16 @@ extern "C" gb_status gb_cloud_add_times(gb_ctx* ctx, gb_cloud* cloud, size_t n, 
   }));
   memcpy(h.starts, starts.data(), sizeof(int) * starts.size());
   memcpy(h.tau, tau.data(), sizeof(double) * tau.size());
-  void* base = nullptr;
-  GB_CUDA(gb_dev_malloc(ctx->device, bytes, &base));
-  Carver cv{(char*)base};
-  const CtTable d = ct_table_layout(cv, B);
-  const cudaError_t e1 = cudaMemcpyAsync(base, h.starts, bytes, cudaMemcpyHostToDevice, ctx->stream);
+  gb_dev_block block(ctx->device);
+  CtTable d;
+  GB_CHECK(gb_dev_carve(ctx, block, [&](Carver& cv) { d = ct_table_layout(cv, B); }));
+  const cudaError_t e1 = cudaMemcpyAsync(d.starts, h.starts, bytes, cudaMemcpyHostToDevice, ctx->stream);
   const cudaError_t e2 = e1 == cudaSuccess ? cudaStreamSynchronize(ctx->stream) : e1;
   if (e2 != cudaSuccess) {
-    gb_dev_free(ctx->device, base);
     gb_set_error("time table upload failed: %s", cudaGetErrorString(e2));
     return GB_ERR_CUDA;
   }
-  gb_dev_free(cloud->device, cloud->t_base);
-  cloud->t_base = base;
+  block.hand_over(cloud->t_base);  // the old table goes back to the pool on return
   cloud->t_starts = d.starts;
   cloud->t_tau = d.tau;
   cloud->num_entries = B;

@@ -365,35 +365,34 @@ extern "C" gb_status gb_cloud_estimate_fpfh(gb_ctx* ctx, gb_cloud* cloud, double
   GB_REQUIRE(cloud->n == 0 || cloud->normals, "FPFH needs the cloud's normals");
   GB_ENTER(ctx);
   const size_t n = cloud->n;
-  void* base = nullptr;
-  GB_CUDA(gb_dev_malloc(ctx->device, sizeof(float) * kFpfhDim * n, &base));  // replaces the old block only on success
+  gb_dev_block block(ctx->device);  // replaces the old features only on success
+  float* fpfh = nullptr;
+  GB_CHECK(gb_dev_carve(ctx, block, [&](Carver& cv) { fpfh = cv.take<float>(kFpfhDim * n); }));
   if (n > 0) {
     gb_point_grid* gh = nullptr;
     const gb_status st = gb_point_grid_build(ctx, cloud, 1.05 * search_radius, &gh);
     gb_owned<gb_point_grid> grid(gh, grid_release);
-    if (st != GB_OK) { gb_dev_free(ctx->device, base); return st; }
+    GB_CHECK(st);
     const gb_voxelmap* g = grid_map(gh);
     const float max_d2 = (float)(search_radius * search_radius);
     const int m = grid_half_width(g->inv_res, max_d2, g->key_extent);
+    if (m > kGridMaxHalfWidth) {
+      gb_set_error("FPFH search half-width %d exceeds %d", m, kGridMaxHalfWidth);
+      return GB_ERR_INTERNAL;
+    }
     double* spfh = nullptr;
-    gb_status s2 = m <= kGridMaxHalfWidth ? gb_carve(ctx, ctx->scratch, [&](Carver& cv) { spfh = cv.take<double>(kFpfhDim * n); }) : GB_ERR_INTERNAL;
+    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) { spfh = cv.take<double>(kFpfhDim * n); }));
     const FpfhGrid G = fpfh_grid(g, m, max_d2);
     const int blocks = (int)((n + kFpfhThreads - 1) / kFpfhThreads);
-    if (s2 == GB_OK) s2 = gb_launch(ctx, "k_fpfh_spfh", k_fpfh_spfh, blocks, kFpfhThreads, 0, (int)n, G, cloud->normals, cloud->inv_perm, spfh);
-    if (s2 == GB_OK) s2 = gb_launch(ctx, "k_fpfh_final", k_fpfh_final, blocks, kFpfhThreads, 0, (int)n, G, spfh, (float*)base);
-    if (s2 == GB_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
+    GB_CHECK(gb_launch(ctx, "k_fpfh_spfh", k_fpfh_spfh, blocks, kFpfhThreads, 0, (int)n, G, cloud->normals, cloud->inv_perm, spfh));
+    GB_CHECK(gb_launch(ctx, "k_fpfh_final", k_fpfh_final, blocks, kFpfhThreads, 0, (int)n, G, spfh, fpfh));
+    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
       gb_set_error("FPFH estimation failed: %s", cudaGetErrorString(cudaGetLastError()));
-      s2 = GB_ERR_CUDA;
-    }
-    if (s2 != GB_OK) {
-      if (s2 == GB_ERR_INTERNAL) gb_set_error("FPFH search half-width %d exceeds %d", m, kGridMaxHalfWidth);
-      gb_dev_free(ctx->device, base);
-      return s2;
+      return GB_ERR_CUDA;
     }
   }
-  gb_dev_free(cloud->device, cloud->f_base);
-  cloud->f_base = base;
-  cloud->fpfh = (float*)base;
+  block.hand_over(cloud->f_base);
+  cloud->fpfh = fpfh;
   return GB_OK;
 }
 

@@ -172,33 +172,34 @@ gb_status gb_thin(gb_ctx* ctx, int n, const int* cand, const int* count, int m, 
 
 // The hash table of V voxels (vcoord[v] = {x, y, z, points}; d_dropped: one int of scratch, unused when V = 0): num_buckets =
 // init_buckets doubled until >= 8 V, then doubled again while more than drop_rate * total_points points fall out of it.
-// One host synchronisation per attempt.  On failure *buckets may hold a block the caller frees.
+// One host synchronisation per attempt.  A rejected attempt's table goes back to the pool before the next one is taken.
 static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dropped, int init_buckets, int max_scan, double drop_rate, double total_points,
-                             int4** buckets, int* num_buckets, int* num_dropped_points) {
+                             gb_dev_block& table, int* num_buckets, int* num_dropped_points) {
   cudaStream_t st = ctx->stream;
   int nb = init_buckets;
   while ((long long)nb < 8ll * V) nb *= 2;  // load factor <= 1/8: the XOR-of-primes hash clusters, and lookups that
                                                              // MISS (most of them in global mapping) walk until the first empty slot;
                                                              // same rule as the oracle
-  for (;;) {
-    GB_CUDA(gb_dev_malloc(ctx->device, sizeof(int4) * (size_t)nb, (void**)buckets));
-    GB_CHECK(gb_launch(ctx, "k_table_clear", k_table_clear, (nb + 255) / 256, 256, 0, nb, *buckets));
+  for (;; nb *= 2) {
+    gb_dev_block attempt(ctx->device);
+    int4* buckets = nullptr;
+    GB_CHECK(gb_dev_carve(ctx, attempt, [&](Carver& cv) { buckets = cv.take<int4>((size_t)nb); }));
+    GB_CHECK(gb_launch(ctx, "k_table_clear", k_table_clear, (nb + 255) / 256, 256, 0, nb, buckets));
     int dropped = 0;
     if (V > 0) {
       GB_CUDA(cudaMemsetAsync(d_dropped, 0, sizeof(int), st));
-      GB_CHECK(gb_launch(ctx, "k_table_insert", k_table_insert, (V + 255) / 256, 256, 0, V, d_vcoord, *buckets, (uint32_t)nb - 1u, max_scan, d_dropped));
+      GB_CHECK(gb_launch(ctx, "k_table_insert", k_table_insert, (V + 255) / 256, 256, 0, V, d_vcoord, buckets, (uint32_t)nb - 1u, max_scan, d_dropped));
     }
-    GB_CHECK(gb_launch(ctx, "k_table_finalize", k_table_finalize, (nb + 255) / 256, 256, 0, nb, d_vcoord, *buckets));
+    GB_CHECK(gb_launch(ctx, "k_table_finalize", k_table_finalize, (nb + 255) / 256, 256, 0, nb, d_vcoord, buckets));
     if (V > 0) GB_CUDA(cudaMemcpyAsync(&dropped, d_dropped, sizeof(int), cudaMemcpyDeviceToHost, st));
     GB_CUDA(cudaStreamSynchronize(st));
     *num_buckets = nb;
     *num_dropped_points = dropped;
-    if ((double)dropped <= drop_rate * total_points || nb >= (1 << 28)) break;
-    gb_dev_free(ctx->device, *buckets);
-    *buckets = nullptr;
-    nb *= 2;
+    if ((double)dropped <= drop_rate * total_points || nb >= (1 << 28)) {
+      table = std::move(attempt);
+      return GB_OK;
+    }
   }
-  return GB_OK;
 }
 
 // The grouping of a cloud of n > 0 points by the build's fp32 key at inv_res, for the voxel-map build and the point grid: the
@@ -252,21 +253,21 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
   m->max_scan = max_bucket_scan_count;
 
   CloudGroups g{};
+  gb_dev_block records(ctx->device), table(ctx->device);
   if (n > 0) {
     GB_CHECK(group_cloud(ctx, cloud, m->inv_res, g));
     if (g.V > 0) {
-      GB_CUDA(gb_dev_malloc(ctx->device, sizeof(float4) * 3 * (size_t)g.V, &m->base));
-      m->voxels = (float4*)m->base;
+      GB_CHECK(gb_dev_carve(ctx, records, [&](Carver& cv) { m->voxels = cv.take<float4>(3 * (size_t)g.V); }));
       GB_CHECK(gb_group_starts(ctx, n, g.t, g.flags, g.pos, g.starts));
       GB_CHECK(gb_launch(ctx, "k_voxel_reduce", k_voxel_reduce, (g.V + 127) / 128, 128, 0, g.V, g.starts, g.t.keys_s, g.t.idx_s, cloud->p0, cloud->p1, cloud->p2, cloud->inv_perm,
                          m->voxels, g.vcoord));
     }
   }
   m->num_voxels = g.V;
-  m->bytes = sizeof(float4) * 3 * (size_t)g.V;
-  GB_CHECK(table_build(ctx, g.V, g.vcoord, g.dropped, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, (double)n, &m->buckets, &m->num_buckets,
+  GB_CHECK(table_build(ctx, g.V, g.vcoord, g.dropped, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, (double)n, table, &m->num_buckets,
                        &m->num_dropped_points));
-  m->bytes += sizeof(int4) * (size_t)m->num_buckets;
+  records.hand_over(m->base);
+  table.hand_over(m->buckets);
   *out = m.release();
   return GB_OK;
 }
@@ -289,9 +290,9 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
 //   7. emit                the survivors, in ascending key order, into a new state block of the kind's layout (k_ins_emit:
 //                          keys, n, stamps, sums, fp32 records; k_ivox_emit: point records, cells, keys, stamps)
 //   8. table_build         the build's table kernels and sizing rule; an iVox has drop rate 0 and fails if a voxel is left out
-// Two host synchronisations (survivor count; dropped points of each table attempt).  The map is replaced only when every
-// step has succeeded.  The old blocks go back to the pool through gb_dev_free, which waits for every stream of the device:
-// a sweep of another context still reading them is safe.
+// Two host synchronisations (survivor count; dropped points of each table attempt).  The new blocks stay in their owners until
+// every step has succeeded; then they replace the map's, and the old blocks go back to the pool through gb_dev_free, which
+// waits for every stream of the device: a sweep of another context still reading them is safe.
 // ---------------------------------------------------------------------------------------------
 namespace {
 
@@ -566,6 +567,7 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
   gb_voxelmap next = *m;  // the map after this insert; m is replaced only when every step has succeeded
   next.lru_counter = m->lru_counter + 1;
   next.version = m->version + 1;
+  gb_dev_block table(ctx->device), base(ctx->device);  // the new blocks until the hand-over, then m's replaced ones (base ends first)
   if (N > 0) {
     const size_t cub_b = gb_cub_temp_bytes((size_t)N);
     InsertScratch s;
@@ -607,35 +609,18 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
     const int V = (int)info[1];
     next.num_voxels = V;
     next.num_points = (size_t)info[0];
-    next.base = nullptr;
-    next.buckets = nullptr;
     Carver size;
-    Rule::layout(size, &next);  // measures, and leaves every state pointer null
-    next.bytes = V > 0 ? size.off : 0;
-    gb_status r = GB_OK;
+    Rule::layout(size, &next);  // measures, and leaves every state pointer null: the layout of an empty map
     if (V > 0) {
-      GB_CUDA(gb_dev_malloc(ctx->device, size.off, &next.base));
-      Carver cv{(char*)next.base};
-      Rule::layout(cv, &next);
-      r = rule.emit(ctx, s, N, next);
+      GB_CHECK(gb_dev_carve(ctx, base, [&](Carver& cv) { Rule::layout(cv, &next); }));
+      GB_CHECK(rule.emit(ctx, s, N, next));
     }
-    if (r == GB_OK)
-      r = table_build(ctx, V, s.vcoord, s.dropped, m->init_buckets, m->max_scan, m->drop_rate, (double)info[0], &next.buckets, &next.num_buckets, &next.num_dropped_points);
-    if (r == GB_OK) r = rule.check_table(next);
-    if (r != GB_OK) {  // the insert's one failure exit once its block exists: m is unchanged
-      gb_dev_free(ctx->device, next.base);
-      gb_dev_free(ctx->device, next.buckets);
-      return r;
-    }
-    next.bytes += sizeof(int4) * (size_t)next.num_buckets;
+    GB_CHECK(table_build(ctx, V, s.vcoord, s.dropped, m->init_buckets, m->max_scan, m->drop_rate, (double)info[0], table, &next.num_buckets, &next.num_dropped_points));
+    GB_CHECK(rule.check_table(next));
+    base.hand_over(next.base);  // next held m's blocks until here
+    table.hand_over(next.buckets);
   }
-  void* old_base = m->base;
-  int4* old_buckets = m->buckets;
   *m = next;
-  if (N > 0) {
-    gb_dev_free(ctx->device, old_base);
-    gb_dev_free(ctx->device, old_buckets);
-  }
   return GB_OK;
 }
 
@@ -646,8 +631,9 @@ static gb_status map_create_empty(gb_ctx* ctx, const gb_voxelmap& init, gb_voxel
   gb_owned<gb_voxelmap> m(new (std::nothrow) gb_voxelmap(init), voxelmap_free);
   if (!m) return GB_ERR_INTERNAL;
   m->device = ctx->device;
-  GB_CHECK(table_build(ctx, 0, nullptr, nullptr, m->init_buckets, m->max_scan, m->drop_rate, 0.0, &m->buckets, &m->num_buckets, &m->num_dropped_points));
-  m->bytes = sizeof(int4) * (size_t)m->num_buckets;
+  gb_dev_block table(ctx->device);
+  GB_CHECK(table_build(ctx, 0, nullptr, nullptr, m->init_buckets, m->max_scan, m->drop_rate, 0.0, table, &m->num_buckets, &m->num_dropped_points));
+  table.hand_over(m->buckets);
   *out = m.release();
   return GB_OK;
 }
@@ -856,28 +842,25 @@ extern "C" gb_status gb_point_grid_build(gb_ctx* ctx, const gb_cloud* cloud, dou
   const int n = (int)cloud->n;
   cudaStream_t st = ctx->stream;
   CloudGroups c{};
+  gb_dev_block points(ctx->device), table(ctx->device);
   if (n > 0) {
     GB_CHECK(group_cloud(ctx, cloud, g->inv_res, c));
     g->num_voxels = c.V;
     g->num_points = (size_t)n;
-    Carver size;
-    grid_layout(size, g.get());
-    GB_CUDA(gb_dev_malloc(ctx->device, size.off, &g->base));
-    g->bytes = size.off;
-    Carver cv{(char*)g->base};
-    grid_layout(cv, g.get());
+    GB_CHECK(gb_dev_carve(ctx, points, [&](Carver& cv) { grid_layout(cv, g.get()); }));
     GB_CUDA(cudaMemsetAsync(c.extent, 0, sizeof(int), st));
     GB_CHECK(gb_group_starts(ctx, n, c.t, c.flags, c.pos, c.starts));
     GB_CHECK(gb_launch(ctx, "k_grid_emit", k_grid_emit, (n + 255) / 256, 256, 0, n, c.t.keys_s, c.t.idx_s, c.flags, c.pos, c.starts, cloud->p0, cloud->p1, cloud->p2,
                        cloud->inv_perm, g->voxels, g->cells, g->vkeys, c.vcoord, c.extent));
     GB_CUDA(cudaMemcpyAsync(&g->key_extent, c.extent, sizeof(int), cudaMemcpyDeviceToHost, st));  // read by table_build's synchronisation
   }
-  GB_CHECK(table_build(ctx, c.V, c.vcoord, c.dropped, g->init_buckets, g->max_scan, 0.0, (double)n, &g->buckets, &g->num_buckets, &g->num_dropped_points));
-  g->bytes += sizeof(int4) * (size_t)g->num_buckets;
+  GB_CHECK(table_build(ctx, c.V, c.vcoord, c.dropped, g->init_buckets, g->max_scan, 0.0, (double)n, table, &g->num_buckets, &g->num_dropped_points));
   if (g->num_dropped_points != 0) {
     gb_set_error("point grid table: %d points left out of a table of %d buckets", g->num_dropped_points, g->num_buckets);
     return GB_ERR_INTERNAL;
   }
+  points.hand_over(g->base);
+  table.hand_over(g->buckets);
   *out = reinterpret_cast<gb_point_grid*>(g.release());
   return GB_OK;
 }
@@ -940,21 +923,18 @@ __global__ void k_permute_cloud(int n, const int* __restrict__ perm, const float
 gb_status gb_cloud_build(gb_ctx* ctx, gb_cloud* c, size_t n_, const gb_planes& s, const gb_sort_tmp& t) {
   const int n = (int)n_;
   gb_planes d;
-  auto layout = [&](Carver& cv) {
+  gb_dev_block block(ctx->device);
+  GB_CHECK(gb_dev_carve(ctx, block, [&](Carver& cv) {
     d = gb_cloud_planes(cv, n_, s.normals != nullptr);
     c->perm = cv.take<int>(n_);
     c->inv_perm = cv.take<int>(n_);
-  };
-  Carver size;
-  layout(size);
-  GB_CUDA(gb_dev_malloc(ctx->device, size.off, &c->base));
-  c->bytes = size.off;
+  }));
   c->n = n_;
-  Carver cv{(char*)c->base};
-  layout(cv);
   c->p0 = d.p0; c->p1 = d.p1; c->p2 = d.p2; c->normals = d.normals;
   const int tb = 256, gb = (n + tb - 1) / tb;
   GB_CHECK(gb_launch(ctx, "k_morton_keys", k_morton_keys, gb, tb, 0, n, s.p0, t.keys, t.idx));
   GB_CUB(ctx, cub::DeviceRadixSort::SortPairs, t.cub, t.cub_bytes, t.keys, t.keys_s, t.idx, c->perm, n, 0, 64);
-  return gb_launch(ctx, "k_permute_cloud", k_permute_cloud, gb, tb, 0, n, c->perm, s.p0, s.p1, s.p2, s.normals, c->p0, c->p1, c->p2, c->normals, c->inv_perm);
+  GB_CHECK(gb_launch(ctx, "k_permute_cloud", k_permute_cloud, gb, tb, 0, n, c->perm, s.p0, s.p1, s.p2, s.normals, c->p0, c->p1, c->p2, c->normals, c->inv_perm));
+  block.hand_over(c->base);
+  return GB_OK;
 }

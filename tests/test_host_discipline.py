@@ -9,6 +9,8 @@
 5. align_up is called only by Carver: every block the host lays out is a Carver layout, run once to size and once to carve.
 6. delete (of a handle) and cudaFree / cudaFreeHost appear only in the free and release functions listed below: each
    handle has one free function, which every destroy entry point and every failed creation calls.
+7. gb_dev_malloc is called only by gb_dev_carve, and gb_dev_free only by the pool block's owner (gb_dev_block) and the free
+   functions: every pool block is taken by one carve and held by one owner until a handle takes it over.
 
 The function bodies are found by brace matching on the sources with comments, strings and preprocessor lines removed."""
 import os
@@ -169,12 +171,30 @@ def struct_body(code, name):
     return (m.end() - 1, match_brace(code, m.end() - 1)) if m else None
 
 
+def pool_uses(code, funcs):
+    """[(pos, 'malloc' | 'free', allowed)] of every use of gb_dev_malloc / gb_dev_free other than their declarations and
+    definitions (rule 7)."""
+    owner = struct_body(code, "gb_dev_block")
+    out = []
+    for m in re.finditer(r"\bgb_dev_(malloc|free)\b", code):
+        if re.search(r"\b(cudaError_t|void)\s+$", code[max(0, m.start() - 40):m.start()]):
+            continue
+        if m.group(1) == "malloc":
+            allowed = enclosing(funcs, m.start()) == "gb_dev_carve"
+        else:
+            allowed = enclosing(funcs, m.start()) in FREE_FUNCTIONS or bool(owner and owner[0] < m.start() < owner[1])
+        out.append((m.start(), m.group(1), allowed))
+    return out
+
+
 def violations(csrc):
-    """{rule: [offending site]} for rules 1-6 of this module's docstring."""
-    bad = {1: [], 2: [], 3: [], 4: [], 5: [], 6: []}
+    """{rule: [offending site]} for rules 1-7 of this module's docstring."""
+    bad = {1: [], 2: [], 3: [], 4: [], 5: [], 6: [], 7: []}
     enters = 0
     for f, code, directives, funcs in sources(csrc):
         where = lambda pos: f"{f}:{line_of(code, pos)} ({enclosing(funcs, pos)})"
+        bad[7] += [where(pos) for pos, _, allowed in pool_uses(code, funcs) if not allowed]
+        bad[7] += [f"{f}: {d.splitlines()[0].strip()}" for d in directives if re.search(r"\bgb_dev_(malloc|free)\b", d)]
         carver = struct_body(code, "Carver")
         for m in re.finditer(r"\balign_up\b", code):
             definition = re.search(r"\bsize_t\s+$", code[max(0, m.start() - 40):m.start()])
@@ -221,6 +241,7 @@ def violations(csrc):
 def parsed_inventory(csrc):
     """Sanity numbers of the parse, so that a rule cannot pass because the parser found nothing."""
     names, launches_in_helper, cub_calls, carver_align, frees = set(), 0, 0, 0, 0
+    pool = {"malloc": 0, "free": 0}  # allowed uses of gb_dev_malloc / gb_dev_free (rule 7)
     for f, code, _, funcs in sources(csrc):
         names.update(n for n, *_ in funcs)
         launches_in_helper += sum(1 for m in re.finditer(r"<<<", code) if enclosing(funcs, m.start()) == "gb_launch")
@@ -229,17 +250,21 @@ def parsed_inventory(csrc):
         if carver:
             carver_align += len(re.findall(r"\balign_up\s*\(", code[carver[0]:carver[1]]))
         frees += sum(1 for m in re.finditer(r"\bdelete\b|\bcudaFree(Host)?\s*\(", code) if enclosing(funcs, m.start()) in FREE_FUNCTIONS)
-    return names, launches_in_helper, cub_calls, carver_align, frees
+        for _, kind, allowed in pool_uses(code, funcs):
+            pool[kind] += allowed
+    return names, launches_in_helper, cub_calls, carver_align, frees, pool
 
 
 def test_parser_sees_the_library():
-    names, launches_in_helper, cub_calls, carver_align, frees = parsed_inventory(CSRC)
-    assert {"gb_launch", "sweep_linearize", "gb_preprocess", "gb_vgicp_align", "gb_deskew", "knn_device", "table_build"} <= names
+    names, launches_in_helper, cub_calls, carver_align, frees, pool = parsed_inventory(CSRC)
+    assert {"gb_launch", "sweep_linearize", "gb_preprocess", "gb_vgicp_align", "gb_deskew", "knn_device", "table_build", "gb_dev_carve"} <= names
     assert set(FREE_FUNCTIONS) <= names
     assert launches_in_helper == 1
     assert cub_calls >= 10
     assert carver_align == 1
     assert frees >= len(FREE_FUNCTIONS)
+    # the carve's one allocation; the owner's free and those of cloud_free (3 blocks) and voxelmap_free (2)
+    assert pool == {"malloc": 1, "free": 6}
     _, enters = violations(CSRC)
     assert enters >= 29  # gb_peer_slab_destroy is teardown now: peer_slab_free locks the context by hand
 
@@ -266,3 +291,7 @@ def test_align_up_only_in_carver():
 
 def test_handles_freed_only_by_their_free_functions():
     assert violations(CSRC)[0][6] == []
+
+
+def test_pool_blocks_taken_by_one_carve_and_returned_by_one_owner():
+    assert violations(CSRC)[0][7] == []
