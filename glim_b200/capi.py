@@ -11,31 +11,98 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.path.join(_HERE, "libglim_b200.so")
 
-# every symbol include/glim_b200.h declares (tests check the library exports exactly these)
-SYMBOLS = [
-    "gb_status_string", "gb_last_error", "gb_device_count", "gb_mem_info",
-    "gb_ctx_create", "gb_ctx_create_on_stream", "gb_ctx_destroy", "gb_ctx_synchronize", "gb_ctx_stream", "gb_ctx_kernel_launches",
-    "gb_cloud_upload", "gb_cloud_size", "gb_cloud_download", "gb_cloud_device_ptrs", "gb_cloud_destroy",
-    "gb_hessian_blocks", "gb_slab_row_hessian_blocks",
-    "gb_voxelmap_build", "gb_voxelmap_info", "gb_voxelmap_download", "gb_voxelmap_destroy",
-    "gb_voxelmap_create_incremental", "gb_voxelmap_insert",
-    "gb_vgicp_factor_create", "gb_vgicp_factor_destroy", "gb_vgicp_linearize", "gb_vgicp_error",
-    "gb_factor_set_linearize", "gb_factor_set_error",
-    "gb_sweep_create", "gb_sweep_destroy", "gb_sweep_attach_slab", "gb_sweep_set_poses", "gb_sweep_launch", "gb_sweep_fetch", "gb_sweep_linearize",
-    "gb_sweep_results_device", "gb_sweep_stats",
-    "gb_peer_slab_create", "gb_peer_slab_export", "gb_peer_slab_connect", "gb_peer_slab_destroy", "gb_sweep_attach_peer_slab",
-    "gb_peer_slab_signal_wait", "gb_peer_slab_device_ptr", "gb_peer_slab_fetch", "gb_peer_slab_fetch_async",
-    "gb_overlap", "gb_covariances", "gb_find_neighbors", "gb_voxelgrid_sampling", "gb_preprocess_default_params", "gb_preprocess", "gb_merge_frames",
-    "gb_deskew_pose_table", "gb_deskew",
-    "gb_align_default_params", "gb_vgicp_align",
-    "gb_ivox_create", "gb_ivox_insert", "gb_ivox_info", "gb_ivox_download", "gb_ivox_destroy", "gb_gicp_factor_create",
-    "gb_cloud_add_times", "gb_cloud_time_table", "gb_ct_gicp_factor_create", "gb_ct_gicp_linearize", "gb_ct_gicp_error",
-    "gb_ct_default_params", "gb_ct_gicp_align", "gb_ct_deskew",
-    "gb_point_grid_build", "gb_point_grid_info", "gb_point_grid_download", "gb_point_grid_destroy", "gb_gicp_grid_factor_create",
-    "gb_gicp_grid_factor_half_width",
-    "gb_cloud_estimate_fpfh", "gb_cloud_fpfh", "gb_fpfh_match", "gb_ransac_default_params", "gb_ransac_align",
-    "gb_gnc_default_params", "gb_gnc_align",
-]
+# every function include/glim_b200.h declares -> (argtypes, restype): pointers and arrays are c_void_p, and st is the gb_status
+# code (tests/test_binding_host.py checks the table against the header's prototypes)
+vp, i32, f32, f64, sz, u64, st = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_size_t, C.c_uint64, C.c_int
+_SIGNATURES = {
+    "gb_status_string": ([i32], C.c_char_p),
+    "gb_last_error": ([], C.c_char_p),
+    "gb_device_count": ([], i32),
+    "gb_mem_info": ([i32, vp, vp], st),
+    "gb_ctx_create": ([i32, vp], st),
+    "gb_ctx_create_on_stream": ([i32, vp, vp], st),
+    "gb_ctx_destroy": ([vp], st),
+    "gb_ctx_synchronize": ([vp], st),
+    "gb_ctx_stream": ([vp], vp),
+    "gb_ctx_kernel_launches": ([vp], u64),
+    "gb_cloud_upload": ([vp, sz, vp, vp, vp, vp], st),
+    "gb_cloud_size": ([vp, vp], st),
+    "gb_cloud_download": ([vp, vp, vp], st),
+    "gb_cloud_device_ptrs": ([vp, vp, vp, vp, vp], st),
+    "gb_cloud_destroy": ([vp], st),
+    "gb_hessian_blocks": ([vp, f64, vp, vp, vp, vp, vp, vp], st),
+    "gb_slab_row_hessian_blocks": ([vp, f64, vp, vp, vp, vp, vp, vp, vp], st),
+    "gb_voxelmap_build": ([vp, vp, f32, i32, i32, f64, vp], st),
+    "gb_voxelmap_info": ([vp, vp, vp, vp], st),
+    "gb_voxelmap_download": ([vp, vp, vp, vp, vp], st),
+    "gb_voxelmap_destroy": ([vp], st),
+    "gb_voxelmap_create_incremental": ([vp, f32, i32, i32, f64, i32, i32, vp], st),
+    "gb_voxelmap_insert": ([vp, vp, vp, vp, f64, u64], st),
+    "gb_vgicp_factor_create": ([vp, vp, vp, i32, vp], st),
+    "gb_vgicp_factor_destroy": ([vp], st),
+    "gb_vgicp_linearize": ([vp, vp, vp], st),
+    "gb_vgicp_error": ([vp, vp, vp, vp], st),
+    "gb_factor_set_linearize": ([vp, sz, vp, vp, vp], st),
+    "gb_factor_set_error": ([vp, sz, vp, vp, vp, vp], st),
+    "gb_sweep_create": ([vp, sz, vp, vp, vp], st),
+    "gb_sweep_destroy": ([vp], st),
+    "gb_sweep_attach_slab": ([vp, vp, sz], st),
+    "gb_sweep_set_poses": ([vp, vp], st),
+    "gb_sweep_launch": ([vp], st),
+    "gb_sweep_fetch": ([vp, vp], st),
+    "gb_sweep_linearize": ([vp, vp, vp], st),
+    "gb_sweep_results_device": ([vp, vp], st),
+    "gb_sweep_stats": ([vp, vp, vp, vp, vp], st),
+    "gb_peer_slab_create": ([vp, sz, i32, i32, vp], st),
+    "gb_peer_slab_export": ([vp, vp], st),
+    "gb_peer_slab_connect": ([vp, vp], st),
+    "gb_peer_slab_destroy": ([vp], st),
+    "gb_sweep_attach_peer_slab": ([vp, vp], st),
+    "gb_peer_slab_signal_wait": ([vp], st),
+    "gb_peer_slab_device_ptr": ([vp, vp], st),
+    "gb_peer_slab_fetch": ([vp, vp], st),
+    "gb_peer_slab_fetch_async": ([vp, vp], st),
+    "gb_overlap": ([vp, sz, vp, vp, vp, vp], st),
+    "gb_covariances": ([vp, sz, vp, vp, i32, i32, vp, vp], st),
+    "gb_find_neighbors": ([vp, sz, vp, i32, vp], st),
+    "gb_voxelgrid_sampling": ([vp, sz, vp, vp, vp, f64, vp, vp, vp, vp], st),
+    "gb_preprocess_default_params": ([vp], st),
+    "gb_preprocess": ([vp, sz, vp, vp, vp, vp, vp], st),
+    "gb_merge_frames": ([vp, sz, vp, vp, f64, i32, u64, vp, vp, vp, vp], st),
+    "gb_deskew_pose_table": ([vp, vp, vp, sz, vp, vp, f64, sz, vp, vp, vp, vp], st),
+    "gb_deskew": ([vp, vp, vp, vp, sz, vp, vp, f64, sz, vp, vp, vp, vp], st),
+    "gb_align_default_params": ([vp], st),
+    "gb_vgicp_align": ([vp, sz, vp, vp, vp, vp, vp], st),
+    "gb_ivox_create": ([vp, f64, f64, i32, i32, i32, i32, vp], st),
+    "gb_ivox_insert": ([vp, vp, vp, vp, f64, u64], st),
+    "gb_ivox_info": ([vp, vp, vp, vp], st),
+    "gb_ivox_download": ([vp, vp, vp, vp, vp], st),
+    "gb_ivox_destroy": ([vp], st),
+    "gb_gicp_factor_create": ([vp, vp, vp, f64, vp], st),
+    "gb_cloud_add_times": ([vp, vp, sz, vp], st),
+    "gb_cloud_time_table": ([vp, vp, vp, vp, vp, vp], st),
+    "gb_ct_gicp_factor_create": ([vp, vp, vp, f64, vp], st),
+    "gb_ct_gicp_linearize": ([vp, vp, vp, vp], st),
+    "gb_ct_gicp_error": ([vp, vp, vp, vp, vp, vp], st),
+    "gb_ct_default_params": ([vp], st),
+    "gb_ct_gicp_align": ([vp, sz, vp, vp, vp, vp, vp, vp], st),
+    "gb_ct_deskew": ([vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp], st),
+    "gb_point_grid_build": ([vp, vp, f64, vp], st),
+    "gb_point_grid_info": ([vp, vp, vp, vp], st),
+    "gb_point_grid_download": ([vp, vp, vp, vp, vp, vp], st),
+    "gb_point_grid_destroy": ([vp], st),
+    "gb_gicp_grid_factor_create": ([vp, vp, vp, f64, vp], st),
+    "gb_gicp_grid_factor_half_width": ([vp, vp], st),
+    "gb_cloud_estimate_fpfh": ([vp, vp, f64], st),
+    "gb_cloud_fpfh": ([vp, vp], st),
+    "gb_fpfh_match": ([vp, vp, vp, vp], st),
+    "gb_ransac_default_params": ([vp], st),
+    "gb_ransac_align": ([vp, vp, vp, vp, vp, vp], st),
+    "gb_gnc_default_params": ([vp], st),
+    "gb_gnc_align": ([vp, vp, vp, vp, vp, vp, vp], st),
+}
+del vp, i32, f32, f64, sz, u64, st
+SYMBOLS = tuple(_SIGNATURES)  # tests check the library exports exactly these
 
 GB_SLAB_STRIDE = 96
 GB_IPC_HANDLE_BYTES = 64
@@ -129,97 +196,9 @@ def lib():
     if not os.path.exists(SO_PATH):
         raise GlimB200Error(f"{SO_PATH} is missing: the CUDA extension is not built (python __graft_entry__.py build); there is no CPU fallback")
     L = C.CDLL(SO_PATH)
-    vp, i32, f32, f64, sz, u64 = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_size_t, C.c_uint64
-    L.gb_status_string.restype = C.c_char_p
-    L.gb_status_string.argtypes = [i32]
-    L.gb_last_error.restype = C.c_char_p
-    L.gb_device_count.restype = i32
-    L.gb_mem_info.argtypes = [i32, vp, vp]
-    L.gb_ctx_create.argtypes = [i32, vp]
-    L.gb_ctx_create_on_stream.argtypes = [i32, vp, vp]
-    L.gb_ctx_destroy.argtypes = [vp]
-    L.gb_ctx_synchronize.argtypes = [vp]
-    L.gb_ctx_stream.restype = vp
-    L.gb_ctx_stream.argtypes = [vp]
-    L.gb_ctx_kernel_launches.restype = u64
-    L.gb_ctx_kernel_launches.argtypes = [vp]
-    L.gb_cloud_upload.argtypes = [vp, sz, vp, vp, vp, vp]
-    L.gb_cloud_size.argtypes = [vp, vp]
-    L.gb_cloud_download.argtypes = [vp, vp, vp]
-    L.gb_cloud_destroy.argtypes = [vp]
-    L.gb_cloud_device_ptrs.argtypes = [vp, vp, vp, vp, vp]
-    L.gb_sweep_linearize.argtypes = [vp, vp, vp]
-    L.gb_preprocess_default_params.argtypes = [vp]
-    L.gb_preprocess.argtypes = [vp, sz, vp, vp, vp, vp, vp]
-    L.gb_merge_frames.argtypes = [vp, sz, vp, vp, f64, i32, u64, vp, vp, vp, vp]
-    L.gb_hessian_blocks.argtypes = [vp, f64, vp, vp, vp, vp, vp, vp]
-    L.gb_slab_row_hessian_blocks.argtypes = [vp, f64, vp, vp, vp, vp, vp, vp, vp]
-    L.gb_voxelmap_build.argtypes = [vp, vp, f32, i32, i32, f64, vp]
-    L.gb_voxelmap_info.argtypes = [vp, vp, vp, vp]
-    L.gb_voxelmap_download.argtypes = [vp, vp, vp, vp, vp]
-    L.gb_voxelmap_destroy.argtypes = [vp]
-    L.gb_voxelmap_create_incremental.argtypes = [vp, f32, i32, i32, f64, i32, i32, vp]
-    L.gb_voxelmap_insert.argtypes = [vp, vp, vp, vp, f64, u64]
-    L.gb_vgicp_factor_create.argtypes = [vp, vp, vp, i32, vp]
-    L.gb_vgicp_factor_destroy.argtypes = [vp]
-    L.gb_vgicp_linearize.argtypes = [vp, vp, vp]
-    L.gb_vgicp_error.argtypes = [vp, vp, vp, vp]
-    L.gb_factor_set_linearize.argtypes = [vp, sz, vp, vp, vp]
-    L.gb_factor_set_error.argtypes = [vp, sz, vp, vp, vp, vp]
-    L.gb_sweep_create.argtypes = [vp, sz, vp, vp, vp]
-    L.gb_sweep_destroy.argtypes = [vp]
-    L.gb_sweep_attach_slab.argtypes = [vp, vp, sz]
-    L.gb_sweep_set_poses.argtypes = [vp, vp]
-    L.gb_sweep_launch.argtypes = [vp]
-    L.gb_sweep_fetch.argtypes = [vp, vp]
-    L.gb_sweep_results_device.argtypes = [vp, vp]
-    L.gb_sweep_stats.argtypes = [vp, vp, vp, vp, vp]
-    L.gb_peer_slab_create.argtypes = [vp, sz, i32, i32, vp]
-    L.gb_peer_slab_export.argtypes = [vp, vp]
-    L.gb_peer_slab_connect.argtypes = [vp, vp]
-    L.gb_peer_slab_destroy.argtypes = [vp]
-    L.gb_sweep_attach_peer_slab.argtypes = [vp, vp]
-    L.gb_peer_slab_signal_wait.argtypes = [vp]
-    L.gb_peer_slab_device_ptr.argtypes = [vp, vp]
-    L.gb_peer_slab_fetch.argtypes = [vp, vp]
-    L.gb_peer_slab_fetch_async.argtypes = [vp, vp]
-    L.gb_overlap.argtypes = [vp, sz, vp, vp, vp, vp]
-    L.gb_covariances.argtypes = [vp, sz, vp, vp, i32, i32, vp, vp]
-    L.gb_find_neighbors.argtypes = [vp, sz, vp, i32, vp]
-    L.gb_voxelgrid_sampling.argtypes = [vp, sz, vp, vp, vp, f64, vp, vp, vp, vp]
-    L.gb_deskew_pose_table.argtypes = [vp, vp, vp, sz, vp, vp, f64, sz, vp, vp, vp, vp]
-    L.gb_deskew.argtypes = [vp, vp, vp, vp, sz, vp, vp, f64, sz, vp, vp, vp, vp]
-    L.gb_align_default_params.argtypes = [vp]
-    L.gb_vgicp_align.argtypes = [vp, sz, vp, vp, vp, vp, vp]
-    L.gb_ivox_create.argtypes = [vp, f64, f64, i32, i32, i32, i32, vp]
-    L.gb_ivox_insert.argtypes = [vp, vp, vp, vp, f64, u64]
-    L.gb_ivox_info.argtypes = [vp, vp, vp, vp]
-    L.gb_ivox_download.argtypes = [vp, vp, vp, vp, vp]
-    L.gb_ivox_destroy.argtypes = [vp]
-    L.gb_gicp_factor_create.argtypes = [vp, vp, vp, f64, vp]
-    L.gb_cloud_add_times.argtypes = [vp, vp, sz, vp]
-    L.gb_cloud_time_table.argtypes = [vp, vp, vp, vp, vp, vp]
-    L.gb_ct_gicp_factor_create.argtypes = [vp, vp, vp, f64, vp]
-    L.gb_ct_gicp_linearize.argtypes = [vp, vp, vp, vp]
-    L.gb_ct_gicp_error.argtypes = [vp, vp, vp, vp, vp, vp]
-    L.gb_ct_default_params.argtypes = [vp]
-    L.gb_ct_gicp_align.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp]
-    L.gb_ct_deskew.argtypes = [vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]
-    L.gb_point_grid_build.argtypes = [vp, vp, f64, vp]
-    L.gb_point_grid_info.argtypes = [vp, vp, vp, vp]
-    L.gb_point_grid_download.argtypes = [vp, vp, vp, vp, vp, vp]
-    L.gb_point_grid_destroy.argtypes = [vp]
-    L.gb_gicp_grid_factor_create.argtypes = [vp, vp, vp, f64, vp]
-    L.gb_gicp_grid_factor_half_width.argtypes = [vp, vp]
-    L.gb_cloud_estimate_fpfh.argtypes = [vp, vp, f64]
-    L.gb_cloud_fpfh.argtypes = [vp, vp]
-    L.gb_fpfh_match.argtypes = [vp, vp, vp, vp]
-    L.gb_ransac_default_params.argtypes = [vp]
-    L.gb_ransac_align.argtypes = [vp, vp, vp, vp, vp, vp]
-    L.gb_gnc_default_params.argtypes = [vp]
-    L.gb_gnc_align.argtypes = [vp, vp, vp, vp, vp, vp, vp]
-    for name in SYMBOLS:
-        getattr(L, name)  # AttributeError here means the library and include/glim_b200.h are out of sync
+    for name, (argtypes, restype) in _SIGNATURES.items():
+        fn = getattr(L, name)  # AttributeError here means the library and include/glim_b200.h are out of sync
+        fn.argtypes, fn.restype = argtypes, restype
     _lib = L
     return L
 

@@ -38,16 +38,43 @@ LIN_DTYPE = np.dtype([("H_tt", "f8", (36,)), ("H_ss", "f8", (36,)), ("H_ts", "f8
 assert LIN_DTYPE.itemsize == 122 * 8
 
 
-class Context:
+class _Handle:
+    """An object holding one C-ABI handle `h`, which the class's `_destroy` function releases exactly once: on close() or when
+    the object is collected.  The release does not depend on the Context being open: clouds and maps keep no context, and
+    factors, sweeps and peer slabs hold a reference to theirs that their destroy function drops."""
+
+    _destroy = ""  # the gb_*_destroy entry point of the class
+    h = None
+
+    @staticmethod
+    def _create(create, *args) -> C.c_void_p:
+        """create(*args, &handle) -> handle; raises if the call fails"""
+        h = C.c_void_p()
+        check(create(*args, C.byref(h)))
+        return h
+
+    def close(self):
+        h, self.h = self.h, None
+        if h:
+            getattr(lib(), self._destroy)(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # at interpreter shutdown the module globals may already be gone
+            pass
+
+
+class Context(_Handle):
     """gtsam_points::CUDAStream + StreamTempBufferRoundRobin (odometry_estimation_gpu.cpp:76-77)."""
 
+    _destroy = "gb_ctx_destroy"
+
     def __init__(self, device: int = 0, cuda_stream: int | None = None):
-        h = C.c_void_p()
         if cuda_stream is None:
-            check(lib().gb_ctx_create(device, C.byref(h)))
+            self.h = self._create(lib().gb_ctx_create, device)
         else:
-            check(lib().gb_ctx_create_on_stream(device, C.c_void_p(cuda_stream), C.byref(h)))
-        self.h = h
+            self.h = self._create(lib().gb_ctx_create_on_stream, device, C.c_void_p(cuda_stream))
         self.device = device
 
     def synchronize(self):
@@ -61,17 +88,6 @@ class Context:
     def kernel_launches(self) -> int:
         return lib().gb_ctx_kernel_launches(self.h)
 
-    def close(self):
-        if self.h:
-            lib().gb_ctx_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 _default_ctx = {}
 
@@ -82,8 +98,10 @@ def default_context(device: int = 0) -> Context:
     return _default_ctx[device]
 
 
-class PointCloudGPU:
+class PointCloudGPU(_Handle):
     """gtsam_points::PointCloudGPU (device copy of points / covs / normals in fp32)."""
+
+    _destroy = "gb_cloud_destroy"
 
     def __init__(self, ctx: Context, handle, n: int):
         self.ctx, self.h, self.n = ctx, handle, n
@@ -100,9 +118,7 @@ class PointCloudGPU:
             # [i,row,col] -> column-major 4x4 per point
             c16 = np.ascontiguousarray(np.swapaxes(covs.reshape(n, 4, 4), 1, 2)).reshape(n, 16)
         nr = f64(normals) if normals is not None else None
-        h = C.c_void_p()
-        check(lib().gb_cloud_upload(ctx.h, n, ptr(points), ptr(c16), ptr(nr), C.byref(h)))
-        return PointCloudGPU(ctx, h, n)
+        return PointCloudGPU(ctx, PointCloudGPU._create(lib().gb_cloud_upload, ctx.h, n, ptr(points), ptr(c16), ptr(nr)), n)
 
     def size(self) -> int:
         return self.n
@@ -141,14 +157,11 @@ class PointCloudGPU:
         check(lib().gb_cloud_fpfh(self.h, ptr(out)))
         return out
 
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            lib().gb_cloud_destroy(self.h)
-            self.h = None
 
-
-class GaussianVoxelMapGPU:
+class GaussianVoxelMapGPU(_Handle):
     """gtsam_points::GaussianVoxelMapGPU(resolution, init_num_buckets, max_bucket_scan_count, target_points_drop_rate)."""
+
+    _destroy = "gb_voxelmap_destroy"
 
     def __init__(self, resolution: float, init_num_buckets: int = 8192 * 2, max_bucket_scan_count: int = 10, target_points_drop_rate: float = 1e-3, ctx: Context | None = None):
         self.resolution = float(resolution)
@@ -156,7 +169,6 @@ class GaussianVoxelMapGPU:
         self.max_bucket_scan_count = max_bucket_scan_count
         self.target_points_drop_rate = target_points_drop_rate
         self.ctx = ctx
-        self.h = None
         self.num_voxels = 0
         self.num_buckets = 0
         self._cloud = None
@@ -165,13 +177,14 @@ class GaussianVoxelMapGPU:
         if self.h is not None:
             raise capi.GlimB200Error("GaussianVoxelMapGPU::insert may be called once (as every GLIM call site does)")
         self.ctx = self.ctx or cloud.ctx
-        h = C.c_void_p()
-        check(lib().gb_voxelmap_build(self.ctx.h, cloud.h, self.resolution, self.init_num_buckets, self.max_bucket_scan_count, self.target_points_drop_rate, C.byref(h)))
-        self.h = h
-        nv, nb, res = C.c_int(), C.c_int(), C.c_float()
-        check(lib().gb_voxelmap_info(h, C.byref(nv), C.byref(nb), C.byref(res)))
-        self.num_voxels, self.num_buckets = nv.value, nb.value
+        self.h = self._create(lib().gb_voxelmap_build, self.ctx.h, cloud.h, self.resolution, self.init_num_buckets, self.max_bucket_scan_count, self.target_points_drop_rate)
+        self._info()
         return self
+
+    def _info(self):
+        nv, nb, res = C.c_int(), C.c_int(), C.c_float()
+        check(lib().gb_voxelmap_info(self.h, C.byref(nv), C.byref(nb), C.byref(res)))
+        self.num_voxels, self.num_buckets = nv.value, nb.value
 
     def voxel_resolution(self) -> float:
         return self.resolution
@@ -184,32 +197,23 @@ class GaussianVoxelMapGPU:
         check(lib().gb_voxelmap_download(self.h, ptr(buckets), ptr(vnum), ptr(vmean), ptr(vcov)))
         return buckets, vnum, vmean, vcov
 
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx and self.ctx.h:
-            lib().gb_voxelmap_destroy(self.h)
-            self.h = None
 
-
-class IncrementalVoxelMapGPU:
+class IncrementalVoxelMapGPU(_Handle):
     """A Gaussian voxel map kept on the device across frames (gb_voxelmap_create_incremental / gb_voxelmap_insert): the
     GaussianVoxelMapCPU::insert + set_lru_horizon target of GLIM's odometry (odometry_estimation_cpu.cpp:67, :177-191).  Accepted
     wherever a GaussianVoxelMapGPU is (factors, align_vgicp, overlap_gpu); factors and sweeps follow its inserts."""
+
+    _destroy = "gb_voxelmap_destroy"
 
     def __init__(self, resolution: float, lru_horizon: int = 0, lru_clear_cycle: int = 10, init_num_buckets: int = 16384, max_bucket_scan_count: int = 10,
                  target_points_drop_rate: float = 1e-3, ctx: Context | None = None):
         self.ctx = ctx or default_context()
         self.resolution = float(resolution)
-        self.h = None
-        h = C.c_void_p()
-        check(lib().gb_voxelmap_create_incremental(self.ctx.h, self.resolution, init_num_buckets, max_bucket_scan_count, target_points_drop_rate,
-                                                   int(lru_horizon), int(lru_clear_cycle), C.byref(h)))
-        self.h = h
+        self.h = self._create(lib().gb_voxelmap_create_incremental, self.ctx.h, self.resolution, init_num_buckets, max_bucket_scan_count,
+                              target_points_drop_rate, int(lru_horizon), int(lru_clear_cycle))
         self._info()
 
-    def _info(self):
-        nv, nb, res = C.c_int(), C.c_int(), C.c_float()
-        check(lib().gb_voxelmap_info(self.h, C.byref(nv), C.byref(nb), C.byref(res)))
-        self.num_voxels, self.num_buckets = nv.value, nb.value
+    _info = GaussianVoxelMapGPU._info
 
     def insert(self, cloud: PointCloudGPU, T=None, sampling_rate: float = 1.0, seed: int = 0):
         """Insert `cloud` at T_map_cloud (4x4, None = identity), keeping a sampling_rate share of its points."""
@@ -222,11 +226,6 @@ class IncrementalVoxelMapGPU:
         return self.resolution
 
     download = GaussianVoxelMapGPU.download
-
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx and self.ctx.h:
-            lib().gb_voxelmap_destroy(self.h)
-            self.h = None
 
 
 def unpack_linearized(rec) -> dict:
@@ -242,12 +241,14 @@ def unpack_linearized(rec) -> dict:
     }
 
 
-class IntegratedVGICPFactorGPU:
+class IntegratedVGICPFactorGPU(_Handle):
     """gtsam_points::IntegratedVGICPFactorGPU.
 
     Binary form: (target_key, source_key, voxelmap, source); unary form: (fixed_target_pose 4x4, source_key, ...).
-    `values` is a dict key -> 4x4 pose.  delta = T_target^-1 T_source (SURVEY A.1).
+    `values` is a dict key -> 4x4 pose.  delta = T_target^-1 T_source (SURVEY A.1).  The handle is created on first use.
     """
+
+    _destroy = "gb_vgicp_factor_destroy"
 
     def __init__(self, target, source_key, voxelmap: GaussianVoxelMapGPU, source: PointCloudGPU, ctx: Context | None = None):
         self.ctx = ctx or source.ctx
@@ -260,7 +261,6 @@ class IntegratedVGICPFactorGPU:
         self.source_key = source_key
         self.voxelmap, self.source = voxelmap, source  # keep alive, as the reference factor's shared_ptrs do
         self.flags = 0
-        self.h = None
         self._lin_point = None
 
     def set_enable_surface_validation(self, enable: bool):
@@ -270,9 +270,7 @@ class IntegratedVGICPFactorGPU:
 
     def _handle(self):
         if self.h is None:
-            h = C.c_void_p()
-            check(lib().gb_vgicp_factor_create(self.ctx.h, self.voxelmap.h, self.source.h, self.flags, C.byref(h)))
-            self.h = h
+            self.h = self._create(lib().gb_vgicp_factor_create, self.ctx.h, self.voxelmap.h, self.source.h, self.flags)
         return self.h
 
     def keys(self):
@@ -310,25 +308,19 @@ class IntegratedVGICPFactorGPU:
         check(lib().gb_vgicp_error(self._handle(), ptr(pose16(lin)), ptr(pose16(d)), C.byref(e)))
         return e.value
 
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            lib().gb_vgicp_factor_destroy(self.h)
-            self.h = None
 
-
-class IVoxGPU:
+class IVoxGPU(_Handle):
     """gtsam_points::iVox kept on the device (gb_ivox_create / gb_ivox_insert): the GICP target of GLIM's CPU odometry
     (odometry_estimation_cpu.cpp:57-61, update_target :177-191).  Factors and sweeps on it follow its inserts."""
+
+    _destroy = "gb_ivox_destroy"
 
     def __init__(self, resolution: float, min_dist_in_cell: float = 0.1, max_points_in_cell: int = 10, neighbor_voxel_mode: int = 1,
                  lru_horizon: int = 100, lru_clear_cycle: int = 10, ctx: Context | None = None):
         self.ctx = ctx or default_context()
         self.resolution = float(resolution)
-        self.h = None
-        h = C.c_void_p()
-        check(lib().gb_ivox_create(self.ctx.h, self.resolution, float(min_dist_in_cell), int(max_points_in_cell), int(neighbor_voxel_mode),
-                                   int(lru_horizon), int(lru_clear_cycle), C.byref(h)))
-        self.h = h
+        self.h = self._create(lib().gb_ivox_create, self.ctx.h, self.resolution, float(min_dist_in_cell), int(max_points_in_cell), int(neighbor_voxel_mode),
+                              int(lru_horizon), int(lru_clear_cycle))
         self.info()
 
     def info(self):
@@ -357,24 +349,18 @@ class IVoxGPU:
         check(lib().gb_ivox_download(self.h, ptr(coords), ptr(counts), ptr(xyz), ptr(cov6)))
         return coords, counts, xyz, cov6
 
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx and self.ctx.h:
-            lib().gb_ivox_destroy(self.h)
-            self.h = None
 
-
-class PointGridGPU:
+class PointGridGPU(_Handle):
     """A whole frame's points on the device, grouped in cubic cells (gb_point_grid_build): the target of a GICP factor between
     two frames, where gtsam_points builds a KdTree (global_mapping_pose_graph.cpp:273).  Built once from a PointCloudGPU, which
     may be released afterwards."""
 
+    _destroy = "gb_point_grid_destroy"
+
     def __init__(self, cloud: PointCloudGPU, cell_size: float, ctx: Context | None = None):
         self.ctx = ctx or cloud.ctx
         self.cell_size = float(cell_size)
-        self.h = None
-        h = C.c_void_p()
-        check(lib().gb_point_grid_build(self.ctx.h, cloud.h, self.cell_size, C.byref(h)))
-        self.h = h
+        self.h = self._create(lib().gb_point_grid_build, self.ctx.h, cloud.h, self.cell_size)
         nc, npt = C.c_int(), C.c_size_t()
         check(lib().gb_point_grid_info(self.h, C.byref(nc), C.byref(npt), None))
         self.num_cells, self.num_points = nc.value, npt.value
@@ -387,11 +373,6 @@ class PointGridGPU:
         xyz, cov6 = np.empty((P, 3), np.float32), np.empty((P, 6), np.float32)
         check(lib().gb_point_grid_download(self.h, ptr(coords), ptr(counts), ptr(idx), ptr(xyz), ptr(cov6)))
         return coords, counts, idx, xyz, cov6
-
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx and self.ctx.h:
-            lib().gb_point_grid_destroy(self.h)
-            self.h = None
 
 
 class IntegratedGICPFactorGPU(IntegratedVGICPFactorGPU):
@@ -411,10 +392,8 @@ class IntegratedGICPFactorGPU(IntegratedVGICPFactorGPU):
 
     def _handle(self):
         if self.h is None:
-            h = C.c_void_p()
             create = lib().gb_gicp_grid_factor_create if isinstance(self.ivox, PointGridGPU) else lib().gb_gicp_factor_create
-            check(create(self.ctx.h, self.ivox.h, self.source.h, self.max_correspondence_distance, C.byref(h)))
-            self.h = h
+            self.h = self._create(create, self.ctx.h, self.ivox.h, self.source.h, self.max_correspondence_distance)
         return self.h
 
     def search_half_width(self) -> int:
@@ -424,22 +403,21 @@ class IntegratedGICPFactorGPU(IntegratedVGICPFactorGPU):
         return m.value
 
 
-class IntegratedCT_GICPFactorGPU:
+class IntegratedCT_GICPFactorGPU(_Handle):
     """IntegratedCT_GICPFactor_<iVox, PointCloud>(X, Y, ivox, frame, ivox) + max_correspondence_distance
     (odometry_estimation_ct.cpp:159-163) on the device.  Its two keys are the poses at the scan's first and last time-table
     entries; the source must carry times (PointCloudGPU.add_times).  linearize(values) returns the usual dict with X in the
     target slot (H_tt = H_XX, b_t = b_X) and Y in the source slot (H_ss = H_YY, b_s = b_Y), H_ts = H_XY."""
+
+    _destroy = "gb_vgicp_factor_destroy"
 
     def __init__(self, key_X, key_Y, ivox: IVoxGPU, source: PointCloudGPU, max_correspondence_distance: float, ctx: Context | None = None):
         self.ctx = ctx or source.ctx
         self.key_X, self.key_Y = key_X, key_Y
         self.ivox, self.source = ivox, source  # keep alive
         self.max_correspondence_distance = float(max_correspondence_distance)
-        self.h = None
         self._lin_point = None
-        h = C.c_void_p()
-        check(lib().gb_ct_gicp_factor_create(self.ctx.h, ivox.h, source.h, self.max_correspondence_distance, C.byref(h)))
-        self.h = h
+        self.h = self._create(lib().gb_ct_gicp_factor_create, self.ctx.h, ivox.h, source.h, self.max_correspondence_distance)
 
     def keys(self):
         return [self.key_X, self.key_Y]
@@ -465,11 +443,6 @@ class IntegratedCT_GICPFactorGPU:
         check(lib().gb_ct_gicp_error(self.h, ptr(pose16(Xl)), ptr(pose16(Yl)), ptr(pose16(X)), ptr(pose16(Y)), C.byref(e)))
         return e.value
 
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            lib().gb_vgicp_factor_destroy(self.h)
-            self.h = None
-
 
 def _params(p, fill, name, overrides):
     """p as fill (a gb_*_default_params) leaves it, with the given fields replaced; the fields of a nested gb_align_params `lm`
@@ -485,9 +458,14 @@ def _params(p, fill, name, overrides):
     return p
 
 
+def _pose(col16) -> np.ndarray:
+    """a result struct's 16 column-major doubles -> (4,4)"""
+    return np.array(col16[:]).reshape(4, 4).T.copy()
+
+
 def _result(r, *poses) -> dict:
     """a gb_align_result / gb_ct_result as a dict: the named poses (4,4), then the fields the two share"""
-    out = {k: np.array(getattr(r, k)[:]).reshape(4, 4).T.copy() for k in poses}
+    out = {k: _pose(getattr(r, k)) for k in poses}
     out.update({"error": r.error, "num_inliers": r.num_inliers, "lambda": r.lambda_, "iterations": r.iterations, "trials": r.trials,
                 "status": r.status, "status_name": capi.ALIGN_STATUS_NAMES.get(r.status, "?")})
     return out
@@ -528,9 +506,8 @@ def deskew_ct(cloud: PointCloudGPU, X, Y, neighbors, k_neighbors: int, host_outp
     pts = np.empty((n, 4)) if host_outputs else None
     cov = np.empty((n, 16)) if host_outputs else None
     nrm = np.empty((n, 4)) if host_outputs else None
-    h = C.c_void_p()
-    check(lib().gb_ct_deskew(ctx.h, cloud.h, ptr(pose16(np.asarray(X, dtype=np.float64).reshape(4, 4))), ptr(pose16(np.asarray(Y, dtype=np.float64).reshape(4, 4))), ptr(nb),
-                             int(kc), int(k_neighbors), ptr(pts), ptr(cov), ptr(nrm), C.byref(h)))
+    h = PointCloudGPU._create(lib().gb_ct_deskew, ctx.h, cloud.h, ptr(pose16(np.asarray(X, dtype=np.float64).reshape(4, 4))), ptr(pose16(np.asarray(Y, dtype=np.float64).reshape(4, 4))),
+                              ptr(nb), int(kc), int(k_neighbors), ptr(pts), ptr(cov), ptr(nrm))
     out = PointCloudGPU(ctx, h, n)
     if not host_outputs:
         return None, None, None, out
@@ -561,7 +538,7 @@ def estimate_pose_ransac(target: PointCloudGPU, source: PointCloudGPU, ctx: Cont
     r = capi.RansacResult()
     counts = np.empty(p.max_iterations, np.int32) if hypothesis_inliers else None
     check(lib().gb_ransac_align(ctx.h, target.h, source.h, C.byref(p), C.byref(r), ptr(counts)))
-    out = {"T_target_source": np.array(r.T_target_source[:]).reshape(4, 4).T.copy(), "inliers": r.inliers, "inlier_rate": r.inlier_rate,
+    out = {"T_target_source": _pose(r.T_target_source), "inliers": r.inliers, "inlier_rate": r.inlier_rate,
            "best_hypothesis": r.best_hypothesis, "evaluated": r.evaluated, "status": r.status, "status_name": capi.RANSAC_STATUS_NAMES.get(r.status, "?")}
     if counts is not None:
         out["hypothesis_inliers"] = counts
@@ -612,8 +589,10 @@ class NonlinearFactorSetGPU:
         return out
 
 
-class Sweep:
+class Sweep(_Handle):
     """A prepared, device-resident batch (gb_sweep): upload poses / launch / fetch are separate steps."""
+
+    _destroy = "gb_sweep_destroy"
 
     def __init__(self, ctx: Context, factors: list[IntegratedVGICPFactorGPU], pair_index=None):
         self.ctx = ctx
@@ -621,12 +600,10 @@ class Sweep:
         F = len(factors)
         arr = (C.c_void_p * F)(*[f._handle() for f in factors])
         pi = np.ascontiguousarray(pair_index, dtype=np.int32) if pair_index is not None else None
-        h = C.c_void_p()
-        check(lib().gb_sweep_create(ctx.h, F, C.cast(arr, C.c_void_p), ptr(pi), C.byref(h)))
-        self.h = h
+        self.h = self._create(lib().gb_sweep_create, ctx.h, F, C.cast(arr, C.c_void_p), ptr(pi))
         self.F = F
         pf, ab, nt, gs = C.c_uint64(), C.c_uint64(), C.c_uint32(), C.c_uint32()
-        check(lib().gb_sweep_stats(h, C.byref(pf), C.byref(ab), C.byref(nt), C.byref(gs)))
+        check(lib().gb_sweep_stats(self.h, C.byref(pf), C.byref(ab), C.byref(nt), C.byref(gs)))
         self.point_factors, self.algorithmic_bytes, self.num_tiles, self.grid = pf.value, ab.value, nt.value, gs.value
 
     def attach_peer_slab(self, peer_slab: "PeerSlab | None"):
@@ -666,23 +643,18 @@ class Sweep:
         check(lib().gb_sweep_results_device(self.h, C.byref(p)))
         return p.value or 0
 
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            lib().gb_sweep_destroy(self.h)
-            self.h = None
 
-
-class PeerSlab:
+class PeerSlab(_Handle):
     """gb_peer_slab: ping-pong fp32 [num_pairs][96] result buffers shared with the other ranks of the box through CUDA
     IPC; the sweep's epilogue stores finished pair rows straight into every rank's buffer (multi-GPU exchange fused into
     the kernel, SURVEY 8(e)).  `exchange(handle_bytes) -> list[bytes]` must all-gather the 64-byte handles in rank order
     (torch.distributed in the bench); with world == 1 nothing is exchanged."""
 
+    _destroy = "gb_peer_slab_destroy"
+
     def __init__(self, ctx: Context, num_pairs: int, world: int = 1, rank: int = 0, exchange=None):
         self.ctx, self.num_pairs, self.world, self.rank = ctx, num_pairs, world, rank
-        h = C.c_void_p()
-        check(lib().gb_peer_slab_create(ctx.h, num_pairs, world, rank, C.byref(h)))
-        self.h = h
+        self.h = self._create(lib().gb_peer_slab_create, ctx.h, num_pairs, world, rank)
         if world > 1:
             buf = (C.c_ubyte * capi.GB_IPC_HANDLE_BYTES)()
             check(lib().gb_peer_slab_export(self.h, C.cast(buf, C.c_void_p)))
@@ -709,11 +681,6 @@ class PeerSlab:
         p = C.c_void_p()
         check(lib().gb_peer_slab_device_ptr(self.h, C.byref(p)))
         return p.value or 0
-
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            lib().gb_peer_slab_destroy(self.h)
-            self.h = None
 
 
 def align_params(**overrides) -> capi.AlignParams:
@@ -767,8 +734,8 @@ def merge_frames_gpu(poses, frames, downsample_resolution: float, target_num_poi
     pts = np.empty((cap, 4)) if host_outputs else None
     cov = np.empty((cap, 16)) if host_outputs else None
     m = C.c_size_t()
-    h = C.c_void_p()
-    check(lib().gb_merge_frames(ctx.h, K, C.cast(arr, C.c_void_p), ptr(T), float(downsample_resolution), int(target_num_points), int(seed), ptr(pts), ptr(cov), C.byref(m), C.byref(h)))
+    h = PointCloudGPU._create(lib().gb_merge_frames, ctx.h, K, C.cast(arr, C.c_void_p), ptr(T), float(downsample_resolution), int(target_num_points), int(seed), ptr(pts), ptr(cov),
+                              C.byref(m))
     cloud = PointCloudGPU(ctx, h, m.value) if h.value else None
     if not host_outputs:
         return None, None, cloud
@@ -808,7 +775,7 @@ def estimate_pose_gnc(target: PointCloudGPU, source: PointCloudGPU, ctx: Context
     pairs = np.empty((m, 2), np.int32) if correspondences else None
     weights = np.empty(m) if correspondences else None
     check(lib().gb_gnc_align(ctx.h, target.h, source.h, C.byref(p), C.byref(r), ptr(pairs), ptr(weights)))
-    out = {"T_target_source": np.array(r.T_target_source[:]).reshape(4, 4).T.copy(), "inliers": r.inliers, "inlier_rate": r.inlier_rate,
+    out = {"T_target_source": _pose(r.T_target_source), "inliers": r.inliers, "inlier_rate": r.inlier_rate,
            "samples": r.samples, "correspondences": r.correspondences, "iterations": r.iterations, "status": r.status,
            "status_name": capi.GNC_STATUS_NAMES.get(r.status, "?")}
     if correspondences:
