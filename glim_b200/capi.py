@@ -93,6 +93,9 @@ _SIGNATURES = {
     "gb_point_grid_destroy": ([vp], st),
     "gb_gicp_grid_factor_create": ([vp, vp, vp, f64, vp], st),
     "gb_gicp_grid_factor_half_width": ([vp, vp], st),
+    "gb_icp_grid_factor_create": ([vp, vp, vp, f64, vp], st),
+    "gb_cloud_estimate_normals": ([vp, vp], st),
+    "gb_cloud_normals": ([vp, vp], st),
     "gb_cloud_estimate_fpfh": ([vp, vp, f64], st),
     "gb_cloud_fpfh": ([vp, vp], st),
     "gb_fpfh_match": ([vp, vp, vp, vp], st),

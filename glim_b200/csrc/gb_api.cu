@@ -221,7 +221,7 @@ gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes) {
 void cloud_free(gb_cloud* c) {
   gb_dev_free(c->device, c->base);  // waits for every stream that may still read the cloud, then recycles the block
   gb_dev_free(c->device, c->t_base);
-  gb_dev_free(c->device, c->f_base);
+  for (void* b : {c->n_base, c->f_base}) gb_dev_free(c->device, b);  // what gb_cloud_estimate_normals / _fpfh estimated
   delete c;
 }
 
@@ -369,22 +369,44 @@ extern "C" gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, c
   return GB_OK;
 }
 
-extern "C" gb_status gb_gicp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out) {
+// The argument checks of a GICP (icp = false) or ICP factor on a point grid, and the factor's correspondence bound and search
+// half-width.  Only the GICP factor reads the source's covariances.
+static gb_status grid_factor_args(const gb_ctx* ctx, const gb_point_grid* target, const gb_cloud* source, double max_correspondence_distance, bool icp, gb_factor** out,
+                                  float* max_corr2, int* half_width) {
   GB_REQUIRE(ctx && target && source && out, "null argument");
   *out = nullptr;
   GB_REQUIRE(std::isfinite(max_correspondence_distance) && max_correspondence_distance > 0.0, "max_correspondence_distance must be positive and finite");
   const gb_voxelmap* m = grid_map(target);
   GB_REQUIRE(m->kind == GB_MAP_POINTS, "the target is not a point grid (gb_point_grid_build)");
   GB_REQUIRE(m->device == ctx->device && source->device == ctx->device, "cloud / point grid live on another device");
-  GB_REQUIRE(source->covs, "the source carries no covariances");
-  const float max_corr2 = (float)(max_correspondence_distance * max_correspondence_distance);
-  const int half_width = grid_half_width(m->inv_res, max_corr2, m->key_extent);
-  GB_REQUIRE(half_width <= kGridMaxHalfWidth, "max_correspondence_distance / cell_size too large: the search would span more than 17^3 cells");
+  GB_REQUIRE(icp || source->covs, "the source carries no covariances");
+  *max_corr2 = (float)(max_correspondence_distance * max_correspondence_distance);
+  *half_width = grid_half_width(m->inv_res, *max_corr2, m->key_extent);
+  GB_REQUIRE(*half_width <= kGridMaxHalfWidth, "max_correspondence_distance / cell_size too large: the search would span more than 17^3 cells");
+  return GB_OK;
+}
+extern "C" gb_status gb_gicp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out) {
+  float max_corr2 = 0.f;
+  int half_width = 0;
+  GB_CHECK(grid_factor_args(ctx, target, source, max_correspondence_distance, false, out, &max_corr2, &half_width));
   GB_ENTER(ctx);
-  gb_factor* f = factor_new(ctx, GB_FACTOR_POSE, m, source);
+  gb_factor* f = factor_new(ctx, GB_FACTOR_POSE, grid_map(target), source);
   if (!f) return GB_ERR_INTERNAL;
   f->max_corr2 = max_corr2;
   f->grid_m = half_width;
+  *out = f;
+  return GB_OK;
+}
+extern "C" gb_status gb_icp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out) {
+  float max_corr2 = 0.f;
+  int half_width = 0;
+  GB_CHECK(grid_factor_args(ctx, target, source, max_correspondence_distance, true, out, &max_corr2, &half_width));
+  GB_ENTER(ctx);
+  gb_factor* f = factor_new(ctx, GB_FACTOR_POSE, grid_map(target), source);
+  if (!f) return GB_ERR_INTERNAL;
+  f->max_corr2 = max_corr2;
+  f->grid_m = half_width;
+  f->icp = true;
   *out = f;
   return GB_OK;
 }
@@ -577,13 +599,14 @@ void desc_target_gicp(FactorDesc& D, GicpDesc& G, const gb_factor* fa) {
 // The bucket term is charged at the SMALLEST table that could hold the voxels (16384 doubled until >= V), not at
 // our deliberately sparse table (>= 8 V): padding we added for speed must not inflate the achieved-GB/s figure.
 // A GICP factor is charged 48 B per STORED target point in place of the voxel records (its voxels' or cells' buckets the
-// same way).
+// same way); an ICP factor reads one float4 of each: 16 B per source point and per stored target point.
 static uint64_t factor_bytes(const gb_factor* fa) {
   const bool sv = (fa->flags & GB_FACTOR_SURFACE_VALIDATION) != 0;
   const uint64_t V = (uint64_t)fa->target->num_voxels;
   const uint64_t records = gb_target_class(fa->target) != 0 ? (uint64_t)fa->target->num_points : V;
   uint64_t nb_ref = 16384;
   while (nb_ref < V) nb_ref *= 2;
+  if (fa->icp) return ((uint64_t)fa->source->n + records + nb_ref) * 16 + 64 + 488;
   return (uint64_t)fa->source->n * (48 + (sv ? 12 : 0)) + records * 48 + nb_ref * 16 + 64 + 488;  // +12 B / point: the normals, when they are read
 }
 
@@ -651,12 +674,12 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     GB_REQUIRE(factors[f], "null factor");
     GB_REQUIRE(factors[f]->kind != GB_FACTOR_CT, "a CT factor has two poses: only the gb_ct_* entry points take it");
     GB_REQUIRE(factors[f]->source->device == ctx->device && factors[f]->target->device == ctx->device, "factor lives on another device");
-    GB_REQUIRE(gb_target_class(factors[f]->target) == gb_target_class(factors[0]->target),
-               "the factors of one sweep must all be VGICP factors, all GICP factors on iVoxes or all GICP factors on point grids");
+    GB_REQUIRE(gb_factor_class(factors[f]) == gb_factor_class(factors[0]),
+               "the factors of one sweep must all be VGICP factors, all GICP factors on iVoxes, all GICP factors on point grids or all ICP factors");
     total_pts += factors[f]->source->n;
   }
-  const int target_class = F > 0 ? gb_target_class(factors[0]->target) : 0;
-  const bool gicp = target_class != 0;
+  const int factor_class = F > 0 ? gb_factor_class(factors[0]) : 0;
+  const bool gicp = factor_class != 0;
   GB_REQUIRE(!gicp || !pair_index, "GICP sweeps take no pair_index (no slab can be attached to them)");
   GB_ENTER(ctx);
   gb_owned<gb_sweep> s(new (std::nothrow) gb_sweep(), sweep_free);
@@ -664,7 +687,8 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   ctx_retain(ctx);
   s->ctx = ctx; s->F = F; s->factors.assign(factors, factors + F);
   s->gicp = gicp;
-  s->point_grid = target_class == 2;
+  s->point_grid = factor_class >= 2;
+  s->icp = factor_class == 3;
 
   // kernel generation and work-item policy
   // Kernel policy (A/B runs of the kernels, scripts/ab_sweep.py): small sweeps -- about one item per warp: an odometry
@@ -676,7 +700,7 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   const uint64_t warps = (uint64_t)s->capacity * 8;
   const bool small = F > 0 && total_pts <= warps * 2048;
   s->kernel_version = (kv == 3 || kv == 5) ? kv : (small ? 5 : 3);
-  if (gicp) s->kernel_version = 5;  // k_gicp_sweep and k_gicp_grid_sweep run sweep5's strided items at every size
+  if (gicp) s->kernel_version = 5;  // k_gicp_sweep, k_gicp_grid_sweep and k_icp_grid_sweep run sweep5's strided items at every size
   {
     // sweep3's items: ~6 items per warp (first one static, the rest drawn dynamically), between 128 and 2048 points each,
     // in whole rows of 32 points

@@ -162,4 +162,21 @@ GB_CHD double4 plane_covariance(int i, const double4* __restrict__ pts, const in
   return p;
 }
 
+// estimate_normals of one stored point (gb_cloud_estimate_normals, k_cloud_normals; the rule is written once in
+// include/glim_b200.h): the unit eigenvector of the smallest eigenvalue of its fp32 covariance (c00 c01 c02 c11 c12 c22) widened
+// to fp64, turned away from p when (px nx + py ny) + pz nz > 0, stored as fp32 in n.  Zero for a point whose position or
+// covariance is not finite.
+GB_CHD void covariance_normal(float px, float py, float pz, float c00, float c01, float c02, float c11, float c12, float c22, float (&n)[3]) {
+  const double p[3] = {px, py, pz};
+  const double A[9] = {c00, c01, c02, c01, c11, c12, c02, c12, c22};
+  bool finite = isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]);
+  for (int k = 0; k < 9; k++) finite = finite && isfinite(A[k]);
+  if (!finite) { n[0] = n[1] = n[2] = 0.f; return; }
+  double evals[3], V[9];
+  eigen_sym3_direct(A, evals, V);
+  double v[3] = {V[0], V[3], V[6]};
+  if (dot3(p, v) > 0.0) { v[0] = -v[0]; v[1] = -v[1]; v[2] = -v[2]; }
+  n[0] = (float)v[0]; n[1] = (float)v[1]; n[2] = (float)v[2];
+}
+
 }  // namespace

@@ -1,4 +1,5 @@
-// gb_grid_math.cuh -- the correspondence search of the GICP sweep on a device point grid (k_gicp_grid_sweep, gb_kernels_gicp.cu),
+// gb_grid_math.cuh -- the correspondence search of the GICP and ICP sweeps on a device point grid (k_gicp_grid_sweep,
+// k_icp_grid_sweep, gb_kernels_gicp.cu),
 // kept free of anything that only exists on the device so that the SAME TEXT also compiles for the host:
 // tests/cpp/grid_search_host.cpp builds it with g++ and tests/test_grid_host.py checks it against the numpy restatement of the
 // rule (tests/grid_oracle.py) on the CPU-only box.  The rule is written once, in include/glim_b200.h (gb_point_grid_build,

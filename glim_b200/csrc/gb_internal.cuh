@@ -51,7 +51,8 @@ struct gb_cloud {
   float4* p0 = nullptr;
   float4* p1 = nullptr;
   float* p2 = nullptr;
-  float4* normals = nullptr;  // {nx, ny, nz, 0} or nullptr
+  float4* normals = nullptr;  // {nx, ny, nz, 0} or nullptr: in `base` when uploaded with the cloud, else in `n_base`
+  void* n_base = nullptr;     // the normals of gb_cloud_estimate_normals on a cloud built without them: a pool block of their own
   // Points are stored in Morton order of their 1/16 m cell (gather locality of the sweep kernel: lanes of a warp
   // then hit the same few voxels).  perm[j] = original index of stored point j, inv_perm = its inverse; nullptr = identity.
   int* perm = nullptr;
@@ -169,7 +170,8 @@ struct gb_factor {
   gb_ctx* ctx = nullptr;
   const gb_voxelmap* target = nullptr;  // a built or incremental map (VGICP), an iVox or a point grid (GICP)
   float max_corr2 = 0.f;                // GICP: (float)(max_correspondence_distance^2)
-  int grid_m = 0;                       // GICP on a point grid: the search half-width m (grid_half_width)
+  int grid_m = 0;                       // GICP or ICP on a point grid: the search half-width m (grid_half_width)
+  bool icp = false;                     // a point-to-point ICP factor on a point grid (gb_icp_grid_factor_create)
   const gb_cloud* source = nullptr;
   int flags = 0;
   gb_sweep* single = nullptr;  // lazily created 1-factor sweep
@@ -177,6 +179,8 @@ struct gb_factor {
   uint64_t id = 0;             // process-wide unique
   std::vector<gb_sweep*> users;  // sweeps (of any context) that reference this factor; guarded by the registry mutex
 };
+// The class of a pose factor: a sweep or call holds one.  gb_target_class's 0 (VGICP), 1 and 2 (GICP), or 3: ICP on point grids.
+inline int gb_factor_class(const gb_factor* f) { return f->icp ? 3 : gb_target_class(f->target); }
 
 #define GB_MAX_PEERS 8
 // device-resident parameter block of the fused result exchange (one per step parity)
@@ -260,7 +264,8 @@ struct gb_sweep {
   // GICP sweeps (every factor on an iVox, or every factor on a point grid; a sweep holds one target class): k_gicp_sweep or
   // k_gicp_grid_sweep over sweep5's strided items, with the GICP half of each descriptor next to the FactorDesc table
   bool gicp = false;
-  bool point_grid = false;          // a GICP sweep over point grids
+  bool point_grid = false;          // a GICP or ICP sweep over point grids
+  bool icp = false;                 // an ICP sweep (k_icp_grid_sweep; every factor from gb_icp_grid_factor_create)
   GicpDesc* d_gdescs = nullptr;
   GicpDesc* h_gdescs = nullptr;
 };

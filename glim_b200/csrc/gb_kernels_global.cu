@@ -4,6 +4,8 @@
 // without an initial guess.  The rules are written once in include/glim_b200.h; the per-pair and per-hypothesis arithmetic is
 // gb_global_math.cuh, which the host test build compiles as well.
 //
+//   gb_cloud_estimate_normals  k_cloud_normals: one launch, each point's normal from its own covariance (covariance_normal,
+//                           gb_cov_math.cuh, which the host test build compiles as well), into the normals plane.
 //   gb_cloud_estimate_fpfh  a point grid of the cloud (gb_point_grid_build, cell 1.05 r), then k_fpfh_spfh (every point's SPFH,
 //                           fp64, in scratch) and k_fpfh_final (the weighted sum of the neighbours' SPFH plus the own, stored
 //                           fp32): the grid build's launches + 2.  Neighbour lists are never stored.
@@ -30,6 +32,7 @@
 
 namespace {
 
+constexpr int kNormalThreads = 256;
 constexpr int kFpfhThreads = 128;
 constexpr int kMatchThreads = 128;
 constexpr int kMatchTile = 128;     // target features per shared-memory tile
@@ -52,6 +55,17 @@ struct FpfhGrid {
 };
 
 __device__ __forceinline__ void load3(const float4 p, double* x) { x[0] = p.x; x[1] = p.y; x[2] = p.z; }
+
+// one thread per stored point: its normal from its own covariance (covariance_normal), into the normals plane in stored order
+__global__ void __launch_bounds__(kNormalThreads) k_cloud_normals(int n, const float4* __restrict__ p0, const float4* __restrict__ p1, const float* __restrict__ p2,
+                                                                  float4* __restrict__ normals) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const float4 a = p0[j], b = p1[j];
+  float v[3];
+  covariance_normal(a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w, p2[j], v);
+  normals[j] = make_float4(v[0], v[1], v[2], 0.f);
+}
 
 // one thread per grid record: the SPFH of the record's point, cnt_b * (100 / K) for the K neighbours, into spfh (caller order)
 __global__ void __launch_bounds__(kFpfhThreads) k_fpfh_spfh(int n, FpfhGrid G, const float4* __restrict__ normals, const int* __restrict__ inv_perm,
@@ -358,6 +372,47 @@ gb_status match_args(gb_ctx* ctx, const gb_cloud* target, const gb_cloud* source
 // ---------------------------------------------------------------------------------------------
 // entry points
 // ---------------------------------------------------------------------------------------------
+extern "C" gb_status gb_cloud_estimate_normals(gb_ctx* ctx, gb_cloud* cloud) {
+  GB_REQUIRE(ctx && cloud, "null argument");
+  GB_REQUIRE(cloud->device == ctx->device, "the cloud lives on another device");
+  GB_REQUIRE(cloud->covs, "normals are estimated from covariances: the cloud carries none");
+  GB_ENTER(ctx);
+  {  // the features were computed from the old normals: their block goes back to the pool here
+    gb_dev_block old(ctx->device);
+    old.hand_over(cloud->f_base);
+    cloud->fpfh = nullptr;
+  }
+  const size_t n = cloud->n;
+  if (n == 0) return GB_OK;
+  gb_dev_block block(ctx->device);  // a cloud built without normals: a block of their own, handed over on success
+  float4* normals = cloud->normals;
+  if (!normals) GB_CHECK(gb_dev_carve(ctx, block, [&](Carver& cv) { normals = cv.take<float4>(n); }));
+  GB_CHECK(gb_launch(ctx, "k_cloud_normals", k_cloud_normals, (int)((n + kNormalThreads - 1) / kNormalThreads), kNormalThreads, 0, (int)n, cloud->p0, cloud->p1,
+                     cloud->p2, normals));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (!cloud->normals) {
+    block.hand_over(cloud->n_base);
+    cloud->normals = normals;
+  }
+  return GB_OK;
+}
+
+extern "C" gb_status gb_cloud_normals(const gb_cloud* cloud, float* out) {
+  GB_REQUIRE(cloud && out, "null argument");
+  if (cloud->n == 0) return GB_OK;
+  GB_REQUIRE(cloud->normals, "the cloud has no normals (gb_cloud_estimate_normals)");
+  std::vector<float4> h(cloud->n);
+  std::vector<int> perm;
+  // every producer returned after its stream had drained: plain synchronous copies are safe
+  GB_CUDA(cudaMemcpy(h.data(), cloud->normals, sizeof(float4) * cloud->n, cudaMemcpyDefault));
+  if (cloud->perm) { perm.resize(cloud->n); GB_CUDA(cudaMemcpy(perm.data(), cloud->perm, sizeof(int) * cloud->n, cudaMemcpyDefault)); }
+  for (size_t j = 0; j < cloud->n; j++) {
+    float* o = out + 3 * (cloud->perm ? (size_t)perm[j] : j);  // stored slot j holds the caller's point perm[j]
+    o[0] = h[j].x; o[1] = h[j].y; o[2] = h[j].z;
+  }
+  return GB_OK;
+}
+
 extern "C" gb_status gb_cloud_estimate_fpfh(gb_ctx* ctx, gb_cloud* cloud, double search_radius) {
   GB_REQUIRE(ctx && cloud, "null argument");
   GB_REQUIRE(std::isfinite(search_radius) && search_radius > 0.0, "search_radius must be positive and finite");

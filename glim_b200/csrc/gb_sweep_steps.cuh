@@ -227,6 +227,17 @@ __device__ __forceinline__ void accumulate_queue(float (&acc)[32], const FactorD
   }
 }
 
+// phase B of an ICP sweep (k_icp_grid_sweep): as accumulate_queue, but a hit reads only the source point's first plane and the
+// target record's first float4 (16 + 16 B instead of 36 + 48 B).
+template <int MODE>
+__device__ __forceinline__ void accumulate_icp_queue(float (&acc)[32], const FactorDesc& D, const PoseF& Pe, const uint2* __restrict__ q, int nq, int lane) {
+#pragma unroll 2
+  for (int k = lane; k < nq; k += 32) {
+    const uint2 e = q[k];
+    accumulate_icp_hit<MODE>(acc, Pe, __ldg(&D.p0[e.x]), __ldg(&D.voxels[3 * (size_t)e.y]));
+  }
+}
+
 // An item's sums into its factor's accumulator copy (item mod acc_slots): all 29 (linearize) or the error and the inlier
 // count (error).
 template <int MODE>

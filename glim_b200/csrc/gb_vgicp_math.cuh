@@ -162,6 +162,36 @@ GB_HD void accumulate_hit(float (&acc)[32], const PoseF& Pe, const float4 a0, co
   }
 }
 
+// One inlier of a point-to-point ICP factor (k_icp_grid_sweep): accumulate_hit with M = I, reading only the source point
+// a0 = {x y z .} and the target point v0 = {x y z .}.  r = p - q, error += r^T r; G = hat(q), so H_rr = hat(q) hat(q)^T,
+// H_rt = hat(q), H_tt = I and b_t = [q x r ; r].  The correspondence search (grid_nearest) only returns points with a finite
+// d2 < max_d2, so r is finite here.
+template <int MODE>
+GB_HD void accumulate_icp_hit(float (&acc)[32], const PoseF& Pe, const float4 a0, const float4 v0) {
+  float qx, qy, qz;
+  transform(Pe, a0.x, a0.y, a0.z, qx, qy, qz);
+  const float rx = v0.x - qx, ry = v0.y - qy, rz = v0.z - qz;
+  acc[27] += rx * rx + ry * ry + rz * rz;
+  acc[28] += 1.0f;
+  if (MODE == GB_MODE_LINEARIZE_VALUE) {
+    // the upper triangle of H_tt in accumulate_hit's order; the entries that are zero for M = I are left out
+    acc[0] += qy * qy + qz * qz;
+    acc[1] -= qx * qy;
+    acc[2] -= qx * qz;
+    acc[4] -= qz; acc[5] += qy;
+    acc[6] += qz * qz + qx * qx;
+    acc[7] -= qy * qz;
+    acc[8] += qz; acc[10] -= qx;
+    acc[11] += qx * qx + qy * qy;
+    acc[12] -= qy; acc[13] += qx;
+    acc[15] += 1.0f; acc[18] += 1.0f; acc[20] += 1.0f;
+    acc[21] += qy * rz - qz * ry;
+    acc[22] += qz * rx - qx * rz;
+    acc[23] += qx * ry - qy * rx;
+    acc[24] += rx; acc[25] += ry; acc[26] += rz;
+  }
+}
+
 // Surface validation (set_enable_surface_validation(true), odometry_estimation_gpu.cpp:145, :162).  The reference rule lives
 // in the un-vendored gtsam_points and is not recoverable here (SURVEY A.6): ours is an ORIENTATION-CONSISTENCY gate that needs
 // no eigen-decomposition.  With n = R n_A (source normal, flipped towards the sensor by the covariance estimator, rotated into

@@ -14,12 +14,14 @@ include/glim_b200/gtsam_points_compat.hpp.
     PointGridGPU(cloud, cell_size)                          the target frame's KdTree (global_mapping_pose_graph.cpp:273)
     IntegratedGICPFactorGPU(target, source_key, grid, source, max_corr)   IntegratedGICPFactor between frames: sub_mapping.cpp:189-211,
                                                             global_mapping.cpp:379-428, global_mapping_pose_graph.cpp:391-405
+    IntegratedICPFactorGPU(target, source_key, grid, source, max_corr)   IntegratedICPFactor, manual_loop_close_modal.cpp:479-492
     align_vgicp(problems, T_init, params)                   the LM loop of odometry_estimation_cpu.cpp:105-150 /
                                                             global_mapping_pose_graph.cpp:405-417, many problems per call
     PointCloudGPU.add_times(times)                          PointCloud::add_times, odometry_estimation_ct.cpp:101
     IntegratedCT_GICPFactorGPU(key_X, key_Y, ivox, source, max_corr)   odometry_estimation_ct.cpp:159-163
     align_ct_gicp(factors, X_init, Y_init, X_prior, params) the CT LM solve with its motion priors, odometry_estimation_ct.cpp:166-182
     deskew_ct(cloud, X, Y, neighbors, k_neighbors)          deskewed_source_points + covariances, odometry_estimation_ct.cpp:199-204
+    PointCloudGPU.estimate_normals() / .normals()           gtsam_points::estimate_normals, manual_loop_close_modal.cpp:391, :410
     PointCloudGPU.estimate_fpfh(radius) / .fpfh()           gtsam_points::estimate_fpfh, manual_loop_close_modal.cpp:382-397, :415
     fpfh_match(target, source)                              the target's KdTreeX over FPFH features, manual_loop_close_modal.cpp:402
     estimate_pose_ransac(target, source, **params)          gtsam_points::estimate_pose_ransac, manual_loop_close_modal.cpp:435-443
@@ -144,6 +146,19 @@ class PointCloudGPU(_Handle):
         t0, t1 = C.c_double(), C.c_double()
         check(lib().gb_cloud_time_table(self.h, None, ptr(starts), ptr(tau), C.byref(t0), C.byref(t1)))
         return (starts if B.value else np.zeros(0, np.int32)), tau, t0.value, t1.value
+
+    def estimate_normals(self):
+        """gtsam_points::estimate_normals(points, covs, n) (manual_loop_close_modal.cpp:391, :410): every point's normal from its
+        own covariance, sign-ruled away from the origin, into the cloud's normals (gb_cloud_estimate_normals); the cloud must
+        carry covariances.  Discards FPFH features computed earlier."""
+        check(lib().gb_cloud_estimate_normals(self.ctx.h, self.h))
+        return self
+
+    def normals(self) -> np.ndarray:
+        """-> (n, 3) float32 normals in the original point order"""
+        out = np.empty((self.n, 3), np.float32)
+        check(lib().gb_cloud_normals(self.h, ptr(out)))
+        return out
 
     def estimate_fpfh(self, radius: float):
         """gtsam_points::estimate_fpfh with search_radius = radius (manual_loop_close_modal.cpp:382-397): the cloud's FPFH features,
@@ -401,6 +416,21 @@ class IntegratedGICPFactorGPU(IntegratedVGICPFactorGPU):
         m = C.c_int()
         check(lib().gb_gicp_grid_factor_half_width(self._handle(), C.byref(m)))
         return m.value
+
+
+class IntegratedICPFactorGPU(IntegratedGICPFactorGPU):
+    """IntegratedICPFactor(target, source_key, target_frame, source_frame) + set_max_correspondence_distance
+    (manual_loop_close_modal.cpp:479-492, the fine registration of clouds without covariances) with the target's KdTree a
+    PointGridGPU: point-to-point residuals on the grid factor's correspondences, no covariances needed.  NonlinearFactorSetGPU,
+    Sweep and align_vgicp take it (ICP factors only per set, sweep or call)."""
+
+    def __init__(self, target, source_key, grid: PointGridGPU, source: PointCloudGPU, max_correspondence_distance: float, ctx: Context | None = None):
+        super().__init__(target, source_key, grid, source, max_correspondence_distance, ctx=ctx)
+
+    def _handle(self):
+        if self.h is None:
+            self.h = self._create(lib().gb_icp_grid_factor_create, self.ctx.h, self.ivox.h, self.source.h, self.max_correspondence_distance)
+        return self.h
 
 
 class IntegratedCT_GICPFactorGPU(_Handle):

@@ -238,7 +238,8 @@ GB_API gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, const
  *      point by a bounded cell search.
  *
  *      The point grid.  gb_point_grid_build copies every point of a device cloud (position and covariance) into a map of its
- *      own kind.  Each point with finite x, y, z is keyed with the fp32 lookup rule k = floor((float)(p * (float)(1 / cell_size)))
+ *      own kind; a cloud without covariances is accepted, and its records then hold zero covariances (the ICP factor below
+ *      reads positions only).  Each point with finite x, y, z is keyed with the fp32 lookup rule k = floor((float)(p * (float)(1 / cell_size)))
  *      per axis (as every sweep keys its queries); points that are not finite, or whose key is outside the 21-bit range
  *      (+-2^20 cells), are stored but never match.  Cells are in ascending packed-key order, and the points of a cell in
  *      ascending original index (the cloud's caller order); a cell is {first point, count}.  Records have the iVox's layout
@@ -260,7 +261,8 @@ GB_API gb_status gb_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target, const
  *
  *      A grid factor is an ordinary pose gb_factor: gb_vgicp_linearize / _error / _factor_destroy, gb_factor_set_*, gb_sweep_*
  *      and gb_vgicp_align take it.  A sweep or call holds one target class -- voxel maps, iVoxes or point grids -- and a mix is
- *      GB_ERR_INVALID_ARGUMENT before any launch; grid sweeps take no pair_index, slab or peer slab.  gb_sweep_stats of a grid
+ *      GB_ERR_INVALID_ARGUMENT before any launch (ICP factors, gb_icp_grid_factor_create, are a class of their own); grid sweeps
+ *      take no pair_index, slab or peer slab.  gb_sweep_stats of a grid
  *      sweep: 48 B per source point, 48 B per stored target point, 16 B per bucket of the smallest power-of-two table >= 16384
  *      holding the cells, plus pose and record.
  *      A grid is not a voxel map and not an iVox: gb_vgicp_factor_create, gb_gicp_factor_create, gb_ct_gicp_factor_create,
@@ -279,6 +281,28 @@ GB_API gb_status gb_point_grid_destroy(gb_point_grid* grid);
 GB_API gb_status gb_gicp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* target, const gb_cloud* source, double max_correspondence_distance, gb_factor** out);
 /* the factor's search half-width m (0 for a factor of another kind) */
 GB_API gb_status gb_gicp_grid_factor_half_width(const gb_factor* factor, int* m);
+
+/* ---- IntegratedICPFactor(target_key, source_key, target, source) + set_max_correspondence_distance
+ *      (manual_loop_close_modal.cpp:485-487), the target's KdTree being a point grid: the modal's fine registration of clouds
+ *      without covariances (GICP falls back to it, with 200 LM iterations instead of 20, :479-492).  Neither cloud needs
+ *      covariances: gb_point_grid_build takes a cloud without them (its records then hold zero covariances).
+ *
+ *      The rule.  The correspondence is exactly gb_gicp_grid_factor_create's: the same search half-width m (the same refusal
+ *      above m = 8) and the same brute-force argmin of the fp32 d2 < (float)(r^2), ties to the smaller original index.  Per
+ *      matched point the residual is the GICP grid factor's r = p - q with M = I: error = sum r^T r (no 1/2), and H and b are
+ *      that factor's blocks with M = I.  error() takes its correspondences at T_lin and evaluates at T_eval.  [EXT] the
+ *      un-vendored IntegratedICPFactor's error convention is this library's statement of it.
+ *
+ *      An ICP factor is an ordinary pose gb_factor: gb_vgicp_linearize / _error / _factor_destroy, gb_factor_set_*,
+ *      gb_sweep_*, gb_vgicp_align and gb_gicp_grid_factor_half_width take it.  A sweep or call holds ICP factors only or none:
+ *      a mix with VGICP or GICP factors of any target class is GB_ERR_INVALID_ARGUMENT before any launch.  ICP sweeps take no
+ *      pair_index, slab or peer slab, and the gb_ct_* entry points refuse the factor.  gb_sweep_stats of an ICP sweep: 16 B per
+ *      source point, 16 B per stored target point, 16 B per bucket of the smallest power-of-two table >= 16384 holding the
+ *      cells, plus pose and record. ---- */
+/* GB_ERR_INVALID_ARGUMENT before any launch, creating nothing, for a non-finite or non-positive max_correspondence_distance, a
+ * target that is not a point grid, a grid or source on another device than ctx, or a search half-width m above 8. */
+GB_API gb_status gb_icp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* target, const gb_cloud* source, double max_correspondence_distance,
+                                           gb_factor** out);
 
 /* ---- Global registration: T_target_source between two clouds with no initial guess, as GLIM's manual loop closure runs it
  *      (ManualLoopCloseModal::align_global, src/glim/viewer/interactive/manual_loop_close_modal.cpp:370-468): FPFH features of
@@ -322,6 +346,27 @@ GB_API gb_status gb_gicp_grid_factor_half_width(const gb_factor* factor, int* m)
  *      Launches: gb_cloud_estimate_fpfh, the point grid build's (gb_point_grid_build) + 2; gb_fpfh_match, 1 (0 for an empty
  *      source); gb_ransac_align, 1 (the match) + the target grid's build + 2 per wave, with one copy of the wave's counts and one
  *      stream synchronisation per wave. ---- */
+/* ---- gtsam_points::estimate_normals(points, covs, n) (manual_loop_close_modal.cpp:391,410; map_editor.cpp:186): the normals of a
+ *      cloud that has covariances but no normals (a merged submap, gb_merge_frames), before FPFH.
+ *
+ *      The rule.  Per point, from the stored fp32 position p and fp32 covariance (6 entries), both widened to fp64: n = the unit
+ *      eigenvector of the smallest eigenvalue as eigen_sym3_direct computes it (the solver of the covariance estimation, so n
+ *      agrees with gb_preprocess's normal on the same covariance); if (px nx + py ny) + pz nz > 0 (fp64, uncontracted) then
+ *      n = -n (cloud_covariance_estimation.cpp:98-100); n is stored once as fp32.  A point whose position or covariance is not
+ *      finite gets (0, 0, 0).  A finite covariance that is exactly zero or has a repeated smallest eigenvalue gets what the
+ *      solver returns (for zero: the axis (1, 0, 0), sign-ruled).  [EXT] gtsam_points is not vendored: this is this library's
+ *      statement of estimate_normals.
+ *
+ *      The normals go into the cloud's normals plane, in its stored order, so every consumer of normals reads them unchanged
+ *      (gb_cloud_estimate_fpfh, GB_FACTOR_SURFACE_VALIDATION, gb_cloud_device_ptrs).  A cloud uploaded with normals has them
+ *      overwritten in place; a cloud without gets a block of its own, which gb_cloud_destroy releases.  FPFH features computed
+ *      earlier are discarded (gb_cloud_fpfh and the matchers refuse the cloud until they are estimated again).
+ *      GB_ERR_INVALID_ARGUMENT before any launch for a cloud without covariances or on another device than ctx.  An empty
+ *      cloud makes no launch; any other makes one launch and one stream synchronisation.  Threading as for gb_cloud_add_times:
+ *      do not call it while another thread uses the cloud. ---- */
+GB_API gb_status gb_cloud_estimate_normals(gb_ctx* ctx, gb_cloud* cloud);
+/* host copy of the normals, N x 3 in the caller's point order; GB_ERR_INVALID_ARGUMENT for a non-empty cloud without normals */
+GB_API gb_status gb_cloud_normals(const gb_cloud* cloud, float* out);
 /* The FPFH features of `cloud` with search radius r, kept on the device with the cloud (cloud_destroy releases them); a second
  * call replaces them.  GB_ERR_INVALID_ARGUMENT before any launch for a cloud without normals, a non-finite or non-positive r,
  * or a cloud on another device than ctx. */
@@ -407,7 +452,7 @@ GB_API gb_status gb_factor_set_error(gb_ctx* ctx, size_t num_factors, gb_factor*
  *      A problem is the set of factors (levels) that share one unknown T_target_source, the target pose fixed to identity;
  *      the factors of problem p are factors[factor_offsets[p] .. factor_offsets[p+1]).  Factors keep their flags.  The factors
  *      may be VGICP (gb_vgicp_factor_create), GICP on iVoxes (gb_gicp_factor_create) or GICP on point grids
- *      (gb_gicp_grid_factor_create) factors, all of one target class per call.
+ *      (gb_gicp_grid_factor_create) factors, or ICP factors on point grids (gb_icp_grid_factor_create), all of one class per call.
  *
  *      The rule (gtsam_points' LevenbergMarquardtOptimizerExt is not vendored: GTSAM's documented LM defaults plus GLIM's
  *      termination callback, DESIGN.md section 7 [EXT]).  Per problem, T = T_init, lambda = lambda_initial, need_lin = 1;

@@ -9,6 +9,11 @@ of yaw and 18 m away:
   gnc       gb_gnc_align (reciprocal matches of 10000 samples, the Geman-McClure schedule, the score);
   e2e       both maps' features, RANSAC and the fine registration (LM on a grid GICP factor, r = 1.0), from device clouds;
   gnc_e2e   the same with GNC as the global method;
+  normals   gb_cloud_estimate_normals of one merged submap (gb_merge_frames of the map: covariances, no normals);
+  icp       one linearization of a point-to-point ICP factor on a point grid (r = 1.0) between the two maps uploaded without
+            covariances, and the modal's 200-iteration align (GTSAM's LM defaults, no step tests) from 0.1 m / 0.01 rad off;
+  submap_e2e  the right-click recipe from two merged device submaps: normals, features, RANSAC and the fine registration
+            (20 iterations);
   host      the numpy restatement of the match (tests/global_oracle.py) on 2 k x 2 k of the same features; the restatement of
             the FPFH and of RANSAC takes minutes at these sizes and is not run.
 
@@ -122,6 +127,38 @@ def main():
             et, er = error(fine["r"]["T_target_source"])
             out[key + "_err_m"] = round(et, 4)
             out[key + "_err_deg"] = round(er, 4)
+        def merged(p, c):
+            return gpu.merge_frames_gpu([np.eye(4)], [gpu.PointCloudGPU.clone(p, c, ctx=ctx)], 0.01, ctx=ctx, host_outputs=False)[2]
+
+        ta = merged(tp, tc)
+        out["normals_ms"] = timed(ta.estimate_normals, args.repeats)
+        out["normals_points"] = ta.n
+        ti, si = gpu.PointCloudGPU.clone(tp, ctx=ctx), gpu.PointCloudGPU.clone(sp, ctx=ctx)
+        fi = gpu.IntegratedICPFactorGPU(np.eye(4), 0, gpu.PointGridGPU(ti, 1.05, ctx=ctx), si, 1.0, ctx=ctx)
+        out["icp_linearize_ms"] = timed(lambda: fi.linearize({0: T_gt}), args.repeats)
+        T0 = synth.perturb(T_gt, np.random.default_rng(3), 0.01, 0.1)
+        modal = {"max_iterations": 200, "lambda_initial": 1e-5, "lambda_factor": 10.0, "lambda_upper_bound": 1e5, "relative_error_tol": 1e-5,
+                 "absolute_error_tol": 1e-5, "step_translation_tol": 0.0, "step_rotation_tol": 0.0}
+        icp = {}
+
+        def icp_align():
+            icp["r"] = gpu.align_vgicp([[fi]], [T0], params=modal)[0]
+
+        out["icp_align_ms"] = timed(icp_align, args.repeats)
+        et, er = error(icp["r"]["T_target_source"])
+        out["icp_align_result"] = {"status": icp["r"]["status_name"], "iterations": icp["r"]["iterations"], "err_m": round(et, 4), "err_deg": round(er, 4)}
+
+        def submap_e2e():
+            a = merged(tp, tc).estimate_normals().estimate_fpfh(5.0)
+            b = merged(sp, sc).estimate_normals().estimate_fpfh(5.0)
+            r = gpu.estimate_pose_ransac(a, b)
+            f = gpu.IntegratedGICPFactorGPU(np.eye(4), 0, gpu.PointGridGPU(a, 1.05, ctx=ctx), b, 1.0, ctx=ctx)
+            fine["r"] = gpu.align_vgicp([[f]], [r["T_target_source"]], params=dict(modal, max_iterations=20))[0]
+
+        out["submap_e2e_ms"] = timed(submap_e2e, args.repeats)
+        et, er = error(fine["r"]["T_target_source"])
+        out["submap_e2e_err_m"] = round(et, 4)
+        out["submap_e2e_err_deg"] = round(er, 4)
         ft, fs = tgt.fpfh()[:2000], src.fpfh()[:2000]
         t0 = time.perf_counter()
         gl.match(ft, fs)
