@@ -103,6 +103,9 @@ _SIGNATURES = {
     "gb_ransac_align": ([vp, vp, vp, vp, vp, vp], st),
     "gb_gnc_default_params": ([vp], st),
     "gb_gnc_align": ([vp, vp, vp, vp, vp, vp, vp], st),
+    "gb_concat_frames": ([vp, sz, vp, vp, vp, vp, vp, vp], st),
+    "gb_region_growing_default_params": ([vp], st),
+    "gb_region_growing": ([vp, vp, vp, vp, vp, vp, vp], st),
 }
 del vp, i32, f32, f64, sz, u64, st
 SYMBOLS = tuple(_SIGNATURES)  # tests check the library exports exactly these
@@ -174,6 +177,25 @@ class GncResult(C.Structure):
     _fields_ = [("T_target_source", C.c_double * 16), ("inlier_rate", C.c_double), ("inliers", C.c_int), ("samples", C.c_int), ("correspondences", C.c_int),
                 ("iterations", C.c_int), ("status", C.c_int)]
 
+
+class CellWindow(C.Structure):
+    """gb_cell_window (include/glim_b200.h)."""
+    _fields_ = [("cell_size", C.c_double), ("lo", C.c_int32 * 3), ("hi", C.c_int32 * 3)]
+
+
+class RegionGrowingParams(C.Structure):
+    """gb_region_growing_params (include/glim_b200.h)."""
+    _fields_ = [("distance_threshold", C.c_double), ("angle_threshold", C.c_double), ("dilation_radius", C.c_double)]
+
+
+class RegionGrowingResult(C.Structure):
+    """gb_region_growing_result (include/glim_b200.h)."""
+    _fields_ = [("seed", C.c_int32), ("status", C.c_int32), ("num_region", C.c_size_t), ("num_selected", C.c_size_t), ("num_components", C.c_size_t)]
+
+
+# gb_region_growing_result::status
+REGION_FOUND, REGION_NO_SEED = 0, 1
+REGION_STATUS_NAMES = {0: "FOUND", 1: "NO_SEED"}
 
 # gb_ransac_result::status
 RANSAC_FOUND, RANSAC_EARLY_STOP, RANSAC_DEGENERATE = 0, 1, 2

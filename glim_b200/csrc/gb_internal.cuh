@@ -507,6 +507,10 @@ gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_de
 // of device scratch for the frame descriptor.  One launch.
 #define GB_FRAME_DESC_BYTES 256
 gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T_colmajor, void* d_frame, double4* pts, double* cov6);
+// The same for K frames at poses (K x 16, column-major) in one launch, frame-major and each frame in its original point order:
+// h_frames (pinned) and d_frames hold K x GB_FRAME_DESC_BYTES for the descriptor table.  Shared by gb_merge_frames and
+// gb_concat_frames (gb_kernels_segment.cu).  No launch when the frames hold no point.
+gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, void* h_frames, void* d_frames, double4* pts, double* cov6);
 // k_grid_keys of the voxel-grid paths: key = packed floor(p * inv_res) in fp64 (~0 for non-finite / out-of-range points,
 // and for every point with keep[i] == 0 when keep is given), idx[i] = i.  One launch.
 gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, const int* keep, unsigned long long* keys, int* idx);

@@ -821,14 +821,23 @@ gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T, vo
   return gb_launch(ctx, "k_merge_transform", k_merge_transform, (n + 255) / 256, 256, 0, 1, (const MergeFrame*)d_frame, n, pts, cov6);
 }
 
+gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, void* h_frames, void* d_frames, double4* pts, double* cov6) {
+  MergeFrame* h = (MergeFrame*)h_frames;
+  size_t total = 0;
+  for (size_t k = 0; k < K; k++) {
+    h[k] = merge_frame(frames[k], poses + k * 16, (int)total);
+    total += frames[k]->n;
+  }
+  if (total == 0) return GB_OK;
+  GB_CUDA(cudaMemcpyAsync(d_frames, h, sizeof(MergeFrame) * K, cudaMemcpyHostToDevice, ctx->stream));
+  const int n = (int)total;
+  return gb_launch(ctx, "k_merge_transform", k_merge_transform, (n + 255) / 256, 256, 0, (int)K, (const MergeFrame*)d_frames, n, pts, cov6);
+}
+
 static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out) {
   cudaStream_t st = ctx->stream;
   size_t total = 0;
-  std::vector<MergeFrame> mf((size_t)K);
-  for (int k = 0; k < K; k++) {
-    mf[(size_t)k] = merge_frame(frames[k], poses + (size_t)k * 16, (int)total);
-    total += frames[k]->n;
-  }
+  for (int k = 0; k < K; k++) total += frames[k]->n;
   *num_out = 0;
   if (total == 0) return GB_OK;
   const int n = (int)total;
@@ -856,11 +865,9 @@ static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames,
   }));
   MergeFrame* h_mf = nullptr;
   GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h_mf = cv.take<MergeFrame>((size_t)K); }));
-  memcpy(h_mf, mf.data(), sizeof(MergeFrame) * (size_t)K);
-  GB_CUDA(cudaMemcpyAsync(d_mf, h_mf, sizeof(MergeFrame) * (size_t)K, cudaMemcpyHostToDevice, st));
   GB_CUDA(cudaMemsetAsync(d_cnt, 0, 256, st));
   const int tb = 256, gb = (n + tb - 1) / tb;
-  GB_CHECK(gb_launch(ctx, "k_merge_transform", k_merge_transform, gb, tb, 0, K, d_mf, n, d_pts, d_cov));
+  GB_CHECK(gb_transform_frames(ctx, (size_t)K, frames, poses, h_mf, d_mf, d_pts, d_cov));
   GB_CHECK(gb_grid_keys(ctx, n, d_pts, 1.0 / resolution, nullptr, t.keys, t.idx));
   GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
   GB_CHECK(gb_launch(ctx, "k_copy_last_pos", k_copy_last_pos, 1, 1, 0, n, d_pos, d_cnt));  // V

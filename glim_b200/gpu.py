@@ -26,6 +26,9 @@ include/glim_b200/gtsam_points_compat.hpp.
     fpfh_match(target, source)                              the target's KdTreeX over FPFH features, manual_loop_close_modal.cpp:402
     estimate_pose_ransac(target, source, **params)          gtsam_points::estimate_pose_ransac, manual_loop_close_modal.cpp:435-443
     estimate_pose_gnc(target, source, **params)             gtsam_points::estimate_pose_gnc, manual_loop_close_modal.cpp:446-458
+    concat_frames(poses, frames, window)                    the map editor's world-frame cloud, points_selector.cpp:85-177;
+                                                            GlobalMapping::export_points, global_mapping.cpp:638-680
+    region_growing(cloud, seed_point, **params)             gtsam_points::region_growing_init / _update, points_selector.cpp:798-810
 """
 from __future__ import annotations
 
@@ -811,4 +814,47 @@ def estimate_pose_gnc(target: PointCloudGPU, source: PointCloudGPU, ctx: Context
     if correspondences:
         out["pairs"] = pairs[:r.correspondences].copy()
         out["weights"] = weights[:r.correspondences].copy()
+    return out
+
+
+def concat_frames(poses, frames, window=None, ctx: Context | None = None):
+    """The submaps' device clouds in one world-frame device cloud (gb_concat_frames): poses K x (4,4) T_world_frame, frames K
+    PointCloudGPU, window None (every point) or (cell_size, lo (3,), hi (3,)) inclusive cell bounds.  -> (PointCloudGPU, ids
+    (M,) uint64 = (frame << 32) | original index, the map editor's point ids)"""
+    K = len(frames)
+    ctx = ctx or (frames[0].ctx if K else default_context())
+    arr = (C.c_void_p * max(K, 1))(*[f.h for f in frames])
+    T = pose16(np.stack([np.asarray(p, dtype=np.float64) for p in poses])) if K else np.zeros((0, 16))
+    w = None
+    if window is not None:
+        cell, lo, hi = window
+        w = capi.CellWindow(float(cell), (C.c_int32 * 3)(*[int(v) for v in lo]), (C.c_int32 * 3)(*[int(v) for v in hi]))
+    ids = np.empty(sum(f.n for f in frames), np.uint64)
+    h, m = C.c_void_p(), C.c_size_t()
+    check(lib().gb_concat_frames(ctx.h, K, C.cast(arr, C.c_void_p), ptr(T), C.byref(w) if w is not None else None, C.byref(h), ptr(ids), C.byref(m)))
+    return PointCloudGPU(ctx, h, m.value), ids[: m.value].copy()
+
+
+def region_growing_params(**overrides) -> capi.RegionGrowingParams:
+    """gb_region_growing_default_params (this library's choice, not gtsam_points') with the given fields replaced."""
+    return _params(capi.RegionGrowingParams(), lib().gb_region_growing_default_params, "gb_region_growing_params", overrides)
+
+
+def region_growing(cloud: PointCloudGPU, seed_point, ctx: Context | None = None, labels: bool = False, **params) -> dict:
+    """gtsam_points::region_growing_init + region_growing_update (points_selector.cpp:798-810) on the device
+    (gb_region_growing): the connected surface of `cloud` (with normals) through the point nearest seed_point, dilated by
+    dilation_radius.  params are fields of gb_region_growing_params (distance_threshold, angle_threshold in radians,
+    dilation_radius).  -> {seed, status, status_name, num_region, num_selected, num_components, selected (num_selected,) int32
+    in ascending original index} and, with labels, labels (n,) int32 (the component's smallest index, -1 for non-finite points)."""
+    ctx = ctx or cloud.ctx
+    p = region_growing_params(**params)
+    r = capi.RegionGrowingResult()
+    q = f64(np.asarray(seed_point, dtype=np.float64).reshape(-1)[:3])
+    sel = np.empty(cloud.n, np.int32)
+    lab = np.empty(cloud.n, np.int32) if labels else None
+    check(lib().gb_region_growing(ctx.h, cloud.h, ptr(q), C.byref(p), C.byref(r), ptr(sel), ptr(lab)))
+    out = {"seed": r.seed, "status": r.status, "status_name": capi.REGION_STATUS_NAMES.get(r.status, "?"), "num_region": r.num_region,
+           "num_selected": r.num_selected, "num_components": r.num_components, "selected": sel[: r.num_selected].copy()}
+    if lab is not None:
+        out["labels"] = lab
     return out

@@ -710,6 +710,78 @@ GB_API gb_status gb_preprocess(gb_ctx* ctx, size_t n_raw, const double* xyzw, co
 GB_API gb_status gb_merge_frames(gb_ctx* ctx, size_t num_frames, const gb_cloud* const* frames, const double* poses /* K x 16 */, double downsample_resolution, int target_num_points, uint64_t seed,
                                  double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud** out_cloud);
 
+/* ---- The map editor's world-frame cloud (PointsSelector::update_cells / collect_neighbor_point_ids / collect_submap_points,
+ *      src/glim/viewer/editor/points_selector.cpp:85-177) and GlobalMapping::export_points (global_mapping.cpp:638-680): the
+ *      submaps' DEVICE clouds transformed by T_world_submap and concatenated into one device cloud, optionally only the points
+ *      whose cell lies in a window.
+ *
+ *      The rule.  Per point a of frame k with covariance C and normal n, at pose (R, t): q = R a + t and C' = R C R^T exactly
+ *      as gb_merge_frames transforms them (un-contracted fp64, the same association order, the same kernel), n' = R n with
+ *      row r as (R_r0 nx + R_r1 ny) + R_r2 nz (fp64, not renormalised); each value is stored once as fp32.  The result carries
+ *      covariances iff every frame does (else they are zero) and normals iff every frame does (the editor assumes all submaps
+ *      alike, :118-122); zero frames give neither.  With a window, a point is kept iff k = floor(q * (1.0 / cell_size)) (fp64,
+ *      per axis, on the fp64 q before it is stored) satisfies lo <= k <= hi on every axis; a non-finite q is never kept.  The
+ *      editor keys its fp64 submap points; here q comes from the frames' stored fp32 positions widened to fp64, so a point
+ *      within an ulp of a cell face may land in the neighbouring cell.  Without a window every point is kept, NaN included.
+ *      Output order: frame-major, then ascending original index; ids[i] = (frame << 32) | original index, the editor's point id
+ *      (:84, :139-140).  Zero frames, or nothing kept, give an empty cloud.
+ *
+ *      GB_ERR_INVALID_ARGUMENT before any launch for a non-finite pose entry, a frame on another device than ctx, a non-finite
+ *      or non-positive cell_size, lo > hi on any axis, a frame of 2^32 points or more, or 2^30 points or more in all.
+ *      Launches: 4 (the shared frame transform, the window flags, their scan, the emit) + 3 (gb_cloud_build's Morton reorder)
+ *      = 7; 4 when nothing is kept; none when the frames hold no point.  Two stream synchronisations (the kept count, the end).
+ *      ---- */
+typedef struct gb_cell_window {
+  double cell_size;    /* m, > 0 (the editor's map_cell_resolution) */
+  int32_t lo[3], hi[3]; /* inclusive cell bounds per axis (the editor: centre -/+ cell_selection_window) */
+} gb_cell_window;
+/* poses: K x 16 column-major T_world_frame; window NULL = every point; ids: capacity the sum of the frames' sizes, or NULL */
+GB_API gb_status gb_concat_frames(gb_ctx* ctx, size_t num_frames, const gb_cloud* const* frames, const double* poses, const gb_cell_window* window,
+                                  gb_cloud** out_cloud, uint64_t* ids, size_t* num_out);
+
+/* ---- gtsam_points::region_growing_init / region_growing_update (points_selector.cpp:798-810; docs/edit.md "Plane selection
+ *      and removal"): the connected surface through a picked point of a cloud with normals, and its dilation.  [EXT]
+ *      gtsam_points is not vendored: the rule below is this library's statement of region growing.
+ *
+ *      The rule.  Distances are the fp32 point_d2 = (dx^2 + dy^2) + dz^2 (d = p_j - p_i, uncontracted) of the stored
+ *      positions.  Points i != j are joined iff both are finite, point_d2 < (float)(distance_threshold^2) and
+ *      (nx_i nx_j + ny_i ny_j) + nz_i nz_j >= cos(angle_threshold) (the dot in fp64 from the fp32 normals, each operation
+ *      rounded; cos in fp64; signed; a NaN dot never joins).  The joins are found in a point grid of the cloud at cell
+ *      1.05 distance_threshold with the half-width grid_half_width proves, as FPFH's neighbours are; a point whose key at a
+ *      grid's cell leaves the 21-bit range takes part in no search of that grid.  labels[i] = the smallest original index of
+ *      i's connected component for a finite point, -1 for a non-finite one; num_components = the number of distinct labels
+ *      >= 0.  The seed is the finite point with the smallest point_d2 to (float)seed_point, ties to the smaller original index
+ *      (region_growing_init's nearest-point query); without one, status NO_SEED, seed -1 and nothing selected (labels are
+ *      still written).  The region R = {i : labels[i] == labels[seed]}.  With dilation_radius > 0, the dilation adds every
+ *      finite j outside R for which some i in R has point_d2(i, j) < (float)(dilation_radius^2): the brute-force set, found in
+ *      a point grid of the cloud at cell 1.05 dilation_radius (with the same key-range rule).  selected = R plus the added
+ *      points in ascending original index; num_region = |R|, num_selected = |selected|.  The result is a set: it does not
+ *      depend on the order the device visits points in.
+ *
+ *      GB_ERR_INVALID_ARGUMENT before any launch for a non-empty cloud without normals, a cloud on another device than ctx, a
+ *      non-finite seed_point, or parameters outside the bounds below.  An empty cloud makes no launch.  Launches: the point
+ *      grid builds (gb_point_grid_build at 1.05 distance_threshold, and at 1.05 dilation_radius when it is > 0) + 4 (the
+ *      parents and the seed, the hooks, the labels and the region, the compaction of the selection) + 1 with dilation: the
+ *      same for every size and shape of the graph.  Then one copy and one stream synchronisation. ---- */
+#define GB_REGION_FOUND 0
+#define GB_REGION_NO_SEED 1
+typedef struct gb_region_growing_params {
+  double distance_threshold; /* m, finite, > 0 (editor UI: 0.01-1 m) */
+  double angle_threshold;    /* rad, in [0, pi] (UI: 0.01-180 deg) */
+  double dilation_radius;    /* m, finite, >= 0; 0 = no dilation (UI: 0.01-100 m) */
+} gb_region_growing_params;
+typedef struct gb_region_growing_result {
+  int32_t seed;   /* original index, -1 for none */
+  int32_t status; /* GB_REGION_* */
+  size_t num_region, num_selected, num_components; /* before / after dilation; components over finite points */
+} gb_region_growing_result;
+/* this library's defaults, chosen for a LiDAR map at about 0.1-0.5 m spacing (not gtsam_points' values): 0.5 m, 10 deg, 0 */
+GB_API gb_status gb_region_growing_default_params(gb_region_growing_params* params);
+/* selected: capacity N, ascending original index (the first num_selected written), or NULL; labels: N in the caller's point
+ * order, or NULL */
+GB_API gb_status gb_region_growing(gb_ctx* ctx, const gb_cloud* cloud, const double seed_point[3], const gb_region_growing_params* params,
+                                   gb_region_growing_result* result, int32_t* selected, int32_t* labels);
+
 /* ---- glim::CloudDeskewing::deskew (src/glim/common/cloud_deskewing.cpp:11-55 constant velocity, :57-133 predicted IMU poses;
  *      called at src/glim/odometry/odometry_estimation_imu.cpp:313).  n_imu > 0: imu_times / imu_poses (n_imu x 16, T_world_imu)
  *      and `stamp` select the IMU-pose overload; n_imu == 0: linear_vel / angular_vel (either may be NULL = zero) select the
