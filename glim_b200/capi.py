@@ -106,6 +106,8 @@ _SIGNATURES = {
     "gb_concat_frames": ([vp, sz, vp, vp, vp, vp, vp, vp], st),
     "gb_region_growing_default_params": ([vp], st),
     "gb_region_growing": ([vp, vp, vp, vp, vp, vp, vp], st),
+    "gb_min_cut_default_params": ([vp], st),
+    "gb_min_cut": ([vp, vp, vp, vp, vp, vp, vp, vp], st),
 }
 del vp, i32, f32, f64, sz, u64, st
 SYMBOLS = tuple(_SIGNATURES)  # tests check the library exports exactly these
@@ -196,6 +198,24 @@ class RegionGrowingResult(C.Structure):
 # gb_region_growing_result::status
 REGION_FOUND, REGION_NO_SEED = 0, 1
 REGION_STATUS_NAMES = {0: "FOUND", 1: "NO_SEED"}
+
+
+class MinCutParams(C.Structure):
+    """gb_min_cut_params (include/glim_b200.h)."""
+    _fields_ = [("distance_sigma", C.c_double), ("angle_sigma", C.c_double), ("foreground_mask_radius", C.c_double),
+                ("background_mask_radius", C.c_double), ("foreground_weight", C.c_double), ("k_neighbors", C.c_int)]
+
+
+class MinCutResult(C.Structure):
+    """gb_min_cut_result (include/glim_b200.h)."""
+    _fields_ = [("seed", C.c_int32), ("status", C.c_int32), ("num_points", C.c_size_t), ("num_foreground", C.c_size_t),
+                ("num_background", C.c_size_t), ("num_edges", C.c_size_t), ("num_selected", C.c_size_t), ("cut_value", C.c_int64),
+                ("rounds", C.c_int32)]
+
+
+# gb_min_cut_result::status
+MINCUT_FOUND, MINCUT_NO_SEED, MINCUT_NOT_CONVERGED = 0, 1, 2
+MINCUT_STATUS_NAMES = {0: "FOUND", 1: "NO_SEED", 2: "NOT_CONVERGED"}
 
 # gb_ransac_result::status
 RANSAC_FOUND, RANSAC_EARLY_STOP, RANSAC_DEGENERATE = 0, 1, 2

@@ -8,6 +8,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -316,6 +317,26 @@ gb_status gb_launch(gb_ctx* ctx, const char* name, void (*kernel)(P...), dim3 gr
   ctx->launches++;
   return GB_OK;
 }
+// The same for a cooperative kernel (one that synchronises its whole grid with cooperative_groups' grid.sync()): launched by
+// cudaLaunchCooperativeKernel, which refuses a grid larger than can be resident at once instead of letting it deadlock.  The
+// arguments are converted to the kernel's parameter types first, as a direct launch would.
+struct gb_cooperative_t {};
+constexpr gb_cooperative_t gb_cooperative{};
+template <typename... P, typename... A>
+gb_status gb_launch(gb_ctx* ctx, const char* name, gb_cooperative_t, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+  std::tuple<P...> params(std::forward<A>(args)...);
+  const cudaError_t e = std::apply([&](auto&... p) {
+    void* argv[] = {(void*)&p..., nullptr};
+    return cudaLaunchCooperativeKernel((const void*)kernel, grid, block, argv, smem, ctx->stream);
+  }, params);
+  if (e != cudaSuccess) {
+    (void)cudaGetLastError();
+    gb_set_error("cooperative launch of %s failed: %s", name, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? GB_ERR_OUT_OF_MEMORY : GB_ERR_CUDA;
+  }
+  ctx->launches++;
+  return GB_OK;
+}
 // Every cub device-wide call of the library with temporary storage: fn(storage, bytes, args..., ctx->stream), counted as
 // one launch (a radix sort is several kernels; the counter's unit is the call).  The size queries of gb_cub_temp_bytes
 // launch nothing and do not come here.
@@ -511,6 +532,22 @@ gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T_col
 // h_frames (pinned) and d_frames hold K x GB_FRAME_DESC_BYTES for the descriptor table.  Shared by gb_merge_frames and
 // gb_concat_frames (gb_kernels_segment.cu).  No launch when the frames hold no point.
 gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, void* h_frames, void* d_frames, double4* pts, double* cov6);
+// The exact k-NN of gb_preprocess and gb_find_neighbors (gb_kernels_preprocess.cu), shared with gb_min_cut: the k nearest of
+// the first *d_count points of d_pts (device resident, n slots) to each of them, by un-contracted fp64 d2 with ties to the
+// smaller index, the query included, in neighbors[i * k + j]; the row of a point whose cell of h0 leaves the 21-bit range, or
+// of a slot at or beyond *d_count, is i itself k times, and such a point is nobody's neighbour.  Six launches.  Its
+// temporaries for up to n points come from take_knn_tmp (the cub storage is the caller's); gb_knn_instantiated(k) tells
+// whether k is one of the instantiated neighbour counts (1-10, 12, 15, 16, 20, 24, 32), which entry points check before any
+// launch.
+struct KnnTmp {
+  gb_sort_tmp s;
+  double4* pts_s;
+  void* tables;  // the per-level cell hash tables
+  unsigned ts;   // hash table size per level
+};
+KnnTmp take_knn_tmp(Carver& cv, int n, void* cub, size_t cub_bytes);
+gb_status knn_device(gb_ctx* ctx, int n, const int* d_count, const double4* d_pts, int k, double h0, int* neighbors, const KnnTmp& t);
+bool gb_knn_instantiated(int k);
 // k_grid_keys of the voxel-grid paths: key = packed floor(p * inv_res) in fp64 (~0 for non-finite / out-of-range points,
 // and for every point with keep[i] == 0 when keep is given), idx[i] = i.  One launch.
 gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, const int* keep, unsigned long long* keys, int* idx);

@@ -91,8 +91,7 @@ template <typename Launch> static gb_status knn_dispatch(int k, Launch&& launch)
   gb_set_error("k = %d is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)", k);
   return GB_ERR_INVALID_ARGUMENT;
 }
-// true iff k_knn_pyramid is instantiated for k neighbours; entry points check it before any launch
-static bool gb_knn_instantiated(int k) {
+bool gb_knn_instantiated(int k) {
   return knn_dispatch(k, [](auto) { return GB_OK; }) == GB_OK;
 }
 
@@ -512,15 +511,7 @@ gb_status gb_covariance_cloud(gb_ctx* ctx, int M, const int* d_count, const doub
   return GB_OK;
 }
 
-// Temporaries of knn_device for up to n points.  The outlier removal's k-NN and the frame's k-NN run one after the other
-// on the same stream and share them.
-struct KnnTmp {
-  gb_sort_tmp s;
-  double4* pts_s;
-  MlCell* tables;
-  unsigned ts;  // hash table size per level
-};
-static KnnTmp take_knn_tmp(Carver& cv, int n, void* cub, size_t cub_bytes) {
+KnnTmp take_knn_tmp(Carver& cv, int n, void* cub, size_t cub_bytes) {
   KnnTmp t;
   t.ts = 1024;
   while (t.ts < 2u * (unsigned)n) t.ts <<= 1;
@@ -530,17 +521,17 @@ static KnnTmp take_knn_tmp(Carver& cv, int n, void* cub, size_t cub_bytes) {
   return t;
 }
 
-// exact k-NN of the first *d_count points of d_pts (device resident); neighbors[i * k + j]
-static gb_status knn_device(gb_ctx* ctx, int n, const int* d_count, const double4* d_pts, int k, double h0, int* d_nb, const KnnTmp& t) {
+gb_status knn_device(gb_ctx* ctx, int n, const int* d_count, const double4* d_pts, int k, double h0, int* d_nb, const KnnTmp& t) {
   const int tb = 256, gb = (n + tb - 1) / tb;
   GB_CHECK(gb_launch(ctx, "k_fill_self", k_fill_self, (int)(((size_t)n * k + 255) / 256), 256, 0, n, k, d_nb));
   GB_CHECK(gb_launch(ctx, "k_ml_keys", k_ml_keys, gb, tb, 0, n, d_count, d_pts, 1.0 / h0, t.s.keys, t.s.idx));
   GB_CUB(ctx, cub::DeviceRadixSort::SortPairs, t.s.cub, t.s.cub_bytes, t.s.keys, t.s.keys_s, t.s.idx, t.s.idx_s, n, 0, 64);
   GB_CHECK(gb_launch(ctx, "k_ml_gather", k_ml_gather, gb, tb, 0, n, t.s.keys_s, t.s.idx_s, d_pts, t.pts_s));
-  GB_CUDA(cudaMemsetAsync(t.tables, 0xff, sizeof(MlCell) * (size_t)kMlLevels * t.ts, ctx->stream));
-  GB_CHECK(gb_launch(ctx, "k_ml_cells", k_ml_cells, gb, tb, 0, n, t.s.keys_s, t.tables, t.ts));
+  MlCell* tables = (MlCell*)t.tables;
+  GB_CUDA(cudaMemsetAsync(tables, 0xff, sizeof(MlCell) * (size_t)kMlLevels * t.ts, ctx->stream));
+  GB_CHECK(gb_launch(ctx, "k_ml_cells", k_ml_cells, gb, tb, 0, n, t.s.keys_s, tables, t.ts));
   return knn_dispatch(k, [&](auto K) {
-    return gb_launch(ctx, "k_knn_pyramid", k_knn_pyramid<decltype(K)::value>, (n + 127) / 128, 128, 0, n, t.pts_s, t.s.keys_s, t.s.idx_s, t.tables, t.ts, 1.0 / h0, h0, d_nb);
+    return gb_launch(ctx, "k_knn_pyramid", k_knn_pyramid<decltype(K)::value>, (n + 127) / 128, 128, 0, n, t.pts_s, t.s.keys_s, t.s.idx_s, tables, t.ts, 1.0 / h0, h0, d_nb);
   });
 }
 

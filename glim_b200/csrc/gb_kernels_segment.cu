@@ -11,9 +11,18 @@
 //                       seg_seed_key), k_rg_hook (one thread per grid record: each join (i, j > i) hooked once, ECL-CC),
 //                       k_rg_label (the labels, which also compress the parents, the region and the counts), k_rg_dilate,
 //                       and one cub compaction of the selection; one copy back and one stream synchronisation.
+//   gb_min_cut          k_mc_flags (the participants, and the seed by the same 64-bit atomicMin of seg_seed_key), a cub scan,
+//                       k_mc_nodes (the fp64 node positions, normals, original indices and roles, in ascending original
+//                       index), knn_device on the nodes (6 launches), k_mc_arcs (each row's arcs both ways), a cub radix sort
+//                       on (u << 32 | v), k_mc_unique and a cub scan of its packed (arc, edge) counts, k_mc_csr (the unique
+//                       arcs), k_mc_graph (heads, reverse arcs, capacities, rows and the exported edges), the cooperative
+//                       k_mc_solve (push-relabel, gb_mincut_math.cuh) and one cub compaction of the selection; one copy back
+//                       and one stream synchronisation.
 #include "gb_internal.cuh"
 #include "gb_segment_math.cuh"
+#include "gb_mincut_math.cuh"
 
+#include <cooperative_groups.h>
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <cmath>
@@ -169,6 +178,263 @@ gb_status rg_grid(gb_ctx* ctx, const gb_cloud* cloud, double r, gb_owned<gb_poin
     return GB_ERR_INTERNAL;
   }
   return GB_OK;
+}
+
+// ---- gb_min_cut ----
+constexpr int kMcThreads = 256;
+
+// What gb_min_cut leaves for the host, ahead of the selection and the exported graph in one copy.
+struct McOut {
+  unsigned long long seed_key;  // seg_seed_key of the seed among the participants, ~0 for none
+  long long cut_value;
+  int num_points, num_foreground, num_background, num_arcs, num_edges, num_selected, rounds, status, seed_node, pad;
+};
+
+// one thread per stored slot: flags[i] = point i (original index) takes part, and the seed's key among the participants
+__global__ void __launch_bounds__(kSegThreads) k_mc_flags(int n, const float4* __restrict__ p0, const int* __restrict__ perm, double cx, double cy, double cz, double r2,
+                                                          int* __restrict__ flags, McOut* __restrict__ out) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long key = ~0ull;
+  if (j < n) {
+    const int i = perm ? perm[j] : j;
+    const float4 p = p0[j];
+    const bool in = isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && mc_d2(p.x, p.y, p.z, cx, cy, cz) < r2;
+    flags[i] = in ? 1 : 0;
+    if (in) key = seg_seed_key(p, (float)cx, (float)cy, (float)cz, i);
+  }
+  for (int o = 16; o > 0; o >>= 1) key = min(key, __shfl_xor_sync(0xffffffffu, key, o));
+  if ((threadIdx.x & 31) == 0 && key != ~0ull) atomicMin(&out->seed_key, key);
+}
+
+// one thread per original index i: participant i becomes node pos[i] - 1 with its fp64 position, normal, index and role
+__global__ void __launch_bounds__(kSegThreads) k_mc_nodes(int n, const float4* __restrict__ p0, const float4* __restrict__ normals, const int* __restrict__ inv_perm,
+                                                          const int* __restrict__ flags, const int* __restrict__ pos, double cx, double cy, double cz, double fg2, double bg2,
+                                                          double4* __restrict__ pts, float4* __restrict__ nrm, int* __restrict__ orig, int* __restrict__ role,
+                                                          McOut* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool fg = false, bg = false;
+  if (i < n && flags[i]) {
+    const int u = pos[i] - 1, j = inv_perm ? inv_perm[i] : i;
+    const float4 p = p0[j];
+    pts[u] = make_double4(p.x, p.y, p.z, 1.0);
+    nrm[u] = normals[j];
+    orig[u] = i;
+    const bool seed = (unsigned long long)(uint32_t)i == (out->seed_key & 0xffffffffull) && out->seed_key != ~0ull;
+    const int r = seed ? MC_SEED : mc_role(mc_d2(p.x, p.y, p.z, cx, cy, cz), fg2, bg2);
+    role[u] = r;
+    if (seed) out->seed_node = u;
+    fg = r == MC_FOREGROUND;
+    bg = r == MC_BACKGROUND;
+  }
+  if (i == n - 1) out->num_points = pos[n - 1];
+  warp_count(fg, &out->num_foreground);
+  warp_count(bg, &out->num_background);
+}
+
+// one thread per k-NN slot (u, j): the arcs u -> v and v -> u of neighbour v != u, else two empty keys.  The rows of slots
+// past the participants, and of nodes without a key, hold only the node itself.
+__global__ void k_mc_arcs(int nk, int k, const int* __restrict__ nb, unsigned long long* __restrict__ keys) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nk) return;
+  const unsigned long long u = (unsigned)(t / k), v = (unsigned)nb[t];
+  const bool ok = u != v;
+  keys[2 * (size_t)t] = ok ? (u << 32 | v) : ~0ull;
+  keys[2 * (size_t)t + 1] = ok ? (v << 32 | u) : ~0ull;
+}
+
+__device__ __forceinline__ bool mc_first(const unsigned long long* keys_s, int s) {
+  const unsigned long long k = keys_s[s];
+  return k != ~0ull && (s == 0 || keys_s[s - 1] != k);
+}
+
+// one thread per sorted slot: 1 for the first copy of an arc, plus 2^32 when it is an edge's arc u -> v with u < v
+__global__ void k_mc_unique(int na, const unsigned long long* __restrict__ keys_s, unsigned long long* __restrict__ flags) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= na) return;
+  const unsigned long long k = keys_s[s];
+  flags[s] = mc_first(keys_s, s) ? (1ull | ((k >> 32) < (k & 0xffffffffull) ? 1ull << 32 : 0ull)) : 0ull;
+}
+
+// one thread per sorted slot: the unique arcs in (u, v) order, each with its edge's rank (u < v) or -1, and their counts
+__global__ void k_mc_csr(int na, const unsigned long long* __restrict__ keys_s, const unsigned long long* __restrict__ pos, unsigned long long* __restrict__ ukeys,
+                         int* __restrict__ eidx, McOut* __restrict__ out) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= na) return;
+  const unsigned long long k = keys_s[s], p = pos[s];
+  if (mc_first(keys_s, s)) {
+    const int a = (int)(uint32_t)p - 1;
+    ukeys[a] = k;
+    eidx[a] = (k >> 32) < (k & 0xffffffffull) ? (int)(p >> 32) - 1 : -1;
+  }
+  if (s == na - 1) {
+    out->num_arcs = (int)(uint32_t)p;
+    out->num_edges = (int)(p >> 32);
+  }
+}
+
+// the first index of keys[0, n) (ascending) that is >= x
+__device__ __forceinline__ int mc_lower_bound(const unsigned long long* keys, int n, unsigned long long x) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (keys[mid] < x) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// one thread per arc a and per row start: head, reverse arc, capacity (and the exported edge row), row[u] = first arc of u
+__global__ void k_mc_graph(int slots, const unsigned long long* __restrict__ ukeys, const int* __restrict__ eidx, const double4* __restrict__ pts, const float4* __restrict__ nrm,
+                           const int* __restrict__ orig, double s2d, double s2a, const McOut* __restrict__ out, int* __restrict__ head, int* __restrict__ rev,
+                           int* __restrict__ cap, int* __restrict__ row, int* __restrict__ edges, int* __restrict__ ecap) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= slots) return;
+  const int A = out->num_arcs, m = out->num_points;
+  if (t < A) {
+    const unsigned long long k = ukeys[t];
+    const int u = (int)(k >> 32), v = (int)(uint32_t)k;
+    head[t] = v;
+    rev[t] = mc_lower_bound(ukeys, A, (unsigned long long)v << 32 | (unsigned)u);
+    const double4 a = pts[u], b = pts[v];
+    const float4 na = nrm[u], nb = nrm[v];
+    const int q = mc_edge_capacity((float)a.x, (float)a.y, (float)a.z, na.x, na.y, na.z, (float)b.x, (float)b.y, (float)b.z, nb.x, nb.y, nb.z, s2d, s2a);
+    cap[t] = q;
+    const int e = eidx[t];
+    if (edges && e >= 0) {
+      edges[2 * (size_t)e] = orig[u];
+      edges[2 * (size_t)e + 1] = orig[v];
+      ecap[e] = q;
+    }
+  }
+  if (t <= m) row[t] = mc_lower_bound(ukeys, A, (unsigned long long)t << 32);
+}
+
+// The flow network and the solver's state (gb_mincut_math.cuh): m nodes of n slots, CSR rows, arcs with their heads, reverse
+// arcs and capacities.  e, incoming and cnt are zero at launch.
+struct McSolve {
+  int n;
+  int fg_cap;
+  const int* row;
+  const int* head;
+  const int* rev;
+  const int* cap;
+  const int* role;
+  int* res;
+  int* fg_res;
+  int* h0;  // the heights, double-buffered
+  int* h1;
+  long long* e;
+  long long* incoming;
+  int* cnt;  // [3]: the rotating grid-wide counters
+  int* sel;
+  McOut* out;
+};
+
+__device__ __forceinline__ bool mc_inner(int r) { return r == MC_FREE || r == MC_FOREGROUND; }
+
+// The whole solve in one cooperative grid (grid.sync() between steps; every thread runs every loop the same number of
+// times).  Initialise (every arc out of the background saturated), a global relabel, then rounds of push / relabel with a
+// global relabel every kMcRelabelPeriod rounds, until no node is active or kMcMaxRounds rounds have run.  A global relabel
+// is a level-synchronous breadth-first search from the seed over reverse residual arcs: exact distances, H for the nodes
+// that cannot reach the seed.  The last one labels the selection.
+__global__ void __launch_bounds__(kMcThreads, 4) k_mc_solve(McSolve g) {
+  namespace cg = cooperative_groups;
+  cg::grid_group grid = cg::this_grid();
+  const int t0 = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+  for (int u = t0; u < g.n; u += stride) g.sel[u] = 0;
+  const int m = g.out->num_points;
+  if (m == 0) return;  // every thread alike
+  const int seed = g.out->seed_node, H = m + 2;
+  for (int u = t0; u < m; u += stride) {
+    const int ru = g.role[u];
+    g.fg_res[u] = ru == MC_FOREGROUND ? g.fg_cap : 0;
+    for (int a = g.row[u]; a < g.row[u + 1]; a++) {
+      const int rv = g.role[g.head[a]];
+      g.res[a] = mc_initial_residual(ru, rv, g.cap[a]);
+      if (ru == MC_BACKGROUND && rv != MC_BACKGROUND) mc_add(&g.e[g.head[a]], g.cap[a]);
+    }
+  }
+  grid.sync();
+  int phase = 0;
+  // the grid-wide sum of every thread's x (a grid barrier): counter phase % 3 collects it while the next one is cleared
+  const auto total = [&](int x) {
+    int* c = g.cnt + phase % 3;
+    if (t0 == 0) g.cnt[(phase + 1) % 3] = 0;
+    x = __reduce_add_sync(0xffffffffu, x);
+    if ((threadIdx.x & 31) == 0 && x) atomicAdd(c, x);
+    grid.sync();
+    phase++;
+    return *(volatile int*)c;
+  };
+  const auto global_relabel = [&](int* h) {
+    for (int u = t0; u < m; u += stride) h[u] = u == seed ? 0 : H;
+    grid.sync();
+    volatile int* vh = h;
+    for (int d = 0; d < m; d++) {
+      int added = 0;
+      for (int v = t0; v < m; v += stride) {
+        if (d == 0 && g.role[v] == MC_FOREGROUND && g.fg_res[v] > 0 && vh[v] == H) {
+          vh[v] = 1;
+          added++;
+        }
+        if (vh[v] != d) continue;
+        for (int a = g.row[v]; a < g.row[v + 1]; a++) {
+          const int u = g.head[a];
+          if (vh[u] == H && g.role[u] != MC_BACKGROUND && g.res[g.rev[a]] > 0) {
+            vh[u] = d + 1;
+            added++;
+          }
+        }
+      }
+      if (total(added) == 0) break;
+    }
+  };
+  const auto active = [&](const int* h) {
+    int x = 0;
+    for (int u = t0; u < m; u += stride) x += mc_inner(g.role[u]) && h[u] < H && g.e[u] > 0;
+    return total(x);
+  };
+  int *h = g.h0, *hn = g.h1, rounds = 0;
+  global_relabel(h);
+  int act = active(h);
+  while (act > 0 && rounds < kMcMaxRounds) {
+    rounds++;
+    for (int u = t0; u < m; u += stride)
+      if (mc_inner(g.role[u]) && h[u] < H && g.e[u] > 0) g.e[u] = mc_push_node(u, g.e[u], g.row, g.head, g.rev, g.res, g.fg_res, h, g.incoming, seed);
+    grid.sync();
+    int x = 0;
+    for (int u = t0; u < m; u += stride) {
+      const int ru = g.role[u];
+      long long ex = g.e[u];
+      int hu = h[u];
+      if (mc_inner(ru) && hu < H && ex > 0) hu = mc_relabel_node(u, ru, g.row, g.head, g.res, g.fg_res, h, H);
+      hn[u] = hu;
+      ex += g.incoming[u];
+      g.incoming[u] = 0;
+      g.e[u] = ex;
+      x += mc_inner(ru) && hu < H && ex > 0;
+    }
+    int* t = h;
+    h = hn;
+    hn = t;
+    act = total(x);
+    if (act > 0 && rounds % kMcRelabelPeriod == 0) {
+      global_relabel(h);
+      act = active(h);
+    }
+  }
+  if (act > 0) {  // the round cap: nothing selected
+    if (t0 == 0) {
+      g.out->status = GB_MINCUT_NOT_CONVERGED;
+      g.out->rounds = rounds;
+    }
+    return;
+  }
+  global_relabel(h);
+  for (int u = t0; u < m; u += stride) g.sel[u] = h[u] < H && g.role[u] != MC_BACKGROUND ? 1 : 0;
+  if (t0 == 0) {
+    g.out->cut_value = g.e[seed];
+    g.out->rounds = rounds;
+  }
 }
 
 }  // namespace
@@ -355,5 +621,157 @@ extern "C" gb_status gb_region_growing(gb_ctx* ctx, const gb_cloud* cloud, const
   result->num_components = (size_t)h_out->num_components;
   if (selected) memcpy(selected, h_selected, sizeof(int32_t) * result->num_selected);
   if (labels) memcpy(labels, h_labels, sizeof(int32_t) * N);
+  return GB_OK;
+}
+
+extern "C" gb_status gb_min_cut_default_params(gb_min_cut_params* p) {
+  GB_REQUIRE(p, "null argument");
+  p->distance_sigma = 0.25;
+  p->angle_sigma = 10.0 * 3.141592653589793 / 180.0;
+  p->foreground_mask_radius = 0.5;
+  p->background_mask_radius = 5.0;
+  p->foreground_weight = 10.0;
+  p->k_neighbors = 20;
+  return GB_OK;
+}
+
+extern "C" gb_status gb_min_cut(gb_ctx* ctx, const gb_cloud* cloud, const double c[3], const gb_min_cut_params* prm, gb_min_cut_result* result, int32_t* selected,
+                                int32_t* edges, int32_t* capacities) {
+  GB_REQUIRE(ctx && cloud && c && prm && result, "null argument");
+  GB_REQUIRE(cloud->device == ctx->device, "the cloud lives on another device");
+  GB_REQUIRE(cloud->n == 0 || cloud->normals, "min cut needs the cloud's normals");
+  GB_REQUIRE(std::isfinite(c[0]) && std::isfinite(c[1]) && std::isfinite(c[2]), "a non-finite picked point");
+  GB_REQUIRE(std::isfinite(prm->distance_sigma) && prm->distance_sigma > 0.0, "distance_sigma must be positive and finite");
+  GB_REQUIRE(prm->angle_sigma > 0.0 && prm->angle_sigma <= 3.141592653589793, "angle_sigma must be in (0, pi]");
+  GB_REQUIRE(std::isfinite(prm->foreground_mask_radius) && prm->foreground_mask_radius > 0.0, "foreground_mask_radius must be positive and finite");
+  GB_REQUIRE(std::isfinite(prm->background_mask_radius) && prm->background_mask_radius > prm->foreground_mask_radius,
+             "background_mask_radius must be finite and larger than foreground_mask_radius");
+  GB_REQUIRE(prm->foreground_weight >= 0.0 && prm->foreground_weight <= 1000.0, "foreground_weight must be in [0, 1000]");
+  GB_REQUIRE(gb_knn_instantiated(prm->k_neighbors), "k_neighbors is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
+  GB_REQUIRE(cloud->n * (size_t)prm->k_neighbors < ((size_t)1 << 30), "N * k_neighbors must be below 2^30");
+  GB_ENTER(ctx);
+  memset(result, 0, sizeof(*result));
+  result->seed = -1;
+  result->status = GB_MINCUT_NO_SEED;
+  const size_t N = cloud->n;
+  if (N == 0) return GB_OK;
+  const int n = (int)N, k = prm->k_neighbors, nk = n * k, na = 2 * nk;
+  const bool graph = edges || capacities;
+  int end_bit = 33;  // the arc keys (u << 32 | v) with u, v < n, and ~0 for none, which sorts last on these bits too
+  while (end_bit < 64 && ((size_t)1 << (end_bit - 32)) < N) end_bit++;
+  size_t cub_b = gb_cub_temp_bytes(N), b = 0;
+  cub::DeviceRadixSort::SortKeys(nullptr, b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, na, 0, end_bit);
+  cub_b = std::max(cub_b, b);
+  cub::DeviceScan::InclusiveSum(nullptr, b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, na);
+  cub_b = std::max(cub_b, b);
+  cub::DeviceSelect::Flagged(nullptr, b, (const int*)nullptr, (const int*)nullptr, (int*)nullptr, (int*)nullptr, n);
+  cub_b = std::max(cub_b, b);
+  KnnTmp knn;
+  void* d_cub;
+  int *d_flags, *d_pos, *d_orig, *d_role, *d_nb, *d_eidx, *d_head, *d_rev, *d_cap, *d_res, *d_row, *d_fg, *d_h0, *d_h1, *d_cnt, *d_sel, *d_selected, *d_edges, *d_ecap;
+  double4* d_pts;
+  float4* d_nrm;
+  unsigned long long *d_keys, *d_keys_s, *d_apos;
+  long long *d_e, *d_in;
+  McOut* d_out;
+  // out, selected and the graph are adjacent: one copy brings them back, into the same layout of the pinned arena
+  const auto tail = [&](Carver& cv, McOut*& o, int*& s, int*& e, int*& q) {
+    o = cv.take<McOut>(1);
+    s = cv.take<int>(N);
+    e = graph ? cv.take<int>(2 * (size_t)nk) : nullptr;
+    q = graph ? cv.take<int>((size_t)nk) : nullptr;
+  };
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+    d_cub = cv.take<char>(cub_b);
+    knn = take_knn_tmp(cv, n, d_cub, cub_b);
+    d_flags = cv.take<int>(N);
+    d_pos = cv.take<int>(N);
+    d_pts = cv.take<double4>(N);
+    d_nrm = cv.take<float4>(N);
+    d_orig = cv.take<int>(N);
+    d_role = cv.take<int>(N);
+    d_nb = cv.take<int>((size_t)nk);
+    d_keys = cv.take<unsigned long long>((size_t)na);  // the arcs, then the unique flags, then the unique arcs
+    d_keys_s = cv.take<unsigned long long>((size_t)na);
+    d_apos = cv.take<unsigned long long>((size_t)na);
+    d_eidx = cv.take<int>((size_t)na);
+    d_head = cv.take<int>((size_t)na);
+    d_rev = cv.take<int>((size_t)na);
+    d_cap = cv.take<int>((size_t)na);
+    d_res = cv.take<int>((size_t)na);
+    d_row = cv.take<int>(N + 1);
+    d_fg = cv.take<int>(N);
+    d_h0 = cv.take<int>(N);
+    d_h1 = cv.take<int>(N);
+    d_sel = cv.take<int>(N);
+    d_e = cv.take<long long>(2 * N);  // excess, then incoming
+    d_cnt = cv.take<int>(3);
+    tail(cv, d_out, d_selected, d_edges, d_ecap);
+  }));
+  d_in = d_e + N;
+  McOut* h_out;
+  int *h_selected, *h_edges, *h_ecap;
+  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { tail(cv, h_out, h_selected, h_edges, h_ecap); }));
+  cudaStream_t st = ctx->stream;
+  GB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(McOut), st));
+  GB_CUDA(cudaMemsetAsync(&d_out->seed_key, 0xff, sizeof(unsigned long long), st));
+  GB_CUDA(cudaMemsetAsync(d_e, 0, sizeof(long long) * 2 * N, st));
+  GB_CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(int) * 3, st));
+  const double r1 = prm->background_mask_radius + 1.0;
+  const double fg = prm->foreground_mask_radius, bg = prm->background_mask_radius, sd = prm->distance_sigma, sa = prm->angle_sigma;
+  const int gb = (n + kSegThreads - 1) / kSegThreads;
+  GB_CHECK(gb_launch(ctx, "k_mc_flags", k_mc_flags, gb, kSegThreads, 0, n, cloud->p0, cloud->perm, c[0], c[1], c[2], r1 * r1, d_flags, d_out));
+  GB_CUB(ctx, cub::DeviceScan::InclusiveSum, d_cub, cub_b, d_flags, d_pos, n);
+  GB_CHECK(gb_launch(ctx, "k_mc_nodes", k_mc_nodes, gb, kSegThreads, 0, n, cloud->p0, cloud->normals, cloud->inv_perm, d_flags, d_pos, c[0], c[1], c[2], fg * fg, bg * bg,
+                     d_pts, d_nrm, d_orig, d_role, d_out));
+  GB_CHECK(knn_device(ctx, n, &d_out->num_points, d_pts, k, 0.25, d_nb, knn));
+  GB_CHECK(gb_launch(ctx, "k_mc_arcs", k_mc_arcs, (nk + kSegThreads - 1) / kSegThreads, kSegThreads, 0, nk, k, d_nb, d_keys));
+  GB_CUB(ctx, cub::DeviceRadixSort::SortKeys, d_cub, cub_b, d_keys, d_keys_s, na, 0, end_bit);
+  const int ga = (na + kSegThreads - 1) / kSegThreads;
+  GB_CHECK(gb_launch(ctx, "k_mc_unique", k_mc_unique, ga, kSegThreads, 0, na, d_keys_s, d_keys));
+  GB_CUB(ctx, cub::DeviceScan::InclusiveSum, d_cub, cub_b, d_keys, d_apos, na);
+  GB_CHECK(gb_launch(ctx, "k_mc_csr", k_mc_csr, ga, kSegThreads, 0, na, d_keys_s, d_apos, d_keys, d_eidx, d_out));
+  const int slots = std::max(na, n + 1);
+  GB_CHECK(gb_launch(ctx, "k_mc_graph", k_mc_graph, (slots + kSegThreads - 1) / kSegThreads, kSegThreads, 0, slots, d_keys, d_eidx, d_pts, d_nrm, d_orig, 2.0 * sd * sd,
+                     2.0 * sa * sa, d_out, d_head, d_rev, d_cap, d_row, d_edges, d_ecap));
+  McSolve S;
+  S.n = n;
+  S.fg_cap = (int)floor(prm->foreground_weight * kMcScale);
+  S.row = d_row;
+  S.head = d_head;
+  S.rev = d_rev;
+  S.cap = d_cap;
+  S.role = d_role;
+  S.res = d_res;
+  S.fg_res = d_fg;
+  S.h0 = d_h0;
+  S.h1 = d_h1;
+  S.e = d_e;
+  S.incoming = d_in;
+  S.cnt = d_cnt;
+  S.sel = d_sel;
+  S.out = d_out;
+  // a persistent grid: as many CTAs as can be resident at once (the runtime refuses more), and no more than the slots need
+  int per_sm = 0;
+  GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_mc_solve, kMcThreads, 0));
+  const int blocks = std::max(1, std::min(per_sm * ctx->num_sms, (n + kMcThreads - 1) / kMcThreads));
+  GB_CHECK(gb_launch(ctx, "k_mc_solve", gb_cooperative, k_mc_solve, blocks, kMcThreads, 0, S));
+  GB_CUB(ctx, cub::DeviceSelect::Flagged, d_cub, cub_b, d_orig, d_sel, d_selected, &d_out->num_selected, n);
+  const char* end = graph ? (const char*)(d_ecap + nk) : (const char*)(d_selected + N);
+  GB_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)(end - (const char*)d_out), cudaMemcpyDeviceToHost, st));
+  GB_CUDA(cudaStreamSynchronize(st));
+  result->num_points = (size_t)h_out->num_points;
+  result->num_foreground = (size_t)h_out->num_foreground;
+  result->num_background = (size_t)h_out->num_background;
+  result->num_edges = (size_t)h_out->num_edges;
+  if (h_out->seed_key == ~0ull) return GB_OK;
+  result->seed = (int32_t)(uint32_t)h_out->seed_key;
+  result->status = h_out->status;
+  result->num_selected = (size_t)h_out->num_selected;
+  result->cut_value = h_out->cut_value;
+  result->rounds = h_out->rounds;
+  if (selected) memcpy(selected, h_selected, sizeof(int32_t) * result->num_selected);
+  if (edges) memcpy(edges, h_edges, sizeof(int32_t) * 2 * result->num_edges);
+  if (capacities) memcpy(capacities, h_ecap, sizeof(int32_t) * result->num_edges);
   return GB_OK;
 }

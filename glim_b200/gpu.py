@@ -29,6 +29,7 @@ include/glim_b200/gtsam_points_compat.hpp.
     concat_frames(poses, frames, window)                    the map editor's world-frame cloud, points_selector.cpp:85-177;
                                                             GlobalMapping::export_points, global_mapping.cpp:638-680
     region_growing(cloud, seed_point, **params)             gtsam_points::region_growing_init / _update, points_selector.cpp:798-810
+    min_cut(cloud, picked_point, **params)                  gtsam_points::min_cut, points_selector.cpp:774-796
 """
 from __future__ import annotations
 
@@ -857,4 +858,34 @@ def region_growing(cloud: PointCloudGPU, seed_point, ctx: Context | None = None,
            "num_selected": r.num_selected, "num_components": r.num_components, "selected": sel[: r.num_selected].copy()}
     if lab is not None:
         out["labels"] = lab
+    return out
+
+
+def min_cut_params(**overrides) -> capi.MinCutParams:
+    """gb_min_cut_default_params (the editor's radii and weight; this library's sigmas and k) with the given fields replaced."""
+    return _params(capi.MinCutParams(), lib().gb_min_cut_default_params, "gb_min_cut_params", overrides)
+
+
+def min_cut(cloud: PointCloudGPU, picked_point, ctx: Context | None = None, graph: bool = False, **params) -> dict:
+    """gtsam_points::min_cut (points_selector.cpp:774-796) on the device (gb_min_cut): the object of `cloud` (with normals)
+    around picked_point, cut from the background shell by a minimum s-t cut.  params are fields of gb_min_cut_params
+    (distance_sigma, angle_sigma in radians, foreground_mask_radius, background_mask_radius, foreground_weight,
+    k_neighbors).  -> {seed, status, status_name, num_points, num_foreground, num_background, num_edges, num_selected,
+    cut_value (units of 2^-16), rounds, selected (num_selected,) int32 in ascending original index} and, with graph, edges
+    (num_edges, 2) int32 original indices i < j ascending and capacities (num_edges,) int32: the graph the cut was taken on."""
+    ctx = ctx or cloud.ctx
+    p = min_cut_params(**params)
+    r = capi.MinCutResult()
+    q = f64(np.asarray(picked_point, dtype=np.float64).reshape(-1)[:3])
+    sel = np.empty(cloud.n, np.int32)
+    cap = cloud.n * max(int(p.k_neighbors), 0) if graph else 0
+    e = np.empty((cap, 2), np.int32) if graph else None
+    w = np.empty(cap, np.int32) if graph else None
+    check(lib().gb_min_cut(ctx.h, cloud.h, ptr(q), C.byref(p), C.byref(r), ptr(sel), ptr(e), ptr(w)))
+    out = {"seed": r.seed, "status": r.status, "status_name": capi.MINCUT_STATUS_NAMES.get(r.status, "?"), "num_points": r.num_points,
+           "num_foreground": r.num_foreground, "num_background": r.num_background, "num_edges": r.num_edges, "num_selected": r.num_selected,
+           "cut_value": r.cut_value, "rounds": r.rounds, "selected": sel[: r.num_selected].copy()}
+    if graph:
+        out["edges"] = e[: r.num_edges].copy()
+        out["capacities"] = w[: r.num_edges].copy()
     return out

@@ -782,6 +782,69 @@ GB_API gb_status gb_region_growing_default_params(gb_region_growing_params* para
 GB_API gb_status gb_region_growing(gb_ctx* ctx, const gb_cloud* cloud, const double seed_point[3], const gb_region_growing_params* params,
                                    gb_region_growing_result* result, int32_t* selected, int32_t* labels);
 
+/* ---- gtsam_points::min_cut (points_selector.cpp:774-796, the editor's default segmentation; docs/edit.md "Object selection
+ *      and removal"): the object around a picked point of a cloud with normals, cut from its surroundings by a minimum s-t
+ *      cut.  [EXT] gtsam_points is not vendored: the rule below is this library's statement of min-cut segmentation.
+ *
+ *      The rule.  Positions and normals are the cloud's stored fp32 values; c = picked_point; fp64 d2 = (dx^2 + dy^2) + dz^2,
+ *      each operation rounded.
+ *      1. Participants: the finite points with d2(p, c) < (background_mask_radius + 1)^2 (the editor's filter, :777-783),
+ *         numbered as nodes in ascending original index.  Other points take no part, not even as neighbours.
+ *      2. Seed: the participant with the smallest fp32 point_d2 to (float)c, ties to the smaller index (gb_region_growing's
+ *         seed rule).  With no participant: status NO_SEED, seed -1, nothing selected, no solve.
+ *      3. Roles of the other participants: foreground if d2(p, c) < foreground_mask_radius^2, background if
+ *         d2(p, c) > background_mask_radius^2, free otherwise.
+ *      4. Edges: N(i) is participant i's row of the k_neighbors nearest participants by gb_find_neighbors' rule (fp64 d2,
+ *         ties to the smaller index, the query included), with i itself dropped; a participant whose 0.25 m cell leaves the
+ *         21-bit range has an empty row and is in no row.  {i, j} is an edge iff j in N(i) or i in N(j), of weight
+ *         w = exp(-d2 / (2 distance_sigma^2)) * exp(-theta^2 / (2 angle_sigma^2)), theta = acos(min(|n_i . n_j|, 1)) with the
+ *         dot (x + y) + z in fp64 from the fp32 normals (blind to a normal's sign); a NaN dot or a zero normal gives w = 0.
+ *         Capacity q = (int32)floor(w * 65536), the same both ways.
+ *      5. Network: source s = the seed, sink t = every background participant contracted (both hard); each edge is a pair of
+ *         arcs of capacity q; each foreground participant has an arc s -> i of capacity floor(foreground_weight * 65536);
+ *         free participants have no terminal arc.
+ *      6. Cut: selected = the seed plus every participant reachable from s in the residual graph of a maximum s-t flow: the
+ *         intersection of the source sides of all minimum cuts, unique whatever algorithm finds the flow, so ties between
+ *         equal cuts resolve to the smallest object.  cut_value = the flow value, in units of 2^-16.  Background points are
+ *         never selected; a point joined to the seed only by zero-capacity edges is not selected unless its foreground arc
+ *         is not saturated.
+ *      The flow is found by synchronous push-relabel with the roles swapped (the background is the source and the seed the
+ *      sink), with a global relabel every 16 rounds; its rounds are bit-deterministic.  Beyond 65536 rounds the status is
+ *      NOT_CONVERGED, with nothing selected and cut_value 0.  The transcendental weights may differ from another libm's by
+ *      an ulp, and so a capacity by 1; edges and capacities (may be NULL) return the graph the cut was taken on: num_edges
+ *      rows {i, j} of original indices, i < j, ascending, and their capacities.
+ *
+ *      GB_ERR_INVALID_ARGUMENT before any launch for null arguments, a cloud on another device than ctx, a non-empty cloud
+ *      without normals, a non-finite picked_point, parameters outside the bounds below, or N * k_neighbors >= 2^30.  An empty
+ *      cloud makes no launch.  Launches: 3 (participant flags and the seed, their scan, the nodes and their roles) + 6 (the
+ *      k-NN) + 6 (the arcs, their sort, the unique flags, their scan, the CSR, the reverse arcs and capacities) + 1 (the
+ *      cooperative solve) + 1 (the compaction of the selection) = 17, for every size and shape, NO_SEED included (its kernels
+ *      find no node and return).  Then one copy and one stream synchronisation.  The work and scratch scale with the cloud's
+ *      N (2 N k_neighbors arc slots), not with the participants: pass a window of the map, as the editor does. ---- */
+#define GB_MINCUT_FOUND 0
+#define GB_MINCUT_NO_SEED 1
+#define GB_MINCUT_NOT_CONVERGED 2
+typedef struct gb_min_cut_params {
+  double distance_sigma;         /* m, finite, > 0: 0.25 (this library's) */
+  double angle_sigma;            /* rad, in (0, pi]: 10 deg (this library's) */
+  double foreground_mask_radius; /* m, finite, > 0: 0.5 (points_selector.cpp:43) */
+  double background_mask_radius; /* m, finite, > foreground_mask_radius: 5.0 (:44) */
+  double foreground_weight;      /* in [0, 1000]: 10 (:42) */
+  int k_neighbors;               /* an instantiated k-NN count (1-10, 12, 15, 16, 20, 24, 32): 20 (this library's) */
+} gb_min_cut_params;
+typedef struct gb_min_cut_result {
+  int32_t seed, status; /* original index (-1 for none); GB_MINCUT_* */
+  size_t num_points, num_foreground, num_background, num_edges, num_selected; /* participants, their roles, undirected edges */
+  int64_t cut_value;    /* the maximum flow, in units of 2^-16 */
+  int32_t rounds;       /* push-relabel rounds (diagnostic; deterministic) */
+} gb_min_cut_result;
+/* 0.25 m, 10 deg, 0.5 m, 5.0 m, 10, 20 */
+GB_API gb_status gb_min_cut_default_params(gb_min_cut_params* params);
+/* selected: capacity N, ascending original index, or NULL.  edges (capacity N * k_neighbors rows of 2 original indices i < j,
+ * ascending) and capacities (same rows) may be NULL: the graph the cut was taken on. */
+GB_API gb_status gb_min_cut(gb_ctx* ctx, const gb_cloud* cloud, const double picked_point[3], const gb_min_cut_params* params,
+                            gb_min_cut_result* result, int32_t* selected, int32_t* edges, int32_t* capacities);
+
 /* ---- glim::CloudDeskewing::deskew (src/glim/common/cloud_deskewing.cpp:11-55 constant velocity, :57-133 predicted IMU poses;
  *      called at src/glim/odometry/odometry_estimation_imu.cpp:313).  n_imu > 0: imu_times / imu_poses (n_imu x 16, T_world_imu)
  *      and `stamp` select the IMU-pose overload; n_imu == 0: linear_vel / angular_vel (either may be NULL = zero) select the

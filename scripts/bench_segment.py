@@ -1,6 +1,7 @@
 """Map segmentation on the device (not a gate): an editor-sized window cut out of a synthetic map of a few hundred submaps
-by gb_concat_frames, then gb_region_growing at the editor's typical settings, against the host restatement
-(tests/segment_oracle.py) on the same input.  Prints one JSON line per leg with the card and its power limit.
+by gb_concat_frames, then gb_region_growing at the editor's typical settings, and gb_min_cut with the editor's defaults on the
+same window, each against the host restatement (tests/segment_oracle.py, tests/mincut_oracle.py) on the
+same input.  Prints one JSON line per leg with the card and its power limit.
 
     python scripts/bench_segment.py [--submaps 300] [--points 10000] [--reps 5]"""
 import argparse
@@ -17,6 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from glim_b200 import gpu  # noqa: E402
+from tests import mincut_oracle as mo  # noqa: E402
 from tests import segment_oracle as so  # noqa: E402
 
 
@@ -74,7 +76,16 @@ def main():
     t_host = (time.perf_counter() - t0) * 1e3
     same = bool(np.array_equal(ids[got["selected"]], ref_cat["ids"][ref["selected"]]))
     print(json.dumps(dict(base, leg="host_oracle", window_points=len(ref_cat["xyz"]), ms=round(t_host, 3), identical=same)), flush=True)
-    if not same:
+    # the editor's default method on the same window, picked at the same point, with the editor's radii and weight
+    mc, t_mc = timed(lambda: gpu.min_cut(cloud, picked, ctx=ctx))
+    print(json.dumps(dict(base, leg="min_cut", window_points=cloud.size(), participants=int(mc["num_points"]), edges=int(mc["num_edges"]),
+                          rounds=int(mc["rounds"]), selected=int(mc["num_selected"]), ms=round(t_mc, 3))), flush=True)
+    t0 = time.perf_counter()
+    ref_mc = mo.min_cut(ref_cat["xyz"], ref_cat["normals"], picked)
+    t_host = (time.perf_counter() - t0) * 1e3
+    same_mc = bool(np.array_equal(ids[mc["selected"]], ref_cat["ids"][ref_mc["selected"]]))
+    print(json.dumps(dict(base, leg="min_cut_host_oracle", participants=int(ref_mc["num_points"]), ms=round(t_host, 3), identical=same_mc)), flush=True)
+    if not (same and same_mc):
         sys.exit(1)
 
 
