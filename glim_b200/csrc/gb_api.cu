@@ -212,6 +212,18 @@ gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes) {
   return GB_OK;
 }
 
+gb_status gb_upload(gb_ctx* ctx, std::initializer_list<gb_xfer> parts) {
+  for (const gb_xfer& p : parts)
+    if (p.src && p.bytes) GB_CUDA(cudaMemcpyAsync(p.dst, p.src, p.bytes, cudaMemcpyHostToDevice, ctx->stream));
+  return GB_OK;
+}
+gb_status gb_download(gb_ctx* ctx, std::initializer_list<gb_xfer> parts) {
+  for (const gb_xfer& p : parts)
+    if (p.dst && p.bytes) GB_CUDA(cudaMemcpyAsync(p.dst, p.src, p.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return GB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // clouds
 // ---------------------------------------------------------------------------------------------

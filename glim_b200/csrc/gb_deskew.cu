@@ -185,7 +185,6 @@ extern "C" gb_status gb_deskew(gb_ctx* ctx, const double T_imu_lidar[16], const 
   size_t m = 0;
   GB_CHECK(gb_deskew_pose_table(T_imu_lidar, linear_vel, angular_vel, n_imu, imu_times, imu_poses, stamp, n, times, idx.data(), table.data(), &m));
   GB_ENTER(ctx);
-  cudaStream_t st = ctx->stream;
   double4 *d_pts, *d_out;
   int* d_idx;
   double* d_tab;
@@ -196,12 +195,8 @@ extern "C" gb_status gb_deskew(gb_ctx* ctx, const double T_imu_lidar[16], const 
     d_tab = cv.take<double>(16 * (m + 1));  // the table, then T_post
   }));
   double* d_post = T_post ? d_tab + 16 * m : nullptr;
-  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * n, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(d_idx, idx.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(d_tab, table.data(), sizeof(double) * 16 * m, cudaMemcpyHostToDevice, st));
-  if (T_post) GB_CUDA(cudaMemcpyAsync(d_post, T_post, sizeof(double) * 16, cudaMemcpyHostToDevice, st));
+  GB_CHECK(gb_upload(ctx, {{d_pts, xyzw, sizeof(double4) * n}, {d_idx, idx.data(), sizeof(int) * n}, {d_tab, table.data(), sizeof(double) * 16 * m},
+                           {d_post, T_post, sizeof(double) * 16}}));
   GB_CHECK(gb_launch(ctx, "k_deskew", k_deskew, (unsigned)((n + 255) / 256), 256, 0, (int)n, d_pts, d_idx, d_tab, d_post, d_out));
-  GB_CUDA(cudaMemcpyAsync(out_xyzw, d_out, sizeof(double4) * n, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));  // idx / table are locals; out_xyzw is the caller's
-  return GB_OK;
+  return gb_download(ctx, {{out_xyzw, d_out, sizeof(double4) * n}});
 }

@@ -5,6 +5,7 @@
 #include <stddef.h>
 #include <cassert>
 #include <atomic>
+#include <initializer_list>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -365,6 +366,15 @@ struct gb_dev_block {
   template <typename T> void hand_over(T*& field) { void* old = field; field = (T*)base; base = old; }
 };
 gb_status gb_arena_reserve(gb_ctx* ctx, gb_arena& a, size_t bytes);  // a.base holds at least `bytes` afterwards
+// The host transfers of an entry point: gb_xfer parts, each one copy on ctx->stream straight between a device array and a
+// host array (skipped when the host pointer is null or the size zero).  gb_upload makes the H2D copies and does not
+// synchronise; gb_download makes the D2H copies, then one cudaStreamSynchronize.  A call that uploads ends with a download,
+// whose synchronisation is the last read of its host arrays: a pinned caller array is read after gb_upload has returned.
+// A call that fails between the two leaves those copies pending until gb_ctx_synchronize or the context's next call that
+// synchronises.  Staging through ctx->pinned instead was slower: see DESIGN.md §2 (scripts/ab_host_transfers.py).
+struct gb_xfer { void* dst; const void* src; size_t bytes; };
+gb_status gb_upload(gb_ctx* ctx, std::initializer_list<gb_xfer> parts);
+gb_status gb_download(gb_ctx* ctx, std::initializer_list<gb_xfer> parts);
 // the parameter bounds of gb_vgicp_align (gb_align.cu), shared by gb_ct_gicp_align
 gb_status gb_align_params_check(const gb_align_params* prm);
 // The round loop of gb_vgicp_align and gb_ct_gicp_align.  round(need_lin) launches one round for every problem: the
@@ -523,15 +533,13 @@ enum { GB_MODE_LINEARIZE = 0, GB_MODE_ERROR = 1 };
 gb_status gb_launch_sweep(gb_sweep* s, int mode);
 gb_status gb_launch_gicp_sweep(gb_sweep* s, int mode);  // gb_launch_sweep of a GICP sweep
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count);
-// Shared with gb_merge_frames (gb_kernels_preprocess.cu): one frame's points q = R a + t and covariances R C R^T in
-// un-contracted fp64, in the caller's point order (pts: n x double4, cov6: n x 6 upper triangle).  d_frame: GB_FRAME_DESC_BYTES
-// of device scratch for the frame descriptor.  One launch.
-#define GB_FRAME_DESC_BYTES 256
-gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T_colmajor, void* d_frame, double4* pts, double* cov6);
-// The same for K frames at poses (K x 16, column-major) in one launch, frame-major and each frame in its original point order:
-// h_frames (pinned) and d_frames hold K x GB_FRAME_DESC_BYTES for the descriptor table.  Shared by gb_merge_frames and
-// gb_concat_frames (gb_kernels_segment.cu).  No launch when the frames hold no point.
-gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, void* h_frames, void* d_frames, double4* pts, double* cov6);
+// The frame transform of gb_merge_frames (gb_kernels_preprocess.cu), shared with the map insert and gb_concat_frames
+// (gb_kernels_segment.cu): the points q = R a + t and covariances R C R^T in un-contracted fp64 of K frames at poses (K x 16,
+// column-major), frame-major and each frame in its original point order (pts: total x double4, cov6: total x 6 upper
+// triangle).  gb_frame_table writes the frames' descriptor table on the host; the caller uploads it to d_table and
+// gb_transform_frames launches over the frames' `total` points: one launch, none when total is 0.
+std::vector<char> gb_frame_table(size_t K, const gb_cloud* const* frames, const double* poses);
+gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const void* d_table, int total, double4* pts, double* cov6);
 // The exact k-NN of gb_preprocess and gb_find_neighbors (gb_kernels_preprocess.cu), shared with gb_min_cut: the k nearest of
 // the first *d_count points of d_pts (device resident, n slots) to each of them, by un-contracted fp64 d2 with ties to the
 // smaller index, the query included, in neighbors[i * k + j]; the row of a point whose cell of h0 leaves the 21-bit range, or

@@ -610,32 +610,11 @@ extern "C" gb_status gb_ct_deskew(gb_ctx* ctx, const gb_cloud* source, const dou
     d_nb = cv.take<int>(n * (size_t)kc);
     d_cnt = cv.take<int>(1);
   }));
-  // pinned: poses | neighbours (staged up) | the requested host outputs (staged down)
-  double *h_XY, *h_pts, *h_cov, *h_nrm;
-  int* h_nb;
-  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) {
-    h_XY = cv.take<double>(32);
-    h_nb = cv.take<int>(n * (size_t)kc);
-    h_pts = out_xyzw ? cv.take<double>(4 * n) : nullptr;
-    h_cov = out_cov4x4 ? cv.take<double>(16 * n) : nullptr;
-    h_nrm = out_normals4 ? cv.take<double>(4 * n) : nullptr;
-  }));
-  memcpy(h_XY, X, sizeof(double) * 16);
-  memcpy(h_XY + 16, Y, sizeof(double) * 16);
-  memcpy(h_nb, neighbors, sizeof(int) * n * (size_t)kc);
-  cudaStream_t st = ctx->stream;
-  GB_CUDA(cudaMemcpyAsync(d_XY, h_XY, sizeof(double) * 32, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(d_nb, h_nb, sizeof(int) * n * (size_t)kc, cudaMemcpyHostToDevice, st));
+  GB_CHECK(gb_upload(ctx, {{d_XY, X, sizeof(double) * 16}, {d_XY + 16, Y, sizeof(double) * 16}, {d_nb, neighbors, sizeof(int) * n * (size_t)kc}}));
   const int M = (int)n;
   GB_CHECK(gb_launch(ctx, "k_ct_deskew", k_ct_deskew, (M + 255) / 256, 256, 0, M, source->p0, source->perm, source->t_starts, source->t_tau, source->num_entries, d_XY, d_pts, d_cnt));
   GB_CHECK(gb_covariance_cloud(ctx, M, d_cnt, d_pts, d_nb, kc, k, d_nrm, d_cov, staged, t, c.get()));
-  if (h_pts) GB_CUDA(cudaMemcpyAsync(h_pts, d_pts, sizeof(double4) * n, cudaMemcpyDeviceToHost, st));
-  if (h_cov) GB_CUDA(cudaMemcpyAsync(h_cov, d_cov, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, st));
-  if (h_nrm) GB_CUDA(cudaMemcpyAsync(h_nrm, d_nrm, sizeof(double4) * n, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  if (out_xyzw) memcpy(out_xyzw, h_pts, sizeof(double) * 4 * n);
-  if (out_cov4x4) memcpy(out_cov4x4, h_cov, sizeof(double) * 16 * n);
-  if (out_normals4) memcpy(out_normals4, h_nrm, sizeof(double) * 4 * n);
+  GB_CHECK(gb_download(ctx, {{out_xyzw, d_pts, sizeof(double4) * n}, {out_cov4x4, d_cov, sizeof(double) * 16 * n}, {out_normals4, d_nrm, sizeof(double4) * n}}));
   if (out_cloud) *out_cloud = c.release();
   return GB_OK;
 }

@@ -465,14 +465,9 @@ extern "C" gb_status gb_fpfh_match(gb_ctx* ctx, const gb_cloud* target, const gb
   const size_t ns = source->n;
   if (ns == 0) return GB_OK;
   int* d_nearest = nullptr;
-  int* h_nearest = nullptr;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) { d_nearest = cv.take<int>(ns); }));
-  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h_nearest = cv.take<int>(ns); }));
   GB_CHECK(match_launch(ctx, target, source, d_nearest));
-  GB_CUDA(cudaMemcpyAsync(h_nearest, d_nearest, sizeof(int) * ns, cudaMemcpyDeviceToHost, ctx->stream));
-  GB_CUDA(cudaStreamSynchronize(ctx->stream));
-  memcpy(nearest, h_nearest, sizeof(int) * ns);
-  return GB_OK;
+  return gb_download(ctx, {{nearest, d_nearest, sizeof(int) * ns}});
 }
 
 extern "C" gb_status gb_ransac_default_params(gb_ransac_params* p) {

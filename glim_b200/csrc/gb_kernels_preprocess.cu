@@ -119,7 +119,6 @@ extern "C" gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, c
       GB_REQUIRE(q >= 0 && (size_t)q < n, "neighbour index out of range [0, n)");
     }
   GB_ENTER(ctx);
-  cudaStream_t st = ctx->stream;
   double4 *d_pts, *d_nrm;
   int *d_nb, *d_cnt;
   double* d_cov;
@@ -131,14 +130,9 @@ extern "C" gb_status gb_covariances(gb_ctx* ctx, size_t n, const double* xyzw, c
     d_cnt = cv.take<int>(1);
   }));
   const int count = (int)n;
-  GB_CUDA(cudaMemcpyAsync(d_cnt, &count, sizeof(int), cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * n, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(d_nb, neighbors, sizeof(int) * n * k_correspondences, cudaMemcpyHostToDevice, st));
+  GB_CHECK(gb_upload(ctx, {{d_cnt, &count, sizeof(int)}, {d_pts, xyzw, sizeof(double4) * n}, {d_nb, neighbors, sizeof(int) * n * k_correspondences}}));
   GB_CHECK(gb_covariance_cloud(ctx, count, d_cnt, d_pts, d_nb, k_correspondences, k_neighbors, d_nrm, d_cov, gb_planes{}, gb_sort_tmp{}, nullptr));
-  GB_CUDA(cudaMemcpyAsync(normals4, d_nrm, sizeof(double4) * n, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaMemcpyAsync(cov4x4, d_cov, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  return GB_OK;
+  return gb_download(ctx, {{normals4, d_nrm, sizeof(double4) * n}, {cov4x4, d_cov, sizeof(double) * 16 * n}});
 }
 
 extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* xyzw, const double* times, const double* intensities, double resolution, double* out_xyzw, double* out_times, double* out_intensities, size_t* num_out) {
@@ -147,7 +141,6 @@ extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* 
   if (n == 0) return GB_OK;
   GB_REQUIRE(xyzw && out_xyzw && resolution > 0.0, "null argument");
   GB_ENTER(ctx);
-  cudaStream_t st = ctx->stream;
   const size_t cub_b = gb_cub_temp_bytes(n);
   gb_sort_tmp t;
   double4 *d_pts, *d_opts;
@@ -165,22 +158,18 @@ extern "C" gb_status gb_voxelgrid_sampling(gb_ctx* ctx, size_t n, const double* 
     d_pos = cv.take<int>(n + 1);
     d_starts = cv.take<int>(n + 1);
   }));
-  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * n, cudaMemcpyHostToDevice, st));
-  if (times) GB_CUDA(cudaMemcpyAsync(d_t, times, sizeof(double) * n, cudaMemcpyHostToDevice, st));
-  if (intensities) GB_CUDA(cudaMemcpyAsync(d_i, intensities, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  GB_CHECK(gb_upload(ctx, {{d_pts, xyzw, sizeof(double4) * n}, {d_t, times, sizeof(double) * n}, {d_i, intensities, sizeof(double) * n}}));
   GB_CHECK(gb_grid_keys(ctx, (int)n, d_pts, 1.0 / resolution, nullptr, t.keys, t.idx));
   GB_CHECK(gb_group_by_key(ctx, (int)n, t, d_flags, d_pos));
   int V = 0;
-  GB_CUDA(cudaMemcpyAsync(&V, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
+  GB_CHECK(gb_download(ctx, {{&V, d_pos + (n - 1), sizeof(int)}}));
   if (V > 0) {
     GB_CHECK(gb_group_starts(ctx, (int)n, t, d_flags, d_pos, d_starts));
     GB_CHECK(gb_launch(ctx, "k_grid_means_counted", k_grid_means_counted, (n + 127) / 128, 128, 0, d_pos + (n - 1), d_starts, t.idx_s, d_pts, times ? d_t : nullptr,
                        intensities ? d_i : nullptr, nullptr, d_opts, d_ot, d_oi, nullptr));
-    GB_CUDA(cudaMemcpyAsync(out_xyzw, d_opts, sizeof(double4) * (size_t)V, cudaMemcpyDeviceToHost, st));
-    if (times && out_times) GB_CUDA(cudaMemcpyAsync(out_times, d_ot, sizeof(double) * (size_t)V, cudaMemcpyDeviceToHost, st));
-    if (intensities && out_intensities) GB_CUDA(cudaMemcpyAsync(out_intensities, d_oi, sizeof(double) * (size_t)V, cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
+    const size_t v = (size_t)V;
+    GB_CHECK(gb_download(ctx, {{out_xyzw, d_opts, sizeof(double4) * v}, {times ? out_times : nullptr, d_ot, sizeof(double) * v},
+                               {intensities ? out_intensities : nullptr, d_oi, sizeof(double) * v}}));
   }
   *num_out = (size_t)V;
   return GB_OK;
@@ -580,9 +569,7 @@ static gb_status preprocess(gb_ctx* ctx, size_t n_, const double* xyzw, const do
   }));
   const int tb = 256, gb = (n + tb - 1) / tb;
 
-  GB_CUDA(cudaMemcpyAsync(d_raw, xyzw, sizeof(double4) * N, cudaMemcpyHostToDevice, st));
-  if (times) GB_CUDA(cudaMemcpyAsync(d_t, times, sizeof(double) * N, cudaMemcpyHostToDevice, st));
-  if (intensities) GB_CUDA(cudaMemcpyAsync(d_i, intensities, sizeof(double) * N, cudaMemcpyHostToDevice, st));
+  GB_CHECK(gb_upload(ctx, {{d_raw, xyzw, sizeof(double4) * N}, {d_t, times, sizeof(double) * N}, {d_i, intensities, sizeof(double) * N}}));
   GB_CUDA(cudaMemsetAsync(d_cnt, 0, 256, st));
   GB_CHECK(gb_launch(ctx, "k_set_int", k_set_int, 1, 1, 0, d_cnt + 0, n));
 
@@ -643,35 +630,19 @@ static gb_status preprocess(gb_ctx* ctx, size_t n_, const double* xyzw, const do
   GB_CHECK(knn_device(ctx, n, frame_cnt, d_fr, k, h0, d_nb, knn));
   // ---- the frame's point count (the one host synchronisation before the results) ----
   int M = 0;
-  GB_CUDA(cudaMemcpyAsync(&M, frame_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
+  GB_CHECK(gb_download(ctx, {{&M, frame_cnt, sizeof(int)}}));
   out->num_points = (size_t)M;
+  out->last_time = 0.0;
+  if (M == 0) return GB_OK;
   // ---- covariances, written straight into the staged fp32 planes of the cloud (PointCloudGPU::clone on the device) ----
-  if (P->estimate_covariances && M > 0)  // the frame is gathered: t is free again
+  if (P->estimate_covariances)  // the frame is gathered: t is free again
     GB_CHECK(gb_covariance_cloud(ctx, M, frame_cnt, d_fr, d_nb, k, P->k_neighbors_cov > 0 ? P->k_neighbors_cov : k, d_nrm, d_cov, staged, t, cloud_out));
-  // ---- host products: D2H into the context's pinned staging (full PCIe rate), then one memcpy each into the caller's arrays ----
-  if (M > 0) {
-    const size_t m = (size_t)M;
-    const bool cov_out = P->estimate_covariances != 0;
-    struct Part { void* dst; const void* src; size_t bytes; char* staged; };
-    Part parts[6] = {{out->xyzw, d_fr, sizeof(double4) * m}, {out->times, d_frt, sizeof(double) * m}, {(out->intensities && intensities) ? out->intensities : nullptr, d_fri, sizeof(double) * m},
-                     {out->neighbors, d_nb, sizeof(int) * m * (size_t)k}, {(cov_out ? out->normals4 : nullptr), d_nrm, sizeof(double4) * m}, {(cov_out ? out->cov4x4 : nullptr), d_cov, sizeof(double) * 16 * m}};
-    double* h_last_time = nullptr;
-    GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) {
-      h_last_time = cv.take<double>(1);
-      for (Part& q : parts) q.staged = q.dst ? cv.take<char>(q.bytes) : nullptr;
-    }));
-    GB_CUDA(cudaMemcpyAsync(h_last_time, d_frt + (M - 1), sizeof(double), cudaMemcpyDeviceToHost, st));
-    for (const Part& q : parts)
-      if (q.dst) GB_CUDA(cudaMemcpyAsync(q.staged, q.src, q.bytes, cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    out->last_time = *h_last_time;
-    for (const Part& q : parts)
-      if (q.dst) memcpy(q.dst, q.staged, q.bytes);
-  } else {
-    out->last_time = 0.0;
-  }
-  return GB_OK;
+  // ---- host products ----
+  const size_t m = (size_t)M;
+  const bool cov_out = P->estimate_covariances != 0;
+  return gb_download(ctx, {{&out->last_time, d_frt + (M - 1), sizeof(double)}, {out->xyzw, d_fr, sizeof(double4) * m}, {out->times, d_frt, sizeof(double) * m},
+                           {intensities ? out->intensities : nullptr, d_fri, sizeof(double) * m}, {out->neighbors, d_nb, sizeof(int) * m * (size_t)k},
+                           {cov_out ? out->normals4 : nullptr, d_nrm, sizeof(double4) * m}, {cov_out ? out->cov4x4 : nullptr, d_cov, sizeof(double) * 16 * m}});
 }
 
 extern "C" gb_status gb_preprocess_default_params(gb_preprocess_params* p) {
@@ -719,7 +690,6 @@ extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n_, const double* xyz
   GB_REQUIRE(gb_knn_instantiated(k), "k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
   GB_ENTER(ctx);
   const int n = (int)n_;
-  cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n, cub_b = gb_cub_temp_bytes(N);
   KnnTmp knn;
   int *d_cnt, *d_nb;
@@ -730,12 +700,10 @@ extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n_, const double* xyz
     d_pts = cv.take<double4>(N);
     d_nb = cv.take<int>(N * (size_t)k);
   }));
-  GB_CUDA(cudaMemcpyAsync(d_pts, xyzw, sizeof(double4) * N, cudaMemcpyHostToDevice, st));
+  GB_CHECK(gb_upload(ctx, {{d_pts, xyzw, sizeof(double4) * N}}));
   GB_CHECK(gb_launch(ctx, "k_set_int", k_set_int, 1, 1, 0, d_cnt, n));
   GB_CHECK(knn_device(ctx, n, d_cnt, d_pts, k, 0.25, d_nb, knn));
-  GB_CUDA(cudaMemcpyAsync(neighbors, d_nb, sizeof(int) * N * (size_t)k, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  return GB_OK;
+  return gb_download(ctx, {{neighbors, d_nb, sizeof(int) * N * (size_t)k}});
 }
 
 // =============================================================================================
@@ -802,27 +770,20 @@ static MergeFrame merge_frame(const gb_cloud* c, const double* T, int offset) {
   return F;
 }
 
-static_assert(sizeof(MergeFrame) <= GB_FRAME_DESC_BYTES, "frame descriptor scratch");
-gb_status gb_transform_frame(gb_ctx* ctx, const gb_cloud* c, const double* T, void* d_frame, double4* pts, double* cov6) {
-  MergeFrame* h = nullptr;
-  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h = cv.take<MergeFrame>(1); }));
-  *h = merge_frame(c, T, 0);
-  GB_CUDA(cudaMemcpyAsync(d_frame, h, sizeof(MergeFrame), cudaMemcpyHostToDevice, ctx->stream));
-  const int n = (int)c->n;
-  return gb_launch(ctx, "k_merge_transform", k_merge_transform, (n + 255) / 256, 256, 0, 1, (const MergeFrame*)d_frame, n, pts, cov6);
-}
-
-gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, void* h_frames, void* d_frames, double4* pts, double* cov6) {
-  MergeFrame* h = (MergeFrame*)h_frames;
+std::vector<char> gb_frame_table(size_t K, const gb_cloud* const* frames, const double* poses) {
+  std::vector<char> table(sizeof(MergeFrame) * K);
   size_t total = 0;
   for (size_t k = 0; k < K; k++) {
-    h[k] = merge_frame(frames[k], poses + k * 16, (int)total);
+    const MergeFrame F = merge_frame(frames[k], poses + k * 16, (int)total);
+    memcpy(table.data() + sizeof(MergeFrame) * k, &F, sizeof(F));
     total += frames[k]->n;
   }
+  return table;
+}
+
+gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const void* d_table, int total, double4* pts, double* cov6) {
   if (total == 0) return GB_OK;
-  GB_CUDA(cudaMemcpyAsync(d_frames, h, sizeof(MergeFrame) * K, cudaMemcpyHostToDevice, ctx->stream));
-  const int n = (int)total;
-  return gb_launch(ctx, "k_merge_transform", k_merge_transform, (n + 255) / 256, 256, 0, (int)K, (const MergeFrame*)d_frames, n, pts, cov6);
+  return gb_launch(ctx, "k_merge_transform", k_merge_transform, (total + 255) / 256, 256, 0, (int)K, (const MergeFrame*)d_table, total, pts, cov6);
 }
 
 static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out) {
@@ -833,17 +794,18 @@ static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames,
   if (total == 0) return GB_OK;
   const int n = (int)total;
   const size_t N = total, cub_b = gb_cub_temp_bytes(N);
+  const std::vector<char> table = gb_frame_table((size_t)K, frames, poses);
   gb_planes staged;  // fp32 planes of the merged cloud, in output order
   gb_sort_tmp t;
   int *d_cnt, *d_flags, *d_pos, *d_starts, *d_keep;
-  MergeFrame* d_mf;
+  char* d_table;
   double4 *d_pts, *d_vpts;
   double *d_cov, *d_vcov, *d_ocov;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     staged = gb_cloud_planes(cv, N, false);
     t = gb_take_sort_tmp(cv, N, cv.take<char>(cub_b), cub_b);
     d_cnt = cv.take<int>(64);
-    d_mf = cv.take<MergeFrame>((size_t)K);
+    d_table = cv.take<char>(table.size());
     d_pts = cv.take<double4>(N);
     d_vpts = cv.take<double4>(N);
     d_cov = cv.take<double>(6 * N);
@@ -854,11 +816,10 @@ static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames,
     d_starts = cv.take<int>(N + 1);
     d_keep = cv.take<int>(N + 1);
   }));
-  MergeFrame* h_mf = nullptr;
-  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h_mf = cv.take<MergeFrame>((size_t)K); }));
   GB_CUDA(cudaMemsetAsync(d_cnt, 0, 256, st));
   const int tb = 256, gb = (n + tb - 1) / tb;
-  GB_CHECK(gb_transform_frames(ctx, (size_t)K, frames, poses, h_mf, d_mf, d_pts, d_cov));
+  GB_CHECK(gb_upload(ctx, {{d_table, table.data(), table.size()}}));
+  GB_CHECK(gb_transform_frames(ctx, (size_t)K, d_table, n, d_pts, d_cov));
   GB_CHECK(gb_grid_keys(ctx, n, d_pts, 1.0 / resolution, nullptr, t.keys, t.idx));
   GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
   GB_CHECK(gb_launch(ctx, "k_copy_last_pos", k_copy_last_pos, 1, 1, 0, n, d_pos, d_cnt));  // V
@@ -869,16 +830,12 @@ static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames,
   GB_CHECK(gb_thin(ctx, n, nullptr, d_cnt, target, seed, t, d_keep));
   GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_keep, d_pos, n);
   int M = 0;
-  GB_CUDA(cudaMemcpyAsync(&M, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
+  GB_CHECK(gb_download(ctx, {{&M, d_pos + (n - 1), sizeof(int)}}));
   *num_out = (size_t)M;
   if (M == 0) return GB_OK;
   GB_CHECK(gb_launch(ctx, "k_merge_emit", k_merge_emit, gb, tb, 0, n, d_keep, d_pos, d_vpts, d_vcov, d_pts /* reused: emitted points */, d_ocov, staged.p0, staged.p1, staged.p2));
   if (cloud_out) GB_CHECK(gb_cloud_build(ctx, cloud_out, (size_t)M, staged, t));
-  if (out_xyzw) GB_CUDA(cudaMemcpyAsync(out_xyzw, d_pts, sizeof(double4) * (size_t)M, cudaMemcpyDeviceToHost, st));
-  if (out_cov4x4) GB_CUDA(cudaMemcpyAsync(out_cov4x4, d_ocov, sizeof(double) * 16 * (size_t)M, cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  return GB_OK;
+  return gb_download(ctx, {{out_xyzw, d_pts, sizeof(double4) * (size_t)M}, {out_cov4x4, d_ocov, sizeof(double) * 16 * (size_t)M}});
 }
 
 extern "C" gb_status gb_merge_frames(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, double resolution, int target, uint64_t seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud** out_cloud) {

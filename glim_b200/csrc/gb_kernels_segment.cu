@@ -474,37 +474,9 @@ extern "C" gb_status gb_concat_frames(gb_ctx* ctx, size_t K, const gb_cloud* con
   }
   const int n = (int)total;
   const size_t N = total, cub_b = gb_cub_temp_bytes(N);
-  gb_planes staged;
-  gb_sort_tmp t;
-  void* d_table;
-  ConcatFrame* d_frames;
-  int *d_offsets, *d_flags, *d_pos;
-  double4* d_pts;
-  double* d_cov;
-  unsigned long long* d_ids;
-  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
-    staged = gb_cloud_planes(cv, N, normals);
-    t = gb_take_sort_tmp(cv, N, cv.take<char>(cub_b), cub_b);
-    d_table = cv.take<char>(K * GB_FRAME_DESC_BYTES);
-    d_frames = cv.take<ConcatFrame>(K);
-    d_offsets = cv.take<int>(K);
-    d_flags = cv.take<int>(N);
-    d_pos = cv.take<int>(N);
-    d_pts = cv.take<double4>(N);
-    d_cov = cv.take<double>(6 * N);
-    d_ids = cv.take<unsigned long long>(N);
-  }));
-  void* h_table;
-  ConcatFrame* h_frames;
-  int *h_offsets, *h_count;
-  unsigned long long* h_ids = nullptr;
-  GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) {
-    h_table = cv.take<char>(K * GB_FRAME_DESC_BYTES);
-    h_frames = cv.take<ConcatFrame>(K);
-    h_offsets = cv.take<int>(K);
-    h_count = cv.take<int>(1);
-    if (ids) h_ids = cv.take<unsigned long long>(N);
-  }));
+  const std::vector<char> table = gb_frame_table(K, frames, poses);
+  std::vector<ConcatFrame> h_frames(K);
+  std::vector<int> h_offsets(K);
   size_t off = 0;
   for (size_t k = 0; k < K; k++) {
     const double* T = poses + 16 * k;
@@ -515,10 +487,28 @@ extern "C" gb_status gb_concat_frames(gb_ctx* ctx, size_t K, const gb_cloud* con
     h_offsets[k] = (int)off;
     off += frames[k]->n;
   }
-  cudaStream_t st = ctx->stream;
-  GB_CUDA(cudaMemcpyAsync(d_frames, h_frames, sizeof(ConcatFrame) * K, cudaMemcpyHostToDevice, st));
-  GB_CUDA(cudaMemcpyAsync(d_offsets, h_offsets, sizeof(int) * K, cudaMemcpyHostToDevice, st));
-  GB_CHECK(gb_transform_frames(ctx, K, frames, poses, h_table, d_table, d_pts, d_cov));
+  gb_planes staged;
+  gb_sort_tmp t;
+  char* d_table;
+  ConcatFrame* d_frames;
+  int *d_offsets, *d_flags, *d_pos;
+  double4* d_pts;
+  double* d_cov;
+  unsigned long long* d_ids;
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+    staged = gb_cloud_planes(cv, N, normals);
+    t = gb_take_sort_tmp(cv, N, cv.take<char>(cub_b), cub_b);
+    d_table = cv.take<char>(table.size());
+    d_frames = cv.take<ConcatFrame>(K);
+    d_offsets = cv.take<int>(K);
+    d_flags = cv.take<int>(N);
+    d_pos = cv.take<int>(N);
+    d_pts = cv.take<double4>(N);
+    d_cov = cv.take<double>(6 * N);
+    d_ids = cv.take<unsigned long long>(N);
+  }));
+  GB_CHECK(gb_upload(ctx, {{d_frames, h_frames.data(), sizeof(ConcatFrame) * K}, {d_offsets, h_offsets.data(), sizeof(int) * K}, {d_table, table.data(), table.size()}}));
+  GB_CHECK(gb_transform_frames(ctx, K, d_table, n, d_pts, d_cov));
   const int gb = (n + kSegThreads - 1) / kSegThreads;
   const double inv = window ? 1.0 / window->cell_size : 0.0;
   const int3 lo = window ? make_int3(window->lo[0], window->lo[1], window->lo[2]) : make_int3(0, 0, 0);
@@ -527,14 +517,12 @@ extern "C" gb_status gb_concat_frames(gb_ctx* ctx, size_t K, const gb_cloud* con
   GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_flags, d_pos, n);
   GB_CHECK(gb_launch(ctx, "k_concat_emit", k_concat_emit, gb, kSegThreads, 0, n, (int)K, d_offsets, d_frames, d_flags, d_pos, d_pts, d_cov, covs ? 1 : 0,
                      staged.p0, staged.p1, staged.p2, staged.normals, d_ids));
-  GB_CUDA(cudaMemcpyAsync(h_count, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-  GB_CUDA(cudaStreamSynchronize(st));
-  const size_t M = (size_t)*h_count;
+  int count = 0;
+  GB_CHECK(gb_download(ctx, {{&count, d_pos + (n - 1), sizeof(int)}}));
+  const size_t M = (size_t)count;
   if (M > 0) {
     GB_CHECK(gb_cloud_build(ctx, c.get(), M, staged, t));
-    if (ids) GB_CUDA(cudaMemcpyAsync(h_ids, d_ids, sizeof(unsigned long long) * M, cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
-    if (ids) memcpy(ids, h_ids, sizeof(uint64_t) * M);
+    GB_CHECK(gb_download(ctx, {{ids, d_ids, sizeof(uint64_t) * M}}));
   }
   *num_out = M;
   *out_cloud = c.release();

@@ -191,8 +191,7 @@ static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dr
       GB_CHECK(gb_launch(ctx, "k_table_insert", k_table_insert, (V + 255) / 256, 256, 0, V, d_vcoord, buckets, (uint32_t)nb - 1u, max_scan, d_dropped));
     }
     GB_CHECK(gb_launch(ctx, "k_table_finalize", k_table_finalize, (nb + 255) / 256, 256, 0, nb, d_vcoord, buckets));
-    if (V > 0) GB_CUDA(cudaMemcpyAsync(&dropped, d_dropped, sizeof(int), cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
+    GB_CHECK(gb_download(ctx, {{&dropped, d_dropped, V > 0 ? sizeof(int) : 0}}));
     *num_buckets = nb;
     *num_dropped_points = dropped;
     if ((double)dropped <= drop_rate * total_points || nb >= (1 << 28)) {
@@ -225,9 +224,7 @@ static gb_status group_cloud(gb_ctx* ctx, const gb_cloud* cloud, float inv_res, 
   }));
   GB_CHECK(gb_launch(ctx, "k_point_keys", k_point_keys, (n + 255) / 256, 256, 0, n, cloud->p0, cloud->inv_perm, inv_res, g.t.keys, g.t.idx));
   GB_CHECK(gb_group_by_key(ctx, n, g.t, g.flags, g.pos));
-  GB_CUDA(cudaMemcpyAsync(&g.V, g.pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  GB_CUDA(cudaStreamSynchronize(ctx->stream));
-  return GB_OK;
+  return gb_download(ctx, {{&g.V, g.pos + (n - 1), sizeof(int)}});
 }
 
 // (the caller has made the map's device current)
@@ -277,7 +274,7 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
 // One insert is one pass over (the map's stored entries, the frame's points), the same steps for both kinds:
 //   1. old keys            the stored entries, tagged old (idx = -1 - entry), ahead of the points: one per voxel
 //                          (k_ins_old_keys) or one per stored iVox point (k_ivox_old_keys)
-//   2. k_merge_transform   (gb_transform_frame, shared with gb_merge_frames) q = R a + t, R C R^T in un-contracted fp64
+//   2. k_merge_transform   (gb_transform_frames, shared with gb_merge_frames) q = R a + t, R C R^T in un-contracted fp64
 //   3. k_grid_keys         (gb_grid_keys) packed floor(q * key_inv_res) in fp64; with sampling_rate < 1, gb_thin first keeps
 //                          the m points with the smallest rg_hash(seed, index) and the others get no key
 //   4. gb_group_by_key     stable: a voxel's group is its old entries first, then its new points in index order
@@ -473,7 +470,7 @@ struct InsertScratch {
   int *flags, *pos, *starts, *keep, *kpos, *dropped;
   int4* vcoord;
   unsigned long long* info;
-  void* frame;
+  char* frame;
   double4* pts = nullptr;
   double* cov = nullptr;
 };
@@ -558,7 +555,6 @@ struct IvoxRule {
 // Steps 1-8 for either kind; `rule` is the kind's per-voxel part.
 template <typename Rule>
 gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const double* T, double sampling_rate, unsigned long long seed, Rule rule) {
-  cudaStream_t st = ctx->stream;
   const int n = (int)cloud->n;
   const int No = (int)gb_stored_entries(m);
   const int kept = sampling_rate < 1.0 ? (int)(size_t)((double)n * sampling_rate) : n;  // random_sampling's count
@@ -570,6 +566,7 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
   gb_dev_block table(ctx->device), base(ctx->device);  // the new blocks until the hand-over, then m's replaced ones (base ends first)
   if (N > 0) {
     const size_t cub_b = gb_cub_temp_bytes((size_t)N);
+    const std::vector<char> frame = gb_frame_table(1, &cloud, T);
     InsertScratch s;
     GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
       s.t = gb_take_sort_tmp(cv, (size_t)N, cv.take<char>(cub_b), cub_b);
@@ -581,16 +578,17 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
       s.vcoord = cv.take<int4>(N);
       s.dropped = cv.take<int>(1);
       s.info = cv.take<unsigned long long>(2);
-      s.frame = cv.take<char>(GB_FRAME_DESC_BYTES);
+      s.frame = cv.take<char>(frame.size());
       if (np > 0) {
         s.pts = cv.take<double4>(np);
         s.cov = cv.take<double>(6 * (size_t)np);
       }
       rule.scratch(cv, (size_t)N);
     }));
+    if (np > 0) GB_CHECK(gb_upload(ctx, {{s.frame, frame.data(), frame.size()}}));
     if (m->num_voxels > 0) GB_CHECK(rule.old_keys(ctx, s.t));
     if (np > 0) {
-      GB_CHECK(gb_transform_frame(ctx, cloud, T, s.frame, s.pts, s.cov));
+      GB_CHECK(gb_transform_frames(ctx, 1, s.frame, np, s.pts, s.cov));
       const int* sampled = nullptr;  // the sampling's keep flags (in s.keep until the merge writes it)
       if (kept < n) {
         gb_sort_tmp pt = s.t;  // the hashes pass through the points' keys, which k_grid_keys writes next
@@ -604,8 +602,7 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
     GB_CHECK(gb_group_starts(ctx, N, s.t, s.flags, s.pos, s.starts));
     GB_CHECK(rule.merge(ctx, s, N));
     unsigned long long info[2] = {0, 0};
-    GB_CUDA(cudaMemcpyAsync(info, s.info, sizeof(info), cudaMemcpyDeviceToHost, st));
-    GB_CUDA(cudaStreamSynchronize(st));
+    GB_CHECK(gb_download(ctx, {{info, s.info, sizeof(info)}}));
     const int V = (int)info[1];
     next.num_voxels = V;
     next.num_points = (size_t)info[0];
@@ -852,7 +849,7 @@ extern "C" gb_status gb_point_grid_build(gb_ctx* ctx, const gb_cloud* cloud, dou
     GB_CHECK(gb_group_starts(ctx, n, c.t, c.flags, c.pos, c.starts));
     GB_CHECK(gb_launch(ctx, "k_grid_emit", k_grid_emit, (n + 255) / 256, 256, 0, n, c.t.keys_s, c.t.idx_s, c.flags, c.pos, c.starts, cloud->p0, cloud->p1, cloud->p2,
                        cloud->inv_perm, g->voxels, g->cells, g->vkeys, c.vcoord, c.extent));
-    GB_CUDA(cudaMemcpyAsync(&g->key_extent, c.extent, sizeof(int), cudaMemcpyDeviceToHost, st));  // read by table_build's synchronisation
+    GB_CHECK(gb_download(ctx, {{&g->key_extent, c.extent, sizeof(int)}}));
   }
   GB_CHECK(table_build(ctx, c.V, c.vcoord, c.dropped, g->init_buckets, g->max_scan, 0.0, (double)n, table, &g->num_buckets, &g->num_dropped_points));
   if (g->num_dropped_points != 0) {

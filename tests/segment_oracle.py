@@ -114,14 +114,14 @@ def region_growing(xyz, nrm, seed_point, distance_threshold, angle_threshold, di
 
 
 def transform_points(T, a):
-    """q = R a + t in gb_transform_frame's order: ((T_r0 x + T_r1 y) + T_r2 z) + T_r3, fp64 from fp32 a"""
+    """q = R a + t in gb_transform_frames' order: ((T_r0 x + T_r1 y) + T_r2 z) + T_r3, fp64 from fp32 a"""
     a = np.asarray(a, F32).astype(F64)
     T = np.asarray(T, F64)
     return np.stack([((T[r, 0] * a[:, 0] + T[r, 1] * a[:, 1]) + T[r, 2] * a[:, 2]) + T[r, 3] for r in range(3)], axis=1)
 
 
 def transform_covs(T, cov6):
-    """R C R^T in gb_transform_frame's order, upper triangle (c00 c01 c02 c11 c12 c22), fp64 from the fp32 entries"""
+    """R C R^T in gb_transform_frames' order, upper triangle (c00 c01 c02 c11 c12 c22), fp64 from the fp32 entries"""
     c = np.asarray(cov6, F32).astype(F64)
     C = [[c[:, 0], c[:, 1], c[:, 2]], [c[:, 1], c[:, 3], c[:, 4]], [c[:, 2], c[:, 4], c[:, 5]]]
     T = np.asarray(T, F64)

@@ -11,6 +11,11 @@
    handle has one free function, which every destroy entry point and every failed creation calls.
 7. gb_dev_malloc is called only by gb_dev_carve, and gb_dev_free only by the pool block's owner (gb_dev_block) and the free
    functions: every pool block is taken by one carve and held by one owner until a handle takes it over.
+8. An asynchronous copy that may touch host memory (any cudaMemcpy*Async -- 1D, 2D, 3D, peer or symbol -- that is not
+   explicitly cudaMemcpyDeviceToDevice) appears only in gb_upload, gb_download and gb_align_rounds, and in the functions
+   listed below with their reasons: every other entry point moves its host arrays through the two helpers.  Every function
+   that carves the context's pinned arena synchronises its stream in its own body (a stream synchronisation, gb_download or
+   gb_align_rounds), or is listed with the callers that do, so no copy from the arena is pending when a call returns.
 
 The function bodies are found by brace matching on the sources with comments, strings and preprocessor lines removed."""
 import os
@@ -53,6 +58,32 @@ FREE_FUNCTIONS = {
     "pool_block_free": "a sweep block evicted from the context's pool, or not kept by it",
     "dev_block_realloc": "a sweep's pair CSR block and a peer slab's pair list, replaced when a slab is attached",
 }
+XFER_HELPERS = {"gb_upload", "gb_download", "gb_align_rounds"}
+# the only other functions that may copy between host and device asynchronously: each copies a pinned block of its own, or a
+# layout of the context's pinned arena that the helpers' one copy per array cannot express
+PINNED_COPIES = {
+    "gb_sweep_create": "the sweep's own pinned descriptors and items",
+    "gb_sweep_set_poses": "the sweep's own double-buffered pinned pose slots (no synchronisation)",
+    "gb_sweep_fetch": "the sweep's own pinned results",
+    "sweep_error": "the sweep's own pinned poses and results",
+    "sweep_linearize": "the sweep's own pinned poses and results, captured into its graph",
+    "sweep_learn_inliers": "the sweep's own pinned descriptors and items, re-uploaded when the items are re-sized",
+    "sweep_follow_targets": "the sweep's own pinned descriptors, re-uploaded when a target changed",
+    "gb_vgicp_align": "the align call's pinned block: states, offsets and poses written in place",
+    "ct_upload": "the CT call block: descriptors and poses written in place, one copy",
+    "ct_evaluate": "the CT call block's results",
+    "gb_ct_gicp_align": "the CT call block's states",
+    "gb_cloud_add_times": "the time table written in place in the pinned arena, one copy",
+    "gb_peer_slab_fetch_async": "the peer slab's own pinned fetch block",
+    "gb_overlap": "descriptors and poses adjacent in the pinned arena, one copy",
+    "gb_region_growing": "a result-word tail: how many entries are used depends on the word the same copy brings back",
+    "gb_min_cut": "a result-word tail: how many entries are used depends on the word the same copy brings back",
+    "gb_gnc_align": "a result-word tail: how many entries are used depends on the word the same copy brings back",
+    "gb_ransac_align": "per-block reads of the hypothesis counts into the pinned arena",
+    "cloud_upload": "the fp64 -> fp32 pack writes the pinned planes directly, with threads",
+}
+# functions that carve ctx->pinned and leave the synchronisation to their callers
+PINNED_SYNCED_BY_CALLER = {"ct_prepare": "the CT call block: ct_evaluate and gb_ct_gicp_align synchronise before they return"}
 
 
 def strip_source(text):
@@ -187,14 +218,37 @@ def pool_uses(code, funcs):
     return out
 
 
+def host_copies(code, funcs):
+    """[(pos, enclosing function)] of every asynchronous copy that may touch host memory (rule 8)."""
+    out = []
+    for m in re.finditer(r"\bcudaMemcpy\w*Async\s*\(", code):
+        if not re.search(r"\bcudaMemcpyDeviceToDevice\b", code[m.end():code.find(";", m.end())]):
+            out.append((m.start(), enclosing(funcs, m.start())))
+    return out
+
+
+def pinned_carvers(code, funcs):
+    """[(pos, function, synchronises in its body)] of every carve of a context's pinned arena (rule 8)."""
+    out = []
+    for m in re.finditer(r"\bgb_carve\s*\([^,;]+,\s*[\w.>-]*\bpinned\b", code):
+        name = enclosing(funcs, m.start())
+        b, e = next((b, e) for n, _, b, e in funcs if n == name)
+        out.append((m.start(), name, bool(re.search(r"\bcudaStreamSynchronize\s*\(|\bgb_download\s*\(|\bgb_align_rounds\s*\(", code[b:e]))))
+    return out
+
+
 def violations(csrc):
-    """{rule: [offending site]} for rules 1-7 of this module's docstring."""
-    bad = {1: [], 2: [], 3: [], 4: [], 5: [], 6: [], 7: []}
+    """{rule: [offending site]} for rules 1-8 of this module's docstring."""
+    bad = {1: [], 2: [], 3: [], 4: [], 5: [], 6: [], 7: [], 8: []}
     enters = 0
     for f, code, directives, funcs in sources(csrc):
         where = lambda pos: f"{f}:{line_of(code, pos)} ({enclosing(funcs, pos)})"
         bad[7] += [where(pos) for pos, _, allowed in pool_uses(code, funcs) if not allowed]
         bad[7] += [f"{f}: {d.splitlines()[0].strip()}" for d in directives if re.search(r"\bgb_dev_(malloc|free)\b", d)]
+        bad[8] += [where(pos) for pos, name in host_copies(code, funcs) if name not in XFER_HELPERS and name not in PINNED_COPIES]
+        bad[8] += [f"{f}: {d.splitlines()[0].strip()}" for d in directives if re.search(r"\bcudaMemcpy\w*Async\b", d)]
+        bad[8] += [where(pos) + " carves the pinned arena and does not synchronise" for pos, name, syncs in pinned_carvers(code, funcs)
+                   if not syncs and name not in PINNED_SYNCED_BY_CALLER]
         carver = struct_body(code, "Carver")
         for m in re.finditer(r"\balign_up\b", code):
             definition = re.search(r"\bsize_t\s+$", code[max(0, m.start() - 40):m.start()])
@@ -242,6 +296,7 @@ def parsed_inventory(csrc):
     """Sanity numbers of the parse, so that a rule cannot pass because the parser found nothing."""
     names, launches_in_helper, cub_calls, carver_align, frees = set(), 0, 0, 0, 0
     pool = {"malloc": 0, "free": 0}  # allowed uses of gb_dev_malloc / gb_dev_free (rule 7)
+    xfer = {"gb_upload": 0, "gb_download": 0, "copies": {}, "carvers": set()}  # the helpers' uses, the copies, the pinned carves (rule 8)
     for f, code, _, funcs in sources(csrc):
         names.update(n for n, *_ in funcs)
         launches_in_helper += sum(1 for m in re.finditer(r"<<<", code) if enclosing(funcs, m.start()) == "gb_launch")
@@ -252,11 +307,17 @@ def parsed_inventory(csrc):
         frees += sum(1 for m in re.finditer(r"\bdelete\b|\bcudaFree(Host)?\s*\(", code) if enclosing(funcs, m.start()) in FREE_FUNCTIONS)
         for _, kind, allowed in pool_uses(code, funcs):
             pool[kind] += allowed
-    return names, launches_in_helper, cub_calls, carver_align, frees, pool
+        for m in re.finditer(r"\b(gb_upload|gb_download)\s*\(", code):
+            if enclosing(funcs, m.start()) not in (None, m.group(1)):  # a call, not the declaration or the definition
+                xfer[m.group(1)] += 1
+        for _, name in host_copies(code, funcs):
+            xfer["copies"][name] = xfer["copies"].get(name, 0) + 1
+        xfer["carvers"] |= {name for _, name, _ in pinned_carvers(code, funcs)}
+    return names, launches_in_helper, cub_calls, carver_align, frees, pool, xfer
 
 
 def test_parser_sees_the_library():
-    names, launches_in_helper, cub_calls, carver_align, frees, pool = parsed_inventory(CSRC)
+    names, launches_in_helper, cub_calls, carver_align, frees, pool, xfer = parsed_inventory(CSRC)
     assert {"gb_launch", "sweep_linearize", "gb_preprocess", "gb_vgicp_align", "gb_deskew", "knn_device", "table_build", "gb_dev_carve"} <= names
     assert set(FREE_FUNCTIONS) <= names
     assert launches_in_helper == 1
@@ -265,6 +326,11 @@ def test_parser_sees_the_library():
     assert frees >= len(FREE_FUNCTIONS)
     # the carve's one allocation; the owner's free and those of cloud_free (3 blocks) and voxelmap_free (2)
     assert pool == {"malloc": 1, "free": 6}
+    # the helpers' calls; each listed site still copies, and each helper copies in one place
+    assert xfer["gb_upload"] >= 9 and xfer["gb_download"] >= 17
+    assert set(PINNED_COPIES) <= set(xfer["copies"])
+    assert all(xfer["copies"].get(h) == 1 for h in XFER_HELPERS)
+    assert set(PINNED_SYNCED_BY_CALLER) <= xfer["carvers"] and len(xfer["carvers"]) >= 8
     _, enters = violations(CSRC)
     assert enters >= 29  # gb_peer_slab_destroy is teardown now: peer_slab_free locks the context by hand
 
@@ -295,3 +361,7 @@ def test_handles_freed_only_by_their_free_functions():
 
 def test_pool_blocks_taken_by_one_carve_and_returned_by_one_owner():
     assert violations(CSRC)[0][7] == []
+
+
+def test_host_transfers_go_through_the_two_helpers():
+    assert violations(CSRC)[0][8] == []
