@@ -108,6 +108,13 @@ _SIGNATURES = {
     "gb_region_growing": ([vp, vp, vp, vp, vp, vp, vp], st),
     "gb_min_cut_default_params": ([vp], st),
     "gb_min_cut": ([vp, vp, vp, vp, vp, vp, vp, vp], st),
+    "gb_plane_patch_default_params": ([vp], st),
+    "gb_plane_patch": ([vp, sz, vp, vp, vp, vp, vp], st),
+    "gb_plane_auto_radius": ([vp, sz, vp, vp, vp, vp], st),
+    "gb_plane_evm_factor_create": ([vp, sz, vp, vp, vp, vp], st),
+    "gb_plane_evm_factor_info": ([vp, vp, vp, vp, vp], st),
+    "gb_plane_evm_linearize": ([vp, sz, vp, vp, vp, vp, vp, vp], st),
+    "gb_plane_evm_error": ([vp, sz, vp, vp, vp], st),
 }
 del vp, i32, f32, f64, sz, u64, st
 SYMBOLS = tuple(_SIGNATURES)  # tests check the library exports exactly these
@@ -216,6 +223,25 @@ class MinCutResult(C.Structure):
 # gb_min_cut_result::status
 MINCUT_FOUND, MINCUT_NO_SEED, MINCUT_NOT_CONVERGED = 0, 1, 2
 MINCUT_STATUS_NAMES = {0: "FOUND", 1: "NO_SEED", 2: "NOT_CONVERGED"}
+
+class PlanePatchParams(C.Structure):
+    """gb_plane_patch_params (include/glim_b200.h)."""
+    _fields_ = [("center", C.c_double * 3), ("radius", C.c_double), ("max_frame_distance", C.c_double), ("min_radius", C.c_double),
+                ("max_radius", C.c_double), ("plane_eps", C.c_double)]
+
+
+PLANE_MAX_TRIALS = 10
+
+
+class PlanePatchResult(C.Structure):
+    """gb_plane_patch_result (include/glim_b200.h)."""
+    _fields_ = [("radius", C.c_double), ("num_points", C.c_size_t), ("eigenvalues", C.c_double * 3), ("num_trials", C.c_int32),
+                ("trial_radius", C.c_double * PLANE_MAX_TRIALS), ("trial_points", C.c_size_t * PLANE_MAX_TRIALS)]
+
+
+# gb_plane_evm_linearize's status
+PLANE_EVM_OK, PLANE_EVM_DEGENERATE = 0, 1
+PLANE_EVM_STATUS_NAMES = {0: "OK", 1: "DEGENERATE"}
 
 # gb_ransac_result::status
 RANSAC_FOUND, RANSAC_EARLY_STOP, RANSAC_DEGENERATE = 0, 1, 2

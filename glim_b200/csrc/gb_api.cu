@@ -684,7 +684,8 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   uint64_t total_pts = 0;
   for (size_t f = 0; f < F; f++) {
     GB_REQUIRE(factors[f], "null factor");
-    GB_REQUIRE(factors[f]->kind != GB_FACTOR_CT, "a CT factor has two poses: only the gb_ct_* entry points take it");
+    GB_REQUIRE(factors[f]->kind == GB_FACTOR_POSE,
+               "not a pose factor: a CT factor has two poses (the gb_ct_* entry points), a plane factor one per key (gb_plane_evm_*)");
     GB_REQUIRE(factors[f]->source->device == ctx->device && factors[f]->target->device == ctx->device, "factor lives on another device");
     GB_REQUIRE(gb_factor_class(factors[f]) == gb_factor_class(factors[0]),
                "the factors of one sweep must all be VGICP factors, all GICP factors on iVoxes, all GICP factors on point grids or all ICP factors");

@@ -160,12 +160,14 @@ static_assert(sizeof(GicpDesc) == 16, "GicpDesc size");
 // a GICP factor's target part (gb_api.cu): the iVox's or point grid's table and point records in D, the rest in G
 void desc_target_gicp(FactorDesc& D, GicpDesc& G, const gb_factor* fa);
 
-// A factor is one of two kinds, fixed at creation.  A pose factor (gb_vgicp_factor_create, gb_gicp_factor_create) has one
+// A factor is one of three kinds, fixed at creation.  A pose factor (gb_vgicp_factor_create, gb_gicp_factor_create) has one
 // unknown pose and goes through sweeps; a CT factor (gb_ct_gicp_factor_create) has two and only the gb_ct_* entry points
-// take it: gb_sweep_create refuses it, and so every consumer of sweeps.
+// take it; a plane factor (gb_plane_evm_factor_create) has one per key and only the gb_plane_evm_* entry points take it.
+// gb_sweep_create takes pose factors only, and so every consumer of sweeps refuses the other kinds.
 enum gb_factor_kind {
   GB_FACTOR_POSE,
   GB_FACTOR_CT,
+  GB_FACTOR_PLANE_EVM,
 };
 struct gb_factor {
   gb_factor_kind kind = GB_FACTOR_POSE;
@@ -180,6 +182,12 @@ struct gb_factor {
   float inlier_frac = -1.f;    // inlier fraction of the last linearization (< 0: unknown) -- sizes the work items of the next sweep
   uint64_t id = 0;             // process-wide unique
   std::vector<gb_sweep*> users;  // sweeps (of any context) that reference this factor; guarded by the registry mutex
+  // A plane factor keeps everything on the host and borrows no cloud: per key the caller's frame index and the moments
+  // {N, mean, scatter} (GB_PLANE_MOMENTS doubles, gb_plane_math.cuh) of its points, the offset o and the point count.
+  std::vector<int32_t> plane_frames;
+  std::vector<double> plane_moments;
+  double plane_offset[3] = {0.0, 0.0, 0.0};
+  size_t plane_points = 0;
 };
 // The class of a pose factor: a sweep or call holds one.  gb_target_class's 0 (VGICP), 1 and 2 (GICP), or 3: ICP on point grids.
 inline int gb_factor_class(const gb_factor* f) { return f->icp ? 3 : gb_target_class(f->target); }
@@ -536,8 +544,8 @@ gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_de
 // The frame transform of gb_merge_frames (gb_kernels_preprocess.cu), shared with the map insert and gb_concat_frames
 // (gb_kernels_segment.cu): the points q = R a + t and covariances R C R^T in un-contracted fp64 of K frames at poses (K x 16,
 // column-major), frame-major and each frame in its original point order (pts: total x double4, cov6: total x 6 upper
-// triangle).  gb_frame_table writes the frames' descriptor table on the host; the caller uploads it to d_table and
-// gb_transform_frames launches over the frames' `total` points: one launch, none when total is 0.
+// triangle; nullptr: no covariances).  gb_frame_table writes the frames' descriptor table on the host; the caller uploads it
+// to d_table and gb_transform_frames launches over the frames' `total` points: one launch, none when total is 0.
 std::vector<char> gb_frame_table(size_t K, const gb_cloud* const* frames, const double* poses);
 gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const void* d_table, int total, double4* pts, double* cov6);
 // The exact k-NN of gb_preprocess and gb_find_neighbors (gb_kernels_preprocess.cu), shared with gb_min_cut: the k nearest of

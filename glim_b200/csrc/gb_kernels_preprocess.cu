@@ -736,6 +736,7 @@ __global__ void k_merge_transform(int num_frames, const MergeFrame* __restrict__
   double q[3];
   for (int r = 0; r < 3; r++) q[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[r * 4 + 0], x), __dmul_rn(T[r * 4 + 1], y)), __dmul_rn(T[r * 4 + 2], z)), T[r * 4 + 3]);
   pts[g] = make_double4(q[0], q[1], q[2], 1.0);
+  if (!cov6) return;
   const double C[9] = {a0.w, a1.x, a1.y, a1.x, a1.z, a1.w, a1.y, a1.w, a2};
   double RC[9];
   for (int r = 0; r < 3; r++)

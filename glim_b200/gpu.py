@@ -30,6 +30,10 @@ include/glim_b200/gtsam_points_compat.hpp.
                                                             GlobalMapping::export_points, global_mapping.cpp:638-680
     region_growing(cloud, seed_point, **params)             gtsam_points::region_growing_init / _update, points_selector.cpp:798-810
     min_cut(cloud, picked_point, **params)                  gtsam_points::min_cut, points_selector.cpp:774-796
+    plane_patch(frames, poses, center, **params)            the bundle adjustment modal's Update, bundle_adjustment_modal.cpp:137-184
+    plane_auto_radius(frames, poses, center, **params)      its Auto Radius, bundle_adjustment_modal.cpp:186-227
+    PlaneEVMFactorGPU(frames, poses, center, **params)      gtsam_points::PlaneEVMFactor of its Create Factor, :229-245
+    linearize_plane_evm(factors, poses_per_factor)          many PlaneEVMFactors relinearized in one launch
 """
 from __future__ import annotations
 
@@ -888,4 +892,116 @@ def min_cut(cloud: PointCloudGPU, picked_point, ctx: Context | None = None, grap
     if graph:
         out["edges"] = e[: r.num_edges].copy()
         out["capacities"] = w[: r.num_edges].copy()
+    return out
+
+
+def plane_patch_params(center=(0.0, 0.0, 0.0), **overrides) -> capi.PlanePatchParams:
+    """gb_plane_patch_default_params (the bundle adjustment modal's) at `center`, with the given fields replaced."""
+    p = _params(capi.PlanePatchParams(), lib().gb_plane_patch_default_params, "gb_plane_patch_params", overrides)
+    p.center = (C.c_double * 3)(*[float(v) for v in np.asarray(center, dtype=np.float64).reshape(-1)[:3]])
+    return p
+
+
+def _frames(frames, poses):
+    """(K, handle array, K x 16 column-major poses) of a frame list and its T_world_frame poses"""
+    K = len(frames)
+    arr = (C.c_void_p * max(K, 1))(*[f.h for f in frames])
+    T = pose16(np.stack([np.asarray(p, dtype=np.float64) for p in poses])) if K else np.zeros((0, 16))
+    return K, C.cast(arr, C.c_void_p), T
+
+
+def _patch(r: capi.PlanePatchResult) -> dict:
+    t = r.num_trials
+    return {"radius": r.radius, "num_points": r.num_points, "eigenvalues": np.array(r.eigenvalues[:]),
+            "trials": [(r.trial_radius[i], r.trial_points[i]) for i in range(t)]}
+
+
+def plane_patch(frames, poses, center, ids: bool = False, ctx: Context | None = None, **params) -> dict:
+    """The bundle adjustment modal's Update (gb_plane_patch): the points of the submaps within max_frame_distance of `center`
+    that lie within `radius` of it, their count and covariance eigenvalues (ascending).  frames K PointCloudGPU, poses K x (4,4)
+    T_world_submap; params are fields of gb_plane_patch_params.  -> {radius, num_points, eigenvalues (3,), trials []} and, with
+    ids, ids (num_points,) uint64 = (frame << 32) | original index, frame-major and ascending."""
+    ctx = ctx or (frames[0].ctx if len(frames) else default_context())
+    K, arr, T = _frames(frames, poses)
+    p = plane_patch_params(center, **params)
+    r = capi.PlanePatchResult()
+    buf = np.empty(sum(f.n for f in frames), np.uint64) if ids else None
+    check(lib().gb_plane_patch(ctx.h, K, arr, ptr(T), C.byref(p), C.byref(r), ptr(buf)))
+    out = _patch(r)
+    if ids:
+        out["ids"] = buf[: r.num_points].copy()
+    return out
+
+
+def plane_auto_radius(frames, poses, center, ctx: Context | None = None, **params) -> dict:
+    """The bundle adjustment modal's Auto Radius (gb_plane_auto_radius): the radius its loop settles on, with the count and
+    eigenvalues there, and trials [(radius, count)] of every evaluated trial in order."""
+    ctx = ctx or (frames[0].ctx if len(frames) else default_context())
+    K, arr, T = _frames(frames, poses)
+    p = plane_patch_params(center, **params)
+    r = capi.PlanePatchResult()
+    check(lib().gb_plane_auto_radius(ctx.h, K, arr, ptr(T), C.byref(p), C.byref(r)))
+    return _patch(r)
+
+
+class PlaneEVMFactorGPU(_Handle):
+    """gtsam_points::PlaneEVMFactor of the bundle adjustment modal's Create Factor (gb_plane_evm_factor_create): the submap
+    points within `radius` of `center`, keyed by their submap.  keys: the frame indices (in the creating list) that hold
+    selected points; key_points: their counts.  linearize(poses) / error(poses) take the keys' T_world_submap poses, as a
+    (K, 4, 4) array in key order or a dict {frame index: (4, 4)}.  The factor keeps its moments on the host: its frames may be
+    destroyed after creation."""
+
+    _destroy = "gb_vgicp_factor_destroy"
+
+    def __init__(self, frames, poses, center, ctx: Context | None = None, **params):
+        self.ctx = ctx or (frames[0].ctx if len(frames) else default_context())
+        K, arr, T = _frames(frames, poses)
+        p = plane_patch_params(center, **params)
+        self.h = self._create(lib().gb_plane_evm_factor_create, self.ctx.h, K, arr, ptr(T), C.byref(p))
+        nk, npts = C.c_size_t(), C.c_size_t()
+        check(lib().gb_plane_evm_factor_info(self.h, C.byref(nk), C.byref(npts), None, None))
+        self.keys = np.empty(nk.value, np.int32)
+        self.key_points = np.empty(nk.value, np.uint64)
+        check(lib().gb_plane_evm_factor_info(self.h, None, None, ptr(self.keys), ptr(self.key_points)))
+        self.num_points = npts.value
+
+    def _handle(self):
+        return self.h
+
+    def key_poses(self, poses) -> np.ndarray:
+        if isinstance(poses, dict):
+            poses = [poses[int(k)] for k in self.keys]
+        return np.asarray(poses, dtype=np.float64).reshape(len(self.keys), 4, 4)
+
+    def linearize(self, poses) -> dict:
+        """{H (6K, 6K), b (6K,), error, status, status_name}: e(xi) ~ error + 2 b^T xi + xi^T H xi along X_k Exp(xi_k)"""
+        return linearize_plane_evm([self], [poses], ctx=self.ctx)[0]
+
+    def error(self, poses) -> float:
+        e = np.zeros(1)
+        arr = (C.c_void_p * 1)(self.h)
+        check(lib().gb_plane_evm_error(self.ctx.h, 1, C.cast(arr, C.c_void_p), ptr(pose16(self.key_poses(poses))), ptr(e)))
+        return float(e[0])
+
+
+def linearize_plane_evm(factors: list[PlaneEVMFactorGPU], poses_per_factor, ctx: Context | None = None) -> list[dict]:
+    """Linearize many PlaneEVMFactorGPU in one call (gb_plane_evm_linearize: one upload, one launch, one download)."""
+    F = len(factors)
+    ctx = ctx or (factors[0].ctx if F else default_context())
+    X = [f.key_poses(p) for f, p in zip(factors, poses_per_factor)]
+    Ks = [len(f.keys) for f in factors]
+    T = pose16(np.concatenate(X)) if F else np.zeros((0, 16))
+    H = np.zeros(sum(36 * k * k for k in Ks))
+    b = np.zeros(sum(6 * k for k in Ks))
+    e = np.zeros(F)
+    s = np.zeros(F, np.int32)
+    arr = (C.c_void_p * max(F, 1))(*[f.h for f in factors])
+    check(lib().gb_plane_evm_linearize(ctx.h, F, C.cast(arr, C.c_void_p), ptr(T), ptr(H), ptr(b), ptr(e), ptr(s)))
+    out, h0, b0 = [], 0, 0
+    for f, K in enumerate(Ks):
+        n6 = 6 * K
+        out.append({"H": H[h0:h0 + n6 * n6].reshape(n6, n6).T.copy(), "b": b[b0:b0 + n6].copy(), "error": float(e[f]), "status": int(s[f]),
+                    "status_name": capi.PLANE_EVM_STATUS_NAMES.get(int(s[f]), "?")})
+        h0 += n6 * n6
+        b0 += n6
     return out

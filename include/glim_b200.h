@@ -845,6 +845,113 @@ GB_API gb_status gb_min_cut_default_params(gb_min_cut_params* params);
 GB_API gb_status gb_min_cut(gb_ctx* ctx, const gb_cloud* cloud, const double picked_point[3], const gb_min_cut_params* params,
                             gb_min_cut_result* result, int32_t* selected, int32_t* edges, int32_t* capacities);
 
+/* ---- The interactive viewer's plane bundle adjustment (src/glim/viewer/interactive/bundle_adjustment_modal.cpp:37-60,
+ *      :137-245; interactive_viewer.cpp:393, :412-418): the submap points around a right-clicked point, their covariance's
+ *      eigenvalues (Update), the modal's radius search (Auto Radius), and the gtsam_points::PlaneEVMFactor made of them
+ *      (Create Factor), which global mapping's iSAM2 then relinearizes.
+ *
+ *      Inputs of the three patch calls: K device clouds (submaps, in their local frame), poses T_k = (R_k, t_k) (K x 16
+ *      doubles, column-major, T_world_submap) and the parameters below, whose `center` c is the picked point (fp64).
+ *
+ *      Selection (set_frames, extract_points).
+ *      1. Frame k takes part iff sqrt((u_x^2 + u_y^2) + u_z^2) <= max_frame_distance for u = t_k - c (the modal skips a submap
+ *         whose norm is > 25).
+ *      2. A stored fp32 point a of a participating frame is widened to fp64 and transformed as q = R_k a + u, row r as
+ *         ((R_r0 a_x + R_r1 a_y) + R_r2 a_z) + u_r, un-contracted: gb_merge_frames' transform at the pose [R_k | t_k - c], the
+ *         modal's Translation(-center) * pose.
+ *      3. The point is selected iff (q_x^2 + q_y^2) + q_z^2 < radius * radius, both sides fp64; a NaN never is.
+ *      4. Selected ids are (k << 32) | original index, frame-major and ascending: gb_concat_frames' editor ids.
+ *      5. The modal keys its fp64 host points, this library the stored fp32 ones: a point within about 1e-7 relative of the
+ *         sphere may fall on the other side (the caveat of gb_concat_frames).
+ *
+ *      Patch statistics (calc_eigenvalues).  Over the n selected points in fp64: s = sum q, S = sum q q^T, mean = s / n,
+ *      Cov(r, c) = (S(r, c) - mean_r s_c) / n for r <= c, mirrored; the eigenvalues, ascending, from eigen_sym3_direct (the
+ *      modal's computeDirect, the solver of the covariance estimation).  n == 0 gives NaN eigenvalues (the modal's 0 / 0).  The
+ *      sums are taken in a fixed order that depends on the candidates only: the same inputs give the same bits.
+ *
+ *      Auto radius (exactly the modal's loop, :186-227):
+ *          r = radius; (n, ev) = stats(r)                      no size check on this first extraction
+ *          for i in 0..9:
+ *              trial = ev[0] / ev[2] > plane_eps ? r * 0.8 : r * 1.1        a NaN ratio grows
+ *              if trial < min_radius or trial > max_radius: break
+ *              (n', ev') = stats(trial)                        recorded as trial i: (trial, n')
+ *              if n' < 10: break
+ *              if trial > radius and ev'[0] / ev'[2] > plane_eps: break     `radius` is the starting radius
+ *              r, n, ev = trial, n', ev'
+ *          result: r, n, ev (what update_indicator then shows) and the trials.
+ *
+ *      The factor (Create Factor, :229-245).  The selection at `radius` gives the keys: the participating frames with at least
+ *      one selected point, in the caller's frame order.  Per key, from its selected stored local points a widened to fp64:
+ *      N_k, the mean m_k and the scatter S_k = sum (a - m_k)(a - m_k)^T (two passes, fixed order).  The factor keeps the
+ *      offset o = c, which keeps world coordinates far from the origin out of the fp64 sums (the error does not depend on it).
+ *      [EXT] gtsam_points is not vendored: the error e = lambda_0 (not N lambda_0), the exact Hessian and the record convention
+ *      below are this library's statement of PlaneEVMFactor.
+ *        Error at the key poses X_k: p_i = X_k a_i - o, pbar = mean p, C = (1/N) sum (p_i - pbar)(p_i - pbar)^T with ascending
+ *        eigenpairs (lambda_m, u_m), e = lambda_0.  It is evaluated from the moments,
+ *        C = (1/N) sum_k [R_k S_k R_k^T + N_k (q_k - pbar)(q_k - pbar)^T], q_k = R_k m_k + t_k - o, which is algebraically the
+ *        definition, so a linearization costs O(K^2) whatever the point count.  C is decomposed by eigen_sym3_direct.
+ *        Linearization along the chart X_k Exp(xi_k), xi_k = [omega; nu] (GTSAM Pose3 Expmap): b = (1/2) de/dxi (6K) and
+ *        H = (1/2) d2e/dxi2 (6K x 6K, dense, column-major), the exact Hessian at xi = 0, including the term of the second-order
+ *        expansion of Exp.  So e(xi) ~ e + 2 b^T xi + xi^T H xi, the relation of every gb_linearized6 record:
+ *        HessianFactor(keys, G = H, g = -b, f = e) hands it to GTSAM as gb_hessian_blocks does for the other factors.
+ *        Status DEGENERATE iff !(lambda_1 - lambda_0 > 0): then H = 0, b = 0 and e = lambda_0 (a repeated lambda_1 = lambda_2
+ *        is fine).
+ *
+ *      Every input is validated before any launch (GB_ERR_INVALID_ARGUMENT, nothing created): null arguments, a non-finite
+ *      pose or centre, a frame on another device than ctx, a frame of 2^32 points or more or 2^30 in all, and parameters
+ *      outside the bounds below.  Launches (none when the participating frames hold no point):
+ *        gb_plane_patch:             4 (the shared frame transform, the sphere flags, their scan, the emit) + 1 (the reduction);
+ *                                    one stream synchronisation, and a second one when ids are asked for and n > 0.
+ *        gb_plane_auto_radius:       4 (the selection at max(radius, max_radius)) + 1 per evaluated radius (1 + num_trials);
+ *                                    one stream synchronisation per evaluated radius.
+ *        gb_plane_evm_factor_create: 4 (the selection at radius, with the local points) + 1 (the per-key moments); one stream
+ *                                    synchronisation.  Fewer than 3 selected points is GB_ERR_INVALID_ARGUMENT after these
+ *                                    launches, and creates nothing (the modal would build a factor whose error is NaN).
+ *      ---- */
+#define GB_PLANE_MAX_TRIALS 10
+#define GB_PLANE_EVM_OK 0
+#define GB_PLANE_EVM_DEGENERATE 1
+typedef struct gb_plane_patch_params {
+  double center[3];          /* the picked point; finite */
+  double radius;             /* m, finite, > 0: 1.0 (the modal's) */
+  double max_frame_distance; /* m, >= 0, +inf allowed: 25.0 */
+  double min_radius;         /* m, finite, 0 < min_radius <= max_radius: 0.1 */
+  double max_radius;         /* m, finite: 5.0 */
+  double plane_eps;          /* finite, >= 0: 0.01 */
+} gb_plane_patch_params;
+typedef struct gb_plane_patch_result {
+  double radius;                                  /* the radius the statistics are taken at */
+  size_t num_points;                              /* n */
+  double eigenvalues[3];                          /* ascending; NaN for n == 0 */
+  int32_t num_trials;                             /* gb_plane_auto_radius: evaluated trials (<= 10); 0 otherwise */
+  double trial_radius[GB_PLANE_MAX_TRIALS];       /* in evaluation order */
+  size_t trial_points[GB_PLANE_MAX_TRIALS];
+} gb_plane_patch_result;
+/* the modal's defaults: centre 0, 1.0, 25.0, 0.1, 5.0, 0.01 */
+GB_API gb_status gb_plane_patch_default_params(gb_plane_patch_params* params);
+/* Update: n and the eigenvalues at params->radius; ids (capacity the sum of the frames' sizes, or NULL) the selected ids */
+GB_API gb_status gb_plane_patch(gb_ctx* ctx, size_t num_frames, const gb_cloud* const* frames, const double* poses, const gb_plane_patch_params* params,
+                                gb_plane_patch_result* result, uint64_t* ids);
+/* Auto Radius: the returned radius with n and the eigenvalues there, and the trial path */
+GB_API gb_status gb_plane_auto_radius(gb_ctx* ctx, size_t num_frames, const gb_cloud* const* frames, const double* poses, const gb_plane_patch_params* params,
+                                      gb_plane_patch_result* result);
+/* Create Factor: uses center, radius and max_frame_distance.  The factor keeps K x 10 doubles on the host: it borrows no
+ * cloud (its frames may be destroyed afterwards) and owns no device memory; gb_vgicp_factor_destroy frees it.  Every other
+ * factor entry point (gb_vgicp_linearize, gb_vgicp_error, gb_factor_set_*, gb_sweep_create, gb_vgicp_align, gb_ct_*) refuses
+ * it with GB_ERR_INVALID_ARGUMENT before any launch, and the gb_plane_evm_* calls refuse every other kind. */
+GB_API gb_status gb_plane_evm_factor_create(gb_ctx* ctx, size_t num_frames, const gb_cloud* const* frames, const double* poses, const gb_plane_patch_params* params,
+                                            gb_factor** out);
+/* num_keys, num_points; frame_indices and key_points (capacity num_keys each, or NULL): each key's frame index in the
+ * creating call's list and its point count.  No launch. */
+GB_API gb_status gb_plane_evm_factor_info(const gb_factor* factor, size_t* num_keys, size_t* num_points, int32_t* frame_indices, uint64_t* key_points);
+/* F plane factors at once: poses (sum K_f x 16, each factor's keys in key order), H (sum (6 K_f)^2, each column-major),
+ * b (sum 6 K_f), errors (F), status (F, GB_PLANE_EVM_*, or NULL).  One upload, one launch (one CTA per factor), one download
+ * and its stream synchronisation; none for F == 0.  The factors' context does not matter: they own no device memory. */
+GB_API gb_status gb_plane_evm_linearize(gb_ctx* ctx, size_t num_factors, gb_factor* const* factors, const double* poses, double* H, double* b, double* errors,
+                                        int32_t* status);
+/* the errors only: the same transfers and one launch */
+GB_API gb_status gb_plane_evm_error(gb_ctx* ctx, size_t num_factors, gb_factor* const* factors, const double* poses, double* errors);
+
 /* ---- glim::CloudDeskewing::deskew (src/glim/common/cloud_deskewing.cpp:11-55 constant velocity, :57-133 predicted IMU poses;
  *      called at src/glim/odometry/odometry_estimation_imu.cpp:313).  n_imu > 0: imu_times / imu_poses (n_imu x 16, T_world_imu)
  *      and `stamp` select the IMU-pose overload; n_imu == 0: linear_vel / angular_vel (either may be NULL = zero) select the
