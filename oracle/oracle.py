@@ -42,6 +42,8 @@ def lib():
         L.go_vgicp_linearize_gpumap_sv.argtypes = [vp, i32, vp, vp, vp, vp, i32, vp, vp]
         L.go_vgicp_error_gpumap.restype = f64
         L.go_vgicp_error_gpumap.argtypes = [vp, i32, vp, vp, vp, vp]
+        L.go_vgicp_error_gpumap_sv.restype = f64
+        L.go_vgicp_error_gpumap_sv.argtypes = [vp, i32, vp, vp, vp, vp, vp]
         L.go_overlap_gpumap.restype = f64
         L.go_overlap_gpumap.argtypes = [i32, vp, i32, vp, vp]
         L.go_pack_cloud_f32.argtypes = [i32, vp, vp, vp, vp]
@@ -170,9 +172,12 @@ def linearize_gpumap(m, xyz, cov6, T, with_derivs=True, normals=None):
     return out, corr
 
 
-def error_gpumap(m, xyz, cov6, T_lin, T_eval):
+def error_gpumap(m, xyz, cov6, T_lin, T_eval, normals=None):
+    """error at T_eval with the correspondences of T_lin.  normals: (n,3|4) source normals -> surface validation on, the gate
+    deciding at T_lin (where the correspondences are found)."""
     xyz, cov6 = _f32(xyz), _f32(cov6)
-    return lib().go_vgicp_error_gpumap(m.h, xyz.shape[0], _p(xyz), _p(cov6), _p(pose_colmajor(T_lin)), _p(pose_colmajor(T_eval)))
+    nr = _f32(np.asarray(normals)[:, :3]) if normals is not None else None
+    return lib().go_vgicp_error_gpumap_sv(m.h, xyz.shape[0], _p(xyz), _p(cov6), _p(nr), _p(pose_colmajor(T_lin)), _p(pose_colmajor(T_eval)))
 
 
 def overlap_gpumap(maps, xyz, Ts):

@@ -8,6 +8,7 @@ import pytest
 from oracle import oracle
 from glim_b200 import gpu, synth
 from tests import util
+from tests.util import check_linearized
 
 pytestmark = pytest.mark.gpu
 
@@ -30,20 +31,6 @@ def dev(ctx, pair):
         d["cov6"].append(cov6)
     d["T_gt"] = synth.inv_pose(pair["poses"][0]) @ pair["poses"][1]
     return d
-
-
-def check_linearized(got: dict, ref122: np.ndarray, tol=REL_TOL):
-    ref = oracle.split122(ref122)
-    assert got["num_inliers"] == ref["num_inliers"]  # inlier set bit-exact
-    for k in ("H_tt", "H_ss", "H_ts"):
-        assert util.rel_err(got[k], ref[k]) < tol, (k, util.rel_err(got[k], ref[k]))
-    # The gradient b = sum J^T M r is a sum of terms that cancel as the pose converges, so its fp32 rounding noise does
-    # not shrink with |b|.  Its natural magnitude is the Cauchy-Schwarz bound sqrt(tr(H) * error) of the un-cancelled
-    # sum; the tolerance is 1e-4 of max(|b|, a tenth of that bound).
-    for k, hk in (("b_t", "H_tt"), ("b_s", "H_ss")):
-        scale = max(np.linalg.norm(ref[k]), 0.1 * np.sqrt(np.trace(ref[hk]) * max(ref["error"], 1e-30)))
-        assert np.linalg.norm(got[k] - ref[k]) < tol * scale, (k, np.linalg.norm(got[k] - ref[k]) / scale, np.linalg.norm(got[k] - ref[k]) / np.linalg.norm(ref[k]))
-    assert abs(got["error"] - ref["error"]) <= tol * abs(ref["error"]) + 1e-12
 
 
 def test_cloud_upload_is_bit_exact(dev):

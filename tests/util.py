@@ -40,6 +40,25 @@ def scan_pair(sensor="hdl32", n_rays=32 * 300, step=1.0, key=0, scene="hall"):
     return out
 
 
+def check_linearized(got: dict, ref, tol=REL_TOL):
+    """A device record (unpacked) against a reference: a 122-double oracle record or a dict of blocks indexed [row, col].
+    Inlier count exact; Hessians, gradients and error within `tol` relative of the reference (a factor without inliers: zeros)."""
+    from oracle import oracle
+
+    if not isinstance(ref, dict):
+        ref = oracle.split122(ref)
+    assert got["num_inliers"] == ref["num_inliers"]  # inlier set bit-exact
+    for k in ("H_tt", "H_ss", "H_ts"):
+        assert rel_err(got[k], ref[k]) < tol, (k, rel_err(got[k], ref[k]))
+    # The gradient b = sum J^T M r is a sum of terms that cancel as the pose converges, so its fp32 rounding noise does
+    # not shrink with |b|.  Its natural magnitude is the Cauchy-Schwarz bound sqrt(tr(H) * error) of the un-cancelled
+    # sum; the tolerance is 1e-4 of max(|b|, a tenth of that bound).
+    for k, hk in (("b_t", "H_tt"), ("b_s", "H_ss")):
+        scale = max(np.linalg.norm(ref[k]), 0.1 * np.sqrt(np.trace(ref[hk]) * max(ref["error"], 1e-30)))
+        assert np.linalg.norm(got[k] - ref[k]) <= tol * scale, (k, np.linalg.norm(got[k] - ref[k]) / scale, np.linalg.norm(got[k] - ref[k]) / np.linalg.norm(ref[k]))
+    assert abs(got["error"] - ref["error"]) <= tol * abs(ref["error"]) + 1e-12
+
+
 def test_poses(T_gt, n=4, key=0):
     """Ground-truth delta and a handful of perturbed / adversarial deltas."""
     rng = synth.rng_for(99, key)
