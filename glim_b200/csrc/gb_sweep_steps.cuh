@@ -71,18 +71,27 @@ __device__ __forceinline__ void probe_compact(int v, int i, int limit, uint2* __
   nq += __popc(m);
 }
 
+// One stage of warp_reduce_scatter32: lanes STEP apart swap halves of v[0, 2 STEP) and keep the sums in v[0, STEP).
+// STEP is a template argument so that every v[] index is a compile-time constant: with a runtime step the inner loop is not
+// unrolled and acc[32] lives on the stack (an LDL -> SHFL -> STL chain per item and the stack copy zeroed at every item start).
+template <int STEP>
+__device__ __forceinline__ void reduce_scatter_stage(float (&v)[32], int lane) {
+  const bool upper = (lane & STEP) != 0;
+#pragma unroll
+  for (int j = 0; j < STEP; j++) {
+    const float send = upper ? v[j] : v[j + STEP];
+    const float keep = upper ? v[j + STEP] : v[j];
+    v[j] = keep + __shfl_xor_sync(0xffffffffu, send, STEP);
+  }
+}
+
 // Transposing warp reduction: on return lane l holds sum over the warp of v[l] (in v[0]).
 __device__ __forceinline__ float warp_reduce_scatter32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int step = 16; step >= 1; step >>= 1) {
-    const bool upper = (lane & step) != 0;
-#pragma unroll
-    for (int j = 0; j < step; j++) {
-      const float send = upper ? v[j] : v[j + step];
-      const float keep = upper ? v[j + step] : v[j];
-      v[j] = keep + __shfl_xor_sync(0xffffffffu, send, step);
-    }
-  }
+  reduce_scatter_stage<16>(v, lane);
+  reduce_scatter_stage<8>(v, lane);
+  reduce_scatter_stage<4>(v, lane);
+  reduce_scatter_stage<2>(v, lane);
+  reduce_scatter_stage<1>(v, lane);
   return v[0];
 }
 

@@ -134,7 +134,8 @@ def main():
     print("  `fence.acq_rel.gpu` (`fence_acquire`, :226) that only the warp drawing a factor's / pair's LAST ticket executes; the two")
     print("  `CCTL.IVALL` (L1 invalidate) belong to that acquire, i.e. once per factor, not once per item; there is no `MEMBAR.SC`")
     print("  (`__threadfence()`) in the sweep kernels -- `MEMBAR.ALL.SYS` appears only in the two exchange kernels (`__threadfence_system`);")
-    print("* local-memory instructions of sweep3 / sweep5 sit at the item boundary, outside the lookup and derivative loops.")
+    print("* local-memory instructions of sweep3 / sweep5 are the call frame of the `__noinline__` epilogue (`factor_epilogue`): the")
+    print("  argument stores ahead of its two calls and one load inside it; `acc[32]` stays in registers through the item reduction.")
 
 
 if __name__ == "__main__":
