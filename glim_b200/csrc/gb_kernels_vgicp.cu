@@ -42,14 +42,31 @@ namespace {
 // atom.release issued while the next item's first loads are in flight (no __threadfence, i.e. no MEMBAR.SC + L1
 // invalidation per item), and a factor's epilogue runs after the next item's reduction.  Measured on the global-mapping
 // sweep and its 1/8 shards: faster than a fence + ticket per item.
+// An item's 29 accumulators are in registers only while a round's hits are accumulated (phase B); between rounds each lane
+// parks them in its column of the warp's shared memory, so that phase A has those registers for probes in flight.  A lane
+// adds its hits in the same order as with the accumulators live across the item, so the results are bit-identical.
 // Tried and dropped: reading the queue one item ahead in registers (slower: the kernel sits at the 128-register
-// cap) and copying the next item's descriptor / pose to shared memory with cp.async during the current item (slower: the
-// three dependent L2 round trips between two items are already covered by the other 15 warps of the SM).
+// cap); copying the next item's descriptor / pose to shared memory with cp.async during the current item (slower: the
+// three dependent L2 round trips between two items are already covered by the other 15 warps of the SM); folding each
+// round's accumulators over the warp (warp_reduce_scatter32) into one running float per lane instead of parking them
+// (some 150 instructions per round; slower than the live accumulators at every probe count tried, DESIGN.md 4.1).
 // =============================================================================================
-constexpr int kSubMax = 512;   // queue capacity per warp (points per round)
-constexpr int kLookupUnroll3 = 5;  // probes per lane in flight (4: 2 % slower on the global-mapping sweep; 6: spills)
-constexpr int kRound3 = 32 * kLookupUnroll3 * ((kSubMax - 31) / (32 * kLookupUnroll3));  // points per round: whole lookup groups
-static_assert(kRound3 + 31 <= kSubMax, "a round's hits and the up to 31 carried from the previous round fit the queue");
+// sweep3's shared memory per warp: the queue (a round's hits and the up to 31 carried from the previous round) and the
+// parked accumulators.  48 KB per CTA, so at 2 CTAs / SM the carve-out, and with it the L1, stays what the 32 KB of
+// 512-entry queues got.
+constexpr int kQueue3 = 304;
+struct Sweep3Warp {
+  uint2 q[kQueue3];
+  float acc[29][32];  // acc[k][lane]: conflict-free
+};
+static_assert(sizeof(Sweep3Warp) * kWarps <= 48 * 1024, "static shared memory");
+// Probes per lane in flight.  Linearize: 8 (6 or 7 measured no faster than 5 with live accumulators on the global-mapping
+// sweep, 8 is 4.7 % faster).  Error: 7 (8 spills).  With surface validation (a dense odometry frame, livox_stress): 5, which
+// measured 1.2 % faster than 8 there (7: 0.8 %, 6: 0.5 %).
+template <int MODE, bool SV> constexpr int kLookupUnroll3 = SV ? 5 : MODE == GB_MODE_LINEARIZE ? 8 : 7;
+template <int MODE, bool SV> constexpr int kRound3 = 32 * kLookupUnroll3<MODE, SV> * ((kQueue3 - 31) / (32 * kLookupUnroll3<MODE, SV>));  // points per round: whole lookup groups
+static_assert(kRound3<GB_MODE_LINEARIZE, false> > 0 && kRound3<GB_MODE_ERROR, false> > 0 && kRound3<GB_MODE_LINEARIZE, true> > 0,
+              "a round's hits and the up to 31 carried from the previous round fit the queue");
 
 template <int MODE, bool PEER, bool SV>
 __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
@@ -57,11 +74,13 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
   const int2* __restrict__ items, int num_items,
   unsigned long long* __restrict__ item_ctr, unsigned long long ctr_base,
   double* __restrict__ accum, int acc_slots, unsigned* __restrict__ done, double* __restrict__ out, float* __restrict__ slab, const PeerPush* __restrict__ peer) {
-  __shared__ __align__(16) uint2 s_q[kWarps][kSubMax];
+  __shared__ __align__(16) Sweep3Warp s_w[kWarps];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned lt_mask = (1u << lane) - 1u;
-  uint2* __restrict__ q = s_q[warp];
+  uint2* __restrict__ q = s_w[warp].q;
+  float (*__restrict__ parked)[32] = s_w[warp].acc;
   auto desc_of = [&](int f) { return descs[f]; };  // a copy, for retire_factor
+  constexpr int U = kLookupUnroll3<MODE, SV>, kRound = kRound3<MODE, SV>;
 
   // first item: static (warp id); further items (only when there are more items than warps) come from the global queue
   const int total_warps = gridDim.x * kWarps;
@@ -82,17 +101,19 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
     if (MODE == GB_MODE_ERROR) Pe = pose_from_colmajor(poses_eval + (size_t)f * 16);
     const int item_end = min(it.y + D.chunk, D.n);  // per-factor item size (the tail of a sweep is tapered)
     bool published = pend_f < 0;
-    float acc[32];
+    bool held = false;  // warp-uniform: the item's accumulators are parked (else they are all zero)
+    auto unpark = [&](float (&acc)[32]) {
 #pragma unroll
-    for (int k = 0; k < 32; k++) acc[k] = 0.f;
+      for (int k = 0; k < 32; k++) acc[k] = held && k < 29 && (MODE == GB_MODE_LINEARIZE || k >= 27) ? parked[k][lane] : 0.f;
+    };
 
     int nq = 0;  // warp-uniform queue length
-    for (int wb = it.y; wb < item_end; wb += kRound3) {
-      const int we = min(wb + kRound3, item_end);
-      for (int i0 = wb; i0 < we; i0 += 32 * kLookupUnroll3) {
-        Probe p[kLookupUnroll3];
+    for (int wb = it.y; wb < item_end; wb += kRound) {
+      const int we = min(wb + kRound, item_end);
+      for (int i0 = wb; i0 < we; i0 += 32 * U) {
+        Probe p[U];
 #pragma unroll
-        for (int u = 0; u < kLookupUnroll3; u++) {
+        for (int u = 0; u < U; u++) {
           const float4 a0 = __ldg(&D.p0[min(i0 + u * 32 + lane, we - 1)]);
           probe_issue(D, P, a0.x, a0.y, a0.z, p[u]);
         }
@@ -101,17 +122,25 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
           __syncwarp();
           if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
         }
-        int v[kLookupUnroll3];
+        int v[U];
         probe_resolve(D, p, v);
 #pragma unroll
-        for (int u = 0; u < kLookupUnroll3; u++) probe_compact(v[u], i0 + u * 32 + lane, we, q, nq, lt_mask);
+        for (int u = 0; u < U; u++) probe_compact(v[u], i0 + u * 32 + lane, we, q, nq, lt_mask);
       }
       __syncwarp();
       // Whole passes of 32 hits only: the last nq % 32 hits are carried to the front of the queue for the next round (a
       // pass costs a round trip however few lanes it fills), except in the item's last round.
       const int nacc = we == item_end ? nq : (nq & ~31);
-      // surface validation is a compile-time variant here (GLIM enables it for odometry factors only, which run sweep5)
-      accumulate_queue<MODE, SV>(acc, D, P, Pe, q, nacc, lane);
+      if (nacc > 0) {
+        float acc[32];
+        unpark(acc);
+        // surface validation is a compile-time variant here (GLIM enables it for odometry factors only, which run sweep5)
+        accumulate_queue<MODE, SV>(acc, D, P, Pe, q, nacc, lane);
+#pragma unroll
+        for (int k = 0; k < 29; k++)
+          if (MODE == GB_MODE_LINEARIZE || k >= 27) parked[k][lane] = acc[k];
+        held = true;
+      }
       __syncwarp();  // the queue is overwritten by the next round
       nq -= nacc;
       if (nacc > 0 && lane < nq) q[lane] = q[nacc + lane];  // nacc >= 32 > nq: the ranges do not overlap
@@ -122,6 +151,8 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
       if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
     }
 
+    float acc[32];
+    unpark(acc);
     reduce_item<MODE>(acc, accum, f, acc_slots, item, lane);
     if (pend_f >= 0 && __shfl_sync(0xffffffffu, pend_last, 0)) {  // the PREVIOUS item completed its factor
       fence_acquire();
@@ -141,6 +172,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
   }
 }
 
+constexpr int kSubMax = 512;  // queue capacity per warp (points per round)
 constexpr int kLookupUnroll5 = 4;  // probes per lane in flight (5 spills)
 constexpr int kDescCache = 40;  // factors whose descriptor + fp32 pose are cached in shared memory (an odometry graph has <= 34)
 struct CtaCache {
