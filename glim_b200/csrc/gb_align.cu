@@ -76,7 +76,7 @@ gb_status validate(size_t P, const size_t* off, gb_factor* const* factors, const
   GB_REQUIRE(off[P] < ((size_t)1 << 30), "too many factors");
   GB_REQUIRE(factors, "null factor list");
   for (size_t f = 0; f < off[P]; f++) GB_REQUIRE(factors[f], "null factor");
-  for (size_t k = 0; k < 16 * P; k++) GB_REQUIRE(isfinite(T_init[k]), "T_init must be finite");
+  GB_REQUIRE(gb_all_finite(T_init, 16 * P), "T_init must be finite");
   return gb_align_params_check(prm);
 }
 

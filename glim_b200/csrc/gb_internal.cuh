@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/glim_b200.h"
+#include "gb_segment_math.cuh"  // gb_frame, gb_frame_of (shared with the host-compiled CPU test of the segmentation arithmetic)
 
 // ---------------------------------------------------------------------------------------------
 // error plumbing
@@ -409,6 +410,7 @@ void cloud_free(gb_cloud* c);
 void sweep_free(gb_sweep* s);
 void ctx_retain(gb_ctx* ctx);
 void ctx_release(gb_ctx* ctx);
+void grid_release(gb_point_grid* g);  // gb_point_grid_destroy, as the free function of a gb_owned point grid
 // A new factor of `kind` on (target, source) with its context retained and a process-wide unique id; nullptr when out of
 // host memory.  Every *_factor_create calls it after its own argument checks.
 gb_factor* factor_new(gb_ctx* ctx, gb_factor_kind kind, const gb_voxelmap* target, const gb_cloud* source);
@@ -541,13 +543,19 @@ enum { GB_MODE_LINEARIZE = 0, GB_MODE_ERROR = 1 };
 gb_status gb_launch_sweep(gb_sweep* s, int mode);
 gb_status gb_launch_gicp_sweep(gb_sweep* s, int mode);  // gb_launch_sweep of a GICP sweep
 gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count);
-// The frame transform of gb_merge_frames (gb_kernels_preprocess.cu), shared with the map insert and gb_concat_frames
-// (gb_kernels_segment.cu): the points q = R a + t and covariances R C R^T in un-contracted fp64 of K frames at poses (K x 16,
-// column-major), frame-major and each frame in its original point order (pts: total x double4, cov6: total x 6 upper
-// triangle; nullptr: no covariances).  gb_frame_table writes the frames' descriptor table on the host; the caller uploads it
-// to d_table and gb_transform_frames launches over the frames' `total` points: one launch, none when total is 0.
-std::vector<char> gb_frame_table(size_t K, const gb_cloud* const* frames, const double* poses);
-gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const void* d_table, int total, double4* pts, double* cov6);
+// The posed frame list of gb_merge_frames (gb_kernels_preprocess.cu), shared with the map insert, gb_concat_frames
+// (gb_kernels_segment.cu) and the plane selection (gb_kernels_plane.cu): K device clouds and their poses (K x 16,
+// column-major).  gb_frame_list_check refuses, before any launch, a null list when K > 0, a null frame, a frame on another
+// device than ctx's, a frame of 2^32 points or more and 2^30 points or more in all, and gives the total; it does not look at
+// the poses' values (gb_all_finite says whether n doubles are all finite).  gb_frame_table writes the list's descriptors
+// (gb_frame, gb_segment_math.cuh) on the host, index[k] as the caller's index of frame k (k without index); the caller
+// uploads them to d_table, which the kernels search with gb_frame_of.  gb_transform_frames writes the points q = R a + t and
+// covariances R C R^T in un-contracted fp64, frame-major and each frame in its original point order (pts: total x double4,
+// cov6: total x 6 upper triangle; nullptr: no covariances): one launch, none when total is 0.
+gb_status gb_frame_list_check(const gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, size_t* total);
+bool gb_all_finite(const double* v, size_t n);
+std::vector<gb_frame> gb_frame_table(size_t K, const gb_cloud* const* frames, const double* poses, const int* index);
+gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const gb_frame* d_table, int total, double4* pts, double* cov6);
 // The exact k-NN of gb_preprocess and gb_find_neighbors (gb_kernels_preprocess.cu), shared with gb_min_cut: the k nearest of
 // the first *d_count points of d_pts (device resident, n slots) to each of them, by un-contracted fp64 d2 with ties to the
 // smaller index, the query included, in neighbors[i * k + j]; the row of a point whose cell of h0 leaves the 21-bit range, or

@@ -342,12 +342,6 @@ gb_status ct_check_factor(const gb_factor* f, const gb_ctx* ctx) {
   return GB_OK;
 }
 
-bool finite16(const double* T) {
-  for (int k = 0; k < 16; k++)
-    if (!isfinite(T[k])) return false;
-  return true;
-}
-
 // A prepared call: the work items and descriptors of P CT factors staged in pinned memory, the device block carved.
 struct CtCall {
   gb_ctx* ctx = nullptr;
@@ -509,7 +503,7 @@ extern "C" gb_status gb_ct_gicp_factor_create(gb_ctx* ctx, const gb_ivox* target
 extern "C" gb_status gb_ct_gicp_linearize(gb_factor* f, const double X[16], const double Y[16], gb_linearized6* out) {
   GB_REQUIRE(f && X && Y && out, "null argument");
   GB_CHECK(ct_check_factor(f, f->ctx));
-  GB_REQUIRE(finite16(X) && finite16(Y), "X and Y must be finite");
+  GB_REQUIRE(gb_all_finite(X, 16) && gb_all_finite(Y, 16), "X and Y must be finite");
   GB_ENTER(f->ctx);
   return ct_evaluate(f->ctx, 1, &f, X, Y, nullptr, nullptr, GB_MODE_LINEARIZE, out, nullptr);
 }
@@ -517,7 +511,7 @@ extern "C" gb_status gb_ct_gicp_linearize(gb_factor* f, const double X[16], cons
 extern "C" gb_status gb_ct_gicp_error(gb_factor* f, const double X_lin[16], const double Y_lin[16], const double X_eval[16], const double Y_eval[16], double* error) {
   GB_REQUIRE(f && X_lin && Y_lin && X_eval && Y_eval && error, "null argument");
   GB_CHECK(ct_check_factor(f, f->ctx));
-  GB_REQUIRE(finite16(X_lin) && finite16(Y_lin) && finite16(X_eval) && finite16(Y_eval), "poses must be finite");
+  GB_REQUIRE(gb_all_finite(X_lin, 16) && gb_all_finite(Y_lin, 16) && gb_all_finite(X_eval, 16) && gb_all_finite(Y_eval, 16), "poses must be finite");
   GB_ENTER(f->ctx);
   return ct_evaluate(f->ctx, 1, &f, X_lin, Y_lin, X_eval, Y_eval, GB_MODE_ERROR, nullptr, error);
 }
@@ -543,7 +537,7 @@ extern "C" gb_status gb_ct_gicp_align(gb_ctx* ctx, size_t P, gb_factor* const* f
   GB_REQUIRE(P < ((size_t)1 << 20), "too many problems");
   for (size_t p = 0; p < P; p++) GB_CHECK(ct_check_factor(factors[p], ctx));
   for (size_t p = 0; p < P; p++)
-    GB_REQUIRE(finite16(X_init + 16 * p) && finite16(Y_init + 16 * p) && finite16(X_prior + 16 * p), "X_init, Y_init and X_prior must be finite");
+    GB_REQUIRE(gb_all_finite(X_init + 16 * p, 16) && gb_all_finite(Y_init + 16 * p, 16) && gb_all_finite(X_prior + 16 * p, 16), "X_init, Y_init and X_prior must be finite");
   GB_CHECK(gb_align_params_check(&prm->lm));
   GB_REQUIRE(isfinite(prm->location_consistency_inf_scale) && prm->location_consistency_inf_scale >= 0.0, "location_consistency_inf_scale must be finite and >= 0");
   GB_REQUIRE(isfinite(prm->constant_velocity_inf_scale) && prm->constant_velocity_inf_scale >= 0.0, "constant_velocity_inf_scale must be finite and >= 0");
@@ -582,7 +576,7 @@ extern "C" gb_status gb_ct_deskew(gb_ctx* ctx, const gb_cloud* source, const dou
   if (out_cloud) *out_cloud = nullptr;
   GB_REQUIRE(source->device == ctx->device, "the cloud lives on another device");
   GB_REQUIRE(source->num_entries > 0, "the source has no times (gb_cloud_add_times)");
-  GB_REQUIRE(finite16(X) && finite16(Y), "X and Y must be finite");
+  GB_REQUIRE(gb_all_finite(X, 16) && gb_all_finite(Y, 16), "X and Y must be finite");
   GB_REQUIRE(k >= 1 && k <= kc, "need 1 <= k_neighbors <= k_correspondences");
   const size_t n = source->n;
   for (size_t i = 0; i < n; i++)

@@ -348,8 +348,6 @@ __global__ void __launch_bounds__(kGncThreads) k_gnc_solve(const int2* __restric
   if (tid == 0) { out->inliers = 0; out->iterations = iterations; out->status = GB_GNC_FOUND; }
 }
 
-void grid_release(gb_point_grid* g) { gb_point_grid_destroy(g); }
-
 FpfhGrid fpfh_grid(const gb_voxelmap* g, int m, float max_d2) {
   return FpfhGrid{g->buckets, g->cells, g->voxels, (uint32_t)(g->num_buckets - 1), g->max_scan, m, g->inv_res, max_d2};
 }

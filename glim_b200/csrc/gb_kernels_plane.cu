@@ -23,13 +23,6 @@ namespace {
 constexpr int kPlaneThreads = 256;
 constexpr int kReduceBlocks = 128;  // fixed: the reduction's order depends on the candidate count only
 
-// what k_plane_emit needs of a participating frame: its stored points and order, and its index in the caller's list
-struct PlaneFrame {
-  const float4* p0;
-  const int* inv_perm;
-  int index;
-};
-
 struct PlaneStatsOut {
   double n, ev[3];
 };
@@ -58,18 +51,13 @@ __global__ void __launch_bounds__(kPlaneThreads) k_plane_flags(int n, const doub
 }
 
 // one thread per point g: a flagged point goes to slot pos[g] - 1 with its q, its id and (loc given) its stored local point
-__global__ void __launch_bounds__(kPlaneThreads) k_plane_emit(int n, int K, const int* __restrict__ offsets, const PlaneFrame* __restrict__ frames, const int* __restrict__ flags,
+__global__ void __launch_bounds__(kPlaneThreads) k_plane_emit(int n, int K, const gb_frame* __restrict__ frames, const int* __restrict__ flags,
                                                               const int* __restrict__ pos, const double4* __restrict__ pts, double4* __restrict__ cand,
                                                               unsigned long long* __restrict__ ids, float4* __restrict__ loc) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= n || !flags[g]) return;
-  int a = 0, b = K - 1;  // the last frame whose first point is at or before g
-  while (a < b) {
-    const int mid = (a + b + 1) / 2;
-    if (offsets[mid] <= g) a = mid; else b = mid - 1;
-  }
-  const int i = g - offsets[a], o = pos[g] - 1;
-  const PlaneFrame& F = frames[a];
+  const gb_frame& F = frames[gb_frame_of(frames, K, g)];
+  const int i = g - F.offset, o = pos[g] - 1;
   cand[o] = pts[g];
   ids[o] = ((unsigned long long)F.index << 32) | (unsigned)i;
   if (loc) loc[o] = F.p0[F.inv_perm ? F.inv_perm[i] : i];
@@ -115,12 +103,12 @@ __global__ void __launch_bounds__(kPlaneThreads) k_plane_reduce(const double4* _
 }
 
 // one CTA per participating frame f: the moments {N, mean, scatter} (GB_PLANE_MOMENTS) of its selected stored points, widened
-// to fp64, in two passes over its share of the compacted candidates [pos[offsets[f] - 1], pos[offsets[f + 1] - 1])
-__global__ void __launch_bounds__(kPlaneThreads) k_plane_moments(int K, int total, const int* __restrict__ offsets, const int* __restrict__ pos, const float4* __restrict__ loc,
+// to fp64, in two passes over its share of the compacted candidates [pos[o0 - 1], pos[o1 - 1]), [o0, o1) its points
+__global__ void __launch_bounds__(kPlaneThreads) k_plane_moments(const gb_frame* __restrict__ frames, const int* __restrict__ pos, const float4* __restrict__ loc,
                                                                  double* __restrict__ moments) {
   __shared__ double sh[6 * kPlaneThreads];
   const int f = blockIdx.x;
-  const int o0 = offsets[f], o1 = f + 1 < K ? offsets[f + 1] : total;
+  const int o0 = frames[f].offset, o1 = o0 + frames[f].n;
   const int begin = o0 > 0 ? pos[o0 - 1] : 0, end = o1 > 0 ? pos[o1 - 1] : 0;
   double s[3] = {0, 0, 0};
   for (int i = begin + threadIdx.x; i < end; i += blockDim.x) {
@@ -199,16 +187,16 @@ __global__ void __launch_bounds__(kPlaneThreads) k_plane_evm(const PlaneEvmDesc*
 }
 
 // The selection shared by the three patch calls: the candidates inside the sphere of radius r about the centre, from the
-// frames within max_frame_distance of it.  Host side: the participating frames, their shifted poses and tables.
+// frames within max_frame_distance of it.  Host side: the participating frames and their shifted poses; on the device, their one
+// descriptor table.
 struct PlaneSelection {
   std::vector<int> part;          // caller's indices of the participating frames
-  std::vector<int> offsets;       // their first point in the concatenation
   size_t total = 0;               // their points
+  gb_frame* d_frames = nullptr;   // their descriptors (gb_frame_table)
   int* d_pos = nullptr;           // inclusive scan of the flags; d_pos[total - 1] = the candidates
   double4* d_cand = nullptr;      // candidates' fp64 q, frame-major
   unsigned long long* d_ids = nullptr;
   float4* d_loc = nullptr;        // candidates' stored local points (factor only)
-  int* d_offsets = nullptr;
   double* d_partials = nullptr;
   unsigned* d_ticket = nullptr;
   PlaneStatsOut* d_stats = nullptr;
@@ -218,15 +206,9 @@ struct PlaneSelection {
 // validation shared by the three patch calls: every input before any launch
 gb_status plane_args(const gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, const gb_plane_patch_params* p) {
   GB_REQUIRE(ctx && p, "null argument");
-  GB_REQUIRE(K == 0 || (frames && poses), "null frames / poses");
   size_t total = 0;
-  for (size_t k = 0; k < K; k++) {
-    GB_REQUIRE(frames[k] && frames[k]->device == ctx->device, "null frame / frame on another device");
-    GB_REQUIRE(frames[k]->n < ((size_t)1 << 32), "a frame of 2^32 points or more");
-    for (int e = 0; e < 16; e++) GB_REQUIRE(std::isfinite(poses[16 * k + e]), "a non-finite pose");
-    total += frames[k]->n;
-  }
-  GB_REQUIRE(total < ((size_t)1 << 30), "too many points");
+  GB_CHECK(gb_frame_list_check(ctx, K, frames, poses, &total));
+  GB_REQUIRE(gb_all_finite(poses, 16 * K), "a non-finite pose");
   GB_REQUIRE(K < ((size_t)1 << 31), "too many frames");
   for (int a = 0; a < 3; a++) GB_REQUIRE(std::isfinite(p->center[a]), "a non-finite center");
   GB_REQUIRE(std::isfinite(p->radius) && p->radius > 0.0, "radius must be positive and finite");
@@ -243,32 +225,26 @@ gb_status plane_select(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, con
                        PlaneSelection& s) {
   std::vector<const gb_cloud*> pf;
   std::vector<double> shifted;
-  std::vector<PlaneFrame> h_frames;
   for (size_t k = 0; k < K; k++) {
     const double* T = poses + 16 * k;
     const double u[3] = {T[12] - p->center[0], T[13] - p->center[1], T[14] - p->center[2]};
     if (!(std::sqrt((u[0] * u[0] + u[1] * u[1]) + u[2] * u[2]) <= p->max_frame_distance)) continue;
     s.part.push_back((int)k);
-    s.offsets.push_back((int)s.total);
     s.total += frames[k]->n;
     pf.push_back(frames[k]);
     shifted.insert(shifted.end(), T, T + 16);
     for (int a = 0; a < 3; a++) shifted[shifted.size() - 4 + a] = u[a];
-    h_frames.push_back({frames[k]->p0, frames[k]->inv_perm, (int)k});
   }
   if (s.total == 0) return GB_OK;
   const size_t N = s.total, P = s.part.size(), cub_b = gb_cub_temp_bytes(N);
   const int n = (int)N;
-  const std::vector<char> table = gb_frame_table(P, pf.data(), shifted.data());
-  char *d_table, *d_cub;
-  PlaneFrame* d_frames;
+  const std::vector<gb_frame> table = gb_frame_table(P, pf.data(), shifted.data(), s.part.data());
+  char* d_cub;
   int* d_flags;
   double4* d_pts;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     d_cub = cv.take<char>(cub_b);
-    d_table = cv.take<char>(table.size());
-    d_frames = cv.take<PlaneFrame>(P);
-    s.d_offsets = cv.take<int>(P);
+    s.d_frames = cv.take<gb_frame>(P);
     d_flags = cv.take<int>(N);
     s.d_pos = cv.take<int>(N);
     d_pts = cv.take<double4>(N);
@@ -280,12 +256,12 @@ gb_status plane_select(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, con
     s.d_stats = cv.take<PlaneStatsOut>(1);
     s.d_moments = cv.take<double>(GB_PLANE_MOMENTS * P);
   }));
-  GB_CHECK(gb_upload(ctx, {{d_table, table.data(), table.size()}, {d_frames, h_frames.data(), sizeof(PlaneFrame) * P}, {s.d_offsets, s.offsets.data(), sizeof(int) * P}}));
-  GB_CHECK(gb_transform_frames(ctx, P, d_table, n, d_pts, nullptr));
+  GB_CHECK(gb_upload(ctx, {{s.d_frames, table.data(), sizeof(gb_frame) * P}}));
+  GB_CHECK(gb_transform_frames(ctx, P, s.d_frames, n, d_pts, nullptr));
   const int gb = (n + kPlaneThreads - 1) / kPlaneThreads;
   GB_CHECK(gb_launch(ctx, "k_plane_flags", k_plane_flags, gb, kPlaneThreads, 0, n, d_pts, r * r, d_flags));
   GB_CUB(ctx, cub::DeviceScan::InclusiveSum, d_cub, cub_b, d_flags, s.d_pos, n);
-  return gb_launch(ctx, "k_plane_emit", k_plane_emit, gb, kPlaneThreads, 0, n, (int)P, s.d_offsets, d_frames, d_flags, s.d_pos, d_pts, s.d_cand, s.d_ids, s.d_loc);
+  return gb_launch(ctx, "k_plane_emit", k_plane_emit, gb, kPlaneThreads, 0, n, (int)P, s.d_frames, d_flags, s.d_pos, d_pts, s.d_cand, s.d_ids, s.d_loc);
 }
 
 // n and the eigenvalues of the candidates inside radius r: one launch and one 32-byte copy with its synchronisation (none
@@ -383,7 +359,7 @@ extern "C" gb_status gb_plane_evm_factor_create(gb_ctx* ctx, size_t K, const gb_
   const size_t P = s.part.size();
   std::vector<double> mom(GB_PLANE_MOMENTS * P);
   if (s.total > 0) {
-    GB_CHECK(gb_launch(ctx, "k_plane_moments", k_plane_moments, (unsigned)P, kPlaneThreads, 0, (int)P, (int)s.total, s.d_offsets, s.d_pos, s.d_loc, s.d_moments));
+    GB_CHECK(gb_launch(ctx, "k_plane_moments", k_plane_moments, (unsigned)P, kPlaneThreads, 0, s.d_frames, s.d_pos, s.d_loc, s.d_moments));
     GB_CHECK(gb_download(ctx, {{mom.data(), s.d_moments, sizeof(double) * mom.size()}}));
   }
   size_t num_points = 0;
@@ -433,7 +409,7 @@ static gb_status plane_evm_args(const gb_ctx* ctx, size_t F, gb_factor* const* f
     keys += K;
     h_total += 36 * K * K;
   }
-  for (size_t e = 0; e < 16 * keys; e++) GB_REQUIRE(std::isfinite(poses[e]), "a non-finite pose");
+  GB_REQUIRE(gb_all_finite(poses, 16 * keys), "a non-finite pose");
   return GB_OK;
 }
 

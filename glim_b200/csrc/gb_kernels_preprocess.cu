@@ -717,14 +717,10 @@ extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n_, const double* xyz
 // =============================================================================================
 namespace {
 
-struct MergeFrame { const float4* p0; const float4* p1; const float* p2; const int* inv_perm; int n; int offset; double T[12]; };
-
-__global__ void k_merge_transform(int num_frames, const MergeFrame* __restrict__ frames, int total, double4* __restrict__ pts, double* __restrict__ cov6) {
+__global__ void k_merge_transform(int num_frames, const gb_frame* __restrict__ frames, int total, double4* __restrict__ pts, double* __restrict__ cov6) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= total) return;
-  int f = 0;
-  while (f + 1 < num_frames && frames[f + 1].offset <= g) f++;
-  const MergeFrame& F = frames[f];
+  const gb_frame& F = frames[gb_frame_of(frames, num_frames, g)];
   const int i = g - F.offset;
   const int slot = F.inv_perm ? F.inv_perm[i] : i;
   const float4 a0 = F.p0[slot];
@@ -763,28 +759,42 @@ __global__ void k_merge_emit(int n_upper, const int* __restrict__ keep, const in
 
 }  // namespace
 
-// the descriptor of cloud c at pose T (column-major 4x4) whose points are numbered from offset on
-static MergeFrame merge_frame(const gb_cloud* c, const double* T, int offset) {
-  MergeFrame F;
-  F.p0 = c->p0; F.p1 = c->p1; F.p2 = c->p2; F.inv_perm = c->inv_perm; F.n = (int)c->n; F.offset = offset;
-  for (int r = 0; r < 3; r++) for (int cc = 0; cc < 4; cc++) F.T[r * 4 + cc] = T[cc * 4 + r];
-  return F;
+gb_status gb_frame_list_check(const gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, size_t* total) {
+  GB_REQUIRE(K == 0 || (frames && poses), "null frames / poses");
+  *total = 0;
+  for (size_t k = 0; k < K; k++) {
+    GB_REQUIRE(frames[k] && frames[k]->device == ctx->device, "null frame / frame on another device");
+    GB_REQUIRE(frames[k]->n < ((size_t)1 << 32), "a frame of 2^32 points or more");
+    *total += frames[k]->n;
+  }
+  GB_REQUIRE(*total < ((size_t)1 << 30), "too many points");
+  return GB_OK;
 }
 
-std::vector<char> gb_frame_table(size_t K, const gb_cloud* const* frames, const double* poses) {
-  std::vector<char> table(sizeof(MergeFrame) * K);
-  size_t total = 0;
+bool gb_all_finite(const double* v, size_t n) {
+  for (size_t i = 0; i < n; i++)
+    if (!std::isfinite(v[i])) return false;
+  return true;
+}
+
+std::vector<gb_frame> gb_frame_table(size_t K, const gb_cloud* const* frames, const double* poses, const int* index) {
+  std::vector<gb_frame> table(K);
+  int offset = 0;
   for (size_t k = 0; k < K; k++) {
-    const MergeFrame F = merge_frame(frames[k], poses + k * 16, (int)total);
-    memcpy(table.data() + sizeof(MergeFrame) * k, &F, sizeof(F));
-    total += frames[k]->n;
+    const gb_cloud* c = frames[k];
+    const double* T = poses + 16 * k;  // column-major 4x4
+    gb_frame& F = table[k];
+    F.p0 = c->p0; F.p1 = c->p1; F.p2 = c->p2; F.normals = c->normals; F.inv_perm = c->inv_perm;
+    F.n = (int)c->n; F.offset = offset; F.index = index ? index[k] : (int)k;
+    for (int r = 0; r < 3; r++) for (int cc = 0; cc < 4; cc++) F.T[r * 4 + cc] = T[cc * 4 + r];
+    offset += F.n;
   }
   return table;
 }
 
-gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const void* d_table, int total, double4* pts, double* cov6) {
+gb_status gb_transform_frames(gb_ctx* ctx, size_t K, const gb_frame* d_table, int total, double4* pts, double* cov6) {
   if (total == 0) return GB_OK;
-  return gb_launch(ctx, "k_merge_transform", k_merge_transform, (total + 255) / 256, 256, 0, (int)K, (const MergeFrame*)d_table, total, pts, cov6);
+  return gb_launch(ctx, "k_merge_transform", k_merge_transform, (total + 255) / 256, 256, 0, (int)K, d_table, total, pts, cov6);
 }
 
 static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames, const double* poses, double resolution, int target, unsigned long long seed, double* out_xyzw, double* out_cov4x4, size_t* num_out, gb_cloud* cloud_out) {
@@ -795,18 +805,18 @@ static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames,
   if (total == 0) return GB_OK;
   const int n = (int)total;
   const size_t N = total, cub_b = gb_cub_temp_bytes(N);
-  const std::vector<char> table = gb_frame_table((size_t)K, frames, poses);
+  const std::vector<gb_frame> table = gb_frame_table((size_t)K, frames, poses, nullptr);
   gb_planes staged;  // fp32 planes of the merged cloud, in output order
   gb_sort_tmp t;
   int *d_cnt, *d_flags, *d_pos, *d_starts, *d_keep;
-  char* d_table;
+  gb_frame* d_table;
   double4 *d_pts, *d_vpts;
   double *d_cov, *d_vcov, *d_ocov;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     staged = gb_cloud_planes(cv, N, false);
     t = gb_take_sort_tmp(cv, N, cv.take<char>(cub_b), cub_b);
     d_cnt = cv.take<int>(64);
-    d_table = cv.take<char>(table.size());
+    d_table = cv.take<gb_frame>(K);
     d_pts = cv.take<double4>(N);
     d_vpts = cv.take<double4>(N);
     d_cov = cv.take<double>(6 * N);
@@ -819,7 +829,7 @@ static gb_status merge_frames(gb_ctx* ctx, int K, const gb_cloud* const* frames,
   }));
   GB_CUDA(cudaMemsetAsync(d_cnt, 0, 256, st));
   const int tb = 256, gb = (n + tb - 1) / tb;
-  GB_CHECK(gb_upload(ctx, {{d_table, table.data(), table.size()}}));
+  GB_CHECK(gb_upload(ctx, {{d_table, table.data(), sizeof(gb_frame) * K}}));
   GB_CHECK(gb_transform_frames(ctx, (size_t)K, d_table, n, d_pts, d_cov));
   GB_CHECK(gb_grid_keys(ctx, n, d_pts, 1.0 / resolution, nullptr, t.keys, t.idx));
   GB_CHECK(gb_group_by_key(ctx, n, t, d_flags, d_pos));
@@ -844,14 +854,10 @@ extern "C" gb_status gb_merge_frames(gb_ctx* ctx, size_t K, const gb_cloud* cons
   *num_out = 0;
   if (out_cloud) *out_cloud = nullptr;
   if (K == 0) return GB_OK;
-  GB_REQUIRE(frames && poses, "null frames / poses");
   GB_REQUIRE(resolution > 0.0, "downsample_resolution must be positive");
   size_t total = 0;
-  for (size_t k = 0; k < K; k++) {
-    GB_REQUIRE(frames[k] && frames[k]->device == ctx->device, "null frame / frame on another device");
-    total += frames[k]->n;
-  }
-  GB_REQUIRE(total < (size_t)1 << 30 && K < 65536, "too many points / frames");
+  GB_CHECK(gb_frame_list_check(ctx, K, frames, poses, &total));  // poses may be non-finite: their points get no voxel key
+  GB_REQUIRE(K < 65536, "too many frames");
   GB_ENTER(ctx);
   gb_owned<gb_cloud> c(out_cloud ? new (std::nothrow) gb_cloud() : nullptr, cloud_free);
   if (out_cloud && !c) return GB_ERR_INTERNAL;

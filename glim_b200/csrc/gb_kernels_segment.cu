@@ -34,13 +34,6 @@ namespace {
 constexpr int kSegThreads = 256;
 constexpr int kHookThreads = 128;
 
-// what gb_concat_frames' emit needs of frame k beyond the shared transform: its normals, its storage order, R row-major
-struct ConcatFrame {
-  const float4* normals;
-  const int* inv_perm;
-  double R[9];
-};
-
 // flags[g] = 1 iff point g of the concatenation (fp64 q) is kept: always without a window
 __global__ void k_concat_flags(int n, const double4* __restrict__ pts, int windowed, double inv, int3 lo, int3 hi, int* __restrict__ flags) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
@@ -53,30 +46,25 @@ __global__ void k_concat_flags(int n, const double4* __restrict__ pts, int windo
 
 // one thread per point g of the concatenation: a kept point goes to slot pos[g] - 1 as fp32 planes (zero covariances unless
 // every frame has them), its rotated normal and its id
-__global__ void k_concat_emit(int n, int K, const int* __restrict__ offsets, const ConcatFrame* __restrict__ frames, const int* __restrict__ flags,
+__global__ void k_concat_emit(int n, int K, const gb_frame* __restrict__ frames, const int* __restrict__ flags,
                               const int* __restrict__ pos, const double4* __restrict__ pts, const double* __restrict__ cov6, int covs, float4* __restrict__ s0,
                               float4* __restrict__ s1, float* __restrict__ s2, float4* __restrict__ sn, unsigned long long* __restrict__ ids) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= n || !flags[g]) return;
-  int a = 0, b = K - 1;  // the last frame whose first point is at or before g
-  while (a < b) {
-    const int mid = (a + b + 1) / 2;
-    if (offsets[mid] <= g) a = mid; else b = mid - 1;
-  }
-  const int i = g - offsets[a], o = pos[g] - 1;
+  const gb_frame& F = frames[gb_frame_of(frames, K, g)];
+  const int i = g - F.offset, o = pos[g] - 1;
   const double4 p = pts[g];
   const double* c = cov6 + 6 * (size_t)g;
   s0[o] = make_float4((float)p.x, (float)p.y, (float)p.z, covs ? (float)c[0] : 0.f);
   s1[o] = covs ? make_float4((float)c[1], (float)c[2], (float)c[3], (float)c[4]) : make_float4(0.f, 0.f, 0.f, 0.f);
   s2[o] = covs ? (float)c[5] : 0.f;
   if (sn) {
-    const ConcatFrame& F = frames[a];
     const float4 nr = F.normals[F.inv_perm ? F.inv_perm[i] : i];
     float v[3];
-    seg_rotate_normal(F.R, nr.x, nr.y, nr.z, v);
+    seg_rotate_normal(F.T, nr.x, nr.y, nr.z, v);
     sn[o] = make_float4(v[0], v[1], v[2], 0.f);
   }
-  ids[o] = ((unsigned long long)a << 32) | (unsigned)i;
+  ids[o] = ((unsigned long long)F.index << 32) | (unsigned)i;
 }
 
 // What gb_region_growing leaves for the host, ahead of the selection and the labels in one copy.
@@ -161,8 +149,6 @@ __global__ void __launch_bounds__(kHookThreads) k_rg_dilate(int n, const int4* _
   }
   sel[j] = s;
 }
-
-void grid_release(gb_point_grid* g) { gb_point_grid_destroy(g); }
 
 // a point grid of the cloud at 1.05 r and its search half-width for (float)(r^2)
 gb_status rg_grid(gb_ctx* ctx, const gb_cloud* cloud, double r, gb_owned<gb_point_grid>& grid, int& m, float& max_d2) {
@@ -447,18 +433,14 @@ extern "C" gb_status gb_concat_frames(gb_ctx* ctx, size_t K, const gb_cloud* con
   GB_REQUIRE(ctx && out_cloud && num_out, "null argument");
   *out_cloud = nullptr;
   *num_out = 0;
-  GB_REQUIRE(K == 0 || (frames && poses), "null frames / poses");
   size_t total = 0;
+  GB_CHECK(gb_frame_list_check(ctx, K, frames, poses, &total));
+  GB_REQUIRE(gb_all_finite(poses, 16 * K), "a non-finite pose");
   bool covs = K > 0, normals = K > 0;
   for (size_t k = 0; k < K; k++) {
-    GB_REQUIRE(frames[k] && frames[k]->device == ctx->device, "null frame / frame on another device");
-    GB_REQUIRE(frames[k]->n < ((size_t)1 << 32), "a frame of 2^32 points or more");
-    for (int e = 0; e < 16; e++) GB_REQUIRE(std::isfinite(poses[16 * k + e]), "a non-finite pose");
-    total += frames[k]->n;
     covs = covs && frames[k]->covs;
     normals = normals && (frames[k]->normals || frames[k]->n == 0);
   }
-  GB_REQUIRE(total < ((size_t)1 << 30), "too many points");
   if (window) {
     GB_REQUIRE(std::isfinite(window->cell_size) && window->cell_size > 0.0, "cell_size must be positive and finite");
     for (int a = 0; a < 3; a++) GB_REQUIRE(window->lo[a] <= window->hi[a], "lo > hi");
@@ -474,40 +456,25 @@ extern "C" gb_status gb_concat_frames(gb_ctx* ctx, size_t K, const gb_cloud* con
   }
   const int n = (int)total;
   const size_t N = total, cub_b = gb_cub_temp_bytes(N);
-  const std::vector<char> table = gb_frame_table(K, frames, poses);
-  std::vector<ConcatFrame> h_frames(K);
-  std::vector<int> h_offsets(K);
-  size_t off = 0;
-  for (size_t k = 0; k < K; k++) {
-    const double* T = poses + 16 * k;
-    h_frames[k].normals = frames[k]->normals;
-    h_frames[k].inv_perm = frames[k]->inv_perm;
-    for (int r = 0; r < 3; r++)
-      for (int cc = 0; cc < 3; cc++) h_frames[k].R[3 * r + cc] = T[4 * cc + r];
-    h_offsets[k] = (int)off;
-    off += frames[k]->n;
-  }
+  const std::vector<gb_frame> table = gb_frame_table(K, frames, poses, nullptr);
   gb_planes staged;
   gb_sort_tmp t;
-  char* d_table;
-  ConcatFrame* d_frames;
-  int *d_offsets, *d_flags, *d_pos;
+  gb_frame* d_table;
+  int *d_flags, *d_pos;
   double4* d_pts;
   double* d_cov;
   unsigned long long* d_ids;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
     staged = gb_cloud_planes(cv, N, normals);
     t = gb_take_sort_tmp(cv, N, cv.take<char>(cub_b), cub_b);
-    d_table = cv.take<char>(table.size());
-    d_frames = cv.take<ConcatFrame>(K);
-    d_offsets = cv.take<int>(K);
+    d_table = cv.take<gb_frame>(K);
     d_flags = cv.take<int>(N);
     d_pos = cv.take<int>(N);
     d_pts = cv.take<double4>(N);
     d_cov = cv.take<double>(6 * N);
     d_ids = cv.take<unsigned long long>(N);
   }));
-  GB_CHECK(gb_upload(ctx, {{d_frames, h_frames.data(), sizeof(ConcatFrame) * K}, {d_offsets, h_offsets.data(), sizeof(int) * K}, {d_table, table.data(), table.size()}}));
+  GB_CHECK(gb_upload(ctx, {{d_table, table.data(), sizeof(gb_frame) * K}}));
   GB_CHECK(gb_transform_frames(ctx, K, d_table, n, d_pts, d_cov));
   const int gb = (n + kSegThreads - 1) / kSegThreads;
   const double inv = window ? 1.0 / window->cell_size : 0.0;
@@ -515,7 +482,7 @@ extern "C" gb_status gb_concat_frames(gb_ctx* ctx, size_t K, const gb_cloud* con
   const int3 hi = window ? make_int3(window->hi[0], window->hi[1], window->hi[2]) : make_int3(0, 0, 0);
   GB_CHECK(gb_launch(ctx, "k_concat_flags", k_concat_flags, gb, kSegThreads, 0, n, d_pts, window ? 1 : 0, inv, lo, hi, d_flags));
   GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, cub_b, d_flags, d_pos, n);
-  GB_CHECK(gb_launch(ctx, "k_concat_emit", k_concat_emit, gb, kSegThreads, 0, n, (int)K, d_offsets, d_frames, d_flags, d_pos, d_pts, d_cov, covs ? 1 : 0,
+  GB_CHECK(gb_launch(ctx, "k_concat_emit", k_concat_emit, gb, kSegThreads, 0, n, (int)K, d_table, d_flags, d_pos, d_pts, d_cov, covs ? 1 : 0,
                      staged.p0, staged.p1, staged.p2, staged.normals, d_ids));
   int count = 0;
   GB_CHECK(gb_download(ctx, {{&count, d_pos + (n - 1), sizeof(int)}}));

@@ -470,7 +470,7 @@ struct InsertScratch {
   int *flags, *pos, *starts, *keep, *kpos, *dropped;
   int4* vcoord;
   unsigned long long* info;
-  char* frame;
+  gb_frame* frame;
   double4* pts = nullptr;
   double* cov = nullptr;
 };
@@ -566,7 +566,7 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
   gb_dev_block table(ctx->device), base(ctx->device);  // the new blocks until the hand-over, then m's replaced ones (base ends first)
   if (N > 0) {
     const size_t cub_b = gb_cub_temp_bytes((size_t)N);
-    const std::vector<char> frame = gb_frame_table(1, &cloud, T);
+    const std::vector<gb_frame> frame = gb_frame_table(1, &cloud, T, nullptr);
     InsertScratch s;
     GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
       s.t = gb_take_sort_tmp(cv, (size_t)N, cv.take<char>(cub_b), cub_b);
@@ -578,14 +578,14 @@ gb_status map_insert(gb_ctx* ctx, gb_voxelmap* m, const gb_cloud* cloud, const d
       s.vcoord = cv.take<int4>(N);
       s.dropped = cv.take<int>(1);
       s.info = cv.take<unsigned long long>(2);
-      s.frame = cv.take<char>(frame.size());
+      s.frame = cv.take<gb_frame>(1);
       if (np > 0) {
         s.pts = cv.take<double4>(np);
         s.cov = cv.take<double>(6 * (size_t)np);
       }
       rule.scratch(cv, (size_t)N);
     }));
-    if (np > 0) GB_CHECK(gb_upload(ctx, {{s.frame, frame.data(), frame.size()}}));
+    if (np > 0) GB_CHECK(gb_upload(ctx, {{s.frame, frame.data(), sizeof(gb_frame)}}));
     if (m->num_voxels > 0) GB_CHECK(rule.old_keys(ctx, s.t));
     if (np > 0) {
       GB_CHECK(gb_transform_frames(ctx, 1, s.frame, np, s.pts, s.cov));
@@ -882,6 +882,7 @@ extern "C" gb_status gb_point_grid_download(const gb_point_grid* grid, int32_t* 
   return download_records(g->voxels, P, nullptr, xyz, cov6);
 }
 extern "C" gb_status gb_point_grid_destroy(gb_point_grid* grid) { return gb_voxelmap_destroy(grid_map(grid)); }
+void grid_release(gb_point_grid* g) { gb_point_grid_destroy(g); }
 
 // ---------------------------------------------------------------------------------------------
 // Morton reordering of a new cloud (PointCloudGPU::clone keeps the caller's order on the host side of the

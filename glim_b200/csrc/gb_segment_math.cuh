@@ -1,12 +1,37 @@
 // gb_segment_math.cuh -- the per-point and per-pair arithmetic of the map segmentation (gb_concat_frames, gb_region_growing,
-// gb_kernels_segment.cu), kept free of anything that only exists on the device so that the SAME TEXT also compiles for the
-// host: tests/cpp/segment_math_host.cpp builds it with g++ -ffp-contract=off and tests/test_segment_host.py checks it against
-// the numpy restatement of the rules (tests/segment_oracle.py).  The rules are written once, in include/glim_b200.h.
+// gb_kernels_segment.cu), and the posed frame list that gb_concat_frames shares with gb_merge_frames, the map insert and the
+// plane selection (gb_frame, gb_frame_of), kept free of anything that only exists on the device so that the SAME TEXT also
+// compiles for the host: tests/cpp/segment_math_host.cpp builds it with g++ -ffp-contract=off and tests/test_segment_host.py
+// checks it against the numpy restatement of the rules (tests/segment_oracle.py).  The rules are written once, in
+// include/glim_b200.h.
 #pragma once
 #include "gb_grid_math.cuh"  // GB_HD, gb_coord, point_d2, grid_within, the fp32 intrinsics' host shims
 #include "gb_cov_math.cuh"   // the fp64 intrinsics' host shims
 
+// The descriptor of frame k of a posed frame list (gb_frame_table): the cloud's stored planes, normals and storage order, its
+// point count, its first point in the concatenation of the list, the caller's index of the frame, and the rows of its 3x4 pose.
+struct gb_frame {
+  const float4* p0;
+  const float4* p1;
+  const float* p2;
+  const float4* normals;
+  const int* inv_perm;
+  int n, offset, index;
+  double T[12];
+};
+
 namespace {
+
+// The frame of K (K >= 1) that holds point g of the concatenation: the last whose first point is at or before g.  A frame
+// with no points shares its offset with the next one, so it never holds g.
+GB_HD int gb_frame_of(const gb_frame* frames, int K, int g) {
+  int a = 0, b = K - 1;
+  while (a < b) {
+    const int mid = (a + b + 1) / 2;
+    if (frames[mid].offset <= g) a = mid; else b = mid - 1;
+  }
+  return a;
+}
 
 // The 21-bit key range of every grid: a point takes part in a search of a grid of fp32 cell inverse inv iff it is finite and
 // each gb_coord(x, inv) lies in [-2^20, 2^20) (the points without a key are in no cell of the grid).
@@ -32,11 +57,11 @@ GB_HD unsigned long long seg_seed_key(float4 p, float qx, float qy, float qz, in
   return ((unsigned long long)(uint32_t)__float_as_int(point_d2(p, qx, qy, qz)) << 32) | (uint32_t)i;
 }
 
-// A point's normal rotated into the world frame: n' = R n, row r as (R_r0 nx + R_r1 ny) + R_r2 nz in un-contracted fp64 (R
-// row-major), stored fp32, not renormalised.
-GB_HD void seg_rotate_normal(const double* R, float nx, float ny, float nz, float* out) {
+// A point's normal rotated into the world frame: n' = R n, row r as (R_r0 nx + R_r1 ny) + R_r2 nz in un-contracted fp64 (T:
+// the rows of the 3x4 pose [R | t], gb_frame::T), stored fp32, not renormalised.
+GB_HD void seg_rotate_normal(const double* T, float nx, float ny, float nz, float* out) {
   for (int r = 0; r < 3; r++)
-    out[r] = (float)__dadd_rn(__dadd_rn(__dmul_rn(R[3 * r], (double)nx), __dmul_rn(R[3 * r + 1], (double)ny)), __dmul_rn(R[3 * r + 2], (double)nz));
+    out[r] = (float)__dadd_rn(__dadd_rn(__dmul_rn(T[4 * r], (double)nx), __dmul_rn(T[4 * r + 1], (double)ny)), __dmul_rn(T[4 * r + 2], (double)nz));
 }
 
 // The window test of gb_concat_frames: floor(q * (1.0 / cell_size)) in fp64 within [lo, hi] on every axis; never for a

@@ -765,14 +765,12 @@ def merge_frames_gpu(poses, frames, downsample_resolution: float, target_num_poi
     """gtsam_points::merge_frames(poses, frames, downsample_resolution, target_num_points) on the device (sub_mapping.cpp:481-497).
     poses: K x (4,4) T_origin_frame; frames: K PointCloudGPU.  -> (points (M,4), covs (M,4,4) [i,row,col], PointCloudGPU)"""
     ctx = ctx or frames[0].ctx
-    K = len(frames)
-    arr = (C.c_void_p * K)(*[f.h for f in frames])
-    T = pose16(np.stack([np.asarray(p, dtype=np.float64) for p in poses]))
+    K, arr, T = _frames(frames, poses)
     cap = sum(f.n for f in frames)
     pts = np.empty((cap, 4)) if host_outputs else None
     cov = np.empty((cap, 16)) if host_outputs else None
     m = C.c_size_t()
-    h = PointCloudGPU._create(lib().gb_merge_frames, ctx.h, K, C.cast(arr, C.c_void_p), ptr(T), float(downsample_resolution), int(target_num_points), int(seed), ptr(pts), ptr(cov),
+    h = PointCloudGPU._create(lib().gb_merge_frames, ctx.h, K, arr, ptr(T), float(downsample_resolution), int(target_num_points), int(seed), ptr(pts), ptr(cov),
                               C.byref(m))
     cloud = PointCloudGPU(ctx, h, m.value) if h.value else None
     if not host_outputs:
@@ -826,17 +824,15 @@ def concat_frames(poses, frames, window=None, ctx: Context | None = None):
     """The submaps' device clouds in one world-frame device cloud (gb_concat_frames): poses K x (4,4) T_world_frame, frames K
     PointCloudGPU, window None (every point) or (cell_size, lo (3,), hi (3,)) inclusive cell bounds.  -> (PointCloudGPU, ids
     (M,) uint64 = (frame << 32) | original index, the map editor's point ids)"""
-    K = len(frames)
-    ctx = ctx or (frames[0].ctx if K else default_context())
-    arr = (C.c_void_p * max(K, 1))(*[f.h for f in frames])
-    T = pose16(np.stack([np.asarray(p, dtype=np.float64) for p in poses])) if K else np.zeros((0, 16))
+    ctx = ctx or (frames[0].ctx if len(frames) else default_context())
+    K, arr, T = _frames(frames, poses)
     w = None
     if window is not None:
         cell, lo, hi = window
         w = capi.CellWindow(float(cell), (C.c_int32 * 3)(*[int(v) for v in lo]), (C.c_int32 * 3)(*[int(v) for v in hi]))
     ids = np.empty(sum(f.n for f in frames), np.uint64)
     h, m = C.c_void_p(), C.c_size_t()
-    check(lib().gb_concat_frames(ctx.h, K, C.cast(arr, C.c_void_p), ptr(T), C.byref(w) if w is not None else None, C.byref(h), ptr(ids), C.byref(m)))
+    check(lib().gb_concat_frames(ctx.h, K, arr, ptr(T), C.byref(w) if w is not None else None, C.byref(h), ptr(ids), C.byref(m)))
     return PointCloudGPU(ctx, h, m.value), ids[: m.value].copy()
 
 

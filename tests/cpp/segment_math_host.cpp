@@ -1,7 +1,9 @@
 // Host build of the map segmentation's per-point and per-pair arithmetic (glim_b200/csrc/gb_segment_math.cuh, the text
-// k_concat_flags, k_concat_emit and the k_rg_* kernels compile).  tests/test_segment_host.py compiles this with
+// k_merge_transform, k_concat_flags, k_concat_emit, k_plane_emit and the k_rg_* kernels compile).  tests/test_segment_host.py compiles this with
 // g++ -ffp-contract=off and compares it with the numpy restatement (tests/segment_oracle.py).
 #include "../../glim_b200/csrc/gb_segment_math.cuh"
+
+#include <vector>
 
 extern "C" {
 
@@ -27,9 +29,21 @@ void seed_keys(int n, const float* xyz, const float* q, unsigned long long* out)
   }
 }
 
-// out (n x 3) = R (row-major 9) applied to the fp32 normals
-void rotate_normals(int n, const double* R, const float* nrm, float* out) {
-  for (int i = 0; i < n; i++) seg_rotate_normal(R, nrm[3 * i], nrm[3 * i + 1], nrm[3 * i + 2], out + 3 * i);
+// out (n x 3) = R of the 3x4 pose rows T (row-major 12, gb_frame::T) applied to the fp32 normals
+void rotate_normals(int n, const double* T, const float* nrm, float* out) {
+  for (int i = 0; i < n; i++) seg_rotate_normal(T, nrm[3 * i], nrm[3 * i + 1], nrm[3 * i + 2], out + 3 * i);
+}
+
+// out[g] = gb_frame_of for every point g of the concatenation of K >= 1 frames of counts[k] points, the table's offsets
+// numbered as gb_frame_table numbers them
+void frame_of(int K, const int* counts, int* out) {
+  std::vector<gb_frame> frames(K);
+  int total = 0;
+  for (int k = 0; k < K; k++) {
+    frames[k].offset = total;
+    total += counts[k];
+  }
+  for (int g = 0; g < total; g++) out[g] = gb_frame_of(frames.data(), K, g);
 }
 
 // out[i] = seg_in_window of fp64 q_i

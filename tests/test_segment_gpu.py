@@ -200,10 +200,16 @@ def upload_frame(ctx, xyz, C, nrm):
     return upload(ctx, xyz, nrm, c4)
 
 
-@pytest.mark.parametrize("window", [None, (2.0, (-10, -9, -10), (10, 8, 9))])
-def test_concat_bit_exact(ctx, window):
+WINDOW = (2.0, (-10, -9, -10), (10, 8, 9))
+
+
+@pytest.mark.parametrize("window, K, n, empty_every", [pytest.param(None, 4, 3000, 0, id="None"), pytest.param(WINDOW, 4, 3000, 0, id="window1"),
+                                                      pytest.param(None, 64, 300, 3, id="empty-frames"), pytest.param(WINDOW, 64, 300, 3, id="empty-frames-window")])
+def test_concat_bit_exact(ctx, window, K, n, empty_every):
     rng = np.random.default_rng(8)
-    poses, host = frames_and_poses(rng, 4, 3000)
+    poses, host = frames_and_poses(rng, K, n)
+    if empty_every:  # frames with no points among the others, the first and the last included
+        host = [tuple(a[:0] for a in h) if k % empty_every == 0 else h for k, h in enumerate(host)]
     frames = [upload_frame(ctx, *h) for h in host]
     cloud, ids = gpu.concat_frames(poses, frames, window=window, ctx=ctx)
     ref = so.concat_frames(poses, [as_oracle_frame(*h) for h in host], window)
@@ -243,7 +249,8 @@ def test_concat_carries_only_common_planes(ctx):
 
 def test_merge_frames_unchanged_by_the_shared_transform(ctx):
     """gb_merge_frames without downsampling effect (a tiny voxel) keeps the transformed points: they match the oracle's
-    transform of the same frames, through the same kernel gb_concat_frames uses"""
+    transform of the same frames, through the same kernel gb_concat_frames uses.  A frame at a NaN pose is accepted and
+    changes nothing: its points get no voxel key, and the other frames keep their order."""
     rng = np.random.default_rng(10)
     poses, host = frames_and_poses(rng, 3, 400)
     host = [(x[np.isfinite(x).all(axis=1)], C[np.isfinite(x).all(axis=1)], n) for x, C, n in host]
@@ -255,6 +262,9 @@ def test_merge_frames_unchanged_by_the_shared_transform(ctx):
     assert np.array_equal(rows(pts[:, :3]), rows(q))
     cat, _ = gpu.concat_frames(poses, frames, ctx=ctx)
     assert np.array_equal(cat.download()[0], q.astype(F32))
+    nan_pose = np.full((4, 4), np.nan)
+    pts_nan, covs_nan, _ = gpu.merge_frames_gpu(poses[:1] + [nan_pose] + poses[1:], frames[:1] + [frames[1]] + frames[1:], 1e-4, ctx=ctx)
+    assert np.array_equal(pts_nan, pts) and np.array_equal(covs_nan, covs)
 
 
 def test_editor_recipe_end_to_end(ctx):

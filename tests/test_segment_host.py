@@ -2,6 +2,7 @@
   * the per-point and per-pair functions of glim_b200/csrc/gb_segment_math.cuh, compiled for the host
     (tests/cpp/segment_math_host.cpp), against the numpy restatement (tests/segment_oracle.py) on seeded and adversarial inputs:
     NaN and zero normals, coincident points, d2 exactly at the bound, saturated keys;
+  * the frame lookup of the posed frame list (gb_frame_of) against np.searchsorted, empty frames included;
   * the union-find hook run sequentially on random edge lists agrees with scipy's connected_components, whatever the order;
   * the oracle itself against a pure-Python breadth-first search on small scenes;
   * the arguments gb_region_growing and gb_concat_frames reject before they touch a device."""
@@ -32,6 +33,7 @@ def hl(tmp_path_factory):
     L.seed_keys.argtypes = [C.c_int, vp, vp, vp]
     L.rotate_normals.argtypes = [C.c_int, vp, vp, vp]
     L.in_window.argtypes = [C.c_int, vp, C.c_double, vp, vp, vp]
+    L.frame_of.argtypes = [C.c_int, vp, vp]
     L.union_find.argtypes = [C.c_int, C.c_int, vp, vp, vp]
     return L
 
@@ -107,7 +109,7 @@ def test_seed_keys_order_as_the_oracle(hl):
     assert so.seed_of(bad, [0, 0, 0]) == -1
 
 
-def test_rotate_normals_and_window_match_oracle(hl):
+def test_rotate_normals_by_pose_rows_and_window_match_oracle(hl):
     rng = np.random.default_rng(4)
     n = 2000
     nrm = unit(rng, n)
@@ -123,7 +125,7 @@ def test_rotate_normals_and_window_match_oracle(hl):
         T[:3, :3] = R
         T[:3, 3] = rng.uniform(-100, 100, 3)
         out = np.empty((n, 3), F32)
-        hl.rotate_normals(n, p(c(R, F64)), p(c(nrm, F32)), p(out))
+        hl.rotate_normals(n, p(c(T[:3], F64)), p(c(nrm, F32)), p(out))  # the pose rows, translation column included
         ref = so.rotate_normals(T, nrm).astype(F32)
         assert np.array_equal(out, ref, equal_nan=True)
     cell = 2.0
@@ -134,6 +136,19 @@ def test_rotate_normals_and_window_match_oracle(hl):
     ref = so.in_window(qq, cell, lo, hi)
     assert np.array_equal(out.astype(bool), ref)
     assert ref.sum() > 50 and not ref[-4] and not ref[-3] and ref[-2] and ref[-1]  # faces of the window are inclusive
+
+
+@pytest.mark.parametrize("counts", [[0, 0, 5, 3], [4, 0, 0, 7, 0, 1], [6, 2, 0, 0], [1], [37],
+                                    np.random.default_rng(5).integers(0, 3, 3000) * np.random.default_rng(6).integers(0, 40, 3000)],
+                         ids=["empty-first", "empty-middle", "empty-last", "one-point", "one-frame", "3000-frames"])
+def test_frame_of_matches_searchsorted(hl, counts):
+    counts = c(counts, np.int32)
+    offsets = np.concatenate([[0], np.cumsum(counts)[:-1]])
+    g = np.arange(int(counts.sum()))
+    out = np.empty(len(g), np.int32)
+    hl.frame_of(len(counts), p(counts), p(out))
+    assert np.array_equal(out, np.searchsorted(offsets, g, side="right") - 1)
+    assert (counts[out] > 0).all()  # an empty frame never holds a point
 
 
 @pytest.mark.parametrize("seed", range(5))
