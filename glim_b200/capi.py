@@ -108,6 +108,10 @@ _SIGNATURES = {
     "gb_region_growing": ([vp, vp, vp, vp, vp, vp, vp], st),
     "gb_min_cut_default_params": ([vp], st),
     "gb_min_cut": ([vp, vp, vp, vp, vp, vp, vp, vp], st),
+    "gb_select_gizmo": ([vp, sz, vp, vp, vp, i32, vp, vp], st),
+    "gb_select_radius_default_params": ([vp], st),
+    "gb_select_radius": ([vp, vp, vp, vp, vp, vp], st),
+    "gb_remove_points": ([vp, sz, vp, sz, vp, vp, vp, vp], st),
     "gb_plane_patch_default_params": ([vp], st),
     "gb_plane_patch": ([vp, sz, vp, vp, vp, vp, vp], st),
     "gb_plane_auto_radius": ([vp, sz, vp, vp, vp, vp], st),
@@ -223,6 +227,31 @@ class MinCutResult(C.Structure):
 # gb_min_cut_result::status
 MINCUT_FOUND, MINCUT_NO_SEED, MINCUT_NOT_CONVERGED = 0, 1, 2
 MINCUT_STATUS_NAMES = {0: "FOUND", 1: "NO_SEED", 2: "NOT_CONVERGED"}
+
+# gb_select_gizmo's shape
+GIZMO_BOX, GIZMO_SPHERE = 0, 1
+
+
+class SelectRadiusParams(C.Structure):
+    """gb_select_radius_params (include/glim_b200.h)."""
+    _fields_ = [("radius", C.c_double), ("radius_offset", C.c_double), ("stddev_thresh", C.c_double), ("mode", C.c_int32), ("k", C.c_int32)]
+
+
+class SelectRadiusResult(C.Structure):
+    """gb_select_radius_result (include/glim_b200.h)."""
+    _fields_ = [("status", C.c_int32), ("num_participants", C.c_size_t), ("num_selected", C.c_size_t), ("threshold", C.c_double)]
+
+
+# gb_select_radius_params::mode and gb_select_radius_result::status
+RADIUS_INSIDE, RADIUS_OUTLIERS = 0, 1
+RADIUS_OK, RADIUS_NOT_ENOUGH_POINTS = 0, 1
+RADIUS_STATUS_NAMES = {0: "OK", 1: "NOT_ENOUGH_POINTS"}
+
+
+class RemovePointsResult(C.Structure):
+    """gb_remove_points_result (include/glim_b200.h)."""
+    _fields_ = [("num_removed", C.c_size_t), ("num_ignored", C.c_size_t), ("num_changed", C.c_size_t)]
+
 
 class PlanePatchParams(C.Structure):
     """gb_plane_patch_params (include/glim_b200.h)."""

@@ -572,6 +572,10 @@ struct KnnTmp {
 KnnTmp take_knn_tmp(Carver& cv, int n, void* cub, size_t cub_bytes);
 gb_status knn_device(gb_ctx* ctx, int n, const int* d_count, const double4* d_pts, int k, double h0, int* neighbors, const KnnTmp& t);
 bool gb_knn_instantiated(int k);
+// The mean neighbour distance of the statistical outlier removal (gb_kernels_preprocess.cu), shared with gb_select_radius:
+// for each of the first *d_count of n points, d_i = (the sum over its k-NN row, in row order, of the fp64 distances) / k and
+// dist2[i] = d_i^2, each operation rounded; 0 for the slots beyond.  One launch.
+gb_status gb_sor_dists(gb_ctx* ctx, int n, const int* d_count, const double4* pts, const int* nb, int k, double* dist, double* dist2);
 // k_grid_keys of the voxel-grid paths: key = packed floor(p * inv_res) in fp64 (~0 for non-finite / out-of-range points,
 // and for every point with keep[i] == 0 when keep is given), idx[i] = i.  One launch.
 gb_status gb_grid_keys(gb_ctx* ctx, int n, const double4* pts, double inv_res, const int* keep, unsigned long long* keys, int* idx);

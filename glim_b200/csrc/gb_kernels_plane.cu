@@ -1,11 +1,14 @@
 // gb_kernels_plane.cu -- the interactive viewer's plane bundle adjustment on the device (sm_90a): the patch of submap points
 // around a picked point (gb_plane_patch), its auto radius (gb_plane_auto_radius), and the PlaneEVMFactor made of it
-// (gb_plane_evm_factor_create, gb_plane_evm_linearize, gb_plane_evm_error).  The rules are written once in
-// include/glim_b200.h; the per-factor arithmetic is gb_plane_math.cuh, which the host test build compiles as well.
+// (gb_plane_evm_factor_create, gb_plane_evm_linearize, gb_plane_evm_error), and the map editor's gizmo selection
+// (gb_select_gizmo), which shares the patch's selection.  The rules are written once in include/glim_b200.h; the per-factor
+// arithmetic is gb_plane_math.cuh and the inside tests gb_editor_math.cuh, which the host test builds compile as well.
 //
 //   selection            the participating frames (host), k_merge_transform over them at the shifted poses [R | t - c]
 //                        (gb_transform_frames, without covariances), k_plane_flags (inside the sphere), a cub inclusive
 //                        scan, k_plane_emit (the candidates' fp64 q, ids and, for a factor, stored local points, frame-major)
+//   gizmo                the same four launches over every frame at M_k = T_local_world T_world_submap_k (composed on the
+//                        host), k_plane_flags with the box or the unit sphere, and only the ids emitted
 //   statistics           k_plane_reduce: one fixed-grid fp64 reduction of {n, sum q, sum q q^T} over the candidates inside a
 //                        radius, whose last block turns it into the eigenvalues; one 32-byte copy back
 //   factor               k_plane_moments: one CTA per participating frame, two passes over its selected points; one copy back
@@ -13,6 +16,7 @@
 //                        b and the (6K)^2 Hessian
 #include "gb_internal.cuh"
 #include "gb_plane_math.cuh"
+#include "gb_editor_math.cuh"
 
 #include <cub/cub.cuh>
 #include <cmath>
@@ -26,8 +30,6 @@ constexpr int kReduceBlocks = 128;  // fixed: the reduction's order depends on t
 struct PlaneStatsOut {
   double n, ev[3];
 };
-
-__device__ __forceinline__ double plane_d2(double4 q) { return __dadd_rn(__dadd_rn(__dmul_rn(q.x, q.x), __dmul_rn(q.y, q.y)), __dmul_rn(q.z, q.z)); }
 
 // v[0 .. W) summed over the block in a fixed tree order; the block's sums in v of thread 0.  sh: W x blockDim doubles.
 template <int W>
@@ -44,13 +46,17 @@ __device__ void block_sum(double (&v)[W], double* sh) {
   __syncthreads();
 }
 
-// flags[g] = point g (fp64 q about the centre) lies inside the sphere; NaN never does
-__global__ void __launch_bounds__(kPlaneThreads) k_plane_flags(int n, const double4* __restrict__ pts, double r2, int* __restrict__ flags) {
+// flags[g] = point g (fp64 q) lies inside the gizmo's box (box), else inside the sphere of squared radius r2; NaN never does
+__global__ void __launch_bounds__(kPlaneThreads) k_plane_flags(int n, const double4* __restrict__ pts, int box, double r2, int* __restrict__ flags) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g < n) flags[g] = plane_d2(pts[g]) < r2 ? 1 : 0;
+  if (g >= n) return;
+  const double4 p = pts[g];
+  const double q[3] = {p.x, p.y, p.z};
+  flags[g] = (box ? ed_in_box(q) : ed_in_sphere(q, r2)) ? 1 : 0;
 }
 
-// one thread per point g: a flagged point goes to slot pos[g] - 1 with its q, its id and (loc given) its stored local point
+// one thread per point g: a flagged point goes to slot pos[g] - 1 with its id and (cand / loc given) its q and its stored
+// local point
 __global__ void __launch_bounds__(kPlaneThreads) k_plane_emit(int n, int K, const gb_frame* __restrict__ frames, const int* __restrict__ flags,
                                                               const int* __restrict__ pos, const double4* __restrict__ pts, double4* __restrict__ cand,
                                                               unsigned long long* __restrict__ ids, float4* __restrict__ loc) {
@@ -58,7 +64,7 @@ __global__ void __launch_bounds__(kPlaneThreads) k_plane_emit(int n, int K, cons
   if (g >= n || !flags[g]) return;
   const gb_frame& F = frames[gb_frame_of(frames, K, g)];
   const int i = g - F.offset, o = pos[g] - 1;
-  cand[o] = pts[g];
+  if (cand) cand[o] = pts[g];
   ids[o] = ((unsigned long long)F.index << 32) | (unsigned)i;
   if (loc) loc[o] = F.p0[F.inv_perm ? F.inv_perm[i] : i];
 }
@@ -76,8 +82,8 @@ __global__ void __launch_bounds__(kPlaneThreads) k_plane_reduce(const double4* _
   double v[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   for (int i = begin + threadIdx.x; i < end; i += blockDim.x) {
     const double4 q = cand[i];
-    if (!(plane_d2(q) < r2)) continue;
     const double p[3] = {q.x, q.y, q.z};
+    if (!ed_in_sphere(p, r2)) continue;
     v[0] += 1.0;
     for (int r = 0; r < 3; r++) v[1 + r] = __dadd_rn(v[1 + r], p[r]);
     for (int r = 0; r < 3; r++)
@@ -219,26 +225,19 @@ gb_status plane_args(const gb_ctx* ctx, size_t K, const gb_cloud* const* frames,
   return GB_OK;
 }
 
-// The candidates at radius r (selection rules 1-4): nothing launched when the participating frames hold no point.  Four
-// launches otherwise (the frame transform, the flags, their scan, the emit).  Everything the calls need later is carved here.
-gb_status plane_select(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, const gb_plane_patch_params* p, double r, bool local,
+// The posed selection shared by the plane patch and the gizmo: the points of P frames at poses (P x 16, column-major; index:
+// the caller's frame indices, nullptr for 0..P-1) whose fp64 q lies inside the box (box) or the sphere of squared radius r2,
+// their ids and, for the patch, their q (and with local their stored local points) and the patch's reduction buffers.
+// Nothing launched when the frames hold no point; four launches otherwise (the frame transform, the flags, their scan, the
+// emit).  Everything the calls need later is carved here.
+gb_status posed_select(gb_ctx* ctx, size_t P, const gb_cloud* const* frames, const double* poses, const int* index, bool box, double r2, bool patch, bool local,
                        PlaneSelection& s) {
-  std::vector<const gb_cloud*> pf;
-  std::vector<double> shifted;
-  for (size_t k = 0; k < K; k++) {
-    const double* T = poses + 16 * k;
-    const double u[3] = {T[12] - p->center[0], T[13] - p->center[1], T[14] - p->center[2]};
-    if (!(std::sqrt((u[0] * u[0] + u[1] * u[1]) + u[2] * u[2]) <= p->max_frame_distance)) continue;
-    s.part.push_back((int)k);
-    s.total += frames[k]->n;
-    pf.push_back(frames[k]);
-    shifted.insert(shifted.end(), T, T + 16);
-    for (int a = 0; a < 3; a++) shifted[shifted.size() - 4 + a] = u[a];
-  }
+  s.total = 0;
+  for (size_t k = 0; k < P; k++) s.total += frames[k]->n;
   if (s.total == 0) return GB_OK;
-  const size_t N = s.total, P = s.part.size(), cub_b = gb_cub_temp_bytes(N);
+  const size_t N = s.total, cub_b = gb_cub_temp_bytes(N);
   const int n = (int)N;
-  const std::vector<gb_frame> table = gb_frame_table(P, pf.data(), shifted.data(), s.part.data());
+  const std::vector<gb_frame> table = gb_frame_table(P, frames, poses, index);
   char* d_cub;
   int* d_flags;
   double4* d_pts;
@@ -248,8 +247,9 @@ gb_status plane_select(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, con
     d_flags = cv.take<int>(N);
     s.d_pos = cv.take<int>(N);
     d_pts = cv.take<double4>(N);
-    s.d_cand = cv.take<double4>(N);
     s.d_ids = cv.take<unsigned long long>(N);
+    if (!patch) return;
+    s.d_cand = cv.take<double4>(N);
     s.d_loc = local ? cv.take<float4>(N) : nullptr;
     s.d_partials = cv.take<double>(10 * kReduceBlocks);
     s.d_ticket = cv.take<unsigned>(1);
@@ -259,9 +259,26 @@ gb_status plane_select(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, con
   GB_CHECK(gb_upload(ctx, {{s.d_frames, table.data(), sizeof(gb_frame) * P}}));
   GB_CHECK(gb_transform_frames(ctx, P, s.d_frames, n, d_pts, nullptr));
   const int gb = (n + kPlaneThreads - 1) / kPlaneThreads;
-  GB_CHECK(gb_launch(ctx, "k_plane_flags", k_plane_flags, gb, kPlaneThreads, 0, n, d_pts, r * r, d_flags));
+  GB_CHECK(gb_launch(ctx, "k_plane_flags", k_plane_flags, gb, kPlaneThreads, 0, n, d_pts, box ? 1 : 0, r2, d_flags));
   GB_CUB(ctx, cub::DeviceScan::InclusiveSum, d_cub, cub_b, d_flags, s.d_pos, n);
   return gb_launch(ctx, "k_plane_emit", k_plane_emit, gb, kPlaneThreads, 0, n, (int)P, s.d_frames, d_flags, s.d_pos, d_pts, s.d_cand, s.d_ids, s.d_loc);
+}
+
+// The candidates at radius r (selection rules 1-4): the participating frames at their shifted poses, then posed_select.
+gb_status plane_select(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, const gb_plane_patch_params* p, double r, bool local,
+                       PlaneSelection& s) {
+  std::vector<const gb_cloud*> pf;
+  std::vector<double> shifted;
+  for (size_t k = 0; k < K; k++) {
+    const double* T = poses + 16 * k;
+    const double u[3] = {T[12] - p->center[0], T[13] - p->center[1], T[14] - p->center[2]};
+    if (!(std::sqrt((u[0] * u[0] + u[1] * u[1]) + u[2] * u[2]) <= p->max_frame_distance)) continue;
+    s.part.push_back((int)k);
+    pf.push_back(frames[k]);
+    shifted.insert(shifted.end(), T, T + 16);
+    for (int a = 0; a < 3; a++) shifted[shifted.size() - 4 + a] = u[a];
+  }
+  return posed_select(ctx, s.part.size(), pf.data(), shifted.data(), s.part.data(), false, r * r, true, local, s);
 }
 
 // n and the eigenvalues of the candidates inside radius r: one launch and one 32-byte copy with its synchronisation (none
@@ -460,4 +477,29 @@ extern "C" gb_status gb_plane_evm_error(gb_ctx* ctx, size_t F, gb_factor* const*
   GB_CHECK(plane_evm_args(ctx, F, factors, poses, errors, descs, keys, h_total));
   GB_ENTER(ctx);
   return plane_evm_run(ctx, F, factors, poses, descs, keys, h_total, nullptr, nullptr, errors, nullptr);
+}
+
+extern "C" gb_status gb_select_gizmo(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, const double* poses, const double T_local_world[16], int32_t shape,
+                                     uint64_t* ids, size_t* num_selected) {
+  GB_REQUIRE(ctx && T_local_world && num_selected, "null argument");
+  *num_selected = 0;
+  size_t total = 0;
+  GB_CHECK(gb_frame_list_check(ctx, K, frames, poses, &total));
+  GB_REQUIRE(gb_all_finite(poses, 16 * K), "a non-finite pose");
+  GB_REQUIRE(K < ((size_t)1 << 31), "too many frames");
+  GB_REQUIRE(gb_all_finite(T_local_world, 16), "a non-finite T_local_world");
+  const double* A = T_local_world;
+  GB_REQUIRE(A[3] == 0.0 && A[7] == 0.0 && A[11] == 0.0 && A[15] == 1.0, "T_local_world's bottom row must be (0, 0, 0, 1)");
+  GB_REQUIRE(shape == GB_GIZMO_BOX || shape == GB_GIZMO_SPHERE, "shape must be GB_GIZMO_BOX or GB_GIZMO_SPHERE");
+  GB_ENTER(ctx);
+  std::vector<double> M(16 * K);
+  for (size_t k = 0; k < K; k++) ed_compose(A, poses + 16 * k, M.data() + 16 * k);
+  PlaneSelection s;
+  GB_CHECK(posed_select(ctx, K, frames, M.data(), nullptr, shape == GB_GIZMO_BOX, 1.0, false, false, s));
+  if (s.total == 0) return GB_OK;
+  int count = 0;
+  GB_CHECK(gb_download(ctx, {{&count, s.d_pos + (s.total - 1), sizeof(int)}}));
+  if (ids && count > 0) GB_CHECK(gb_download(ctx, {{ids, s.d_ids, sizeof(uint64_t) * (size_t)count}}));
+  *num_selected = (size_t)count;
+  return GB_OK;
 }

@@ -492,6 +492,10 @@ __global__ void k_sor_compact(int n_upper, const int* __restrict__ keep, const i
 
 }  // namespace
 
+gb_status gb_sor_dists(gb_ctx* ctx, int n, const int* d_count, const double4* pts, const int* nb, int k, double* dist, double* dist2) {
+  return gb_launch(ctx, "k_sor_dists", k_sor_dists, (n + 255) / 256, 256, 0, n, d_count, pts, nb, k, dist, dist2);
+}
+
 gb_status gb_covariance_cloud(gb_ctx* ctx, int M, const int* d_count, const double4* pts, const int* neighbors, int kc, int k, double4* normals, double* covs,
                               const gb_planes& staged, const gb_sort_tmp& t, gb_cloud* cloud_out) {
   GB_CHECK(gb_launch(ctx, "k_covariances_planes", k_covariances_planes, (M + 127) / 128, 128, 0, M, d_count, pts, neighbors, kc, k, normals, covs, staged.p0, staged.p1, staged.p2,
@@ -617,7 +621,7 @@ static gb_status preprocess(gb_ctx* ctx, size_t n_, const double* xyzw, const do
   if (P->enable_outlier_removal) {
     const int ko = P->outlier_removal_k;
     GB_CHECK(knn_device(ctx, n, d_cnt + 2, d_fr, ko, h0, d_nbo, knn));
-    GB_CHECK(gb_launch(ctx, "k_sor_dists", k_sor_dists, gb, tb, 0, n, d_cnt + 2, d_fr, d_nbo, ko, d_dist, d_dist2));
+    GB_CHECK(gb_sor_dists(ctx, n, d_cnt + 2, d_fr, d_nbo, ko, d_dist, d_dist2));
     GB_CUB(ctx, cub::DeviceReduce::Sum, t.cub, cub_b, d_dist, d_sums, n);
     GB_CUB(ctx, cub::DeviceReduce::Sum, t.cub, cub_b, d_dist2, d_sums + 1, n);
     GB_CHECK(gb_launch(ctx, "k_sor_flags", k_sor_flags, gb, tb, 0, n, d_cnt + 2, d_dist, d_sums, P->outlier_std_mul_factor, d_keep));

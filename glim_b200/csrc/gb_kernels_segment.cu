@@ -1,6 +1,8 @@
 // gb_kernels_segment.cu -- the map editor's segmentation on the device (sm_90a): submaps concatenated into one world-frame
-// cloud (gb_concat_frames) and region growing from a picked point (gb_region_growing).  The rules are written once in
-// include/glim_b200.h; the per-point and per-pair arithmetic is gb_segment_math.cuh, which the host test build compiles as well.
+// cloud (gb_concat_frames), region growing and min-cut from a picked point (gb_region_growing, gb_min_cut), the radius tools
+// (gb_select_radius) and the removal of selected points (gb_remove_points).  The rules are written once in
+// include/glim_b200.h; the per-point and per-pair arithmetic is gb_segment_math.cuh, gb_mincut_math.cuh and
+// gb_editor_math.cuh, which the host test builds compile as well.
 //
 //   gb_concat_frames    k_merge_transform over every frame through one descriptor table (gb_transform_frames, shared with
 //                       gb_merge_frames), k_concat_flags (the window), a cub inclusive scan of the flags, k_concat_emit (the
@@ -18,9 +20,18 @@
 //                       arcs), k_mc_graph (heads, reverse arcs, capacities, rows and the exported edges), the cooperative
 //                       k_mc_solve (push-relabel, gb_mincut_math.cuh) and one cub compaction of the selection; one copy back
 //                       and one stream synchronisation.
+//   gb_select_radius    k_rs_flags (inside and participant flags by original index); INSIDE: one cub compaction.  OUTLIERS:
+//                       a cub scan of the participants, k_rs_nodes (fp64 positions in ascending original index), one copy
+//                       of the count and a stream synchronisation, knn_device on the nodes (6 launches), gb_sor_dists, two
+//                       cub sums, k_rs_outliers and one cub compaction; one copy back and one stream synchronisation.
+//   gb_remove_points    on the host, the valid ids and the touched frames; k_rm_mark, a cub scan of the marks in original
+//                       order, k_rm_stored (the marks in stored order and each frame's removed count), a cub scan of those,
+//                       one copy of the counts and a stream synchronisation; one pool block per new cloud, then k_rm_emit
+//                       over every touched frame and a stream synchronisation.
 #include "gb_internal.cuh"
 #include "gb_segment_math.cuh"
 #include "gb_mincut_math.cuh"
+#include "gb_editor_math.cuh"
 
 #include <cooperative_groups.h>
 #include <cub/cub.cuh>
@@ -423,6 +434,101 @@ __global__ void __launch_bounds__(kMcThreads, 4) k_mc_solve(McSolve g) {
   }
 }
 
+// ---- gb_select_radius ----
+// What gb_select_radius leaves for the host, ahead of the selection in one copy.
+struct RsOut {
+  double threshold;
+  int num_selected, pad;
+};
+
+// one thread per stored slot: inside[i] and part[i] of its original index i (ed_radius_flags)
+__global__ void __launch_bounds__(kSegThreads) k_rs_flags(int n, const float4* __restrict__ p0, const int* __restrict__ perm, double cx, double cy, double cz, double inner2,
+                                                          double outer2, int* __restrict__ inside, int* __restrict__ part) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int i = perm ? perm[j] : j;
+  const float4 p = p0[j];
+  const double c[3] = {cx, cy, cz};
+  const int f = ed_radius_flags(p.x, p.y, p.z, c, inner2, outer2);
+  inside[i] = f & 1;
+  part[i] = f >> 1;
+}
+
+// one thread per original index i: participant i becomes node pos[i] - 1 with its widened position, index and inside flag
+__global__ void __launch_bounds__(kSegThreads) k_rs_nodes(int n, const float4* __restrict__ p0, const int* __restrict__ inv_perm, const int* __restrict__ part,
+                                                          const int* __restrict__ pos, const int* __restrict__ inside, double4* __restrict__ pts, int* __restrict__ orig,
+                                                          int* __restrict__ in_node) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !part[i]) return;
+  const int u = pos[i] - 1;
+  const float4 p = p0[inv_perm ? inv_perm[i] : i];
+  pts[u] = make_double4(p.x, p.y, p.z, 1.0);
+  orig[u] = i;
+  in_node[u] = inside[i];
+}
+
+// one thread per node slot u: sel[u] = participant u is inside and not an inlier; the threshold from the sums of d and d^2
+__global__ void __launch_bounds__(kSegThreads) k_rs_outliers(int n, const int* __restrict__ count, const double* __restrict__ dist, const double* __restrict__ sums,
+                                                             double stddev_thresh, const int* __restrict__ in_node, int* __restrict__ sel, RsOut* __restrict__ out) {
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= n) return;
+  const int m = *count;
+  const double th = ed_outlier_threshold(sums[0], sums[1], m, stddev_thresh);
+  sel[u] = u < m && ed_outlier_selected(in_node[u] != 0, dist[u], th) ? 1 : 0;
+  if (u == 0) out->threshold = th;
+}
+
+// ---- gb_remove_points ----
+// Where the emit writes the new cloud of touched frame t (all null for a frame that loses every point).
+struct RmOut {
+  float4* p0;
+  float4* p1;
+  float* p2;
+  float4* normals;
+  int* perm;
+  int* inv_perm;
+};
+
+// one thread per valid id: removed[g] = 1 for its point g of the touched frames' concatenation (idempotent: duplicates are harmless)
+__global__ void k_rm_mark(int m, const int* __restrict__ gids, int* __restrict__ removed) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < m) removed[gids[e]] = 1;
+}
+
+// one thread per point g = offset + original index i of a touched frame: its removal mark at the frame's stored slot, and
+// the frame's removed count from the inclusive scan in original order (its last point)
+__global__ void k_rm_stored(int n, int T, const gb_frame* __restrict__ frames, const int* __restrict__ removed, const int* __restrict__ rpos,
+                            int* __restrict__ removed_s, int* __restrict__ counts) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n) return;
+  const int t = gb_frame_of(frames, T, g);
+  const gb_frame& F = frames[t];
+  const int i = g - F.offset;
+  removed_s[F.offset + (F.inv_perm ? F.inv_perm[i] : i)] = removed[g];
+  if (i == F.n - 1) counts[t] = rpos[g] - (F.offset > 0 ? rpos[F.offset - 1] : 0);
+}
+
+// one thread per point g = offset + original index i of a touched frame: a survivor at stored slot j goes to slot
+// j' = j - (removed before j in stored order) of the new cloud with index i' = i - (removed before i), its planes and normal
+// copied bit for bit; perm'[j'] = i' and inv_perm'[i'] = j'
+__global__ void k_rm_emit(int n, int T, const gb_frame* __restrict__ frames, const RmOut* __restrict__ outs, const int* __restrict__ removed,
+                          const int* __restrict__ rpos, const int* __restrict__ spos) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n || removed[g]) return;
+  const int t = gb_frame_of(frames, T, g);
+  const gb_frame& F = frames[t];
+  const RmOut& O = outs[t];
+  const int i = g - F.offset, j = F.inv_perm ? F.inv_perm[i] : i;
+  const int r0 = F.offset > 0 ? rpos[F.offset - 1] : 0, s0 = F.offset > 0 ? spos[F.offset - 1] : 0;
+  const int i2 = i - (rpos[g] - r0), j2 = j - (spos[F.offset + j] - s0);
+  O.p0[j2] = F.p0[j];
+  O.p1[j2] = F.p1[j];
+  O.p2[j2] = F.p2[j];
+  if (O.normals) O.normals[j2] = F.normals[j];
+  O.perm[j2] = i2;
+  O.inv_perm[i2] = j2;
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
@@ -728,5 +834,203 @@ extern "C" gb_status gb_min_cut(gb_ctx* ctx, const gb_cloud* cloud, const double
   if (selected) memcpy(selected, h_selected, sizeof(int32_t) * result->num_selected);
   if (edges) memcpy(edges, h_edges, sizeof(int32_t) * 2 * result->num_edges);
   if (capacities) memcpy(capacities, h_ecap, sizeof(int32_t) * result->num_edges);
+  return GB_OK;
+}
+
+extern "C" gb_status gb_select_radius_default_params(gb_select_radius_params* p) {
+  GB_REQUIRE(p, "null argument");
+  p->radius = 2.0;
+  p->radius_offset = 1.0;
+  p->stddev_thresh = 2.0;
+  p->mode = GB_RADIUS_INSIDE;
+  p->k = 10;
+  return GB_OK;
+}
+
+extern "C" gb_status gb_select_radius(gb_ctx* ctx, const gb_cloud* cloud, const double c[3], const gb_select_radius_params* prm, gb_select_radius_result* result,
+                                      int32_t* selected) {
+  GB_REQUIRE(ctx && cloud && c && prm && result, "null argument");
+  GB_REQUIRE(cloud->device == ctx->device, "the cloud lives on another device");
+  GB_REQUIRE(std::isfinite(c[0]) && std::isfinite(c[1]) && std::isfinite(c[2]), "a non-finite center");
+  GB_REQUIRE(std::isfinite(prm->radius) && prm->radius > 0.0, "radius must be positive and finite");
+  GB_REQUIRE(prm->mode == GB_RADIUS_INSIDE || prm->mode == GB_RADIUS_OUTLIERS, "mode must be GB_RADIUS_INSIDE or GB_RADIUS_OUTLIERS");
+  const bool outliers = prm->mode == GB_RADIUS_OUTLIERS;
+  if (outliers) {
+    GB_REQUIRE(std::isfinite(prm->radius_offset) && prm->radius_offset >= 0.0, "radius_offset must be finite and non-negative");
+    GB_REQUIRE(std::isfinite(prm->stddev_thresh), "stddev_thresh must be finite");
+    GB_REQUIRE(gb_knn_instantiated(prm->k), "k is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
+    GB_REQUIRE(cloud->n * (size_t)prm->k < ((size_t)1 << 30), "N * k must be below 2^30");
+  }
+  GB_ENTER(ctx);
+  memset(result, 0, sizeof(*result));
+  result->status = GB_RADIUS_OK;
+  result->threshold = NAN;
+  const size_t N = cloud->n;
+  if (N == 0) {
+    if (outliers) result->status = GB_RADIUS_NOT_ENOUGH_POINTS;
+    return GB_OK;
+  }
+  const int n = (int)N, k = outliers ? prm->k : 1;
+  const double r2 = prm->radius * prm->radius, ro = prm->radius + prm->radius_offset;
+  size_t cub_b = gb_cub_temp_bytes(N), b = 0;
+  cub::DeviceSelect::Flagged(nullptr, b, thrust::counting_iterator<int>(0), (const int*)nullptr, (int*)nullptr, (int*)nullptr, n);
+  cub_b = std::max(cub_b, b);
+  cub::DeviceSelect::Flagged(nullptr, b, (const int*)nullptr, (const int*)nullptr, (int*)nullptr, (int*)nullptr, n);
+  cub_b = std::max(cub_b, b);
+  void* d_cub;
+  KnnTmp knn;
+  int *d_inside, *d_part, *d_pos, *d_orig, *d_in, *d_nb, *d_sel, *d_selected;
+  double4* d_pts;
+  double *d_dist, *d_dist2, *d_sums;
+  RsOut* d_out;
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+    d_cub = cv.take<char>(cub_b);
+    d_inside = cv.take<int>(N);
+    d_part = cv.take<int>(N);
+    d_out = cv.take<RsOut>(1);
+    d_selected = cv.take<int>(N);
+    if (!outliers) return;
+    knn = take_knn_tmp(cv, n, d_cub, cub_b);
+    d_pos = cv.take<int>(N);
+    d_pts = cv.take<double4>(N);
+    d_orig = cv.take<int>(N);
+    d_in = cv.take<int>(N);
+    d_nb = cv.take<int>(N * (size_t)k);
+    d_dist = cv.take<double>(N);
+    d_dist2 = cv.take<double>(N);
+    d_sums = cv.take<double>(2);
+    d_sel = cv.take<int>(N);
+  }));
+  const int gb = (n + kSegThreads - 1) / kSegThreads;
+  GB_CHECK(gb_launch(ctx, "k_rs_flags", k_rs_flags, gb, kSegThreads, 0, n, cloud->p0, cloud->perm, c[0], c[1], c[2], r2, ro * ro, d_inside, d_part));
+  RsOut h{NAN, 0, 0};
+  if (!outliers) {
+    GB_CUB(ctx, cub::DeviceSelect::Flagged, d_cub, cub_b, thrust::counting_iterator<int>(0), d_inside, d_selected, &d_out->num_selected, n);
+  } else {
+    GB_CUB(ctx, cub::DeviceScan::InclusiveSum, d_cub, cub_b, d_part, d_pos, n);
+    GB_CHECK(gb_launch(ctx, "k_rs_nodes", k_rs_nodes, gb, kSegThreads, 0, n, cloud->p0, cloud->inv_perm, d_part, d_pos, d_inside, d_pts, d_orig, d_in));
+    int m = 0;
+    GB_CHECK(gb_download(ctx, {{&m, d_pos + (n - 1), sizeof(int)}}));
+    result->num_participants = (size_t)m;
+    if (m < k) {
+      result->status = GB_RADIUS_NOT_ENOUGH_POINTS;
+      return GB_OK;
+    }
+    const int* count = d_pos + (n - 1);
+    GB_CHECK(knn_device(ctx, n, count, d_pts, k, 0.25, d_nb, knn));
+    GB_CHECK(gb_sor_dists(ctx, n, count, d_pts, d_nb, k, d_dist, d_dist2));
+    GB_CUB(ctx, cub::DeviceReduce::Sum, d_cub, cub_b, d_dist, d_sums, n);
+    GB_CUB(ctx, cub::DeviceReduce::Sum, d_cub, cub_b, d_dist2, d_sums + 1, n);
+    GB_CHECK(gb_launch(ctx, "k_rs_outliers", k_rs_outliers, gb, kSegThreads, 0, n, count, d_dist, d_sums, prm->stddev_thresh, d_in, d_sel, d_out));
+    GB_CUB(ctx, cub::DeviceSelect::Flagged, d_cub, cub_b, d_orig, d_sel, d_selected, &d_out->num_selected, n);
+  }
+  GB_CHECK(gb_download(ctx, {{&h, d_out, sizeof(RsOut)}, {selected, d_selected, sizeof(int32_t) * N}}));
+  result->num_selected = (size_t)h.num_selected;
+  if (outliers) result->threshold = h.threshold;
+  return GB_OK;
+}
+
+extern "C" gb_status gb_remove_points(gb_ctx* ctx, size_t K, const gb_cloud* const* frames, size_t m, const uint64_t* ids, gb_cloud** out_clouds,
+                                      gb_remove_points_result* result, size_t* sizes) {
+  GB_REQUIRE(ctx && result, "null argument");
+  GB_REQUIRE(K == 0 || (frames && out_clouds), "null frames / out_clouds");
+  GB_REQUIRE(m == 0 || ids, "null ids");
+  for (size_t k = 0; k < K; k++) {
+    GB_REQUIRE(frames[k] && frames[k]->device == ctx->device, "null frame / frame on another device");
+    GB_REQUIRE(frames[k]->n < ((size_t)1 << 32), "a frame of 2^32 points or more");
+  }
+  // the touched frames (ascending frame order) and their offsets in the touched concatenation; the valid ids as points of it
+  std::vector<int> slot(K, -1);
+  std::vector<const gb_cloud*> tf;
+  std::vector<int> tk;
+  size_t ignored = 0, total = 0;
+  for (size_t e = 0; e < m; e++) {
+    const uint64_t f = ids[e] >> 32, i = ids[e] & 0xffffffffull;
+    if (f >= K || i >= frames[f]->n) ignored++;
+    else slot[f] = 0;
+  }
+  for (size_t k = 0; k < K; k++) {
+    if (slot[k] < 0) continue;
+    slot[k] = (int)tf.size();
+    tf.push_back(frames[k]);
+    tk.push_back((int)k);
+    total += frames[k]->n;
+  }
+  GB_REQUIRE(total < ((size_t)1 << 30), "the touched frames hold 2^30 points or more");
+  GB_ENTER(ctx);
+  *result = gb_remove_points_result{0, ignored, 0};
+  for (size_t k = 0; k < K; k++) {
+    out_clouds[k] = nullptr;
+    if (sizes) sizes[k] = frames[k]->n;
+  }
+  const size_t T = tf.size();
+  if (T == 0) return GB_OK;
+  std::vector<gb_frame> table = gb_frame_table(T, tf.data(), std::vector<double>(16 * T, 0.0).data(), tk.data());  // the poses are unused
+  std::vector<int> gids;
+  gids.reserve(m - ignored);
+  for (size_t e = 0; e < m; e++) {
+    const uint64_t f = ids[e] >> 32, i = ids[e] & 0xffffffffull;
+    if (f < K && i < frames[f]->n) gids.push_back(table[slot[f]].offset + (int)i);
+  }
+  const size_t N = total, M = gids.size(), cub_b = gb_cub_temp_bytes(N);
+  const int n = (int)N;
+  void* d_cub;
+  gb_frame* d_table;
+  RmOut* d_outs;
+  int *d_gids, *d_rem, *d_rpos, *d_rem_s, *d_spos, *d_counts;
+  GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+    d_cub = cv.take<char>(cub_b);
+    d_table = cv.take<gb_frame>(T);
+    d_outs = cv.take<RmOut>(T);
+    d_gids = cv.take<int>(M);
+    d_rem = cv.take<int>(N);
+    d_rpos = cv.take<int>(N);
+    d_rem_s = cv.take<int>(N);
+    d_spos = cv.take<int>(N);
+    d_counts = cv.take<int>(T);
+  }));
+  GB_CHECK(gb_upload(ctx, {{d_table, table.data(), sizeof(gb_frame) * T}, {d_gids, gids.data(), sizeof(int) * M}}));
+  GB_CUDA(cudaMemsetAsync(d_rem, 0, sizeof(int) * N, ctx->stream));
+  const int gb = (n + kSegThreads - 1) / kSegThreads;
+  GB_CHECK(gb_launch(ctx, "k_rm_mark", k_rm_mark, (unsigned)((M + kSegThreads - 1) / kSegThreads), kSegThreads, 0, (int)M, d_gids, d_rem));
+  GB_CUB(ctx, cub::DeviceScan::InclusiveSum, d_cub, cub_b, d_rem, d_rpos, n);
+  GB_CHECK(gb_launch(ctx, "k_rm_stored", k_rm_stored, gb, kSegThreads, 0, n, (int)T, d_table, d_rem, d_rpos, d_rem_s, d_counts));
+  GB_CUB(ctx, cub::DeviceScan::InclusiveSum, d_cub, cub_b, d_rem_s, d_spos, n);
+  std::vector<int> counts(T);
+  GB_CHECK(gb_download(ctx, {{counts.data(), d_counts, sizeof(int) * T}}));
+  // one new cloud per touched frame (each lost at least one point), its block laid out as gb_cloud_build's
+  std::vector<gb_owned<gb_cloud>> made;
+  std::vector<RmOut> outs(T);
+  for (size_t t = 0; t < T; t++) {
+    const gb_cloud* src = tf[t];
+    made.emplace_back(new (std::nothrow) gb_cloud(), cloud_free);
+    gb_cloud* c = made.back().get();
+    if (!c) return GB_ERR_INTERNAL;
+    c->device = ctx->device;
+    c->covs = src->covs;
+    const size_t n2 = src->n - (size_t)counts[t];
+    outs[t] = RmOut{};
+    if (n2 == 0) continue;
+    gb_planes d;
+    gb_dev_block block(ctx->device);
+    GB_CHECK(gb_dev_carve(ctx, block, [&](Carver& cv) {
+      d = gb_cloud_planes(cv, n2, src->normals != nullptr);
+      c->perm = cv.take<int>(n2);
+      c->inv_perm = cv.take<int>(n2);
+    }));
+    block.hand_over(c->base);
+    c->n = n2;
+    c->p0 = d.p0; c->p1 = d.p1; c->p2 = d.p2; c->normals = d.normals;
+    outs[t] = RmOut{d.p0, d.p1, d.p2, d.normals, c->perm, c->inv_perm};
+  }
+  GB_CHECK(gb_upload(ctx, {{d_outs, outs.data(), sizeof(RmOut) * T}}));
+  GB_CHECK(gb_launch(ctx, "k_rm_emit", k_rm_emit, gb, kSegThreads, 0, n, (int)T, d_table, d_outs, d_rem, d_rpos, d_spos));
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));  // the new clouds are complete when the call returns (they may be used from another context)
+  for (size_t t = 0; t < T; t++) {
+    result->num_removed += (size_t)counts[t];
+    if (sizes) sizes[tk[t]] = made[t]->n;
+    out_clouds[tk[t]] = made[t].release();
+  }
+  result->num_changed = T;
   return GB_OK;
 }

@@ -30,6 +30,9 @@ include/glim_b200/gtsam_points_compat.hpp.
                                                             GlobalMapping::export_points, global_mapping.cpp:638-680
     region_growing(cloud, seed_point, **params)             gtsam_points::region_growing_init / _update, points_selector.cpp:798-810
     min_cut(cloud, picked_point, **params)                  gtsam_points::min_cut, points_selector.cpp:774-796
+    select_gizmo(poses, frames, T_local_world, shape)       the editor's gizmo tool over the map, points_selector.cpp:623-674
+    select_radius(cloud, center, mode, **params)            the editor's radius and radius-outlier tools, :677-759
+    remove_points(frames, ids)                              the editor's Remove selected points, :513-620
     plane_patch(frames, poses, center, **params)            the bundle adjustment modal's Update, bundle_adjustment_modal.cpp:137-184
     plane_auto_radius(frames, poses, center, **params)      its Auto Radius, bundle_adjustment_modal.cpp:186-227
     PlaneEVMFactorGPU(frames, poses, center, **params)      gtsam_points::PlaneEVMFactor of its Create Factor, :229-245
@@ -889,6 +892,62 @@ def min_cut(cloud: PointCloudGPU, picked_point, ctx: Context | None = None, grap
         out["edges"] = e[: r.num_edges].copy()
         out["capacities"] = w[: r.num_edges].copy()
     return out
+
+
+def select_gizmo(poses, frames, T_local_world, shape: str = "box", ctx: Context | None = None) -> np.ndarray:
+    """The map editor's gizmo tool (points_selector.cpp:623-674) on the device (gb_select_gizmo): the points of the submaps
+    (frames K PointCloudGPU, poses K x (4,4) T_world_submap) inside the gizmo's box or unit sphere in the frame of
+    T_local_world (4,4), the inverse of the gizmo's model matrix.  shape "box" or "sphere".  -> ids (M,) uint64 =
+    (frame << 32) | original index, frame-major and ascending."""
+    ctx = ctx or (frames[0].ctx if len(frames) else default_context())
+    shapes = {"box": capi.GIZMO_BOX, "sphere": capi.GIZMO_SPHERE}
+    if shape not in shapes:
+        raise capi.GlimB200Error(f"unknown gizmo shape {shape!r}")
+    K, arr, T = _frames(frames, poses)
+    A = pose16(np.asarray(T_local_world, dtype=np.float64))
+    ids = np.empty(sum(f.n for f in frames), np.uint64)
+    m = C.c_size_t()
+    check(lib().gb_select_gizmo(ctx.h, K, arr, ptr(T), ptr(A), shapes[shape], ptr(ids), C.byref(m)))
+    return ids[: m.value].copy()
+
+
+def select_radius_params(**overrides) -> capi.SelectRadiusParams:
+    """gb_select_radius_default_params (the editor's 2.0 m, 1.0 m, 2.0, INSIDE, k = 10) with the given fields replaced."""
+    return _params(capi.SelectRadiusParams(), lib().gb_select_radius_default_params, "gb_select_radius_params", overrides)
+
+
+def select_radius(cloud: PointCloudGPU, center, mode: str = "inside", ctx: Context | None = None, **params) -> dict:
+    """The map editor's radius tools (points_selector.cpp:677-759) on the device (gb_select_radius): mode "inside" selects the
+    points within radius of center, "outliers" the radius outliers among them.  params are fields of gb_select_radius_params
+    (radius, radius_offset, stddev_thresh, k).  -> {status, status_name, num_participants, num_selected, threshold, selected
+    (num_selected,) int32 in ascending original index}"""
+    ctx = ctx or cloud.ctx
+    modes = {"inside": capi.RADIUS_INSIDE, "outliers": capi.RADIUS_OUTLIERS}
+    if mode not in modes:
+        raise capi.GlimB200Error(f"unknown radius mode {mode!r}")
+    p = select_radius_params(mode=modes[mode], **params)
+    r = capi.SelectRadiusResult()
+    q = f64(np.asarray(center, dtype=np.float64).reshape(-1)[:3])
+    sel = np.empty(cloud.n, np.int32)
+    check(lib().gb_select_radius(ctx.h, cloud.h, ptr(q), C.byref(p), C.byref(r), ptr(sel)))
+    return {"status": r.status, "status_name": capi.RADIUS_STATUS_NAMES.get(r.status, "?"), "num_participants": r.num_participants,
+            "num_selected": r.num_selected, "threshold": r.threshold, "selected": sel[: r.num_selected].copy()}
+
+
+def remove_points(frames, ids, ctx: Context | None = None) -> dict:
+    """The map editor's Remove selected points (points_selector.cpp:513-620) on the device (gb_remove_points): ids are editor
+    ids (frame << 32) | original index into the list `frames`, in any order.  -> {frames: the list after the removal (an
+    unchanged frame is the same PointCloudGPU, a changed one a new object), num_removed, num_ignored, num_changed}"""
+    ctx = ctx or (frames[0].ctx if len(frames) else default_context())
+    K = len(frames)
+    arr = (C.c_void_p * max(K, 1))(*[f.h for f in frames])
+    out = (C.c_void_p * max(K, 1))()
+    sizes = np.empty(max(K, 1), np.uint64)
+    idv = np.ascontiguousarray(np.asarray(ids, dtype=np.uint64).reshape(-1))
+    r = capi.RemovePointsResult()
+    check(lib().gb_remove_points(ctx.h, K, C.cast(arr, C.c_void_p), idv.shape[0], ptr(idv), C.cast(out, C.c_void_p), C.byref(r), ptr(sizes)))
+    new = [PointCloudGPU(ctx, C.c_void_p(out[k]), int(sizes[k])) if out[k] else frames[k] for k in range(K)]
+    return {"frames": new, "num_removed": r.num_removed, "num_ignored": r.num_ignored, "num_changed": r.num_changed}
 
 
 def plane_patch_params(center=(0.0, 0.0, 0.0), **overrides) -> capi.PlanePatchParams:

@@ -845,6 +845,116 @@ GB_API gb_status gb_min_cut_default_params(gb_min_cut_params* params);
 GB_API gb_status gb_min_cut(gb_ctx* ctx, const gb_cloud* cloud, const double picked_point[3], const gb_min_cut_params* params,
                             gb_min_cut_result* result, int32_t* selected, int32_t* edges, int32_t* capacities);
 
+/* ---- The map editor's gizmo tool over the whole map (PointsSelector::select_points_tool, points_selector.cpp:623-674): the
+ *      points of K device clouds (submaps in their local frames, poses T_world_submap K x 16 column-major) inside the gizmo's
+ *      box or sphere.
+ *
+ *      The rule.  T_local_world (16 doubles, column-major) is the inverse of the gizmo's model matrix, which the caller
+ *      computes (:630).  Per frame, on the host in fp64: M_k = T_local_world T_world_submap_k, entry (r, c) for c < 3 as
+ *      (A_r0 B_0c + A_r1 B_1c) + A_r2 B_2c and the translation as ((A_r0 B_03 + A_r1 B_13) + A_r2 B_23) + A_r3, each
+ *      operation rounded (A = T_local_world, B = the pose, whose bottom row is taken as (0, 0, 0, 1) as in every posed frame
+ *      list).  A stored fp32 point a, widened to fp64, becomes q = M_k a by gb_merge_frames' transform (row r as
+ *      ((M_r0 a_x + M_r1 a_y) + M_r2 a_z) + M_r3, un-contracted).  GB_GIZMO_BOX selects it iff -0.5 < q_r < 0.5 on every axis
+ *      (strict); GB_GIZMO_SPHERE iff (q_x^2 + q_y^2) + q_z^2 < 1, each operation rounded.  A NaN is never selected.  For an
+ *      affine model matrix the editor's 0 < w < 2 test always holds.  The editor transforms its fp64 host points, this
+ *      library the stored fp32 ones: a point within about 1e-7 relative of a face may fall on the other side.
+ *      ids: (k << 32) | original index, frame-major and ascending (gb_concat_frames' editor ids), capacity the sum of the
+ *      frames' sizes, or NULL; num_selected the count.
+ *
+ *      GB_ERR_INVALID_ARGUMENT before any launch for null arguments, a frame on another device than ctx, a non-finite pose,
+ *      a non-finite T_local_world entry, a T_local_world whose bottom row is not exactly (0, 0, 0, 1), an unknown shape, a
+ *      frame of 2^32 points or more, or 2^30 points or more in all.  Launches: 4 (the shared frame transform, the inside
+ *      flags, their scan, the emit: gb_plane_patch's selection); none when the frames hold no point.  One stream
+ *      synchronisation (the count), and a second one when ids are asked for and some point is selected. ---- */
+#define GB_GIZMO_BOX 0
+#define GB_GIZMO_SPHERE 1
+GB_API gb_status gb_select_gizmo(gb_ctx* ctx, size_t num_frames, const gb_cloud* const* frames, const double* poses, const double T_local_world[16],
+                                 int32_t shape, uint64_t* ids, size_t* num_selected);
+
+/* ---- The map editor's two radius tools (PointsSelector::select_points_radius and select_outlier_points_radius,
+ *      points_selector.cpp:677-759) on a device cloud, typically the window gb_concat_frames returns, as gb_min_cut takes it;
+ *      callers map the selection to editor ids with ids[selected].
+ *
+ *      The rule.  c = center; d2 = (dx^2 + dy^2) + dz^2 in fp64 of the stored fp32 position widened to fp64 and c, each
+ *      operation rounded (gb_min_cut's d2).  The editor measures its fp64 host points: a point within about 1e-7 relative of
+ *      a radius may fall on the other side.
+ *      INSIDE: the finite points with d2 < radius^2, in ascending original index.
+ *      OUTLIERS ([EXT] gtsam_points::find_inlier_points is not vendored: this is the editor's call as this library states it):
+ *      1. Participants: the finite points with d2 < (radius + radius_offset)^2, in ascending original index.
+ *      2. Fewer than k participants: status NOT_ENOUGH_POINTS, nothing selected (the editor returns, :730-733).
+ *      3. Each participant's k nearest participants by gb_find_neighbors' rule (fp64 d2, ties to the smaller index, the query
+ *         included; a participant whose 0.25 m cell leaves the 21-bit range has itself k times in its row and is in no row).
+ *      4. d_i = (sum of the k fp64 distances sqrt(d2) in row order, nearest first) / k: gb_preprocess's outlier-removal rule.
+ *      5. threshold = mean + stddev_thresh * sqrt(max(var, 0)) with mean = S / m, var = S2 / m - mean^2 (population), each
+ *         operation rounded, over the m participants' sums S = sum d_i and S2 = sum d_i^2.  The sums are cub's DeviceReduce
+ *         over the cloud's N slots (0 beyond the participants), whose order depends on N and the device only: the same inputs
+ *         give the same bits.  An inlier has d_i < threshold.
+ *      6. Selected: the participants with d2 < radius^2 that are not inliers (:746-752), in ascending original index.
+ *      k must be an instantiated k-NN count (1-10, 12, 15, 16, 20, 24, 32); the editor's UI allows up to 100.
+ *
+ *      GB_ERR_INVALID_ARGUMENT before any launch for null arguments, a cloud on another device than ctx, a non-finite center,
+ *      parameters outside the bounds below, or, for OUTLIERS, N * k >= 2^30.  An empty cloud makes no launch.  Launches:
+ *      INSIDE 2 (the flags, the compaction) and one stream synchronisation; OUTLIERS 3 (the flags, their scan, the nodes),
+ *      one stream synchronisation (the participant count), then, with at least k participants, 6 (the k-NN) + 1 (the mean
+ *      distances) + 2 (the sums) + 1 (the outlier flags) + 1 (the compaction) and a second synchronisation.  selected:
+ *      capacity N, or NULL; its first num_selected entries are the selection, the others are unspecified. ---- */
+#define GB_RADIUS_INSIDE 0
+#define GB_RADIUS_OUTLIERS 1
+#define GB_RADIUS_OK 0
+#define GB_RADIUS_NOT_ENOUGH_POINTS 1
+typedef struct gb_select_radius_params {
+  double radius;          /* m, finite, > 0: 2.0 (points_selector.cpp:34) */
+  double radius_offset;   /* m, finite, >= 0: 1.0 (:35), OUTLIERS only */
+  double stddev_thresh;   /* finite: 2.0 (:37), OUTLIERS only */
+  int32_t mode;           /* GB_RADIUS_INSIDE (default) or GB_RADIUS_OUTLIERS */
+  int32_t k;              /* an instantiated k-NN count: 10 (:36), OUTLIERS only */
+} gb_select_radius_params;
+typedef struct gb_select_radius_result {
+  int32_t status;           /* GB_RADIUS_* */
+  size_t num_participants;  /* OUTLIERS: the participants; INSIDE: 0 */
+  size_t num_selected;
+  double threshold;         /* OUTLIERS with enough participants: the inlier threshold; NaN otherwise */
+} gb_select_radius_result;
+/* 2.0 m, 1.0 m, 2.0, INSIDE, 10 */
+GB_API gb_status gb_select_radius_default_params(gb_select_radius_params* params);
+GB_API gb_status gb_select_radius(gb_ctx* ctx, const gb_cloud* cloud, const double center[3], const gb_select_radius_params* params,
+                                  gb_select_radius_result* result, int32_t* selected);
+
+/* ---- Remove selected points (PointsSelector::remove_selected_points, points_selector.cpp:513-620) from K device clouds:
+ *      ids are editor ids (frame << 32) | original index, the frame being the position in this list (gb_concat_frames'
+ *      ids), in any order, duplicates allowed.
+ *
+ *      The rule.  An id whose frame is >= K or whose index is >= that frame's size is ignored and counted (the editor warns
+ *      and skips it; its check at :549 misses index == size, this one does not).  Every frame that loses at least one point
+ *      gets a NEW cloud in out_clouds[k]: its survivors in their original relative order, renumbered 0..n'-1
+ *      (gtsam_points::sample with ascending indices, :544-561); a frame that loses nothing gets NULL and the caller keeps its
+ *      handle.  The input clouds are never modified: factors, voxel maps and grids built from them stay valid.  A new cloud
+ *      carries the stored fp32 positions, covariances iff the frame has them, and normals iff the frame has them (uploaded or
+ *      from gb_cloud_estimate_normals; the new cloud keeps them in its own block), each value copied bit for bit.  It does
+ *      NOT carry the frame's time table or FPFH features, which depend on the removed points: recompute them with
+ *      gb_cloud_add_times and gb_cloud_estimate_fpfh.  A frame that loses every point becomes an empty cloud.
+ *      A cloud's storage order is a stable sort on the Morton key of each stored fp32 position with the original index as
+ *      the tie-break, so the survivors, taken in stored order, are already in the order gb_cloud_upload of the survivors
+ *      would store them: the removal is a compaction in stored order with no re-sort, and a new cloud is bit-identical, planes,
+ *      perm and inv_perm, to an upload of its survivors' downloaded values.
+ *      result: num_removed = distinct points removed, num_ignored, num_changed = frames given a new cloud.  sizes (K, or NULL):
+ *      every frame's size after the removal.
+ *
+ *      GB_ERR_INVALID_ARGUMENT before any launch for null arguments, a frame on another device than ctx, a frame of 2^32
+ *      points or more, or touched frames of 2^30 points or more in all.  No launch when no id is valid.  Otherwise the work
+ *      and scratch scale with the touched frames, not the map, and the launches are 5 whatever K and num_ids: the marks of
+ *      the removed points, their scan in original order, the marks in stored order (through inv_perm) with each frame's
+ *      removed count, their scan, and one emit over every touched frame into the new clouds' blocks (one pool block per
+ *      non-empty new cloud, laid out as gb_cloud_upload's).  Two uploads (the ids and the touched frames' table, then the new
+ *      clouds' table), one stream synchronisation for the removed counts and one at the end: the new clouds are complete
+ *      when the call returns. ---- */
+typedef struct gb_remove_points_result {
+  size_t num_removed, num_ignored, num_changed;
+} gb_remove_points_result;
+/* out_clouds: K entries, each a new cloud or NULL */
+GB_API gb_status gb_remove_points(gb_ctx* ctx, size_t num_frames, const gb_cloud* const* frames, size_t num_ids, const uint64_t* ids, gb_cloud** out_clouds,
+                                  gb_remove_points_result* result, size_t* sizes);
+
 /* ---- The interactive viewer's plane bundle adjustment (src/glim/viewer/interactive/bundle_adjustment_modal.cpp:37-60,
  *      :137-245; interactive_viewer.cpp:393, :412-418): the submap points around a right-clicked point, their covariance's
  *      eigenvalues (Update), the modal's radius search (Auto Radius), and the gtsam_points::PlaneEVMFactor made of them
