@@ -78,6 +78,7 @@ _SIGNATURES = {
     "gb_ivox_info": ([vp, vp, vp, vp], st),
     "gb_ivox_download": ([vp, vp, vp, vp, vp], st),
     "gb_ivox_destroy": ([vp], st),
+    "gb_ivox_extract": ([vp, vp, vp, i32, u64, vp], st),
     "gb_gicp_factor_create": ([vp, vp, vp, f64, vp], st),
     "gb_cloud_add_times": ([vp, vp, sz, vp], st),
     "gb_cloud_time_table": ([vp, vp, vp, vp, vp, vp], st),

@@ -730,21 +730,9 @@ __global__ void k_merge_transform(int num_frames, const gb_frame* __restrict__ f
   const float4 a0 = F.p0[slot];
   const float4 a1 = F.p1[slot];
   const float a2 = F.p2[slot];
-  const double* T = F.T;  // rows of the 3x4 pose
-  // un-contracted fp64 with a fixed association order: bit-exact with the oracle (go_merge_frames, built with fp-contract=off)
-  const double x = a0.x, y = a0.y, z = a0.z;
   double q[3];
-  for (int r = 0; r < 3; r++) q[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[r * 4 + 0], x), __dmul_rn(T[r * 4 + 1], y)), __dmul_rn(T[r * 4 + 2], z)), T[r * 4 + 3]);
+  gb_pose_record(F.T, a0, a1, a2, q, cov6 ? cov6 + 6 * (size_t)g : nullptr);
   pts[g] = make_double4(q[0], q[1], q[2], 1.0);
-  if (!cov6) return;
-  const double C[9] = {a0.w, a1.x, a1.y, a1.x, a1.z, a1.w, a1.y, a1.w, a2};
-  double RC[9];
-  for (int r = 0; r < 3; r++)
-    for (int c = 0; c < 3; c++) RC[r * 3 + c] = __dadd_rn(__dadd_rn(__dmul_rn(T[r * 4 + 0], C[0 * 3 + c]), __dmul_rn(T[r * 4 + 1], C[1 * 3 + c])), __dmul_rn(T[r * 4 + 2], C[2 * 3 + c]));
-  double* o = cov6 + 6 * (size_t)g;
-  int e = 0;
-  for (int r = 0; r < 3; r++)
-    for (int c = r; c < 3; c++) o[e++] = __dadd_rn(__dadd_rn(__dmul_rn(RC[r * 3 + 0], T[c * 4 + 0]), __dmul_rn(RC[r * 3 + 1], T[c * 4 + 1])), __dmul_rn(RC[r * 3 + 2], T[c * 4 + 2]));
 }
 __global__ void k_merge_emit(int n_upper, const int* __restrict__ keep, const int* __restrict__ pos, const double4* __restrict__ pts, const double* __restrict__ cov6, double4* __restrict__ o_pts, double* __restrict__ o_cov16,
                              float4* __restrict__ s0, float4* __restrict__ s1, float* __restrict__ s2) {

@@ -779,6 +779,81 @@ extern "C" gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords,
 extern "C" gb_status gb_ivox_destroy(gb_ivox* map) { return gb_voxelmap_destroy(ivox_map(map)); }
 
 // ---------------------------------------------------------------------------------------------
+// gb_ivox_extract (the rule is written once in include/glim_b200.h): every stored point of an iVox, in map order, posed by
+// T_out_map and optionally thinned, as a new cloud.  P and m are known on the host, so nothing is read back:
+//   thinning       gb_thin over the P map indices (k_thin_hash, cub SortKeys, k_thin_keep), then a cub inclusive scan of the
+//                  keep flags: the output slot of each kept point
+//   k_ivox_extract one thread per stored point: gb_pose_record (k_merge_transform's arithmetic) on the record, cast once to
+//                  fp32 into the planes staged in output order, as gb_cloud_upload stages the caller's points
+//   gb_cloud_build the Morton reorder of every cloud
+// 4 launches, 8 when thinning; one stream synchronisation at the end.  The map is only read.
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+struct PoseRows { double T[12]; };  // the rows of a 3x4 pose, as gb_frame::T
+
+__global__ void k_ivox_extract(int P, const float4* __restrict__ records, PoseRows pose, const int* __restrict__ keep, const int* __restrict__ pos, float4* __restrict__ s0,
+                               float4* __restrict__ s1, float* __restrict__ s2) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P || (keep && !keep[i])) return;
+  const int o = pos ? pos[i] - 1 : i;
+  const float4* r = records + 3 * (size_t)i;
+  double q[3], c[6];
+  gb_pose_record(pose.T, r[0], r[1], r[2].x, q, c);
+  s0[o] = make_float4((float)q[0], (float)q[1], (float)q[2], (float)c[0]);
+  s1[o] = make_float4((float)c[1], (float)c[2], (float)c[3], (float)c[4]);
+  s2[o] = (float)c[5];
+}
+
+}  // namespace
+
+extern "C" gb_status gb_ivox_extract(gb_ctx* ctx, const gb_ivox* map, const double* T_out_map, int target_num_points, uint64_t seed, gb_cloud** out) {
+  const gb_voxelmap* m = ivox_map(map);
+  GB_REQUIRE(ctx && m && out, "null argument");
+  *out = nullptr;
+  GB_REQUIRE(m->kind == GB_MAP_IVOX, "the map is not an iVox");
+  GB_REQUIRE(m->device == ctx->device, "the map lives on another device");
+  static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  const double* T = T_out_map ? T_out_map : kIdentity;
+  GB_REQUIRE(gb_all_finite(T, 16), "T_out_map must be finite");
+  const size_t P = m->num_points;
+  GB_REQUIRE(P < ((size_t)1 << 30), "a map of 2^30 points or more");
+  const bool thin = target_num_points > 0 && P > (size_t)target_num_points;
+  const size_t M = thin ? (size_t)((double)P * ((double)target_num_points / (double)P)) : P;  // random_sampling's count
+  GB_ENTER(ctx);
+  gb_owned<gb_cloud> c(new (std::nothrow) gb_cloud(), cloud_free);
+  if (!c) return GB_ERR_INTERNAL;
+  c->device = ctx->device;
+  c->covs = true;
+  if (M > 0) {
+    PoseRows pose;
+    for (int r = 0; r < 3; r++) for (int k = 0; k < 4; k++) pose.T[r * 4 + k] = T[k * 4 + r];
+    const int n = (int)P;
+    const size_t cub_b = gb_cub_temp_bytes(P);
+    gb_planes staged;
+    gb_sort_tmp t;
+    int *keep = nullptr, *pos = nullptr;
+    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+      staged = gb_cloud_planes(cv, M, false);
+      t = gb_take_sort_tmp(cv, P, cv.take<char>(cub_b), cub_b);
+      if (thin) {
+        keep = cv.take<int>(P);
+        pos = cv.take<int>(P);
+      }
+    }));
+    if (thin) {
+      GB_CHECK(gb_thin(ctx, n, nullptr, nullptr, (int)M, (unsigned long long)seed, t, keep));
+      GB_CUB(ctx, cub::DeviceScan::InclusiveSum, t.cub, t.cub_bytes, keep, pos, n);
+    }
+    GB_CHECK(gb_launch(ctx, "k_ivox_extract", k_ivox_extract, (n + 255) / 256, 256, 0, n, m->voxels, pose, keep, pos, staged.p0, staged.p1, staged.p2));
+    GB_CHECK(gb_cloud_build(ctx, c.get(), M, staged, t));
+  }
+  GB_CUDA(cudaStreamSynchronize(ctx->stream));
+  *out = c.release();
+  return GB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Point grid (gb_point_grid_build; the rule is written once in include/glim_b200.h): every point of a cloud, grouped by its
 // fp32 lookup key.  group_cloud (the build's fp32 key per original index, grouped) and gb_group_starts (stable: a cell's
 // points in original index order, the points without a key last), k_grid_emit (records, cells, keys, table coordinates and the

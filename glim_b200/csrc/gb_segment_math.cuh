@@ -57,6 +57,23 @@ GB_HD unsigned long long seg_seed_key(float4 p, float qx, float qy, float qz, in
   return ((unsigned long long)(uint32_t)__float_as_int(point_d2(p, qx, qy, qz)) << 32) | (uint32_t)i;
 }
 
+// The posed point of every frame transform (k_merge_transform, k_ivox_extract): from a stored fp32 record {x y z c00}
+// {c01 c02 c11 c12} c22 and the rows T of a 3x4 pose [R | t], q = R a + t with row r as ((R_r0 x + R_r1 y) + R_r2 z) + t_r, and,
+// when cov6 is given, the upper triangle of R C R^T as (R C)_r . R_c with the same association order, all in un-contracted
+// fp64: bit-exact with the oracle (go_merge_frames, built with fp-contract=off).
+GB_HD void gb_pose_record(const double* T, float4 a0, float4 a1, float a2, double* q, double* cov6) {
+  const double x = a0.x, y = a0.y, z = a0.z;
+  for (int r = 0; r < 3; r++) q[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[r * 4 + 0], x), __dmul_rn(T[r * 4 + 1], y)), __dmul_rn(T[r * 4 + 2], z)), T[r * 4 + 3]);
+  if (!cov6) return;
+  const double C[9] = {a0.w, a1.x, a1.y, a1.x, a1.z, a1.w, a1.y, a1.w, a2};
+  double RC[9];
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) RC[r * 3 + c] = __dadd_rn(__dadd_rn(__dmul_rn(T[r * 4 + 0], C[0 * 3 + c]), __dmul_rn(T[r * 4 + 1], C[1 * 3 + c])), __dmul_rn(T[r * 4 + 2], C[2 * 3 + c]));
+  int e = 0;
+  for (int r = 0; r < 3; r++)
+    for (int c = r; c < 3; c++) cov6[e++] = __dadd_rn(__dadd_rn(__dmul_rn(RC[r * 3 + 0], T[c * 4 + 0]), __dmul_rn(RC[r * 3 + 1], T[c * 4 + 1])), __dmul_rn(RC[r * 3 + 2], T[c * 4 + 2]));
+}
+
 // A point's normal rotated into the world frame: n' = R n, row r as (R_r0 nx + R_r1 ny) + R_r2 nz in un-contracted fp64 (T:
 // the rows of the 3x4 pose [R | t], gb_frame::T), stored fp32, not renormalised.
 GB_HD void seg_rotate_normal(const double* T, float nx, float ny, float nz, float* out) {

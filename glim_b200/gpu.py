@@ -10,6 +10,7 @@ include/glim_b200/gtsam_points_compat.hpp.
     NonlinearFactorSetGPU.add(...) / .linearize(values)     odometry_estimation_gpu.cpp:383-386
     overlap_gpu(voxelmap(s), source, delta(s))              odometry_estimation_gpu.cpp:231, :248
     IVoxGPU(resolution, min_dist, ...).insert(cloud, T, rate)   gtsam_points::iVox, odometry_estimation_cpu.cpp:57-61, :177-191
+    IVoxGPU.voxel_data(T_out_map, target_num_points, seed)   voxel_data + transform + random_sampling, sub_mapping_passthrough.cpp:146-153
     IntegratedGICPFactorGPU(target, source_key, ivox, source, max_corr)   odometry_estimation_cpu.cpp:95-104
     PointGridGPU(cloud, cell_size)                          the target frame's KdTree (global_mapping_pose_graph.cpp:273)
     IntegratedGICPFactorGPU(target, source_key, grid, source, max_corr)   IntegratedGICPFactor between frames: sub_mapping.cpp:189-211,
@@ -374,6 +375,24 @@ class IVoxGPU(_Handle):
         xyz, cov6 = np.empty((P, 3), np.float32), np.empty((P, 6), np.float32)
         check(lib().gb_ivox_download(self.h, ptr(coords), ptr(counts), ptr(xyz), ptr(cov6)))
         return coords, counts, xyz, cov6
+
+    def voxel_data(self, T_out_map=None, target_num_points: int = 0, seed: int = 0) -> PointCloudGPU:
+        """voxel_data() + transform(., T_out_map) + random_sampling to target_num_points (sub_mapping_passthrough.cpp:146-153)
+        on the device (gb_ivox_extract): every stored point in map order, posed by T_out_map (4x4, None = identity), thinned
+        by the hash pick when target_num_points > 0 and the map holds more, as a new PointCloudGPU with covariances.
+        target_num_points may be any integer: the C call takes an int, and a target above INT_MAX keeps every point as INT_MAX
+        does (a map holds fewer than 2^30), so it is clamped rather than wrapped; seed must be in [0, 2^64)."""
+        target = int(target_num_points)
+        target = min(target, 2**31 - 1) if target > 0 else 0
+        seed = int(seed)
+        if not 0 <= seed < 2**64:
+            raise ValueError(f"seed {seed} is outside [0, 2^64)")
+        Tc = pose16(np.asarray(T_out_map, dtype=np.float64).reshape(4, 4)) if T_out_map is not None else None
+        cloud = PointCloudGPU(self.ctx, self._create(lib().gb_ivox_extract, self.ctx.h, self.h, ptr(Tc), target, seed), 0)
+        n = C.c_size_t()
+        check(lib().gb_cloud_size(cloud.h, C.byref(n)))
+        cloud.n = n.value
+        return cloud
 
 
 class PointGridGPU(_Handle):

@@ -196,6 +196,31 @@ GB_API gb_status gb_ivox_info(const gb_ivox* map, int* num_voxels, size_t* num_p
 GB_API gb_status gb_ivox_download(const gb_ivox* map, int32_t* voxel_coords /* V x 3 */, int32_t* voxel_counts /* V */,
                                   float* xyz /* P x 3 */, float* cov6 /* P x 6 */);
 GB_API gb_status gb_ivox_destroy(gb_ivox* map);
+/* ---- The submap of GLIM's passthrough sub-mapping (SubMappingPassthrough::create_submap, src/glim/mapping/
+ *      sub_mapping_passthrough.cpp:146-153): voxel_data() of the module's IncrementalVoxelMap<FlatContainer> (this iVox),
+ *      transform(merged, T_world_origin^-1) and random_sampling down to submap_target_num_points, as one device call.
+ *
+ *      The rule.
+ *        1. Points: the P = num_points stored points in map order (gb_ivox_download's: voxels by ascending packed key, each
+ *           voxel's slots in order); a point's index i is its position in that order.
+ *        2. Transform: from the stored fp32 record, q = R a + t and C' = R C R^T in the un-contracted fp64 of gb_merge_frames'
+ *           transform (the same association order, the same per-point code); each value is stored once as fp32.
+ *        3. Thinning iff target_num_points > 0 and P > target_num_points: m = (size_t)((double)P * ((double)target_num_points /
+ *           (double)P)) points stay (the count of random_sampling at the module's rate, :151: not always the target, e.g. P =
+ *           65692 with target 50000 keeps 49999), those with the smallest rg_hash(seed, i) (gb_thin's rule), in map order.
+ *           [EXT] the reference draws with std::mt19937 over voxel_data()'s insertion order: only which points stay differs.
+ *        4. Output: a new cloud with positions and covariances, and no normals, time table or FPFH features (the iVox keeps
+ *           none).  It is stored as every cloud (gb_cloud_build's Morton order) and is bit-identical, planes, perm and inv_perm,
+ *           to gb_cloud_upload of the rule's fp64 q and C' in output order.  An empty map, or m = 0, gives a valid empty cloud.
+ *      target_num_points is an int, as in gb_merge_frames and as GLIM's submap_target_num_points is (the module passes it
+ *      unchanged); callers holding a wider count clamp it to INT_MAX, which keeps the same points of any map this call accepts.
+ *      The call never writes the map.  Launches: 4 (k_ivox_extract, gb_cloud_build's 3), 8 when thinning (gb_thin's 3 and the
+ *      scan of its flags ahead of them), whatever P and the voxel count.  The one exception is an empty result (an empty map,
+ *      or m = 0): no launch at all.  No transfer: P and m are known on the host.  One stream synchronisation, before it returns.
+ *      GB_ERR_INVALID_ARGUMENT before any launch for a null ctx, map or out, a handle that is not an iVox (a voxel map or a
+ *      point grid), a map on another device than ctx, a non-finite T_out_map or a map of 2^30 points or more. ---- */
+GB_API gb_status gb_ivox_extract(gb_ctx* ctx, const gb_ivox* map, const double* T_out_map /* 16 col-major, NULL = I */,
+                                 int target_num_points /* <= 0: keep all */, uint64_t seed, gb_cloud** out);
 
 /* ---- IntegratedVGICPFactorGPU(target_key | fixed_target_pose, source_key, voxelmap, source, stream, buffer)
  *      (odometry_estimation_gpu.cpp:144,161; sub_mapping.cpp:307; global_mapping.cpp:335,466,860).
