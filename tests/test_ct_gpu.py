@@ -12,6 +12,7 @@ from oracle import oracle
 from tests import ct_oracle as co
 from tests import ivox_oracle as io
 from tests import voxelmap_oracle as vo
+from tests import util
 from tests.util import REL_TOL, cov_colmajor16, rel_err
 
 pytestmark = pytest.mark.gpu
@@ -80,6 +81,25 @@ def ct_record_check(got, ref, what):
     assert abs(got["error"] - ref["error"]) < REL_TOL * ref["error"], what
 
 
+def ct_scale(R, xyz, cov6, starts, tau, X, Y, corr):
+    """the entry-wise scale of a CT record, through the kernel's chain: each entry's GICP sums at its fp32-cast pose T_b, its
+    H_ss / b_s through |Ad(T_b)| as factor_epilogue forms them, then the 12 x 12 system through |[D0 D1]|"""
+    A, B = {"H": np.zeros((12, 12)), "b": np.zeros(12), "error": 0.0}, {"H": np.zeros((12, 12)), "b": np.zeros(12), "error": 0.0}
+    for idx, t, c in zip(co.entry_indices(starts), tau, corr):
+        Tb = co.entry_pose(X, Y, t)
+        P = np.abs(util.adjoint_f32(Tb))
+        J = np.abs(np.concatenate(co.entry_blocks(X, Y, t), axis=1))
+        for part, s in zip((A, B), util.hit_scale(util.factor_hits(R.xyz, R.cov6, xyz[idx], cov6[idx], Tb, c))):
+            part["H"] += J.T @ P.T @ s["H_tt"] @ P @ J
+            part["b"] += J.T @ P.T @ s["b_t"]
+            part["error"] += s["error"]
+
+    def blocks(p):
+        return {"H_tt": p["H"][:6, :6], "H_ss": p["H"][6:, 6:], "H_ts": p["H"][:6, 6:], "b_t": p["b"][:6], "b_s": p["b"][6:], "error": p["error"]}
+
+    return util.EntryScale(blocks(A), blocks(B))
+
+
 def test_factor_matches_restatement_on_a_distorted_frame(ctx, scene):
     """linearize at several (X, Y) (the ground truth, perturbed poses, no motion): inlier counts exact, H and error within
     1e-4 relative, b by the project's criterion; error() with lin != eval likewise"""
@@ -89,8 +109,9 @@ def test_factor_matches_restatement_on_a_distorted_frame(ctx, scene):
     f = gpu.IntegratedCT_GICPFactorGPU(0, 1, m, src, MAX_CORR, ctx=ctx)
     for i, (Xc, Yc) in enumerate(cases):
         got = f.linearize({0: Xc, 1: Yc})
-        ref, _ = co.linearize(R, xyz, cov6, starts, tau, Xc, Yc, MAX_CORR)
+        ref, corr = co.linearize(R, xyz, cov6, starts, tau, Xc, Yc, MAX_CORR)
         ct_record_check(got, ref, i)
+        util.check_entrywise(got, ref, ct_scale(R, xyz, cov6, starts, tau, Xc, Yc, corr), what=("CT", i))
         assert np.allclose(got["H_tt"], got["H_tt"].T, rtol=0, atol=1e-9 * np.abs(got["H_tt"]).max())
     Xe, Ye = synth.perturb(X, rng, 0.005, 0.05), synth.perturb(Y, rng, 0.005, 0.05)
     f.linearize({0: X, 1: Y})

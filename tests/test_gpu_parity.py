@@ -72,9 +72,9 @@ def test_linearize_matches_oracle(ctx, dev, res):
     fac = gpu.IntegratedVGICPFactorGPU(0, 1, m, dev["cloud"][1], ctx=ctx)
     for T in util.test_poses(dev["T_gt"], 4, key=int(res * 100)):
         got = fac.linearize({0: np.eye(4), 1: T})
-        ref, _ = oracle.linearize_gpumap(ref_map, dev["xyz"][1], dev["cov6"][1], T)
+        ref, corr = oracle.linearize_gpumap(ref_map, dev["xyz"][1], dev["cov6"][1], T)
         assert ref[121] > 300  # enough inliers for the comparison to mean something (sparse 5 k-point test scans)
-        check_linearized(got, ref)
+        check_linearized(got, ref, hits=util.factor_hits(ref_map.vmean, ref_map.vcov, dev["xyz"][1], dev["cov6"][1], T, corr))
 
 
 def test_linearize_adversarial_poses(ctx, dev):
@@ -85,8 +85,8 @@ def test_linearize_adversarial_poses(ctx, dev):
     poses = [np.eye(4), synth.pose(0, 0, 0, np.pi), synth.pose(3.0, -2.0, 0.1, 0.3, 0.02, -0.01), synth.pose(-7.5, 4.25, 0.0, -2.0)]
     for T in poses:
         got = fac.linearize({1: T})
-        ref, _ = oracle.linearize_gpumap(ref_map, dev["xyz"][1], dev["cov6"][1], T)
-        check_linearized(got, ref)
+        ref, corr = oracle.linearize_gpumap(ref_map, dev["xyz"][1], dev["cov6"][1], T)
+        check_linearized(got, ref, hits=util.factor_hits(ref_map.vmean, ref_map.vcov, dev["xyz"][1], dev["cov6"][1], T, corr))
     far = synth.pose(5000.0, -3000.0, 100.0, 1.0)
     got = fac.linearize({1: far})
     assert got["num_inliers"] == 0 and got["error"] == 0 and not got["H_ss"].any()
@@ -100,6 +100,23 @@ def test_unary_and_binary_forms_agree(ctx, dev):
     b = gpu.IntegratedVGICPFactorGPU(Tt, 1, m, dev["cloud"][1], ctx=ctx).linearize({1: Ts})
     for k in ("H_ss", "b_s", "H_tt"):
         assert util.rel_err(a[k], b[k]) < 1e-6
+
+
+def test_binary_factor_between_poses_3km_out(ctx, dev):
+    """A binary factor whose two world poses are ~3 km from the origin: the device sees only their delta, which is local, so
+    every entry of the record stays within its own bound of the oracle at that delta."""
+    res = 0.5
+    m = gpu.GaussianVoxelMapGPU(res, ctx=ctx).insert(dev["cloud"][0])
+    ref_map = oracle.GpuMap(dev["xyz"][0], dev["cov6"][0], res)
+    fac = gpu.IntegratedVGICPFactorGPU(0, 1, m, dev["cloud"][1], ctx=ctx)
+    Tt = synth.pose(2400.0, -1800.0, 35.0, 0.7, 0.01, -0.02)
+    for T in util.test_poses(dev["T_gt"], 2, key=3000):
+        values = {0: Tt, 1: Tt @ T}
+        d = fac.delta(values)
+        got = fac.linearize(values)
+        ref, corr = oracle.linearize_gpumap(ref_map, dev["xyz"][1], dev["cov6"][1], d)
+        assert ref[121] > 300
+        check_linearized(got, ref, hits=util.factor_hits(ref_map.vmean, ref_map.vcov, dev["xyz"][1], dev["cov6"][1], d, corr))
 
 
 def test_error_matches_oracle(ctx, dev):
@@ -158,8 +175,8 @@ def test_factor_set_batch_equals_individual_and_is_repeatable(ctx, dev):
         assert a[i]["num_inliers"] == single[0]["num_inliers"]
     # against the oracle
     ref_map = oracle.GpuMap(dev["xyz"][0], dev["cov6"][0], 0.25)
-    ref, _ = oracle.linearize_gpumap(ref_map, dev["xyz"][1], dev["cov6"][1], T)
-    check_linearized(gpu.unpack_linearized(a[0]), ref)
+    ref, corr = oracle.linearize_gpumap(ref_map, dev["xyz"][1], dev["cov6"][1], T)
+    check_linearized(gpu.unpack_linearized(a[0]), ref, hits=util.factor_hits(ref_map.vmean, ref_map.vcov, dev["xyz"][1], dev["cov6"][1], T, corr))
     # error sweep
     e = fs.error_deltas(deltas, deltas)
     assert np.allclose(e, a["error"], rtol=1e-5)
@@ -329,8 +346,9 @@ def test_full_size_properties(ctx, sensor, n_rays, res):
     # and the oracle on the full-size input (a few seconds)
     xyz0, cov0 = oracle.pack_cloud(clouds[0][0], util.cov_colmajor16(clouds[0][1]))
     xyz1, cov1 = oracle.pack_cloud(P, util.cov_colmajor16(Cv))
-    ref, _ = oracle.linearize_gpumap(oracle.GpuMap(xyz0, cov0, res), xyz1, cov1, T)
-    check_linearized(whole, ref)
+    ref_map = oracle.GpuMap(xyz0, cov0, res)
+    ref, corr = oracle.linearize_gpumap(ref_map, xyz1, cov1, T)
+    check_linearized(whole, ref, hits=util.factor_hits(ref_map.vmean, ref_map.vcov, xyz1, cov1, T, corr))
 
 
 # ---------------------------------------------------------------------------------------------- round-2 parity holes
@@ -357,7 +375,7 @@ def test_nan_points_and_singular_covariances_match_oracle(ctx, dev, pair):
     ref, corr = oracle.linearize_gpumap(ref_map, xyz1, cov1, T)
     assert corr[5] < 0 and corr[77] < 0 and corr[301] < 0
     assert np.isfinite(got["H_ss"]).all() and np.isfinite(got["b_s"]).all()
-    check_linearized(got, ref)
+    check_linearized(got, ref, hits=util.factor_hits(ref_map.vmean, ref_map.vcov, xyz1, cov1, T, corr))
     assert gpu.overlap_gpu(m, src, T) == oracle.overlap_gpumap([ref_map], xyz1, [T])
     # singular fused covariance: zero covariances on both sides for half of the source points
     Z0 = np.zeros_like(pair["covs"][0])
@@ -373,7 +391,9 @@ def test_nan_points_and_singular_covariances_match_oracle(ctx, dev, pair):
     ref0, corr0 = oracle.linearize_gpumap(r0, x1, c1, T)
     assert (corr0[: len(Z1) // 2] >= 0).sum() > 100  # there ARE correspondences among the singular points ...
     assert ref0[121] < (corr0 >= 0).sum()  # ... and the oracle does not count them
-    check_linearized(got0, ref0)
+    hits0 = util.factor_hits(r0.vmean, r0.vcov, x1, c1, T, corr0)
+    assert len(hits0) == ref0[121]  # the per-hit data skip the singular ones too
+    check_linearized(got0, ref0, hits=hits0)
 
 
 def test_kernel_generations_agree(ctx, dev, monkeypatch):
@@ -418,9 +438,11 @@ def test_large_sweep_matches_oracle(ctx):
     rec = sw.fetch()
     xyz0, cov0 = oracle.pack_cloud(clouds[0][0], util.cov_colmajor16(clouds[0][1]))
     xyz1, cov1 = oracle.pack_cloud(clouds[1][0], util.cov_colmajor16(clouds[1][1]))
-    ref, _ = oracle.linearize_gpumap(oracle.GpuMap(xyz0, cov0, 0.25), xyz1, cov1, T)
+    ref_map = oracle.GpuMap(xyz0, cov0, 0.25)
+    ref, corr = oracle.linearize_gpumap(ref_map, xyz1, cov1, T)
+    scale = util.record_scale(util.factor_hits(ref_map.vmean, ref_map.vcov, xyz1, cov1, T, corr))
     for r in rec:
-        check_linearized(gpu.unpack_linearized(r), ref)
+        check_linearized(gpu.unpack_linearized(r), ref, hits=scale)
 
 
 def _oracle_check_factors(ctx, w, fset, picks, tol=REL_TOL):
@@ -440,9 +462,10 @@ def _oracle_check_factors(ctx, w, fset, picks, tol=REL_TOL):
                 packed[c] = oracle.pack_cloud(w.host_clouds[c][0], util.cov_colmajor16(w.host_clouds[c][1]))
         if (f.target, f.level) not in maps:
             maps[(f.target, f.level)] = oracle.GpuMap(*packed[f.target], w.resolutions[f.level])
-        ref, _ = oracle.linearize_gpumap(maps[(f.target, f.level)], *packed[f.source], fset.deltas[k], normals=w.host_normals[f.source] if w.surface_validation else None)
+        m = maps[(f.target, f.level)]
+        ref, corr = oracle.linearize_gpumap(m, *packed[f.source], fset.deltas[k], normals=w.host_normals[f.source] if w.surface_validation else None)
         got = gpu.unpack_linearized(rec[k])
-        check_linearized(got, ref, tol)
+        check_linearized(got, ref, tol, hits=util.factor_hits(m.vmean, m.vcov, *packed[f.source], fset.deltas[k], corr))
         worst = max(worst, util.rel_err(got["H_ss"], oracle.split122(ref)["H_ss"]))
     return sw, rec, worst
 
@@ -629,7 +652,7 @@ def test_surface_validation_matches_oracle(ctx, dev, pair):
     for T in util.test_poses(dev["T_gt"], 3, key=77):
         got = fac.linearize({0: np.eye(4), 1: T})
         ref, corr = oracle.linearize_gpumap(ref_map, dev["xyz"][1], dev["cov6"][1], T, normals=nrm.astype(np.float32))
-        check_linearized(got, ref)
+        check_linearized(got, ref, hits=util.factor_hits(ref_map.vmean, ref_map.vcov, dev["xyz"][1], dev["cov6"][1], T, corr))
         base = off.linearize({0: np.eye(4), 1: T})
         rejected = int((corr == -2).sum())
         assert rejected > 0 and got["num_inliers"] == base["num_inliers"] - rejected

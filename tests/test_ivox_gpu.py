@@ -10,7 +10,8 @@ from glim_b200 import capi, gpu, synth, workloads
 from oracle import oracle
 from tests import ivox_oracle as io
 from tests import voxelmap_oracle as vo
-from tests.util import REL_TOL, cov_colmajor16, rel_err
+from tests import util
+from tests.util import REL_TOL, check_linearized, cov_colmajor16
 
 pytestmark = pytest.mark.gpu
 
@@ -97,16 +98,6 @@ def target(ctx, frames):
     return m, R, src, packed(frames[3]), frames[3][2]
 
 
-def check_record(got, ref, what):
-    assert got["num_inliers"] == ref["num_inliers"] > 0, what
-    for key in ("H_tt", "H_ss", "H_ts"):
-        assert rel_err(got[key], ref[key]) < REL_TOL, (what, key)
-    for bk, hk in (("b_t", "H_tt"), ("b_s", "H_ss")):
-        scale = max(np.linalg.norm(ref[bk]), 0.1 * np.sqrt(np.trace(ref[hk]) * ref["error"]))
-        assert np.linalg.norm(got[bk] - ref[bk]) < REL_TOL * scale, (what, bk)
-    assert abs(got["error"] - ref["error"]) < REL_TOL * ref["error"], what
-
-
 def test_factor_matches_fp64_restatement(ctx, target):
     """Through the factor set at several poses: inlier counts exact, H / b / error within 1e-4 of the fp64 restatement;
     error() with T_lin != T_eval likewise."""
@@ -117,8 +108,9 @@ def test_factor_matches_fp64_restatement(ctx, target):
     fset = gpu.NonlinearFactorSetGPU(ctx).add(facs)
     recs = fset.linearize_deltas(np.stack(poses))
     for i, T in enumerate(poses):
-        ref, _ = io.linearize(R, xyz, cov6, T, MAX_CORR)
-        check_record(gpu.unpack_linearized(recs[i]), ref, i)
+        ref, corr = io.linearize(R, xyz, cov6, T, MAX_CORR)
+        assert ref["num_inliers"] > 0, i
+        check_linearized(gpu.unpack_linearized(recs[i]), ref, hits=util.factor_hits(R.xyz, R.cov6, xyz, cov6, T, corr))
     T_eval = [synth.perturb(T, rng, 0.005, 0.05) for T in poses]
     errs = fset.error_deltas(np.stack(poses), np.stack(T_eval))
     for i, (Tl, Te) in enumerate(zip(poses, T_eval)):
@@ -127,6 +119,32 @@ def test_factor_matches_fp64_restatement(ctx, target):
     # the factor's own error(): correspondences of its last linearization point, evaluated at the new values
     facs[0].linearize({0: poses[0]})
     assert abs(facs[0].error({0: T_eval[0]}) - io.error(R, xyz, cov6, poses[0], T_eval[0], MAX_CORR)) < REL_TOL * errs[0]
+
+
+def test_factor_3km_from_the_origin(ctx, frames):
+    """GLIM's odometry keeps its iVox in the world frame: frames 0-2 inserted and frame 3 registered ~3 km from the origin,
+    where the fp32 transform rounds q by ~1e-4 m and the adjoint carries the 3 km translation into H_ss, H_ts and b_s.  Inlier
+    counts exact and every entry within its own bound (the relative Frobenius bar is not asked of this case: H_ss = Ad^T H_tt
+    Ad cancels ~|t|^2 of H_tt's fp32 rounding there)."""
+    far = synth.pose(2400.0, -1800.0, 35.0, 0.7)
+    cfg = CONFIGS["mode1"]
+    m, R = make_pair(ctx, cfg)
+    for k in (0, 1, 2):
+        m.insert(gpu.PointCloudGPU.clone(frames[k][0], frames[k][1], ctx=ctx), far @ frames[k][2])
+        R.insert(*packed(frames[k]), far @ frames[k][2])
+    assert_same_ivox(m, R, "3 km")
+    src = gpu.PointCloudGPU.clone(frames[3][0], frames[3][1], ctx=ctx)
+    xyz, cov6 = packed(frames[3])
+    rng = synth.rng_for(916)
+    poses = [far @ frames[3][2]] + [synth.perturb(far @ frames[3][2], rng, 0.01, 0.1) for _ in range(2)]
+    assert min(np.linalg.norm(T[:3, 3]) for T in poses) > 2900.0
+    recs = gpu.NonlinearFactorSetGPU(ctx).add([gpu.IntegratedGICPFactorGPU(np.eye(4), 0, m, src, MAX_CORR, ctx=ctx) for _ in poses]).linearize_deltas(np.stack(poses))
+    for i, T in enumerate(poses):
+        ref, corr = io.linearize(R, xyz, cov6, T, MAX_CORR)
+        got = gpu.unpack_linearized(recs[i])
+        assert got["num_inliers"] == ref["num_inliers"] > 1000, i
+        print("3 km, relative Frobenius error:", {k: f"{util.rel_err(got[k], ref[k]):.2e}" for k in ("H_tt", "H_ss", "H_ts", "b_t", "b_s")})
+        util.check_entrywise(got, ref, util.record_scale(util.factor_hits(R.xyz, R.cov6, xyz, cov6, T, corr)), what=("3 km", i))
 
 
 def test_consumers_follow_the_ivox(ctx, frames):
@@ -150,7 +168,9 @@ def test_consumers_follow_the_ivox(ctx, frames):
         R.insert(*packed(frames[k]), frames[k][2])
     want = gpu.IntegratedGICPFactorGPU(np.eye(4), 0, m, src, MAX_CORR, ctx=ctx).linearize({0: T})
     assert want["num_inliers"] > first["num_inliers"]
-    ref, _ = io.linearize(R, xyz1, cov1, T, MAX_CORR)
+    ref, corr = io.linearize(R, xyz1, cov1, T, MAX_CORR)
+    assert ref["num_inliers"] > 0
+    scale = util.record_scale(util.factor_hits(R.xyz, R.cov6, xyz1, cov1, T, corr))
     got = {
         "factor": f_before.linearize({0: T}),
         "factor_set": gpu.unpack_linearized(fset.linearize_deltas(np.stack([T]))[0]),
@@ -160,7 +180,7 @@ def test_consumers_follow_the_ivox(ctx, frames):
         assert g["num_inliers"] == want["num_inliers"], name
         for key in ("H_ss", "b_s"):
             assert np.abs(g[key] - want[key]).max() <= 1e-12 * np.abs(want[key]).max(), (name, key)
-        check_record(g, ref, name)
+        check_linearized(g, ref, hits=scale)
 
 
 def test_align_matches_restated_lm(ctx, target):

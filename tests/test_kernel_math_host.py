@@ -16,6 +16,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle
+from tests import util
 from tests.util import REL_TOL, cov_colmajor16, rel_err, scan_pair, test_poses
 from glim_b200 import synth
 
@@ -125,6 +126,9 @@ def test_host_build_of_the_kernel_arithmetic_matches_oracle(km, data, res):
         assert rel_err(-H @ Ad, ref["H_ts"]) < REL_TOL
         scale_s = max(np.linalg.norm(ref["b_s"]), 0.1 * np.sqrt(np.trace(ref["H_ss"]) * ref["error"]))
         assert np.linalg.norm(-Ad.T @ b - ref["b_s"]) < REL_TOL * scale_s
+        # every entry of the record the epilogue forms from the host-built sums within its own error bound
+        hits = util.factor_hits(m.vmean, m.vcov, xyz, cov6, T, corr)
+        util.check_entrywise(util.epilogue(H, b, e, n, Ad), ref, util.record_scale(hits), what=("host build", res))
 
 
 def test_item_size_does_not_change_the_result_beyond_rounding(km, data):

@@ -11,7 +11,8 @@ from glim_b200 import capi, gpu, synth
 from oracle import oracle
 from tests import grid_oracle as go
 from tests import voxelmap_oracle as vo
-from tests.util import REL_TOL, cov_colmajor16, rel_err
+from tests import util
+from tests.util import REL_TOL, check_linearized, cov_colmajor16, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -81,16 +82,6 @@ def test_grid_is_bit_exact(ctx, frames, which, cell_size):
     assert (empty.num_cells, empty.num_points) == (0, 0)
 
 
-def check_record(got, ref, what):
-    assert got["num_inliers"] == ref["num_inliers"] > 0, what
-    for key in ("H_tt", "H_ss", "H_ts"):
-        assert rel_err(got[key], ref[key]) < REL_TOL, (what, key)
-    for bk, hk in (("b_t", "H_tt"), ("b_s", "H_ss")):
-        scale = max(np.linalg.norm(ref[bk]), 0.1 * np.sqrt(np.trace(ref[hk]) * ref["error"]))
-        assert np.linalg.norm(got[bk] - ref[bk]) < REL_TOL * scale, (what, bk)
-    assert abs(got["error"] - ref["error"]) < REL_TOL * ref["error"], what
-
-
 @pytest.fixture(scope="module")
 def pair(ctx, frames):
     """frame 2 as the target, frame 3 as the source"""
@@ -111,13 +102,16 @@ def test_factor_matches_fp64_restatement(ctx, pair, cell_size, want_m):
     poses = [T0] + [synth.perturb(T0, rng, 0.02, 0.3) for _ in range(3)]
     facs = [gpu.IntegratedGICPFactorGPU(np.eye(4), 0, g, src, max_corr, ctx=ctx) for _ in poses]
     assert facs[0].search_half_width() == want_m == go.half_width(R.inv, go.max_d2(max_corr), R.key_extent)
-    refs = [go.linearize(R, xyz, cov6, T, max_corr)[0] for T in poses]
-    check_record(facs[0].linearize({0: poses[0]}), refs[0], "factor")
+    lin = [go.linearize(R, xyz, cov6, T, max_corr) for T in poses]
+    refs = [r for r, _ in lin]
+    assert min(r["num_inliers"] for r in refs) > 0
+    hits = [util.record_scale(util.factor_hits(R.xyz, R.cov6, xyz, cov6, T, corr)) for T, (_, corr) in zip(poses, lin)]
+    check_linearized(facs[0].linearize({0: poses[0]}), refs[0], hits=hits[0])
     recs = gpu.NonlinearFactorSetGPU(ctx).add(facs).linearize_deltas(np.stack(poses))
     swept = gpu.Sweep(ctx, facs).linearize(np.stack(poses))
     for i in range(len(poses)):
-        check_record(gpu.unpack_linearized(recs[i]), refs[i], ("set", i))
-        check_record(gpu.unpack_linearized(swept[i]), refs[i], ("sweep", i))
+        check_linearized(gpu.unpack_linearized(recs[i]), refs[i], hits=hits[i])
+        check_linearized(gpu.unpack_linearized(swept[i]), refs[i], hits=hits[i])
     T_eval = [synth.perturb(T, rng, 0.005, 0.05) for T in poses]
     errs = gpu.NonlinearFactorSetGPU(ctx).add(facs).error_deltas(np.stack(poses), np.stack(T_eval))
     for i, (Tl, Te) in enumerate(zip(poses, T_eval)):
@@ -153,7 +147,8 @@ def test_ties_go_to_the_smaller_original_index(ctx):
         f = gpu.IntegratedGICPFactorGPU(np.eye(4), 0, g, sc, 0.5, ctx=ctx)
         ref, corr = go.linearize(R, xs, cs, np.eye(4), 0.5)
         assert (R.index[corr] < n).all()  # the restatement picks the upper point every time
-        check_record(f.linearize({0: np.eye(4)}), ref, cell)
+        assert ref["num_inliers"] > 0
+        check_linearized(f.linearize({0: np.eye(4)}), ref, hits=util.factor_hits(R.xyz, R.cov6, xs, cs, np.eye(4), corr))
 
 
 @pytest.fixture(scope="module")

@@ -24,6 +24,7 @@ from tests import icp_oracle as icp
 from tests import ivox_oracle as io
 from tests import sweep_schedule as ss
 from tests import voxelmap_oracle as vo
+from tests import util
 from tests.util import REL_TOL, check_linearized, cov_colmajor16
 
 pytestmark = pytest.mark.gpu
@@ -86,14 +87,16 @@ def cloud(ctx, S, n):
 
 
 def reference(S, level, n, T, Te, sv):
-    """-> (122-double oracle record at T, error at Te with the correspondences of T, rejected by the gate), cached"""
+    """-> (122-double oracle record at T, error at Te with the correspondences of T, rejected by the gate, its entry-wise
+    scale), cached"""
     key = (level, n, T.tobytes(), Te.tobytes(), sv)
     if key not in S["refs"]:
         m = S["refmaps"][level]
         nr = S["nrm32"][:n] if sv else None
         rec, corr = oracle.linearize_gpumap(m, S["xyz"][:n], S["cov6"][:n], T, normals=nr)
         err = oracle.error_gpumap(m, S["xyz"][:n], S["cov6"][:n], T, Te, normals=nr)
-        S["refs"][key] = (rec, err, int((corr == -2).sum()))
+        scale = util.record_scale(util.factor_hits(m.vmean, m.vcov, S["xyz"][:n], S["cov6"][:n], T, corr))
+        S["refs"][key] = (rec, err, int((corr == -2).sum()), scale)
     return S["refs"][key]
 
 
@@ -121,7 +124,7 @@ class VgicpSet:
     def check(self, rec, what):
         for f, r in enumerate(self.refs):
             try:
-                check_linearized(gpu.unpack_linearized(rec[f]), r[0])
+                check_linearized(gpu.unpack_linearized(rec[f]), r[0], hits=r[3])
             except AssertionError as e:
                 raise AssertionError((what, "factor", f, "points", self.sizes[f])) from e
 
@@ -287,7 +290,8 @@ def test_r8_sweep3_surface_validation(ctx, scene):
 
 
 def slab_rows_match(rows, rec, fset, pair, num_pairs, rtol_h, rtol_b, what):
-    """each slab row against the fp64 sum of the oracle records of its pair (1e-4) and of the device records (fp32 bars)"""
+    """each slab row against the fp64 sum of the oracle records of its pair (1e-4, and entry-wise: the members' bounds plus the
+    fp32 rounding of each summed level and of each fp32 sum of them) and of the device records (fp32 bars)"""
     used = set(pair)
     for q in range(num_pairs):
         if q not in used:
@@ -297,7 +301,11 @@ def slab_rows_match(rows, rec, fset, pair, num_pairs, rtol_h, rtol_b, what):
         members = [f for f in range(len(pair)) if pair[f] == q]
         refs = [oracle.split122(fset.refs[f][0]) for f in members]
         want = {k: sum(r[k] for r in refs) for k in refs[0]}
-        check_linearized(got, want)
+        scale = fset.refs[members[0]][3]
+        for f in members[1:]:
+            scale = scale + fset.refs[f][3]
+        stored = {k: len(members) * util.U32 * sum(np.abs(gpu.unpack_linearized(rec[f])[k]) for f in members) for k in util.KEYS}
+        check_linearized(got, want, hits=scale + util.EntryScale({k: np.zeros_like(v) for k, v in stored.items()}, stored))
         for k in ("H_tt", "H_ss", "H_ts", "b_t", "b_s"):
             dev = sum(gpu.unpack_linearized(rec[f])[k] for f in members)
             rtol = rtol_b if k[0] == "b" else rtol_h
@@ -377,7 +385,8 @@ def gicp_data(ctx):
 
 
 def gicp_reference(D, kind, n, k):
-    """(record dict, error at the eval pose) of prefix n at pose k; correspondences once per pose for the longest prefix"""
+    """(record dict, error at the eval pose, 0, entry-wise scale) of prefix n at pose k; correspondences once per pose for the
+    longest prefix"""
     K = D[kind]
     if (n, k) not in K["refs"]:
         m, T, Te = K["R"], K["poses"][k], K["evals"][k]
@@ -391,10 +400,12 @@ def gicp_reference(D, kind, n, k):
         if kind == "icp_grid":
             rec = icp.linearize(m, xyz, T, GICP_MAX_CORR, corr=corr)[0]
             err = icp.linearize(m, xyz, Te, GICP_MAX_CORR, corr=corr)[0]["error"]
+            scale = util.record_scale(util.factor_hits(m.xyz, None, xyz, None, T, corr))
         else:
             rec = io.linearize(m, xyz, cov6, T, GICP_MAX_CORR, corr=corr)[0]
             err = io.linearize(m, xyz, cov6, Te, GICP_MAX_CORR, corr=corr)[0]["error"]
-        K["refs"][(n, k)] = (rec, err)
+            scale = util.record_scale(util.factor_hits(m.xyz, m.cov6, xyz, cov6, T, corr))
+        K["refs"][(n, k)] = (rec, err, 0, scale)
     return K["refs"][(n, k)]
 
 

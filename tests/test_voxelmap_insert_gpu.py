@@ -8,8 +8,9 @@ import pytest
 
 from glim_b200 import capi, gpu, synth
 from oracle import oracle
+from tests import util
 from tests import voxelmap_oracle as vo
-from tests.util import REL_TOL, cov_colmajor16, rel_err
+from tests.util import REL_TOL, check_linearized, cov_colmajor16, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -134,8 +135,12 @@ def test_consumers_follow_the_map(ctx, frames):
         "factor_set": gpu.unpack_linearized(fset.linearize_deltas(np.stack([T]))[0]),
         "sweep": gpu.unpack_linearized(sweep.linearize(np.stack([T]))[0]),
     }
-    ref = oracle.split122(oracle.linearize_gpumap(oracle_map_of(m), xyz1, cov1, T)[0])
+    rm = oracle_map_of(m)
+    rec, corr = oracle.linearize_gpumap(rm, xyz1, cov1, T)
+    ref = oracle.split122(rec)
+    scale = util.record_scale(util.factor_hits(rm.vmean, rm.vcov, xyz1, cov1, T, corr))
     for name, g in got.items():
+        check_linearized(g, ref, hits=scale)
         assert g["num_inliers"] == want["num_inliers"] == ref["num_inliers"], name
         for key in ("H_ss", "b_s"):
             assert np.abs(g[key] - want[key]).max() <= 1e-12 * np.abs(want[key]).max(), (name, key)
