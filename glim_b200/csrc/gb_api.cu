@@ -714,9 +714,15 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   const bool small = F > 0 && total_pts <= warps * 2048;
   s->kernel_version = (kv == 3 || kv == 5) ? kv : (small ? 5 : 3);
   if (gicp) s->kernel_version = 5;  // k_gicp_sweep, k_gicp_grid_sweep and k_icp_grid_sweep run sweep5's strided items at every size
+  // sweep3 queues a hit's voxel index in 21 bits (gb_sweep_steps.cuh), so it runs a sweep only when every target is a built
+  // map of fewer than 2^21 voxels, whatever GB_KERNEL says.  An incremental map may grow past that after the sweep is made.
+  for (size_t f = 0; f < F; f++) {
+    const gb_voxelmap* t = factors[f]->target;
+    if (t->kind != GB_MAP_BUILT || t->num_voxels >= (1 << 21)) s->kernel_version = 5;
+  }
   {
     // sweep3's items: ~6 items per warp (first one static, the rest drawn dynamically), between 128 and 2048 points each,
-    // in whole rows of 32 points
+    // in whole rows of 32 points (sweep3 queues a point's offset within its item in 11 bits)
     constexpr uint64_t kItemsPerWarp = 6, kMinItem = 128, kMaxItem = 2048;
     const uint64_t want = total_pts / (warps * kItemsPerWarp) + 1;
     const int tile = (int)std::min(kMaxItem, std::max(kMinItem, want));

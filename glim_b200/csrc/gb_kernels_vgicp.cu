@@ -51,20 +51,23 @@ namespace {
 // round's accumulators over the warp (warp_reduce_scatter32) into one running float per lane instead of parking them
 // (some 150 instructions per round; slower than the live accumulators at every probe count tried, DESIGN.md 4.1).
 // =============================================================================================
-// sweep3's shared memory per warp: the queue (a round's hits and the up to 31 carried from the previous round) and the
-// parked accumulators.  48 KB per CTA, so at 2 CTAs / SM the carve-out, and with it the L1, stays what the 32 KB of
-// 512-entry queues got.
-constexpr int kQueue3 = 304;
-struct Sweep3Warp {
-  uint2 q[kQueue3];
+// sweep3's shared memory per warp: the queue (a round's hits and the up to 31 carried from the previous round, one word
+// each: probe_compact) and the parked accumulators.  Four 256-point lookup groups per round: 63.5 KB of dynamic shared
+// memory per CTA, 127 KB per SM at 2 CTAs / SM.  Rounds of two groups in 48 KB per CTA (more L1) measured 1.2 % slower on
+// the global-mapping sweep, and rounds of a whole 2048-point item (96 KB per CTA) 3 % slower (DESIGN.md 4.1).  The block is
+// 16-byte aligned: the retiring warp reuses its queue as double / float4 scratch (retire_factor).
+constexpr int kQueue3 = 4 * 256 + 31;
+struct __align__(16) Sweep3Warp {
+  unsigned q[kQueue3];
   float acc[29][32];  // acc[k][lane]: conflict-free
 };
-static_assert(sizeof(Sweep3Warp) * kWarps <= 48 * 1024, "static shared memory");
+constexpr size_t kSmem3 = sizeof(Sweep3Warp) * kWarps;
 // Probes per lane in flight.  Linearize: 8 (6 or 7 measured no faster than 5 with live accumulators on the global-mapping
-// sweep, 8 is 4.7 % faster).  Error: 7 (8 spills).  With surface validation (a dense odometry frame, livox_stress): 5, which
-// measured 1.2 % faster than 8 there (7: 0.8 %, 6: 0.5 %).
+// sweep, 8 is 4.7 % faster), four groups per 1024-point round.  Error: 7 (8 spills).  With surface validation (a dense odometry
+// frame, livox_stress): 5, which measured 1.2 % faster than 8 there (7: 0.8 %, 6: 0.5 %), one group per round (three
+// groups, 480 points, measured 0.5 % slower there).
 template <int MODE, bool SV> constexpr int kLookupUnroll3 = SV ? 5 : MODE == GB_MODE_LINEARIZE ? 8 : 7;
-template <int MODE, bool SV> constexpr int kRound3 = 32 * kLookupUnroll3<MODE, SV> * ((kQueue3 - 31) / (32 * kLookupUnroll3<MODE, SV>));  // points per round: whole lookup groups
+template <int MODE, bool SV> constexpr int kRound3 = 32 * kLookupUnroll3<MODE, SV> * (SV ? 1 : (kQueue3 - 31) / (32 * kLookupUnroll3<MODE, SV>));  // points per round: whole lookup groups
 static_assert(kRound3<GB_MODE_LINEARIZE, false> > 0 && kRound3<GB_MODE_ERROR, false> > 0 && kRound3<GB_MODE_LINEARIZE, true> > 0,
               "a round's hits and the up to 31 carried from the previous round fit the queue");
 
@@ -74,10 +77,11 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
   const int2* __restrict__ items, int num_items,
   unsigned long long* __restrict__ item_ctr, unsigned long long ctr_base,
   double* __restrict__ accum, int acc_slots, unsigned* __restrict__ done, double* __restrict__ out, float* __restrict__ slab, const PeerPush* __restrict__ peer) {
-  __shared__ __align__(16) Sweep3Warp s_w[kWarps];
+  extern __shared__ __align__(16) unsigned char s_sweep3[];  // kSmem3 bytes
+  Sweep3Warp* const s_w = reinterpret_cast<Sweep3Warp*>(s_sweep3);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned lt_mask = (1u << lane) - 1u;
-  uint2* __restrict__ q = s_w[warp].q;
+  unsigned* __restrict__ q = s_w[warp].q;
   float (*__restrict__ parked)[32] = s_w[warp].acc;
   auto desc_of = [&](int f) { return descs[f]; };  // a copy, for retire_factor
   constexpr int U = kLookupUnroll3<MODE, SV>, kRound = kRound3<MODE, SV>;
@@ -125,7 +129,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
         int v[U];
         probe_resolve(D, p, v);
 #pragma unroll
-        for (int u = 0; u < U; u++) probe_compact(v[u], i0 + u * 32 + lane, we, q, nq, lt_mask);
+        for (int u = 0; u < U; u++) probe_compact(v[u], i0 + u * 32 + lane, we, it.y, q, nq, lt_mask);
       }
       __syncwarp();
       // Whole passes of 32 hits only: the last nq % 32 hits are carried to the front of the queue for the next round (a
@@ -135,7 +139,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
         float acc[32];
         unpark(acc);
         // surface validation is a compile-time variant here (GLIM enables it for odometry factors only, which run sweep5)
-        accumulate_queue<MODE, SV>(acc, D, P, Pe, q, nacc, lane);
+        accumulate_queue<MODE, SV>(acc, D, P, Pe, q, nacc, lane, it.y);
 #pragma unroll
         for (int k = 0; k < 29; k++)
           if (MODE == GB_MODE_LINEARIZE || k >= 27) parked[k][lane] = acc[k];
@@ -364,7 +368,9 @@ static gb_status launch5(gb_sweep* s, const double* poses_eval, float* slab, con
 
 template <int MODE, bool PEER, bool SV>
 static gb_status launch3(gb_sweep* s, const double* poses_eval, float* slab, const PeerPush* pp) {
-  return gb_launch(s->ctx, "k_vgicp_sweep3", k_vgicp_sweep3<MODE, PEER, SV>, s->grid, kThreads, 0, s->d_descs, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr,
+  // above 48 KB of dynamic shared memory a kernel must opt in, per device: set at every launch (a host-side attribute write)
+  GB_CUDA(cudaFuncSetAttribute(k_vgicp_sweep3<MODE, PEER, SV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem3));
+  return gb_launch(s->ctx, "k_vgicp_sweep3", k_vgicp_sweep3<MODE, PEER, SV>, s->grid, kThreads, kSmem3, s->d_descs, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr,
                    s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
 }
 

@@ -71,6 +71,23 @@ __device__ __forceinline__ void probe_compact(int v, int i, int limit, uint2* __
   nq += __popc(m);
 }
 
+// sweep3's queue entry: one word, the point's offset within its item (< 2048: 11 bits) above the voxel index (21 bits).
+// gb_sweep_create runs a sweep on sweep3 only when every voxel index of its targets is below 2^21.
+constexpr int kQueueVoxelBits = 21;
+constexpr unsigned kQueueVoxelMask = (1u << kQueueVoxelBits) - 1u;
+
+// phase A, compaction (sweep3): as probe_compact, queueing offset i - base
+__device__ __forceinline__ void probe_compact(int v, int i, int limit, int base, unsigned* __restrict__ q, int& nq, unsigned lt_mask) {
+  if (i >= limit) v = -1;
+  const unsigned m = __ballot_sync(0xffffffffu, v >= 0);
+  if (v >= 0) q[nq + __popc(m & lt_mask)] = ((unsigned)(i - base) << kQueueVoxelBits) | (unsigned)v;
+  nq += __popc(m);
+}
+
+// a queue entry -> (point, voxel): a (point, voxel) pair as it is, or sweep3's word, whose point is base + its offset
+__device__ __forceinline__ uint2 queue_hit(const uint2 e, int) { return e; }
+__device__ __forceinline__ uint2 queue_hit(const unsigned e, int base) { return make_uint2((unsigned)base + (e >> kQueueVoxelBits), e & kQueueVoxelMask); }
+
 // One stage of warp_reduce_scatter32: lanes STEP apart swap halves of v[0, 2 STEP) and keep the sums in v[0, STEP).
 // STEP is a template argument so that every v[] index is a compile-time constant: with a runtime step the inner loop is not
 // unrolled and acc[32] lives on the stack (an LDL -> SHFL -> STL chain per item and the stack copy zeroed at every item start).
@@ -219,12 +236,12 @@ __device__ __noinline__ void factor_epilogue(int f, const FactorDesc& D, const d
 }
 
 // phase B: the lanes walk the nq queued hits, so the warp stays full whatever the inlier rate.  SV = false compiles the
-// surface validation out (no factor of the sweep has it on).
-template <int MODE, bool SV>
-__device__ __forceinline__ void accumulate_queue(float (&acc)[32], const FactorDesc& D, const PoseF& P, const PoseF& Pe, const uint2* __restrict__ q, int nq, int lane) {
+// surface validation out (no factor of the sweep has it on).  QE: the queue's entry type (queue_hit); base: sweep3's item start.
+template <int MODE, bool SV, class QE>
+__device__ __forceinline__ void accumulate_queue(float (&acc)[32], const FactorDesc& D, const PoseF& P, const PoseF& Pe, const QE* __restrict__ q, int nq, int lane, int base = 0) {
 #pragma unroll 2
   for (int k = lane; k < nq; k += 32) {
-    const uint2 e = q[k];
+    const uint2 e = queue_hit(q[k], base);
     const int i = (int)e.x;
     const float4 a0 = __ldg(&D.p0[i]);
     const float4 a1 = __ldg(&D.p1[i]);
@@ -280,9 +297,9 @@ __device__ __forceinline__ int ticket_last(unsigned* __restrict__ done, int f, c
 // copy taken in here lands ahead of acc[] in sweep3's stack frame, which changed its code and measured slower.
 template <int MODE, bool PEER>
 __device__ __forceinline__ void retire_factor(int f, const FactorDesc& D, const double* __restrict__ poses, const double* __restrict__ poses_eval,
-                                              double* __restrict__ accum, int acc_slots, double* __restrict__ out, float* __restrict__ slab, const PeerPush* __restrict__ peer, uint2* q) {
-  factor_epilogue(f, D, MODE == GB_MODE_ERROR ? poses_eval : poses, accum, acc_slots, out, slab, reinterpret_cast<double*>(q));
-  if (PEER && MODE == GB_MODE_LINEARIZE) pair_push(D, out, peer, reinterpret_cast<float*>(q) + kPairRowOffset);
+                                              double* __restrict__ accum, int acc_slots, double* __restrict__ out, float* __restrict__ slab, const PeerPush* __restrict__ peer, void* q) {
+  factor_epilogue(f, D, MODE == GB_MODE_ERROR ? poses_eval : poses, accum, acc_slots, out, slab, static_cast<double*>(q));
+  if (PEER && MODE == GB_MODE_LINEARIZE) pair_push(D, out, peer, static_cast<float*>(q) + kPairRowOffset);
 }
 
 }  // namespace
