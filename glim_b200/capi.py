@@ -97,6 +97,7 @@ _SIGNATURES = {
     "gb_icp_grid_factor_create": ([vp, vp, vp, f64, vp], st),
     "gb_cloud_estimate_normals": ([vp, vp], st),
     "gb_cloud_normals": ([vp, vp], st),
+    "gb_cloud_estimate_covariances": ([vp, vp, i32, i32], st),
     "gb_cloud_estimate_fpfh": ([vp, vp, f64], st),
     "gb_cloud_fpfh": ([vp, vp], st),
     "gb_fpfh_match": ([vp, vp, vp, vp], st),
@@ -127,6 +128,8 @@ SYMBOLS = tuple(_SIGNATURES)  # tests check the library exports exactly these
 GB_SLAB_STRIDE = 96
 GB_IPC_HANDLE_BYTES = 64
 GB_FACTOR_SURFACE_VALIDATION = 1
+# gb_cloud_estimate_covariances' outputs
+GB_CLOUD_COVARIANCES, GB_CLOUD_NORMALS = 1, 2
 
 
 class GlimB200Error(RuntimeError):

@@ -10,7 +10,8 @@
 // The voxel grouping (sort, head flags, scan, voxel starts), the hash thinning and the device cloud build are shared with the
 // voxel-map paths (gb_group_by_key, gb_group_starts, gb_thin, gb_cloud_build in gb_kernels_voxelmap.cu); the fp64 key kernel
 // and the group means are this file's.
-// The entry points gb_covariances, gb_find_neighbors, gb_voxelgrid_sampling, gb_preprocess and gb_merge_frames are defined here.
+// The entry points gb_covariances, gb_find_neighbors, gb_cloud_estimate_covariances, gb_voxelgrid_sampling, gb_preprocess and
+// gb_merge_frames are defined here.
 #include "gb_internal.cuh"
 #include "gb_cov_math.cuh"  // plane_covariance (shared with the host-compiled CPU test of the covariance arithmetic)
 
@@ -448,6 +449,32 @@ __global__ void __launch_bounds__(128) k_covariances_planes(int n_upper, const i
   s3[i] = make_float4((float)nx, (float)ny, (float)nz, 0.f);
 }
 
+// gb_cloud_estimate_covariances: the cloud's stored positions widened to fp64 (w = 1) in the caller's order (stored slot j
+// holds the caller's point perm[j]), and the device count of them for the k-NN
+__global__ void k_cloud_gather_points(int n, const float4* __restrict__ p0, const int* __restrict__ perm, double4* __restrict__ pts, int* __restrict__ count) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  if (j == 0) *count = n;
+  const float4 a = p0[j];
+  pts[perm ? perm[j] : j] = make_double4(a.x, a.y, a.z, 1.0);
+}
+// plane_covariance of the caller's point i (kc = k), cast once to fp32 as gb_cloud_upload casts it and stored into the cloud's
+// slot inv_perm[i]: the covariance (p0.w, p1, p2) when p1 is given, the normal when normals is given.  Positions are not written.
+__global__ void __launch_bounds__(128) k_cloud_covariances(int n, const double4* __restrict__ pts, const int* __restrict__ neighbors, int k, const int* __restrict__ inv_perm,
+                                                           float4* __restrict__ p0, float4* __restrict__ p1, float* __restrict__ p2, float4* __restrict__ normals) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double C[9], nrm[3];
+  plane_covariance(i, pts, neighbors, k, k, C, nrm);
+  const int o = inv_perm ? inv_perm[i] : i;
+  if (p1) {
+    p0[o].w = (float)C[0];
+    p1[o] = make_float4((float)C[1], (float)C[2], (float)C[4], (float)C[5]);
+    p2[o] = (float)C[8];
+  }
+  if (normals) normals[o] = make_float4((float)nrm[0], (float)nrm[1], (float)nrm[2], 0.f);
+}
+
 // ---- statistical outlier removal (cloud_preprocessor.cpp:165-167: gtsam_points::remove_outliers(frame, k, std_mul, threads)) [EXT]:
 // d_i = mean distance of point i to its k nearest neighbours (the query itself included, as the k-NN returns it);
 // keep i iff d_i < mean(d) + std_mul * sqrt(mean(d^2) - mean(d)^2)   (population variance over the frame) ----
@@ -708,6 +735,50 @@ extern "C" gb_status gb_find_neighbors(gb_ctx* ctx, size_t n_, const double* xyz
   GB_CHECK(gb_launch(ctx, "k_set_int", k_set_int, 1, 1, 0, d_cnt, n));
   GB_CHECK(knn_device(ctx, n, d_cnt, d_pts, k, 0.25, d_nb, knn));
   return gb_download(ctx, {{neighbors, d_nb, sizeof(int) * N * (size_t)k}});
+}
+
+// gb_find_neighbors and gb_covariances on a device cloud's own points, written back into its planes (the rule is in
+// include/glim_b200.h): k_cloud_gather_points, knn_device at 0.25 m, k_cloud_covariances
+extern "C" gb_status gb_cloud_estimate_covariances(gb_ctx* ctx, gb_cloud* cloud, int k_neighbors, int outputs) {
+  GB_REQUIRE(ctx && cloud, "null argument");
+  GB_REQUIRE(cloud->device == ctx->device, "the cloud lives on another device");
+  GB_REQUIRE(gb_knn_instantiated(k_neighbors), "k_neighbors is not an instantiated neighbour count (1-10, 12, 15, 16, 20, 24, 32)");
+  GB_REQUIRE(outputs >= 1 && outputs <= (GB_CLOUD_COVARIANCES | GB_CLOUD_NORMALS), "outputs must be GB_CLOUD_COVARIANCES, GB_CLOUD_NORMALS or both");
+  GB_REQUIRE(cloud->n * (size_t)k_neighbors < (size_t)1 << 30, "N * k_neighbors must be below 2^30");
+  GB_ENTER(ctx);
+  const bool covs = outputs & GB_CLOUD_COVARIANCES, normals = outputs & GB_CLOUD_NORMALS;
+  if (normals) {  // the features were computed from the old normals: their block goes back to the pool here
+    gb_dev_block old(ctx->device);
+    old.hand_over(cloud->f_base);
+    cloud->fpfh = nullptr;
+  }
+  const int n = (int)cloud->n, k = k_neighbors;
+  if (n > 0) {
+    gb_dev_block block(ctx->device);  // normals for a cloud built without them: a block of their own, handed over on success
+    float4* d_normals = cloud->normals;
+    if (normals && !d_normals) GB_CHECK(gb_dev_carve(ctx, block, [&](Carver& cv) { d_normals = cv.take<float4>((size_t)n); }));
+    const size_t N = (size_t)n, cub_b = gb_cub_temp_bytes(N);
+    KnnTmp knn;
+    int *d_cnt, *d_nb;
+    double4* d_pts;
+    GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
+      knn = take_knn_tmp(cv, n, cv.take<char>(cub_b), cub_b);
+      d_cnt = cv.take<int>(1);
+      d_pts = cv.take<double4>(N);
+      d_nb = cv.take<int>(N * (size_t)k);
+    }));
+    GB_CHECK(gb_launch(ctx, "k_cloud_gather_points", k_cloud_gather_points, (n + 255) / 256, 256, 0, n, cloud->p0, cloud->perm, d_pts, d_cnt));
+    GB_CHECK(knn_device(ctx, n, d_cnt, d_pts, k, 0.25, d_nb, knn));
+    GB_CHECK(gb_launch(ctx, "k_cloud_covariances", k_cloud_covariances, (n + 127) / 128, 128, 0, n, d_pts, d_nb, k, cloud->inv_perm, cloud->p0, covs ? cloud->p1 : nullptr,
+                       cloud->p2, normals ? d_normals : nullptr));
+    GB_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (normals && !cloud->normals) {
+      block.hand_over(cloud->n_base);
+      cloud->normals = d_normals;
+    }
+  }
+  if (covs) cloud->covs = true;
+  return GB_OK;
 }
 
 // =============================================================================================

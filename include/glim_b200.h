@@ -392,6 +392,40 @@ GB_API gb_status gb_icp_grid_factor_create(gb_ctx* ctx, const gb_point_grid* tar
 GB_API gb_status gb_cloud_estimate_normals(gb_ctx* ctx, gb_cloud* cloud);
 /* host copy of the normals, N x 3 in the caller's point order; GB_ERR_INVALID_ARGUMENT for a non-empty cloud without normals */
 GB_API gb_status gb_cloud_normals(const gb_cloud* cloud, float* out);
+/* ---- Covariances and normals of a device cloud from its own k nearest neighbours: gtsam_points::estimate_covariances(points, n)
+ *      of SubMap::load (sub_map.cpp:192-196, k = 10), the KdTree k-NN + CloudCovarianceEstimation::estimate of
+ *      ManualLoopCloseModal::preprocess_maps (manual_loop_close_modal.cpp:338-356, k = 10, both outputs) and
+ *      estimate_normals(points, n, k) of PointsSelector::select_points_segmentation (points_selector.cpp:785-787, k = 20).
+ *
+ *      The rule.  Points: the cloud's stored fp32 positions widened to fp64 (w = 1), in the caller's (original) order.
+ *      Neighbours: gb_find_neighbors' rule at its 0.25 m finest cell (fp64 un-contracted d2, ties to the smaller index, the
+ *      query included; the row of a non-finite point, or of a point whose cell leaves the 21-bit range, is itself k times).
+ *      The k-NN is exact, so the cell size affects time only.  Covariance and normal: gb_covariances with k_correspondences =
+ *      k_neighbors = k, i.e. CloudCovarianceEstimation::estimate with PLANE regularization and the sign rule of
+ *      cloud_covariance_estimation.cpp:98-100.  Each value is stored once as fp32, exactly as gb_cloud_upload stores it.
+ *      Postcondition: the cloud's planes, perm and inv_perm are bit-identical to a gb_cloud_upload of the widened positions,
+ *      the computed covariances if GB_CLOUD_COVARIANCES is set (else the cloud's own) and the computed normals if
+ *      GB_CLOUD_NORMALS is set (else the cloud's own).  Positions are never written, so the Morton order does not change.
+ *      [EXT] gtsam_points is not vendored: estimate_covariances(points, n) is this rule with k = 10, and
+ *      estimate_normals(points, n, k) is this rule's normal.
+ *
+ *      Side effects.  GB_CLOUD_COVARIANCES makes the cloud one with covariances: gb_gicp_grid_factor_create then accepts it as
+ *      a source and gb_cloud_estimate_normals accepts it, and the factors that read a source's covariance planes
+ *      (gb_vgicp_factor_create, gb_gicp_factor_create) read the estimated ones.  Covariances alone keep the normals and the
+ *      FPFH features.  GB_CLOUD_NORMALS gives a cloud without normals a block of its own, as gb_cloud_estimate_normals does,
+ *      and discards FPFH features.  Threading as for gb_cloud_estimate_normals: do not call it while another thread uses the
+ *      cloud.
+ *      GB_ERR_INVALID_ARGUMENT before any launch, changing nothing, for a null ctx or cloud, a cloud on another device than
+ *      ctx, a k_neighbors that is not an instantiated k-NN count (1-10, 12, 15, 16, 20, 24, 32), outputs outside {1, 2, 3},
+ *      or N * k_neighbors >= 2^30.
+ *
+ *      Launches: none for an empty cloud; any other makes 8 whatever N (k_cloud_gather_points: the stored planes into
+ *      caller-order fp64 and the device count; the k-NN's 6; k_cloud_covariances: one pass that writes straight into the
+ *      stored slots through inv_perm), then one stream synchronisation and no host transfer.  Scratch: per point 32 B of
+ *      positions and 4 k B of neighbour rows, plus the k-NN's temporaries. ---- */
+#define GB_CLOUD_COVARIANCES 1   /* sub_map.cpp:195 */
+#define GB_CLOUD_NORMALS     2   /* points_selector.cpp:787; both = manual_loop_close_modal.cpp:351-353 */
+GB_API gb_status gb_cloud_estimate_covariances(gb_ctx* ctx, gb_cloud* cloud, int k_neighbors, int outputs);
 /* The FPFH features of `cloud` with search radius r, kept on the device with the cloud (cloud_destroy releases them); a second
  * call replaces them.  GB_ERR_INVALID_ARGUMENT before any launch for a cloud without normals, a non-finite or non-positive r,
  * or a cloud on another device than ctx. */
