@@ -73,6 +73,7 @@ _SIGNATURES = {
     "gb_deskew": ([vp, vp, vp, vp, sz, vp, vp, f64, sz, vp, vp, vp, vp], st),
     "gb_align_default_params": ([vp], st),
     "gb_vgicp_align": ([vp, sz, vp, vp, vp, vp, vp], st),
+    "gb_graph_optimize": ([vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp], st),
     "gb_ivox_create": ([vp, f64, f64, i32, i32, i32, i32, vp], st),
     "gb_ivox_insert": ([vp, vp, vp, vp, f64, u64], st),
     "gb_ivox_info": ([vp, vp, vp, vp], st),
@@ -160,6 +161,14 @@ class AlignResult(C.Structure):
     """gb_align_result (include/glim_b200.h)."""
     _fields_ = [("T_target_source", C.c_double * 16), ("error", C.c_double), ("num_inliers", C.c_double), ("lambda_", C.c_double),
                 ("iterations", C.c_int), ("trials", C.c_int), ("status", C.c_int)]
+
+
+GB_GRAPH_MAX_KEYS = 32
+
+
+class GraphResult(C.Structure):
+    """gb_graph_result (include/glim_b200.h)."""
+    _fields_ = [("error", C.c_double), ("num_inliers", C.c_double), ("lambda_", C.c_double), ("iterations", C.c_int), ("trials", C.c_int), ("status", C.c_int)]
 
 
 class CtParams(C.Structure):

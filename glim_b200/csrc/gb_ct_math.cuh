@@ -232,29 +232,37 @@ GB_AHD void ct_entry_blocks(const double* xi, const double* Jinv_xi, const doubl
   for (int e = 0; e < 36; e++) D0[e] = AdE[e] - T[e];
 }
 
-// The two small terms of the objective at (X, Y): w_prior |Log(Xp^-1 X)|^2 + w_between |Log(X^-1 Y)|^2, added to the 12x12
-// system (row-major H, b over [X; Y]) when H and b are given.  Jacobians: J_r^-1(r) for X in the prior; -J_r^-1(r) Ad(Y^-1 X)
-// for X and J_r^-1(r) for Y in the between term.  No 1/2, as the CT error: e += w r^T r, H += w J^T J, b += w J^T r.
-GB_AHD double ct_small_terms(const double* X, const double* Y, const double* Xp, double w_prior, double w_between, double* H, double* b) {
-  double Xpi[16], D[16], r[6], J[36];
-  ct_inverse(Xp, Xpi);
-  align_compose(Xpi, X, D);
+// The prior term w |Log(Z^-1 T)|^2 of a pose T with prior pose Z, and, when H and b are given, its Jacobian J = J_r^-1(r)
+// added to the pose's 6x6 block: H[i * ldh + j] += w (J^T J)_ij, b[i] += w (J^T r)_i.  No 1/2, as the CT error.  Shared by
+// gb_ct_gicp_align's prior (ct_small_terms) and gb_graph_optimize's priors (gb_graph_math.cuh).
+GB_AHD double se3_prior_term(const double* T, const double* Z, double w, double* H, int ldh, double* b) {
+  double Zi[16], D[16], r[6], J[36];
+  ct_inverse(Z, Zi);
+  align_compose(Zi, T, D);
   ct_log(D, r);
   double e = 0.0;
-  for (int k = 0; k < 6; k++) e += w_prior * r[k] * r[k];
+  for (int k = 0; k < 6; k++) e += w * r[k] * r[k];
   if (H) {
     ct_se3_jr(r, true, J);
     for (int i = 0; i < 6; i++) {
       for (int j = 0; j < 6; j++) {
         double s = 0.0;
         for (int k = 0; k < 6; k++) s += J[k * 6 + i] * J[k * 6 + j];
-        H[i * 12 + j] += w_prior * s;
+        H[i * ldh + j] += w * s;
       }
       double s = 0.0;
       for (int k = 0; k < 6; k++) s += J[k * 6 + i] * r[k];
-      b[i] += w_prior * s;
+      b[i] += w * s;
     }
   }
+  return e;
+}
+
+// The two small terms of the objective at (X, Y): w_prior |Log(Xp^-1 X)|^2 + w_between |Log(X^-1 Y)|^2, added to the 12x12
+// system (row-major H, b over [X; Y]) when H and b are given.  Jacobians: J_r^-1(r) for X in the prior; -J_r^-1(r) Ad(Y^-1 X)
+// for X and J_r^-1(r) for Y in the between term.  No 1/2, as the CT error: e += w r^T r, H += w J^T J, b += w J^T r.
+GB_AHD double ct_small_terms(const double* X, const double* Y, const double* Xp, double w_prior, double w_between, double* H, double* b) {
+  double e = se3_prior_term(X, Xp, w_prior, H, 12, b);
   double xi[6], Jinv[36], AdYX[36];
   ct_problem_blocks(X, Y, xi, Jinv, AdYX);
   for (int k = 0; k < 6; k++) e += w_between * xi[k] * xi[k];

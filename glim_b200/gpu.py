@@ -787,6 +787,53 @@ def align_vgicp(problems: list[list[IntegratedVGICPFactorGPU]], T_init, params=N
     return [_result(r, "T_target_source") for r in res]
 
 
+def optimize_graphs(problems: list[dict], params=None, ctx: Context | None = None) -> list[dict]:
+    """gb_graph_optimize: LevenbergMarquardtOptimizer(graph, values) over binary matching-cost factors and pose priors, every
+    problem in one call (sub_mapping.cpp:428-452, global_mapping.cpp:393-426, manual_loop_close_modal.cpp:476-517).
+    problems[p] = dict(factors=[binary factors, all of one class], values={key: 4x4 T_world_key}, priors=[(key, 4x4, precision)]);
+    each factor's keys() name its (target, source) keys, which must be in values.  params: None (defaults), a dict of
+    gb_align_params overrides or a capi.AlignParams.
+    -> per problem {values {key: 4x4}, error, num_inliers, lambda, iterations, trials, status, status_name}"""
+    P = len(problems)
+    if P == 0:
+        return []
+    if params is None or isinstance(params, dict):
+        params = align_params(**(params or {}))
+    koff, foff, qoff = (np.zeros(P + 1, np.uint64) for _ in range(3))
+    keys, T0, flat, fkeys, qkeys, qposes, qw = [], [], [], [], [], [], []
+    for p, prob in enumerate(problems):
+        local = {k: i for i, k in enumerate(prob["values"])}
+        keys.append(list(local))
+        T0 += [np.asarray(T, dtype=np.float64).reshape(4, 4) for T in prob["values"].values()]
+        for f in prob["factors"]:
+            if not isinstance(f, IntegratedVGICPFactorGPU) or not f.is_binary():
+                raise capi.GlimB200Error("a graph takes binary VGICP, GICP or ICP factors (no fixed target pose)")
+            fkeys.append([local[k] for k in f.keys()])
+            flat.append(f)
+        for k, T, w in prob.get("priors", []):
+            qkeys.append(local[k])
+            qposes.append(np.asarray(T, dtype=np.float64).reshape(4, 4))
+            qw.append(float(w))
+        koff[p + 1], foff[p + 1], qoff[p + 1] = len(T0), len(flat), len(qw)
+    ctx = ctx or (flat[0].ctx if flat else default_context())
+    arr = (C.c_void_p * max(1, len(flat)))(*[f._handle() for f in flat])
+    T0 = pose16(np.stack(T0))
+    fk = np.ascontiguousarray(np.reshape(fkeys, (-1, 2)), dtype=np.int32)
+    qk = np.ascontiguousarray(qkeys, dtype=np.int32)
+    qp = pose16(np.stack(qposes)) if qposes else np.zeros((0, 16))
+    qwa = np.ascontiguousarray(qw, dtype=np.float64)
+    T_out = np.zeros_like(T0)
+    res = (capi.GraphResult * P)()
+    check(lib().gb_graph_optimize(ctx.h, P, ptr(koff), ptr(T0), ptr(foff), C.cast(arr, C.c_void_p), ptr(fk), ptr(qoff), ptr(qk), ptr(qp), ptr(qwa),
+                                  C.byref(params), ptr(T_out), C.cast(res, C.c_void_p)))
+    out = []
+    for p, r in enumerate(res):
+        d = {"values": {k: _pose(T_out[int(koff[p]) + i]) for i, k in enumerate(keys[p])}}
+        d.update(_result(r))
+        out.append(d)
+    return out
+
+
 def overlap_gpu(voxelmaps, source: PointCloudGPU, deltas, ctx: Context | None = None) -> float:
     """gtsam_points::overlap_gpu: single (voxelmap, delta) or lists (odometry_estimation_gpu.cpp:231, :248)."""
     if isinstance(voxelmaps, (GaussianVoxelMapGPU, IncrementalVoxelMapGPU)):

@@ -557,6 +557,43 @@ GB_API gb_status gb_align_default_params(gb_align_params* params); /* the odomet
 GB_API gb_status gb_vgicp_align(gb_ctx* ctx, size_t num_problems, const size_t* factor_offsets /* P + 1 */, gb_factor* const* factors,
                                 const double* T_init /* P x 16 */, const gb_align_params* params, gb_align_result* results /* P */);
 
+/* ---- Pose graphs: Levenberg-Marquardt over several world poses per problem, many problems in one call (sub_mapping.cpp:428-452:
+ *      the submap optimization, a 1e8 prior on X(0) and VGICP factors between every pair of keyframes; global_mapping.cpp:393-426:
+ *      a 1e6 prior on X(0) and a GICP factor; manual_loop_close_modal.cpp:476-517: a 1e6 prior on key 0 and GICP or ICP).
+ *      Problem p has K_p = key_offsets[p+1] - key_offsets[p] keys (2 <= K_p <= GB_GRAPH_MAX_KEYS), their poses T_world_key in
+ *      rows key_offsets[p] .. of T_init, the binary factors factors[factor_offsets[p] ..] on the problem-local keys
+ *      factor_keys[2f] (target) and factor_keys[2f + 1] (source), and the priors prior_offsets[p] .. on the problem-local keys
+ *      prior_keys[q] with poses Z_q (prior_poses, 16 each) and isotropic precisions w_q (prior_precisions).
+ *
+ *      The rule is gb_vgicp_align's above at 6K dof, with these differences:
+ *        1. each factor is linearized at T_t^-1 T_s and its record is assembled into the 6K x 6K system in fp64: H_tt to block
+ *           (t, t), H_ss to (s, s), H_ts to (t, s) and its transpose to (s, t), b_t to t and b_s to s; e and n sum the errors and
+ *           inlier counts.  Every entry sums its contributions in record order.  Then each prior in prior order:
+ *           r = Log(Z^-1 T_k), J = J_r^-1(r), H += w J^T J, b += w J^T r, e += w r^T r (no 1/2: priors weigh as
+ *           gb_ct_gicp_align's).  DEGENERATE when the first linearization has no inlier.
+ *        2. (H + lambda I) delta = -b by a 6K x 6K fp64 Cholesky (lambda on the whole diagonal); T_k' = T_k Exp(delta_k).  A key
+ *           no factor or prior touches has delta_k = 0.
+ *        3. e' = sum error(T_lin = T, T_eval = T') over the factors in record order, then each prior's term at T'.
+ *        4. the step tests read the largest translation step and the largest rotation step over the keys.
+ *      Each round is at most four launches for the whole batch (linearize sweep if any problem needs it, step, error sweep,
+ *      accept) and one 8-byte device-to-host copy, whatever the number of problems.
+ *      Validated before any launch: 2 <= K_p <= GB_GRAPH_MAX_KEYS; offsets that start at 0, factor offsets increasing strictly
+ *      (a factor per problem), key and prior offsets not decreasing; factor keys in range with target != source; no NULL factor,
+ *      all factors of one class of those gb_vgicp_align takes (CT and plane factors are refused) on ctx's device; finite
+ *      poses; finite precisions >= 0; prior keys in range; the bounds of gb_align_params. ---- */
+#define GB_GRAPH_MAX_KEYS 32
+typedef struct gb_graph_result {
+  double error;                /* of the returned poses, with the inliers of their last linearization, priors included */
+  double num_inliers;          /* of the last linearization, summed over the factors */
+  double lambda;
+  int iterations, trials, status; /* GB_ALIGN_* */
+} gb_graph_result;
+GB_API gb_status gb_graph_optimize(gb_ctx* ctx, size_t num_problems, const size_t* key_offsets /* P + 1 */, const double* T_init /* (sum K) x 16 */,
+                                   const size_t* factor_offsets /* P + 1 */, gb_factor* const* factors, const int32_t* factor_keys /* F x 2 */,
+                                   const size_t* prior_offsets /* P + 1 */, const int32_t* prior_keys, const double* prior_poses /* x 16 */,
+                                   const double* prior_precisions, const gb_align_params* params, double* T_out /* (sum K) x 16 */,
+                                   gb_graph_result* results /* P */);
+
 /* ---- Continuous-time GICP: GLIM's LiDAR-only odometry (OdometryEstimationCT, src/glim/odometry/odometry_estimation_ct.cpp,
  *      config/config_odometry_ct.json) on the device: the time table of a frame (:101), IntegratedCT_GICPFactor_<iVox,
  *      PointCloud>(X, Y, ivox, frame, ivox) with max_correspondence_distance (:159-163) and the Levenberg-Marquardt solve with
