@@ -74,6 +74,7 @@ _SIGNATURES = {
     "gb_align_default_params": ([vp], st),
     "gb_vgicp_align": ([vp, sz, vp, vp, vp, vp, vp], st),
     "gb_graph_optimize": ([vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp], st),
+    "gb_pose_graph_optimize": ([vp, sz, vp, sz, vp, vp, sz, vp, vp, vp, sz, vp, vp, vp, vp], st),
     "gb_ivox_create": ([vp, f64, f64, i32, i32, i32, i32, vp], st),
     "gb_ivox_insert": ([vp, vp, vp, vp, f64, u64], st),
     "gb_ivox_info": ([vp, vp, vp, vp], st),
@@ -164,6 +165,9 @@ class AlignResult(C.Structure):
 
 
 GB_GRAPH_MAX_KEYS = 32
+GB_POSE_GRAPH_MAX_KEYS = 1024
+# gb_between_term (include/glim_b200.h): Z and information column-major
+BETWEEN_DTYPE = np.dtype([("key_i", "<i4"), ("key_j", "<i4"), ("Z", "<f8", 16), ("information", "<f8", 36), ("huber_width", "<f8")], align=True)
 
 
 class GraphResult(C.Structure):

@@ -834,6 +834,53 @@ def optimize_graphs(problems: list[dict], params=None, ctx: Context | None = Non
     return out
 
 
+def between_terms(betweens, local=None) -> np.ndarray:
+    """(key_i, key_j, Z 4x4, information, huber_width) tuples -> a gb_between_term array.  information: a scalar precision w
+    (w I) or a 6x6 over [rot; trans]; huber_width: None or 0 for none; local maps keys to indices (identity when None)."""
+    out = np.zeros(len(betweens), capi.BETWEEN_DTYPE)
+    for m, (i, j, Z, info, k) in enumerate(betweens):
+        L = np.asarray(info, dtype=np.float64)
+        L = L * np.eye(6) if L.ndim == 0 else L.reshape(6, 6)
+        out[m]["key_i"], out[m]["key_j"] = (local[i], local[j]) if local is not None else (i, j)
+        out[m]["Z"] = capi.pose16(Z)
+        out[m]["information"] = L.T.reshape(36)
+        out[m]["huber_width"] = 0.0 if k is None else float(k)
+    return out
+
+
+def optimize_pose_graph(factors, values, priors=(), betweens=(), params=None, ctx: Context | None = None) -> dict:
+    """gb_pose_graph_optimize: Levenberg-Marquardt over one global map of up to 1024 poses (global_mapping.cpp:360-377, :285-351,
+    :546; global_mapping_pose_graph.cpp): binary matching-cost factors (all of one class; each factor's keys() name its
+    (target, source) keys), priors [(key, 4x4, precision)] -- GLIM's LinearDampingFactor anchor as a 1e10 prior at X(0)'s
+    initial pose -- and between terms [(key_i, key_j, Z = measured T_i^-1 T_j 4x4, information: precision or 6x6,
+    huber_width or None)].  values = {key: 4x4 T_world_key}; params: None (defaults), a dict of gb_align_params overrides or a
+    capi.AlignParams.  -> {values {key: 4x4}, error, num_inliers, lambda, iterations, trials, status, status_name}"""
+    if params is None or isinstance(params, dict):
+        params = align_params(**(params or {}))
+    local = {k: i for i, k in enumerate(values)}
+    T0 = pose16(np.stack([np.asarray(T, dtype=np.float64).reshape(4, 4) for T in values.values()]))
+    factors = list(factors)
+    fkeys = []
+    for f in factors:
+        if not isinstance(f, IntegratedVGICPFactorGPU) or not f.is_binary():
+            raise capi.GlimB200Error("a pose graph takes binary VGICP, GICP or ICP factors (no fixed target pose)")
+        fkeys.append([local[k] for k in f.keys()])
+    ctx = ctx or (factors[0].ctx if factors else default_context())
+    arr = (C.c_void_p * max(1, len(factors)))(*[f._handle() for f in factors])
+    fk = np.ascontiguousarray(np.reshape(fkeys, (-1, 2)), dtype=np.int32)
+    qk = np.ascontiguousarray([local[k] for k, _, _ in priors], dtype=np.int32)
+    qp = pose16(np.stack([np.asarray(Z, dtype=np.float64).reshape(4, 4) for _, Z, _ in priors])) if len(priors) else np.zeros((0, 16))
+    qw = np.ascontiguousarray([float(w) for _, _, w in priors], dtype=np.float64)
+    bt = between_terms(betweens, local)
+    T_out = np.zeros_like(T0)
+    res = capi.GraphResult()
+    check(lib().gb_pose_graph_optimize(ctx.h, len(T0), ptr(T0), len(factors), C.cast(arr, C.c_void_p), ptr(fk), len(qw), ptr(qk), ptr(qp), ptr(qw),
+                                       len(bt), ptr(bt), C.byref(params), ptr(T_out), C.byref(res)))
+    out = {"values": {k: _pose(T_out[i]) for i, k in enumerate(local)}}
+    out.update(_result(res))
+    return out
+
+
 def overlap_gpu(voxelmaps, source: PointCloudGPU, deltas, ctx: Context | None = None) -> float:
     """gtsam_points::overlap_gpu: single (voxelmap, delta) or lists (odometry_estimation_gpu.cpp:231, :248)."""
     if isinstance(voxelmaps, (GaussianVoxelMapGPU, IncrementalVoxelMapGPU)):

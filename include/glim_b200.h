@@ -594,6 +594,45 @@ GB_API gb_status gb_graph_optimize(gb_ctx* ctx, size_t num_problems, const size_
                                    const double* prior_precisions, const gb_align_params* params, double* T_out /* (sum K) x 16 */,
                                    gb_graph_result* results /* P */);
 
+/* ---- Global maps: Levenberg-Marquardt over one graph of up to GB_POSE_GRAPH_MAX_KEYS poses (global_mapping.cpp:360-377 optimize,
+ *      :285-351 find_overlapping_submaps, :546 save: the X(0) anchor, matching-cost factors between overlapping submaps and
+ *      between factors; global_mapping_pose_graph.cpp: the X(0) anchor, odometry between factors and Huber loop factors).
+ *      num_keys = K poses T_world_key in T_init; the binary factors on keys factor_keys[2f] (target), factor_keys[2f + 1]
+ *      (source); the priors on prior_keys[q] with poses Z_q and isotropic precisions w_q; the between terms betweens[m].
+ *
+ *      The rule is gb_graph_optimize's above for one problem at 6K dof, with these additions:
+ *        1. a between term on keys (i, j) with measurement Z, information L and Huber width k: r = Log(Z^-1 T_i^-1 T_j),
+ *           J_j = J_r^-1(r), J_i = -J_r^-1(r) Ad((T_i^-1 T_j)^-1) (GTSAM's BetweenFactor<Pose3>); m = sqrt(r^T L r); the weight
+ *           w = 1 if k == 0 or m <= k, else k / m (GTSAM's IRLS linearization, taken at the linearization poses).  It adds
+ *           w J^T L J to blocks (i, i), (j, j), (i, j), (j, i) and w J^T L r to b; its error is 2 rho(m), rho Huber's loss
+ *           (m^2 / 2 if m <= k, k m - k^2 / 2 otherwise), which is r^T L r without Huber: no 1/2, as the priors.  At trial poses
+ *           the error is recomputed from r(T'), not with a frozen weight.
+ *        2. every entry of H and b, and e, sums the factor records in record order, then the between terms in term order,
+ *           then the priors in prior order.
+ *        3. DEGENERATE only when F > 0 and the first linearization has no inlier; F = 0 with a between term is a pose graph.
+ *           A key that nothing touches keeps delta_k = 0.
+ *        4. (H + lambda I) delta = -b is solved densely: the system is padded to a multiple of 64 rows with unit diagonal and
+ *           factored by a right-looking tiled Cholesky (64 x 64 fp64 tiles) without atomics, so two identical calls give
+ *           bit-identical results.  A non-positive or non-finite pivot is a rejected trial.
+ *      Each round is at most four launches whatever K, F or the number of between terms (linearize sweep when a linearization
+ *      is needed and F > 0, step, error sweep when F > 0, accept) and one 8-byte device-to-host copy.  The context's scratch
+ *      holds two (6K) x (6K) fp64 matrices: 302 MB each at K = 1024.
+ *      Validated before any launch: 2 <= K <= GB_POSE_GRAPH_MAX_KEYS; F + num_betweens >= 1; factor, prior and between keys in
+ *      range, factor and between keys with target != source; gb_graph_optimize's factor rules (no NULL factor, one class,
+ *      no CT or plane factors, on ctx's device); finite poses and measurements; finite precisions >= 0; each information
+ *      finite and exactly symmetric; huber_width finite and >= 0; the bounds of gb_align_params. ---- */
+#define GB_POSE_GRAPH_MAX_KEYS 1024
+typedef struct gb_between_term {
+  int32_t key_i, key_j;   /* keys in [0, K), key_i != key_j */
+  double Z[16];           /* the measured T_i^-1 T_j, column-major */
+  double information[36]; /* L, symmetric, column-major */
+  double huber_width;     /* k > 0: GTSAM's Huber on the whitened norm; 0: none */
+} gb_between_term;
+GB_API gb_status gb_pose_graph_optimize(gb_ctx* ctx, size_t num_keys, const double* T_init /* K x 16 */, size_t num_factors, gb_factor* const* factors,
+                                        const int32_t* factor_keys /* F x 2 */, size_t num_priors, const int32_t* prior_keys, const double* prior_poses /* x 16 */,
+                                        const double* prior_precisions, size_t num_betweens, const gb_between_term* betweens, const gb_align_params* params,
+                                        double* T_out /* K x 16 */, gb_graph_result* result);
+
 /* ---- Continuous-time GICP: GLIM's LiDAR-only odometry (OdometryEstimationCT, src/glim/odometry/odometry_estimation_ct.cpp,
  *      config/config_odometry_ct.json) on the device: the time table of a frame (:101), IntegratedCT_GICPFactor_<iVox,
  *      PointCloud>(X, Y, ivox, frame, ivox) with max_correspondence_distance (:159-163) and the Levenberg-Marquardt solve with
