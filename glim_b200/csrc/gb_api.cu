@@ -673,6 +673,8 @@ static size_t sweep_layout(gb_sweep* s, Carver& d, Carver& h) {
   s->h_tiles = h.take<int2>(s->tiles_cap);
   s->d_gdescs = s->gicp ? d.take<GicpDesc>(F) : nullptr;
   s->h_gdescs = s->gicp ? h.take<GicpDesc>(F) : nullptr;
+  s->d_idescs = s->kernel_version == 3 ? d.take<IndexDesc>(F) : nullptr;
+  s->h_idescs = s->kernel_version == 3 ? h.take<IndexDesc>(F) : nullptr;
   return zero_bytes;
 }
 
@@ -714,11 +716,12 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
   const bool small = F > 0 && total_pts <= warps * 2048;
   s->kernel_version = (kv == 3 || kv == 5) ? kv : (small ? 5 : 3);
   if (gicp) s->kernel_version = 5;  // k_gicp_sweep, k_gicp_grid_sweep and k_icp_grid_sweep run sweep5's strided items at every size
-  // sweep3 queues a hit's voxel index in 21 bits (gb_sweep_steps.cuh), so it runs a sweep only when every target is a built
-  // map of fewer than 2^21 voxels, whatever GB_KERNEL says.  An incremental map may grow past that after the sweep is made.
+  // sweep3 probes each target's probe index (gb_probe_index.cuh) and queues a hit's voxel index in 21 bits (gb_sweep_steps.cuh),
+  // so it runs a sweep only when every target is a built map with an index -- fewer than 2^21 voxels and a box that fits 14 bits
+  // per axis -- whatever GB_KERNEL says.  An incremental map may grow past that after the sweep is made.
   for (size_t f = 0; f < F; f++) {
     const gb_voxelmap* t = factors[f]->target;
-    if (t->kind != GB_MAP_BUILT || t->num_voxels >= (1 << 21)) s->kernel_version = 5;
+    if (t->kind != GB_MAP_BUILT || !t->index) s->kernel_version = 5;
   }
   {
     // sweep3's items: ~6 items per warp (first one static, the rest drawn dynamically), between 128 and 2048 points each,
@@ -781,6 +784,13 @@ extern "C" gb_status gb_sweep_create(gb_ctx* ctx, size_t F, gb_factor* const* fa
     if (gicp) {
       memcpy(s->h_gdescs, gdescs.data(), sizeof(GicpDesc) * F);
       GB_CUDA(cudaMemcpyAsync(s->d_gdescs, s->h_gdescs, sizeof(GicpDesc) * F, cudaMemcpyHostToDevice, st));
+    }
+    if (s->kernel_version == 3) {  // every target is a built map with a probe index
+      for (size_t f = 0; f < F; f++) {
+        const gb_voxelmap* t = factors[f]->target;
+        s->h_idescs[f] = IndexDesc{t->index, ((uint32_t)t->num_buckets >> kPiSetShift) - 1u, t->box};
+      }
+      GB_CUDA(cudaMemcpyAsync(s->d_idescs, s->h_idescs, sizeof(IndexDesc) * F, cudaMemcpyHostToDevice, st));
     }
     GB_CUDA(cudaMemcpyAsync(s->d_tiles, s->h_tiles, sizeof(int2) * tiles.size(), cudaMemcpyHostToDevice, st));
     GB_CUDA(cudaMemsetAsync(s->d_accum, 0, zero_bytes, st));

@@ -15,6 +15,7 @@
 
 #include "../../include/glim_b200.h"
 #include "gb_segment_math.cuh"  // gb_frame, gb_frame_of (shared with the host-compiled CPU test of the segmentation arithmetic)
+#include "gb_probe_index.cuh"   // PiBox and the probe index of a built map (shared with the host-compiled CPU test of the index)
 
 // ---------------------------------------------------------------------------------------------
 // error plumbing
@@ -94,6 +95,10 @@ struct gb_voxelmap {
   int num_dropped_points = 0;
   int4* buckets = nullptr;
   float4* voxels = nullptr;   // 3 float4 per record: one record per voxel, or per stored point of an iVox
+  // A built map's probe index (gb_probe_index.cuh), in the block of `buckets` behind them: num_buckets >> kPiSetShift sets, or
+  // none (nullptr: another kind of map, or a box or voxel count the index cannot pack).  k_vgicp_sweep3 probes it.
+  const uint4* index = nullptr;
+  PiBox box{};
   void* base = nullptr;
   // Incremental maps and iVoxes also keep, in `base` behind the records, each voxel's packed key and the insert that last
   // touched it.  An incremental map adds each voxel's point count and fp64 sums (Sigma q: 3, Sigma C: 6 unique entries).  An
@@ -149,6 +154,14 @@ struct FactorDesc {
   int chunk;       // sweep3: points per item of THIS factor (the last factors of a sweep get smaller items: tail tapering)
 };
 static_assert(sizeof(FactorDesc) == 80, "FactorDesc size");
+// The rest of a sweep3 factor's descriptor: its target's probe index (gb_probe_index.cuh), which sweep3 probes instead of the
+// buckets.  A table of its own, so that sweep5's descriptors (and its shared-memory cache of them) keep their size.
+struct IndexDesc {
+  const uint4* sets;
+  uint32_t set_mask;  // sets - 1
+  PiBox box;
+};
+static_assert(sizeof(IndexDesc) == 40, "IndexDesc size");
 // The rest of a GICP factor's descriptor (k_gicp_sweep, k_gicp_grid_sweep): its FactorDesc carries the iVox's or point grid's
 // table (buckets, mask, max_scan, inv_res) and its point records (voxels); this adds the cells, the correspondence bound and
 // the searched offsets.
@@ -279,6 +292,8 @@ struct gb_sweep {
   bool icp = false;                 // an ICP sweep (k_icp_grid_sweep; every factor from gb_icp_grid_factor_create)
   GicpDesc* d_gdescs = nullptr;
   GicpDesc* h_gdescs = nullptr;
+  IndexDesc* d_idescs = nullptr;    // sweep3: each factor's probe index, next to the FactorDesc table
+  IndexDesc* h_idescs = nullptr;
 };
 
 // A context's grow-only buffer: device scratch or pinned host staging.  What it holds is valid until the next gb_carve on it.

@@ -14,7 +14,8 @@
 // into the warp's shared-memory queue of hits, phase B (accumulate_queue) accumulates them, then reduce_item and the
 // item's ticket (ticket_last); the warp that draws a factor's last ticket retires it (retire_factor).
 // Per inlier (one lane):
-//   q = R a + t -> voxel coord -> hash probe (16-byte buckets) -> 48-byte voxel record ->
+//   q = R a + t -> voxel coord -> hash probe (sweep3: one 16-byte set of the target's probe index, gb_probe_index.cuh;
+//   sweep5: 16-byte buckets) -> 48-byte voxel record ->
 //   S = C_B + R C_A R^T, M = S^-1 (symmetric 3x3) -> accumulate the 21 unique entries of
 //   H_tt = J_t^T M J_t (J_t = [-hat(q) | I]), the 6 of b_t = J_t^T M r, the error r^T M r and the
 //   inlier count: 29 registers.
@@ -73,7 +74,7 @@ static_assert(kRound3<GB_MODE_LINEARIZE, false> > 0 && kRound3<GB_MODE_ERROR, fa
 
 template <int MODE, bool PEER, bool SV>
 __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
-  const FactorDesc* __restrict__ descs, const double* __restrict__ poses, const double* __restrict__ poses_eval,
+  const FactorDesc* __restrict__ descs, const IndexDesc* __restrict__ idescs, const double* __restrict__ poses, const double* __restrict__ poses_eval,
   const int2* __restrict__ items, int num_items,
   unsigned long long* __restrict__ item_ctr, unsigned long long ctr_base,
   double* __restrict__ accum, int acc_slots, unsigned* __restrict__ done, double* __restrict__ out, float* __restrict__ slab, const PeerPush* __restrict__ peer) {
@@ -100,6 +101,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
     if (dynamic && lane == 0) next_item = (int)(atomicAdd(item_ctr, 1ull) - ctr_base) + total_warps;  // latency hidden behind the item
     const int f = it.x;
     const FactorDesc D = descs[f];
+    const IndexDesc I = idescs[f];
     const PoseF P = pose_from_colmajor(poses + (size_t)f * 16);
     PoseF Pe = P;
     if (MODE == GB_MODE_ERROR) Pe = pose_from_colmajor(poses_eval + (size_t)f * 16);
@@ -115,11 +117,11 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
     for (int wb = it.y; wb < item_end; wb += kRound) {
       const int we = min(wb + kRound, item_end);
       for (int i0 = wb; i0 < we; i0 += 32 * U) {
-        Probe p[U];
+        IndexProbe p[U];
 #pragma unroll
         for (int u = 0; u < U; u++) {
           const float4 a0 = __ldg(&D.p0[min(i0 + u * 32 + lane, we - 1)]);
-          probe_issue(D, P, a0.x, a0.y, a0.z, p[u]);
+          probe_issue(D, I, P, a0.x, a0.y, a0.z, p[u]);
         }
         if (!published) {  // the MEMBAR of the release overlaps with the loads above
           published = true;
@@ -127,7 +129,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep3(
           if (lane == 0) pend_last = ticket_last(done, pend_f, pend_count);
         }
         int v[U];
-        probe_resolve(D, p, v);
+        probe_resolve(I, p, v);
 #pragma unroll
         for (int u = 0; u < U; u++) probe_compact(v[u], i0 + u * 32 + lane, we, it.y, q, nq, lt_mask);
       }
@@ -370,7 +372,7 @@ template <int MODE, bool PEER, bool SV>
 static gb_status launch3(gb_sweep* s, const double* poses_eval, float* slab, const PeerPush* pp) {
   // above 48 KB of dynamic shared memory a kernel must opt in, per device: set at every launch (a host-side attribute write)
   GB_CUDA(cudaFuncSetAttribute(k_vgicp_sweep3<MODE, PEER, SV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem3));
-  return gb_launch(s->ctx, "k_vgicp_sweep3", k_vgicp_sweep3<MODE, PEER, SV>, s->grid, kThreads, kSmem3, s->d_descs, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr,
+  return gb_launch(s->ctx, "k_vgicp_sweep3", k_vgicp_sweep3<MODE, PEER, SV>, s->grid, kThreads, kSmem3, s->d_descs, s->d_idescs, s->d_poses, poses_eval, s->d_tiles, s->num_tiles, s->d_tile_ctr,
                    s->ctr_base, s->d_accum, s->acc_slots, s->d_done, s->d_out, slab, pp);
 }
 

@@ -29,6 +29,7 @@
 
 #include <cub/cub.cuh>
 
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <new>
@@ -110,13 +111,28 @@ __global__ void k_voxel_reduce(int V, const int* __restrict__ starts, const unsi
   vcoord[v] = make_int4(x, y, z, cnt);
 }
 
-__global__ void k_table_clear(int nb, int4* __restrict__ buckets) {
+// A built map's table also gets a probe index (gb_probe_index.cuh): its entries (slots, 2 (nb >> kPiSetShift) of them, nullptr
+// for other maps) are emptied here, the voxels' coordinate box ({min x y z, max x y z}) is reduced by k_table_insert, and
+// k_table_finalize inserts every voxel the final buckets hold, when the box and the voxel count fit the index.
+__global__ void k_table_clear(int nb, int4* __restrict__ buckets, unsigned long long* __restrict__ slots, int* __restrict__ box) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < nb) buckets[i] = make_int4(0, 0, 0, kEmpty);
+  if (slots && i < 2 * (nb >> kPiSetShift)) slots[i] = kPiEmpty;
+  if (box && i < 6) box[i] = i < 3 ? INT_MAX : INT_MIN;
 }
 
-__global__ void k_table_insert(int V, const int4* __restrict__ vcoord, int4* __restrict__ buckets, uint32_t mask, int max_scan, int* __restrict__ dropped_points) {
+__global__ void k_table_insert(int V, const int4* __restrict__ vcoord, int4* __restrict__ buckets, uint32_t mask, int max_scan, int* __restrict__ dropped_points,
+                               int* __restrict__ box) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (box) {  // one atomic per warp and bound (the block is whole warps)
+    const int4 b = v < V ? vcoord[v] : make_int4(INT_MAX, INT_MAX, INT_MAX, 0);
+    const int4 t = v < V ? b : make_int4(INT_MIN, INT_MIN, INT_MIN, 0);
+    const int lo[3] = {__reduce_min_sync(0xffffffffu, b.x), __reduce_min_sync(0xffffffffu, b.y), __reduce_min_sync(0xffffffffu, b.z)};
+    const int hi[3] = {__reduce_max_sync(0xffffffffu, t.x), __reduce_max_sync(0xffffffffu, t.y), __reduce_max_sync(0xffffffffu, t.z)};
+    if ((threadIdx.x & 31) == 0 && v < V) {
+      for (int k = 0; k < 3; k++) { atomicMin(&box[k], lo[k]); atomicMax(&box[3 + k], hi[k]); }
+    }
+  }
   if (v >= V) return;
   int cur = v;
   int4 c = vcoord[cur];
@@ -138,7 +154,7 @@ __global__ void k_table_insert(int V, const int4* __restrict__ vcoord, int4* __r
   }
 }
 
-__global__ void k_table_finalize(int nb, const int4* __restrict__ vcoord, int4* __restrict__ buckets) {
+__global__ void k_table_finalize(int nb, const int4* __restrict__ vcoord, int4* __restrict__ buckets, int V, unsigned long long* __restrict__ slots, const int* __restrict__ box) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nb) return;
   const int w = buckets[i].w;
@@ -147,6 +163,11 @@ __global__ void k_table_finalize(int nb, const int4* __restrict__ vcoord, int4* 
   } else {
     const int4 c = vcoord[w];
     buckets[i] = make_int4(c.x, c.y, c.z, w);
+    PiBox B;
+    if (slots && pi_box(box, V, B)) {
+      pi_insert(B, (uint32_t)(nb >> kPiSetShift) - 1u, w, c.x, c.y, c.z, [&](uint32_t k, unsigned long long expected, unsigned long long desired) { return atomicCAS(&slots[k], expected, desired); },
+                [&](uint32_t k) { atomicOr(&slots[k], 1ull); });
+    }
   }
 }
 
@@ -170,11 +191,16 @@ gb_status gb_thin(gb_ctx* ctx, int n, const int* cand, const int* count, int m, 
   return gb_launch(ctx, "k_thin_keep", k_thin_keep, blocks, 256, 0, n, cand, count, m, seed, t.keys_s, keep);
 }
 
-// The hash table of V voxels (vcoord[v] = {x, y, z, points}; d_dropped: one int of scratch, unused when V = 0): num_buckets =
+// The hash table of V voxels (vcoord[v] = {x, y, z, points}; d_dropped: one int of scratch, seven with `index`, unused when
+// V = 0): num_buckets =
 // init_buckets doubled until >= 8 V, then doubled again while more than drop_rate * total_points points fall out of it.
 // One host synchronisation per attempt.  A rejected attempt's table goes back to the pool before the next one is taken.
+// With `index` (a built map) the block also holds the probe index behind the buckets: *index points at its sets and *box is the
+// voxels' box when they fit it, else *index is nullptr.  The box is reduced into d_dropped[1..6], so that the one download of
+// each attempt brings it back with the dropped points.  A map whose box turns out too wide keeps the index's memory (8 B per
+// bucket) unused: whether the box fits is known only after k_table_insert, in the block the buckets already live in.
 static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dropped, int init_buckets, int max_scan, double drop_rate, double total_points,
-                             gb_dev_block& table, int* num_buckets, int* num_dropped_points) {
+                             gb_dev_block& table, int* num_buckets, int* num_dropped_points, const uint4** index = nullptr, PiBox* box = nullptr) {
   cudaStream_t st = ctx->stream;
   int nb = init_buckets;
   while ((long long)nb < 8ll * V) nb *= 2;  // load factor <= 1/8: the XOR-of-primes hash clusters, and lookups that
@@ -183,18 +209,32 @@ static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dr
   for (;; nb *= 2) {
     gb_dev_block attempt(ctx->device);
     int4* buckets = nullptr;
-    GB_CHECK(gb_dev_carve(ctx, attempt, [&](Carver& cv) { buckets = cv.take<int4>((size_t)nb); }));
-    GB_CHECK(gb_launch(ctx, "k_table_clear", k_table_clear, (nb + 255) / 256, 256, 0, nb, buckets));
-    int dropped = 0;
+    uint4* sets = nullptr;
+    // no index, and no memory for one, when the table is too small to have a set or the voxel indices do not fit an entry
+    const bool with_index = index && (nb >> kPiSetShift) > 0 && V < (1 << kPiVoxelBits);
+    GB_CHECK(gb_dev_carve(ctx, attempt, [&](Carver& cv) {
+      buckets = cv.take<int4>((size_t)nb);
+      if (with_index) sets = cv.take<uint4>((size_t)(nb >> kPiSetShift));
+    }));
+    unsigned long long* slots = reinterpret_cast<unsigned long long*>(sets);
+    int* d_box = with_index && V > 0 ? d_dropped + 1 : nullptr;
+    GB_CHECK(gb_launch(ctx, "k_table_clear", k_table_clear, (nb + 255) / 256, 256, 0, nb, buckets, slots, d_box));
+    int h_info[7] = {0, 0, 0, 0, 0, 0, 0};  // dropped points, then the box
     if (V > 0) {
       GB_CUDA(cudaMemsetAsync(d_dropped, 0, sizeof(int), st));
-      GB_CHECK(gb_launch(ctx, "k_table_insert", k_table_insert, (V + 255) / 256, 256, 0, V, d_vcoord, buckets, (uint32_t)nb - 1u, max_scan, d_dropped));
+      GB_CHECK(gb_launch(ctx, "k_table_insert", k_table_insert, (V + 255) / 256, 256, 0, V, d_vcoord, buckets, (uint32_t)nb - 1u, max_scan, d_dropped, d_box));
     }
-    GB_CHECK(gb_launch(ctx, "k_table_finalize", k_table_finalize, (nb + 255) / 256, 256, 0, nb, d_vcoord, buckets));
-    GB_CHECK(gb_download(ctx, {{&dropped, d_dropped, V > 0 ? sizeof(int) : 0}}));
+    GB_CHECK(gb_launch(ctx, "k_table_finalize", k_table_finalize, (nb + 255) / 256, 256, 0, nb, d_vcoord, buckets, V, slots, d_box));
+    GB_CHECK(gb_download(ctx, {{h_info, d_dropped, V > 0 ? (d_box ? 7 : 1) * sizeof(int) : 0}}));
+    const int dropped = h_info[0];
     *num_buckets = nb;
     *num_dropped_points = dropped;
     if ((double)dropped <= drop_rate * total_points || nb >= (1 << 28)) {
+      if (index) {
+        PiBox B{};
+        *index = with_index && pi_box(h_info + 1, V, B) ? sets : nullptr;
+        *box = B;
+      }
       table = std::move(attempt);
       return GB_OK;
     }
@@ -203,7 +243,7 @@ static gb_status table_build(gb_ctx* ctx, int V, const int4* d_vcoord, int* d_dr
 
 // The grouping of a cloud of n > 0 points by the build's fp32 key at inv_res, for the voxel-map build and the point grid: the
 // scratch, k_point_keys and gb_group_by_key, then the group count V read back (one host synchronisation).  starts is left for
-// gb_group_starts; vcoord and dropped are table_build's, extent the point grid's.
+// gb_group_starts; vcoord and dropped (seven ints: room for a built map's box) are table_build's, extent the point grid's.
 struct CloudGroups {
   gb_sort_tmp t;
   int *flags, *pos, *starts, *dropped, *extent;
@@ -219,7 +259,7 @@ static gb_status group_cloud(gb_ctx* ctx, const gb_cloud* cloud, float inv_res, 
     g.pos = cv.take<int>(n + 1);
     g.starts = cv.take<int>(n + 1);
     g.vcoord = cv.take<int4>(n);
-    g.dropped = cv.take<int>(1);
+    g.dropped = cv.take<int>(7);
     g.extent = cv.take<int>(1);
   }));
   GB_CHECK(gb_launch(ctx, "k_point_keys", k_point_keys, (n + 255) / 256, 256, 0, n, cloud->p0, cloud->inv_perm, inv_res, g.t.keys, g.t.idx));
@@ -262,7 +302,7 @@ extern "C" gb_status gb_voxelmap_build(gb_ctx* ctx, const gb_cloud* cloud, float
   }
   m->num_voxels = g.V;
   GB_CHECK(table_build(ctx, g.V, g.vcoord, g.dropped, init_num_buckets, max_bucket_scan_count, target_points_drop_rate, (double)n, table, &m->num_buckets,
-                       &m->num_dropped_points));
+                       &m->num_dropped_points, &m->index, &m->box));
   records.hand_over(m->base);
   table.hand_over(m->buckets);
   *out = m.release();

@@ -20,7 +20,7 @@ struct Probe {
 
 __device__ __forceinline__ bool bucket_holds(const int4 b, const Probe& p) { return b.w >= 0 && b.x == p.cx && b.y == p.cy && b.z == p.cz; }
 
-// phase A, issue: transform one source point and gather its first bucket.  The second bucket is gathered by probe_resolve,
+// phase A of sweep5 and the GICP sweeps, issue: transform one source point and gather its first bucket.  The second bucket is gathered by probe_resolve,
 // only for the lanes whose first bucket holds another voxel: 12-35 % of the points of the global-mapping sweep, by level and
 // pair kind (scripts/probe_stats.py), so gathering it up front for every point wasted a 16-byte gather on most of them.
 __device__ __forceinline__ void probe_issue(const FactorDesc& D, const PoseF& P, float ax, float ay, float az, Probe& p) {
@@ -60,6 +60,37 @@ __device__ __forceinline__ void probe_resolve(const FactorDesc& D, Probe (&p)[U]
       }
     }
   }
+}
+
+// sweep3's probe in flight: the key (the bits of key << 1 as two words: pi_key), the home set and the set gathered for it.
+struct IndexProbe {
+  uint32_t lo, hi, s;
+  uint4 e;
+};
+
+// phase A of sweep3, issue: transform one source point and gather its home set of the target's probe index
+// (gb_probe_index.cuh).  A point outside the target's box gathers nothing: it is a miss (hi = 0 matches no empty entry).
+__device__ __forceinline__ void probe_issue(const FactorDesc& D, const IndexDesc& I, const PoseF& P, float ax, float ay, float az, IndexProbe& p) {
+  float qx, qy, qz;
+  transform(P, ax, ay, az, qx, qy, qz);
+  const int cx = gb_coord(qx, D.inv_res), cy = gb_coord(qy, D.inv_res), cz = gb_coord(qz, D.inv_res);
+  const bool in = pi_key(I.box, cx, cy, cz, p.lo, p.hi);
+  p.s = pi_home(cx, cy, cz) & I.set_mask;
+  constexpr uint32_t lo = (uint32_t)kPiEmpty, hi = (uint32_t)(kPiEmpty >> 32);
+  p.e = make_uint4(lo, hi, lo, hi);
+  if (in) p.e = __ldg(&I.sets[p.s]);
+  else p.hi = 0u;
+}
+
+// phase A of sweep3, resolve: the voxel index of each probe of a group, as gb_lookup gives it.  A key absent from its home set
+// is a miss unless the set's overflow bit is set; those few probes walk the following sets after the whole group is compared.
+template <int U>
+__device__ __forceinline__ void probe_resolve(const IndexDesc& I, IndexProbe (&p)[U], int (&v)[U]) {
+#pragma unroll
+  for (int u = 0; u < U; u++) v[u] = pi_match_set(p[u].e, p[u].lo, p[u].hi);
+#pragma unroll
+  for (int u = 0; u < U; u++)
+    if (v[u] < 0 && (p[u].e.x & 1u)) v[u] = pi_walk(I.sets, I.set_mask, p[u].s, p[u].lo, p[u].hi);
 }
 
 // phase A, compaction: a hit v >= 0 of point i (none when i >= limit) is appended to the warp's queue as (point, voxel), in
