@@ -75,6 +75,9 @@ _SIGNATURES = {
     "gb_vgicp_align": ([vp, sz, vp, vp, vp, vp, vp], st),
     "gb_graph_optimize": ([vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp], st),
     "gb_pose_graph_optimize": ([vp, sz, vp, sz, vp, vp, sz, vp, vp, vp, sz, vp, vp, vp, vp], st),
+    "gb_imu_default_params": ([vp], st),
+    "gb_imu_preintegrate": ([vp, sz, vp, sz, vp, vp, vp, vp], st),
+    "gb_nav_graph_optimize": ([vp, sz, vp, sz, vp, sz, vp, sz, vp, vp, sz, vp, vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp, vp], st),
     "gb_ivox_create": ([vp, f64, f64, i32, i32, i32, i32, vp], st),
     "gb_ivox_insert": ([vp, vp, vp, vp, f64, u64], st),
     "gb_ivox_info": ([vp, vp, vp, vp], st),
@@ -168,6 +171,24 @@ GB_GRAPH_MAX_KEYS = 32
 GB_POSE_GRAPH_MAX_KEYS = 1024
 # gb_between_term (include/glim_b200.h): Z and information column-major
 BETWEEN_DTYPE = np.dtype([("key_i", "<i4"), ("key_j", "<i4"), ("Z", "<f8", 16), ("information", "<f8", 36), ("huber_width", "<f8")], align=True)
+
+
+GB_NAV_GRAPH_MAX_SLOTS = 2048
+
+
+class ImuParams(C.Structure):
+    """gb_imu_params (include/glim_b200.h)."""
+    _fields_ = [("acc_noise", C.c_double), ("gyro_noise", C.c_double), ("int_noise", C.c_double), ("gravity", C.c_double * 3)]
+
+
+# gb_imu_preintegrated (include/glim_b200.h): 9 x 3 and 9 x 9 matrices row-major
+PREINTEGRATED_DTYPE = np.dtype([("delta_t", "<f8"), ("preintegrated", "<f8", 9), ("H_bias_acc", "<f8", (9, 3)), ("H_bias_omega", "<f8", (9, 3)),
+                                ("covariance", "<f8", (9, 9)), ("bias_hat", "<f8", 6), ("gravity", "<f8", 3), ("num_integrated", "<i4"), ("pad", "<i4")], align=True)
+IMU_TERM_DTYPE = np.dtype([("pose_i", "<i4"), ("vel_i", "<i4"), ("pose_j", "<i4"), ("vel_j", "<i4"), ("bias_i", "<i4"), ("pad", "<i4"),
+                           ("pim", PREINTEGRATED_DTYPE)], align=True)
+VECTOR_TERM_DTYPE = np.dtype([("kind", "<i4"), ("key_a", "<i4"), ("key_b", "<i4"), ("pad", "<i4"), ("z", "<f8", 6), ("precision", "<f8")], align=True)
+# gb_vector_term kinds (GB_VECTOR_*)
+VECTOR_KINDS = {"velocity_prior": 0, "bias_prior": 1, "velocity_between": 2, "bias_between": 3, "rotate_velocity": 4}
 
 
 class GraphResult(C.Structure):

@@ -27,7 +27,7 @@ struct GraphProblem {
 struct GraphContrib {
   int factor, role;
 };
-enum { GB_GRAPH_H_TT = 0, GB_GRAPH_H_SS, GB_GRAPH_H_TS, GB_GRAPH_H_ST, GB_GRAPH_B_T, GB_GRAPH_B_S };
+enum { GB_GRAPH_H_TT = 0, GB_GRAPH_H_SS, GB_GRAPH_H_TS, GB_GRAPH_H_ST, GB_GRAPH_B_T, GB_GRAPH_B_S, GB_GRAPH_NAV_H, GB_GRAPH_NAV_B = GB_GRAPH_NAV_H + 25 };
 
 // What the rule keeps for one problem between rounds: the scalars of gb_vgicp_align's state (a.T, a.Tn, a.H and a.b unused;
 // the poses live in the call's T / Tn arrays).
@@ -44,9 +44,11 @@ GB_AHD int graph_packed_size(int n) { return n * (n + 1) / 2; }
 // The contributions of F factors (problem-local keys[2f] = target, keys[2f + 1] = source, target != source) to the blocks of a
 // K-key system, grouped by block and in record order within each: block k gathers contrib[cptr[k] .. cptr[k + 1]).  Each
 // factor adds H_tt to (t, t), H_ss to (s, s), H_ts to (t, s) -- stored as its transpose in the lower block (s, t) when t < s
-// -- and b_t, b_s to t, s: five contributions.  f_base is the record index of the first factor.  A counting sort: cptr must
-// hold graph_num_blocks(K) + 1 entries, contrib 5 F.
-GB_AHD void graph_contributions(int K, int F, const int* keys, int f_base, int* cptr, GraphContrib* contrib) {
+// -- and b_t, b_s to t, s: five contributions.  f_base is the record index of the first factor.  The R records that follow
+// (record index f_base + F + m) touch up to five distinct keys each, rslots[5 m ..] (-1 past the last): slot pair (a, b) adds
+// its block to the lower block of its keys (role GB_GRAPH_NAV_H + 5 a + b, key of a >= key of b) and slot a its vector
+// (GB_GRAPH_NAV_B + a).  A counting sort: cptr must hold graph_num_blocks(K) + 1 entries, contrib 5 F + 20 R.
+GB_AHD void graph_contributions(int K, int F, const int* keys, int f_base, int* cptr, GraphContrib* contrib, int R = 0, const int* rslots = nullptr) {
   const int nb = graph_num_blocks(K), tri = K * (K + 1) / 2;
   for (int k = 0; k <= nb; k++) cptr[k] = 0;
   for (int pass = 0; pass < 2; pass++) {
@@ -58,6 +60,16 @@ GB_AHD void graph_contributions(int K, int F, const int* keys, int f_base, int* 
         if (pass == 0) cptr[blk[c] + 1]++;
         else contrib[cptr[blk[c]]++] = GraphContrib{f_base + f, role[c]};
       }
+    }
+    for (int m = 0; m < R; m++) {
+      const int* sl = rslots + 5 * (size_t)m;
+      for (int a = 0; a < 5 && sl[a] >= 0; a++)
+        for (int b = 0; b <= 5; b++) {
+          if (b < 5 && (sl[b] < 0 || sl[b] > sl[a])) continue;
+          const int blk = b < 5 ? graph_block(sl[a], sl[b]) : tri + sl[a];
+          if (pass == 0) cptr[blk + 1]++;
+          else contrib[cptr[blk]++] = GraphContrib{f_base + F + m, b < 5 ? GB_GRAPH_NAV_H + 5 * a + b : GB_GRAPH_NAV_B + a};
+        }
     }
     if (pass == 0)
       for (int k = 0; k < nb; k++) cptr[k + 1] += cptr[k];

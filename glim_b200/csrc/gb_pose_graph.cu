@@ -1,4 +1,5 @@
-// gb_pose_graph.cu -- gb_pose_graph_optimize: Levenberg-Marquardt over one graph of up to 1024 poses (sm_90a).
+// gb_pose_graph.cu -- gb_pose_graph_optimize: Levenberg-Marquardt over one graph of up to 1024 poses, and gb_nav_graph_optimize:
+// the same solver over up to 2048 slots of poses, velocities and IMU biases with IMU and vector terms (sm_90a).
 //
 // Solves GLIM's global map on the device: the X(0) anchor, the matching-cost factors between overlapping submaps and the between
 // factors of global mapping (global_mapping.cpp:360-377, :285-351, :546), or the odometry and Huber loop factors of the
@@ -14,12 +15,14 @@
 // scratch; the damped padded copy; the right-looking tiled Cholesky (64 x 64 fp64 tiles: the diagonal tile by CTA 0 in shared
 // memory, the panel's rows over the grid, the trailing tiles one per CTA on the fp64 tensor cores); the blocked forward and
 // backward substitution; the retraction and the terms at the trial poses.  No sum uses an atomic, so two identical calls give
-// bit-identical results.
+// bit-identical results.  gb_pose_graph_optimize is the call of gb_nav_graph_optimize without velocities, biases, IMU terms and
+// vector terms (GLIM's enable_imu: false); both run optimize() below.
 #include "gb_internal.cuh"
 #include "gb_pose_graph_math.cuh"
 
 #include <cooperative_groups.h>
 
+#include <algorithm>
 #include <vector>
 
 namespace {
@@ -173,7 +176,7 @@ __global__ void __launch_bounds__(kAcceptThreads) k_pose_graph_accept(PoseGraphC
 }
 
 struct Inputs {
-  size_t K, F, Q, B;
+  size_t K, F, Q, B;  // K: pose keys
   const double* T_init;
   gb_factor* const* factors;
   const int32_t* fkeys;
@@ -181,12 +184,24 @@ struct Inputs {
   const double* qposes;
   const double* qw;
   const gb_between_term* bt;
+  // the navigation part (gb_nav_graph_optimize)
+  size_t KV, KB, NI, NV;
+  const double* v_init;
+  const double* b_init;
+  const gb_imu_term* it;
+  const gb_vector_term* vt;
 };
 
-gb_status validate(gb_ctx* ctx, const Inputs& in, const gb_align_params* prm) {
+// the pose graph's size
+gb_status validate_size(const Inputs& in, const gb_align_params* prm) {
   GB_REQUIRE(in.T_init && prm, "null argument");
   GB_REQUIRE(in.K >= 2 && in.K <= GB_POSE_GRAPH_MAX_KEYS, "a pose graph needs 2 to GB_POSE_GRAPH_MAX_KEYS keys");
   GB_REQUIRE(in.F + in.B >= 1, "a pose graph needs a factor or a between term");
+  return GB_OK;
+}
+
+// the pose graph's checks that do not concern its size
+gb_status validate_terms(gb_ctx* ctx, const Inputs& in, const gb_align_params* prm) {
   GB_REQUIRE(in.F < ((size_t)1 << 28) && in.B < ((size_t)1 << 24) && in.Q < ((size_t)1 << 20), "too many factors, between terms or priors");
   GB_REQUIRE(in.F == 0 || (in.factors && in.fkeys), "null factor arrays");
   GB_REQUIRE(in.Q == 0 || (in.qkeys && in.qposes && in.qw), "null prior arrays");
@@ -220,44 +235,116 @@ gb_status validate(gb_ctx* ctx, const Inputs& in, const gb_align_params* prm) {
   return gb_align_params_check(prm);
 }
 
-}  // namespace
+// the navigation graph's own checks (its size, its velocities, biases, IMU and vector terms)
+gb_status validate_nav(const Inputs& in, const gb_align_params* prm) {
+  GB_REQUIRE(in.T_init && prm, "null argument");
+  GB_REQUIRE(in.K >= 1 && in.K <= GB_NAV_GRAPH_MAX_SLOTS && in.KV <= GB_NAV_GRAPH_MAX_SLOTS && in.KB <= GB_NAV_GRAPH_MAX_SLOTS && in.K + in.KV + in.KB >= 2 &&
+                 in.K + in.KV + in.KB <= GB_NAV_GRAPH_MAX_SLOTS,
+             "a navigation graph needs a pose and 2 to GB_NAV_GRAPH_MAX_SLOTS variables");
+  GB_REQUIRE(in.NI < ((size_t)1 << 24) && in.NV < ((size_t)1 << 24), "too many IMU or vector terms");
+  GB_REQUIRE(in.F + in.B + in.NI + in.NV >= 1, "a navigation graph needs a factor, a between, an IMU or a vector term");
+  GB_REQUIRE(in.KV == 0 || in.v_init, "null velocities");
+  GB_REQUIRE(in.KB == 0 || in.b_init, "null biases");
+  GB_REQUIRE(in.NI == 0 || in.it, "null IMU terms");
+  GB_REQUIRE(in.NV == 0 || in.vt, "null vector terms");
+  GB_REQUIRE(in.KV == 0 || gb_all_finite(in.v_init, 3 * in.KV), "v_init must be finite");
+  GB_REQUIRE(in.KB == 0 || gb_all_finite(in.b_init, 6 * in.KB), "b_init must be finite");
+  const int64_t KX = (int64_t)in.K, KV = (int64_t)in.KV, KB = (int64_t)in.KB;
+  for (size_t m = 0; m < in.NI; m++) {
+    const gb_imu_term& t = in.it[m];
+    GB_REQUIRE(t.pose_i >= 0 && t.pose_j >= 0 && t.pose_i < KX && t.pose_j < KX && t.pose_i != t.pose_j, "IMU term poses must be in range and differ");
+    GB_REQUIRE(t.vel_i >= 0 && t.vel_j >= 0 && t.vel_i < KV && t.vel_j < KV && t.vel_i != t.vel_j, "IMU term velocities must be in range and differ");
+    GB_REQUIRE(t.bias_i >= 0 && t.bias_i < KB, "IMU term bias must be in range");
+    const gb_imu_preintegrated& p = t.pim;
+    GB_REQUIRE(isfinite(p.delta_t) && p.delta_t > 0.0, "IMU record delta_t must be finite and > 0");
+    GB_REQUIRE(gb_all_finite(p.preintegrated, 9) && gb_all_finite(p.H_bias_acc, 27) && gb_all_finite(p.H_bias_omega, 27) &&
+                   gb_all_finite(p.covariance, 81) && gb_all_finite(p.bias_hat, 6) && gb_all_finite(p.gravity, 3),
+               "IMU records must be finite");
+    for (int i = 0; i < 9; i++)
+      for (int j = 0; j < i; j++) GB_REQUIRE(p.covariance[i * 9 + j] == p.covariance[j * 9 + i], "IMU covariance must be exactly symmetric");
+    // positive definiteness: optimize() factors each covariance once, before any launch, and refuses a failed pivot
+  }
+  for (size_t m = 0; m < in.NV; m++) {
+    const gb_vector_term& v = in.vt[m];
+    const int64_t a = v.key_a, b = v.key_b;
+    switch (v.kind) {
+      case GB_VECTOR_VELOCITY_PRIOR: GB_REQUIRE(a >= 0 && a < KV, "vector term keys must be in range"); break;
+      case GB_VECTOR_BIAS_PRIOR: GB_REQUIRE(a >= 0 && a < KB, "vector term keys must be in range"); break;
+      case GB_VECTOR_VELOCITY_BETWEEN: GB_REQUIRE(a >= 0 && b >= 0 && a < KV && b < KV && a != b, "vector between keys must be in range and differ"); break;
+      case GB_VECTOR_BIAS_BETWEEN: GB_REQUIRE(a >= 0 && b >= 0 && a < KB && b < KB && a != b, "vector between keys must be in range and differ"); break;
+      case GB_VECTOR_ROTATE_VELOCITY: GB_REQUIRE(a >= 0 && b >= 0 && a < KX && b < KV, "vector term keys must be in range"); break;
+      default: GB_REQUIRE(false, "unknown vector term kind");
+    }
+    GB_REQUIRE(gb_all_finite(v.z, 6), "vector measurements must be finite");
+    GB_REQUIRE(isfinite(v.precision) && v.precision >= 0.0, "vector precisions must be finite and >= 0");
+  }
+  return GB_OK;
+}
 
-extern "C" gb_status gb_pose_graph_optimize(gb_ctx* ctx, size_t num_keys, const double* T_init, size_t num_factors, gb_factor* const* factors,
-                                            const int32_t* factor_keys, size_t num_priors, const int32_t* prior_keys, const double* prior_poses,
-                                            const double* prior_precisions, size_t num_betweens, const gb_between_term* betweens, const gb_align_params* prm,
-                                            double* T_out, gb_graph_result* result) {
-  GB_REQUIRE(ctx, "null ctx");
-  GB_REQUIRE(T_out && result, "null output");
-  const Inputs in{num_keys, num_factors, num_priors, num_betweens, T_init, factors, factor_keys, prior_keys, prior_poses, prior_precisions, betweens};
-  GB_CHECK(validate(ctx, in, prm));
-  const int K = (int)num_keys, F = (int)num_factors, Q = (int)num_priors, B = (int)num_betweens;
-  const int n = 6 * K, N = pg_padded(n);
+// The slots of nav term m (IMU terms first): poses at their keys, velocities from K_X, biases from K_X + K_V
+void nav_slots(const Inputs& in, std::vector<int>& slots) {
+  const int v0 = (int)in.K, b0 = (int)(in.K + in.KV);
+  slots.assign(5 * (in.NI + in.NV), -1);
+  for (size_t m = 0; m < in.NI; m++) {
+    const gb_imu_term& t = in.it[m];
+    const int s[5] = {t.pose_i, v0 + t.vel_i, t.pose_j, v0 + t.vel_j, b0 + t.bias_i};
+    for (int a = 0; a < 5; a++) slots[5 * m + a] = s[a];
+  }
+  for (size_t m = 0; m < in.NV; m++) {
+    const gb_vector_term& v = in.vt[m];
+    int* s = slots.data() + 5 * (in.NI + m);
+    switch (v.kind) {
+      case GB_VECTOR_VELOCITY_PRIOR: s[0] = v0 + v.key_a; break;
+      case GB_VECTOR_BIAS_PRIOR: s[0] = b0 + v.key_a; break;
+      case GB_VECTOR_VELOCITY_BETWEEN: s[0] = v0 + v.key_a; s[1] = v0 + v.key_b; break;
+      case GB_VECTOR_BIAS_BETWEEN: s[0] = b0 + v.key_a; s[1] = b0 + v.key_b; break;
+      default: s[0] = v.key_a; s[1] = v0 + v.key_b; break;
+    }
+  }
+}
 
-  // everything derived on the host once per call: the block CSR of the factors and between terms, the priors by key, the rows
+// The solve of a validated graph, entered in ctx.  v_out / b_out receive the velocities and biases (none for a pose graph).
+gb_status optimize(gb_ctx* ctx, const Inputs& in, const gb_align_params* prm, double* T_out, double* v_out, double* b_out, gb_graph_result* result) {
+  const int KX = (int)in.K, KV = (int)in.KV, KB = (int)in.KB, F = (int)in.F, Q = (int)in.Q, B = (int)in.B, NI = (int)in.NI, NV = (int)in.NV;
+  const int K = KX + KV + KB, n = 6 * K, N = pg_padded(n);
+
+  // everything derived on the host once per call: the slot states, the block CSR of the factors, between, IMU and vector terms,
+  // the priors by key, the rows
+  std::vector<double> X(16 * (size_t)K, 0.0);
+  std::copy(in.T_init, in.T_init + 16 * (size_t)KX, X.begin());
+  for (int k = 0; k < KV; k++) std::copy(in.v_init + 3 * k, in.v_init + 3 * k + 3, X.begin() + 16 * (size_t)(KX + k));
+  for (int k = 0; k < KB; k++) std::copy(in.b_init + 6 * k, in.b_init + 6 * k + 6, X.begin() + 16 * (size_t)(KX + KV + k));
   std::vector<int> keys(2 * (size_t)(F + B));
   for (int f = 0; f < F; f++) {
-    keys[2 * f] = factor_keys[2 * f];
-    keys[2 * f + 1] = factor_keys[2 * f + 1];
+    keys[2 * f] = in.fkeys[2 * f];
+    keys[2 * f + 1] = in.fkeys[2 * f + 1];
   }
   for (int m = 0; m < B; m++) {
-    keys[2 * (F + m)] = betweens[m].key_i;
-    keys[2 * (F + m) + 1] = betweens[m].key_j;
+    keys[2 * (F + m)] = in.bt[m].key_i;
+    keys[2 * (F + m) + 1] = in.bt[m].key_j;
   }
-  std::vector<int> cptr(graph_num_blocks(K) + 1), qptr(K + 1), qidx(Q), qkeys(prior_keys, prior_keys + Q);
-  std::vector<GraphContrib> contrib(5 * (size_t)(F + B));
-  graph_contributions(K, F + B, keys.data(), 0, cptr.data(), contrib.data());
+  std::vector<int> nslots;
+  nav_slots(in, nslots);
+  std::vector<double> nchol(81 * (size_t)NI);  // each IMU covariance factored once, here; the device whitens with these factors
+  for (int m = 0; m < NI; m++) {
+    std::copy(in.it[m].pim.covariance, in.it[m].pim.covariance + 81, nchol.begin() + 81 * (size_t)m);
+    GB_REQUIRE(imu_cholesky(nchol.data() + 81 * (size_t)m, 9), "IMU covariance must be positive definite");
+  }
+  std::vector<int> cptr(graph_num_blocks(K) + 1), qptr(K + 1), qidx(Q), qkeys(in.qkeys, in.qkeys + Q);
+  std::vector<GraphContrib> contrib(5 * (size_t)(F + B) + 20 * (size_t)(NI + NV));
+  graph_contributions(K, F + B, keys.data(), 0, cptr.data(), contrib.data(), NI + NV, nslots.data());
   pg_prior_index(K, Q, qkeys.data(), qptr.data(), qidx.data());
   AlignState st;
-  align_init(st, T_init, prm->lambda_initial);
+  align_init(st, in.T_init, prm->lambda_initial);
   std::vector<double> rows(16 * (size_t)F);
-  for (int f = 0; f < F; f++) graph_row(T_init, keys[2 * f], keys[2 * f + 1], rows.data() + 16 * f);
+  for (int f = 0; f < F; f++) graph_row(in.T_init, keys[2 * f], keys[2 * f + 1], rows.data() + 16 * f);
 
-  GB_ENTER(ctx);
   gb_sweep* sweep = nullptr;
-  if (F > 0) GB_CHECK(gb_sweep_create(ctx, num_factors, factors, nullptr, &sweep));
+  if (F > 0) GB_CHECK(gb_sweep_create(ctx, in.F, in.factors, nullptr, &sweep));
   const gb_owned<gb_sweep> s(sweep, sweep_free);  // its blocks go back to the context's pool on every exit
   PoseGraphCall c{};
   c.K = K; c.n = n; c.N = N; c.F = F; c.B = B; c.Q = Q;
+  c.KV = KV; c.KB = KB; c.NI = NI; c.NV = NV;
   unsigned* d_ctr = nullptr;
   unsigned* h_ctr = nullptr;
   GB_CHECK(gb_carve(ctx, ctx->scratch, [&](Carver& cv) {
@@ -283,6 +370,12 @@ extern "C" gb_status gb_pose_graph_optimize(gb_ctx* ctx, size_t num_keys, const 
     c.steps = cv.take<double>(2 * (size_t)K);
     c.ok = cv.take<int>(1);
     c.st = cv.take<AlignState>(1);
+    c.it = cv.take<gb_imu_term>(NI);
+    c.vt = cv.take<gb_vector_term>(NV);
+    c.nslots = cv.take<int>(nslots.size());
+    c.nrec = cv.take<double>(PG_NAV_DOUBLES * (size_t)(NI + NV));
+    c.nterm = cv.take<double>(NI + NV);
+    c.nchol = cv.take<double>(nchol.size());
     d_ctr = cv.take<unsigned>(2);
   }));
   GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { h_ctr = cv.take<unsigned>(2); }));
@@ -296,15 +389,19 @@ extern "C" gb_status gb_pose_graph_optimize(gb_ctx* ctx, size_t num_keys, const 
                            {(void*)c.qptr, qptr.data(), sizeof(int) * qptr.size()},
                            {(void*)c.qidx, qidx.data(), sizeof(int) * Q},
                            {(void*)c.fkeys, keys.data(), sizeof(int) * 2 * (size_t)F},
-                           {(void*)c.bt, betweens, sizeof(gb_between_term) * B},
+                           {(void*)c.bt, in.bt, sizeof(gb_between_term) * B},
                            {(void*)c.pkeys, qkeys.data(), sizeof(int) * Q},
-                           {(void*)c.pposes, prior_poses, sizeof(double) * 16 * Q},
-                           {(void*)c.pw, prior_precisions, sizeof(double) * Q},
-                           {c.T, T_init, sizeof(double) * 16 * K},
-                           {c.Tn, T_init, sizeof(double) * 16 * K},
+                           {(void*)c.pposes, in.qposes, sizeof(double) * 16 * Q},
+                           {(void*)c.pw, in.qw, sizeof(double) * Q},
+                           {c.T, X.data(), sizeof(double) * X.size()},
+                           {c.Tn, X.data(), sizeof(double) * X.size()},
                            {c.st, &st, sizeof(AlignState)},
                            {c.poses, rows.data(), sizeof(double) * 16 * F},
-                           {c.poses_eval, rows.data(), sizeof(double) * 16 * F}}));
+                           {c.poses_eval, rows.data(), sizeof(double) * 16 * F},
+                           {(void*)c.it, in.it, sizeof(gb_imu_term) * NI},
+                           {(void*)c.vt, in.vt, sizeof(gb_vector_term) * NV},
+                           {(void*)c.nslots, nslots.data(), sizeof(int) * nslots.size()},
+                           {(void*)c.nchol, nchol.data(), sizeof(double) * nchol.size()}}));
   // a persistent grid: as many CTAs as can be resident at once (the cooperative launch refuses more)
   GB_CUDA(cudaFuncSetAttribute(k_pose_graph_step, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStepSmem));
   int per_sm = 0;
@@ -317,7 +414,46 @@ extern "C" gb_status gb_pose_graph_optimize(gb_ctx* ctx, size_t num_keys, const 
     if (F > 0) GB_CHECK(gb_launch_sweep(s.get(), GB_MODE_ERROR));
     return gb_launch(ctx, "k_pose_graph_accept", k_pose_graph_accept, 1, kAcceptThreads, 0, c, *prm, d_ctr);
   }));
-  GB_CHECK(gb_download(ctx, {{&st, c.st, sizeof(AlignState)}, {T_out, c.T, sizeof(double) * 16 * K}}));
+  GB_CHECK(gb_download(ctx, {{&st, c.st, sizeof(AlignState)}, {X.data(), c.T, sizeof(double) * X.size()}}));
+  std::copy(X.begin(), X.begin() + 16 * (size_t)KX, T_out);
+  for (int k = 0; k < KV; k++) std::copy(X.begin() + 16 * (size_t)(KX + k), X.begin() + 16 * (size_t)(KX + k) + 3, v_out + 3 * k);
+  for (int k = 0; k < KB; k++) std::copy(X.begin() + 16 * (size_t)(KX + KV + k), X.begin() + 16 * (size_t)(KX + KV + k) + 6, b_out + 6 * k);
   align_result(st, *result);
   return GB_OK;
+}
+
+}  // namespace
+
+extern "C" gb_status gb_pose_graph_optimize(gb_ctx* ctx, size_t num_keys, const double* T_init, size_t num_factors, gb_factor* const* factors,
+                                            const int32_t* factor_keys, size_t num_priors, const int32_t* prior_keys, const double* prior_poses,
+                                            const double* prior_precisions, size_t num_betweens, const gb_between_term* betweens, const gb_align_params* prm,
+                                            double* T_out, gb_graph_result* result) {
+  GB_REQUIRE(ctx, "null ctx");
+  GB_REQUIRE(T_out && result, "null output");
+  Inputs in{};
+  in.K = num_keys; in.F = num_factors; in.Q = num_priors; in.B = num_betweens;
+  in.T_init = T_init; in.factors = factors; in.fkeys = factor_keys; in.qkeys = prior_keys; in.qposes = prior_poses; in.qw = prior_precisions; in.bt = betweens;
+  GB_CHECK(validate_size(in, prm));
+  GB_CHECK(validate_terms(ctx, in, prm));
+  GB_ENTER(ctx);
+  return optimize(ctx, in, prm, T_out, nullptr, nullptr, result);
+}
+
+extern "C" gb_status gb_nav_graph_optimize(gb_ctx* ctx, size_t num_poses, const double* T_init, size_t num_velocities, const double* v_init, size_t num_biases,
+                                           const double* b_init, size_t num_factors, gb_factor* const* factors, const int32_t* factor_keys, size_t num_priors,
+                                           const int32_t* prior_keys, const double* prior_poses, const double* prior_precisions, size_t num_betweens,
+                                           const gb_between_term* betweens, size_t num_imu_terms, const gb_imu_term* imu_terms, size_t num_vector_terms,
+                                           const gb_vector_term* vector_terms, const gb_align_params* prm, double* T_out, double* v_out, double* b_out,
+                                           gb_graph_result* result) {
+  GB_REQUIRE(ctx, "null ctx");
+  GB_REQUIRE(T_out && result && (num_velocities == 0 || v_out) && (num_biases == 0 || b_out), "null output");
+  Inputs in{};
+  in.K = num_poses; in.F = num_factors; in.Q = num_priors; in.B = num_betweens;
+  in.T_init = T_init; in.factors = factors; in.fkeys = factor_keys; in.qkeys = prior_keys; in.qposes = prior_poses; in.qw = prior_precisions; in.bt = betweens;
+  in.KV = num_velocities; in.KB = num_biases; in.NI = num_imu_terms; in.NV = num_vector_terms;
+  in.v_init = v_init; in.b_init = b_init; in.it = imu_terms; in.vt = vector_terms;
+  GB_CHECK(validate_nav(in, prm));
+  GB_CHECK(validate_terms(ctx, in, prm));
+  GB_ENTER(ctx);
+  return optimize(ctx, in, prm, T_out, v_out, b_out, result);
 }

@@ -1,6 +1,7 @@
 // gb_pose_graph_math.cuh -- the arithmetic of gb_pose_graph_optimize (gb_pose_graph.cu): the between term, the assembly of the
 // 6K x 6K system from the factors' records, the between terms and the priors, the damped padded copy, the tiled Cholesky's
-// per-tile steps and its schedule, the blocked substitution, and the two halves of a round around the error sweep.  The accept
+// per-tile steps and its schedule, the blocked substitution, and the two halves of a round around the error sweep; with
+// gb_nav_graph_optimize's velocity and bias slots, IMU and vector terms (gb_imu_math.cuh) in the same code.  The accept
 // / terminate rule is gb_vgicp_align's (align_conclude), the prior term gb_ct_gicp_align's (se3_prior_term), the block CSR and
 // the pose rows gb_graph_optimize's (graph_contributions, graph_row).  Like gb_graph_math.cuh it holds nothing that only exists
 // on the device: the loops a grid or a CTA shares are strided over (tid, nthreads) with a barrier hook, and the tile schedule
@@ -11,15 +12,23 @@
 // factor A ROW-major N x N with N = n rounded up to PG_TILE (its lower tiles used).
 #pragma once
 #include "gb_graph_math.cuh"  // GraphContrib, graph_contributions, graph_num_blocks, graph_row; through gb_ct_math.cuh: se3_prior_term, ct_*
+#include "gb_imu_math.cuh"    // imu_residual, imu_cholesky, vector_residual
 
 #define PG_TILE 64
 #define PG_PRIOR_DOUBLES 43  // a prior's record: its 6x6 block (row-major) | its 6-vector | its error
+#define PG_NAV_DOUBLES 931   // an IMU or vector term's record over its (up to 5) slots: H 30 x 30 row-major | b 30 | its error
 // a loop the device compiler keeps rolled: the between term's 6x6 products, fully unrolled, hold more doubles than a thread has
 // registers
 #ifdef __CUDA_ARCH__
 #define PG_ROLLED _Pragma("unroll 1")
 #else
 #define PG_ROLLED
+#endif
+// a function the device calls out of line: an IMU term's 9 x 30 Jacobian inlined into the step kernel would spill its registers
+#ifdef __CUDACC__
+#define PG_OUT_OF_LINE __host__ __device__ __noinline__
+#else
+#define PG_OUT_OF_LINE static inline
 #endif
 
 namespace {
@@ -117,8 +126,10 @@ GB_AHD void pg_prior_index(int K, int Q, const int* qkeys, int* qptr, int* qidx)
 }
 
 // Device pointers (or host arrays) of one call.  The block CSR (cptr, contrib) is graph_contributions' over the F factors'
-// keys followed by the B between terms' (key_i as target, key_j as source): a contribution's record index f < F reads the
-// sweep's records, f >= F the between records.
+// keys followed by the B between terms' (key_i as target, key_j as source), then the NI IMU terms' and NV vector terms' slots:
+// a contribution's record index f < F reads the sweep's records, f < F + B the between records, the rest the nav records.
+// The K slots hold the poses, then KV velocities, then KB biases (each slot 16 doubles of T / Tn: a pose's 4x4, a velocity's 3
+// or a bias's 6 leading entries); KV = KB = NI = NV = 0 is gb_pose_graph_optimize's graph.
 struct PoseGraphCall {
   int K, n, N;  // keys, 6K, n padded to PG_TILE
   int F, B, Q;
@@ -147,27 +158,101 @@ struct PoseGraphCall {
   double* poses;                  // F x 16: the sweep's linearization rows
   double* poses_eval;             // F x 16: the sweep's evaluation rows
   const double* out;              // F x 122: the sweep's records
+  int KV, KB;                     // velocity and bias slots
+  int NI, NV;                     // IMU terms, vector terms
+  const gb_imu_term* it;          // NI
+  const gb_vector_term* vt;       // NV
+  const int* nslots;              // (NI + NV) x 5: each term's slots, -1 past its last
+  double* nrec;                   // (NI + NV) x PG_NAV_DOUBLES: the terms at T
+  double* nterm;                  // NI + NV: the terms' errors at T'
+  const double* nchol;            // NI x 81: the lower Cholesky factor of each IMU record's covariance, factored by the host
 };
+
+GB_AHD int pg_num_poses(const PoseGraphCall& c) { return c.K - c.KV - c.KB; }
+
+// A dead dof: the last three of a velocity slot
+GB_AHD bool pg_pinned(const PoseGraphCall& c, int i) {
+  const int v0 = 6 * pg_num_poses(c), v1 = 6 * (c.K - c.KB);
+  return i >= v0 && i < v1 && i % 6 >= 3;
+}
+
+// IMU or vector term m (IMU terms first) at the slot states X: its error and, when rec is given, its record.  An IMU term is
+// whitened by the Cholesky factor L of its covariance (r^T S^-1 r = |L^-1 r|^2), the one the host factored when it validated
+// the record; a vector term weighs w.
+PG_OUT_OF_LINE double pg_nav_term(const PoseGraphCall& c, int m, const double* X, double* rec) {
+  const int* sl = c.nslots + 5 * (size_t)m;
+  double J[9 * IMU_TERM_COLS], r[9], w = 1.0;
+  int d, ld, cols;
+  if (m < c.NI) {
+    const gb_imu_preintegrated& p = c.it[m].pim;
+    imu_residual(X + 16 * sl[0], X + 16 * sl[1], X + 16 * sl[2], X + 16 * sl[3], X + 16 * sl[4], p, r, rec ? J : nullptr);
+    const double* L = c.nchol + 81 * (size_t)m;
+    d = 9;
+    ld = cols = IMU_TERM_COLS;
+    for (int i = 0; i < 9; i++) {  // L y = r and L Y = J
+      for (int k = 0; k < i; k++) r[i] -= L[i * 9 + k] * r[k];
+      r[i] /= L[i * 9 + i];
+      if (rec)
+        for (int a = 0; a < cols; a++) {
+          double s = J[i * ld + a];
+          for (int k = 0; k < i; k++) s -= L[i * 9 + k] * J[k * ld + a];
+          J[i * ld + a] = s / L[i * 9 + i];
+        }
+    }
+  } else {
+    const gb_vector_term& v = c.vt[m - c.NI];
+    d = vector_residual(v, X + 16 * sl[0], sl[1] >= 0 ? X + 16 * sl[1] : nullptr, r, rec ? J : nullptr);
+    w = v.precision;
+    ld = 12;
+    cols = sl[1] >= 0 ? 12 : 6;
+  }
+  double e = 0.0;
+  for (int k = 0; k < d; k++) e += r[k] * r[k];
+  e *= w;
+  if (!rec) return e;
+  PG_ROLLED
+  for (int a = 0; a < cols; a++) {
+    for (int b = 0; b <= a; b++) {
+      double s = 0.0;
+      for (int k = 0; k < d; k++) s += J[k * ld + a] * J[k * ld + b];
+      rec[a * 30 + b] = rec[b * 30 + a] = w * s;
+    }
+    double s = 0.0;
+    for (int k = 0; k < d; k++) s += J[k * ld + a] * r[k];
+    rec[900 + a] = w * s;
+  }
+  rec[930] = e;
+  return e;
+}
 
 GB_AHD double pg_entry(const PoseGraphCall& c, GraphContrib x, int r, int col) {
   if (x.factor < c.F) return graph_entry(c.out, x, r, col);
-  GraphContrib y{x.factor - c.F, x.role};
-  return graph_entry(c.brec, y, r, col);
+  if (x.factor < c.F + c.B) {
+    GraphContrib y{x.factor - c.F, x.role};
+    return graph_entry(c.brec, y, r, col);
+  }
+  const double* rec = c.nrec + (size_t)(x.factor - c.F - c.B) * PG_NAV_DOUBLES;
+  if (x.role >= GB_GRAPH_NAV_B) return rec[900 + 6 * (x.role - GB_GRAPH_NAV_B) + r];
+  const int a = (x.role - GB_GRAPH_NAV_H) / 5, b = (x.role - GB_GRAPH_NAV_H) % 5;
+  return rec[(6 * a + r) * 30 + 6 * b + col];
 }
 
-// Rule step 1 before the sums: every between record and prior record at T, one term per thread.
+// Rule step 1 before the sums: every between, prior, IMU and vector record at T, one term per thread.
 GB_AHD void pg_terms_at(const PoseGraphCall& c, int tid, int nt) {
-  for (int m = tid; m < c.B + c.Q; m += nt) {
+  for (int m = tid; m < c.B + c.Q + c.NI + c.NV; m += nt) {
     if (m < c.B) pg_between_term(c.T + 16 * c.bt[m].key_i, c.T + 16 * c.bt[m].key_j, c.bt[m], c.brec + 122 * (size_t)m);
-    else {
+    else if (m >= c.B + c.Q) {
+      const int t = m - c.B - c.Q;
+      pg_nav_term(c, t, c.T, c.nrec + PG_NAV_DOUBLES * (size_t)t);
+    } else {
       const int q = m - c.B;
       pg_prior_record(c.T + 16 * c.pkeys[q], c.pposes + 16 * q, c.pw[q], c.prec + PG_PRIOR_DOUBLES * (size_t)q);
     }
   }
 }
 
-// The lower 6x6 blocks of H and b: every entry the sum of the factor records in record order, then the between terms in term
-// order (one CSR), then the priors of its key in prior order, from 0.0.  One entry per thread; a block's row and column come
+// The lower 6x6 blocks of H and b: every entry the sum of the factor records in record order, then the between terms, the IMU
+// terms and the vector terms in term order (one CSR), then the priors of its key in prior order, from 0.0.  One entry per thread; a block's row and column come
 // from its packed index, not from a search.
 GB_AHD void pg_assemble(const PoseGraphCall& c, int tid, int nt) {
   const int K = c.K, n = c.n, tri = K * (K + 1) / 2;
@@ -200,6 +285,7 @@ GB_AHD void pg_linearized(const PoseGraphCall& c) {
     m += c.out[(size_t)f * 122 + 121];
   }
   for (int t = 0; t < c.B; t++) e += c.brec[(size_t)t * 122 + 120];
+  for (int t = 0; t < c.NI + c.NV; t++) e += c.nrec[PG_NAV_DOUBLES * (size_t)t + 930];
   for (int q = 0; q < c.Q; q++) e += c.prec[PG_PRIOR_DOUBLES * (size_t)q + 42];
   s.e = e;
   s.n = m;
@@ -208,18 +294,18 @@ GB_AHD void pg_linearized(const PoseGraphCall& c) {
   if (c.F > 0 && m == 0.0 && s.iterations == 1) s.status = GB_ALIGN_DEGENERATE;
 }
 
-// A = H + lambda I on the lower tiles (0 above the diagonal of a diagonal tile), a unit diagonal on the padded rows; x = -b, 0
-// on the padded rows.
+// A = H + lambda I on the lower tiles (0 above the diagonal of a diagonal tile), a unit diagonal on the padded rows and the
+// pinned velocity dofs (whose rows and columns of H are zero); x = -b, 0 on the padded rows and the pinned dofs.
 GB_AHD void pg_damped_copy(const PoseGraphCall& c, double lambda, int tid, int nt) {
   const int n = c.n, N = c.N;
   for (long long e = tid; e < (long long)N * N; e += nt) {
     const int i = (int)(e / N), j = (int)(e % N);
     if (j / PG_TILE > i / PG_TILE) continue;
     double v = 0.0;
-    if (j <= i) v = i < n ? c.H[(size_t)i * n + j] + (i == j ? lambda : 0.0) : (i == j ? 1.0 : 0.0);
+    if (j <= i) v = i < n && !pg_pinned(c, i) ? c.H[(size_t)i * n + j] + (i == j ? lambda : 0.0) : (i == j ? 1.0 : 0.0);
     c.A[e] = v;
   }
-  for (int i = tid; i < N; i += nt) c.x[i] = i < n ? -c.b[i] : 0.0;
+  for (int i = tid; i < N; i += nt) c.x[i] = i < n && !pg_pinned(c, i) ? -c.b[i] : 0.0;
 }
 
 // ---- the tile steps of the factorization and the substitution ----
@@ -333,13 +419,17 @@ GB_AHD bool pg_cholesky_solve(G& g, int N) {
 GB_AHD int pg_rows_begin(int kt, bool backward) { return backward ? 0 : (kt + 1) * PG_TILE; }
 GB_AHD int pg_rows_end(int kt, int N, bool backward) { return backward ? kt * PG_TILE : N; }
 
-// Rule step 2 after the solve, by a grid of nt threads (two phases around sync): T'_k = T_k Exp(delta_k) (T' = T when the
-// factorization failed) with each key's step; then the largest steps, the trial count and, for every thread, the between and
-// prior errors at T' and each factor's evaluation row.
+// Rule step 2 after the solve, by a grid of nt threads (two phases around sync): T'_k = T_k Exp(delta_k) with each pose's
+// step, v' = v + delta, b' = b + delta (X' = X when the factorization failed); then the largest pose steps, the trial count
+// and, for every thread, the between, prior, IMU and vector errors at T' and each factor's evaluation row.
 template <class Sync>
 GB_AHD void pg_retract(const PoseGraphCall& c, bool solved, int tid, int nt, Sync sync) {
+  const int KX = pg_num_poses(c);
   for (int k = tid; k < c.K; k += nt) {
-    if (solved) {
+    if (solved && k >= KX) {
+      const int dof = k < KX + c.KV ? 3 : 6;
+      for (int e = 0; e < 16; e++) c.Tn[16 * k + e] = e < dof ? c.T[16 * k + e] + c.x[6 * k + e] : c.T[16 * k + e];
+    } else if (solved) {
       double E[16];
       align_exp(c.x + 6 * k, E);
       align_compose(c.T + 16 * k, E, c.Tn + 16 * k);
@@ -356,13 +446,14 @@ GB_AHD void pg_retract(const PoseGraphCall& c, bool solved, int tid, int nt, Syn
     s.dt = 0.0;
     s.dr = 0.0;
     if (solved)
-      for (int k = 0; k < c.K; k++) {
+      for (int k = 0; k < KX; k++) {
         s.dt = c.steps[2 * k] > s.dt ? c.steps[2 * k] : s.dt;
         s.dr = c.steps[2 * k + 1] > s.dr ? c.steps[2 * k + 1] : s.dr;
       }
   }
-  for (int m = tid; m < c.B + c.Q; m += nt) {
+  for (int m = tid; m < c.B + c.Q + c.NI + c.NV; m += nt) {
     if (m < c.B) c.bterm[m] = pg_between_term(c.Tn + 16 * c.bt[m].key_i, c.Tn + 16 * c.bt[m].key_j, c.bt[m], nullptr);
+    else if (m >= c.B + c.Q) c.nterm[m - c.B - c.Q] = pg_nav_term(c, m - c.B - c.Q, c.Tn, nullptr);
     else {
       const int q = m - c.B;
       c.pterm[q] = se3_prior_term(c.Tn + 16 * c.pkeys[q], c.pposes + 16 * q, c.pw[q], nullptr, 0, nullptr);
@@ -371,12 +462,13 @@ GB_AHD void pg_retract(const PoseGraphCall& c, bool solved, int tid, int nt, Syn
   for (int f = tid; f < c.F; f += nt) graph_row(c.Tn, c.fkeys[2 * f], c.fkeys[2 * f + 1], c.poses_eval + 16 * (size_t)f);
 }
 
-// Rule steps 3-5 (one thread): e' = the factors' errors at T' in record order, then the between terms', then the priors';
-// align_conclude.  Returns whether the trial was accepted (pg_accept_rows follows).
+// Rule steps 3-5 (one thread): e' = the factors' errors at T' in record order, then the between terms', the IMU and vector
+// terms', then the priors'; align_conclude.  Returns whether the trial was accepted (pg_accept_rows follows).
 GB_AHD bool pg_conclude(const PoseGraphCall& c, const gb_align_params& prm) {
   double e = 0.0;
   for (int f = 0; f < c.F; f++) e += c.out[(size_t)f * 122 + 120];
   for (int m = 0; m < c.B; m++) e += c.bterm[m];
+  for (int m = 0; m < c.NI + c.NV; m++) e += c.nterm[m];
   for (int q = 0; q < c.Q; q++) e += c.pterm[q];
   align_conclude(*c.st, prm, e);
   return c.st->need_lin != 0;

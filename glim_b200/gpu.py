@@ -881,6 +881,102 @@ def optimize_pose_graph(factors, values, priors=(), betweens=(), params=None, ct
     return out
 
 
+def imu_params(**overrides) -> capi.ImuParams:
+    """gb_imu_default_params (config_sensors.json's noises, MakeSharedU's gravity) with the given fields replaced."""
+    p = capi.ImuParams()
+    check(lib().gb_imu_default_params(C.byref(p)))
+    for k, v in overrides.items():
+        if k not in dict(capi.ImuParams._fields_):
+            raise capi.GlimB200Error(f"gb_imu_params has no field {k}")
+        if k == "gravity":
+            p.gravity[:] = [float(x) for x in v]
+        else:
+            setattr(p, k, v)
+    return p
+
+
+def imu_preintegrate(samples, intervals, biases, params=None, ctx: Context | None = None) -> np.ndarray:
+    """gb_imu_preintegrate: IMUIntegration::integrate_imu over GTSAM's PreintegratedImuMeasurements for every interval in one
+    launch.  samples: (S,7) rows (t, ax, ay, az, wx, wy, wz), non-decreasing t; intervals: (I,2) rows (start, end); biases: (I,6)
+    [acc; gyro]; params: None (defaults), a dict of gb_imu_params overrides or a capi.ImuParams.
+    -> (I,) capi.PREINTEGRATED_DTYPE records"""
+    if params is None or isinstance(params, dict):
+        params = imu_params(**(params or {}))
+    ctx = ctx or default_context()
+    smp = capi.f64(np.reshape(samples, (-1, 7)))
+    itv = capi.f64(np.reshape(intervals, (-1, 2)))
+    bia = capi.f64(np.reshape(biases, (-1, 6)))
+    out = np.zeros(len(itv), capi.PREINTEGRATED_DTYPE)
+    check(lib().gb_imu_preintegrate(ctx.h, len(smp), ptr(smp), len(itv), ptr(itv), ptr(bia), C.byref(params), ptr(out)))
+    return out
+
+
+def imu_term_array(terms, poses, velocities, biases) -> np.ndarray:
+    """(pose_i, vel_i, pose_j, vel_j, bias_i, record) tuples -> a gb_imu_term array; each key maps through the local index of its
+    own dict (poses, velocities, biases: key -> index)"""
+    out = np.zeros(len(terms), capi.IMU_TERM_DTYPE)
+    for m, (xi, vi, xj, vj, bi, rec) in enumerate(terms):
+        out[m]["pose_i"], out[m]["vel_i"], out[m]["pose_j"], out[m]["vel_j"], out[m]["bias_i"] = poses[xi], velocities[vi], poses[xj], velocities[vj], biases[bi]
+        out[m]["pim"] = rec
+    return out
+
+
+def vector_term_array(terms, poses, velocities, biases) -> np.ndarray:
+    """(kind, key_a, key_b, z, precision) tuples -> a gb_vector_term array.  kind: a key of capi.VECTOR_KINDS; key_b is None for a
+    prior; a rotate_velocity term's key_a is a pose, key_b a velocity; z: 3 entries (velocities, rotate) or 6 (biases)."""
+    out = np.zeros(len(terms), capi.VECTOR_TERM_DTYPE)
+    for m, (kind, a, b, z, w) in enumerate(terms):
+        k = capi.VECTOR_KINDS[kind]
+        da, db = {0: (velocities, None), 1: (biases, None), 2: (velocities, velocities), 3: (biases, biases), 4: (poses, velocities)}[k]
+        out[m]["kind"], out[m]["key_a"], out[m]["key_b"] = k, da[a], db[b] if db is not None else -1
+        z = np.asarray(z, dtype=np.float64).ravel()
+        out[m]["z"][: len(z)] = z
+        out[m]["precision"] = float(w)
+    return out
+
+
+def optimize_nav_graph(factors, poses, velocities, biases, priors=(), betweens=(), imu_terms=(), vector_terms=(), params=None,
+                       ctx: Context | None = None) -> dict:
+    """gb_nav_graph_optimize: optimize_pose_graph over poses, velocities and IMU biases (global_mapping.cpp:166-218 with
+    enable_imu; sub_mapping.cpp:218-243).  poses {key: 4x4}, velocities {key: 3}, biases {key: 6 [acc; gyro]}, each kind with its
+    own keys; factors, priors and betweens as optimize_pose_graph's, on pose keys; imu_terms [(pose_i, vel_i, pose_j, vel_j,
+    bias_i, record)] with a capi.PREINTEGRATED_DTYPE record (imu_preintegrate's); vector_terms [(kind, key_a, key_b, z, w)]
+    (vector_term_array's).  -> {poses, velocities, biases (dicts), error, num_inliers, lambda, iterations, trials, status,
+    status_name}"""
+    if params is None or isinstance(params, dict):
+        params = align_params(**(params or {}))
+    lx = {k: i for i, k in enumerate(poses)}
+    lv = {k: i for i, k in enumerate(velocities)}
+    lb = {k: i for i, k in enumerate(biases)}
+    T0 = pose16(np.stack([np.asarray(T, dtype=np.float64).reshape(4, 4) for T in poses.values()]))
+    v0 = capi.f64(np.reshape([np.asarray(v, dtype=np.float64).reshape(3) for v in velocities.values()], (-1, 3)))
+    b0 = capi.f64(np.reshape([np.asarray(b, dtype=np.float64).reshape(6) for b in biases.values()], (-1, 6)))
+    factors = list(factors)
+    fkeys = []
+    for f in factors:
+        if not isinstance(f, IntegratedVGICPFactorGPU) or not f.is_binary():
+            raise capi.GlimB200Error("a navigation graph takes binary VGICP, GICP or ICP factors (no fixed target pose)")
+        fkeys.append([lx[k] for k in f.keys()])
+    ctx = ctx or (factors[0].ctx if factors else default_context())
+    arr = (C.c_void_p * max(1, len(factors)))(*[f._handle() for f in factors])
+    fk = np.ascontiguousarray(np.reshape(fkeys, (-1, 2)), dtype=np.int32)
+    qk = np.ascontiguousarray([lx[k] for k, _, _ in priors], dtype=np.int32)
+    qp = pose16(np.stack([np.asarray(Z, dtype=np.float64).reshape(4, 4) for _, Z, _ in priors])) if len(priors) else np.zeros((0, 16))
+    qw = np.ascontiguousarray([float(w) for _, _, w in priors], dtype=np.float64)
+    bt = between_terms(betweens, lx)
+    it = imu_term_array(imu_terms, lx, lv, lb)
+    vt = vector_term_array(vector_terms, lx, lv, lb)
+    T_out, v_out, b_out = np.zeros_like(T0), np.zeros_like(v0), np.zeros_like(b0)
+    res = capi.GraphResult()
+    check(lib().gb_nav_graph_optimize(ctx.h, len(T0), ptr(T0), len(v0), ptr(v0), len(b0), ptr(b0), len(factors), C.cast(arr, C.c_void_p), ptr(fk),
+                                      len(qw), ptr(qk), ptr(qp), ptr(qw), len(bt), ptr(bt), len(it), ptr(it), len(vt), ptr(vt), C.byref(params),
+                                      ptr(T_out), ptr(v_out), ptr(b_out), C.byref(res)))
+    out = {"poses": {k: _pose(T_out[i]) for i, k in enumerate(lx)}, "velocities": {k: v_out[i].copy() for i, k in enumerate(lv)},
+           "biases": {k: b_out[i].copy() for i, k in enumerate(lb)}}
+    out.update(_result(res))
+    return out
+
+
 def overlap_gpu(voxelmaps, source: PointCloudGPU, deltas, ctx: Context | None = None) -> float:
     """gtsam_points::overlap_gpu: single (voxelmap, delta) or lists (odometry_estimation_gpu.cpp:231, :248)."""
     if isinstance(voxelmaps, (GaussianVoxelMapGPU, IncrementalVoxelMapGPU)):

@@ -633,6 +633,105 @@ GB_API gb_status gb_pose_graph_optimize(gb_ctx* ctx, size_t num_keys, const doub
                                         const double* prior_precisions, size_t num_betweens, const gb_between_term* betweens, const gb_align_params* params,
                                         double* T_out /* K x 16 */, gb_graph_result* result);
 
+/* ---- IMU preintegration (imu_integration.cpp IMUIntegration::integrate_imu over GTSAM's PreintegratedImuMeasurements, tangent
+ *      variant), many intervals in one call.  [EXT] GTSAM is not vendored: the tangent-space preintegration
+ *      (TangentPreintegration::update / UpdatePreintegrated) and its exact theta-theta derivative are restated here.
+ *
+ *      Samples are rows (t, ax, ay, az, wx, wy, wz) with non-decreasing t.  Interval i has a start time, an end time and a bias
+ *      b_hat = [acc; gyro]; its record starts from zero state, zero Jacobians and zero covariance, then:
+ *        window: every sample with start < t <= end, in array order up to the first with t > end: dt = t - last (last starts at
+ *          start); a sample with dt <= 0 is skipped, every other one is integrated and counted in num_integrated and last = t.
+ *          Then, if end - last > 0, one more step of dt = end - last with the first sample after end, or the last sample when
+ *          there is none.  An empty sample array integrates nothing.
+ *        one step (a = a_meas - b_hat_a, w = w_meas - b_hat_g, [theta; p; v] the preintegrated vector, R = Exp(theta)):
+ *          theta += J_r(theta)^-1 w dt, p += v dt + R a dt^2 / 2, v += R a dt (p with the old v), delta_t += dt;
+ *          A = I_9 + [d(J_r(theta)^-1 w dt)/d theta in the theta-theta block, R [-a]x J_r(theta) dt^2 / 2 in p-theta,
+ *              R [-a]x J_r(theta) dt in v-theta, I dt in p-v];  B = [0; R dt^2 / 2; R dt];  C = [J_r(theta)^-1 dt; 0; 0];
+ *          H_bias_acc = A H_bias_acc - B, H_bias_omega = A H_bias_omega - C;
+ *          covariance = A S A^T + B (acc_noise^2 I / dt) B^T + C (gyro_noise^2 I / dt) C^T, then its p-p block += int_noise^2 I dt
+ *          (each entry computed once for its lower triangle and mirrored: the record is exactly symmetric).
+ *      No Coriolis term and no body_P_sensor, as GLIM uses it.  One launch per call, one thread per interval, fp64.
+ *      Validated before any launch: finite samples with non-decreasing times; finite intervals with start <= end; finite
+ *      biases; finite noises >= 0 and a finite gravity. ---- */
+typedef struct gb_imu_params {
+  double acc_noise;  /* accelerometer noise density: 0.05 (config_sensors.json) */
+  double gyro_noise; /* 0.02 */
+  double int_noise;  /* integration noise: 0.001 */
+  double gravity[3]; /* (0, 0, -9.81): PreintegrationParams::MakeSharedU */
+} gb_imu_params;
+typedef struct gb_imu_preintegrated {
+  double delta_t;
+  double preintegrated[9]; /* [theta; p; v] */
+  double H_bias_acc[27];   /* 9 x 3, row-major */
+  double H_bias_omega[27]; /* 9 x 3, row-major */
+  double covariance[81];   /* preintMeasCov, 9 x 9, row-major, symmetric */
+  double bias_hat[6];      /* [acc; gyro] */
+  double gravity[3];
+  int32_t num_integrated;
+  int32_t pad;
+} gb_imu_preintegrated;
+GB_API gb_status gb_imu_default_params(gb_imu_params* params);
+GB_API gb_status gb_imu_preintegrate(gb_ctx* ctx, size_t num_samples, const double* samples /* S x 7 */, size_t num_intervals,
+                                     const double* intervals /* I x 2: start, end */, const double* biases /* I x 6 */, const gb_imu_params* params,
+                                     gb_imu_preintegrated* out /* I */);
+
+/* ---- Navigation graphs: gb_pose_graph_optimize with velocities, IMU biases and IMU factors (global_mapping.cpp:166-218 with
+ *      enable_imu: the X / E / V / B variables of every submap; sub_mapping.cpp:218-243: X / V / B per odometry frame).
+ *      K_X poses T_world_key (T_init), K_V velocities (v_init, 3 each) and K_B biases [acc; gyro] (b_init, 6 each); keys are
+ *      per kind, from 0.  The factors, priors and between terms are gb_pose_graph_optimize's, on pose keys.
+ *
+ *      An IMU term (GTSAM's ImuFactor, PreintegrationBase::computeError) on (pose_i, vel_i, pose_j, vel_j, bias_i) and a
+ *      preintegrated record p: delta = p.preintegrated + H_bias_acc (b_a - p.bias_hat_a) + H_bias_omega (b_g - p.bias_hat_g);
+ *      R^_j = R_i Exp(delta_theta), p^_j = p_i + v_i dt + g dt^2 / 2 + R_i delta_p, v^_j = v_i + g dt + R_i delta_v (dt, g the
+ *      record's delta_t and gravity); r = [Log(R_j^T R^_j); R_j^T (p^_j - p_j); R_j^T (v^_j - v_j)]; error r^T S^-1 r with S
+ *      the record's covariance (no 1/2, as every term here).
+ *      A vector term with isotropic precision w and error w r^T r:
+ *        GB_VECTOR_VELOCITY_PRIOR (key_a a velocity) r = v - z;  GB_VECTOR_BIAS_PRIOR (key_a a bias) r = b - z;
+ *        GB_VECTOR_VELOCITY_BETWEEN / GB_VECTOR_BIAS_BETWEEN (key_a != key_b of that kind) r = (x_b - x_a) - z;
+ *        GB_VECTOR_ROTATE_VELOCITY (key_a a pose, key_b a velocity) r = R_a z - v_b.  [EXT] gtsam_points' RotateVector3Factor is
+ *        not vendored; under an isotropic precision its error equals that of the other sign convention.
+ *      z holds 3 (velocities, rotate) or 6 (biases, [acc; gyro]) entries.
+ *
+ *      The rule is gb_pose_graph_optimize's, with these differences:
+ *        1. every variable fills a 6-dof slot, poses first, then velocities, then biases; a velocity uses the first three dofs
+ *           of its slot, the other three are pinned as the padding is (unit diagonal, zero right-hand side, step 0).
+ *        2. Jacobians are taken in the solver's charts and the retraction is T' = T Exp(delta), v' = v + delta, b' = b + delta;
+ *           the step tests read the pose slots only.
+ *        3. every entry of H and b, and e, sums the factor records in record order, then the between terms, then the IMU terms,
+ *           then the vector terms (each in term order), then the priors: a call without velocities, biases, IMU and vector terms
+ *           sums exactly as gb_pose_graph_optimize.
+ *      Each round is at most four launches, as gb_pose_graph_optimize's.  The context's scratch holds two (6 slots)^2 fp64
+ *      matrices: 1.21 GB each at GB_NAV_GRAPH_MAX_SLOTS.
+ *      Validated before any launch: K_X >= 1, 2 <= K_X + K_V + K_B <= GB_NAV_GRAPH_MAX_SLOTS; F + betweens + IMU + vector terms
+ *      >= 1; every key of its kind and in range, the two poses and the two velocities of an IMU term distinct, the two keys of a
+ *      between vector term distinct, a known vector kind; finite inputs; each record's delta_t > 0 and its covariance exactly
+ *      symmetric and positive definite under an fp64 Cholesky; finite precisions >= 0; everything gb_pose_graph_optimize
+ *      validates. ---- */
+#define GB_NAV_GRAPH_MAX_SLOTS 2048
+typedef struct gb_imu_term {
+  int32_t pose_i, vel_i, pose_j, vel_j, bias_i, pad;
+  gb_imu_preintegrated pim;
+} gb_imu_term;
+#define GB_VECTOR_VELOCITY_PRIOR 0
+#define GB_VECTOR_BIAS_PRIOR 1
+#define GB_VECTOR_VELOCITY_BETWEEN 2
+#define GB_VECTOR_BIAS_BETWEEN 3
+#define GB_VECTOR_ROTATE_VELOCITY 4
+typedef struct gb_vector_term {
+  int32_t kind;         /* GB_VECTOR_* */
+  int32_t key_a, key_b; /* key_b unused by a prior */
+  int32_t pad;
+  double z[6];
+  double precision;     /* w >= 0 */
+} gb_vector_term;
+GB_API gb_status gb_nav_graph_optimize(gb_ctx* ctx, size_t num_poses, const double* T_init /* K_X x 16 */, size_t num_velocities,
+                                       const double* v_init /* K_V x 3 */, size_t num_biases, const double* b_init /* K_B x 6 */, size_t num_factors,
+                                       gb_factor* const* factors, const int32_t* factor_keys /* F x 2 */, size_t num_priors, const int32_t* prior_keys,
+                                       const double* prior_poses /* x 16 */, const double* prior_precisions, size_t num_betweens,
+                                       const gb_between_term* betweens, size_t num_imu_terms, const gb_imu_term* imu_terms, size_t num_vector_terms,
+                                       const gb_vector_term* vector_terms, const gb_align_params* params, double* T_out /* K_X x 16 */,
+                                       double* v_out /* K_V x 3 */, double* b_out /* K_B x 6 */, gb_graph_result* result);
+
 /* ---- Continuous-time GICP: GLIM's LiDAR-only odometry (OdometryEstimationCT, src/glim/odometry/odometry_estimation_ct.cpp,
  *      config/config_odometry_ct.json) on the device: the time table of a frame (:101), IntegratedCT_GICPFactor_<iVox,
  *      PointCloud>(X, Y, ivox, frame, ivox) with max_correspondence_distance (:159-163) and the Levenberg-Marquardt solve with
