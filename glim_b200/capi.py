@@ -63,6 +63,7 @@ _SIGNATURES = {
     "gb_peer_slab_fetch": ([vp, vp], st),
     "gb_peer_slab_fetch_async": ([vp, vp], st),
     "gb_overlap": ([vp, sz, vp, vp, vp, vp], st),
+    "gb_find_overlapping_submaps": ([vp, sz, vp, vp, vp, sz, sz, vp, f64, f64, sz, vp, vp, vp], st),
     "gb_covariances": ([vp, sz, vp, vp, i32, i32, vp, vp], st),
     "gb_find_neighbors": ([vp, sz, vp, i32, vp], st),
     "gb_voxelgrid_sampling": ([vp, sz, vp, vp, vp, f64, vp, vp, vp, vp], st),
@@ -174,6 +175,7 @@ BETWEEN_DTYPE = np.dtype([("key_i", "<i4"), ("key_j", "<i4"), ("Z", "<f8", 16), 
 
 
 GB_NAV_GRAPH_MAX_SLOTS = 2048
+GB_OVERLAP_SEARCH_MAX_SUBMAPS = 4096
 
 
 class ImuParams(C.Structure):

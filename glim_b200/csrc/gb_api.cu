@@ -3,6 +3,7 @@
 // work, in gb_kernels_voxelmap.cu, gb_kernels_preprocess.cu and gb_peer.cu.
 #include "gb_internal.cuh"
 #include "gb_grid_math.cuh"  // grid_half_width
+#include "gb_overlap_math.cuh"  // kOverlapChunk
 
 #include <stdarg.h>
 #include <stdio.h>
@@ -594,8 +595,7 @@ static gb_status sweep_learn_inliers(gb_sweep* s) {
   return GB_OK;
 }
 
-// the target part of a factor descriptor
-static void desc_target(FactorDesc& D, const gb_voxelmap* t) {
+void desc_target(FactorDesc& D, const gb_voxelmap* t) {
   D.buckets = t->buckets; D.voxels = t->voxels;
   D.mask = (uint32_t)t->num_buckets - 1u;
   D.max_scan = t->max_scan;
@@ -1037,11 +1037,15 @@ extern "C" gb_status gb_overlap(gb_ctx* ctx, size_t T, const gb_voxelmap* const*
   GB_REQUIRE(targets && deltas, "null targets / deltas");
   for (size_t t = 0; t < T; t++) GB_REQUIRE(!targets[t] || targets[t]->kind != GB_MAP_POINTS, "a point grid is not an occupancy target");
   GB_ENTER(ctx);
-  // the same layout in pinned staging and in scratch: descriptors | poses | count
-  struct Staging { FactorDesc* descs; double* poses; int* count; } h, d;
+  // the same layout in pinned staging and in scratch: descriptors | poses | the query | its item count | count.  One query of
+  // T targets: the source is descriptor 0's.
+  struct Staging { FactorDesc* descs; double* poses; OverlapQuery* query; int* num_queries; long long* item_end; int* count; } h, d;
   auto layout = [&](Carver& cv, Staging& b) {
     b.descs = cv.take<FactorDesc>(T);
     b.poses = cv.take<double>(16 * T);
+    b.query = cv.take<OverlapQuery>(1);
+    b.num_queries = cv.take<int>(1);
+    b.item_end = cv.take<long long>(1);
     b.count = cv.take<int>(1);
   };
   GB_CHECK(gb_carve(ctx, ctx->pinned, [&](Carver& cv) { layout(cv, h); }));
@@ -1055,9 +1059,13 @@ extern "C" gb_status gb_overlap(gb_ctx* ctx, size_t T, const gb_voxelmap* const*
     D.n = (int)source->n;
   }
   memcpy(h.poses, deltas, sizeof(double) * 16 * T);
-  GB_CUDA(cudaMemcpyAsync(d.descs, h.descs, (char*)h.count - (char*)h.descs, cudaMemcpyHostToDevice, ctx->stream));  // descriptors and poses
+  const long long items = ((long long)source->n + kOverlapChunk - 1) / kOverlapChunk;  // overlap_chunks(n)
+  *h.query = OverlapQuery{0, 0, 0, (int)T};
+  *h.num_queries = 1;
+  *h.item_end = items;
+  GB_CUDA(cudaMemcpyAsync(d.descs, h.descs, (char*)h.count - (char*)h.descs, cudaMemcpyHostToDevice, ctx->stream));  // all but the count
   GB_CUDA(cudaMemsetAsync(d.count, 0, sizeof(int), ctx->stream));
-  GB_CHECK(gb_launch_overlap(ctx, (int)T, d.descs, d.poses, (int)source->n, d.count));
+  GB_CHECK(gb_launch_overlap(ctx, (int)std::min<long long>(items, ctx->num_sms * 8), (int)T, d.query, d.num_queries, d.item_end, d.descs, d.poses, nullptr, d.count));
   GB_CUDA(cudaMemcpyAsync(h.count, d.count, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(cudaStreamSynchronize(ctx->stream));
   *overlap = (double)*h.count / (double)source->n;

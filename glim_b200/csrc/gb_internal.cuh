@@ -557,7 +557,18 @@ gb_status gb_covariance_cloud(gb_ctx* ctx, int M, const int* d_count, const doub
 enum { GB_MODE_LINEARIZE = 0, GB_MODE_ERROR = 1 };
 gb_status gb_launch_sweep(gb_sweep* s, int mode);
 gb_status gb_launch_gicp_sweep(gb_sweep* s, int mode);  // gb_launch_sweep of a GICP sweep
-gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count);
+// k_overlap (gb_kernels_vgicp.cu), shared by gb_overlap and gb_find_overlapping_submaps: the points of the source cloud of
+// descs[source] (its p0 and n) that hit an occupied voxel of any target descs[target + t], t < num_targets, counted into
+// counts[q] (which the caller zeroes) for each of the *num_queries queries.  Target t's pose is poses[pose + t] (16 doubles,
+// column-major, cast to fp32); a query with pose < 0 has one target, and its pose is the relative pose
+// world[target]^-1 world[source] of gb_overlap_math.cuh (overlap_delta).  item_end is the inclusive scan of the queries'
+// chunk counts overlap_chunks(n), in 64 bits.  One launch of `grid` blocks (none when grid is 0); max_targets bounds every
+// query's num_targets (shared memory).
+struct OverlapQuery { int source, target, pose, num_targets; };
+gb_status gb_launch_overlap(gb_ctx* ctx, int grid, int max_targets, const OverlapQuery* d_queries, const int* d_num_queries, const long long* d_item_end,
+                            const FactorDesc* d_descs, const double* d_poses, const double* d_world, int* d_counts);
+// the target part of a factor descriptor (gb_api.cu): a map's table (buckets, mask, max_scan, inv_res) and records
+void desc_target(FactorDesc& D, const gb_voxelmap* t);
 // The posed frame list of gb_merge_frames (gb_kernels_preprocess.cu), shared with the map insert, gb_concat_frames
 // (gb_kernels_segment.cu) and the plane selection (gb_kernels_plane.cu): K device clouds and their poses (K x 16,
 // column-major).  gb_frame_list_check refuses, before any launch, a null list when K > 0, a null frame, a frame on another

@@ -32,6 +32,7 @@
 //                   sized by each factor's last inlier fraction, descriptor / pose cache in shared memory.
 #include "gb_internal.cuh"
 #include "gb_vgicp_math.cuh"  // PoseF, transform, fused_mahalanobis, accumulate_hit, surface_ok, slab_to_record (also compiled for the host by the CPU test)
+#include "gb_overlap_math.cuh"  // overlap_delta and k_overlap's item lookup (also compiled for the host by the CPU test)
 
 #include "gb_sweep_steps.cuh"  // the steps every sweep kernel runs (shared with k_gicp_sweep, gb_kernels_gicp.cu)
 
@@ -328,33 +329,54 @@ __global__ void __launch_bounds__(kThreads, 2) k_vgicp_sweep5(
   }
 }
 
-// overlap: one thread per source point, count points that hit an occupied voxel of any target
-__global__ void __launch_bounds__(256) k_overlap(int num_targets, const FactorDesc* __restrict__ descs, const double* __restrict__ poses, int n, int* __restrict__ count) {
-  extern __shared__ float s_poses[];  // num_targets x 12
-  for (int k = threadIdx.x; k < num_targets * 12; k += blockDim.x) {
-    const int t = k / 12, e = k % 12;
-    const int r = e < 9 ? e / 3 : e - 9, c = e < 9 ? e % 3 : 3;
-    s_poses[k] = (float)poses[(size_t)t * 16 + c * 4 + r];
-  }
-  __syncthreads();
-  int local = 0;
-  const FactorDesc D0 = descs[0];
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float4 a0 = __ldg(&D0.p0[i]);
-    for (int t = 0; t < num_targets; t++) {
-      const PoseF P = load_pose(s_poses + 12 * t);
-      float qx, qy, qz;
-      transform(P, a0.x, a0.y, a0.z, qx, qy, qz);
-      const float sum = (qx + qy) + qz;
-      if (!(sum == sum)) continue;  // NaN point: no voxel
-      const float inv_res = descs[t].inv_res;
-      const int v = gb_lookup(descs[t].buckets, descs[t].mask, descs[t].max_scan, gb_coord(qx, inv_res), gb_coord(qy, inv_res), gb_coord(qz, inv_res));
-      if (v >= 0) { local++; break; }
+// overlap: the source points of each query that hit an occupied voxel of any of its targets.  A query (OverlapQuery) is a
+// source cloud and a range of (target descriptor, pose); gb_overlap is one query of T targets, gb_find_overlapping_submaps
+// P queries of one target each, whose relative pose is computed here from the world poses of the pair.  Work items are
+// (query, chunk of kOverlapChunk consecutive points), numbered query-major in 64 bits (gb_overlap_math.cuh).  A block takes
+// items from a static grid stride, one point per thread, and adds the item's hits to the query's int count with one atomic:
+// the counts do not depend on the order.
+__global__ void __launch_bounds__(kOverlapChunk) k_overlap(const OverlapQuery* __restrict__ queries, const int* __restrict__ num_queries, const long long* __restrict__ item_end,
+                                                           const FactorDesc* __restrict__ descs, const double* __restrict__ poses, const double* __restrict__ world,
+                                                           int* __restrict__ counts) {
+  extern __shared__ float s_poses[];  // the item's query: num_targets x 12
+  __shared__ int s_q;
+  const int nq = *num_queries;
+  if (nq <= 0) return;
+  const long long items = item_end[nq - 1];
+  int q_lo = 0;  // a block's items ascend, and so do their queries
+  for (long long item = blockIdx.x; item < items; item += gridDim.x) {
+    if (threadIdx.x == 0) s_q = overlap_item_query(item_end, nq, q_lo, item);
+    __syncthreads();
+    const int q = s_q;
+    q_lo = q;
+    const OverlapQuery Q = queries[q];
+    for (int k = threadIdx.x; k < Q.num_targets * 12; k += blockDim.x) {
+      const int t = k / 12, e = k % 12;
+      const int r = e < 9 ? e / 3 : e - 9, c = e < 9 ? e % 3 : 3;
+      // a query with pose < 0 (one target): the relative pose of the pair (target, source), one entry per thread
+      const double v = Q.pose < 0 ? overlap_delta_entry(world + 16 * (size_t)Q.target, world + 16 * (size_t)Q.source, r, c) : poses[(size_t)(Q.pose + t) * 16 + c * 4 + r];
+      s_poses[k] = (float)v;
     }
+    __syncthreads();
+    const int i = overlap_item_point(item_end, q, item) + threadIdx.x;
+    const int n = descs[Q.source].n;
+    bool hit = false;
+    if (i < n) {
+      const float4 a0 = __ldg(&descs[Q.source].p0[i]);
+      for (int t = 0; t < Q.num_targets && !hit; t++) {
+        const PoseF P = load_pose(s_poses + 12 * t);
+        float qx, qy, qz;
+        transform(P, a0.x, a0.y, a0.z, qx, qy, qz);
+        const float sum = (qx + qy) + qz;
+        if (!(sum == sum)) continue;  // NaN point: no voxel
+        const FactorDesc& D = descs[Q.target + t];
+        const float inv_res = D.inv_res;
+        hit = gb_lookup(D.buckets, D.mask, D.max_scan, gb_coord(qx, inv_res), gb_coord(qy, inv_res), gb_coord(qz, inv_res)) >= 0;
+      }
+    }
+    const int c = __syncthreads_count(hit);  // also the barrier before s_q and s_poses are rewritten
+    if (threadIdx.x == 0 && c) atomicAdd(&counts[q], c);
   }
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) local += __shfl_xor_sync(0xffffffffu, local, o);
-  if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
 }
 
 }  // namespace
@@ -405,8 +427,9 @@ gb_status gb_launch_sweep(gb_sweep* s, int mode) {
   return GB_OK;
 }
 
-gb_status gb_launch_overlap(gb_ctx* ctx, int num_targets, const FactorDesc* d_descs, const double* d_poses, int n, int* d_count) {
-  if (n <= 0 || num_targets <= 0) return GB_OK;
-  const int grid = min((n + 255) / 256, ctx->num_sms * 8);
-  return gb_launch(ctx, "k_overlap", k_overlap, grid, 256, (size_t)num_targets * 12 * sizeof(float), num_targets, d_descs, d_poses, n, d_count);
+gb_status gb_launch_overlap(gb_ctx* ctx, int grid, int max_targets, const OverlapQuery* d_queries, const int* d_num_queries, const long long* d_item_end,
+                            const FactorDesc* d_descs, const double* d_poses, const double* d_world, int* d_counts) {
+  if (grid <= 0 || max_targets <= 0) return GB_OK;
+  return gb_launch(ctx, "k_overlap", k_overlap, grid, kOverlapChunk, (size_t)max_targets * 12 * sizeof(float), d_queries, d_num_queries, d_item_end, d_descs, d_poses,
+                   d_world, d_counts);
 }

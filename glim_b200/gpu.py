@@ -990,6 +990,32 @@ def overlap_gpu(voxelmaps, source: PointCloudGPU, deltas, ctx: Context | None = 
     return out.value
 
 
+def find_overlapping_submaps(maps, sources, T_world_submap, existing=(), max_distance: float = 100.0, min_overlap: float = 0.2, first_source: int = 0,
+                             ctx: Context | None = None):
+    """GlobalMapping::find_overlapping_submaps / the overlap test of create_matching_cost_factors on the device
+    (gb_find_overlapping_submaps): maps[k] = submap k's coarsest voxel map, sources[k] = its (subsampled) cloud, T_world_submap
+    S x (4,4).  existing: (i, j) pairs that already have a factor.  -> (pairs (M, 2) int32 in lexicographic order, overlaps (M,))"""
+    S = len(maps)
+    ctx = ctx or (sources[0].ctx if S else default_context())
+    marr = (C.c_void_p * max(1, S))(*[m.h for m in maps])
+    sarr = (C.c_void_p * max(1, S))(*[s.h for s in sources])
+    T = pose16(np.stack([np.asarray(x, dtype=np.float64) for x in T_world_submap])) if S else np.zeros((0, 16))
+    ex = np.ascontiguousarray(np.reshape(np.asarray(existing, dtype=np.int32), (-1, 2)))
+    found = C.c_size_t()
+    cap = min(S * (S - 1) // 2, 1 << 22)  # room for every candidate up to 4 M (untouched pages cost nothing); a second call only beyond
+
+    def call(cap):
+        pairs, ovs = np.empty((cap, 2), np.int32), np.empty(cap)
+        check(lib().gb_find_overlapping_submaps(ctx.h, S, C.cast(marr, C.c_void_p), C.cast(sarr, C.c_void_p), ptr(T), first_source, len(ex), ptr(ex),
+                                                max_distance, min_overlap, cap, C.byref(found), ptr(pairs) if cap else None, ptr(ovs) if cap else None))
+        return pairs, ovs
+
+    pairs, ovs = call(cap)
+    if found.value > cap:
+        pairs, ovs = call(found.value)
+    return pairs[:found.value], ovs[:found.value]
+
+
 def merge_frames_gpu(poses, frames, downsample_resolution: float, target_num_points: int = 0, seed: int = 0, ctx: Context | None = None, host_outputs: bool = True):
     """gtsam_points::merge_frames(poses, frames, downsample_resolution, target_num_points) on the device (sub_mapping.cpp:481-497).
     poses: K x (4,4) T_origin_frame; frames: K PointCloudGPU.  -> (points (M,4), covs (M,4,4) [i,row,col], PointCloudGPU)"""

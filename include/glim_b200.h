@@ -873,6 +873,39 @@ GB_API gb_status gb_peer_slab_fetch_async(gb_peer_slab* slab, const float** host
  *      fraction of source points that fall in an occupied voxel of any target ---- */
 GB_API gb_status gb_overlap(gb_ctx* ctx, size_t num_targets, const gb_voxelmap* const* targets, const gb_cloud* source, const double* deltas /* T x 16 */, double* overlap);
 
+/* ---- GlobalMapping::find_overlapping_submaps (src/glim/mapping/global_mapping.cpp:285-351) and the overlap test of
+ *      GlobalMapping::create_matching_cost_factors (:441-453): every candidate pair of S submaps gated, counted and
+ *      thresholded in one call.  maps[k] is submap k's coarsest level (voxelmaps.back()), sources[k] the cloud its overlap is
+ *      measured for (subsampled_submaps[k]), T_world_submap S x 16 column-major.
+ *   - Candidates: the pairs (i, j) with i < j and j >= first_source that are not in `existing` (E x 2 (i, j) pairs that
+ *     already have a factor).  The lookup is ordered, as the reference's set lookup is: an entry (j, i) does not exclude
+ *     (i, j).  first_source 0 is find_overlapping_submaps; S - 1 is create_matching_cost_factors for the newest submap.
+ *   - Delta: delta = T_i^-1 T_j in fp64, R = R_i^T R_j and t = R_i^T t_j + (-(R_i^T t_i)), as Eigen's Isometry3d::inverse() * T;
+ *     every dot product is summed in index order ((a0 b0 + a1 b1) + a2 b2) with no FMA contraction.
+ *   - Distance gate: a candidate is kept iff (t0 t0 + t1 t1) + t2 t2 <= max_distance * max_distance.
+ *   - Overlap: count / n_j, exactly as gb_overlap(ctx, 1, &maps[i], sources[j], delta, &overlap) computes it (the same fp32
+ *     cast of delta, NaN skip and lookup; 0 for an empty source), and so bit-identical to that call.
+ *   - Output: every candidate with overlap >= min_overlap, in lexicographic (i, j) order (the order of both reference loops);
+ *     min_overlap = 0 returns every gated pair.  The first min(found, capacity) results go to pairs (capacity x 2: i, j) and
+ *     overlaps; *num_found is the full count, as with snprintf.  capacity = 0 with NULL arrays is allowed.
+ *   - GB_ERR_INVALID_ARGUMENT before any launch unless ctx, num_found, maps, sources and T_world_submap are non-NULL,
+ *     1 <= S <= GB_OVERLAP_SEARCH_MAX_SUBMAPS, first_source < S, the poses are finite, max_distance is finite and >= 0,
+ *     min_overlap is finite, existing is non-NULL when E > 0 and its keys are in [0, S), pairs and overlaps are non-NULL
+ *     when capacity > 0, and every map and source is non-NULL, on ctx's device and no map is a point grid.
+ *   - Cost: 8 launches (4 kernels around k_overlap, gb_overlap's kernel, and 3 cub calls), whatever S and the number of
+ *     candidates; none for S = 1, which has no pair.  One upload (descriptors, poses and the S x S exclusion bitmap) and at
+ *     most two downloads: the count, then the pairs and overlaps.
+ *   - Size: any cloud gb_cloud_upload accepts, at any distance bound.  The work (one item per pair and 256 source points)
+ *     is counted in 64 bits, so a search whose pairs probe more than 2^31 x 256 points is not refused and is not cut short.
+ *   - Scratch: N = S (S - 1) / 2 - first_source (first_source - 1) / 2 candidate slots (8.4 M at S = 4096), 68 bytes each
+ *     (570 MB at S = 4096, 36 MB at S = 1024), plus S x 208 bytes and S^2 / 8 bytes of bitmap (2 MB at S = 4096).  The
+ *     context's scratch keeps that size until it is destroyed. ---- */
+#define GB_OVERLAP_SEARCH_MAX_SUBMAPS 4096
+GB_API gb_status gb_find_overlapping_submaps(gb_ctx* ctx, size_t num_submaps, const gb_voxelmap* const* maps, const gb_cloud* const* sources,
+                                             const double* T_world_submap /* S x 16 */, size_t first_source, size_t num_existing,
+                                             const int32_t* existing /* E x 2 */, double max_distance, double min_overlap, size_t capacity,
+                                             size_t* num_found, int32_t* pairs /* capacity x 2 */, double* overlaps /* capacity */);
+
 /* ---- CloudCovarianceEstimation::estimate(points, neighbors, k, normals, covs) with PLANE regularization
  *      (src/glim/common/cloud_covariance_estimation.cpp:43-122, :181-196).  GB_ERR_INVALID_ARGUMENT, before any launch,
  *      unless 1 <= k_neighbors <= k_correspondences and the first k_neighbors indices of every row are in [0, n) ---- */

@@ -11,6 +11,7 @@
 //   gtsam_points::NonlinearFactorSetGPU::add / linearize    odometry_estimation_gpu.cpp:383-386
 //   gtsam_points::overlap_gpu / overlap_auto                 odometry_estimation_gpu.cpp:231, :248; src/glim/mapping/global_mapping.cpp:448
 //   gtsam_points::median_distance                            odometry_estimation_gpu.cpp:91
+//   glim_b200::find_overlapping_submaps (the pair loops of)   src/glim/mapping/global_mapping.cpp:285-351, :441-453
 //
 // Ownership and threading (what a drop-in must get right, and round 1 did not):
 //   * PointCloudGPU OWNS its host data.  GLIM replaces the only owner of a frame with its clone
@@ -784,3 +785,61 @@ inline double median_distance(const PointCloud::ConstPtr& frame, int max_scan_co
 }
 
 }  // namespace gtsam_points
+
+namespace glim_b200 {
+
+/// The (i, j) key of an entry of the caller's set of existing factors: a std::pair, or anything indexable such as the
+/// Eigen::Vector3i of GlobalMapping::find_overlapping_submaps (global_mapping.cpp:290).
+template <class A, class B> inline std::array<int32_t, 2> existing_key(const std::pair<A, B>& e) { return {{static_cast<int32_t>(e.first), static_cast<int32_t>(e.second)}}; }
+template <class V> inline std::array<int32_t, 2> existing_key(const V& e) { return {{static_cast<int32_t>(e[0]), static_cast<int32_t>(e[1])}}; }
+
+/// The pair loops of GlobalMapping::find_overlapping_submaps (global_mapping.cpp:308-351: first_source 0) and
+/// create_matching_cost_factors (:441-453: first_source = current, min_overlap 0 to read previous_overlap as well) as one
+/// gb_find_overlapping_submaps call.  maps[k] = submaps[k]->voxelmaps.back(), sources[k] = subsampled_submaps[k] (or the
+/// current submap's frame), T_world_submap[k] = submaps[k]->T_world_origin (glim_b200::Pose or Eigen::Isometry3d); `existing`
+/// holds the (i, j) pairs that already have a factor.  Returns (i, j, overlap) for every candidate with overlap >= min_overlap
+/// in lexicographic (i, j) order, the order of both loops.
+template <class PoseT, class Alloc, class Existing>
+inline std::vector<std::tuple<int, int, double>> find_overlapping_submaps(const std::vector<gtsam_points::GaussianVoxelMap::ConstPtr>& maps,
+                                                                          const std::vector<gtsam_points::PointCloud::ConstPtr>& sources,
+                                                                          const std::vector<PoseT, Alloc>& T_world_submap, const Existing& existing,
+                                                                          double max_distance, double min_overlap, std::size_t first_source = 0,
+                                                                          CUstream_st* stream = nullptr) {
+  const std::size_t S = maps.size();
+  if (sources.size() != S || T_world_submap.size() != S) throw std::runtime_error("find_overlapping_submaps: maps, sources and poses differ in size");
+  std::vector<const gb_voxelmap*> m(S);
+  std::vector<const gb_cloud*> c(S);
+  std::vector<double> T(16 * S);
+  for (std::size_t k = 0; k < S; k++) {
+    const auto t = std::dynamic_pointer_cast<const gtsam_points::GaussianVoxelMapGPU>(maps[k]);
+    const auto s = std::dynamic_pointer_cast<const gtsam_points::PointCloudGPU>(sources[k]);
+    if (!t || !s) throw std::runtime_error("find_overlapping_submaps: GPU voxel maps / GPU point clouds required");
+    m[k] = t->handle();
+    c[k] = s->handle();
+    const Pose P(T_world_submap[k]);
+    std::copy(P.m.begin(), P.m.end(), T.begin() + 16 * k);
+  }
+  std::vector<int32_t> ex;
+  for (const auto& e : existing) {
+    const auto key = existing_key(e);
+    ex.insert(ex.end(), key.begin(), key.end());
+  }
+  gb_ctx* ctx = Context::of_stream(stream);
+  std::size_t found = 0, capacity = std::min<std::size_t>(S * (S > 0 ? S - 1 : 0) / 2, 1 << 18);  // a first guess; a second call only when more are found
+  std::vector<int32_t> pairs;
+  std::vector<double> overlaps;
+  for (int attempt = 0; attempt < 2; attempt++) {
+    pairs.resize(2 * capacity);
+    overlaps.resize(capacity);
+    check(gb_find_overlapping_submaps(ctx, S, m.data(), c.data(), T.data(), first_source, ex.size() / 2, ex.empty() ? nullptr : ex.data(), max_distance, min_overlap,
+                                      capacity, &found, capacity ? pairs.data() : nullptr, capacity ? overlaps.data() : nullptr),
+          "gb_find_overlapping_submaps");
+    if (found <= capacity) break;
+    capacity = found;
+  }
+  std::vector<std::tuple<int, int, double>> out(found);
+  for (std::size_t r = 0; r < found; r++) out[r] = std::make_tuple(pairs[2 * r], pairs[2 * r + 1], overlaps[r]);
+  return out;
+}
+
+}  // namespace glim_b200
