@@ -11,6 +11,7 @@ from oracle import oracle
 from tests import graph_oracle as gro
 from tests import grid_oracle as go
 from tests import lm_oracle as lm
+from tests import solve_check as sc
 from tests import voxelmap_oracle as vo
 from tests.util import cov_colmajor16
 
@@ -64,7 +65,9 @@ def start3(kf, seed):
 
 def test_one_round_matches_downstream_of_the_records(kf, ctx):
     """max_iterations = 1: the device's poses against the restatement fed the records of a gpu.Sweep over the same factors in
-    the same order at the same poses; everything after the sweep is fp64, so only the solve's order of operations differs."""
+    the same order at the same poses; everything after the sweep is fp64, so only the solve's order of operations differs.
+    The step's scaled backward error (tests/solve_check.py) is held to the restatement's, a second sweep measuring the
+    records' own spread."""
     T0 = start3(kf, 1400)
     priors = [(0, T0[0], 1e6)]
     facs = vgicp(kf, SPEC3)
@@ -80,13 +83,19 @@ def test_one_round_matches_downstream_of_the_records(kf, ctx):
     def err(f, dl, d):
         return float(gpu.NonlinearFactorSetGPU(ctx).add([facs[f]]).error_deltas(dl[None], d[None])[0])
 
-    ref = gro.optimize(lin, err, [(t, s) for t, s, _ in SPEC3], T0, priors, {"max_iterations": 1})
+    with sc.systems() as seen:
+        ref = gro.optimize(lin, err, [(t, s) for t, s, _ in SPEC3], T0, priors, {"max_iterations": 1})
+    recs2 = gpu.Sweep(ctx, facs).linearize(rows0)
+    with sc.systems() as again:
+        gro.optimize(lambda f, d: (gpu.unpack_linearized(recs2[f]), d), err, [(t, s) for t, s, _ in SPEC3], T0, priors, {"max_iterations": 1})
     got = gpu.optimize_graphs([prob], params={"max_iterations": 1})[0]
     assert (got["iterations"], got["trials"], got["status"]) == (ref["iterations"], ref["trials"], ref["status"]) == (1, 1, lm.ALIGN_MAX_ITERATIONS)
     for k in range(3):
         step = np.linalg.norm(gro.se3_log(rel(T0[k], ref["T"][k])))
         diff = np.linalg.norm(gro.se3_log(rel(ref["T"][k], got["values"][k])))
         assert diff <= 1e-8 * max(step, 1e-3), (k, diff, step)
+    Tg = [got["values"][k] for k in range(3)]
+    sc.check("graph K 3", seen[0], sc.pose_steps(T0, Tg), sc.pose_steps(T0, ref["T"]), sc.pose_eps(T0, Tg), noise=again[0][:2])
     assert got["num_inliers"] == ref["num_inliers"]
 
 

@@ -11,6 +11,7 @@ from glim_b200 import capi, gpu, synth, workloads
 from oracle import oracle
 from tests import imu_oracle as io
 from tests import nav_graph_oracle as ngo
+from tests import solve_check as sc
 from tests.util import cov_colmajor16
 
 pytestmark = pytest.mark.gpu
@@ -162,7 +163,9 @@ def test_one_round_matches_downstream_of_the_records(ctx, gm32):
     """max_iterations = 1 on GLIM's global-mapping IMU recipe: the device's poses, velocities and biases against the restatement
     fed the records of a gpu.Sweep over the same factors at the same poses.  Everything after the sweep is fp64 (the IMU and
     vector terms, the pinned dofs, the solve), so only the order of operations differs: the steps agree to about the system's
-    condition number times the unit roundoff, which the test computes from the restatement's first system."""
+    condition number times the unit roundoff, which the test computes from the restatement's first system.  The step's scaled
+    backward error (tests/solve_check.py) is held to the restatement's whatever the condition number, a second sweep
+    measuring the records' own spread."""
     g = gm32
     dev, refargs, _, remap = recipe(ctx, g)
     facs = g["facs"]
@@ -189,7 +192,8 @@ def test_one_round_matches_downstream_of_the_records(ctx, gm32):
 
     ngo.assemble = spy
     try:
-        ref, lx, lv, lb = restated((keys, lin, err), *refargs, {"max_iterations": 1})
+        with sc.systems() as seen:
+            ref, lx, lv, lb = restated((keys, lin, err), *refargs, {"max_iterations": 1})
     finally:
         ngo.assemble = assemble
     got = call()
@@ -212,6 +216,14 @@ def test_one_round_matches_downstream_of_the_records(ctx, gm32):
     print(f"one round: condition {cond:.3g}, relative step difference {err_rel:.3g}; restated velocity step {vmove:.3g}, bias step {bmove:.3g}")
     assert vmove > 1e-3 and bmove > 0.0
     assert err_rel <= max(1e-9, 1e-15 * cond), (err_rel, cond)
+    recs2 = gpu.Sweep(ctx, facs).linearize(rows0)
+    with sc.systems() as again:
+        restated((keys, lambda f, d: (gpu.unpack_linearized(recs2[f]), d), err), *refargs, {"max_iterations": 1})
+    mask = np.zeros(len(systems[0]), bool)
+    mask[live] = True
+    X0s = ([X0[0][k] for k in lx], [X0[1][k] for k in lv], [X0[2][k] for k in lb])
+    Xg = ([got["poses"][remap.get(k, k)] for k in lx], [got["velocities"][k] for k in lv], [got["biases"][k] for k in lb])
+    sc.check("nav graph gm32 IMU recipe", seen[0], sc.nav_steps(X0s, Xg), sc.nav_steps(X0s, ref["x"]), sc.nav_eps(X0s, Xg), live=mask, noise=again[0][:2])
     assert got["num_inliers"] == ref["num_inliers"]
 
 

@@ -11,6 +11,7 @@ from oracle import oracle
 from tests import graph_oracle as go
 from tests import lm_oracle as lm
 from tests import pose_graph_oracle as pgo
+from tests import solve_check as sc
 from tests.util import cov_colmajor16
 
 pytestmark = pytest.mark.gpu
@@ -84,16 +85,19 @@ def condition_1norm(T0, priors, bts, lam):
 def test_one_round_between_only(ctx, K):
     """max_iterations = 1 on well-conditioned between-only graphs with random SPD information: the device's step against the
     restatement's.  Only the solve's order of operations differs (fp64 throughout), so the steps agree to about the condition
-    number times the unit roundoff; 1e-9 relative holds with margin below a condition number of 1e6, which the test checks."""
+    number times the unit roundoff; 1e-9 relative holds with margin below a condition number of 1e6, which the test checks.
+    The step's scaled backward error (tests/solve_check.py) is held to the restatement's, whatever the condition number."""
     T0, bts, priors = well_conditioned_graph(K, 500 + K)
     assert condition_1norm(T0, priors, bts, lm.ALIGN_DEFAULTS["lambda_initial"]) < 1e6
     got = gpu.optimize_pose_graph([], dict(enumerate(T0)), priors=priors, betweens=as_betweens(bts), params={"max_iterations": 1}, ctx=ctx)
-    ref = pgo.optimize(None, None, [], T0, priors, bts, {"max_iterations": 1})
+    with sc.systems() as seen:
+        ref = pgo.optimize(None, None, [], T0, priors, bts, {"max_iterations": 1})
     assert (got["iterations"], got["trials"], got["status"]) == (ref["iterations"], ref["trials"], ref["status"]) == (1, 1, lm.ALIGN_MAX_ITERATIONS)
     assert got["num_inliers"] == 0.0
     d_got = np.concatenate([go.se3_log(rel(T0[k], got["values"][k])) for k in range(K)])
     d_ref = np.concatenate([go.se3_log(rel(T0[k], ref["T"][k])) for k in range(K)])
     assert np.linalg.norm(d_got - d_ref) <= 1e-9 * np.linalg.norm(d_ref), np.linalg.norm(d_got - d_ref) / np.linalg.norm(d_ref)
+    sc.check(f"pose graph K {K}, well conditioned", seen[0], d_got, d_ref, sc.pose_eps(T0, [got["values"][k] for k in range(K)]))
     assert abs(got["error"] - ref["error"]) <= 1e-9 * ref["error"]
 
 
