@@ -59,6 +59,10 @@ extern "C" gb_status gb_mem_info(int device, size_t* free_bytes, size_t* total_b
 // ---------------------------------------------------------------------------------------------
 namespace {
 struct DevPool {
+  // Lock order: a context's mu, then drain_mu, then mu.  drain_mu is held while a free drains the streams of ctxs, while a
+  // context leaves ctxs (so its stream is never synchronised after ctx_release destroys it), and while the library captures
+  // a sweep graph on a context's stream (so a free never synchronises a stream the library is capturing on).
+  std::mutex drain_mu;
   std::mutex mu;
   std::map<void*, size_t> live;            // block -> capacity
   std::multimap<size_t, void*> free_list;  // capacity -> block
@@ -102,23 +106,41 @@ cudaError_t gb_dev_malloc(int device, size_t bytes, void** out) {
   P.live[*out] = cap;
   return cudaSuccess;
 }
+// Before the block is recycled, nobody may still be reading it (cudaFree's implicit guarantee): every live context's stream
+// is drained.  A stream with a capture in progress is skipped: synchronising it would invalidate that capture, and a capture
+// begins on a drained stream (the library's own under drain_mu, right after a synchronise; a caller's as the header asks).
+// Whatever fails here is not the caller's error: the calling thread's last-error slot is left clear, and a block whose
+// drain failed goes back to the driver instead of the pool.
 void gb_dev_free(int device, void* p) {
   if (!p) return;
   DevPool& P = g_pools[device & 15];
-  std::vector<cudaStream_t> streams;
   size_t cap = 0;
   {
     std::lock_guard<std::mutex> lock(P.mu);
     auto it = P.live.find(p);
     if (it != P.live.end()) { cap = it->second; P.live.erase(it); }
-    for (gb_ctx* c : P.ctxs) streams.push_back(c->stream);
   }
-  if (cap == 0) { cudaFree(p); return; }
-  for (cudaStream_t st : streams) cudaStreamSynchronize(st);  // nobody may still be reading the block (cudaFree's implicit guarantee)
-  std::lock_guard<std::mutex> lock(P.mu);
-  if (P.free_bytes + cap > kPoolMaxFreeBytes) { cudaFree(p); return; }
-  P.free_list.emplace(cap, p);
-  P.free_bytes += cap;
+  bool drained = cap != 0;
+  if (drained) {
+    std::lock_guard<std::mutex> drain(P.drain_mu);
+    std::vector<cudaStream_t> streams;
+    { std::lock_guard<std::mutex> lock(P.mu); for (gb_ctx* c : P.ctxs) streams.push_back(c->stream); }
+    for (cudaStream_t st : streams) {
+      cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+      if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) { (void)cudaGetLastError(); continue; }  // the legacy stream beside a capture
+      if (cs != cudaStreamCaptureStatusNone) continue;
+      if (cudaStreamSynchronize(st) != cudaSuccess) { (void)cudaGetLastError(); drained = false; }
+    }
+  }
+  if (drained) {
+    std::lock_guard<std::mutex> lock(P.mu);
+    if (P.free_bytes + cap <= kPoolMaxFreeBytes) {
+      P.free_list.emplace(cap, p);
+      P.free_bytes += cap;
+      return;
+    }
+  }
+  if (cudaFree(p) != cudaSuccess) (void)cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -172,7 +194,12 @@ void ctx_release(gb_ctx* ctx) {
   if (ctx->refs.fetch_sub(1) != 1) return;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  { DevPool& P = g_pools[ctx->device & 15]; std::lock_guard<std::mutex> lock(P.mu); P.ctxs.erase(std::remove(P.ctxs.begin(), P.ctxs.end(), ctx), P.ctxs.end()); }
+  {  // under drain_mu: a free that listed this stream has finished synchronising it before the stream can be destroyed
+    DevPool& P = g_pools[ctx->device & 15];
+    std::lock_guard<std::mutex> drain(P.drain_mu);
+    std::lock_guard<std::mutex> lock(P.mu);
+    P.ctxs.erase(std::remove(P.ctxs.begin(), P.ctxs.end(), ctx), P.ctxs.end());
+  }
   for (const gb_pool_block& b : ctx->pool) pool_block_free(b);
   if (ctx->scratch.base) cudaFree(ctx->scratch.base);
   if (ctx->pinned.base) cudaFreeHost(ctx->pinned.base);
@@ -916,16 +943,21 @@ static gb_status sweep_linearize(gb_sweep* s, const double* T, gb_linearized6* o
   cudaStream_t st = ctx->stream;
   const size_t pose_bytes = sizeof(double) * 16 * s->F, out_bytes = sizeof(double) * GB_OUT_DOUBLES * s->F;
   if (s->graph_state == 0) {
-    GB_CUDA(cudaStreamSynchronize(st));  // nothing of this sweep may be in flight while its work is captured
     cudaGraph_t graph = nullptr;
-    bool ok = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
-    if (ok) {
-      ok = cudaMemcpyAsync(s->d_poses, s->h_pose_slot[0], pose_bytes, cudaMemcpyHostToDevice, st) == cudaSuccess;
-      const uint64_t launches = ctx->launches;
-      ok = ok && gb_launch_sweep(s, GB_MODE_LINEARIZE) == GB_OK;
-      ctx->launches = launches;  // counted per graph launch below
-      ok = ok && cudaMemcpyAsync(s->h_out, s->d_out, out_bytes, cudaMemcpyDeviceToHost, st) == cudaSuccess;
-      ok = (cudaStreamEndCapture(st, &graph) == cudaSuccess) && ok && graph != nullptr;
+    bool ok;
+    {
+      // under the pool's drain lock: no gb_dev_free of another thread synchronises the stream during the capture
+      std::lock_guard<std::mutex> drain(g_pools[ctx->device & 15].drain_mu);
+      GB_CUDA(cudaStreamSynchronize(st));  // nothing of this sweep may be in flight while its work is captured
+      ok = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;  // refused on the legacy stream
+      if (ok) {
+        ok = cudaMemcpyAsync(s->d_poses, s->h_pose_slot[0], pose_bytes, cudaMemcpyHostToDevice, st) == cudaSuccess;
+        const uint64_t launches = ctx->launches;
+        ok = ok && gb_launch_sweep(s, GB_MODE_LINEARIZE) == GB_OK;
+        ctx->launches = launches;  // counted per graph launch below
+        ok = ok && cudaMemcpyAsync(s->h_out, s->d_out, out_bytes, cudaMemcpyDeviceToHost, st) == cudaSuccess;
+        ok = (cudaStreamEndCapture(st, &graph) == cudaSuccess) && ok && graph != nullptr;
+      }
     }
     if (ok) ok = cudaGraphInstantiate(&s->graph_exec, graph, 0) == cudaSuccess;
     if (graph) cudaGraphDestroy(graph);

@@ -20,6 +20,20 @@
  *     one ctx may be used by factors and sweeps of another ctx of the same device: frames migrate from
  *     the odometry thread to sub-mapping to global mapping (async_sub_mapping.cpp:8,
  *     async_global_mapping.cpp:24).  Every upload / build call returns after its stream has drained.
+ *     Any thread may destroy a cloud, map, factor or sweep, whichever context made it.  A context destroyed while its
+ *     factors or sweeps are alive lives on until the last of them is destroyed; they keep working meanwhile.
+ *     A factor destroyed while sweeps cached by other contexts name it leaves those sweeps stale: each context drops its
+ *     own on its next factor-set call; a caller-owned gb_sweep that names it is refused from then on.
+ *   - a freed cloud / map block is recycled only after the stream of every live context of the device has drained (what
+ *     cudaFree would wait for).  A stream with a capture in progress is skipped, not synchronised: that would invalidate the
+ *     capture.  A free never fails and never leaves a CUDA error in the calling thread's last-error slot.
+ *   - caller-owned streams (gb_ctx_create_on_stream): the library orders its work on the stream and may synchronise it.
+ *     A caller that captures on such a stream (e.g. a torch CUDA graph, best in thread-local mode) must begin the capture on
+ *     a drained stream, must make no call through that context while capturing, and must not destroy library objects that
+ *     work still in flight on the stream reads.  Frees made by other threads during the capture do not touch the stream.
+ *     On the legacy default stream (0) no graph capture can begin: small sweeps run as plain launches, with the same
+ *     results.  Device results (gb_sweep_results_device) may be read on the same stream right after gb_sweep_launch.
+ *   - gb_last_error() is per thread: a failure in one thread does not change another thread's message.
  *   - 4x4 poses are 16 doubles, COLUMN-MAJOR (Eigen::Isometry3d::data()).
  *   - 6x6 blocks are column-major, tangent order [rotation(3); translation(3)] (gtsam::Pose3).
  *   - there is NO CPU fallback: without a CUDA device every call fails with GB_ERR_NO_DEVICE.
